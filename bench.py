@@ -1,6 +1,7 @@
-"""bench.py — benchmark of the SO-Net forward hot path on B200 (BASELINE.json metric).
+"""bench.py — benchmark of the SO-Net forward hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config cfg2]
+                    [--dump-outputs DIR]
 
 Default (--config cfg2, BASELINE.json configs[1], the headline): a "step" is one eval-mode
 classifier forward (ModelNet40 shape: batch 64 per GPU, N=5000 points, 8x8 SOM, k=3, som_k=9,
@@ -28,6 +29,10 @@ line.
             host cores on a bounded sample (8 clouds of this run's inputs). Its outputs are also
             the parity check of the timed GPU steps ("parity")
   --impl reference   only that CPU arm, same JSON shape with "impl": "reference"
+  --dump-outputs DIR   rank 0 writes the outputs of the last timed step (what
+            Model.test_model() hands its caller: the scores of all ranks, or the Chamfer losses of
+            all ranks plus its own reconstructed clouds) as DIR/<name>.npy in float32; inputs and weights are seeded, so two builds run with the
+            same arguments can be compared output for output
 """
 import argparse
 import json
@@ -68,15 +73,11 @@ CONFIGS = {
 }
 METRIC = CONFIGS["cfg2"]["metric"]
 WORKLOAD = CONFIGS["cfg2"]["workload"]
-# dram__bytes_read.sum + dram__bytes_write.sum per launch at the cfg2 workload, from the committed
-# `ncu --set full` captures (profiles/); None until a capture exists.
-NCU_TRAFFIC = {"index_max_f32": 1.4871e9,
-               # profiles/r01h_pointresnet_tc_pool_compact.ncu-rep: 33.89 MB read + 2.8 KB written
-               "pointresnet_tc_pool_forward": 33.895e6,
-               # profiles/r02d_query_topk.ncu-rep: 3.92 MB read + 198.3 MB written (245.8 MB
-               # algorithmic: part of the mask was still in L2 when the capture ended)
-               "query_topk": 202.26e6}
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+# DRAM bytes per launch at the cfg2 workload, measured by a profiler capture of the current
+# kernels; empty until such a capture exists (the roofline then reports no traffic figure).
+NCU_TRAFFIC = {}
+# NVIDIA H100 SXM data sheet (dense BF16, HBM3), for a card allowed 700 W; MEASURED_PEAKS.json wins
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
 
 
 def load_peaks():
@@ -93,7 +94,7 @@ def load_peaks():
     return d
 
 
-# ---- clocks sampling (B200_PROFILING.md recipe) -----------------------------------------------------
+# ---- clocks sampling (nvidia-smi queries, read only) -----------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -169,6 +170,28 @@ def input_list(task, inp, B, N):
             seg = inp["seg"] = (torch.arange(B * N, dtype=torch.int64).view(B, N) * 7) % 50
         return [inp["pc"], inp["sn"], inp["label"], seg, inp["node"], inp["node_knn_I"]]
     return [inp["pc"], inp["sn"], inp["label"], inp["node"], inp["node_knn_I"]]
+
+
+def result_name(task):
+    return {"classifier": "score", "segmenter": "score_segmenter"}.get(task, "chamfer_loss")
+
+
+DUMP_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(dirname, task, model, gathered):
+    """The last timed step's outputs as DIR/<name>.npy (float32): the result rows of every rank
+    (all-gathered) and, for the auto-encoder, this rank's reconstructed clouds. Arrays are cut to
+    their first clouds if they would exceed DUMP_BYTES together (never at the bench's shapes)."""
+    import numpy as np
+    arrays = {result_name(task): gathered}
+    if task == "autoencoder":
+        arrays["predicted_pc"] = model.predicted_pc
+    per_cloud = sum(a[0].numel() * 4 for a in arrays.values())
+    keep = max(1, min(min(a.shape[0] for a in arrays.values()), DUMP_BYTES // per_cloud))
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(dirname, name + ".npy"), a[:keep].detach().float().cpu().numpy())
 
 
 def result_rows(task, model):
@@ -370,7 +393,7 @@ def kernel_report(profile_steps, peaks):
 
 
 def fused_kernel_clock(model, dev):
-    """SM clock the fused tcgen05 kernel actually runs at: SM cycles counted by CTA 0 (clock64, the
+    """SM clock the fused wgmma kernel actually runs at: SM cycles counted by CTA 0 (clock64, the
     kernel's debug timeline entry point) against the CUDA-event duration of the same launch.
     nvidia-smi's samples (>= 20 ms apart) cannot see inside a 0.7 ms kernel; under tensor load the
     chip is power-managed below clocks.max.sm within the kernel."""
@@ -476,6 +499,8 @@ def main():
                          "sonet_allgather (the same NCCL, resolved by libsonet_b200)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="eager op calls instead of CUDA-graph replay")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's result rows as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else args.warmup
     cfg = CONFIGS[args.config]
@@ -574,6 +599,8 @@ def main():
     wall = time.perf_counter() - wall0
     timed_rows = result_rows(task, model).detach().clone()  # result of the last timed step
     timed_gather = out.detach().clone()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, task, model, timed_gather)
     launches = ops.KERNEL_LAUNCHES - l0
     step_ms = [a.elapsed_time(b) for a, b in evs]
     total_ms = torch.tensor([sum(step_ms)], dtype=torch.float64, device=dev)
@@ -658,7 +685,7 @@ def main():
     kernels = kernel_report(prof_steps, peaks)
     kernel_ms = sum(r["ms"] for r in kernels)
     # the dominant kernel = the launch with the largest measured device time among those with a
-    # roofline model (the fused tcgen05 PointResNet on the default path)
+    # roofline model (the fused wgmma PointResNet on the default path)
     modelled = [r for r in kernels if "bound" in r]
     dom = max(modelled, key=lambda r: r["ms"])
     roofline = {"kernel": dom["kernel"], "bound": dom["bound"], "achieved": dom["achieved"],

@@ -1,5 +1,5 @@
 /*
- * sonet_b200.h — C-ABI of libsonet_b200.so, the B200 (sm_100a) implementation of SO-Net's
+ * sonet_b200.h — C-ABI of libsonet_b200.so, the H100 (sm_90a) implementation of SO-Net's
  * per-batch forward hot path (SURVEY.md §8).
  *
  * Conventions (all entry points):
@@ -31,7 +31,7 @@ typedef void* sonet_stream_t; /* cudaStream_t */
 
 /* ---- library ------------------------------------------------------------------------------ */
 const char* sonet_last_error_string(void);
-/* "sonet_b200 <version> sm_100a" */
+/* "sonet_b200 <version> sm_90a" */
 const char* sonet_version(void);
 
 /* ---- a-6/a-7: per-node indexed arg-max pool ---------------------------------------------------
@@ -121,7 +121,7 @@ int sonet_comm_destroy(void* comm);
  * up-sampling are pre-summed by the host into four [Cout, 4*Cin] matrices, tap-major K).
  *   sonet_upconv_im2col_f32: in [B,Cin,H,W] -> xcol [4][B][4*Cin][H*W]: group g = py*2+px, tap
  *     t = a*2+c reads in[b, ci, i + a-1+py, j + c-1+px] (0 outside the map).
- *   sonet_pointwise_tc_pack_groups: G weight matrices [G,Cout,Cin] -> G consecutive tcgen05 blobs
+ *   sonet_pointwise_tc_pack_groups: G weight matrices [G,Cout,Cin] -> G consecutive wgmma blobs
  *     (sonet_pointwise_tc_blob_bytes(Cout,Cin) each) with one common pre-scale (*inv_scale).
  *   sonet_pointwise_tc_grouped_forward: out_g = act(inv_scale * W_g x_g + shift) for G groups in
  *     ONE launch. x [G*B, C, P]; with scat_w = W > 0 (G must be 4, P = H*W, P_out = 4P) row
@@ -161,10 +161,10 @@ int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, int P, cons
  *     recomputed from x (gamma*xhat+beta > 0), so the forward output need not be kept.
  *   sonet_index_max_backward_f32: grad_data [B,C,N] = 0; grad_data[b,c,idx[b,c,k]] += grad_out[b,c,k]
  *     (k ascending, one thread per (b,c): deterministic also when empty nodes all gather point 0).
- *   sonet_pointwise_tc_pack_device: fp32 W [Cout,Cin] on the DEVICE -> tcgen05 blob (optionally of
+ *   sonet_pointwise_tc_pack_device: fp32 W [Cout,Cin] on the DEVICE -> wgmma blob (optionally of
  *     W^T, for the dgrad GEMM) with the power-of-two pre-scale computed on the device;
  *     scale2[0]=scale, scale2[1]=1/scale; scratch_bits: one uint32 of scratch.
- *   sonet_pointwise_tc_forward_dev: the generic tcgen05 layer with that blob (1/scale read from
+ *   sonet_pointwise_tc_forward_dev: the generic wgmma layer with that blob (1/scale read from
  *     device memory): the forward GEMM y = W x + b and the dgrad GEMM dx = W^T dy of a training step.
  *   sonet_wgrad_tc_f32: the wgrad GEMM dW[co][ci] = sum_{b,p} dy[b,co,p] x[b,ci,p] on the same kernel:
  *     dy is transposed to [K = B*P][Cout] and pre-scaled by a power of two (gradients are far below
@@ -315,11 +315,11 @@ int sonet_chamfer_f32(const float* pred, const float* gt, int B, int Mp, int N, 
                       int32_t* idx_bwd, float* elem_fwd, float* elem_bwd, float* loss_fwd_arr,
                       float* loss_bwd_arr, float* loss, sonet_stream_t stream);
 
-/* ---- a-5 on tensor cores: the whole first PointResNet as one tcgen05 kernel ----------------------
+/* ---- a-5 on tensor cores: the whole first PointResNet as one wgmma kernel ----------------------
  * Replaces Encoder.first_pointnet = PointResNet(Cin,[64,128,256,384]).forward in eval mode
  * (models/layers.py:419-432, models/networks.py:82-83,176): three Conv1d(k=1)+BN+ReLU layers, the
  * skip-concat of layer-0's output and the bare 320->384 layer, for every stacked point copy.
- * Activations stay in tensor memory between the layers; fp32 parity comes from a 3-product bf16
+ * Activations stay in shared memory between the layers; fp32 parity comes from a 3-product fp16
  * hi/lo split (see csrc/pointmlp_tc.cu).
  *   pack (host pointers): W0 [64,Cin], W1 [128,64], W2 [256,128], W3 [384,320] row-major with the
  *     eval BatchNorm scale already folded in; shift0..3 = folded bias/BN shift. Writes the bf16
@@ -357,7 +357,7 @@ int sonet_knn_assemble_pool_f32(const float* coord, int32_t* pool_keys, const fl
                                 const int64_t* idx, int B, int C, int M, int K, int Kstride,
                                 int center_type, float* masked_max, float* center, float* x_aug,
                                 sonet_stream_t stream);
-/* ---- a-3 + a-5 + a-6/a-7 fused: node-sorted copies -> tcgen05 PointResNet -> per-node max -----
+/* ---- a-3 + a-5 + a-6/a-7 fused: node-sorted copies -> wgmma PointResNet -> per-node max -----
  * The classifier / auto-encoder path, where first_pn_out [B,384,kN] itself is never needed
  * (models/networks.py:168-185): it is neither written nor re-read.
  *   sonet_som_sort_decenter: buckets the k*N stacked copies of each cloud by node (order inside a
@@ -383,7 +383,7 @@ int sonet_pool_keys_init(int32_t* keys, long long n, sonet_stream_t stream);
 int sonet_pool_finalize(int32_t* keys, const float* p0, int B, int C, int M, float* out_val,
                         sonet_stream_t stream);
 
-/* ---- a-8/a-9/a-10 on tensor cores: generic point-wise layer on tcgen05 --------------------------
+/* ---- a-8/a-9/a-10 on tensor cores: generic point-wise layer on wgmma --------------------------
  * Same contract as sonet_pointwise_layer_f32 (EquivariantLayer / MyConv2d 1x1 eval forward,
  * models/layers.py:203-210, 282-296) for layers dense enough for tensor cores (KNNModule,
  * final PointNet, segmenter head). fp32 parity through the fp16 hi/lo 3-product split.
@@ -400,25 +400,24 @@ int sonet_pointwise_tc_forward(const float* x0, int C0, const float* x1, int C1,
                                float* out, sonet_stream_t stream);
 
 /* ---- diagnostics -------------------------------------------------------------------------------
- * One 128 x N x K bf16 GEMM on tcgen05 (fp32 accumulate in TMEM), D = bf16(A) * bf16(Bm)^T.
+ * One 128 x N x K bf16 GEMM on wgmma (fp32 accumulate in registers), D = bf16(A) * bf16(Bm)^T.
  * A [128,K], Bm [N,K], D [128,N] fp32 row-major device pointers. mode 0: A from shared memory
- * (SS), 1: A from tensor memory (TS). layout 0/1 selects which of the two canonical no-swizzle
+ * (SS), 1: A from registers (RS). layout 0/1 selects which of the two canonical no-swizzle
  * K-major core-matrix arrangements is used; swap_fields exchanges the LBO/SBO descriptor fields.
  * Exists so that tests can pin the descriptor encodings the fused point-MLP kernel relies on. */
-/* Same as sonet_pointresnet_tc_forward, additionally writing clock64() stamps of the phase
- * boundaries of CTA 0's tile number timeline64[125] (host-set) into timeline64[128] (device): [0..31] MMA warp, [32..63] an
- * epilogue warp, [64..123] act0-ready time of every tile, [126] kernel start, [127] kernel end.
- * Used by tools/tc_timeline.py to see where a tile's cycles go. */
+/* Same as sonet_pointresnet_tc_forward, additionally writing clock64() stamps of CTA 0 into
+ * timeline64[128] (device): [126] kernel start, [127] kernel end. */
 int sonet_debug_pointresnet_tc_timeline(const float* x, int Cin, int B, int P, const void* blob,
                                         const float* fparams, float* out, long long* timeline64,
                                         sonet_stream_t stream);
 /* sonet_pointwise_tc_forward (single source, ReLU, no shift) with clock64() stamps of CTA 0 in
- * timeline128[128] (device): TMA issue / MMA waits+issue / converter / epilogue; tools/tc_timeline.py */
+ * timeline128[128] (device): [127] kernel start, [126] kernel end. */
 int sonet_debug_pointwise_tc_timeline(const float* x0, int C0, int B, int P, const void* blob,
                                       float inv_scale, int Cout, float* out, long long* timeline128,
                                       sonet_stream_t stream);
-/* Cycles for `iters` back-to-back M=128 x N x 16 fp16 MMAs issued by one CTA: mode 0 = A and B from
- * shared memory (SS, no-swizzle K-major, 8-row-group stride `sbo`), 1 = A from tensor memory (TS). */
+/* Cycles for `iters` back-to-back M=64 x N x 16 fp16 wgmmas issued by one warpgroup (N = 64, 96,
+ * 128 or 256), A and B from shared memory (no-swizzle K-major, 8-row-group stride `sbo`); mode must
+ * be 0. */
 int sonet_debug_tc_mma_rate(int mode, int N, int sbo, int iters, long long* cycles,
                             sonet_stream_t stream);
 int sonet_debug_pointresnet_tc_pool_timeline(const float* x_sorted, int Cin, int B, int P,

@@ -50,7 +50,7 @@ def build_ref(force=False):
     if not os.path.isdir(REF_SRC):
         return None
     os.makedirs(REFDIR, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "4")
     from torch.utils.cpp_extension import load
     scratch = os.path.join(REFDIR, "_scratch")

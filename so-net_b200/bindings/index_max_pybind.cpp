@@ -57,6 +57,6 @@ torch::Tensor forward_cpu(const torch::Tensor data, const torch::Tensor index, c
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("forward_cpu", &forward_cpu, "index_max forward (host, single thread)");
   m.def("forward_multi_thread_cpu", &forward_multi_thread_cpu, "index_max forward (host, threads)");
-  m.def("forward_cuda", &forward_cuda, "index_max forward (sm_100a kernel of libsonet_b200)");
+  m.def("forward_cuda", &forward_cuda, "index_max forward (sm_90a kernel of libsonet_b200)");
   m.def("forward_cuda_shared_mem", &forward_cuda, "same kernel");
 }

@@ -1,4 +1,4 @@
-"""Build libsonet_b200.so (C-ABI, no libtorch dependency) with nvcc for sm_100a, in-tree.
+"""Build libsonet_b200.so (C-ABI, no libtorch dependency) with nvcc for sm_90a, in-tree.
 
     python so-net_b200/build.py [--force] [--verbose]
 
@@ -18,7 +18,7 @@ LIB = os.path.join(LIBDIR, "libsonet_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--use_fast_math=false",
           "-Xptxas", "-v", "-I", INCLUDE]
 # --use_fast_math is NOT used: parity needs IEEE division/sqrt and no FMA contraction surprises

@@ -1,4 +1,4 @@
-// augment.cu — on-device training augmentation of a whole batch (SURVEY.md §8f-3) for sm_100a.
+// augment.cu — on-device training augmentation of a whole batch (SURVEY.md §8f-3) for sm_90a.
 //
 // Replaces the per-item numpy pipeline of the reference's loader
 // (data/modelnet_shrec_loader.py:218-247 calling data/augmentation.py:52-144): rotation about the

@@ -1,4 +1,4 @@
-// chamfer.cu — Chamfer distance of the auto-encoder for sm_100a.
+// chamfer.cu — Chamfer distance of the auto-encoder for sm_90a.
 //
 // Replaces ChamferLoss.forward (models/losses.py:237-290): the reference does, per cloud, two
 // Faiss IndexFlatL2 builds + two k=1 searches through host numpy (losses.py:247-276), then
@@ -6,8 +6,8 @@
 // with no host round trip, and BOTH directions come from ONE evaluation of each (pred, gt) pair:
 //
 //   chamfer_pair_kernel   a warp owns 256 gt points (8 per lane, in registers) and streams a tile
-//       of pred points from shared memory (broadcast LDS). The arithmetic is packed two columns
-//       per instruction (FADD2/FMUL2, sm_100's f32x2 ops: IEEE rn per half). Every squared distance is computed
+//       of pred points from shared memory (broadcast LDS). Two columns are kept per register
+//       pair, each half computed with explicitly rounded scalar ops (IEEE rn). Every squared distance is computed
 //       once — exact direct differences, ((dx*dx+dy*dy)+dz*dz) with separate roundings, the
 //       arithmetic of the brute-force oracle — and feeds the running minimum of its gt point
 //       (in-register FMNMX) and of its pred point (in-thread FMNMX over the lane's 8 columns, one
@@ -68,9 +68,8 @@ __global__ void __launch_bounds__(CH_WARPS * 32)
   __syncthreads();
   if (n0 >= N) return;                 // (after the only CTA-wide barrier but the last)
 
-  // NEGATED gt coordinates, two columns per register pair: p - g == p + (-g) bit for bit, and the
-  // packed add.rn.f32x2 / mul.rn.f32x2 (sm_100 FADD2/FMUL2) round each half like the scalar op —
-  // half the issue slots for the same arithmetic (the kernel is issue-bound, not pipe-bound)
+  // NEGATED gt coordinates, two columns per register pair: p - g == p + (-g) bit for bit, and each
+  // half is rounded like the reference's scalar op (common.cuh: add2_rn / mul2_rn)
   float2 ngx[CH_RN / 2], ngy[CH_RN / 2], ngz[CH_RN / 2];
   float cmin[CH_RN];
   int cidx[CH_RN];

@@ -61,4 +61,4 @@ int max_smem_optin() {
 }  // namespace sonet
 
 extern "C" const char* sonet_last_error_string(void) { return sonet::g_err; }
-extern "C" const char* sonet_version(void) { return "sonet_b200 0.2.0 sm_100a"; }
+extern "C" const char* sonet_version(void) { return "sonet_b200 0.2.0 sm_90a"; }

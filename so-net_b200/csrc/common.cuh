@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for libsonet_b200 (sm_100a only).
+// common.cuh — shared helpers for libsonet_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -63,28 +63,16 @@ __device__ __forceinline__ float ldg_stream_f1(const float* p) {
   return r;
 }
 
-// ---- packed fp32x2 arithmetic (sm_100 FADD2 / FMUL2): IEEE round-to-nearest per half ------------
-// Inline PTX with explicit .rn: the CUDA intrinsics __fmul2_rn/__fadd2_rn were observed to be
-// contracted into FFMA2 by nvcc 12.9, which changes the rounding of (dx*dx + dy*dy) + dz*dz and
-// with it the bit-exact distance parity the arg-min kernels rely on.
+// ---- fp32 pairs: IEEE round-to-nearest per half ---------------------------------------------------
+// sm_90 has no packed fp32x2 instructions; each half is one explicitly rounded scalar op. __fadd_rn /
+// __fmul_rn are never contracted into an FMA, which keeps (dx*dx + dy*dy) + dz*dz rounded like the
+// reference and with it the bit-exact distance parity the arg-min kernels rely on.
 __device__ __forceinline__ float2 add2_rn(float2 a, float2 b) {
-  unsigned long long r;
-  asm("add.rn.f32x2 %0, %1, %2;"
-      : "=l"(r)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&r);
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 }
 __device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) {
-  unsigned long long r;
-  asm("mul.rn.f32x2 %0, %1, %2;"
-      : "=l"(r)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&r);
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
-// NOTE: ptxas 12.9 contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 even with explicit .rn and
-// under --fmad=false (it also rewrites fma.rn.f32x2(a,b,-0) back into a mul and re-fuses it). Where
-// the separate rounding of a product and a sum matters, do the PRODUCT packed and the SUM with the
-// scalar __fadd_rn (explicitly rounded scalar ops are never contracted).
 __device__ __forceinline__ float2 sqsum3_rn(float2 dx, float2 dy, float2 dz) {
   const float2 xx = mul2_rn(dx, dx), yy = mul2_rn(dy, dy), zz = mul2_rn(dz, dz);
   return make_float2(__fadd_rn(__fadd_rn(xx.x, yy.x), zz.x), __fadd_rn(__fadd_rn(xx.y, yy.y), zz.y));

@@ -1,11 +1,11 @@
-// index_max.cu — per-node indexed arg-max pool for sm_100a.
+// index_max.cu — per-node indexed arg-max pool for sm_90a.
 //
 // Semantics follow the reference plugin (models/index_max_ext/index_max.cpp:73-112 and
 // index_max_cuda.cu:10-26): for data[B,C,N], index[B,N] in [0,K):
 //   max_idx[b,c,k] = first n (ascending) with index[b,n]==k that attains the maximum of
 //   data[b,c,n] over that node, if the maximum is > -1000.0f; else 0.
 //
-// B200 design (HBM-bound, 4 B/element must stream at ~6.5 TB/s):
+// Design (HBM-bound: 4 B/element must stream at close to the HBM bandwidth):
 //   * persistent grid, one CTA per SM; a work item is (b, group of NW channels); warp w of the CTA
 //     streams channel row c = group*NW + w with 128-bit no-allocate loads (fully coalesced, 4
 //     loads in flight per lane).

@@ -1,5 +1,5 @@
 // pointmlp_tc.cu — the first PointResNet (6|3 -> 64 -> 128 -> 256 -> [64+256] -> 384) of the SO-Net
-// encoder as ONE persistent tcgen05 kernel for sm_100a.
+// encoder as ONE persistent Hopper warpgroup-MMA (wgmma) kernel for sm_90a.
 //
 // Replaces Encoder.first_pointnet = PointResNet.forward (models/layers.py:419-432, wired at
 // models/networks.py:82-83,176): four EquivariantLayers (Conv1d k=1 + eval BatchNorm + ReLU,
@@ -7,44 +7,25 @@
 // FLOPs. The reference round-trips every activation through HBM (~7.4 GB at B=64,N=5000); here a
 // 128-point tile walks through all four layers inside one SM:
 //
-//   * points are the MMA M dimension (128 TMEM lanes = 128 point copies), channels are N/K;
-//   * layer 0 (K=3|6, degenerate for tensor cores) runs on CUDA cores, one thread per point;
-//   * layers 1-3 are tcgen05.mma kind::f16 with the ACTIVATIONS AS THE A OPERAND READ FROM TENSOR
-//     MEMORY: the epilogue warps read the fp32 accumulator (tcgen05.ld), add the folded-BN shift,
-//     ReLU, split into fp16 hi/lo and write the pair back IN PLACE over the accumulator columns
-//     (tcgen05.st) — a 16-channel group of fp32 columns becomes 8 hi + 8 lo packed columns, which
-//     is exactly the K-major A layout the next layer's MMA consumes. Activations never touch
-//     shared memory or HBM;
+//   * points are the MMA M dimension, channels are N/K. Two consumer warpgroups own 64 points of
+//     the tile each (wgmma M = 64) and run independently except for the shared weight stream;
+//   * layer 0 (K=3|6, degenerate for tensor cores) runs on CUDA cores, one thread per point and
+//     32 channels;
+//   * layers 1-3 are wgmma f16 with fp32 accumulators in registers. The epilogue of a layer adds
+//     the folded-BN shift, applies the ReLU, splits into fp16 hi/lo and writes the pair straight
+//     into the K-major no-swizzle A image of the next layer in the warpgroup's own shared-memory
+//     region — activations never touch HBM. act2 overwrites act1 once layer 2's wgmmas are done;
 //   * fp32 parity (1e-4) on 16-bit tensor cores comes from the 3-product split
 //     x*w ~= hi(x)*hi(w) + lo(x)*hi(w) + hi(x)*lo(w) with FP16 halves (hi+lo carry 22 mantissa
 //     bits; the same split in bf16 carries 16 and measured 1.1e-4, outside the bar). Weights are
 //     pre-scaled per layer by a power of two (undone exactly in the epilogue FMA) so their lo
 //     halves stay normal fp16 numbers; activations saturate at the fp16 range (65504) in the conversion;
 //   * weights (B operand, K-major no-swizzle core-matrix images packed once by the host) stream
-//     L2 -> shared memory through a 5-slot TMA ring (cp.async.bulk + mbarrier); layer-1 weights
-//     stay resident;
-//   * MMA shapes are as wide as TMEM allows (the first version issued 480 N=64 MMAs per tile and
-//     was issue-bound): layer 1 = 12 MMAs of N=128, layer 2 = 24 of N=256, layer 3 = 4 chunks x
-//     60 of N=96 over two accumulator buffers (a chunk's epilogue overlaps the next chunk's
-//     MMAs): 276 MMAs per tile;
-//   * the MMA issue runs in the UNIFORM datapath: one asm statement per K stage (one elect.sync,
-//     addresses advanced inside the PTX, tc::mma_ts_stage), mbarrier waits as single asm loops and
-//     a shuffle-broadcast warp index let ptxas keep descriptors in uniform registers (UIADD3 +
-//     UTCHMMA, ~5 instructions per MMA). One asm statement per MMA cost 4 R2UR + ELECT + votes
-//     (~50 issue cycles, as long as an N=96 MMA executes); issuing from a divergent
-//     `if (lane == 0)` is worse still (nvcc wraps every UTCHMMA in an ELECT/BRA loop);
-//   * layers overlap inside a tile through fine-grained barriers: each layer-2 K slab waits only
-//     for its 32 act1 channels, layer-3 chunk 0 starts when layer 2's MMAs complete and each of
-//     its K stages waits only for its act2 quarter; the next tile's layer 0 is computed while the
-//     last chunk's MMAs run (b_a0free), and that chunk is read out and PARKED in registers so the
-//     next tile starts at once (its pooling happens inside the next tile's layer-2 MMA window);
-//   * code size is a first-order constraint: stage loops are not unrolled and the big blocks
-//     have one call site each (2.3 k SASS instructions; the first version's 9 k hot instructions
-//     cost 22 % of its non-idle stall samples in instruction fetch);
-//   * warp roles: warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-11
-//     epilogue (two warpgroups splitting the columns; warp%4 selects the TMEM lane quarter);
-//   * TMEM map (512 columns): [0,64) act0 | [64,320) D2/act2 | [320,448) D1/act1, and after
-//     layer 2: [320,416), [416,512) the two D3 buffers.
+//     L2 -> shared memory through a 2-slot ring (cp.async.bulk + mbarrier), 25 stages per tile:
+//     layer 1 (N=128), four layer-2 K slabs (N=256), 4 chunks x 5 K slabs of layer 3 (N=96);
+//   * shared memory: 2 x 80 KB activation regions + 2 x 32 KB weight slots = 224 KB of the 227 KB
+//     a block may use on H100;
+//   * warp roles: warps 0-7 the two consumer warpgroups, warp 8 the TMA producer.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -56,53 +37,43 @@ namespace sonet {
 
 namespace pm {
 constexpr int C0 = 64, C1 = 128, C2 = 256, C3 = 384, K3 = C0 + C2;  // layer widths
-constexpr int TILE = 128;                                            // points per tile (MMA M)
-constexpr int SLOT_BYTES = 32768, NSLOT = 5;
+constexpr int TILE = 128;                                            // points per tile
+constexpr int SLOT_BYTES = 32768, NSLOT = 2;
 constexpr int W1_BYTES = 2 * C1 * C0 * 2;                            // hi + lo images, 32 KB
 constexpr int L2_STAGES = 4, L2_KT = 32;                             // [256 rows x 32 k] per stage
 constexpr int L3_CHUNKS = 4, L3_N = 96, L3_KSTAGES = 5, L3_KT = 64;  // [96 rows x 64 k] per stage
 constexpr int L2_STAGE_BYTES = C2 * L2_KT * 2 * 2;                   // 32768
 constexpr int L3_STAGE_BYTES = L3_N * L3_KT * 2 * 2;                 // 24576
-constexpr int STAGES_PER_TILE = L2_STAGES + L3_CHUNKS * L3_KSTAGES;  // 24
+constexpr int STAGES_PER_TILE = 1 + L2_STAGES + L3_CHUNKS * L3_KSTAGES;  // 25
 constexpr int BLOB_BYTES =
     W1_BYTES + L2_STAGES * L2_STAGE_BYTES + L3_CHUNKS * L3_KSTAGES * L3_STAGE_BYTES;  // 655360
 constexpr int NFP = C0 * 6 + C0 + C1 + C2 + C3 + 4;   // W0 | shift0..3 | 1/wscale1..3 (floats)
-constexpr int NUM_THREADS = 384;
-constexpr int NBAR = 2 * NSLOT + 3 + 4 + 4 + 4 + 2;
-// shared memory carve-up
-constexpr int OFF_W1 = 0;
-constexpr int OFF_RING = OFF_W1 + W1_BYTES;
-constexpr int OFF_FP = OFF_RING + NSLOT * SLOT_BYTES;
-constexpr int OFF_BAR = OFF_FP + NFP * 4;
-constexpr int OFF_TMEM = OFF_BAR + NBAR * 8;
-constexpr int SMEM_BYTES = OFF_TMEM + 16;
-// TMEM columns
-constexpr uint32_t COL_A0 = 0, COL_D2 = 64, COL_D1 = 320, COL_D3 = 320;
+constexpr int NUM_THREADS = 288;
+// per-warpgroup activation region: act0 [64 x 64] hi | lo, then act1 [64 x 128] / act2 [64 x 256]
+constexpr int ACT0_HALF = 64 * C0 * 2;                 // 8 KB
+constexpr int ACT1_HALF = 64 * C1 * 2;                 // 16 KB
+constexpr int ACT2_HALF = 64 * C2 * 2;                 // 32 KB
+constexpr int OFF_ACT12 = 2 * ACT0_HALF;
+constexpr int REGION_BYTES = OFF_ACT12 + 2 * ACT2_HALF;   // 80 KB
+constexpr int OFF_RING = 2 * REGION_BYTES;
+constexpr int OFF_W0 = OFF_RING + NSLOT * SLOT_BYTES;     // W0 | shift0 (floats)
+constexpr int OFF_BAR = OFF_W0 + (C0 * 6 + C0) * 4;
+constexpr int NBAR = 2 * NSLOT;
+constexpr int SMEM_BYTES = OFF_BAR + NBAR * 8;
 
 __host__ __device__ constexpr int stage_bytes(int s) {
-  return s < L2_STAGES ? L2_STAGE_BYTES : L3_STAGE_BYTES;
-}
-// descriptor: lo word = start address >> 4 | (LBO=128 >> 4) << 16; hi word = SBO >> 4 | version 1.
-// Advancing the start address by n bytes is desc + (n >> 4).
-__device__ __forceinline__ uint64_t bdesc(uint32_t saddr, uint32_t sbo) {
-  const uint32_t lo = ((saddr & 0x3FFFFu) >> 4) | (8u << 16);
-  const uint32_t hi = (sbo >> 4) | (1u << 14);
-  return (static_cast<uint64_t>(hi) << 32) | lo;
+  return s == 0 ? W1_BYTES : (s <= L2_STAGES ? L2_STAGE_BYTES : L3_STAGE_BYTES);
 }
 }  // namespace pm
 
-// CL = thread-block-cluster size: the CL CTAs of a cluster consume the same weight stream, each
-// fetches 1/CL of every stage from L2 and multicasts it into all CL shared memories. Measured: no
-// gain at CL=2 and a loss at CL=4 (the stream is not the bound; lockstep coupling costs), so the
-// default is CL=1; kept as a tested option (SONET_TC_CLUSTER).
-//
 // POOL variant (the classifier / auto-encoder path): the input rows are the stacked copies SORTED
 // BY NODE (csrc/som_sort.cu) and the layer-3 epilogue, instead of storing the 384 channels of
 // every copy (1.47 GB at B=64,N=5000) for a separate index_max launch to re-read, reduces them
-// per node right away: for every run of lanes that share a node (one run in 87 % of the warps)
-// a shuffle transpose-reduce over the RAW accumulators leaves one channel's maximum per lane
-// pair, which then applies scale/shift, converts to an order-preserving integer key and issues
-// ONE 16-lane `red.global.max` into keys[b,c,node]. models/index_max_ext semantics (max must be
+// per node right away: for every run of rows in a warp that share a node (rows are node-sorted,
+// so usually one) a shuffle reduction over the RAW accumulators leaves each column's maximum in
+// lanes 0-3, which apply scale/shift, convert to an order-preserving integer key and issue
+// `red.global.max` into keys[b,c,node]. y = fmaf(raw, inv3 > 0, shift) is monotone, so
+// max_rows(y) == fmaf(max_rows(raw), ...) bit for bit. models/index_max_ext semantics (max must be
 // > -1000, else the feature of copy 0) are restored when the keys are read
 // (knn_assemble_pool_kernel / pool_finalize_kernel). first_pn_out is never written.
 struct PoolArgs {
@@ -113,484 +84,308 @@ struct PoolArgs {
   int M;
 };
 
-template <int CL, bool POOL>
+template <bool POOL>
 __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     pointresnet_tc_kernel(const float* __restrict__ x_in, int Cin, int B, int P,
                           const unsigned char* __restrict__ blob, const float* __restrict__ fparams,
                           float* __restrict__ out, long long* __restrict__ dbg, PoolArgs pool) {
   using namespace pm;
-  // optional timeline (debug entry point only): clock64 at phase boundaries of CTA 0's tile
-  // number dbg[125] (set by the host before the launch)
-  const int tl_tile = (dbg != nullptr) ? static_cast<int>(dbg[125]) : -1;
-#define PM_TL(role, idx)                                                          \
-  do {                                                                            \
-    if (dbg != nullptr && blockIdx.x == 0 && t == tl_tile && lane == 0)           \
-      dbg[(role) * 32 + (idx)] = clock64();                                       \
-  } while (0)
   extern __shared__ __align__(1024) unsigned char smem[];
-  float* fp = reinterpret_cast<float*>(smem + OFF_FP);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* full = bars;                   // [NSLOT]  TMA -> MMA
-  uint64_t* empty = bars + NSLOT;          // [NSLOT]  MMA -> TMA
-  uint64_t* b_act0 = bars + 2 * NSLOT;     // epilogue -> MMA
-  uint64_t* b_d1 = b_act0 + 1;             // MMA -> epilogue
-  uint64_t* b_d2 = b_act0 + 2;
-  uint64_t* b_act1s = b_act0 + 3;          // [4] one per layer-2 K slab (32 act1 channels)
-  uint64_t* b_act2q = b_act1s + 4;         // [4] one per layer-3 K stage (64 act2 channels)
-  uint64_t* d3full = b_act2q + 4;          // [2]
-  uint64_t* d3empty = d3full + 2;          // [2]
-  uint64_t* w1_full = d3empty + 2;
-  uint64_t* b_a0free = w1_full + 1;        // MMA -> epilogue: act0 of this tile is no longer read
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + OFF_TMEM);
+  float* w0s = reinterpret_cast<float*>(smem + OFF_W0);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + OFF_BAR);   // [NSLOT] TMA -> MMA
+  uint64_t* empty = full + NSLOT;                                  // [NSLOT] MMA -> TMA
 
-  // warp index through a shuffle: tells ptxas it is warp-uniform, so the role branches below are
-  // convergent regions and the MMA warp's address arithmetic can live in uniform registers
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[64 + 62] = clock64();
   const int tiles_per_cloud = (P + TILE - 1) / TILE;
   const int num_tiles = B * tiles_per_cloud;
-  // every CTA runs the same number of iterations (a cluster consumes the weight stream in
-  // lockstep); iterations past the last tile compute on zeros and store nothing
-  const int my_tiles = (num_tiles + gridDim.x - 1) / gridDim.x;
-  constexpr uint16_t CL_MASK = static_cast<uint16_t>((1u << CL) - 1);
-  const uint32_t cta_rank = (CL > 1) ? tc::cluster_ctarank() : 0;
+  const int my_tiles = (static_cast<int>(blockIdx.x) < num_tiles)
+                           ? (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
-  for (int i = threadIdx.x; i < NFP; i += NUM_THREADS) fp[i] = fparams[i];
+  for (int i = threadIdx.x; i < C0 * 6 + C0; i += NUM_THREADS) w0s[i] = fparams[i];
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSLOT; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], CL);
+      mbar_init(&empty[s], 8);   // one arrival per consumer warp
     }
-    mbar_init(b_act0, 8);
-    mbar_init(b_d1, 1);
-    mbar_init(b_d2, 1);
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&b_act1s[i], 8);
-      mbar_init(&b_act2q[i], 8);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&d3full[i], 1);
-      mbar_init(&d3empty[i], 8);
-    }
-    mbar_init(w1_full, 1);
-    mbar_init(b_a0free, 1);
     mbar_fence_init();
   }
-  if (warp == 2) {
-    tc::tmem_alloc(tmem_ptr, 512);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
   __syncthreads();
-  if (CL > 1) tc::cluster_sync_all();   // peers' barriers are initialised before any multicast lands
-  tc::fence_after_sync();
-  // All 512 columns are allocated, so the allocation base is column 0 / lane 0 by construction;
-  // using the constant keeps every TMEM address an immediate (checked once here).
-  if (*tmem_ptr != 0u) __trap();
-  constexpr uint32_t tm = 0;
 
-  // Code-size discipline: every stage loop below is deliberately NOT unrolled and every large
-  // block (layer 0, the chunk epilogue) has exactly one call site. The first version of this kernel
-  // was ~9k hot SASS instructions (147 KB) and ncu attributed 22 % of its non-idle stall samples to
-  // instruction fetch (stall_no_inst); see profiles/r01_summary.md.
-  if (warp == 0) {
+  if (warp == 8) {
     // =========================== TMA producer ===========================
     if (lane == 0) {
-      mbar_arrive_expect_tx(w1_full, W1_BYTES);
-      bulk_g2s(smem + OFF_W1, blob, W1_BYTES, w1_full);
-      uint32_t slot = 0, use_par = 1;     // parity of the `empty` phase that frees `slot` (first lap: free)
+      uint32_t q = 0;
 #pragma unroll 1
       for (int t = 0; t < my_tiles; ++t) {
-        uint32_t off = W1_BYTES;
+        uint32_t off = 0;
 #pragma unroll 1
-        for (int s = 0; s < STAGES_PER_TILE; ++s) {
-          if (t > 0 || s >= NSLOT) tc::mbar_wait_relaxed(&empty[slot], use_par, 100 + s);
+        for (int s = 0; s < STAGES_PER_TILE; ++s, ++q) {
+          const uint32_t slot = q % NSLOT, use = q / NSLOT;
+          if (use > 0) tc::mbar_wait_relaxed(&empty[slot], (use - 1) & 1, 100 + s);
           const uint32_t bytes = stage_bytes(s);
-          mbar_arrive_expect_tx(&full[slot], bytes);   // all CL slices land on this barrier
-          if (CL == 1) {
-            bulk_g2s(smem + OFF_RING + slot * SLOT_BYTES, blob + off, bytes, &full[slot]);
-          } else {
-            const uint32_t slice = bytes / CL;
-            tc::bulk_g2s_multicast(smem + OFF_RING + slot * SLOT_BYTES + cta_rank * slice,
-                                   blob + off + cta_rank * slice, slice, &full[slot], CL_MASK);
-          }
+          mbar_arrive_expect_tx(&full[slot], bytes);
+          bulk_g2s(smem + OFF_RING + slot * SLOT_BYTES, blob + off, bytes, &full[slot]);
           off += bytes;
-          if (++slot == NSLOT) {
-            slot = 0;
-            use_par ^= 1;
-          }
         }
       }
     }
-  } else if (warp == 1) {
-    // ============ MMA issuer: the warp stays converged, elect.sync issues from one lane ============
-    constexpr uint32_t ID1 = tc::idesc_f16_f32(TILE, C1), ID2 = tc::idesc_f16_f32(TILE, C2),
-                       ID3 = tc::idesc_f16_f32(TILE, L3_N);
-    // addresses through the compiler-visible cvta (not inline asm): candidates for the uniform path
-    const uint32_t w1_addr = static_cast<uint32_t>(__cvta_generic_to_shared(smem + OFF_W1));
-    const uint32_t ring_addr = static_cast<uint32_t>(__cvta_generic_to_shared(smem + OFF_RING));
-    tc::mbar_wait_bounded(w1_full, 0, 1);
-    uint32_t slot = 0, full_par = 0;
-    auto next_slot = [&]() {
-      if (++slot == NSLOT) {
-        slot = 0;
-        full_par ^= 1;
-      }
-    };
-    auto release_slot = [&]() {
-      if (CL == 1) tc::commit_elect(&empty[slot]);
-      else tc::commit_multicast_elect(&empty[slot], CL_MASK);
-    };
-#pragma unroll 1
-    for (int t = 0; t < my_tiles; ++t) {
-      const uint32_t par = t & 1;
-      // ---- layer 1: D1[128 x 128] = act0[128 x 64] * W1^T (one N=128 MMA per product) ----
-      tc::mbar_wait_bounded(b_act0, par, 2);
-      if (t > 0) {  // D1 overlaps both D3 buffers of the previous tile: wait for their last drain
-        tc::mbar_wait_bounded(&d3empty[0], 1, 3);
-        tc::mbar_wait_bounded(&d3empty[1], 1, 4);
-      }
-      tc::fence_after_sync();
-      PM_TL(0, 0);
-      if (dbg != nullptr && blockIdx.x == 0 && lane == 0 && t < 60) dbg[64 + t] = clock64();
-      tc::mma_ts_stage<4>(tm + COL_D1, tm + COL_A0, bdesc(w1_addr, 1024),
-                          bdesc(w1_addr + W1_BYTES / 2, 1024), ID1, 0);
-      tc::commit_elect(b_d1);
-      PM_TL(0, 1);
-      // ---- layer 2: D2[128 x 256] = act1[128 x 128] * W2^T: 4 streamed K slabs of 32, N=256.
-      // Each slab starts as soon as ITS 32 act1 channels are converted (per-slab barriers), so
-      // the layer-1 epilogue overlaps the layer-2 MMAs ----
-#pragma unroll 1
-      for (int kc = 0; kc < L2_STAGES; ++kc) {
-        tc::mbar_wait_bounded(&b_act1s[kc], par, 5);
-        if (kc == 0) PM_TL(0, 2);
-        tc::mbar_wait_bounded(&full[slot], full_par, 6);
-        tc::fence_after_sync();
-        const uint32_t sb = ring_addr + slot * SLOT_BYTES;
-        tc::mma_ts_stage<2>(tm + COL_D2, tm + COL_D1 + 32 * kc, bdesc(sb, 512),
-                            bdesc(sb + L2_STAGE_BYTES / 2, 512), ID2, kc != 0);
-        release_slot();
-        next_slot();
-      }
-      tc::commit_elect(b_d2);
-      PM_TL(0, 3);
-      // ---- layer 3: D3[128 x 384] = cat(act0, act2)[128 x 320] * W3^T: 4 chunks of N=96.
-      // Chunk 0 starts when layer 2's MMAs are complete (its accumulator aliases act1): K stage 0
-      // reads act0, K stage s >= 1 waits for act2 quarter s-1 only (already complete for chunks
-      // 1-3, where the wait falls through), so the layer-2 epilogue overlaps chunk 0's MMAs ----
-      tc::mbar_wait_bounded(b_d2, par, 7);
-      tc::fence_after_sync();
-      PM_TL(0, 4);
-#pragma unroll 1
-      for (int nc = 0; nc < L3_CHUNKS; ++nc) {
-        const int buf = nc & 1;
-        if (nc >= 2) tc::mbar_wait_bounded(&d3empty[buf], 0, 8);   // drain of chunk nc-2 (this tile)
-        tc::fence_after_sync();
-        const uint32_t d = tm + COL_D3 + L3_N * buf;
-        PM_TL(0, 5 + 2 * nc);
-#pragma unroll 1
-        for (int kc = 0; kc < L3_KSTAGES; ++kc) {
-          if (kc > 0) tc::mbar_wait_bounded(&b_act2q[kc - 1], par, 9);
-          tc::mbar_wait_bounded(&full[slot], full_par, 10);
-          tc::fence_after_sync();
-          const uint32_t sb = ring_addr + slot * SLOT_BYTES;
-          // 16-channel K groups: stage 0 = act0 (4 groups), stages 1-4 = act2 quarters
-          const uint32_t a0 = tm + (kc == 0 ? COL_A0 : COL_D2 + 64 * (kc - 1));
-          tc::mma_ts_stage<4>(d, a0, bdesc(sb, 1024), bdesc(sb + L3_STAGE_BYTES / 2, 1024), ID3,
-                              kc != 0);
-          // the last chunk's first K stage is the tile's last reader of act0
-          if (nc == L3_CHUNKS - 1 && kc == 0) tc::commit_elect(b_a0free);
-          release_slot();
-          next_slot();
-        }
-        tc::commit_elect(&d3full[buf]);
-        PM_TL(0, 6 + 2 * nc);
-      }
-    }
-  } else if (warp >= 4) {
-    // =========================== epilogue warps ===========================
-    const int q4 = warp & 3;            // TMEM lane quarter this warp may access
-    const int h = (warp - 4) >> 2;      // column half handled by this warpgroup
-    const int r = q4 * 32 + lane;       // point within the tile == TMEM lane
-    const uint32_t lane_base = tm + (static_cast<uint32_t>(q4 * 32) << 16);
-    const float* W0 = fp;
-    const float* sh0 = fp + C0 * 6;
-    const float* sh1 = sh0 + C0;
+  } else {
+    // =========================== consumer warpgroups ===========================
+    constexpr unsigned FULL = 0xffffffffu;
+    const int wg = warp >> 2;
+    const int tw = threadIdx.x & 127;
+    unsigned char* region = smem + wg * REGION_BYTES;
+    const uint32_t act0_a = smem_u32(region), act12_a = smem_u32(region + OFF_ACT12);
+    const uint32_t ring_a = smem_u32(smem + OFF_RING);
+    const float* sh1 = fparams + C0 * 6 + C0;
     const float* sh2 = sh1 + C1;
     const float* sh3 = sh2 + C2;
-    const float inv1 = sh3[C3], inv2 = sh3[C3 + 1], inv3 = sh3[C3 + 2];  // 1 / weight pre-scale
-    constexpr unsigned FULL = 0xffffffffu;
+    const float inv1 = __ldg(sh3 + C3), inv2 = __ldg(sh3 + C3 + 1), inv3 = __ldg(sh3 + C3 + 2);
+    // accumulator fragment: rows r0 = 16*(warp%4) + lane/4 and r0 + 8 of the warpgroup's 64,
+    // columns 8j + 2*(lane%4) + {0,1} (registers 4j+{0,1} for r0, 4j+{2,3} for r0 + 8)
+    const int r0 = 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    uint32_t q = 0;   // weight stages consumed
 
-    float xn[6];                        // layer-0 inputs of the NEXT tile, prefetched
-    auto prefetch_x = [&](int tn) {
-      const int tile_n = blockIdx.x + tn * gridDim.x;
-      const int bn = tile_n / tiles_per_cloud;
-      const int jn = (tile_n - bn * tiles_per_cloud) * TILE + r;
-      const bool vn = (tile_n < num_tiles) && (jn < P);
-#pragma unroll
-      for (int c = 0; c < 6; ++c)
-        xn[c] = (vn && c < Cin) ? __ldg(x_in + (static_cast<size_t>(bn) * Cin + c) * P + jn) : 0.f;
+    auto stage_wait = [&]() -> uint32_t {
+      const uint32_t slot = q % NSLOT;
+      tc::mbar_wait_bounded(&full[slot], (q / NSLOT) & 1, 1);
+      return ring_a + slot * SLOT_BYTES;
     };
-    // Max of 16 channels over the warp's 32 rows as a shuffle transpose-reduce: recursive halving
-    // (xor 16, 8, 4, 2, then 1) leaves the max of channel c(lane) = lane bits 4..1 (bit 4 = MSB) in
-    // every lane pair after 16 shuffles — one per channel. (48 redux.sync per chunk serialise on
-    // two uniform registers: measured 4.7-5.8k cycles per chunk.) It runs on the RAW accumulators:
-    // y = fmaf(raw, inv3 > 0, shift) is monotone, so max_rows(y) == fmaf(max_rows(raw), ...) bit
-    // for bit and the affine map + key conversion are paid once per lane, not once per element.
-    auto tmax16 = [&](const float (&k16)[16]) {
-      float a8[8], b4[4], c2[2];
-      {
-        const bool hi = (lane & 16) != 0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float keep = hi ? k16[8 + i] : k16[i], send = hi ? k16[i] : k16[8 + i];
-          a8[i] = fmaxf(keep, __shfl_xor_sync(FULL, send, 16));
-        }
-      }
-      {
-        const bool hi = (lane & 8) != 0;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float keep = hi ? a8[4 + i] : a8[i], send = hi ? a8[i] : a8[4 + i];
-          b4[i] = fmaxf(keep, __shfl_xor_sync(FULL, send, 8));
-        }
-      }
-      {
-        const bool hi = (lane & 4) != 0;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const float keep = hi ? b4[2 + i] : b4[i], send = hi ? b4[i] : b4[2 + i];
-          c2[i] = fmaxf(keep, __shfl_xor_sync(FULL, send, 4));
-        }
-      }
-      const bool hi = (lane & 2) != 0;
-      const float keep = hi ? c2[1] : c2[0], send = hi ? c2[0] : c2[1];
-      const float d1 = fmaxf(keep, __shfl_xor_sync(FULL, send, 2));
-      return fmaxf(d1, __shfl_xor_sync(FULL, d1, 1));
+    auto stage_release = [&](uint32_t qq) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[qq % NSLOT]);
     };
-    const int my_chan = ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 +
-                        ((lane >> 1) & 1);
+    // fp32 accumulator pair (row r, columns k, k+1) -> fp16 hi/lo words of an A image with SBO sbo
+    auto put_pair = [&](unsigned char* img_hi, int half_bytes, int sbo, int r, int k, float a, float b) {
+      uint32_t hi, lo;
+      tc::split2_f16(a, b, hi, lo);
+      const int off = (r >> 3) * sbo + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2;
+      *reinterpret_cast<uint32_t*>(img_hi + off) = hi;
+      *reinterpret_cast<uint32_t*>(img_hi + half_bytes + off) = lo;
+    };
+    auto publish = [&]() {   // A-image writes of this warpgroup -> its next wgmmas
+      tc::fence_proxy_async();
+      tc::named_sync(1 + wg, 128);
+    };
 
-    // The tile whose layer-3 chunks are being finished (plain scalars: a struct went to local
-    // memory). During the first step of an iteration they still describe the PREVIOUS tile.
-    int cx_b = 0, cx_nd = -1;
-    unsigned cx_vmask = 0;              // lanes holding a real row
-    bool cx_valid = false, cx_is_p0 = false, cx_any_p0 = false;
-    float* cx_orow = nullptr;
-
-    // POOL: per-node max of 16 channels. Rows are node-sorted, so the lanes of a warp fall into
-    // 1 (87 % of warps on the bench input), 2 or rarely more runs of equal node id; one pass of
-    // the loop per run: masked transpose-reduce, then the even lanes issue ONE 16-lane RED.MAX.
-    // The trip count is warp-uniform by construction.
-    auto pool_group = [&](const uint32_t (&v)[16], int cbase) {
-      const int co = cbase + my_chan;             // the channel this lane pair ends up owning
-      int32_t* kb = pool.keys + (static_cast<size_t>(cx_b) * C3 + co) * pool.M;
-      const float shift = sh3[co];
-      unsigned rem = cx_vmask;
 #pragma unroll 1
-      while (rem != 0) {
-        const int node = __shfl_sync(FULL, cx_nd, __ffs(rem) - 1);
-        const bool in = (cx_nd == node);
-        const unsigned run = __ballot_sync(FULL, in);
-        float ka[16];
-        if (run == FULL) {                        // the whole warp is one node: nothing to mask
-#pragma unroll
-          for (int i = 0; i < 16; ++i) ka[i] = __uint_as_float(v[i]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) ka[i] = in ? __uint_as_float(v[i]) : -INFINITY;
-        }
-        const int bits = __float_as_int(fmaf(tmax16(ka), inv3, shift));
-        const int key = bits ^ ((bits >> 31) & 0x7fffffff);   // order-preserving float -> int
-        if (!(lane & 1)) atomicMax(kb + node, key);
-        rem &= ~run;
-      }
-      if (cx_any_p0) {              // warp-uniform and rare: one warp per cloud and column half
-        if (cx_is_p0) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            pool.p0[static_cast<size_t>(cx_b) * C3 + cbase + i] =
-                fmaf(__uint_as_float(v[i]), inv3, sh3[cbase + i]);
-        }
-      }
-    };
-    auto store_group = [&](const uint32_t (&v)[16], int cbase) {   // lane = point: coalesced
-      float* o = cx_orow + static_cast<size_t>(cbase) * P;           // pointer bump, no 64-bit multiply
-#pragma unroll                                                       // per element (csrc/pointwise_tc.cu)
-      for (int i = 0; i < 16; ++i) {
-        *o = fmaf(__uint_as_float(v[i]), inv3, sh3[cbase + i]);
-        o += P;
-      }
-    };
-
-    uint32_t v0[16], v1[16], v2[16];    // this warp's 48 accumulator columns of one chunk
-    bool parked = false;                // v0..v2 hold the previous tile's last chunk
-    if (my_tiles > 0) prefetch_x(0);
-    // Iteration t: layer-1/2 epilogues of tile t, then the chunk steps. Step -1 finishes the chunk
-    // parked by tile t-1 (its pooling runs while this tile's layer-2 MMAs execute) and runs the
-    // layer-2 epilogue; steps 0..3 read chunk nc out of TMEM, release the buffer and finish it at
-    // once — except the last chunk, which stays parked. Before reading the last chunk (its MMAs
-    // are still running, but act0 is free: b_a0free) the NEXT tile's layer 0 is computed, so the
-    // MMA warp can start that tile the moment the chunk has been read. Iteration -1 only computes
-    // the first tile's layer 0; iteration my_tiles only drains the last parked chunk.
-#pragma unroll 1
-    for (int t = -1; t <= my_tiles; ++t) {
-      const bool live = t >= 0 && t < my_tiles;
+    for (int t = 0; t < my_tiles; ++t) {
       const int tile = blockIdx.x + t * gridDim.x;
       const int b = tile / tiles_per_cloud;
-      const int j = (tile - b * tiles_per_cloud) * TILE + r;
-      const bool valid = live && (tile < num_tiles) && (j < P);
-      const uint32_t par = t & 1;
-      int nd_next = -1, p0row = -1;
-      if (live) {
-        if (warp == 4) PM_TL(1, 1);
-        // this tile's node ids / copy-0 row: their L2 latency hides behind layers 1-2
-        if (POOL) {
-          if (valid) nd_next = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + j);
-          p0row = __ldg(pool.pos0 + b);
-        }
+      const int jbase = (tile - b * tiles_per_cloud) * TILE + wg * 64;   // first point of this warpgroup
 
-        // ---- layer 1 epilogue, in place: K slab kc of layer 2 = act1 channels [32kc, 32kc+32),
-        // 16 per warpgroup, announced slab by slab ----
-        tc::mbar_wait_bounded(b_d1, par, 20);
-        tc::fence_after_sync();
-        if (warp == 4) PM_TL(1, 2);
-#pragma unroll 1
-        for (int kc = 0; kc < 4; ++kc) {
-          const int ch0 = 32 * kc + 16 * h;
-          uint32_t v[16];
-          tc::ld16(lane_base + COL_D1 + ch0, v);
-          tc::wait_ld();
-          float y[16];
+      // ---- layer 0 on CUDA cores: point m, channels [32 half, 32 half + 32) ----
+      {
+        const int m = tw & 63, half = tw >> 6;
+        const int j = jbase + m;
+        float xv[6];
 #pragma unroll
-          for (int i = 0; i < 16; ++i)
-            y[i] = fmaxf(fmaf(__uint_as_float(v[i]), inv1, sh1[ch0 + i]), 0.f);   // split16_f16 saturates
-          tc::split16_f16(y, v);
-          tc::st16(lane_base + COL_D1 + ch0, v);
-          tc::wait_st();
-          tc::fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&b_act1s[kc]);
+        for (int c = 0; c < 6; ++c)
+          xv[c] = (j < P && c < Cin) ? __ldg(x_in + (static_cast<size_t>(b) * Cin + c) * P + j) : 0.f;
+        unsigned char* a_hi = region + (m >> 3) * 1024 + (m & 7) * 16;
+#pragma unroll
+        for (int o = 0; o < 4; ++o) {
+          uint32_t hi[4], lo[4];
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            float y[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int ch = half * 32 + o * 8 + 2 * jj + e;
+              float a = w0s[C0 * 6 + ch];
+#pragma unroll
+              for (int c = 0; c < 6; ++c) a = fmaf(w0s[ch * 6 + c], xv[c], a);
+              y[e] = fmaxf(a, 0.f);
+            }
+            tc::split2_f16(y[0], y[1], hi[jj], lo[jj]);
+          }
+          const int oct = half * 4 + o;
+          *reinterpret_cast<uint4*>(a_hi + oct * 128) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+          *reinterpret_cast<uint4*>(a_hi + ACT0_HALF + oct * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
         }
-        if (warp == 4) PM_TL(1, 3);
-
+        publish();
       }
 
-      // ---- layer 3 epilogue: four chunks of 96 channels, 48 per warpgroup; bare layer (no ReLU) ----
-      const int nc_begin = (t < 0) ? L3_CHUNKS - 1 : -1;
-      const int nc_end = (live || t < 0) ? L3_CHUNKS : 0;
-#pragma unroll 1
-      for (int nc = nc_begin; nc < nc_end; ++nc) {
-        if (nc == L3_CHUNKS - 1 && t + 1 < my_tiles) {
-          // ---- layer 0 of tile t+1 on CUDA cores (32 of the 64 channels per warpgroup, from the
-          // prefetched xn[]), as soon as tile t's MMAs no longer read act0 ----
-          if (t >= 0) {
-            tc::mbar_wait_bounded(b_a0free, par, 23);
-            tc::fence_after_sync();
-          }
-          if (warp == 4) PM_TL(1, 0);
-#pragma unroll 1
-          for (int g = 0; g < 2; ++g) {
-            const int ch0 = 32 * h + 16 * g;
-            float y[16];
+      // ---- layer 1: D1[64 x 128] = act0[64 x 64] * W1^T ----
+      {
+        float acc[64];
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float* w = W0 + (ch0 + i) * 6;
-              float a = sh0[ch0 + i];
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        const uint32_t sb = stage_wait();
+        tc::wg_fence();
 #pragma unroll
-              for (int c = 0; c < 6; ++c) a = fmaf(w[c], xn[c], a);
-              y[i] = fmaxf(a, 0.f);
-            }
-            uint32_t wds[16];
-            tc::split16_f16(y, wds);
-            tc::st16(lane_base + COL_A0 + ch0, wds);
-          }
-          tc::wait_st();
-          tc::fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(b_act0);
+        for (int ks = 0; ks < 4; ++ks) {
+          const uint64_t ah = tc::smem_desc(act0_a + ks * 256, 128, 1024),
+                         al = tc::smem_desc(act0_a + ACT0_HALF + ks * 256, 128, 1024),
+                         bh = tc::smem_desc(sb + ks * 256, 128, 1024),
+                         bl = tc::smem_desc(sb + W1_BYTES / 2 + ks * 256, 128, 1024);
+          tc::wgmma_f16_n128(acc, ah, bh, 1);
+          tc::wgmma_f16_n128(acc, al, bh, 1);
+          tc::wgmma_f16_n128(acc, ah, bl, 1);
         }
-        if (nc == 0) {                  // from here on the chunks belong to tile t
-          cx_b = b;
-          cx_valid = valid;
-          cx_orow = POOL ? nullptr : out + (static_cast<size_t>(b) * C3) * P + j;
-          if (POOL) {
-            cx_nd = nd_next;
-            cx_vmask = __ballot_sync(FULL, nd_next >= 0);
-            cx_is_p0 = valid && (j == p0row);
-            cx_any_p0 = __any_sync(FULL, cx_is_p0);
-          }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        stage_release(q++);
+        unsigned char* img = region + OFF_ACT12;
+#pragma unroll
+        for (int jn = 0; jn < 16; ++jn) {
+          const int k = 8 * jn + cq;
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr)
+            put_pair(img, ACT1_HALF, 2048, r0 + 8 * rr, k,
+                     fmaxf(fmaf(acc[4 * jn + 2 * rr], inv1, __ldg(sh1 + k)), 0.f),
+                     fmaxf(fmaf(acc[4 * jn + 2 * rr + 1], inv1, __ldg(sh1 + k + 1)), 0.f));
         }
-        if (nc >= 0 && t >= 0) {
-          const int buf = nc & 1;
-          tc::mbar_wait_bounded(&d3full[buf], (nc >> 1) & 1, 22);   // two uses per tile: parity = use&1
-          tc::fence_after_sync();
-          if (warp == 4) PM_TL(1, 6 + 2 * nc);
-          const uint32_t cb = lane_base + COL_D3 + L3_N * buf + 48 * h;
-          tc::ld16(cb, v0);
-          tc::ld16(cb + 16, v1);
-          tc::ld16(cb + 32, v2);
-          tc::wait_ld();
-          tc::fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&d3empty[buf]);
-        }
-        const bool finish = (nc < 0) ? parked : (nc < L3_CHUNKS - 1);
-        if (finish) {
-          const int co0 = L3_N * (nc < 0 ? L3_CHUNKS - 1 : nc) + 48 * h;
-          if (POOL) {
-            pool_group(v0, co0);
-            pool_group(v1, co0 + 16);
-            pool_group(v2, co0 + 32);
-          } else if (cx_valid) {
-            store_group(v0, co0);
-            store_group(v1, co0 + 16);
-            store_group(v2, co0 + 32);
-          }
-          if (warp == 4) PM_TL(1, nc < 0 ? 13 : 7 + 2 * nc);
-        }
-        if (nc < 0 && live) {
-          // (the parked chunk of tile t-1 was pooled just above, inside the window in which this
-          // tile's layer-2 MMAs run and the epilogue warps would otherwise wait for b_d2)
-          // ---- layer 2 epilogue, in place: quarter qd = act2 channels [64qd, 64qd+64) = K stage
-          // qd+1 of layer 3, 32 per warpgroup (two groups of 16), announced quarter by quarter ----
-          tc::mbar_wait_bounded(b_d2, par, 21);
-          tc::fence_after_sync();
-          if (warp == 4) PM_TL(1, 4);
+        publish();
+      }
+
+      // ---- layer 2: D2[64 x 256] = act1[64 x 128] * W2^T, four K slabs of 32 ----
+      {
+        float acc[128];
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
 #pragma unroll 1
-          for (int g = 0; g < 8; ++g) {
-            const int qd = g >> 1;
-            const int ch0 = 64 * qd + 32 * h + 16 * (g & 1);
-            uint32_t v[16];
-            tc::ld16(lane_base + COL_D2 + ch0, v);
-            tc::wait_ld();
-            float y[16];
+        for (int kc = 0; kc < L2_STAGES; ++kc) {
+          const uint32_t sb = stage_wait();
+          tc::wg_fence();
 #pragma unroll
-            for (int i = 0; i < 16; ++i)
-              y[i] = fmaxf(fmaf(__uint_as_float(v[i]), inv2, sh2[ch0 + i]), 0.f);
-            tc::split16_f16(y, v);
-            tc::st16(lane_base + COL_D2 + ch0, v);
-            if (g & 1) {
-              tc::wait_st();
-              tc::fence_before_sync();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(&b_act2q[qd]);
-            }
+          for (int ks = 0; ks < 2; ++ks) {
+            const uint32_t ka = act12_a + (kc * 4 + ks * 2) * 128;
+            const uint64_t ah = tc::smem_desc(ka, 128, 2048),
+                           al = tc::smem_desc(ka + ACT1_HALF, 128, 2048),
+                           bh = tc::smem_desc(sb + ks * 256, 128, 512),
+                           bl = tc::smem_desc(sb + L2_STAGE_BYTES / 2 + ks * 256, 128, 512);
+            tc::wgmma_f16_n256(acc, ah, bh, 1);
+            tc::wgmma_f16_n256(acc, al, bh, 1);
+            tc::wgmma_f16_n256(acc, ah, bl, 1);
           }
-          if (warp == 4) PM_TL(1, 5);
-          if (t + 1 < my_tiles) prefetch_x(t + 1);   // in flight during the layer-3 MMAs
+          tc::wg_commit();
+          tc::wg_wait<1>();
+          if (kc > 0) stage_release(q - 1);
+          ++q;
+        }
+        tc::wg_wait<0>();
+        stage_release(q - 1);
+        // act2 overwrites act1, including rows other warps' wgmmas read: wait_group only covers
+        // the executing warp's own groups, so every warp of the warpgroup must be past it first
+        tc::named_sync(1 + wg, 128);
+        unsigned char* img = region + OFF_ACT12;
+#pragma unroll
+        for (int jn = 0; jn < 32; ++jn) {
+          const int k = 8 * jn + cq;
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr)
+            put_pair(img, ACT2_HALF, 4096, r0 + 8 * rr, k,
+                     fmaxf(fmaf(acc[4 * jn + 2 * rr], inv2, __ldg(sh2 + k)), 0.f),
+                     fmaxf(fmaf(acc[4 * jn + 2 * rr + 1], inv2, __ldg(sh2 + k + 1)), 0.f));
+        }
+        publish();
+      }
+
+      // ---- layer 3: D3[64 x 384] = cat(act0, act2)[64 x 320] * W3^T, 4 chunks of N=96; bare ----
+      int nd[2] = {-1, -1};
+      bool is_p0[2] = {false, false};
+      const bool valid0 = jbase + r0 < P, valid1 = jbase + r0 + 8 < P;
+      if (POOL) {
+        const int p0row = __ldg(pool.pos0 + b);
+        if (valid0) nd[0] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0);
+        if (valid1) nd[1] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0 + 8);
+        is_p0[0] = valid0 && jbase + r0 == p0row;
+        is_p0[1] = valid1 && jbase + r0 + 8 == p0row;
+      }
+#pragma unroll 1
+      for (int nc = 0; nc < L3_CHUNKS; ++nc) {
+        float acc[48];
+#pragma unroll
+        for (int i = 0; i < 48; ++i) acc[i] = 0.f;
+#pragma unroll 1
+        for (int kc = 0; kc < L3_KSTAGES; ++kc) {
+          const uint32_t sb = stage_wait();
+          // 16-channel K groups: stage 0 = act0, stages 1-4 = act2 quarters
+          const uint32_t a0 = kc == 0 ? act0_a : act12_a + (kc - 1) * 8 * 128;
+          const uint32_t sbo = kc == 0 ? 1024 : 4096, ahalf = kc == 0 ? ACT0_HALF : ACT2_HALF;
+          tc::wg_fence();
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            const uint64_t ah = tc::smem_desc(a0 + ks * 256, 128, sbo),
+                           al = tc::smem_desc(a0 + ahalf + ks * 256, 128, sbo),
+                           bh = tc::smem_desc(sb + ks * 256, 128, 1024),
+                           bl = tc::smem_desc(sb + L3_STAGE_BYTES / 2 + ks * 256, 128, 1024);
+            tc::wgmma_f16_n96(acc, ah, bh, 1);
+            tc::wgmma_f16_n96(acc, al, bh, 1);
+            tc::wgmma_f16_n96(acc, ah, bl, 1);
+          }
+          tc::wg_commit();
+          tc::wg_wait<1>();
+          if (kc > 0) stage_release(q - 1);
+          ++q;
+        }
+        tc::wg_wait<0>();
+        stage_release(q - 1);
+
+        const int cbase = L3_N * nc + cq;
+        if (!POOL) {
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int j = jbase + r0 + 8 * rr;
+            if (j >= P) continue;
+            float* o = out + (static_cast<size_t>(b) * C3 + cbase) * P + j;
+#pragma unroll
+            for (int jn = 0; jn < 12; ++jn)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                o[static_cast<size_t>(8 * jn + e) * P] =
+                    fmaf(acc[4 * jn + 2 * rr + e], inv3, __ldg(sh3 + cbase + 8 * jn + e));
+          }
+        } else {
+          // per-node max over the warp's 16 rows, one pass per run of equal node ids
+          unsigned rem0 = __ballot_sync(FULL, nd[0] >= 0), rem1 = __ballot_sync(FULL, nd[1] >= 0);
+#pragma unroll 1
+          while ((rem0 | rem1) != 0) {
+            const int node = rem0 ? __shfl_sync(FULL, nd[0], __ffs(rem0) - 1)
+                                  : __shfl_sync(FULL, nd[1], __ffs(rem1) - 1);
+            const bool in0 = nd[0] == node, in1 = nd[1] == node;
+            rem0 &= ~__ballot_sync(FULL, in0);
+            rem1 &= ~__ballot_sync(FULL, in1);
+            int32_t* kb = pool.keys + (static_cast<size_t>(b) * C3 + cbase) * pool.M + node;
+#pragma unroll
+            for (int jn = 0; jn < 12; ++jn)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                float mx = fmaxf(in0 ? acc[4 * jn + e] : -INFINITY, in1 ? acc[4 * jn + 2 + e] : -INFINITY);
+                mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 4));
+                mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 8));
+                mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 16));
+                if (lane < 4) {
+                  const int co = 8 * jn + e;
+                  const int bits = __float_as_int(fmaf(mx, inv3, __ldg(sh3 + cbase + co)));
+                  const int key = bits ^ ((bits >> 31) & 0x7fffffff);   // order-preserving float -> int
+                  atomicMax(kb + static_cast<size_t>(co) * pool.M, key);
+                }
+              }
+          }
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            if (!is_p0[rr]) continue;   // rare: one row per cloud
+#pragma unroll
+            for (int jn = 0; jn < 12; ++jn)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                pool.p0[static_cast<size_t>(b) * C3 + cbase + 8 * jn + e] =
+                    fmaf(acc[4 * jn + 2 * rr + e], inv3, __ldg(sh3 + cbase + 8 * jn + e));
+          }
         }
       }
-      parked = live;
+      // the next tile's layer 0 overwrites act0, which this tile's layer-3 wgmmas read: all are
+      // complete (wait_group 0 above); the other warps of the warpgroup must be past them too
+      tc::named_sync(1 + wg, 128);
     }
   }
-  tc::fence_before_sync();
   __syncthreads();
   if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[64 + 63] = clock64();
-  if (CL > 1) tc::cluster_sync_all();   // no CTA leaves while peers may still signal its barriers
-  if (warp == 2) tc::tmem_dealloc(tm, 512);
-#undef PM_TL
 }
 
 // ---- host-side packing -------------------------------------------------------------------------------
@@ -687,40 +482,12 @@ static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const vo
   SONET_REQUIRE(tiles < (1LL << 31), "pointresnet_tc: too many tiles");
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "pointresnet_tc: needs %d B of shared memory",
                 SMEM_BYTES);
-  // cluster size: 1 by default; SONET_TC_CLUSTER=2|4 enables the multicast weight stream
-  static int cl_env = -1;
-  if (cl_env < 0) {
-    const char* e = getenv("SONET_TC_CLUSTER");
-    cl_env = e ? atoi(e) : 1;
-    if (cl_env != 1 && cl_env != 2 && cl_env != 4) cl_env = 1;
-  }
-  int cl = cl_env;
-  const int sms = sm_count();
-  while (cl > 1 && (tiles < cl || sms % cl != 0)) cl >>= 1;
-  int grid = static_cast<int>(std::min<long long>(tiles, sms));
-  grid -= grid % cl;
-  auto kern = pool ? (cl == 4 ? pointresnet_tc_kernel<4, true>
-                              : (cl == 2 ? pointresnet_tc_kernel<2, true>
-                                         : pointresnet_tc_kernel<1, true>))
-                   : (cl == 4 ? pointresnet_tc_kernel<4, false>
-                              : (cl == 2 ? pointresnet_tc_kernel<2, false>
-                                         : pointresnet_tc_kernel<1, false>));
+  const int grid = static_cast<int>(std::min<long long>(tiles, sm_count()));
+  auto kern = pool ? pointresnet_tc_kernel<true> : pointresnet_tc_kernel<false>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = SMEM_BYTES;
-  cfg.stream = as_stream(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cl;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
   PoolArgs pa = pool ? *pool : PoolArgs{nullptr, nullptr, nullptr, nullptr, 0};
-  cudaLaunchKernelEx(&cfg, kern, x, Cin, B, P, static_cast<const unsigned char*>(blob), fparams, out,
-                     dbg, pa);
+  kern<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
+      x, Cin, B, P, static_cast<const unsigned char*>(blob), fparams, out, dbg, pa);
   return check_launch("pointresnet_tc");
 }
 

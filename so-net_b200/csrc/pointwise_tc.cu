@@ -1,4 +1,5 @@
-// pointwise_tc.cu — generic point-wise shared-MLP layer (1x1 conv + folded BN + ReLU) on tcgen05.
+// pointwise_tc.cu — generic point-wise shared-MLP layer (1x1 conv + folded BN + ReLU) on Hopper
+// warpgroup MMA (wgmma).
 //
 // Same contract as sonet_pointwise_layer_f32 (csrc/pointwise.cu; EquivariantLayer / MyConv2d 1x1 eval
 // forward, models/layers.py:203-210, 282-296) for the layers that are dense enough for tensor
@@ -7,64 +8,50 @@
 //
 //   out[b,co,p] = act( inv * sum_ci Ws[co,ci] * X[b,ci,p] + shift[co] (+ addend[b,co,g(b,p)]) )
 //
-// Rows (b,p) are flattened and tiled by 128 = MMA M = TMEM lanes; an item is (row tile, 256-wide
-// out-channel tile); K streams in 64-channel activation chunks (2-stage ring of converted A images,
-// two fp32 staging tiles ahead of it) and 32-channel weight stages (3-stage ring; the small weight
-// stage is what leaves room for the second staging tile — with one, fetch and conversion of a
-// chunk were serial and ncu showed the kernel latency-bound at 12 % DRAM / 38 % tensor pipe):
-//   * converter warps (8): fetch the fp32 activations with cp.async into a staging buffer — 16 B
-//     per thread (4 consecutive rows of one channel: a warp instruction moves one channel's 128
-//     rows) when P and the base pointers allow it, 4 B otherwise; LDGSTS costs ~8 LSU cycles per
-//     warp instruction whatever its width, and at 4 B the 256 instructions of a chunk took longer
-//     than its MMAs — then clamp to the fp16 range, split into fp16 hi/lo and write the K-major
-//     no-swizzle A images with one 128-bit shared store per 8 channels (conflict free),
-//     fence.proxy.async, arrive. When P % 64 == 0 and the layer has one source tensor, the chunk
-//     is fetched by TENSOR-MAP TMA instead: a 128-row tile is exactly two [64 p x 64 c] boxes of a
-//     3-D map over x[B][C][P] (out-of-range channels / clouds are zero-filled by the hardware), two
-//     instructions per chunk instead of 64 LDGSTS whose outstanding-request limit set the pace;
-//   * TMA warp: streams the pre-packed fp16 hi/lo weight images (cp.async.bulk + mbarrier);
-//   * MMA warp (one thread): 3 tcgen05.mma.kind::f16 per 16-channel K step (hi*hi + lo*hi + hi*lo),
-//     SS mode, M=128, N<=256, fp32 accumulation in TMEM, two 256-column accumulator buffers so the
-//     epilogue of item i overlaps the MMAs of item i+1;
-//   * epilogue warps (8, two warpgroups split the columns): tcgen05.ld, fused scale/shift (+ gathered addend) + ReLU, stores with
-//     lane = row => 128-byte coalesced along p.
+// Rows (b,p) are flattened and tiled by 128; an item is (row tile, 128-wide out-channel tile); K
+// streams in 64-channel chunks:
+//   * two consumer warpgroups, one per 64 rows of the tile (wgmma M = 64). Each thread fetches 32
+//     channels of one row of the next chunk with coalesced loads (a warp instruction reads 32
+//     consecutive points of one channel) while the current chunk's wgmmas run, splits them into
+//     fp16 hi/lo and writes the K-major no-swizzle A images with one 128-bit shared store per 8
+//     channels (conflict free), then issues 3 wgmma per 16-channel K step (hi*hi + lo*hi + hi*lo)
+//     with fp32 accumulators in registers (64 per thread at N = 128). A 2-slot A ring: a slot is
+//     rewritten once wgmma.wait_group shows the chunk that read it complete;
+//   * producer warp: streams the pre-packed fp16 hi/lo weight images (cp.async.bulk + mbarrier)
+//     through a 4-stage ring shared by both warpgroups;
+//   * epilogue in registers: fused scale/shift (+ gathered addend) + ReLU; eight lanes of a warp
+//     hold eight consecutive points of one channel, so every store fills 32-byte sectors.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
 
-#include <cuda.h>   // CUtensorMap (types only: the encoder is fetched with cudaGetDriverEntryPoint)
-
 #include "tc_common.cuh"
 
 namespace sonet {
 namespace pwt {
-constexpr int TILE = 128, KCH = 64, NT = 256;
-constexpr int WK = 32;                         // K extent of one weight stage (two per A chunk)
-constexpr int A_BYTES = 2 * TILE * KCH * 2;   // hi + lo images of the activation chunk, 32 KB
-constexpr int W_BYTES = 2 * NT * KCH * 2;     // hi + lo weight images of one (n-tile, 64-k chunk) in the blob
-constexpr int WS_BYTES = 2 * NT * WK * 2;     // one weight stage in shared memory, 32 KB
-constexpr int NSTAGE = 2;                      // A ring
-constexpr int NSTAGE_W = 3;                    // weight ring
-constexpr int NSTG = 2;                        // fp32 staging tiles (TMA fetch runs two chunks ahead)
-constexpr int NUM_THREADS = 640;   // warps: 0 TMA, 1 MMA, 2 TMEM alloc, 4-11 epilogue, 12-19 converters
+constexpr int TILE = 128, KCH = 64, NT = 256;   // NT: out-channel width of one weight-blob tile
+constexpr int NSUB = 128;                       // out channels per item (two per blob tile)
+constexpr int WK = 32;                          // K extent of one weight stage in the blob
+constexpr int A_HALF = TILE * KCH * 2;          // one fp16 image of an activation chunk, 16 KB
+constexpr int A_BYTES = 2 * A_HALF;             // hi + lo
+constexpr int W_BYTES = 2 * NT * KCH * 2;       // hi + lo weight images of one (blob tile, 64-k chunk)
+constexpr int WIMG = NSUB * WK * 2;             // one [128 x 32] fp16 weight image, 8 KB
+constexpr int WS_BYTES = 4 * WIMG;              // one chunk in shared memory: [half][hi|lo], 32 KB
+constexpr int NSTAGE = 2;                       // A ring
+constexpr int NSTAGE_W = 4;                     // weight ring
+constexpr int NUM_THREADS = 288;                // warps 0-7: two consumer warpgroups, warp 8: producer
 constexpr int OFF_A = 0;
 constexpr int OFF_W = OFF_A + NSTAGE * A_BYTES;
-constexpr int OFF_STG = OFF_W + NSTAGE_W * WS_BYTES;   // fp32 staging of activation chunks
-constexpr int STG_BYTES = KCH * TILE * 4;               // [64 ch][128 rows] fp32, 32 KB
-constexpr int OFF_BAR = OFF_STG + NSTG * STG_BYTES;
-constexpr int NBAR = 2 * NSTAGE_W + 2 * NSTAGE + 4 + NSTG;
-constexpr int OFF_TMEM = OFF_BAR + NBAR * 8;
-constexpr int SMEM_BYTES = OFF_TMEM + 16;
+constexpr int OFF_BAR = OFF_W + NSTAGE_W * WS_BYTES;
+constexpr int NBAR = 2 * NSTAGE_W;
+constexpr int SMEM_BYTES = OFF_BAR + NBAR * 8;
 
 struct Dims {
   int C0, C1, B, P, Cout, relu, G;
   int kchunks;   // ceil(pad16(Cin) / 64)
-  int ntiles;    // out-channel tiles of <= 256 (each a multiple of 64)
+  int ntiles;    // out-channel items of <= 128 (each a multiple of 64)
   int cin_pad;   // Cin rounded up to 16
-  int vec4;      // 16-byte activation fetch is legal (P % 4 == 0, 16-byte aligned bases)
-  int tma;       // activation chunks by tensor-map TMA (P % 64 == 0). Two sources: maps 1-3 (XMaps)
-  int h0;        // two-source TMA: channels of the chunk that straddles x0 | x1 coming from x0 (C0 % 64)
   float inv;     // 1 / weight pre-scale
   // ---- grouped / split-K / scatter extensions (the up-convolution decoder, csrc/upconv.cu) ----
   int groups;    // independent GEMMs sharing shapes: x is [groups*B, C, P], one weight blob each
@@ -76,9 +63,8 @@ struct Dims {
   int P_out;     // point stride of `out` (= P unless scattering)
   int conv_w;    // > 0: up-convolution mode without im2col. x is [3*B, Cin, H*W] = the input shifted
                  //      horizontally by -1, 0, +1 (csrc/upconv.cu); K chunk kc = (tap t = a*2+c,
-                 //      64-channel chunk): the TMA box is fetched from block c-1+px+1 at point
-                 //      coordinate p + (a-1+py)*W — vertical shifts are plain coordinate offsets,
-                 //      whose out-of-range part the TMA unit zero-fills
+                 //      64-channel chunk): rows are read from block c-1+px+1 at point p + (a-1+py)*W
+                 //      — vertical shifts are plain coordinate offsets, out of range reads zeros
   int cpt;       // 64-channel chunks per tap (= Cin / 64) in conv mode
   const float* inv_ptr;     // non-null: 1 / weight pre-scale lives in device memory (train mode:
                             // the weights are packed on the device every step, csrc/train.cu)
@@ -90,12 +76,14 @@ struct Dims {
   long long out_sstride;    // floats between the partial sums of consecutive K splits
 };
 struct Item {
-  int g, tile, nt, kc0;
+  int g, tile, nt, sub, kc0;
 };
 __device__ __forceinline__ Item decode_item(const Dims& d, int item) {
   // n-tile fastest: the activation tile stays hot in L2; then K split, row tile, group
   Item r;
-  r.nt = item % d.ntiles;
+  const int s = item % d.ntiles;
+  r.nt = s >> 1;
+  r.sub = s & 1;
   int t = item / d.ntiles;
   const int sp = t % d.splits;
   t /= d.splits;
@@ -108,45 +96,22 @@ __host__ __device__ inline int ntile_width(int Cout, int nt) {
   const int cpad = (Cout + 63) / 64 * 64;
   return min(NT, cpad - nt * NT);
 }
-}  // namespace pwt
-
-__device__ __forceinline__ bool sonet_aligned16_dev(const void* p) {
-  return (reinterpret_cast<uintptr_t>(p) & 15u) == 0;
+__host__ __device__ inline int item_width(int Cout, int nt, int sub) {
+  return min(NSUB, ntile_width(Cout, nt) - sub * NSUB);
 }
-
-// Tensor maps of the activation operand. 0: x0, box [64 p][64 c]; two sources (x0 | x1 along the
-// channel axis): 1: x1, box [64 p][64 c]; 2: x0, box [64 p][h0 c]; 3: x1, box [64 p][64 - h0 c] —
-// the one chunk that straddles the two tensors is fetched as two shorter boxes that land back to back
-// in the staging tile.
-struct XMaps {
-  CUtensorMap m[4];
-};
+}  // namespace pwt
 
 __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
     pointwise_tc_kernel(const float* __restrict__ x0, const float* __restrict__ x1,
                         const unsigned char* __restrict__ blob, const float* __restrict__ shift,
                         const float* __restrict__ addend, const int32_t* __restrict__ gidx,
-                        float* __restrict__ out, pwt::Dims d, long long* __restrict__ dbg,
-                        const __grid_constant__ XMaps xm) {
+                        float* __restrict__ out, pwt::Dims d, long long* __restrict__ dbg) {
   using namespace pwt;
-#define PW_TL(role, idx)                                                   \
-  do {                                                                     \
-    if (dbg != nullptr && blockIdx.x == 0 && lane == 0 && (idx) < 32)      \
-      dbg[(role) * 32 + (idx)] = clock64();                                \
-  } while (0)
   if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[127] = clock64();
   extern __shared__ __align__(1024) unsigned char smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* full_w = bars;                        // [NSTAGE_W] TMA -> MMA
-  uint64_t* empty_w = full_w + NSTAGE_W;          // [NSTAGE_W] MMA -> TMA
-  uint64_t* full_a = empty_w + NSTAGE_W;          // [NSTAGE] converters -> MMA
-  uint64_t* empty_a = full_a + NSTAGE;            // [NSTAGE] MMA -> converters
-  uint64_t* d_full = empty_a + NSTAGE;            // [2] MMA -> epilogue
-  uint64_t* d_empty = d_full + 2;                 // [2] epilogue -> MMA
-  uint64_t* stg_full = d_empty + 2;               // [NSTG] TMA -> converters (staging tile landed)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + OFF_TMEM);
+  uint64_t* full_w = reinterpret_cast<uint64_t*>(smem + OFF_BAR);   // [NSTAGE_W] producer -> MMA
+  uint64_t* empty_w = full_w + NSTAGE_W;                             // [NSTAGE_W] MMA -> producer
 
-  // warp index through a shuffle: ptxas then knows the role branches are warp-uniform
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const long long rows = static_cast<long long>(d.B) * d.P;   // rows of ONE group
@@ -158,400 +123,195 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSTAGE_W; ++s) {
       mbar_init(&full_w[s], 1);
-      mbar_init(&empty_w[s], 1);
+      mbar_init(&empty_w[s], 8);   // one arrival per consumer warp
     }
-    for (int s = 0; s < NSTAGE; ++s) {
-      mbar_init(&full_a[s], 8);
-      mbar_init(&empty_a[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&d_full[i], 1);
-      mbar_init(&d_empty[i], 8);
-    }
-    for (int i = 0; i < NSTG; ++i) mbar_init(&stg_full[i], 1);
     mbar_fence_init();
   }
-  if (warp == 2) {
-    tc::tmem_alloc(tmem_ptr, 512);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  if (*tmem_ptr != 0u) __trap();   // all 512 columns allocated: the base is 0 by construction
-  constexpr uint32_t tm = 0;
 
-  if (warp == 0) {
-    // ================= TMA producer: weight chunk images =================
+  if (warp == 8) {
+    // ================= producer: weight chunk images =================
     if (lane == 0) {
       uint32_t q = 0;
       for (int it = 0; it < my_items; ++it) {
         const Item im = decode_item(d, blockIdx.x + it * gridDim.x);
-        const int nt = im.nt;
-        const int nw = ntile_width(d.Cout, nt);
-        // blob: n-tile nt starts after nt full-width tiles; a 64-k chunk = two [nw x 32] stages
+        const int nw = ntile_width(d.Cout, im.nt);
+        const int ns = item_width(d.Cout, im.nt, im.sub);
+        // blob: tile nt starts after nt full-width tiles; a 64-k chunk = two [nw x 32] stages, each
+        // a hi image then a lo image; this item's rows are [128 sub, 128 sub + ns) of each image
         const size_t off0 = static_cast<size_t>(im.g) * d.blob_gstride +
-                            static_cast<size_t>(nt) * d.kchunks * W_BYTES;
-        const uint32_t bytes = static_cast<uint32_t>(nw) * WK * 4;
-        for (int kc = im.kc0; kc < im.kc0 + d.kpi; ++kc) {
-          const int halves = (d.cin_pad - kc * KCH > WK) ? 2 : 1;   // the MMA warp agrees
-          for (int hh = 0; hh < halves; ++hh, ++q) {
-            const uint32_t slot = q % NSTAGE_W, use = q / NSTAGE_W;
-            if (use > 0) tc::mbar_wait_relaxed(&empty_w[slot], (use - 1) & 1, 200);
-            mbar_arrive_expect_tx(&full_w[slot], bytes);
-            bulk_g2s(smem + OFF_W + slot * WS_BYTES,
-                     blob + off0 + (static_cast<size_t>(kc) * 2 + hh) * bytes, bytes, &full_w[slot]);
-            if (it == 0 && hh == 0) PW_TL(0, kc - im.kc0);
+                            static_cast<size_t>(im.nt) * d.kchunks * W_BYTES;
+        const uint32_t stage = static_cast<uint32_t>(nw) * WK * 4;
+        const uint32_t bytes = static_cast<uint32_t>(ns) * WK * 2;
+        for (int kc = im.kc0; kc < im.kc0 + d.kpi; ++kc, ++q) {
+          const int halves = (d.cin_pad - kc * KCH > WK) ? 2 : 1;   // the consumers agree
+          const uint32_t slot = q % NSTAGE_W, use = q / NSTAGE_W;
+          if (use > 0) tc::mbar_wait_relaxed(&empty_w[slot], (use - 1) & 1, 200);
+          mbar_arrive_expect_tx(&full_w[slot], 2 * halves * bytes);
+          unsigned char* dst = smem + OFF_W + slot * WS_BYTES;
+          for (int hh = 0; hh < halves; ++hh) {
+            const unsigned char* src = blob + off0 + (static_cast<size_t>(kc) * 2 + hh) * stage +
+                                       static_cast<size_t>(im.sub) * NSUB * WK * 2;
+            bulk_g2s(dst + (2 * hh) * WIMG, src, bytes, &full_w[slot]);
+            bulk_g2s(dst + (2 * hh + 1) * WIMG, src + static_cast<size_t>(nw) * WK * 2, bytes,
+                     &full_w[slot]);
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ========== MMA issuer: converged warp, elect.sync issues from one lane ==========
-    {
-      const uint32_t a_base = static_cast<uint32_t>(__cvta_generic_to_shared(smem + OFF_A)),
-                     w_base = static_cast<uint32_t>(__cvta_generic_to_shared(smem + OFF_W));
-      uint32_t qa = 0, qw = 0;
-      for (int it = 0; it < my_items; ++it) {
-        const Item im = decode_item(d, blockIdx.x + it * gridDim.x);
-        const int nt = im.nt;
-        const int nw = ntile_width(d.Cout, nt);
-        const uint32_t idesc = tc::idesc_f16_f32(TILE, nw);
-        const int buf = it & 1;
-        const uint32_t use = it >> 1;
-        if (use > 0) tc::mbar_wait_bounded(&d_empty[buf], (use - 1) & 1, 201);
-        tc::fence_after_sync();
-        const uint32_t dcol = tm + buf * NT;
-        for (int kc = im.kc0; kc < im.kc0 + d.kpi; ++kc, ++qa) {
-          const uint32_t sa = qa % NSTAGE, pa = (qa / NSTAGE) & 1;
-          tc::mbar_wait_bounded(&full_a[sa], pa, 203);
-          if (it == 0) PW_TL(1, 3 * (kc - im.kc0) + 1);
-          const uint32_t as = a_base + sa * A_BYTES;
-          const int nks = min(4, (d.cin_pad - kc * KCH) / 16);
-          const int halves = (nks > 2) ? 2 : 1;
-          for (int hh = 0; hh < halves; ++hh, ++qw) {
-            const uint32_t sw = qw % NSTAGE_W, pw = (qw / NSTAGE_W) & 1;
-            tc::mbar_wait_bounded(&full_w[sw], pw, 202);
-            tc::fence_after_sync();
-            if (it == 0 && hh == 0) PW_TL(1, 3 * (kc - im.kc0));
-            const uint32_t ws = w_base + sw * WS_BYTES;
-            // A: [128 x 64] image, SBO 1024, this half starts 2 k-steps (512 B) in;
-            // B: [nw x 32] image, SBO 512
-            const uint64_t ah = tc::smem_desc(as + hh * 512, 128, 1024),
-                           al = tc::smem_desc(as + A_BYTES / 2 + hh * 512, 128, 1024),
-                           bh = tc::smem_desc(ws, 128, 512),
-                           bl = tc::smem_desc(ws + nw * WK * 2, 128, 512);
-            const uint32_t acc = ((kc - im.kc0) | hh) != 0;
-            const int nk = (hh == 0) ? min(nks, 2) : nks - 2;
-            if (nk == 2) tc::mma_ss_stage<2>(dcol, ah, al, bh, bl, idesc, acc);
-            else tc::mma_ss_stage<1>(dcol, ah, al, bh, bl, idesc, acc);
-            tc::commit_elect(&empty_w[sw]);
-          }
-          tc::commit_elect(&empty_a[sa]);
-          if (it == 0) PW_TL(1, 3 * (kc - im.kc0) + 2);
-        }
-        tc::commit_elect(&d_full[buf]);
-      }
-    }
-  } else if (warp >= 12) {
-    // ================= converters: fp32 activations -> fp16 hi/lo K-major A images =================
-    const int t = threadIdx.x - 384;
-    const int m = t & 127, half = t >> 7;   // row in tile; which 32 of the chunk's 64 channels
-    // The fp32 activations of a chunk are fetched with cp.async (LDGSTS) into a staging buffer
-    // [64 ch][128 rows]: the whole 32 KB chunk is in flight without holding registers.
-    // (Register-staged loads were bytes-in-flight bound: 4-5k cycles per chunk in the timeline.)
-    // Each thread converts row m's 32 channels, which other threads copied: wait_group + a named
-    // barrier before the read, another one before the tile is refilled with the next chunk.
-    const uint32_t total = static_cast<uint32_t>(my_items) * d.kpi;
+  } else {
+    // ================= consumers: 64 rows each =================
+    const int wg = warp >> 2;                 // which 64 rows of the tile
+    const int tw = threadIdx.x & 127;
+    const int m = tw & 63, half = tw >> 6;    // conversion: row m, channels [32 half, 32 half + 32)
     const float act_s = d.act_ptr != nullptr ? __ldg(d.act_ptr) : 1.f;
-    float* stg = reinterpret_cast<float*>(smem + OFF_STG) + (half * 32) * TILE + m;
-    const uint32_t stg_s = smem_u32(stg);
-    auto issue = [&](uint32_t qq) {
-      // TMA mode: one thread issues the boxes, and only that thread pays for the item decode (its
-      // integer divisions were 8.5 % of the kernel's executed instructions when all 256 converter
-      // threads evaluated them per chunk)
-      if (d.tma && t != 0) return;
-      const int it = qq / d.kpi;
-      const Item im = decode_item(d, blockIdx.x + it * gridDim.x);
-      const int kc = im.kc0 + (qq - it * d.kpi);
-      const long long R0 = static_cast<long long>(im.tile) * TILE;
-      const int gb = im.g * d.B;                 // first cloud of this group in x [groups*B, C, P]
-      if (d.tma) {
-        // two [64 p][64 c] boxes; staging layout [box][c][64 p]. Rows past the last cloud give
-        // b >= B (fully out of range): the box is zero-filled and still counts its bytes.
-        {
-          uint64_t* sfull = &stg_full[qq % NSTG];
-          const uint32_t sdst = smem_u32(smem + OFF_STG) + (qq % NSTG) * STG_BYTES;
-          mbar_arrive_expect_tx(sfull, STG_BYTES);
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const long long R = R0 + 64 * i;
-            const int bl = static_cast<int>(R / d.P);
-            int p = static_cast<int>(R - static_cast<long long>(bl) * d.P);
-            // rows past the group's last cloud must not read the next group: push them out of range
-            int b = (bl < d.B) ? gb + bl : d.groups * d.B;
-            int cc = kc * KCH;
-            if (d.conv_w > 0) {
-              const int tap = kc / d.cpt;
-              cc = (kc - tap * d.cpt) * KCH;
-              const int py = im.g >> 1, px = im.g & 1;
-              p += ((tap >> 1) - 1 + py) * d.conv_w;                 // vertical shift: OOB -> zeros
-              b = (bl < d.B) ? ((tap & 1) + px) * d.B + bl : 3 * d.B;   // horizontal-shift block 0..2
-            }
-            auto box = [&](const CUtensorMap* mp, uint32_t dst, int c) {
-              asm volatile(
-                  "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes "
-                  "[%0], [%1, {%2, %3, %4}], [%5];" ::"r"(dst),
-                  "l"(reinterpret_cast<uint64_t>(mp)), "r"(p), "r"(c), "r"(b), "r"(smem_u32(sfull))
-                  : "memory");
-            };
-            const uint32_t dst = sdst + i * (STG_BYTES / 2);
-            if (d.C1 == 0 || cc + KCH <= d.C0) {
-              box(&xm.m[0], dst, cc);
-            } else if (cc < d.C0) {        // the straddling chunk: h0 channels of x0, then x1's first
-              box(&xm.m[2], dst, cc);
-              box(&xm.m[3], dst + static_cast<uint32_t>(d.h0) * 64 * 4, 0);
-            } else {
-              box(&xm.m[1], dst, cc - d.C0);
-            }
-          }
-        }
-        return;
-      }
-      if (d.vec4) {
-        // warp w copies channels w, w+8, ..., w+56 of the chunk; lane l the rows 4l..4l+3 (never
-        // across a cloud boundary because P % 4 == 0)
-        const long long R = R0 + 4 * lane;
-        const bool valid = R < rows;
-        const int bl = valid ? static_cast<int>(R / d.P) : 0;
-        const int p = valid ? static_cast<int>(R - static_cast<long long>(bl) * d.P) : 0;
-        const int b = gb + bl;
-        const float* r0 = x0 + static_cast<size_t>(b) * d.C0 * d.P + p;
-        const float* r1 = d.C1 ? x1 + static_cast<size_t>(b) * d.C1 * d.P + p : x0;
-        const int w8 = (t >> 5);
-        const uint32_t dst0 = smem_u32(smem + OFF_STG) + (w8 * TILE + 4 * lane) * 4;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int ci = kc * KCH + w8 + 8 * i;
-          const bool ok = valid && ci < Cin;
-          const float* src = !ok ? x0
-                                 : (ci < d.C0 ? r0 + static_cast<size_t>(ci) * d.P
-                                              : r1 + static_cast<size_t>(ci - d.C0) * d.P);
-          const uint32_t nbytes = ok ? 16u : 0u;   // 0 -> zero fill
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst0 + i * 8 * TILE * 4),
-                       "l"(src), "r"(nbytes)
-                       : "memory");
-        }
-      } else {
-        const long long R = R0 + m;
-        const bool valid = R < rows;
-        const int bl = valid ? static_cast<int>(R / d.P) : 0;
-        const int p = valid ? static_cast<int>(R - static_cast<long long>(bl) * d.P) : 0;
-        const int b = gb + bl;
-        const float* r0 = x0 + static_cast<size_t>(b) * d.C0 * d.P + p;
-        const float* r1 = d.C1 ? x1 + static_cast<size_t>(b) * d.C1 * d.P + p : x0;
-        const int c_base = kc * KCH + half * 32;
-#pragma unroll 4
-        for (int i = 0; i < 32; ++i) {
-          const int ci = c_base + i;
-          const bool ok = valid && ci < Cin;
-          const float* src = !ok ? x0
-                                 : (ci < d.C0 ? r0 + static_cast<size_t>(ci) * d.P
-                                              : r1 + static_cast<size_t>(ci - d.C0) * d.P);
-          const uint32_t nbytes = ok ? 4u : 0u;   // 0 -> zero fill
-          asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(stg_s + i * TILE * 4),
-                       "l"(src), "r"(nbytes)
-                       : "memory");
-        }
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    // the 256 converter threads exchange data through the staging tile: named barrier 1
-    auto conv_sync = [&]() { asm volatile("bar.sync 1, 256;" ::: "memory"); };
-    // TMA mode runs NSTG chunks ahead (alternating staging tiles); cp.async mode one (tile 0)
-    if (total > 0) issue(0);
-    if (d.tma && total > 1) issue(1);
-    for (uint32_t qq = 0; qq < total; ++qq) {
-      float v[32];
-      if (d.tma) {
-        tc::mbar_wait_bounded(&stg_full[qq % NSTG], (qq / NSTG) & 1, 206);   // both boxes landed
-        if (warp == 12 && qq >= 6 && qq < 16) PW_TL(2, 3 * (qq - 6));
-        const float* sb = reinterpret_cast<const float*>(smem + OFF_STG + (qq % NSTG) * STG_BYTES) +
-                          (m >> 6) * (KCH * 64) + (half * 32) * 64 + (m & 63);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = sb[i * 64];
-      } else {
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        conv_sync();                        // every thread's copies have landed
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = stg[i * TILE];
-      }
-      conv_sync();                          // the staging tile has been read: refill it
-      if (d.tma) {
-        if (qq + NSTG < total) issue(qq + NSTG);
-      } else if (qq + 1 < total) {
-        issue(qq + 1);
-      }
-      const uint32_t slot = qq % NSTAGE, use = qq / NSTAGE;
-      if (use > 0) tc::mbar_wait_bounded(&empty_a[slot], (use - 1) & 1, 204);
-      if (warp == 12 && qq >= 6 && qq < 16) PW_TL(2, 3 * (qq - 6) + 1);
-      if (d.act_ptr != nullptr) {        // train-mode gradient pre-scale (warp-uniform)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] *= act_s;
-      }
-      unsigned char* a_hi = smem + OFF_A + slot * A_BYTES + (m >> 3) * 1024 + (m & 7) * 16;
-#pragma unroll
-      for (int o = 0; o < 4; ++o) {
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          // saturating conversions keep |hi|, |lo| inside the fp16 range without clamp instructions
-          const float a = v[o * 8 + 2 * j], c = v[o * 8 + 2 * j + 1];
-          hi[j] = tc::pack_f16x2_sat(a, c);
-          const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi[j]));
-          lo[j] = tc::pack_f16x2_sat(a - hf.x, c - hf.y);
-        }
-        const int oct = half * 4 + o;
-        *reinterpret_cast<uint4*>(a_hi + oct * 128) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(a_hi + A_BYTES / 2 + oct * 128) =
-            make_uint4(lo[0], lo[1], lo[2], lo[3]);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full_a[slot]);
-      if (warp == 12 && qq >= 6 && qq < 16) PW_TL(2, 3 * (qq - 6) + 2);
-    }
-  } else if (warp >= 4) {
-    // ================= epilogue: two warpgroups split the item's columns =================
-    const int q4 = warp & 3;
-    const int h = (warp - 4) >> 2;
-    const int m = q4 * 32 + lane;
-    const uint32_t lane_base = tm + (static_cast<uint32_t>(q4 * 32) << 16);
     const float floor_v = d.relu ? 0.f : -__int_as_float(0x7f800000);   // ReLU as one max
     const float inv_w = d.inv_ptr != nullptr ? __ldg(d.inv_ptr) : d.inv;
+    const uint32_t a_base = smem_u32(smem + OFF_A) + wg * (A_HALF / 2);
+    const uint32_t w_base = smem_u32(smem + OFF_W);
+    uint32_t qa = 0;   // chunks consumed by this CTA so far (A and weight ring position)
+
+    // fetch 32 channels of row m of chunk kc of item im
+    auto fetch = [&](const Item& im, int kc, float (&v)[32]) {
+      const long long R = static_cast<long long>(im.tile) * TILE + wg * 64 + m;
+      const bool valid = R < rows;
+      const int bl = valid ? static_cast<int>(R / d.P) : 0;
+      int p = valid ? static_cast<int>(R - static_cast<long long>(bl) * d.P) : 0;
+      if (d.conv_w > 0) {
+        const int tap = kc / d.cpt;
+        const int cc = (kc - tap * d.cpt) * KCH + half * 32;
+        const int py = im.g >> 1, px = im.g & 1;
+        p += ((tap >> 1) - 1 + py) * d.conv_w;                 // vertical shift: out of range -> 0
+        const int b = ((tap & 1) + px) * d.B + bl;             // horizontal-shift block 0..2
+        const bool ok = valid && p >= 0 && p < d.P;
+        const float* src = x0 + (static_cast<size_t>(b) * d.C0 + cc) * d.P + p;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) v[i] = ok ? __ldg(src + static_cast<size_t>(i) * d.P) : 0.f;
+        return;
+      }
+      const int b = im.g * d.B + bl;
+      const float* r0 = x0 + static_cast<size_t>(b) * d.C0 * d.P + p;
+      const float* r1 = d.C1 ? x1 + static_cast<size_t>(bl) * d.C1 * d.P + p : x0;
+      const int c_base = kc * KCH + half * 32;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int ci = c_base + i;
+        const bool ok = valid && ci < Cin;
+        const float* src = ci < d.C0 ? r0 + static_cast<size_t>(ci) * d.P
+                                     : r1 + static_cast<size_t>(ci - d.C0) * d.P;
+        v[i] = ok ? __ldg(src) : 0.f;
+      }
+    };
+
     for (int it = 0; it < my_items; ++it) {
       const Item im = decode_item(d, blockIdx.x + it * gridDim.x);
-      const int nt = im.nt;
-      const int nw = ntile_width(d.Cout, nt);
-      const long long R = static_cast<long long>(im.tile) * TILE + m;
-      const bool valid = R < rows;
-      const int b = valid ? static_cast<int>(R / d.P) : 0;
-      const int p = valid ? static_cast<int>(R - static_cast<long long>(b) * d.P) : 0;
-      // where row (b, p) of this group / K split lands in `out`
-      size_t obase = static_cast<size_t>(im.g) * d.out_gstride +
-                     static_cast<size_t>(im.kc0 / d.kpi) * d.out_sstride;
-      int po = p;
-      if (d.scat_w > 0) {   // x2 up-convolution: parity (py, px) = group
-        const int i = p / d.scat_w, j = p - i * d.scat_w;
-        po = (2 * i + (im.g >> 1)) * 2 * d.scat_w + 2 * j + (im.g & 1);
-      }
-      const int buf = it & 1;
-      tc::mbar_wait_bounded(&d_full[buf], (it >> 1) & 1, 205);
-      tc::fence_after_sync();
-      if (warp == 4 && it < 4) PW_TL(3, 2 * it);
-      const float* arow = nullptr;
-      if (addend != nullptr && valid) {
-        const int g = min(max(__ldg(gidx + static_cast<long long>(im.g) * rows + R), 0), d.G - 1);
-        arow = addend + static_cast<size_t>(b) * d.Cout * d.G + g;
-      }
-      const int cw = nw >> 1;                      // columns per warpgroup (multiple of 32)
-      const int c_lo = h * cw;
-      const bool sh_vec = shift != nullptr && sonet_aligned16_dev(shift);
-      for (int c0 = c_lo; c0 < c_lo + cw; c0 += 32) {
-        uint32_t v0[16], v1[16];
-        tc::ld16(lane_base + buf * NT + c0, v0);
-        tc::ld16(lane_base + buf * NT + c0 + 16, v1);
-        // the 32 shift values of this column group: 128-bit loads issued before the TMEM-load wait.
-        // (One __ldg per output element put a dependent L1 round trip in front of every FFMA: the
-        // epilogue took 23 k cycles per item, longer than the item's MMAs.)
-        const int cg = nt * NT + c0;
-        float sh[32];
-        if (sh_vec && cg + 32 <= d.Cout) {
-          const float4* s4 = reinterpret_cast<const float4*>(shift + cg);
+      const int ns = item_width(d.Cout, im.nt, im.sub);
+      float acc[64];
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 t4 = __ldg(s4 + q);
-            sh[4 * q] = t4.x;
-            sh[4 * q + 1] = t4.y;
-            sh[4 * q + 2] = t4.z;
-            sh[4 * q + 3] = t4.w;
-          }
-        } else {
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      float v[32];
+      fetch(im, im.kc0, v);
+      uint32_t prev_slot = 0;
+      for (int i = 0; i < d.kpi; ++i, ++qa) {
+        const int kc = im.kc0 + i;
+        const uint32_t sa = qa % NSTAGE, sw = qa % NSTAGE_W;
+        // convert into A slot sa (the chunk that read it last completed: wait_group<1> below)
+        if (d.act_ptr != nullptr) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            sh[i] = (shift != nullptr && cg + i < d.Cout) ? __ldg(shift + cg + i) : 0.f;
+          for (int j = 0; j < 32; ++j) v[j] *= act_s;
         }
-        tc::wait_ld();
-        if (c0 + 32 >= c_lo + cw) {   // this warp's columns are all in registers: release the buffer
-          tc::fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&d_empty[buf]);
+        unsigned char* a_hi = smem + OFF_A + sa * A_BYTES + wg * (A_HALF / 2) + (m >> 3) * 1024 +
+                              (m & 7) * 16;
+#pragma unroll
+        for (int o = 0; o < 4; ++o) {
+          uint32_t hi[4], lo[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) tc::split2_f16(v[o * 8 + 2 * j], v[o * 8 + 2 * j + 1], hi[j], lo[j]);
+          const int oct = half * 4 + o;
+          *reinterpret_cast<uint4*>(a_hi + oct * 128) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+          *reinterpret_cast<uint4*>(a_hi + A_HALF + oct * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
         }
-        if (valid) {
-          float* o = out + obase + (static_cast<size_t>(b) * d.Cout + cg) * d.P_out + po;
-          const size_t ostep = static_cast<size_t>(d.P_out);
-          // The epilogue shares its sub-partitions with the converter warps: every instruction here
-          // is an issue slot the A-operand pipeline does not get (timeline: 2.3 k cycles per K chunk
-          // while no epilogue runs, 3.0 k while one does). The common case — all 32 channels real,
-          // no gathered addend — is therefore a separate warp-uniform path of FFMA, FMNMX, STG and a
-          // pointer bump per element (the general form below costs 19 instructions per element:
-          // 64-bit index multiplies, a bounds test and the addend select each time).
-          if (arow == nullptr && cg + 32 <= d.Cout) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              *o = fmaxf(fmaf(__uint_as_float(v0[i]), inv_w, sh[i]), floor_v);
-              o += ostep;
-            }
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              *o = fmaxf(fmaf(__uint_as_float(v1[i]), inv_w, sh[16 + i]), floor_v);
-              o += ostep;
-            }
-          } else if (cg + 32 <= d.Cout) {
-            // gathered addend (one per output element, segmenter layer 1): 16 loads in flight
-            // before the first dependent add
-            const float* ap = arow + static_cast<size_t>(cg) * d.G;
-            const size_t astep = static_cast<size_t>(d.G);
-            auto emit16 = [&](const uint32_t (&v)[16], int i0) {
-              float ad[16];
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                ad[i] = __ldg(ap);
-                ap += astep;
-              }
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                *o = fmaxf(fmaf(__uint_as_float(v[i]), inv_w, sh[i0 + i]) + ad[i], floor_v);
-                o += ostep;
-              }
-            };
-            emit16(v0, 0);
-            emit16(v1, 16);
+        tc::fence_proxy_async();
+        tc::named_sync(1 + wg, 128);         // the warpgroup's 64 rows are written
+        tc::mbar_wait_bounded(&full_w[sw], (qa / NSTAGE_W) & 1, 202);
+        const int nks = min(4, (d.cin_pad - kc * KCH) / 16);
+        const uint32_t as = a_base + sa * A_BYTES, ws = w_base + sw * WS_BYTES;
+        tc::wg_fence();
+#pragma unroll 1
+        for (int ks = 0; ks < nks; ++ks) {
+          // A: [64 x 64] rows of this warpgroup, SBO 1024; B: [ns x 32] image of half ks/2, SBO 512
+          const uint64_t ah = tc::smem_desc(as + ks * 256, 128, 1024),
+                         al = tc::smem_desc(as + A_HALF + ks * 256, 128, 1024);
+          const uint32_t wb = ws + (ks >> 1) * 2 * WIMG + (ks & 1) * 256;
+          const uint64_t bh = tc::smem_desc(wb, 128, 512), bl = tc::smem_desc(wb + WIMG, 128, 512);
+          if (ns == NSUB) {
+            tc::wgmma_f16_n128(acc, ah, bh, 1);
+            tc::wgmma_f16_n128(acc, al, bh, 1);
+            tc::wgmma_f16_n128(acc, ah, bl, 1);
           } else {
-            // ragged last channel group
-            auto emit16 = [&](const uint32_t (&v)[16], int i0) {
+            float (&a32)[32] = *reinterpret_cast<float (*)[32]>(acc);
+            tc::wgmma_f16_n64(a32, ah, bh, 1);
+            tc::wgmma_f16_n64(a32, al, bh, 1);
+            tc::wgmma_f16_n64(a32, ah, bl, 1);
+          }
+        }
+        tc::wg_commit();
+        if (i + 1 < d.kpi) fetch(im, kc + 1, v);   // global loads in flight during the wgmmas
+        tc::wg_wait<1>();                          // the previous chunk is complete ...
+        // ... for every warp of the warpgroup (wait_group covers only the executing warp's groups):
+        // the next chunk rewrites A rows that other warps' wgmmas of that chunk read
+        tc::named_sync(1 + wg, 128);
+        if (i > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_w[prev_slot]);
+        }
+        prev_slot = sw;
+      }
+      tc::wg_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_w[prev_slot]);
+
+      // ---- epilogue: thread holds rows r0 = 16*(warp%4) + lane/4 and r0 + 8, columns
+      // 8j + 2*(lane%4) + {0,1} (accumulators 4j+{0,1} and 4j+{2,3}) ----
+      const int col0 = im.nt * NT + im.sub * NSUB + 2 * (lane & 3);
 #pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                if (cg + i0 + i < d.Cout) {
-                  const float a = arow != nullptr ? __ldg(arow + static_cast<size_t>(cg + i0 + i) * d.G) : 0.f;
-                  const float y = fmaf(__uint_as_float(v[i]), inv_w, sh[i0 + i]) + a;
-                  o[static_cast<size_t>(i0 + i) * d.P_out] = fmaxf(y, floor_v);
-                }
-              }
-            };
-            emit16(v0, 0);
-            emit16(v1, 16);
+      for (int rr = 0; rr < 2; ++rr) {
+        const long long R = static_cast<long long>(im.tile) * TILE + wg * 64 + 16 * (warp & 3) +
+                            (lane >> 2) + 8 * rr;
+        if (R >= rows) continue;
+        const int b = static_cast<int>(R / d.P);
+        const int p = static_cast<int>(R - static_cast<long long>(b) * d.P);
+        // where row (b, p) of this group / K split lands in `out`
+        const size_t obase = static_cast<size_t>(im.g) * d.out_gstride +
+                             static_cast<size_t>(im.kc0 / d.kpi) * d.out_sstride;
+        int po = p;
+        if (d.scat_w > 0) {   // x2 up-convolution: parity (py, px) = group
+          const int i = p / d.scat_w, j = p - i * d.scat_w;
+          po = (2 * i + (im.g >> 1)) * 2 * d.scat_w + 2 * j + (im.g & 1);
+        }
+        const float* arow = nullptr;
+        if (addend != nullptr) {
+          const int g = min(max(__ldg(gidx + static_cast<long long>(im.g) * rows + R), 0), d.G - 1);
+          arow = addend + static_cast<size_t>(b) * d.Cout * d.G + g;
+        }
+        float* o = out + obase + static_cast<size_t>(b) * d.Cout * d.P_out + po;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          if (8 * j >= ns) break;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int co = col0 + 8 * j + e;
+            if (co < d.Cout) {
+              float y = fmaf(acc[4 * j + 2 * rr + e], inv_w, shift != nullptr ? __ldg(shift + co) : 0.f);
+              if (arow != nullptr) y += __ldg(arow + static_cast<size_t>(co) * d.G);
+              o[static_cast<size_t>(co) * d.P_out] = fmaxf(y, floor_v);
+            }
           }
         }
       }
-      if (warp == 4 && it < 4) PW_TL(3, 2 * it + 1);
     }
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc(tm, 512);
   if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[126] = clock64();
-#undef PW_TL
 }
 
 }  // namespace sonet
@@ -636,37 +396,6 @@ extern "C" int sonet_pointwise_tc_pack_groups(const float* W, int G, int Cout, i
   return SONET_OK;
 }
 
-// cuTensorMapEncodeTiled through the runtime's driver entry point lookup (no link against libcuda)
-typedef CUresult (*TensorMapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                      const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                      const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static TensorMapEncodeFn tensor_map_encoder() {
-  static TensorMapEncodeFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      p = nullptr;
-    cudaGetLastError();
-    return reinterpret_cast<TensorMapEncodeFn>(p);
-  }();
-  return fn;
-}
-// 3-D map over x[B][C][P] fp32, box [64 p][64 c][1]; false when the layout does not qualify
-static bool make_activation_map(CUtensorMap* m, const float* x, int B, int C, int P, int box_c = 64) {
-  TensorMapEncodeFn enc = tensor_map_encoder();
-  if (enc == nullptr || P % 64 != 0 || !sonet::aligned16(x)) return false;
-  const cuuint64_t gdim[3] = {static_cast<cuuint64_t>(P), static_cast<cuuint64_t>(C),
-                              static_cast<cuuint64_t>(B)};
-  const cuuint64_t gstr[2] = {static_cast<cuuint64_t>(P) * 4, static_cast<cuuint64_t>(C) * P * 4};
-  const cuuint32_t box[3] = {64, static_cast<cuuint32_t>(box_c), 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), gdim, gstr, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 struct TcExt {   // grouped / split-K / scatter launch options (defaults = the plain layer)
   int groups = 1, splits = 1, scat_w = 0, P_out = 0, conv_w = 0;
   const float* inv_ptr = nullptr;
@@ -686,13 +415,13 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   if (B == 0 || P == 0) return SONET_OK;
   SONET_REQUIRE(x0 && blob && out, "pointwise_tc: null pointer");
   SONET_REQUIRE(C1 == 0 || x1 != nullptr, "pointwise_tc: x1 null with C1=%d", C1);
+  SONET_REQUIRE(C1 == 0 || ext.groups == 1, "pointwise_tc: two sources need groups == 1");
   SONET_REQUIRE(!addend || (gidx && G >= 1), "pointwise_tc: addend needs gidx and G");
   SONET_REQUIRE(aligned16(blob), "pointwise_tc: weight blob must be 16-byte aligned");
   Dims d;
   d.C0 = C0; d.C1 = C1; d.B = B; d.P = P; d.Cout = Cout; d.relu = relu; d.G = G;
   d.conv_w = ext.conv_w;
   d.cpt = 1;
-  d.h0 = 0;
   if (ext.conv_w > 0) {
     SONET_REQUIRE(C1 == 0 && C0 % KCH == 0 && P % 64 == 0 && P % ext.conv_w == 0 && ext.groups == 4,
                   "pointwise_tc: conv mode needs Cin %% 64 == 0, H*W %% 64 == 0 and the 4 parity groups");
@@ -700,16 +429,8 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   }
   d.cin_pad = ext.conv_w > 0 ? 4 * C0 : (C0 + C1 + 15) / 16 * 16;
   d.kchunks = (d.cin_pad + KCH - 1) / KCH;
-  d.ntiles = ((Cout + 63) / 64 * 64 + NT - 1) / NT;
+  d.ntiles = ((Cout + 63) / 64 * 64 + NSUB - 1) / NSUB;
   d.inv = inv_scale;
-  d.vec4 = (P % 4 == 0) && aligned16(x0) && (C1 == 0 || aligned16(x1));
-  XMaps xm;
-  std::memset(&xm, 0, sizeof(xm));
-  CUtensorMap& xmap = xm.m[0];
-  static const bool tma_off = [] {
-    const char* e = getenv("SONET_PW_TMA");
-    return e != nullptr && e[0] == '0';
-  }();
   SONET_REQUIRE(ext.groups >= 1 && ext.splits >= 1 && d.kchunks % ext.splits == 0,
                 "pointwise_tc: %d K chunks cannot be split %d ways", d.kchunks, ext.splits);
   d.groups = ext.groups;
@@ -722,24 +443,6 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   d.blob_gstride = ext.blob_gstride;
   d.out_gstride = ext.out_gstride;
   d.out_sstride = ext.out_sstride;
-  if (ext.conv_w > 0) {   // x = three horizontally shifted copies [3*B, Cin, P]; TMA is mandatory
-    d.tma = make_activation_map(&xmap, x0, 3 * B, C0, P) ? 1 : 0;
-    SONET_REQUIRE(d.tma, "pointwise_tc: conv mode needs the tensor-map TMA path");
-  } else {
-    d.tma = (!tma_off && make_activation_map(&xmap, x0, ext.groups * B, C0, P)) ? 1 : 0;
-    if (d.tma && C1 > 0) {   // two sources: x1's map and the two short boxes of the straddling chunk
-      static const bool tma2_off = [] {
-        const char* e = getenv("SONET_PW_TMA2");
-        return e != nullptr && e[0] == '0';
-      }();
-      d.h0 = C0 % KCH;
-      bool ok = !tma2_off && ext.groups == 1 && make_activation_map(&xm.m[1], x1, B, C1, P);
-      if (ok && d.h0 > 0)
-        ok = make_activation_map(&xm.m[2], x0, B, C0, P, d.h0) &&
-             make_activation_map(&xm.m[3], x1, B, C1, P, KCH - d.h0);
-      d.tma = ok ? 1 : 0;
-    }
-  }
   const long long rows = static_cast<long long>(B) * P;
   d.row_tiles = static_cast<int>((rows + TILE - 1) / TILE);
   const long long items = static_cast<long long>(d.row_tiles) * d.ntiles * ext.groups * ext.splits;
@@ -748,7 +451,7 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   cudaFuncSetAttribute(pointwise_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   const int grid = static_cast<int>(std::min<long long>(items, sm_count()));
   pointwise_tc_kernel<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
-      x0, x1, static_cast<const unsigned char*>(blob), shift, addend, gidx, out, d, dbg, xm);
+      x0, x1, static_cast<const unsigned char*>(blob), shift, addend, gidx, out, d, dbg);
   return check_launch("pointwise_tc");
 }
 

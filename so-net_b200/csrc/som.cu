@@ -1,4 +1,4 @@
-// som.cu — SOM node <-> point assignment for sm_100a.
+// som.cu — SOM node <-> point assignment for sm_90a.
 //
 // Replaces BatchSOM.query_topk (util/som.py:237-269) and the dense-mask arithmetic that
 // Encoder.forward builds on top of it (models/networks.py:127-143, 168-172). The reference
@@ -30,7 +30,7 @@ __global__ void __launch_bounds__(256)
                       int32_t* __restrict__ idx32, int64_t* __restrict__ idx64,
                       int32_t* __restrict__ row_flag, int32_t* __restrict__ mask) {
   // nodes NEGATED and packed two per register pair: p - n == p + (-n) bit for bit, and the packed
-  // add/mul (FADD2/FMUL2) round each half like the scalar ops (sums stay scalar: common.cuh)
+  // add/mul round each half like the scalar ops (sums stay scalar: common.cuh)
   __shared__ float2 snx[SOM_MAX_M / 2], sny[SOM_MAX_M / 2], snz[SOM_MAX_M / 2];
   const int b = blockIdx.y;
   const float* nb = node + static_cast<size_t>(b) * 3 * M;

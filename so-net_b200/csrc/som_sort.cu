@@ -2,10 +2,10 @@
 //
 // The reference pools the first PointResNet's output per SOM node with index_max on the stacked
 // copies in their original order (models/networks.py:181-185). When `first_pn_out` itself is not
-// needed (classifier, auto-encoder) sonet_b200 never writes it: the tcgen05 kernel consumes the
-// stacked copies GROUPED BY NODE, so that the 32 lanes of an epilogue warp (32 consecutive
-// sorted copies) belong to one or two nodes and the per-node max of 16 channels is one shuffle
-// transpose-reduce plus one 16-lane atomic max (csrc/pointmlp_tc.cu, POOL variant). This file
+// needed (classifier, auto-encoder) sonet_b200 never writes it: the wgmma kernel consumes the
+// stacked copies GROUPED BY NODE, so that the 16 rows an epilogue warp holds (16 consecutive
+// sorted copies) usually belong to one node and the per-node max of a column is one shuffle
+// reduction plus one atomic max per column (csrc/pointmlp_tc.cu, POOL variant). This file
 // provides
 //
 //   som_sort_decenter_kernel   per cloud: bucket the k*N stacked copies by node (offsets from the

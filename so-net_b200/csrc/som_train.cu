@@ -1,4 +1,4 @@
-// som_train.cu — batch-SOM training (SURVEY.md §8f-4) for sm_100a.
+// som_train.cu — batch-SOM training (SURVEY.md §8f-4) for sm_90a.
 //
 // Replaces BatchSOM.batch_update / BatchSOM.optimize (util/som.py:295-366): T assign-and-update
 // iterations per cloud. The reference materialises diff[B,3,N,M], a float one-hot mask [B,N,M] and
@@ -11,7 +11,7 @@
 //   1. assignment (util/som.py:301-309): d = ((x-n)**2).sum(1) evaluated as (dx*dx+dy*dy)+dz*dz
 //      with separate roundings (no FMA) — bit-equal distances; torch.min -> first minimal index
 //      (strict '<' over ascending node index).
-//      Nodes are kept negated and packed two per register pair for the FADD2/FMUL2 forms.
+//      Nodes are kept negated and packed two per register pair (add2_rn / mul2_rn, common.cuh).
 //   2. per-node statistics (:313-321): count and coordinate sums. The reference's torch.sum is a
 //      cascade summation (error ~1 ulp); sums here are accumulated in fp64 in a FIXED order and
 //      rounded once to fp32 — measured: a plain fp32 accumulation drifts by 1e-7 per sum, which
@@ -58,8 +58,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1)
   const float* xg = x + static_cast<size_t>(b) * 3 * N;
   const float* ni = node_init + (node_init_batched ? static_cast<size_t>(b) * 3 * M : 0);
   for (int m = tid; m < M; m += ST_THREADS) snode[m] = make_float4(ni[m], ni[M + m], ni[2 * M + m], 0.f);
-  // packed, negated copies of the nodes for the assignment (p - n == p + (-n) bit for bit; FADD2 /
-  // FMUL2 round each half like the scalar ops, sums stay scalar — common.cuh); odd M: the last
+  // packed, negated copies of the nodes for the assignment (p - n == p + (-n) bit for bit; add2_rn /
+  // mul2_rn round each half like the scalar ops, sums stay scalar — common.cuh); odd M: the last
   // pair repeats its node and the duplicate is skipped
   auto pack_nodes = [&]() {
     for (int m2 = tid; m2 < MP; m2 += ST_THREADS) {

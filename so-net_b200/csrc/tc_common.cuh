@@ -1,348 +1,76 @@
-// tc_common.cuh — tcgen05 / TMEM / UMMA-descriptor helpers (sm_100a inline PTX).
+// tc_common.cuh — Hopper warpgroup MMA (wgmma) helpers and operand conversions (sm_90a inline PTX).
 //
-// Encodings follow the PTX ISA "tcgen05" matrix/instruction descriptors (cross-checked against
-// the field layouts in CUTLASS cute/arch/mma_sm100_desc.hpp, which is only read, not included).
+// Encodings follow the PTX ISA "wgmma" shared-memory matrix descriptor. Every operand image in
+// this project is K-major without swizzle ("interleave"): core matrices of 8 rows x 16 bytes
+// (128 contiguous bytes, row r at +16*r).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "wgmma_ops.cuh"
 
 namespace sonet {
 namespace tc {
 
-// ---- TMEM allocation (one warp, .sync.aligned) -------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// all previously issued tcgen05.mma of this thread arrive on `bar` when complete
-__device__ __forceinline__ void commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// as commit(), but arrives on the barrier at the same offset in every CTA of cta_mask (cluster)
-__device__ __forceinline__ void commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-// 1-D bulk copy global -> the same shared-memory offset of every CTA in cta_mask; each destination
-// CTA's mbarrier (same offset) receives complete_tx for `bytes`.
-__device__ __forceinline__ void bulk_g2s_multicast(void* dst_smem, const void* src_gmem,
-                                                   uint32_t bytes, uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster "
-      "[%0], [%1], %2, [%3], %4;" ::"r"(smem_u32(dst_smem)),
-      "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
 // ---- descriptors ---------------------------------------------------------------------------------
-// Instruction descriptor, kind::f16: D=F32 (c_format=1, bit 4), A=B=BF16 (format 1, bits 7 and
-// 10), both operands K-major (bits 15,16 = 0), N>>3 at bit 17, M>>4 at bit 24.
-__host__ __device__ constexpr uint32_t idesc_bf16_f32(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-// Shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"): the operand is stored as
-// core matrices of 8 rows x 16 bytes (128 contiguous bytes, row r at +16*r);
+// Shared-memory matrix descriptor, K-major, no swizzle:
 //   LBO = byte distance between the two core matrices adjacent along K (bits 16..29, >>4)
 //   SBO = byte distance between 8-row groups along M/N            (bits 32..45, >>4)
-// bits 46..47 = descriptor version 1 (Blackwell); layout type (bits 61..63) = 0.
+// layout type (bits 62..63) = 0. Advancing the start address by n bytes is desc + (n >> 4).
 __host__ __device__ constexpr uint64_t smem_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   return static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4) |
          (static_cast<uint64_t>((lbo >> 4) & 0x3FFFu) << 16) |
-         (static_cast<uint64_t>((sbo >> 4) & 0x3FFFu) << 32) | (1ull << 46);
+         (static_cast<uint64_t>((sbo >> 4) & 0x3FFFu) << 32);
 }
 
-// ---- MMA issue (single thread) -----------------------------------------------------------------
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                       uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// ---- wgmma ordering ------------------------------------------------------------------------------
+// fence before the first wgmma that reads accumulator registers written by ordinary instructions
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-// D[tmem] (+)= A[tmem] * B[smem desc]^T   (A: lane = row, 2 bf16 per 32-bit column along K)
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                       uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// wait until at most N committed groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// shared-memory writes of ordinary instructions become visible to wgmma / TMA (the async proxy)
+__device__ __forceinline__ void fence_proxy_async() {
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+// named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// ---- warp-converged issue: every lane of the (converged) MMA warp calls these with warp-uniform
-// operands; elect.sync picks one lane that actually issues. Issuing from inside a divergent
-// `if (lane == 0)` region instead makes nvcc wrap every UTCHMMA in an ELECT/BRA uniformisation
-// loop (~100 cycles per MMA, measured: the kernel became issue-bound).
-__device__ __forceinline__ void mma_ts_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, e;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "elect.sync _|e, 0xffffffff;\n"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// The three products of one fp16 hi/lo split K step — hi(a)*hi(b), lo(a)*hi(b), hi(a)*lo(b) —
-// behind ONE elect: a third of the ELECT/VOTE traffic of three mma_ts_elect calls on the issuing
-// warp, whose instruction stream is what bounds layer 3 when the epilogue warps are busy.
-__device__ __forceinline__ void mma_ts_elect3(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo,
-                                              uint64_t b_hi, uint64_t b_lo, uint32_t idesc,
-                                              uint32_t accumulate_first) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, e, t;\n"
-      "setp.ne.b32 p, %6, 0;\n"
-      "setp.eq.b32 t, 0, 0;\n"
-      "elect.sync _|e, 0xffffffff;\n"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %3, %5, p;\n"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [%2], %3, %5, t;\n"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %4, %5, t;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_hi), "r"(a_lo), "l"(b_hi), "l"(b_lo), "r"(idesc), "r"(accumulate_first)
-      : "memory");
-}
-// One K STAGE of the split product — KS k-steps of 16, three MMAs each — behind ONE elect, with
-// the running TMEM / descriptor addresses advanced inside the PTX block. ptxas then keeps them in
-// the uniform datapath (UIADD3 + UTCHMMA, ~4 instructions per MMA); one asm statement per MMA cost
-// four R2UR.BROADCAST plus votes per MMA (~50 issue cycles, more than an N=96 MMA executes).
-// a0: TMEM address of the first hi column group (lo = +8, next k-step = +16);
-// bh0/bl0: descriptors of the hi/lo weight images (next k-step = +16 encoded = +256 B).
-#define SONET_MMA3 \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [ah], bh, %4, t;\n" \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [al], bh, %4, t;\n" \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [ah], bl, %4, t;\n"
-#define SONET_ADV \
-  "add.u32 ah, ah, 16;\n add.u32 al, al, 16;\n add.u64 bh, bh, 16;\n add.u64 bl, bl, 16;\n"
-#define SONET_STAGE_HEAD \
-  "{\n" \
-  ".reg .pred p, e, t;\n" \
-  ".reg .b32 ah, al;\n" \
-  ".reg .b64 bh, bl;\n" \
-  "setp.ne.b32 p, %5, 0;\n" \
-  "setp.eq.b32 t, 0, 0;\n" \
-  "elect.sync _|e, 0xffffffff;\n" \
-  "mov.b32 ah, %1;\n" \
-  "add.u32 al, ah, 8;\n" \
-  "mov.b64 bh, %2;\n" \
-  "mov.b64 bl, %3;\n" \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [ah], bh, %4, p;\n" \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [al], bh, %4, t;\n" \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [ah], bl, %4, t;\n"
-template <int KS>
-__device__ __forceinline__ void mma_ts_stage(uint32_t d_tmem, uint32_t a0, uint64_t bh0,
-                                             uint64_t bl0, uint32_t idesc,
-                                             uint32_t accumulate_first) {
-  static_assert(KS == 2 || KS == 4, "mma_ts_stage: 2 or 4 k-steps");
-  if constexpr (KS == 2) {
-    asm volatile(SONET_STAGE_HEAD SONET_ADV SONET_MMA3 "}\n" ::"r"(d_tmem), "r"(a0), "l"(bh0),
-                 "l"(bl0), "r"(idesc), "r"(accumulate_first)
-                 : "memory");
-  } else {
-    asm volatile(SONET_STAGE_HEAD SONET_ADV SONET_MMA3 SONET_ADV SONET_MMA3 SONET_ADV SONET_MMA3
-                 "}\n" ::"r"(d_tmem),
-                 "r"(a0), "l"(bh0), "l"(bl0), "r"(idesc), "r"(accumulate_first)
-                 : "memory");
-  }
-}
-#undef SONET_MMA3
-#undef SONET_ADV
-#undef SONET_STAGE_HEAD
-// SS-mode K stage: NKS k-steps (1..4) of the split product, A and B images in shared memory, one
-// elect; descriptors advance by +16 encoded (= 256 B = one 16-wide k-step) inside the block.
-template <int NKS>
-__device__ __forceinline__ void mma_ss_stage(uint32_t d_tmem, uint64_t ah0, uint64_t al0,
-                                             uint64_t bh0, uint64_t bl0, uint32_t idesc,
-                                             uint32_t accumulate_first) {
-  static_assert(NKS >= 1 && NKS <= 4, "mma_ss_stage: 1..4 k-steps");
-#define SONET_SS3(P0)                                                   \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bh, %5, " P0 ";\n" \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], al, bh, %5, t;\n"      \
-  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], ah, bl, %5, t;\n"
-#define SONET_SSADV \
-  "add.u64 ah, ah, 16;\n add.u64 al, al, 16;\n add.u64 bh, bh, 16;\n add.u64 bl, bl, 16;\n"
-#define SONET_SSHEAD               \
-  "{\n"                           \
-  ".reg .pred p, e, t;\n"         \
-  ".reg .b64 ah, al, bh, bl;\n"   \
-  "setp.ne.b32 p, %6, 0;\n"       \
-  "setp.eq.b32 t, 0, 0;\n"        \
-  "elect.sync _|e, 0xffffffff;\n" \
-  "mov.b64 ah, %1;\n mov.b64 al, %2;\n mov.b64 bh, %3;\n mov.b64 bl, %4;\n"
-#define SONET_SSOPS                                                                          \
-  ::"r"(d_tmem), "l"(ah0), "l"(al0), "l"(bh0), "l"(bl0), "r"(idesc), "r"(accumulate_first) \
-      : "memory"
-  if constexpr (NKS == 1) {
-    asm volatile(SONET_SSHEAD SONET_SS3("p") "}\n" SONET_SSOPS);
-  } else if constexpr (NKS == 2) {
-    asm volatile(SONET_SSHEAD SONET_SS3("p") SONET_SSADV SONET_SS3("t") "}\n" SONET_SSOPS);
-  } else if constexpr (NKS == 3) {
-    asm volatile(SONET_SSHEAD SONET_SS3("p") SONET_SSADV SONET_SS3("t") SONET_SSADV SONET_SS3("t")
-                 "}\n" SONET_SSOPS);
-  } else {
-    asm volatile(SONET_SSHEAD SONET_SS3("p") SONET_SSADV SONET_SS3("t") SONET_SSADV SONET_SS3("t")
-                     SONET_SSADV SONET_SS3("t") "}\n" SONET_SSOPS);
-  }
-#undef SONET_SS3
-#undef SONET_SSADV
-#undef SONET_SSHEAD
-#undef SONET_SSOPS
-}
-__device__ __forceinline__ void mma_ss_elect(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, e;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "elect.sync _|e, 0xffffffff;\n"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void commit_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred e;\n"
-      "elect.sync _|e, 0xffffffff;\n"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void commit_multicast_elect(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "{\n"
-      ".reg .pred e;\n"
-      "elect.sync _|e, 0xffffffff;\n"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// ---- TMEM <-> registers: 32x32b shape = each thread its own lane, N consecutive 32-bit columns ----
-__device__ __forceinline__ void ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, "
-      "[%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-      "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-
-// ---- bf16 hi/lo split of 16 fp32 values into 8 + 8 packed words -----------------------------------
-// word j of hi = {bf16(x[2j+1]) : bf16(x[2j])} (low half = even channel = lower K index);
-// lo = bf16(x - float(hi)). hi*W_hi + lo*W_hi + hi*W_lo reproduces the fp32 product to ~2^-16.
+// ---- conversions -----------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
   return r;
 }
-__device__ __forceinline__ void split16(const float (&x)[16], uint32_t (&out)[16]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const uint32_t h = pack_bf16x2(x[2 * j], x[2 * j + 1]);
-    const float h0 = __uint_as_float(h << 16), h1 = __uint_as_float(h & 0xFFFF0000u);
-    out[j] = h;
-    out[8 + j] = pack_bf16x2(x[2 * j] - h0, x[2 * j + 1] - h1);
-  }
-}
-
-// ---- fp16 hi/lo split (22 significant bits, vs 16 for bf16) ---------------------------------------
-// Same instruction kind (kind::f16) and rate as bf16; operands must stay inside the fp16 range
-// (|x| <= 65504) — the conversion saturates activations, weights are pre-scaled by a power of two.
-__host__ __device__ constexpr uint32_t idesc_f16_f32(int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-// Two floats -> packed fp16 pair (lo = low half) with saturation to the largest finite fp16
-// (F2FP.SATFINITE: one instruction, where fminf/fmaxf clamps in front of a plain conversion cost
-// two to four more per pair). NaN stays NaN.
+// fp16 hi/lo split (22 significant bits, vs 16 for bf16): x*w ~= hi(x)*hi(w) + lo(x)*hi(w) +
+// hi(x)*lo(w). Operands must stay inside the fp16 range (|x| <= 65504): the conversion saturates
+// activations, weights are pre-scaled by a power of two.
+// Two floats -> packed fp16 pair (lo = low half = lower K index) with saturation to the largest
+// finite fp16 (one F2FP.SATFINITE, where clamps in front of a plain conversion cost more). NaN
+// stays NaN.
 __device__ __forceinline__ uint32_t pack_f16x2_sat(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
-__device__ __forceinline__ void split16_f16(const float (&x)[16], uint32_t (&out)[16]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const uint32_t h = pack_f16x2_sat(x[2 * j], x[2 * j + 1]);   // low half = even channel
-    const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&h));
-    out[j] = h;
-    out[8 + j] = pack_f16x2_sat(x[2 * j] - hf.x, x[2 * j + 1] - hf.y);
-  }
+// hi and lo words of the pair (a, b)
+__device__ __forceinline__ void split2_f16(float a, float b, uint32_t& hi, uint32_t& lo) {
+  hi = pack_f16x2_sat(a, b);
+  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  lo = pack_f16x2_sat(a - hf.x, b - hf.y);
 }
 
-// bounded mbarrier wait: a protocol bug traps instead of hanging the GPU box
-static __device__ __noinline__ void mbar_timeout(int tag, uint32_t parity) {
-  printf("[sonet] mbarrier wait timed out: tag %d block %d thread %d parity %u\n", tag,
-         (int)blockIdx.x, (int)threadIdx.x, parity);
-  __trap();
-}
-// Spin on the barrier phase; traps (instead of hanging the GPU) after 2^24 failed try_waits.
-// The whole loop is ONE asm statement: a C-level loop on the try_wait result is a divergent loop
-// in the compiler's eyes (it was also unrolled 64x — 2 KB of code per wait site — before
-// `#pragma unroll 1`), and values live across it fall out of the uniform datapath, which the MMA
-// issuing warp needs for its descriptors. A timeout traps (cudaErrorLaunchFailure on the host).
+// Spin on the barrier phase; a protocol bug traps (instead of hanging the GPU) after 2^24 failed
+// try_waits.
+// The whole loop is ONE asm statement so that values live across it stay in the uniform datapath.
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity, int tag) {
   (void)tag;
   asm volatile(
@@ -381,7 +109,10 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity
     if (done) return;
     __nanosleep(100);
   }
-  mbar_timeout(tag, parity);
+  (void)tag;
+  // no call here (not even printf): a call inside a kernel that issues wgmma makes ptxas
+  // serialize every wgmma of the kernel
+  asm volatile("trap;");
 }
 
 }  // namespace tc

@@ -1,7 +1,7 @@
-// tc_probe.cu — diagnostic kernel: one 128 x N x K bf16 GEMM on tcgen05 with A from shared memory
-// (SS) or from tensor memory (TS), fp32 accumulate in TMEM. Used by tests/test_gpu_tcgen05.py to
-// pin the descriptor encodings and the TMEM operand layout that the fused point-MLP kernel
-// (pointmlp_tc.cu) relies on. Not on the product path.
+// tc_probe.cu — diagnostic kernel: one 128 x N x K bf16 GEMM on Hopper wgmma with A from shared
+// memory (SS) or from registers (RS), fp32 accumulate in registers. Used by
+// tests/test_gpu_tcgen05.py to pin the shared-memory descriptor encoding (LBO/SBO roles) and the
+// K-major no-swizzle operand layout that the point-MLP kernels rely on. Not on the product path.
 #include "tc_common.cuh"
 
 namespace sonet {
@@ -11,16 +11,29 @@ __device__ __forceinline__ uint32_t canon_off(int r, int k, uint32_t lbo, uint32
   return (r >> 3) * sbo + (k >> 3) * lbo + (r & 7) * 16 + (k & 7) * 2;
 }
 
+template <int N>
+__device__ __forceinline__ void probe_mma(float (&acc)[N / 2], uint64_t adesc, const uint32_t (&a)[4],
+                                          uint64_t bdesc, int mode) {
+  if constexpr (N == 16) {
+    if (mode == 0) tc::wgmma_bf16_n16(acc, adesc, bdesc, 1); else tc::wgmma_bf16_rs_n16(acc, a, bdesc, 1);
+  } else if constexpr (N == 32) {
+    if (mode == 0) tc::wgmma_bf16_n32(acc, adesc, bdesc, 1); else tc::wgmma_bf16_rs_n32(acc, a, bdesc, 1);
+  } else if constexpr (N == 64) {
+    if (mode == 0) tc::wgmma_bf16_n64(acc, adesc, bdesc, 1); else tc::wgmma_bf16_rs_n64(acc, a, bdesc, 1);
+  } else {
+    if (mode == 0) tc::wgmma_bf16_n128(acc, adesc, bdesc, 1); else tc::wgmma_bf16_rs_n128(acc, a, bdesc, 1);
+  }
+}
+
+template <int N>
 __global__ void __launch_bounds__(128, 1)
-    tc_probe_kernel(const float* __restrict__ A, const float* __restrict__ Bm, int N, int K,
-                    int mode, uint32_t lbo_a, uint32_t sbo_a, uint32_t lbo_b, uint32_t sbo_b,
+    tc_probe_kernel(const float* __restrict__ A, const float* __restrict__ Bm, int K, int mode,
+                    uint32_t lbo_a, uint32_t sbo_a, uint32_t lbo_b, uint32_t sbo_b,
                     int swap_fields, float* __restrict__ D) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_base_s;
   unsigned char* a_img = smem;
   unsigned char* b_img = smem + 128 * K * 2;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   for (int i = tid; i < 128 * K; i += 128) {
     const int r = i / K, k = i % K;
@@ -32,68 +45,44 @@ __global__ void __launch_bounds__(128, 1)
     *reinterpret_cast<__nv_bfloat16*>(b_img + canon_off(r, k, lbo_b, sbo_b)) =
         __float2bfloat16_rn(Bm[i]);
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  if (tid == 0) {
-    mbar_init(&bar, 1);
-    mbar_fence_init();
-  }
-  if (warp == 0) {
-    tc::tmem_alloc(&tmem_base_s, 256);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
+  tc::fence_proxy_async();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tbase = tmem_base_s;
-  const uint32_t lane_base = tbase + (static_cast<uint32_t>(warp * 32) << 16);
-  const uint32_t a_col = 128;  // A operand (TS mode) lives at columns [128, 128 + K/2)
 
-  if (mode == 1) {
-    // thread = row: pack its K bf16 values, 2 per 32-bit column
-    for (int c0 = 0; c0 < K / 2; c0 += 16) {
-      uint32_t w[16];
+  // accumulator / register-A fragment: rows g and g + 8 (g = 16*warp + lane/4), k / n pairs at
+  // 2*(lane%4)
+  const int g = 16 * warp + (lane >> 2), c2 = 2 * (lane & 3);
+  for (int h = 0; h < 2; ++h) {   // two M=64 halves of the 128-row tile
+    float acc[N / 2];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int k = 2 * (c0 + j);
-        w[j] = tc::pack_bf16x2(A[tid * K + k], A[tid * K + k + 1]);
-      }
-      tc::st16(lane_base + a_col + c0, w);
-    }
-    tc::wait_st();
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-
-  if (tid == 0) {
-    const uint32_t idesc = tc::idesc_bf16_f32(128, N);
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    tc::wg_fence();
     for (int ks = 0; ks < K / 16; ++ks) {
-      // one K step = 16 bf16 = two 16-byte chunks along K
-      const uint32_t a_addr = smem_u32(a_img) + 2 * ks * lbo_a;
+      // one K step = 16 bf16 = two 16-byte core matrices along K
+      const uint32_t a_addr = smem_u32(a_img) + 8 * h * sbo_a + 2 * ks * lbo_a;
       const uint32_t b_addr = smem_u32(b_img) + 2 * ks * lbo_b;
       const uint64_t adesc = swap_fields ? tc::smem_desc(a_addr, sbo_a, lbo_a)
                                          : tc::smem_desc(a_addr, lbo_a, sbo_a);
       const uint64_t bdesc = swap_fields ? tc::smem_desc(b_addr, sbo_b, lbo_b)
                                          : tc::smem_desc(b_addr, lbo_b, sbo_b);
-      if (mode == 0)
-        tc::mma_ss(tbase, adesc, bdesc, idesc, ks > 0);
-      else
-        tc::mma_ts(tbase, tbase + a_col + ks * 8, bdesc, idesc, ks > 0);
+      uint32_t a[4] = {0, 0, 0, 0};
+      if (mode == 1) {
+        const float* r0 = A + static_cast<size_t>(64 * h + g) * K + 16 * ks + c2;
+        const float* r1 = r0 + 8 * K;
+        a[0] = tc::pack_bf16x2(r0[0], r0[1]);
+        a[1] = tc::pack_bf16x2(r1[0], r1[1]);
+        a[2] = tc::pack_bf16x2(r0[8], r0[9]);
+        a[3] = tc::pack_bf16x2(r1[8], r1[9]);
+      }
+      probe_mma<N>(acc, adesc, a, bdesc, mode);
     }
-    tc::commit(&bar);
-  }
-  tc::mbar_wait_bounded(&bar, 0, 1);
-  tc::fence_after_sync();
-  for (int c0 = 0; c0 < N; c0 += 16) {
-    uint32_t v[16];
-    tc::ld16(lane_base + c0, v);
-    tc::wait_ld();
+    tc::wg_commit();
+    tc::wg_wait<0>();
 #pragma unroll
-    for (int j = 0; j < 16; ++j) D[tid * N + c0 + j] = __uint_as_float(v[j]);
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        D[static_cast<size_t>(64 * h + g + 8 * (e >> 1)) * N + 8 * j + c2 + (e & 1)] = acc[4 * j + e];
   }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tbase, 256);
 }
 
 }  // namespace sonet
@@ -101,8 +90,9 @@ __global__ void __launch_bounds__(128, 1)
 extern "C" int sonet_debug_tc_probe(const float* A, const float* Bm, int N, int K, int mode,
                                     int layout, int swap_fields, float* D, sonet_stream_t stream) {
   using namespace sonet;
-  SONET_REQUIRE(N >= 16 && N <= 128 && N % 16 == 0, "tc_probe: N must be a multiple of 16 in [16,128]");
+  SONET_REQUIRE(N == 16 || N == 32 || N == 64 || N == 128, "tc_probe: N must be 16, 32, 64 or 128");
   SONET_REQUIRE(K >= 16 && K <= 256 && K % 32 == 0, "tc_probe: K must be a multiple of 32 in [32,256]");
+  SONET_REQUIRE(mode == 0 || mode == 1, "tc_probe: mode must be 0 (A in shared memory) or 1 (registers)");
   SONET_REQUIRE(A && Bm && D, "tc_probe: null pointer");
   uint32_t lbo_a, sbo_a, lbo_b, sbo_b;
   if (layout == 0) {  // K chunks adjacent (128 B apart), 8-row groups K*16 B apart
@@ -114,62 +104,57 @@ extern "C" int sonet_debug_tc_probe(const float* A, const float* Bm, int N, int 
     lbo_b = static_cast<uint32_t>(N) * 16;
   }
   const size_t smem = static_cast<size_t>(128 + N) * K * 2;
-  cudaFuncSetAttribute(tc_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       static_cast<int>(smem));
-  tc_probe_kernel<<<1, 128, smem, as_stream(stream)>>>(A, Bm, N, K, mode, lbo_a, sbo_a, lbo_b, sbo_b,
-                                                       swap_fields, D);
+  auto kern = N == 16 ? tc_probe_kernel<16> : N == 32 ? tc_probe_kernel<32>
+            : N == 64 ? tc_probe_kernel<64> : tc_probe_kernel<128>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  kern<<<1, 128, smem, as_stream(stream)>>>(A, Bm, K, mode, lbo_a, sbo_a, lbo_b, sbo_b, swap_fields, D);
   return check_launch("tc_probe");
 }
 
-// ---- MMA rate microbenchmark: `iters` back-to-back M=128 x N x 16 MMAs, SS or TS mode -----------
+// ---- MMA rate microbenchmark: `iters` back-to-back M=64 x N x 16 fp16 wgmmas (A and B in shared
+// memory) of one warpgroup ----------------------------------------------------------------------------
 namespace sonet {
+template <int N>
 __global__ void __launch_bounds__(128, 1)
-    tc_rate_kernel(int mode, int N, uint32_t sbo, int iters, long long* __restrict__ cycles) {
+    tc_rate_kernel(uint32_t sbo, int iters, long long* __restrict__ cycles) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_base_s;
-  const int warp = threadIdx.x >> 5;
   for (int i = threadIdx.x; i < 48 * 1024 / 4; i += 128) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  tc::fence_proxy_async();
+  __syncthreads();
+  const uint32_t a_addr = smem_u32(smem), b_addr = smem_u32(smem) + 16384;
+  const uint64_t ad = tc::smem_desc(a_addr, 128, sbo), bd = tc::smem_desc(b_addr, 128, sbo);
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  const long long t0 = clock64();
+  tc::wg_fence();
+  for (int i = 0; i < iters; ++i) {
+    if constexpr (N == 64) tc::wgmma_f16_n64(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
+    else if constexpr (N == 96) tc::wgmma_f16_n96(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
+    else if constexpr (N == 128) tc::wgmma_f16_n128(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
+    else tc::wgmma_f16_n256(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
+  }
+  tc::wg_commit();
+  tc::wg_wait<0>();
+  const long long t1 = clock64();
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) s += acc[i];
   if (threadIdx.x == 0) {
-    mbar_init(&bar, 1);
-    mbar_fence_init();
+    cycles[0] = t1 - t0;
+    if (s == 12345.f) cycles[1] = 0;   // keeps the accumulators live
   }
-  if (warp == 0) {
-    tc::tmem_alloc(&tmem_base_s, 512);
-    tc::tmem_relinquish();
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tm = tmem_base_s;
-  if (warp == 1) {
-    const uint32_t idesc = tc::idesc_f16_f32(128, N);
-    const uint32_t a_addr = smem_u32(smem), b_addr = smem_u32(smem) + 16384;
-    const uint64_t ad = tc::smem_desc(a_addr, 128, sbo), bd = tc::smem_desc(b_addr, 128, sbo);
-    const long long t0 = clock64();
-    for (int i = 0; i < iters; ++i) {
-      if (mode == 0)
-        tc::mma_ss_elect(tm, ad + (i & 3) * 16, bd + (i & 3) * 16, idesc, 1);
-      else
-        tc::mma_ts_elect(tm, tm + 256 + (i & 3) * 8, bd + (i & 3) * 16, idesc, 1);
-    }
-    tc::commit_elect(&bar);
-    tc::mbar_wait_bounded(&bar, 0, 77);
-    const long long t1 = clock64();
-    if ((threadIdx.x & 31) == 0) cycles[0] = t1 - t0;
-  }
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc(tm, 512);
 }
 }  // namespace sonet
 
 extern "C" int sonet_debug_tc_mma_rate(int mode, int N, int sbo, int iters, long long* cycles,
                                        sonet_stream_t stream) {
   using namespace sonet;
-  SONET_REQUIRE(N >= 16 && N <= 256 && N % 16 == 0 && cycles, "tc_mma_rate: bad args");
-  cudaFuncSetAttribute(tc_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
-  tc_rate_kernel<<<1, 128, 64 * 1024, as_stream(stream)>>>(mode, N, static_cast<uint32_t>(sbo), iters, cycles);
+  SONET_REQUIRE(mode == 0 && (N == 64 || N == 96 || N == 128 || N == 256) && cycles,
+                "tc_mma_rate: mode 0 with N in {64, 96, 128, 256}");
+  auto kern = N == 64 ? tc_rate_kernel<64> : N == 96 ? tc_rate_kernel<96>
+            : N == 128 ? tc_rate_kernel<128> : tc_rate_kernel<256>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+  kern<<<1, 128, 64 * 1024, as_stream(stream)>>>(static_cast<uint32_t>(sbo), iters, cycles);
   return check_launch("tc_mma_rate");
 }

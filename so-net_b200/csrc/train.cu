@@ -1,4 +1,4 @@
-// train.cu — train-mode kernels of the point-wise layers (SURVEY.md §8f-2) for sm_100a.
+// train.cu — train-mode kernels of the point-wise layers (SURVEY.md §8f-2) for sm_90a.
 //
 // The reference trains through EquivariantLayer = Conv1d(k=1) -> MyBatchNorm1d (batch statistics,
 // models/layers.py:22-70) -> ReLU, and back-propagates through the per-node pool as the backward
@@ -13,10 +13,10 @@
 //   index_max_backward           grad of first_pn_out through the masked gather: zero-fill +
 //                                scatter-add of grad[b,c,k] at idx[b,c,k] (duplicates — every empty
 //                                node gathers point 0 — are added by ONE thread in ascending k)
-//   tc_pack_device               fp32 weights -> tcgen05 hi/lo blob ON THE DEVICE (weights change
+//   tc_pack_device               fp32 weights -> wgmma hi/lo blob ON THE DEVICE (weights change
 //                                every optimizer step; the eval path packs on the host once), also
 //                                transposed: the dgrad GEMM dx = W^T dy runs on the same generic
-//                                tcgen05 layer kernel as the forward (csrc/pointwise_tc.cu)
+//                                wgmma layer kernel as the forward (csrc/pointwise_tc.cu)
 //
 // All reductions are two-stage with fp64 partial sums in a fixed order: bit-reproducible.
 #include <algorithm>
@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(128)
   }
 }
 
-// ---- device-side weight packing for the tcgen05 layer ---------------------------------------------
+// ---- device-side weight packing for the wgmma layer ---------------------------------------------
 __global__ void __launch_bounds__(256)
     absmax_kernel(const float* __restrict__ w, long long n, unsigned* __restrict__ out_bits) {
   float m = 0.f;
@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(256)
 
 // ---- wgrad helpers ------------------------------------------------------------------------------------
 // dyT[k = b*P + p][co] = dy[b][co][p] * s  (s = scale2[0], a power of two): the "activation" operand
-// of the wgrad GEMM in the [K][rows] layout the generic tcgen05 layer consumes. 32x32 smem tiles.
+// of the wgrad GEMM in the [K][rows] layout the generic wgmma layer consumes. 32x32 smem tiles.
 __global__ void __launch_bounds__(256)
     transpose_scale_kernel(const float* __restrict__ dy, int C, int P, const float* __restrict__ scale2,
                            float* __restrict__ dyT) {
@@ -250,7 +250,7 @@ __global__ void inv_product_kernel(const float* __restrict__ a, const float* __r
   out[0] = a[1] * b[1];
 }
 // x [B][Cin][P] as the "weight" matrix Wl[n = ci][k = b*P + p] of the wgrad GEMM, packed into the
-// tcgen05 blob layout (see tc_pack_device_kernel); K padded with zeros up to kch*64.
+// wgmma blob layout (see tc_pack_device_kernel); K padded with zeros up to kch*64.
 __global__ void __launch_bounds__(256)
     tc_pack_points_kernel(const float* __restrict__ x, int B, int Cin, int P,
                           const float* __restrict__ scale2, unsigned char* __restrict__ blob, int cpad,
@@ -386,7 +386,7 @@ extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, in
                                               const float* shift, int Cout, int relu, int splits,
                                               float* out, float* scratch, sonet_stream_t stream);
 
-// wgrad of a 1x1 convolution on tcgen05: dW[co][ci] = sum_{b,p} dy[b,co,p] * x[b,ci,p].
+// wgrad of a 1x1 convolution on wgmma: dW[co][ci] = sum_{b,p} dy[b,co,p] * x[b,ci,p].
 // Written as the generic layer GEMM out[rows = co][n = ci] = sum_k A[k][co] * Wl[ci][k] with the
 // contraction index k = (b, p): A = dy transposed to [K][Cout] (and pre-scaled: gradients are far
 // below fp16's normal range), Wl = x packed as a weight blob, K split over CTAs with a

@@ -1,4 +1,4 @@
-// upconv.cu — the auto-encoder's up-convolution decoder (SURVEY.md §8f-1) for sm_100a.
+// upconv.cu — the auto-encoder's up-convolution decoder (SURVEY.md §8f-1) for sm_90a.
 //
 // Replaces UpConv.forward (models/layers.py:214-240: nn.Upsample(scale_factor=2) + Conv2d 3x3 pad 1
 // + BatchNorm2d + ReLU) as used by DecoderConv (models/networks.py:394-431).
@@ -14,7 +14,7 @@
 //   upconv_im2col_kernel    gathers the 2x2 neighbourhoods of all four parities,
 //                           xcol[g][b][t*Cin+ci][i*W+j], coalesced along j;
 //   sonet_pointwise_tc_grouped_forward (csrc/pointwise_tc.cu) runs the four GEMMs as ONE grouped
-//                           tcgen05 launch (fp16 hi/lo split, fp32 accumulate) whose epilogue —
+//                           wgmma launch (fp16 hi/lo split, fp32 accumulate) whose epilogue —
 //                           or, for the small maps that need a K split to fill the SMs, the
 //                           split-K reduce kernel — adds the folded shift, applies ReLU and
 //                           interleaves the parities into the [B, Cout, 2H, 2W] output.
@@ -88,9 +88,9 @@ __global__ void __launch_bounds__(256)
 }
 
 // The three horizontally shifted copies [3][B][Cin][H*W] (dx = -1, 0, +1, zero at the row ends)
-// that the conv mode of the grouped tcgen05 kernel reads instead of a 16x im2col: a vertical shift
-// is a plain offset of the TMA point coordinate (its out-of-range part is zero-filled by the TMA
-// unit), only the horizontal one wraps across image rows and has to be materialised.
+// that the conv mode of the grouped wgmma kernel reads instead of a 16x im2col: a vertical shift
+// is a plain offset of the point coordinate (the kernel reads zeros for its out-of-range part),
+// only the horizontal one wraps across image rows and has to be materialised.
 __global__ void __launch_bounds__(256)
     upconv_hshift_kernel(const float* __restrict__ in, long long rows, int H, int W,
                          float* __restrict__ out) {

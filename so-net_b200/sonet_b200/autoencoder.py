@@ -1,4 +1,4 @@
-"""autoencoder.Model — caller-facing wrapper of models/autoencoder.py:13-161 on the B200
+"""autoencoder.Model — caller-facing wrapper of models/autoencoder.py:13-161 on the H100
 networks: encoder + decoder + Chamfer, all on the hand-written kernels in eval mode.
 Double-buffered asynchronous set_input and CUDA-graph replay of test_model():
 _model_base.GraphedModel."""

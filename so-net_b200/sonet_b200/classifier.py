@@ -1,5 +1,5 @@
 """classifier.Model — the caller-facing wrapper of models/classifier.py:15-153 (set_input /
-forward / test_model / optimize), built on the B200 networks. This is the public API bench.py
+forward / test_model / optimize), built on the H100 networks. This is the public API bench.py
 times end to end: host tensors in through set_input, scores out.
 
 set_input is double-buffered and asynchronous, test_model() can replay as one CUDA graph

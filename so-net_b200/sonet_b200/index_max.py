@@ -6,7 +6,7 @@
     forward_cpu(data, index, K)             host tensors, single thread
     forward_multi_thread_cpu(data, index, K, thread_num)
 
-The CUDA entry points run the sm_100a kernel of libsonet_b200 (csrc/index_max.cu) and raise
+The CUDA entry points run the sm_90a kernel of libsonet_b200 (csrc/index_max.cu) and raise
 RuntimeError on non-CUDA / non-contiguous inputs like the reference's CHECK_INPUT
 (index_max.cpp:119-121). The host entry points are the plugin's own CPU API (C++ in the same
 library); they are never used as a fallback for the CUDA path.

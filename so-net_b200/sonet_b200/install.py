@@ -2,7 +2,7 @@
 
     import sonet_b200.install; sonet_b200.install.install("/path/to/SO-Net")
     from models import classifier          # the reference's file, byte-identical
-    model = classifier.Model(opt)          # now built from the B200 networks
+    model = classifier.Model(opt)          # now built from the H100 networks
 
 Registers this package's modules under the names the reference imports
 (models/networks.py:10-17, models/losses.py:9): `index_max`, `util.som`, `models.operations`,

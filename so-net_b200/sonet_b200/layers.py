@@ -1,5 +1,5 @@
 """Layer classes with the reference's constructor signatures and state_dict keys
-(models/layers.py:22-432), running on the sm_100a kernels of libsonet_b200 in eval/no-grad mode.
+(models/layers.py:22-432), running on the sm_90a kernels of libsonet_b200 in eval/no-grad mode.
 
 Dispatch rule (SURVEY.md §8b "Autograd"): the hand-written forward kernels run whenever the module
 is in eval() mode and no INPUT tensor carries a gradient — with or without torch.no_grad(), because
@@ -128,7 +128,7 @@ class _FoldedParams:
 
 
 def invalidate(module):
-    """Drop every derived weight cache (BN-folded weights, tcgen05 packings) below `module`.
+    """Drop every derived weight cache (BN-folded weights, wgmma packings) below `module`.
 
     The caches are keyed on (data_ptr, tensor._version) of the parameters and BN statistics, which
     optimizer steps, load_state_dict() and in-place tensor ops all bump. Writes through `.data`
@@ -205,23 +205,23 @@ class _PointwiseConvBase(nn.Module):
                 and self.normalization in (None, 'batch') and self.activation in (None, 'relu'))
 
     def _train_kernels(self, x):
-        """train() mode on CUDA fp32 with the default norm/activation: the sm_100a train kernels
+        """train() mode on CUDA fp32 with the default norm/activation: the sm_90a train kernels
         (train_ops) instead of the PyTorch composition."""
         return (train_ops.ENABLED and self.training and torch.is_grad_enabled() and x.is_cuda
                 and x.dtype == torch.float32 and self._fast_eligible())
 
     def forward_points(self, x0, x1=None, addend=None, gidx=None):
         """x0 [B,C0,P] (+ x1 [B,C1,P] virtually concatenated on channels) -> [B,Cout,P].
-        Dense layers run on tcgen05 (csrc/pointwise_tc.cu, fp16 hi/lo split); thin ones on the
+        Dense layers run on wgmma (csrc/pointwise_tc.cu, fp16 hi/lo split); thin ones on the
         exact-fp32 CUDA-core kernel (csrc/pointwise.cu)."""
         norm = self.norm if self.normalization == 'batch' else None
         cin = x0.shape[1] + (0 if x1 is None else x1.shape[1])
         cout = self.conv.out_channels
         rows = x0.shape[0] * x0.shape[2]
-        # tcgen05 eligibility: a dense enough contraction (cin >= 32) over at least two 128-row
+        # wgmma eligibility: a dense enough contraction (cin >= 32) over at least two 128-row
         # tiles; thin OUTPUTS (the 128 -> 3 ConvToPC heads) qualify too — the layer is then a
-        # streaming read of the activations, which the TMA-fed kernel does at several times the
-        # rate of the register-tiled fp32 kernel
+        # streaming read of the activations into the tensor-core kernel instead of the
+        # register-tiled fp32 kernel
         if cin >= 32 and rows >= 256 and os.environ.get("SONET_TC", "1") != "0":
             w, shift = self._folded.get(self._conv_weight2d(), self.conv.bias, norm,
                                         transpose=False)
@@ -295,7 +295,7 @@ class MyConv2d(_PointwiseConvBase):
 
 
 def _pick_splits(kchunks, base_items, target=120, cap=32):
-    """K split of a grouped tcgen05 launch: the smallest power of two dividing the number of
+    """K split of a grouped wgmma launch: the smallest power of two dividing the number of
     64-channel K chunks that brings the item count to ~one wave of SMs."""
     s = 1
     while s * 2 <= cap and kchunks % (s * 2) == 0 and base_items * s < target:
@@ -306,7 +306,7 @@ def _pick_splits(kchunks, base_items, target=120, cap=32):
 class UpConv(nn.Module):
     """Nearest x2 upsample + 3x3 conv + BN + act (models/layers.py:214-240), the decoder's
     building block. Eval fast path (SURVEY.md §8f-1): four parity GEMMs over the LOW-resolution
-    map on tcgen05 (csrc/upconv.cu, csrc/pointwise_tc.cu) — the up-sampled image is never built
+    map on wgmma (csrc/upconv.cu, csrc/pointwise_tc.cu) — the up-sampled image is never built
     and the 3x3 taps that coincide after up-sampling are pre-summed (K = 4*Cin, not 9*Cin)."""
 
     def __init__(self, in_channels, out_channels, kernel_size=3, stride=1, padding=0,
@@ -339,7 +339,7 @@ class UpConv(nn.Module):
                 and os.environ.get("SONET_TC", "1") != "0")
 
     def _packed(self):
-        """BN-folded, parity-combined weights as tcgen05 blobs; re-packed when a source tensor
+        """BN-folded, parity-combined weights as wgmma blobs; re-packed when a source tensor
         changes. Wg[g=(py,px)][co][(a,c)*Cin + ci] = sum of the 3x3 taps (dy,dx) that read low-res
         neighbour (a,c) for output parity (py,px): rows {0}|{1,2} (py=0) or {0,1}|{2} (py=1)."""
         c = self.conv.conv
@@ -409,7 +409,7 @@ class UpConv(nn.Module):
         splits = _pick_splits(kch, 4 * ((B * P + 127) // 128) * ((Cout + 255) // 256))
         scratch = self._scratch_for(4 * splits * B * Cout * P, x.device) if splits > 1 else None
         # H*W % 64 == 0 and Cin % 64 == 0: no im2col — three horizontally shifted copies, the
-        # vertical shifts are TMA coordinate offsets inside the GEMM (3x the input instead of 16x)
+        # vertical shifts are point-coordinate offsets inside the GEMM (3x the input instead of 16x)
         conv = P % 64 == 0 and Cin % 64 == 0 and os.environ.get("SONET_UPCONV_IM2COL", "0") != "1"
         xin = ops.upconv_hshift(x) if conv else ops.upconv_im2col(x)      # [3B,Cin,HW] | [4B,4Cin,HW]
         y = ops.pointwise_tc_grouped(xin, pk["blob4"], pk["per4"], pk["inv4"], pk["shift"], Cout,
@@ -607,7 +607,7 @@ class PointResNet(nn.Module):
                              bn_momentum_decay_step, bn_momentum_decay,
                              last_extra_in=out_channels_list[0])
 
-    # ---- fused tcgen05 path (csrc/pointmlp_tc.cu): the encoder's first PointResNet -------------
+    # ---- fused wgmma path (csrc/pointmlp_tc.cu): the encoder's first PointResNet -------------
     def _tc_eligible(self, cin, x1):
         if x1 is not None or os.environ.get("SONET_TC", "1") == "0":
             return False

@@ -3,9 +3,9 @@ same constructor (`opt` namespace), same forward signatures, same cached attribu
 state_dict keys — so reference checkpoints load and models/{classifier,segmenter,autoencoder}.py
 call these unchanged.
 
-Eval/no-grad forward = the B200 hot path: SOM assignment, cluster statistics, decentring, the
+Eval/no-grad forward = the H100 hot path: SOM assignment, cluster statistics, decentring, the
 point-wise MLPs, the per-node arg-max pool, node kNN grouping and the heads all run as
-hand-written sm_100a kernels (libsonet_b200). Compared with the reference dataflow
+hand-written sm_90a kernels (libsonet_b200). Compared with the reference dataflow
 (models/networks.py:111-199) the dense one-hot mask [B,kN,M] and the two [B,3,kN,M] products are
 never built: statistics and centres come straight from the assignment indices; `mask`, `centers`
 remain available as lazily materialised attributes for callers that read them
@@ -89,7 +89,7 @@ class Encoder(nn.Module):
         self._first_pn_out = None
         self._lazy_src = None
         # True (default): when first_pn_out itself is not needed, fuse the per-node max into the
-        # tcgen05 PointResNet and never write it. Callers that read encoder.first_pn_out every
+        # wgmma PointResNet and never write it. Callers that read encoder.first_pn_out every
         # forward (the segmenter) set this to False to avoid the lazy recomputation.
         self.fuse_pool = True
         self._fpo_demand = False     # set once a caller has read first_pn_out lazily (see below)
@@ -177,7 +177,7 @@ class Encoder(nn.Module):
         self._x_aug, self._first_pn_out = None, None
         pooled = None
         if fused:
-            # fused path: node-sorted copies -> tcgen05 PointResNet -> per-node max. Neither
+            # fused path: node-sorted copies -> wgmma PointResNet -> per-node max. Neither
             # x_augmented nor first_pn_out [B,384,kN] is materialised (they stay available as
             # lazily recomputed attributes for callers that read them).
             if not group:
@@ -327,7 +327,7 @@ class Segmenter(nn.Module):
         out = self.layer3(self.layer2(self.layer1(layer1_in)))
         return self._tail(out, k, self.opt.input_pc_num)
 
-    # ---- B200 fast entry: node-level features + assignment, no per-point gathers ----------------
+    # ---- fast entry: node-level features + assignment, no per-point gathers ----------------
     def _zero_idx(self, B, M, dev):
         z = getattr(self, "_zidx", None)
         if z is None or z.shape != (B, M) or z.device != dev:
@@ -351,7 +351,7 @@ class Segmenter(nn.Module):
             # whose result enters the node-level GEMM as a broadcast addend
             w_cloud = torch.cat((w[o0:o1], w[o3:]), dim=0).t().contiguous()   # [1024, 1040]
             tc = None
-            if os.environ.get("SONET_TC", "1") != "0":      # tcgen05 images of both halves
+            if os.environ.get("SONET_TC", "1") != "0":      # wgmma images of both halves
                 bp, ip = ops.pointwise_tc_pack(w_point.t().contiguous())
                 # node-level GEMM: one launch of the grouped entry (K split to fill the SMs)
                 bn, pern, inn = ops.pointwise_tc_pack_groups(w_node.t().contiguous().unsqueeze(0))

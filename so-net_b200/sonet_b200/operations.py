@@ -1,6 +1,6 @@
 """kNN gathers on SOM nodes — same names and contracts as models/operations.py:19-54.
 
-CUDA float32 inputs outside autograd run the sm_100a gather kernel; anything else (training, CPU
+CUDA float32 inputs outside autograd run the sm_90a gather kernel; anything else (training, CPU
 tensors handed in by data loaders) composes the equivalent differentiable torch.gather.
 """
 import torch

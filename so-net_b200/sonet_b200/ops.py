@@ -1,6 +1,6 @@
 """Tensor-level wrappers over the C-ABI: validate, allocate outputs, pass the current stream.
 
-Every function here launches hand-written sm_100a kernels from libsonet_b200.so on the tensors'
+Every function here launches hand-written sm_90a kernels from libsonet_b200.so on the tensors'
 device and the current torch stream. Inputs must be CUDA, contiguous, of the stated dtype — the
 same checks the reference plugin does with CHECK_INPUT (models/index_max_ext/index_max.cpp:119-121),
 raised as RuntimeError. Nothing here falls back to PyTorch or the CPU.
@@ -355,7 +355,7 @@ def pointresnet_tc_pack(W, shifts, cin):
 
 
 def pointresnet_tc(x, blob, fparams):
-    """x [B,Cin<=6,P] f32 -> [B,384,P]: the fused tcgen05 first PointResNet."""
+    """x [B,Cin<=6,P] f32 -> [B,384,P]: the fused wgmma first PointResNet."""
     _chk(x, "x", torch.float32)
     _chk(blob, "blob", torch.uint8)
     _chk(fparams, "fparams", torch.float32)
@@ -420,7 +420,7 @@ def upconv_hshift(x):
 
 def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, groups, splits=1,
                          scat_w=0, out=None, scratch=None, conv=False):
-    """Grouped tcgen05 layer: x [G*B, C, P], G weight blobs -> out. scat_w = W > 0: the four groups
+    """Grouped wgmma layer: x [G*B, C, P], G weight blobs -> out. scat_w = W > 0: the four groups
     are the output parities of an up-convolution over [H, W] maps, interleaved into
     out [B, cout, 4*P]; otherwise out [G*B, cout, P]. splits > 1: K split through `scratch`."""
     _chk(x, "x", torch.float32)
@@ -449,7 +449,7 @@ def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, group
 
 
 def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=None, gidx=None):
-    """tcgen05 variant of pointwise_layer: x0 [B,C0,P] (+ x1) -> [B,cout,P]."""
+    """wgmma variant of pointwise_layer: x0 [B,C0,P] (+ x1) -> [B,cout,P]."""
     _chk(x0, "x0", torch.float32)
     _chk(x1, "x1", torch.float32, optional=True)
     _chk(blob, "blob", torch.uint8)
@@ -586,7 +586,7 @@ def knn_assemble_pool(coord, keys, p0, idx, K, center_type, owner=None):
 
 
 def pointresnet_tc_pool(x_sorted, blob, fparams, node_sorted, pos0, M, finalize=True, owner=None):
-    """Fused tcgen05 PointResNet + per-node max: -> first_pn_out_masked_max [B,384,M], or with
+    """Fused wgmma PointResNet + per-node max: -> first_pn_out_masked_max [B,384,M], or with
     finalize=False the raw (keys [B,384,M] i32, p0 [B,384]) for knn_assemble_pool / pool_finalize."""
     _chk(x_sorted, "x_sorted", torch.float32)
     _chk(blob, "blob", torch.uint8)

@@ -1,4 +1,4 @@
-"""segmenter.Model — caller-facing wrapper of models/segmenter.py:14-192 on the B200 networks.
+"""segmenter.Model — caller-facing wrapper of models/segmenter.py:14-192 on the H100 networks.
 
 forward() hands the Segmenter the node-level features and the point->node assignment directly
 (Segmenter.forward_nodes) instead of the three per-point torch.gather copies of

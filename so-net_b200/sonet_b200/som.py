@@ -1,4 +1,4 @@
-"""BatchSOM — util/som.py:176-366 on the sm_100a kernels: the node buffer, query_topk / query
+"""BatchSOM — util/som.py:176-366 on the sm_90a kernels: the node buffer, query_topk / query
 (the assignment half the per-batch forward uses) and batch-SOM training (batch_update /
 optimize, SURVEY.md §8f-4) as ONE kernel launch for all iterations of all clouds
 (csrc/som_train.cu). The potential-field node initialisation (util/potential_field.py) is

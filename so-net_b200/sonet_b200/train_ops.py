@@ -1,9 +1,9 @@
-"""Train-mode building blocks on the sm_100a kernels (SURVEY.md §8f-2, csrc/train.cu): autograd
+"""Train-mode building blocks on the sm_90a kernels (SURVEY.md §8f-2, csrc/train.cu): autograd
 Functions that the layer classes use in train() mode instead of the PyTorch composition
 conv1d -> batch_norm(training=True) -> relu and gather (models/layers.py:22-70, 282-296;
 models/networks.py:185).
 
-    ConvTC        y = W x + b, dx = W^T dy AND dW = dy x^T on the generic tcgen05 layer kernel
+    ConvTC        y = W x + b, dx = W^T dy AND dW = dy x^T on the generic wgmma layer kernel
                   (weights / activations packed on the device each step; gradients pre-scaled by a
                   power of two before the fp16 hi/lo split)
     BNActTrain    batch-statistics BatchNorm + ReLU, forward and backward, fused elementwise passes
@@ -67,7 +67,7 @@ class BNActTrain(torch.autograd.Function):
 
 
 def _pack_device(W, transpose):
-    """W [Cout,Cin] (device) -> (blob, scale2) for the tcgen05 layer; W^T when transpose."""
+    """W [Cout,Cin] (device) -> (blob, scale2) for the wgmma layer; W^T when transpose."""
     Cout, Cin = W.shape
     n, k = (Cin, Cout) if transpose else (Cout, Cin)
     dev = W.device
@@ -94,7 +94,7 @@ def _absmax_scale(t):
 
 
 def _tc_dev(x, blob, inv, shift, cout, act_scale=None):
-    """Generic tcgen05 layer with a device-packed blob: inv (1-element device tensor) = the total
+    """Generic wgmma layer with a device-packed blob: inv (1-element device tensor) = the total
     inverse pre-scale, act_scale (1-element) = activation pre-scale or None."""
     B, C, P = x.shape
     with torch.cuda.device(x.device):
@@ -110,7 +110,7 @@ def tc_eligible(cin, cout, rows):
 
 
 def wgrad_tc(dy, x):
-    """dW [Cout,Cin] = sum_{b,p} dy[b,:,p] x[b,:,p]^T on tcgen05 (csrc/train.cu: sonet_wgrad_tc_f32)."""
+    """dW [Cout,Cin] = sum_{b,p} dy[b,:,p] x[b,:,p]^T on wgmma (csrc/train.cu: sonet_wgrad_tc_f32)."""
     B, Cout, P = dy.shape
     Cin = x.shape[1]
     lib = _C.lib()
@@ -135,7 +135,7 @@ _WGRAD_CACHE = {}
 
 class ConvTC(torch.autograd.Function):
     """x [B,Cin,P], W [Cout,Cin], b [Cout] or None -> W x + b. Forward, dgrad and wgrad all run on
-    the generic tcgen05 layer kernel (fp16 hi/lo split, fp32 accumulation)."""
+    the generic wgmma layer kernel (fp16 hi/lo split, fp32 accumulation)."""
 
     @staticmethod
     def forward(ctx, x, W, b):
@@ -200,7 +200,7 @@ class IndexMaxGather(torch.autograd.Function):
 
 
 def conv_bn_act_train(x3, weight2d, bias, norm, relu, epoch=None):
-    """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (tcgen05 when dense
+    """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (wgmma when dense
     enough) -> batch-stat BN (+ running-stat update with the reference's momentum schedule,
     models/layers.py:57-65) -> ReLU."""
     B, Cin, P = x3.shape

@@ -29,7 +29,7 @@ def test_python_binding_covers_header(lib_built):
     from sonet_b200 import _C
     assert sorted(_C.EXPORTED_SYMBOLS) == declared_symbols()
     lib = _C.lib()
-    assert b"sm_100a" in lib.sonet_version()
+    assert b"sm_90a" in lib.sonet_version()
 
 
 def test_library_has_no_torch_dependency(lib_built):

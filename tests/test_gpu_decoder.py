@@ -1,5 +1,5 @@
 """-m gpu: the up-convolution decoder kernels (SURVEY.md §8f-1; csrc/upconv.cu + the grouped /
-split-K tcgen05 layer of csrc/pointwise_tc.cu) against an fp64 evaluation of the reference
+split-K wgmma layer of csrc/pointwise_tc.cu) against an fp64 evaluation of the reference
 composition UpConv.forward = conv3x3(pad 1)(upsample_nearest_x2(x)) + eval BN + ReLU
 (models/layers.py:214-240). Tolerance |a-b| <= 1e-4 * max(|b|, 1)."""
 import numpy as np

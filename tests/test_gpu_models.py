@@ -107,7 +107,7 @@ def test_segmenter_vs_reference_golden_and_dropin_signature(oracle_mod):
                          enc.first_pn_out, gat(enc.first_pn_out_masked_max),
                          gat(enc.knn_feature_1), gat(enc.final_pn_out), m.feature)
     assert_golden(g, "score_segmenter", s2)
-    # two numeric paths (dense fp32 concat GEMM vs split tcgen05 GEMMs): both inside the 1e-4 bar
+    # two numeric paths (dense fp32 concat GEMM vs split wgmma GEMMs): both inside the 1e-4 bar
     assert_close(s2, m.score_segmenter, "forward vs forward_nodes")
 
 
@@ -122,7 +122,7 @@ def test_autoencoder_vs_reference_golden():
     m.set_input(inp["pc"], inp["sn"], inp["label"], inp["node"], inp["node_knn_I"])
     m.test_model()
     _check_encoder_against_golden(g, m.encoder, opt)
-    # the up-convolution decoder runs on the tcgen05 kernels (csrc/upconv.cu): 1e-4 like
+    # the up-convolution decoder runs on the wgmma kernels (csrc/upconv.cu): 1e-4 like
     # everything else (round 1 ran it through cuDNN and needed 5e-4)
     assert_golden(g, "predicted_pc", m.predicted_pc)
     assert_golden(g, "conv_pc4", m.decoder.conv_pc4)
@@ -168,7 +168,7 @@ def _assert_encoder_slice_vs_oracle(oracle_mod, enc, o, k, n_clouds):
 
 def test_cfg2_benchmarked_pipeline_vs_oracle(oracle_mod):
     """The EXACT pipeline bench.py times — classifier.Model with enable_cuda_graph(True) at
-    BASELINE.json configs[1] (B=64, N=5000: som_group + fused tcgen05 PointResNet/pool at
+    BASELINE.json configs[1] (B=64, N=5000: som_group + fused wgmma PointResNet/pool at
     kN=15000 + graph replay) — against the oracle on a 3-cloud slice: k-sets exact, som_node,
     first_pn_out_masked_max, knn_feature_1, final_pn_out, feature and score within 1e-4
     (|a-b| <= 1e-4 * max(|b|,1)). Checked on the capture run AND on a replay with new inputs."""

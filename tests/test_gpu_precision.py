@@ -5,7 +5,7 @@ results, which themselves carry rounding noise. These tests evaluate the same ne
 (the oracle's value path follows the input dtype; index decisions stay fp32, oracle/oracle.py) and
 compare BOTH the reference-equivalent fp32 CPU evaluation and the CUDA path with it: the CUDA
 path's distance to the fp64 result must be of the same order as fp32's own — i.e. the fp16 hi/lo
-split of the tcgen05 layers (DESIGN.md §3) costs no more accuracy than plain fp32 arithmetic does,
+split of the wgmma layers (csrc/tc_common.cuh) costs no more accuracy than plain fp32 arithmetic does,
 also through the deepest chain the hot path has (segmenter: 13 chained layers).
 """
 import pytest

@@ -1,6 +1,6 @@
-"""-m gpu: pins the tcgen05 encodings the fused point-MLP kernel relies on — instruction
-descriptor, K-major no-swizzle shared-memory descriptors (LBO/SBO roles), and the A-operand
-layout in tensor memory — with a single-tile GEMM probe against an exact bf16 reference."""
+"""-m gpu: pins the wgmma encodings the point-MLP kernels rely on — K-major no-swizzle
+shared-memory descriptors (LBO/SBO roles) with the A operand in shared memory, and the A-operand
+register fragment — with a single-tile GEMM probe against an exact bf16 reference."""
 import ctypes
 
 import numpy as np
@@ -42,7 +42,7 @@ def test_tcgen05_probe_matches_bf16_reference(N, K, mode, layout):
         "N=%d K=%d mode=%d layout=%d: max abs err %.3e" % (N, K, mode, layout, err)
 
 
-# ---- the fused tcgen05 first PointResNet (csrc/pointmlp_tc.cu) -------------------------------------
+# ---- the fused wgmma first PointResNet (csrc/pointmlp_tc.cu) -------------------------------------
 def _resnet(cin, seed):
     from sonet_b200 import layers, synth
     net = layers.PointResNet(cin, [64, 128, 256, 384], 'relu', 'batch')
@@ -84,7 +84,7 @@ def test_pointresnet_tc_vs_fp64_reference(B, cin, P, monkeypatch):
         simt = net(x.to(DEV))
     assert got.shape == (B, 384, P)
     assert_close(simt, want, "fp32 CUDA-core path vs fp64")
-    assert_close(got, want, "tcgen05 bf16x3 path vs fp64")
+    assert_close(got, want, "wgmma bf16x3 path vs fp64")
     # the 3-product split should sit around 1e-5, well inside the 1e-4 bar
     e = float(((got.cpu() - want).abs() / want.abs().clamp(min=1)).max())
     assert e < 5e-5, e
@@ -101,7 +101,7 @@ def test_pointresnet_tc_repacks_after_weight_update(monkeypatch):
     assert torch.allclose(b, a + 1.0, atol=1e-5)
 
 
-# ---- the generic tcgen05 point-wise layer (csrc/pointwise_tc.cu) ------------------------------------
+# ---- the generic wgmma point-wise layer (csrc/pointwise_tc.cu) ------------------------------------
 @pytest.mark.parametrize("B,C0,C1,P,Cout,relu", [
     (2, 387, 0, 576, 512, True),      # KNNModule layer 1 (K padded 387 -> 400)
     (2, 512, 0, 576, 512, True),      # KNNModule layer 2
@@ -127,7 +127,7 @@ def test_pointwise_tc_vs_fp64(B, C0, C1, P, Cout, relu):
     got = ops.pointwise_layer_tc(x0.to(DEV), blob.to(DEV), inv, shift.to(DEV), Cout, relu,
                                  x1=None if x1 is None else x1.to(DEV))
     assert got.shape == (B, Cout, P)
-    assert_close(got, want, "tcgen05 generic layer vs fp64", 2e-5)
+    assert_close(got, want, "wgmma generic layer vs fp64", 2e-5)
 
 
 def test_pointwise_tc_gathered_addend():
@@ -145,14 +145,14 @@ def test_pointwise_tc_gathered_addend():
     blob, inv = ops.pointwise_tc_pack(W)
     got = ops.pointwise_layer_tc(x0.to(DEV), blob.to(DEV), inv, None, Cout, True,
                                  addend=add.to(DEV), gidx=gidx.to(DEV))
-    assert_close(got, want, "tcgen05 layer + gathered addend", 2e-5)
+    assert_close(got, want, "wgmma layer + gathered addend", 2e-5)
 
 
-# ---- fused pool path: node-sorted copies -> tcgen05 PointResNet -> per-node max ---------------------
+# ---- fused pool path: node-sorted copies -> wgmma PointResNet -> per-node max ---------------------
 @pytest.mark.parametrize("B,N,mode", [(3, 1024, "sampled"), (2, 700, "uniform"), (2, 5000, "sampled")])
 def test_fused_pool_matches_unfused_path(B, N, mode, monkeypatch):
     """first_pn_out_masked_max from the fused kernel == index_max(+gather) over the materialised
-    first_pn_out of the same tcgen05 PointResNet (bit-exact: same MMAs, max is order-free), incl.
+    first_pn_out of the same wgmma PointResNet (bit-exact: same MMAs, max is order-free), incl.
     empty nodes (feature of stacked copy 0) — models/networks.py:181-185."""
     from sonet_b200 import ops, synth
     monkeypatch.setenv("SONET_TC", "1")

@@ -68,7 +68,7 @@ def test_conv_tc_forward_dgrad_vs_torch(B, cin, cout, P):
 @pytest.mark.parametrize("B,cin,cout,P,gscale", [(4, 64, 128, 1500, 1.0), (64, 387, 512, 576, 1e-6),
                                                  (3, 320, 384, 1000, 3e-5), (2, 40, 64, 333, 1.0)])
 def test_wgrad_tc_vs_fp64(B, cin, cout, P, gscale):
-    """dW = sum_{b,p} dy x^T on tcgen05 (transpose + pre-scale of dy, x packed as the weight operand,
+    """dW = sum_{b,p} dy x^T on wgmma (transpose + pre-scale of dy, x packed as the weight operand,
     split-K with a fixed-order reduce) against fp64; gradients as small as 1e-6 keep full precision
     because they are pre-scaled by a power of two before the fp16 split."""
     from sonet_b200 import train_ops
@@ -117,7 +117,7 @@ def test_index_max_gather_backward_vs_torch_gather(oracle_mod):
 
 def test_classifier_training_step_kernels_vs_torch_composition():
     """One optimize() step from identical weights with the train kernels ON and OFF: same loss,
-    same gradients (1e-3 of each tensor's scale: the tcgen05 GEMMs carry ~1e-5 per layer),
+    same gradients (1e-3 of each tensor's scale: the wgmma GEMMs carry ~1e-5 per layer),
     same running statistics."""
     from helpers import build_states
     from sonet_b200 import classifier, synth, train_ops

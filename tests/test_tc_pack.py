@@ -1,4 +1,4 @@
-"""Host-side packing of the tcgen05 point-MLP weights (no GPU needed): the fp16 hi/lo K-major
+"""Host-side packing of the wgmma point-MLP weights (no GPU needed): the fp16 hi/lo K-major
 core-matrix images, times the stored inverse power-of-two scale, must reproduce the fp32 weights
 to ~2^-21 and sit at the documented offsets."""
 import numpy as np

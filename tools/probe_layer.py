@@ -1,4 +1,4 @@
-"""Timing probe of the generic tcgen05 layer at a given shape, with / without the gathered addend
+"""Timing probe of the generic wgmma layer at a given shape, with / without the gathered addend
 (segmenter head layer 1). usage: python tools/probe_layer.py [B C P Cout]"""
 import os
 import sys

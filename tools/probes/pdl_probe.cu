@@ -1,5 +1,5 @@
 // Per-edge latency of a captured chain of dependent kernels, with and without programmatic
-// dependent launch. build: nvcc -gencode arch=compute_100a,code=sm_100a -o pdl_probe pdl_probe.cu
+// dependent launch. build: nvcc -gencode arch=compute_90a,code=sm_90a -o pdl_probe pdl_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <vector>

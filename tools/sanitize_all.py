@@ -2,7 +2,7 @@
 
     compute-sanitizer --tool racecheck python tools/sanitize_all.py
 
-classifier (fused tcgen05 + pool at N=5000, graph replay), segmenter, auto-encoder (up-conv decoder,
+classifier (fused wgmma + pool at N=5000, graph replay), segmenter, auto-encoder (up-conv decoder,
 grouped / split-K GEMMs, Chamfer incl. the arg-min pass), BatchSOM training, augmentation,
 query_topk with the fused mask, standalone index_max, and one training step (BN / scatter / device
 pack kernels)."""

@@ -1,4 +1,4 @@
-"""Time one classifier training step (forward + backward + Adam) with the sm_100a train kernels
+"""Time one classifier training step (forward + backward + Adam) with the sm_90a train kernels
 (sonet_b200/train_ops.py) against the PyTorch composition the reference trains with.
     python tools/train_step_bench.py [--batch 32] [--npts 5000] [--steps 6]"""
 import argparse
@@ -44,7 +44,7 @@ def run(enabled, tf32):
     return ms, float(m.loss)
 
 
-for name, en, tf in (("sonet train kernels (tcgen05 fwd/dgrad/wgrad, fused BN)", True, False),
+for name, en, tf in (("sonet train kernels (wgmma fwd/dgrad/wgrad, fused BN)", True, False),
                      ("PyTorch composition, strict fp32", False, False),
                      ("PyTorch composition, TF32 allowed (torch default for cuDNN)", False, True)):
     ms, loss = run(en, tf)
