@@ -343,8 +343,17 @@ int sonet_pointresnet_tc_forward(const float* x, int Cin, int B, int P, const vo
  * batch sharding), cluster_mean = sum / (count + 1e-5), then x_sorted / node_sorted / pos0 exactly
  * as sonet_som_sort_decenter defines them (rows of a node in ascending stacked order).
  * count [B,M] i32, cluster_mean [B,3,M] are outputs. Needs sonet_som_group_smem_bytes(N,M,k)
- * bytes of shared memory per block (4*k*N + small); fails with a message beyond the device limit. */
+ * bytes of shared memory per block (4*k*N + small); fails with a message beyond the device limit.
+ * When another 4*(6|3)*N bytes fit as well, the cloud (and its normals) is staged in shared memory.
+ * sonet_som_group_mode: how sonet_som_group_decenter runs on a device with smem_optin bytes of
+ * opt-in shared memory per block (cudaDevAttrMaxSharedMemoryPerBlockOptin): SONET_SOM_GROUP_STAGED,
+ * SONET_SOM_GROUP_UNSTAGED, or SONET_SOM_GROUP_NONE (it would fail: M > 256, N >= 2^24 or too
+ * little shared memory). with_sn: 1 when sn is passed. Negative on a bad argument. */
+#define SONET_SOM_GROUP_NONE 0
+#define SONET_SOM_GROUP_UNSTAGED 1
+#define SONET_SOM_GROUP_STAGED 2
 long long sonet_som_group_smem_bytes(int N, int M, int k);
+int sonet_som_group_mode(int N, int M, int k, int with_sn, long long smem_optin);
 int sonet_som_group_decenter(const float* x, const float* sn, const int32_t* min_idx_i32, int B,
                              int N, int M, int k, int32_t* count, float* cluster_mean,
                              float* x_sorted, int32_t* node_sorted, int32_t* pos0,

@@ -111,6 +111,23 @@ def run_encoder_checks(tag, opt, enc, inp, st_enc, out):
     return orc
 
 
+# options a fixture may set away from synth.make_opt's defaults; each one is stored in the
+# fixture (tests/helpers.golden_case rebuilds `opt` from them)
+OPTION_KEYS = ("node_num", "k", "som_k", "som_k_type", "surface_normal", "input_pc_num",
+               "output_fc_pc_num", "output_conv_pc_num")
+
+
+def header(opt, B, N, seed, node_mode, over):
+    unknown = set(over) - set(OPTION_KEYS)
+    assert not unknown, "options not stored in the fixture: %s" % sorted(unknown)
+    out = dict(B=np.int64(B), N=np.int64(N), seed=np.int64(seed), node_mode=np.asarray(node_mode),
+               som_k=np.int64(opt.som_k), classes=np.int64(opt.classes))
+    for key in over:
+        if key != "som_k":                       # stored above for every fixture
+            out["opt_" + key] = np.asarray(getattr(opt, key))
+    return out
+
+
 def gen_classifier(ref, tag, B, N, node_mode, seed, **over):
     opt = synth.make_opt("classifier", batch_size=B, input_pc_num=N, **over)
     model = ref.classifier.Model(opt)
@@ -121,9 +138,7 @@ def gen_classifier(ref, tag, B, N, node_mode, seed, **over):
     model.set_input(inp["pc"], inp["sn"], inp["label"], inp["node"], inp["node_knn_I"])
     with torch.no_grad():
         model.test_model()
-    out = dict(B=np.int64(B), N=np.int64(N), seed=np.int64(seed),
-               node_mode=np.asarray(node_mode), som_k=np.int64(opt.som_k),
-               classes=np.int64(opt.classes))
+    out = header(opt, B, N, seed, node_mode, over)
     orc = run_encoder_checks(tag, opt, model.encoder, inp, st_enc, out)
     put(out, "score", model.score.detach())
     s = oracle.classifier_forward(st_cls, orc["feature"])
@@ -132,19 +147,18 @@ def gen_classifier(ref, tag, B, N, node_mode, seed, **over):
     print("wrote", tag)
 
 
-def gen_segmenter(ref, tag, B, N, seed):
-    opt = synth.make_opt("segmenter", batch_size=B, input_pc_num=N)
+def gen_segmenter(ref, tag, B, N, seed, node_mode="sampled", **over):
+    opt = synth.make_opt("segmenter", batch_size=B, input_pc_num=N, **over)
     model = ref.segmenter.Model(opt)
     st_enc = load_encoder(model.encoder, seed)
     st_seg = synth.synth_state_dict(model.segmenter, seed=seed + 1)
     model.segmenter.load_state_dict(st_seg)
-    inp = synth.synth_inputs(B, N, opt.node_num, opt.som_k, seed=seed)
+    inp = synth.synth_inputs(B, N, opt.node_num, max(opt.som_k, 1), seed=seed, node_mode=node_mode)
     seg = torch.zeros(B, N, dtype=torch.int64)
     model.set_input(inp["pc"], inp["sn"], inp["label"], seg, inp["node"], inp["node_knn_I"])
     with torch.no_grad():
         model.test_model()
-    out = dict(B=np.int64(B), N=np.int64(N), seed=np.int64(seed), node_mode=np.asarray("sampled"),
-               som_k=np.int64(opt.som_k), classes=np.int64(opt.classes))
+    out = header(opt, B, N, seed, node_mode, over)
     orc = run_encoder_checks(tag, opt, model.encoder, inp, st_enc, out)
     put(out, "score_segmenter", model.score_segmenter.detach())
     put(out, "centers", model.encoder.centers.detach())
@@ -157,20 +171,23 @@ def gen_segmenter(ref, tag, B, N, seed):
     print("wrote", tag)
 
 
-def gen_autoencoder(ref, tag, B, N, seed):
-    opt = synth.make_opt("autoencoder", batch_size=B, input_pc_num=N)
+def gen_autoencoder(ref, tag, B, N, seed, node_mode="sampled", **over):
+    opt = synth.make_opt("autoencoder", batch_size=B, input_pc_num=N, **over)
     model = ref.autoencoder.Model(opt)
     st_enc = load_encoder(model.encoder, seed)
     model.decoder.load_state_dict(synth.synth_state_dict(model.decoder, seed=seed + 1))
-    inp = synth.synth_inputs(B, N, opt.node_num, opt.som_k, seed=seed)
+    inp = synth.synth_inputs(B, N, opt.node_num, max(opt.som_k, 1), seed=seed, node_mode=node_mode)
     model.set_input(inp["pc"], inp["sn"], inp["label"], inp["node"], inp["node_knn_I"])
     with torch.no_grad():
         model.test_model()
-    out = dict(B=np.int64(B), N=np.int64(N), seed=np.int64(seed), node_mode=np.asarray("sampled"),
-               som_k=np.int64(opt.som_k), classes=np.int64(opt.classes))
+    out = header(opt, B, N, seed, node_mode, over)
     run_encoder_checks(tag, opt, model.encoder, inp, st_enc, out)
     put(out, "predicted_pc", model.predicted_pc.detach())
     put(out, "conv_pc4", model.decoder.conv_pc4.detach())
+    if opt.output_conv_pc_num == 4096:           # the test-time conv5 loss exists only then
+        put(out, "conv_pc5", model.decoder.conv_pc5.detach())
+        put(out, "conv_pc6", model.decoder.conv_pc6.detach())
+        out["loss_chamfer_conv5"] = model.loss_chamfer_conv5.detach().numpy()
     out["loss_chamfer"] = model.loss_chamfer.detach().numpy()
     out["loss_chamfer_conv4"] = model.loss_chamfer_conv4.detach().numpy()
     out["loss"] = model.loss.detach().numpy()
@@ -271,13 +288,34 @@ def gen_augment(ref):
     print("wrote augment.npz")
 
 
+STATE_KEY_CASES = (("classifier", 9, True), ("classifier", 0, True), ("segmenter", 9, True),
+                   ("autoencoder", 9, True), ("classifier", 1, True), ("segmenter", 1, True),
+                   ("classifier", 9, False), ("segmenter", 9, False), ("autoencoder", 9, False))
+
+
+def gen_options(ref):
+    """Fixtures at non-default options of the reference's scripts: node_num (any square, up to the
+    library's 256), k from 1 to 4, som_k / som_k_type, surface_normal off, the 4096-point
+    auto-encoder output. Each run also pins the oracle against the reference at those options."""
+    gen_classifier(ref, "classifier_b2_n300_m121_k4", 2, 300, "sampled", seed=6, node_num=121, k=4,
+                   som_k=9, som_k_type="center", surface_normal=False)
+    gen_classifier(ref, "classifier_b3_n150_m16_k1", 3, 150, "uniform", seed=7, node_num=16, k=1,
+                   som_k=2, som_k_type="avg")
+    gen_classifier(ref, "classifier_b1_n700_m256_k2", 1, 700, "sampled", seed=8, node_num=256, k=2,
+                   som_k=9, som_k_type="avg")
+    gen_segmenter(ref, "segmenter_b2_n200_m100_k2", 2, 200, seed=9, node_num=100, k=2, som_k=9,
+                  som_k_type="avg", surface_normal=False)
+    gen_autoencoder(ref, "autoencoder_b2_n300_m36_conv4096", 2, 300, seed=10, node_num=36, k=3,
+                    som_k=5, som_k_type="avg", output_conv_pc_num=4096)
+
+
 def gen_state_keys(ref):
     """Names and shapes of every state_dict tensor of the reference networks (checkpoint
     compatibility contract, SURVEY.md §5 'Checkpoint / resume')."""
     import json
     out = {}
-    for task, som_k in (("classifier", 9), ("classifier", 0), ("segmenter", 9), ("autoencoder", 9)):
-        opt = synth.make_opt(task, batch_size=2, input_pc_num=64, som_k=som_k)
+    for task, som_k, sn in STATE_KEY_CASES:
+        opt = synth.make_opt(task, batch_size=2, input_pc_num=64, som_k=som_k, surface_normal=sn)
         mods = {"encoder": ref.networks.Encoder(opt)}
         if task == "classifier":
             mods["classifier"] = ref.networks.Classifier(opt)
@@ -286,8 +324,8 @@ def gen_state_keys(ref):
         else:
             mods["decoder"] = ref.networks.Decoder(opt)
         for name, m in mods.items():
-            out["%s/som_k=%d/%s" % (task, som_k, name)] = {
-                k: list(v.shape) for k, v in m.state_dict().items()}
+            key = "%s/som_k=%d%s/%s" % (task, som_k, "" if sn else "/no_sn", name)
+            out[key] = {k: list(v.shape) for k, v in m.state_dict().items()}
     with open(os.path.join(GOLDEN, "state_keys.json"), "w") as f:
         json.dump(out, f, indent=0, sort_keys=True)
     print("wrote state_keys.json")
@@ -312,6 +350,7 @@ def main():
     gen_classifier(ref, "classifier_b2_n256_somk0", 2, 256, "sampled", seed=3, som_k=0)
     gen_segmenter(ref, "segmenter_b2_n128", 2, 128, seed=4)
     gen_autoencoder(ref, "autoencoder_b2_n256", 2, 256, seed=5)
+    gen_options(ref)
 
 
 if __name__ == "__main__":

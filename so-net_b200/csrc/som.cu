@@ -273,7 +273,8 @@ static int som_assign_impl(const float* x, const float* node, int B, int N, int 
   using namespace sonet;
   SONET_REQUIRE(B >= 0 && N >= 0, "som_assign: negative dimension");
   SONET_REQUIRE(M >= 1 && M <= SOM_MAX_M, "som_assign: M=%d out of range [1,%d]", M, SOM_MAX_M);
-  SONET_REQUIRE(k >= 1 && k <= SOM_MAX_K && k <= M, "som_assign: k=%d out of range", k);
+  SONET_REQUIRE(k >= 1 && k <= SOM_MAX_K && k <= M,
+                "som_assign: k=%d out of range [1,%d] (and k <= M=%d)", k, SOM_MAX_K, M);
   SONET_REQUIRE(B <= 65535, "som_assign: B=%d exceeds grid limit", B);
   if (B == 0) return SONET_OK;
   SONET_REQUIRE(x && node && min_idx_i32, "som_assign: null pointer");

@@ -335,6 +335,21 @@ static long long som_group_stage_bytes(int N, bool with_sn) {
   return static_cast<long long>(with_sn ? 6 : 3) * N * 4;
 }
 
+// the one place that decides whether and how sonet_som_group_decenter runs
+static int som_group_mode(int N, int M, int k, bool with_sn, long long smem_optin) {
+  if (M > sonet::SORT_MAX_M || N >= (1 << 24)) return SONET_SOM_GROUP_NONE;
+  const long long smem = sonet_som_group_smem_bytes(N, M, k);
+  if (smem > smem_optin) return SONET_SOM_GROUP_NONE;
+  return smem + som_group_stage_bytes(N, with_sn) <= smem_optin ? SONET_SOM_GROUP_STAGED
+                                                                 : SONET_SOM_GROUP_UNSTAGED;
+}
+
+extern "C" int sonet_som_group_mode(int N, int M, int k, int with_sn, long long smem_optin) {
+  SONET_REQUIRE(N >= 0 && M >= 1 && k >= 1 && smem_optin >= 0,
+                "som_group_mode: bad dimension (N=%d, M=%d, k=%d)", N, M, k);
+  return som_group_mode(N, M, k, with_sn != 0, smem_optin);
+}
+
 extern "C" int sonet_som_group_decenter(const float* x, const float* sn, const int32_t* min_idx_i32,
                                         int B, int N, int M, int k, int32_t* count,
                                         float* cluster_mean, float* x_sorted, int32_t* node_sorted,
@@ -347,12 +362,12 @@ extern "C" int sonet_som_group_decenter(const float* x, const float* sn, const i
   SONET_REQUIRE(x && min_idx_i32 && count && cluster_mean && x_sorted && node_sorted && pos0,
                 "som_group_decenter: null pointer");
   const long long smem = sonet_som_group_smem_bytes(N, M, k);
-  SONET_REQUIRE(smem <= max_smem_optin(),
+  const int mode = som_group_mode(N, M, k, sn != nullptr, max_smem_optin());
+  SONET_REQUIRE(mode != SONET_SOM_GROUP_NONE,
                 "som_group_decenter: k*N=%d rows need %lld B of shared memory (use "
                 "sonet_som_assign statistics + sonet_som_sort_decenter instead)", k * N, smem);
-  long long total = smem + som_group_stage_bytes(N, sn != nullptr);
-  const int stage = total <= max_smem_optin();
-  if (!stage) total = smem;
+  const int stage = mode == SONET_SOM_GROUP_STAGED;
+  const long long total = stage ? smem + som_group_stage_bytes(N, sn != nullptr) : smem;
   cudaFuncSetAttribute(som_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                        static_cast<int>(total));
   som_group_kernel<<<B, GROUP_THREADS, static_cast<size_t>(total), as_stream(stream)>>>(

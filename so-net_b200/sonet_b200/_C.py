@@ -92,6 +92,7 @@ _SIGNATURES = {
     "sonet_pointresnet_tc_pool_forward": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_int, c_void_p, c_void_p, c_void_p],
     "sonet_som_group_smem_bytes": [c_int, c_int, c_int],
+    "sonet_som_group_mode": [c_int, c_int, c_int, c_int, ctypes.c_longlong],
     "sonet_som_group_decenter": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sonet_knn_assemble_pool_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,

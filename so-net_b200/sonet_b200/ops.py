@@ -490,15 +490,25 @@ def som_sort_decenter(x, sn, cluster_mean, min_idx_i32, count, k):
 
 
 _MAX_SMEM = {}
+# sonet_som_group_mode results (include/sonet_b200.h)
+SOM_GROUP_NONE, SOM_GROUP_UNSTAGED, SOM_GROUP_STAGED = 0, 1, 2
+
+
+def som_group_mode(N, M, k, with_sn, dev):
+    """How sonet_som_group_decenter runs on this device: SOM_GROUP_STAGED (cloud staged in shared
+    memory), SOM_GROUP_UNSTAGED (read from global memory) or SOM_GROUP_NONE (does not fit)."""
+    cap = _MAX_SMEM.get(dev)
+    if cap is None:
+        cap = _MAX_SMEM[dev] = torch.cuda.get_device_properties(dev).shared_memory_per_block_optin
+    mode = _C.lib().sonet_som_group_mode(int(N), int(M), int(k), int(bool(with_sn)), int(cap))
+    if mode < 0:
+        _C.check(mode, "sonet_som_group_mode")
+    return mode
 
 
 def som_group_fits(N, M, k, dev):
     """Does sonet_som_group_decenter's per-cloud shared-memory footprint fit on this device?"""
-    cap = _MAX_SMEM.get(dev)
-    if cap is None:
-        cap = _MAX_SMEM[dev] = torch.cuda.get_device_properties(dev).shared_memory_per_block_optin
-    return N < (1 << 24) and M <= 256 and \
-        _C.lib().sonet_som_group_smem_bytes(int(N), int(M), int(k)) <= cap
+    return som_group_mode(N, M, k, False, dev) != SOM_GROUP_NONE
 
 
 def som_group_decenter(x, sn, min_idx_i32, M, k):

@@ -57,13 +57,40 @@ def build_states(task, opt, seed):
     return st
 
 
+def golden_options(g):
+    """The non-default options a fixture was generated with (oracle/make_golden.py stores each
+    one as opt_<name>)."""
+    return {key[4:]: g[key].item() for key in g.files if key.startswith("opt_")}
+
+
 def golden_case(g, task, **over):
     B, N, seed = int(g["B"]), int(g["N"]), int(g["seed"])
     som_k = int(g["som_k"])
-    opt = synth.make_opt(task, batch_size=B, input_pc_num=N, som_k=som_k, **over)
+    kw = dict(batch_size=B, input_pc_num=N, som_k=som_k)
+    kw.update(golden_options(g))
+    kw.update(over)
+    opt = synth.make_opt(task, **kw)
     inp = synth.synth_inputs(B, N, opt.node_num, max(som_k, 1), seed=seed,
                              node_mode=str(g["node_mode"]))
     return opt, inp, seed
+
+
+def check_encoder_against_golden(g, enc, opt):
+    """Every cached encoder attribute of a CUDA run against a reference fixture: k-sets and mask
+    statistics exact, node-level tensors and (in the reference's slot order) first_pn_out within
+    TOL."""
+    from oracle import oracle
+    assert np.array_equal(oracle.canon_sets(enc.min_idx.cpu(), opt.k).numpy(), g["knn_sets"])
+    mask = enc.mask
+    assert mask.dtype == torch.int32
+    assert np.array_equal(torch.max(mask, dim=1)[0].cpu().numpy(), g["mask_row_max"])
+    assert np.array_equal(torch.sum(mask, dim=1).cpu().numpy(), g["mask_row_sum"])
+    for n in ("som_node", "first_pn_out_masked_max", "final_pn_out", "feature"):
+        assert_golden(g, n, getattr(enc, n))
+    assert_golden(g, "first_pn_out", to_ref_slot_order(enc.first_pn_out, enc.min_idx, g, opt.k))
+    if opt.som_k >= 2:
+        assert_golden(g, "knn_center_1", enc.knn_center_1)
+        assert_golden(g, "knn_feature_1", enc.knn_feature_1)
 
 
 def to_ref_slot_order(t, our_min_idx, g, k):

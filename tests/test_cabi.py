@@ -74,6 +74,27 @@ def test_bad_arguments_return_error_codes(lib_built):
                                          None, 0, None, None) == 0
 
 
+def test_som_group_mode_arithmetic(lib_built):
+    """sonet_som_group_mode on an H100's 232448 B of opt-in shared memory: at M=64, k=3 the cloud
+    (with normals) is staged up to N=6200 and som_group runs at all up to N=18601; one more point
+    changes the mode. Host-only: the capacity is an argument."""
+    from sonet_b200 import _C, ops
+    lib = _C.lib()
+    cap = 232448
+    mode = lambda N, M=64, k=3, sn=1: lib.sonet_som_group_mode(N, M, k, sn, cap)  # noqa: E731
+    assert (mode(6200), mode(6201)) == (ops.SOM_GROUP_STAGED, ops.SOM_GROUP_UNSTAGED)
+    assert (mode(18601), mode(18602)) == (ops.SOM_GROUP_UNSTAGED, ops.SOM_GROUP_NONE)
+    assert mode(6201, sn=0) == ops.SOM_GROUP_STAGED         # without normals: 3 channels staged
+    for N in (6200, 6201, 18601, 18602):
+        fits = lib.sonet_som_group_smem_bytes(N, 64, 3) <= cap
+        assert (mode(N) != ops.SOM_GROUP_NONE) == fits
+    assert mode(1, M=256, k=4) == ops.SOM_GROUP_STAGED
+    assert mode(1, M=257) == ops.SOM_GROUP_NONE              # every SOM kernel stops at M=256
+    assert mode(1 << 24, k=1) == ops.SOM_GROUP_NONE          # node ids share 32 bits with n
+    assert lib.sonet_som_group_mode(1 << 24, 64, 1, 1, 1 << 40) == ops.SOM_GROUP_NONE
+    assert mode(10, k=0) < 0 and "k=0" in _C.last_error()
+
+
 def test_cuda_entry_points_reject_host_tensors():
     from sonet_b200 import index_max
     data = torch.zeros(1, 2, 8)

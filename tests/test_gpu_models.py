@@ -6,6 +6,7 @@ import torch
 
 from helpers import (assert_close, assert_golden, build_states, golden, golden_case,
                      to_ref_slot_order, to_slot_order)
+from helpers import check_encoder_against_golden as _check_encoder_against_golden
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -23,21 +24,6 @@ def _classifier(opt, st):
     m.encoder.load_state_dict(st["encoder"])
     m.classifier.load_state_dict(st["head"])
     return m
-
-
-def _check_encoder_against_golden(g, enc, opt):
-    from oracle import oracle
-    assert np.array_equal(oracle.canon_sets(enc.min_idx.cpu(), opt.k).numpy(), g["knn_sets"])
-    mask = enc.mask
-    assert mask.dtype == torch.int32
-    assert np.array_equal(torch.max(mask, dim=1)[0].cpu().numpy(), g["mask_row_max"])
-    assert np.array_equal(torch.sum(mask, dim=1).cpu().numpy(), g["mask_row_sum"])
-    for n in ("som_node", "first_pn_out_masked_max", "final_pn_out", "feature"):
-        assert_golden(g, n, getattr(enc, n))
-    assert_golden(g, "first_pn_out", to_ref_slot_order(enc.first_pn_out, enc.min_idx, g, opt.k))
-    if opt.som_k >= 2:
-        assert_golden(g, "knn_center_1", enc.knn_center_1)
-        assert_golden(g, "knn_feature_1", enc.knn_feature_1)
 
 
 @pytest.mark.parametrize("name", ["classifier_b2_n256", "classifier_b2_n200_emptynodes",

@@ -18,12 +18,27 @@ from sonet_b200 import layers, networks, synth
                                              ("segmenter", 9, "segmenter"),
                                              ("autoencoder", 9, "decoder")])
 def test_state_dict_keys_and_shapes_match_reference(task, som_k, head):
+    _check_state_keys(task, som_k, True, head)
+
+
+@pytest.mark.parametrize("task,som_k,sn,head", [("classifier", 1, True, "classifier"),
+                                                ("segmenter", 1, True, "segmenter"),
+                                                ("classifier", 9, False, "classifier"),
+                                                ("segmenter", 9, False, "segmenter"),
+                                                ("autoencoder", 9, False, "decoder")])
+def test_state_dict_keys_match_reference_at_other_options(task, som_k, sn, head):
+    """som_k=1 (the PointResNet final network, no KNN module) and surface_normal=False (3-channel
+    first PointResNet, 9-channel segmenter point part): checkpoints of those networks load too."""
+    _check_state_keys(task, som_k, sn, head)
+
+
+def _check_state_keys(task, som_k, sn, head):
     want = json.load(open(os.path.join(GOLDEN, "state_keys.json")))
-    opt = synth.make_opt(task, batch_size=2, input_pc_num=64, som_k=som_k)
+    opt = synth.make_opt(task, batch_size=2, input_pc_num=64, som_k=som_k, surface_normal=sn)
     mods = {"encoder": networks.Encoder(opt),
             head: getattr(networks, head.capitalize())(opt)}
     for name, m in mods.items():
-        ref = want["%s/som_k=%d/%s" % (task, som_k, name)]
+        ref = want["%s/som_k=%d%s/%s" % (task, som_k, "" if sn else "/no_sn", name)]
         got = {k: list(v.shape) for k, v in m.state_dict().items()}
         assert got == ref, name
 

@@ -6,7 +6,7 @@ import pytest
 import torch
 
 from helpers import (assert_close, assert_golden, build_states, golden, golden_case,
-                     to_ref_slot_order)
+                     golden_options, to_ref_slot_order)
 
 
 def test_index_max_oracle_vs_reference_binary(oracle_mod):
@@ -28,42 +28,121 @@ def test_reference_plugin_binary_if_present(oracle_mod):
     assert np.array_equal(out.numpy(), g["b_out"])
 
 
-@pytest.mark.parametrize("name", ["classifier_b2_n256", "classifier_b2_n200_emptynodes",
-                                  "classifier_b2_n256_somk0"])
-def test_classifier_oracle_vs_reference(oracle_mod, name):
-    g = golden(name)
-    opt, inp, seed = golden_case(g, "classifier")
-    st = build_states("classifier", opt, seed)
+# fixtures at non-default options (oracle/make_golden.py:gen_options)
+OPTION_CLASSIFIERS = ["classifier_b2_n300_m121_k4", "classifier_b3_n150_m16_k1",
+                      "classifier_b1_n700_m256_k2"]
+AUTOENCODERS = ["autoencoder_b2_n256", "autoencoder_b2_n300_m36_conv4096"]
+
+
+def _encoder_vs_reference(oracle_mod, g, opt, st, inp):
     o = oracle_mod.encoder_forward(st["encoder"], opt, inp["pc"], inp["sn"], inp["node"],
                                    inp["node_knn_I"])
+    assert tuple(g["som_node__shape"]) == (opt.batch_size, 3, opt.node_num)
     assert np.array_equal(oracle_mod.canon_sets(o["min_idx"], opt.k).numpy(), g["knn_sets"])
     c_idx, _ = oracle_mod.som_topk(inp["pc"], inp["node"], opt.k)
     assert np.array_equal(oracle_mod.canon_sets(c_idx, opt.k).numpy(), g["knn_sets"])
     assert np.array_equal(o["mask_row_max"].numpy(), g["mask_row_max"])
     assert np.array_equal(o["mask_row_sum"].numpy(), g["mask_row_sum"])
-    if "emptynodes" in name:
+    if str(g["node_mode"]) == "uniform":
         assert (g["mask_row_max"] == 0).any(), "fixture must exercise empty nodes"
-    for n in ("som_node", "first_pn_out_masked_max", "final_pn_out", "feature"):
+    names = ["som_node", "first_pn_out_masked_max", "final_pn_out", "feature"]
+    if opt.som_k >= 2:
+        names += ["knn_center_1", "knn_feature_1"]
+    for n in names:
         assert_golden(g, n, o[n], tol=1e-5)
     # per-copy tensors: compare in the slot order of the reference run (torch.topk(sorted=False)
     # order may differ between machines)
     assert_golden(g, "first_pn_out", to_ref_slot_order(o["first_pn_out"], o["min_idx"], g, opt.k),
                   tol=1e-5)
+    return o
+
+
+@pytest.mark.parametrize("name", ["classifier_b2_n256", "classifier_b2_n200_emptynodes",
+                                  "classifier_b2_n256_somk0"] + OPTION_CLASSIFIERS)
+def test_classifier_oracle_vs_reference(oracle_mod, name):
+    g = golden(name)
+    opt, inp, seed = golden_case(g, "classifier")
+    st = build_states("classifier", opt, seed)
+    o = _encoder_vs_reference(oracle_mod, g, opt, st, inp)
     score = oracle_mod.classifier_forward(st["head"], o["feature"])
     assert_golden(g, "score", score, tol=1e-5)
 
 
+def test_option_fixtures_cover_the_options_they_are_named_for():
+    """Each fixture at non-default options must still hold them (a regenerated file with the
+    defaults would silently turn its tests into duplicates)."""
+    want = {"classifier_b2_n300_m121_k4": dict(node_num=121, k=4, som_k_type="center",
+                                               surface_normal=False),
+            "classifier_b3_n150_m16_k1": dict(node_num=16, k=1),
+            "classifier_b1_n700_m256_k2": dict(node_num=256, k=2),
+            "segmenter_b2_n200_m100_k2": dict(node_num=100, k=2, som_k_type="avg",
+                                              surface_normal=False),
+            "autoencoder_b2_n300_m36_conv4096": dict(node_num=36, output_conv_pc_num=4096)}
+    somk = {"classifier_b2_n300_m121_k4": 9, "classifier_b3_n150_m16_k1": 2,
+            "classifier_b1_n700_m256_k2": 9, "segmenter_b2_n200_m100_k2": 9,
+            "autoencoder_b2_n300_m36_conv4096": 5}
+    for name, opts in want.items():
+        g = golden(name)
+        got = golden_options(g)
+        for key, v in opts.items():
+            assert got.get(key) == v, (name, key, got.get(key))
+        assert int(g["som_k"]) == somk[name]
+    assert int(golden("classifier_b1_n700_m256_k2")["som_k"]) * 256 == 2304   # KA_MAX_MK
+
+
 def test_segmenter_oracle_vs_reference(oracle_mod):
-    g = golden("segmenter_b2_n128")
+    _segmenter_vs_reference(oracle_mod, "segmenter_b2_n128")
+
+
+def test_segmenter_oracle_vs_reference_k2_without_normals(oracle_mod):
+    """k=2, M=100, surface_normal=False, som_k_type='avg': the 9-channel point part of layer 1
+    and the two-copy average of the head."""
+    _segmenter_vs_reference(oracle_mod, "segmenter_b2_n200_m100_k2")
+
+
+def _segmenter_vs_reference(oracle_mod, name):
+    g = golden(name)
     opt, inp, seed = golden_case(g, "segmenter")
     st = build_states("segmenter", opt, seed)
-    o = oracle_mod.encoder_forward(st["encoder"], opt, inp["pc"], inp["sn"], inp["node"],
-                                   inp["node_knn_I"])
+    o = _encoder_vs_reference(oracle_mod, g, opt, st, inp)
     assert_golden(g, "centers", to_ref_slot_order(o["centers"], o["min_idx"], g, opt.k), tol=1e-6)
     assert_golden(g, "x_decentered",
                   to_ref_slot_order(o["x_decentered"], o["min_idx"], g, opt.k), tol=1e-6)
     s = oracle_mod.segmenter_forward(st["head"], opt, o, inp["pc"], inp["sn"], inp["label"])
     assert_golden(g, "score_segmenter", s, tol=1e-5)
+
+
+def _decoder_cpu(opt, st):
+    """networks.Decoder on CPU tensors: every layer takes the PyTorch composition of the
+    reference's modules (the hand-written kernels run on CUDA tensors only)."""
+    from sonet_b200 import networks
+    dec = networks.Decoder(opt)
+    dec.load_state_dict(st)
+    return dec.eval()
+
+
+@pytest.mark.parametrize("name", AUTOENCODERS)
+def test_autoencoder_oracle_vs_reference(oracle_mod, name):
+    g = golden(name)
+    opt, inp, seed = golden_case(g, "autoencoder")
+    st = build_states("autoencoder", opt, seed)
+    o = _encoder_vs_reference(oracle_mod, g, opt, st, inp)
+    with torch.no_grad():
+        dec = _decoder_cpu(opt, st["head"])
+        pred = dec(o["feature"])
+    assert_golden(g, "predicted_pc", pred, tol=1e-5)
+    assert_golden(g, "conv_pc4", dec.conv_pc4, tol=1e-5)
+    losses = {"loss_chamfer": oracle_mod.chamfer(pred, inp["pc"]),
+              "loss_chamfer_conv4": oracle_mod.chamfer(dec.conv_pc4, inp["pc"])}
+    if opt.output_conv_pc_num == 4096:
+        assert tuple(g["predicted_pc__shape"]) == (opt.batch_size, 3, 256 + 4096)
+        assert_golden(g, "conv_pc5", dec.conv_pc5, tol=1e-5)
+        assert_golden(g, "conv_pc6", dec.conv_pc6, tol=1e-5)
+        losses["loss_chamfer_conv5"] = oracle_mod.chamfer(dec.conv_pc5, inp["pc"])
+    for n, ch in losses.items():
+        assert_close(ch["loss"], g[n], n, 1e-5)
+    assert_close(sum(ch["loss"] for ch in losses.values()), g["loss"], "loss", 1e-5)
+    assert_close(losses["loss_chamfer"]["loss_array"], g["loss_array"], "loss_array", 1e-5)
 
 
 def test_chamfer_oracle_vs_reference(oracle_mod):
