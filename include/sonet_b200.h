@@ -167,11 +167,13 @@ int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, int P, cons
  *   sonet_pointwise_tc_forward_dev: the generic wgmma layer with that blob (1/scale read from
  *     device memory): the forward GEMM y = W x + b and the dgrad GEMM dx = W^T dy of a training step.
  *   sonet_wgrad_tc_f32: the wgrad GEMM dW[co][ci] = sum_{b,p} dy[b,co,p] x[b,ci,p] on the same kernel:
- *     dy is transposed to [K = B*P][Cout] and pre-scaled by a power of two (gradients are far below
- *     fp16's normal range), x is packed as the weight operand with k = (b,p), K is split over
- *     CTAs (splits) and reduced in a fixed order. Result dWT [Cin][Cout]. Device scratch: dyT
- *     sonet_wgrad_kpad(B,P,splits)*Cout floats, blob sonet_wgrad_blob_bytes(Cin,Kpad) bytes,
- *     part splits*Cin*Cout floats, small 8 floats. Needs Cout % 64 == 0.
+ *     dy is transposed to [K = B*P][Cout] and every channel pre-scaled by its own power of two
+ *     (gradients are far below fp16's normal range, and one layer's channels span many decades:
+ *     each row of dW keeps fp32-order relative precision), x is packed as the weight operand with
+ *     k = (b,p), K is split over CTAs (splits) and reduced in a fixed order. Result dWT [Cin][Cout].
+ *     Device scratch: dyT sonet_wgrad_kpad(B,P,splits)*Cout floats, blob
+ *     sonet_wgrad_blob_bytes(Cin,Kpad) bytes, part splits*Cin*Cout floats, small
+ *     sonet_wgrad_small_floats(Cout) floats. Needs Cout % 64 == 0.
  *   sonet_absmax_scale_f32: scale2 = (s, 1/s), s the power of two with max|s*t| in [256,512). */
 int sonet_bn_partial_slots(int B, int C);
 int sonet_bn_train_forward_f32(const float* x, const float* gamma, const float* beta, int B, int C,
@@ -194,6 +196,7 @@ int sonet_absmax_scale_f32(const float* t, long long n, float* scale2, unsigned*
                            sonet_stream_t stream);
 long long sonet_wgrad_kpad(int B, int P, int splits);
 long long sonet_wgrad_blob_bytes(int Cin, long long Kpad);
+long long sonet_wgrad_small_floats(int Cout);
 int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Cout, int Cin, int P, int splits,
                        float* dyT, void* blob, float* part, float* small, float* dWT,
                        sonet_stream_t stream);
@@ -327,7 +330,11 @@ int sonet_chamfer_f32(const float* pred, const float* gt, int B, int Mp, int N, 
  *     (sonet_pointresnet_tc_blob_bytes() bytes) and the fp32 side parameters into fparams_host
  *     (sonet_pointresnet_tc_fparam_count() floats).
  *   forward (device pointers): x [B,Cin,P] (Cin <= 6), blob/fparams as packed (blob 16-byte
- *     aligned), out [B,384,P]. */
+ *     aligned), out [B,384,P].
+ *   Range: the activations between the layers are split into fp16 hi/lo halves that each
+ *   saturate at 65504, so an activation with |x| >= 131008 acts as +-131008 (the output stays
+ *   finite); past 65504 precision drops to ~2^-12 of the term. Activations far below unit scale
+ *   carry an absolute floor of 2^-25 each (error envelope: csrc/tc_common.cuh). */
 int sonet_pointresnet_tc_blob_bytes(void);
 int sonet_pointresnet_tc_fparam_count(void);
 int sonet_pointresnet_tc_pack(const float* W0, int Cin, const float* W1, const float* W2,
@@ -400,7 +407,11 @@ int sonet_pool_finalize(int32_t* keys, const float* p0, int B, int C, int M, flo
  *   pack (host pointers): W [Cout,Cin] row-major fp32 with the BN scale folded in -> blob_host,
  *     *inv_scale = 1 / (power-of-two pre-scale applied to the weights).
  *   forward (device pointers): as sonet_pointwise_layer_f32 with (blob, inv_scale) instead of
- *     (Wt, scale). */
+ *     (Wt, scale).
+ *   Range: each activation is split into fp16 hi/lo halves that each saturate at 65504, so an
+ *   input with |x| >= 131008 acts as +-131008 (the output stays finite); past 65504 precision
+ *   drops to ~2^-12 of the term. Error envelope (csrc/tc_common.cuh), per output:
+ *   4e-6 * sum_k |W x| + 2^-24 * (sum_k |W| + sum_k |x| * inv_scale). */
 long long sonet_pointwise_tc_blob_bytes(int Cout, int Cin);
 int sonet_pointwise_tc_pack(const float* W, int Cout, int Cin, void* blob_host, float* inv_scale);
 int sonet_pointwise_tc_forward(const float* x0, int C0, const float* x1, int C1, int B, int P,

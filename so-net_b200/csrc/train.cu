@@ -224,19 +224,48 @@ __global__ void __launch_bounds__(256)
 }
 
 // ---- wgrad helpers ------------------------------------------------------------------------------------
-// dyT[k = b*P + p][co] = dy[b][co][p] * s  (s = scale2[0], a power of two): the "activation" operand
-// of the wgrad GEMM in the [K][rows] layout the generic wgmma layer consumes. 32x32 smem tiles.
+// Per-channel power-of-two pre-scale of dy [B][C][P]: cscale[c] = s_c with max_{b,p} |s_c dy[b,c,p]|
+// in [256,512) (1 for an all-zero or non-finite channel), cscale[C + c] = 1/s_c. Gradients of one
+// layer span many decades between channels; with ONE scale per tensor the small channels' values
+// would fall into fp16's subnormal range and lose their relative precision (each row of dW is its
+// own parameter's gradient). One CTA per channel.
 __global__ void __launch_bounds__(256)
-    transpose_scale_kernel(const float* __restrict__ dy, int C, int P, const float* __restrict__ scale2,
+    channel_scale_kernel(const float* __restrict__ t, int B, int C, int P, float* __restrict__ cscale) {
+  const int c = blockIdx.x;
+  float m = 0.f;
+  for (int b = 0; b < B; ++b) {
+    const float* r = t + (static_cast<size_t>(b) * C + c) * P;
+    for (int p = threadIdx.x; p < P; p += blockDim.x) m = fmaxf(m, fabsf(r[p]));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  __shared__ float wm[8];
+  if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < 8; ++w) m = fmaxf(m, wm[w]);
+    float sc = 1.f;
+    if (m > 0.f && isfinite(m)) {
+      int e;
+      frexpf(m, &e);
+      sc = ldexpf(1.f, min(9 - e, 126));   // 2^126: 1/sc stays a normal float
+    }
+    cscale[c] = sc;
+    cscale[C + c] = 1.f / sc;
+  }
+}
+// dyT[k = b*P + p][co] = dy[b][co][p] * cscale[co] (powers of two): the "activation" operand of the
+// wgrad GEMM in the [K][rows] layout the generic wgmma layer consumes. 32x32 smem tiles.
+__global__ void __launch_bounds__(256)
+    transpose_scale_kernel(const float* __restrict__ dy, int C, int P, const float* __restrict__ cscale,
                            float* __restrict__ dyT) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z;
   const int p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  const float s = scale2[0];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;   // 32 x 8
   for (int i = ty; i < 32; i += 8) {
     const int c = c0 + i, p = p0 + tx;
-    tile[i][tx] = (c < C && p < P) ? dy[(static_cast<size_t>(b) * C + c) * P + p] * s : 0.f;
+    tile[i][tx] = (c < C && p < P) ? dy[(static_cast<size_t>(b) * C + c) * P + p] * cscale[c] : 0.f;
   }
   __syncthreads();
   for (int i = ty; i < 32; i += 8) {
@@ -244,10 +273,12 @@ __global__ void __launch_bounds__(256)
     if (p < P && c < C) dyT[(static_cast<size_t>(b) * P + p) * C + c] = tile[tx][i];
   }
 }
-// out2[0] = a[1] * b[1] (product of two inverse scales); out2[1] unused
-__global__ void inv_product_kernel(const float* __restrict__ a, const float* __restrict__ b,
-                                   float* __restrict__ out) {
-  out[0] = a[1] * b[1];
+// dWT [Cin][Cout] *= 1/s_co: undoes the per-channel pre-scale of dy (exact: powers of two)
+__global__ void __launch_bounds__(256)
+    col_unscale_kernel(float* __restrict__ dWT, long long n, int Cout, const float* __restrict__ inv_c) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    dWT[i] *= inv_c[i % Cout];
 }
 // x [B][Cin][P] as the "weight" matrix Wl[n = ci][k = b*P + p] of the wgrad GEMM, packed into the
 // wgmma blob layout (see tc_pack_device_kernel); K padded with zeros up to kch*64.
@@ -392,7 +423,8 @@ extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, in
 // below fp16's normal range), Wl = x packed as a weight blob, K split over CTAs with a
 // deterministic reduce. Result: dWT [Cin][Cout] (the caller views it transposed).
 // Scratch (device): dyT  Kpad*Cout floats, blob sonet_wgrad_blob_bytes(), part splits*Cin*Cout floats,
-// small: 8 floats + 2 uint32.
+// small: sonet_wgrad_small_floats(Cout) floats.
+extern "C" long long sonet_wgrad_small_floats(int Cout) { return 8 + 2LL * Cout; }
 extern "C" long long sonet_wgrad_kpad(int B, int P, int splits) {
   const long long K = static_cast<long long>(B) * P;
   const long long q = 64LL * splits;
@@ -414,15 +446,12 @@ extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Co
   const long long K = static_cast<long long>(B) * P;
   const long long Kpad = sonet_wgrad_kpad(B, P, splits);
   SONET_REQUIRE(Kpad < (1LL << 31), "wgrad_tc: too many points");
-  float* s_dy = small;            // [2]
-  float* s_x = small + 2;         // [2]
-  float* inv = small + 4;         // [1]
+  float* s_x = small;             // [2]
   unsigned* bits = reinterpret_cast<unsigned*>(small + 6);
-  int rc = sonet_absmax_scale_f32(dy, static_cast<long long>(B) * Cout * P, s_dy, bits, stream);
+  float* s_dy = small + 8;        // [2 * Cout]: per-channel scales, then their inverses
+  channel_scale_kernel<<<Cout, 256, 0, st>>>(dy, B, Cout, P, s_dy);
+  int rc = sonet_absmax_scale_f32(x, static_cast<long long>(B) * Cin * P, s_x, bits, stream);
   if (rc) return rc;
-  rc = sonet_absmax_scale_f32(x, static_cast<long long>(B) * Cin * P, s_x, bits + 1, stream);
-  if (rc) return rc;
-  inv_product_kernel<<<1, 1, 0, st>>>(s_dy, s_x, inv);
   if (Kpad > K)   // zero rows of the padded tail (the matching weight columns are packed as zeros too)
     cudaMemsetAsync(dyT + K * Cout, 0, sizeof(float) * static_cast<size_t>(Kpad - K) * Cout, st);
   transpose_scale_kernel<<<dim3((P + 31) / 32, (Cout + 31) / 32, B), 256, 0, st>>>(dy, Cout, P, s_dy, dyT);
@@ -433,7 +462,13 @@ extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Co
                           st>>>(x, B, Cin, P, s_x, static_cast<unsigned char*>(blob), cpad, kch);
   rc = check_launch("wgrad_tc(prepare)");
   if (rc) return rc;
-  // activations: dyT viewed as [B'=1][C'=Kpad][P'=Cout] (already scaled: no act pre-scale needed)
-  return sonet_pointwise_tc_forward_dev(dyT, static_cast<int>(Kpad), 1, Cout, blob, inv, nullptr, nullptr,
-                                        Cin, 0, splits, dWT, part, stream);
+  // activations: dyT viewed as [B'=1][C'=Kpad][P'=Cout] (already scaled: no act pre-scale needed);
+  // the epilogue undoes x's scale, col_unscale each dy channel's
+  rc = sonet_pointwise_tc_forward_dev(dyT, static_cast<int>(Kpad), 1, Cout, blob, s_x + 1, nullptr,
+                                      nullptr, Cin, 0, splits, dWT, part, stream);
+  if (rc) return rc;
+  const long long n = static_cast<long long>(Cin) * Cout;
+  col_unscale_kernel<<<static_cast<unsigned>(std::min<long long>((n + 255) / 256, 2048)), 256, 0, st>>>(
+      dWT, n, Cout, s_dy + Cout);
+  return check_launch("wgrad_tc(unscale)");
 }

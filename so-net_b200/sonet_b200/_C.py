@@ -47,6 +47,7 @@ _SIGNATURES = {
     "sonet_absmax_scale_f32": [c_void_p, ctypes.c_longlong, c_void_p, c_void_p, c_void_p],
     "sonet_wgrad_kpad": [c_int, c_int, c_int],
     "sonet_wgrad_blob_bytes": [c_int, ctypes.c_longlong],
+    "sonet_wgrad_small_floats": [c_int],
     "sonet_wgrad_tc_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                            c_void_p, c_void_p, c_void_p, c_void_p],
     "sonet_comm_nccl_version": [],
@@ -121,7 +122,8 @@ _RESTYPE = {"sonet_last_error_string": ctypes.c_char_p, "sonet_version": ctypes.
             "sonet_pointwise_tc_blob_bytes": ctypes.c_longlong,
             "sonet_som_group_smem_bytes": ctypes.c_longlong,
             "sonet_seg_loss_scratch_bytes": ctypes.c_longlong,
-            "sonet_wgrad_kpad": ctypes.c_longlong, "sonet_wgrad_blob_bytes": ctypes.c_longlong}
+            "sonet_wgrad_kpad": ctypes.c_longlong, "sonet_wgrad_blob_bytes": ctypes.c_longlong,
+            "sonet_wgrad_small_floats": ctypes.c_longlong}
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

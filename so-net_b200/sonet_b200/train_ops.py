@@ -123,10 +123,11 @@ def wgrad_tc(dy, x):
         blob = _scratch(dev, int(lib.sonet_wgrad_blob_bytes(Cin, Kpad)), torch.uint8,
                         _WGRAD_CACHE.setdefault("blob", {}))
         part = _scratch(dev, splits * Cin * Cout, torch.float32, _WGRAD_CACHE.setdefault("part", {}))
-        small = torch.empty(8, dtype=torch.float32, device=dev)
+        small = torch.empty(int(lib.sonet_wgrad_small_floats(Cout)), dtype=torch.float32, device=dev)
         dWT = torch.empty((Cin, Cout), dtype=torch.float32, device=dev)
         ops._call("sonet_wgrad_tc_f32", _C.ptr(dy), _C.ptr(x), B, Cout, Cin, P, splits, _C.ptr(dyT),
-                  _C.ptr(blob), _C.ptr(part), _C.ptr(small), _C.ptr(dWT), ops._stream(dy), kernels=9)
+                  _C.ptr(blob), _C.ptr(part), _C.ptr(small), _C.ptr(dWT), ops._stream(dy),
+                  kernels=8 if splits > 1 else 7)
     return dWT.t()
 
 
