@@ -322,8 +322,9 @@ int sonet_chamfer_f32(const float* pred, const float* gt, int B, int Mp, int N, 
  * Replaces Encoder.first_pointnet = PointResNet(Cin,[64,128,256,384]).forward in eval mode
  * (models/layers.py:419-432, models/networks.py:82-83,176): three Conv1d(k=1)+BN+ReLU layers, the
  * skip-concat of layer-0's output and the bare 320->384 layer, for every stacked point copy.
- * Activations stay in shared memory between the layers; fp32 parity comes from a 3-product fp16
- * hi/lo split (see csrc/pointmlp_tc.cu).
+ * Activations stay on chip between the layers: layer 0's output as a shared-memory operand image,
+ * layers 1-2's outputs in registers as the next layer's wgmma A operand; fp32 parity comes from a
+ * 3-product fp16 hi/lo split (see csrc/pointmlp_tc.cu).
  *   pack (host pointers): W0 [64,Cin], W1 [128,64], W2 [256,128], W3 [384,320] row-major with the
  *     eval BatchNorm scale already folded in; shift0..3 = folded bias/BN shift. Writes the bf16
  *     K-major core-matrix images streamed by the kernel into blob_host

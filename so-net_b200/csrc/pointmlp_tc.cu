@@ -10,22 +10,38 @@
 //   * points are the MMA M dimension, channels are N/K. Two consumer warpgroups own 64 points of
 //     the tile each (wgmma M = 64) and run independently except for the shared weight stream;
 //   * layer 0 (K=3|6, degenerate for tensor cores) runs on CUDA cores, one thread per point and
-//     32 channels;
-//   * layers 1-3 are wgmma f16 with fp32 accumulators in registers. The epilogue of a layer adds
-//     the folded-BN shift, applies the ReLU, splits into fp16 hi/lo and writes the pair straight
-//     into the K-major no-swizzle A image of the next layer in the warpgroup's own shared-memory
-//     region — activations never touch HBM. act2 overwrites act1 once layer 2's wgmmas are done;
+//     32 channels, and writes act0 as an fp16 hi/lo K-major no-swizzle image into the warpgroup's
+//     16 KB of shared memory: layer 1 and layer 3's skip slab read it as a shared-memory A operand;
+//   * layers 1-3 are wgmma f16 with fp32 accumulators in registers. A wgmma accumulator fragment
+//     (m64nN) has the layout of the register A fragment of m64k16, so the epilogues of layers 1
+//     and 2 (folded-BN shift, ReLU, fp16 hi/lo split) leave act1 / act2 in registers as the A
+//     operand of the next layer (64 / 128 registers per thread). No shared-memory image, fence or
+//     barrier separates the layers, the tensor cores read only weights from shared memory in
+//     layers 2-3, and activations never touch HBM;
 //   * fp32 parity (1e-4) on 16-bit tensor cores comes from the 3-product split
 //     x*w ~= hi(x)*hi(w) + lo(x)*hi(w) + hi(x)*lo(w) with FP16 halves (hi+lo carry 22 mantissa
 //     bits; the same split in bf16 carries 16 and measured 1.1e-4, outside the bar). Weights are
 //     pre-scaled per layer by a power of two (undone exactly in the epilogue FMA) so their lo
 //     halves stay normal fp16 numbers; activations saturate at the fp16 range (65504) in the conversion;
 //   * weights (B operand, K-major no-swizzle core-matrix images packed once by the host) stream
-//     L2 -> shared memory through a 2-slot ring (cp.async.bulk + mbarrier), 25 stages per tile:
-//     layer 1 (N=128), four layer-2 K slabs (N=256), 4 chunks x 5 K slabs of layer 3 (N=96);
-//   * shared memory: 2 x 80 KB activation regions + 2 x 32 KB weight slots = 224 KB of the 227 KB
-//     a block may use on H100;
-//   * warp roles: warps 0-7 the two consumer warpgroups, warp 8 the TMA producer.
+//     L2 -> shared memory through a 5-slot ring (cp.async.bulk + mbarrier), 25 stages per tile:
+//     layer 1 (N=128), four layer-2 K slabs (N=256), 4 chunks x 5 K slabs of layer 3 (N=96).
+//     Every consumer warp releases a slot as soon as the wgmmas that read it have retired;
+//   * shared memory: 2 x 16 KB act0 images + 5 x 32 KB weight slots + W0 and the four shift
+//     vectors = 197 KB (a sixth slot would not leave room for the shifts);
+//   * warp roles: warpgroups 0-1 the consumers, warpgroup 2 the TMA producer (one thread). The
+//     producer gives registers to the consumers (setmaxnreg 24 / 240), where act2, the layer-3
+//     accumulators and the pool epilogue are live together;
+//   * phasing: the consumers share the ring but no barrier, so either may run ahead of the other
+//     by as many stages as the ring holds. An ordered hand-over of the tensor pipe (ping-pong: the
+//     warpgroups take turns issuing each layer's / layer-3 chunk's wgmmas, so one's epilogue runs
+//     under the other's MMAs) was measured against this free drift at cfg-2 on an H100 80GB HBM3.
+//     With the earlier column-at-a-time pool epilogue, at 700 W, both took 1.81-1.83 ms. With the
+//     one below, at 400 W, ping-pong took ~3 % fewer SM cycles but ran at a lower clock, for < 1 %
+//     more clouds/s. That does not pay for the turn protocol, so free drift stays;
+//   * the pool epilogue runs the shuffle reductions of all 24 columns interleaved before lanes 0-3
+//     issue the atomics: one column at a time, each a chain of 3 dependent shuffles behind its own
+//     branch, it was latency-bound and cost ~25 % of the kernel's cycles.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -38,7 +54,7 @@ namespace sonet {
 namespace pm {
 constexpr int C0 = 64, C1 = 128, C2 = 256, C3 = 384, K3 = C0 + C2;  // layer widths
 constexpr int TILE = 128;                                            // points per tile
-constexpr int SLOT_BYTES = 32768, NSLOT = 2;
+constexpr int SLOT_BYTES = 32768, NSLOT = 5;
 constexpr int W1_BYTES = 2 * C1 * C0 * 2;                            // hi + lo images, 32 KB
 constexpr int L2_STAGES = 4, L2_KT = 32;                             // [256 rows x 32 k] per stage
 constexpr int L3_CHUNKS = 4, L3_N = 96, L3_KSTAGES = 5, L3_KT = 64;  // [96 rows x 64 k] per stage
@@ -48,18 +64,20 @@ constexpr int STAGES_PER_TILE = 1 + L2_STAGES + L3_CHUNKS * L3_KSTAGES;  // 25
 constexpr int BLOB_BYTES =
     W1_BYTES + L2_STAGES * L2_STAGE_BYTES + L3_CHUNKS * L3_KSTAGES * L3_STAGE_BYTES;  // 655360
 constexpr int NFP = C0 * 6 + C0 + C1 + C2 + C3 + 4;   // W0 | shift0..3 | 1/wscale1..3 (floats)
-constexpr int NUM_THREADS = 288;
-// per-warpgroup activation region: act0 [64 x 64] hi | lo, then act1 [64 x 128] / act2 [64 x 256]
+// warpgroups 0-1 consume (64 points each), warpgroup 2 produces; registers per thread after the
+// hand-over: 2 * 128 * 240 + 128 * 24 = 64512, the launch's 168 x 384
+constexpr int NUM_THREADS = 384;
+constexpr int CONSUMER_REGS = 240, PRODUCER_REGS = 24;
+// per-warpgroup act0 image [64 x 64] hi | lo (the A operand of layer 1 and of layer 3's skip slab)
 constexpr int ACT0_HALF = 64 * C0 * 2;                 // 8 KB
-constexpr int ACT1_HALF = 64 * C1 * 2;                 // 16 KB
-constexpr int ACT2_HALF = 64 * C2 * 2;                 // 32 KB
-constexpr int OFF_ACT12 = 2 * ACT0_HALF;
-constexpr int REGION_BYTES = OFF_ACT12 + 2 * ACT2_HALF;   // 80 KB
-constexpr int OFF_RING = 2 * REGION_BYTES;
-constexpr int OFF_W0 = OFF_RING + NSLOT * SLOT_BYTES;     // W0 | shift0 (floats)
-constexpr int OFF_BAR = OFF_W0 + (C0 * 6 + C0) * 4;
+constexpr int OFF_RING = 2 * 2 * ACT0_HALF;            // 32 KB
+// W0 | shift0..3 (floats): the epilogues read their shifts with immediate shared-memory offsets;
+// global loads needed a 64-bit address register each, which spilled next to act2
+constexpr int NFP_SMEM = C0 * 6 + C0 + C1 + C2 + C3;
+constexpr int OFF_FP = OFF_RING + NSLOT * SLOT_BYTES;
+constexpr int OFF_BAR = OFF_FP + NFP_SMEM * 4;
 constexpr int NBAR = 2 * NSLOT;
-constexpr int SMEM_BYTES = OFF_BAR + NBAR * 8;
+constexpr int SMEM_BYTES = OFF_BAR + NBAR * 8;         // 201552 (the opt-in limit is 232448)
 
 __host__ __device__ constexpr int stage_bytes(int s) {
   return s == 0 ? W1_BYTES : (s <= L2_STAGES ? L2_STAGE_BYTES : L3_STAGE_BYTES);
@@ -91,7 +109,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
                           float* __restrict__ out, long long* __restrict__ dbg, PoolArgs pool) {
   using namespace pm;
   extern __shared__ __align__(1024) unsigned char smem[];
-  float* w0s = reinterpret_cast<float*>(smem + OFF_W0);
+  float* fps = reinterpret_cast<float*>(smem + OFF_FP);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + OFF_BAR);   // [NSLOT] TMA -> MMA
   uint64_t* empty = full + NSLOT;                                  // [NSLOT] MMA -> TMA
 
@@ -103,7 +121,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
   const int my_tiles = (static_cast<int>(blockIdx.x) < num_tiles)
                            ? (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
-  for (int i = threadIdx.x; i < C0 * 6 + C0; i += NUM_THREADS) w0s[i] = fparams[i];
+  for (int i = threadIdx.x; i < NFP_SMEM; i += NUM_THREADS) fps[i] = fparams[i];
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSLOT; ++s) {
       mbar_init(&full[s], 1);
@@ -113,9 +131,10 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
   }
   __syncthreads();
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // =========================== TMA producer ===========================
-    if (lane == 0) {
+    tc::regs_dec<PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
       uint32_t q = 0;
 #pragma unroll 1
       for (int t = 0; t < my_tiles; ++t) {
@@ -133,16 +152,18 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     }
   } else {
     // =========================== consumer warpgroups ===========================
+    tc::regs_inc<CONSUMER_REGS>();
     constexpr unsigned FULL = 0xffffffffu;
     const int wg = warp >> 2;
     const int tw = threadIdx.x & 127;
-    unsigned char* region = smem + wg * REGION_BYTES;
-    const uint32_t act0_a = smem_u32(region), act12_a = smem_u32(region + OFF_ACT12);
+    unsigned char* act0 = smem + wg * 2 * ACT0_HALF;
+    const uint32_t act0_a = smem_u32(act0);
     const uint32_t ring_a = smem_u32(smem + OFF_RING);
-    const float* sh1 = fparams + C0 * 6 + C0;
+    const float* sh1 = fps + C0 * 6 + C0;
     const float* sh2 = sh1 + C1;
     const float* sh3 = sh2 + C2;
-    const float inv1 = __ldg(sh3 + C3), inv2 = __ldg(sh3 + C3 + 1), inv3 = __ldg(sh3 + C3 + 2);
+    const float* invs = fparams + NFP_SMEM;
+    const float inv1 = __ldg(invs), inv2 = __ldg(invs + 1), inv3 = __ldg(invs + 2);
     // accumulator fragment: rows r0 = 16*(warp%4) + lane/4 and r0 + 8 of the warpgroup's 64,
     // columns 8j + 2*(lane%4) + {0,1} (registers 4j+{0,1} for r0, 4j+{2,3} for r0 + 8)
     const int r0 = 16 * (warp & 3) + (lane >> 2);
@@ -158,17 +179,21 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[qq % NSLOT]);
     };
-    // fp32 accumulator pair (row r, columns k, k+1) -> fp16 hi/lo words of an A image with SBO sbo
-    auto put_pair = [&](unsigned char* img_hi, int half_bytes, int sbo, int r, int k, float a, float b) {
-      uint32_t hi, lo;
-      tc::split2_f16(a, b, hi, lo);
-      const int off = (r >> 3) * sbo + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2;
-      *reinterpret_cast<uint32_t*>(img_hi + off) = hi;
-      *reinterpret_cast<uint32_t*>(img_hi + half_bytes + off) = lo;
-    };
-    auto publish = [&]() {   // A-image writes of this warpgroup -> its next wgmmas
-      tc::fence_proxy_async();
-      tc::named_sync(1 + wg, 128);
+    // Epilogue into the next layer's register A operand: the accumulator fragment of columns
+    // [16kk, 16kk+16) is the m64k16 A fragment of K block kk, word i = registers 8kk+2i, 8kk+2i+1
+    // (row r0 + 8*(i&1), columns 16kk + 8*(i>>1) + cq + {0,1}), split into fp16 hi/lo words.
+    auto to_frags = [&](const float* acc, int kblocks, float inv, const float* sh, uint32_t (*hi)[4],
+                        uint32_t (*lo)[4]) {
+      const float* shq = sh + cq;
+#pragma unroll
+      for (int kk = 0; kk < kblocks; ++kk)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int k = 16 * kk + 8 * (i >> 1);
+          tc::split2_f16(fmaxf(fmaf(acc[8 * kk + 2 * i], inv, shq[k]), 0.f),
+                         fmaxf(fmaf(acc[8 * kk + 2 * i + 1], inv, shq[k + 1]), 0.f),
+                         hi[kk][i], lo[kk][i]);
+        }
     };
 
 #pragma unroll 1
@@ -185,7 +210,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
         for (int c = 0; c < 6; ++c)
           xv[c] = (j < P && c < Cin) ? __ldg(x_in + (static_cast<size_t>(b) * Cin + c) * P + j) : 0.f;
-        unsigned char* a_hi = region + (m >> 3) * 1024 + (m & 7) * 16;
+        unsigned char* a_hi = act0 + (m >> 3) * 1024 + (m & 7) * 16;
 #pragma unroll
         for (int o = 0; o < 4; ++o) {
           uint32_t hi[4], lo[4];
@@ -195,9 +220,9 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int ch = half * 32 + o * 8 + 2 * jj + e;
-              float a = w0s[C0 * 6 + ch];
+              float a = fps[C0 * 6 + ch];
 #pragma unroll
-              for (int c = 0; c < 6; ++c) a = fmaf(w0s[ch * 6 + c], xv[c], a);
+              for (int c = 0; c < 6; ++c) a = fmaf(fps[ch * 6 + c], xv[c], a);
               y[e] = fmaxf(a, 0.f);
             }
             tc::split2_f16(y[0], y[1], hi[jj], lo[jj]);
@@ -206,10 +231,13 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
           *reinterpret_cast<uint4*>(a_hi + oct * 128) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
           *reinterpret_cast<uint4*>(a_hi + ACT0_HALF + oct * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
         }
-        publish();
+        // act0 writes of this warpgroup -> its wgmmas
+        tc::fence_proxy_async();
+        tc::named_sync(1 + wg, 128);
       }
 
-      // ---- layer 1: D1[64 x 128] = act0[64 x 64] * W1^T ----
+      // ---- layer 1: D1[64 x 128] = act0[64 x 64] * W1^T, A from shared memory ----
+      uint32_t a1_hi[C1 / 16][4], a1_lo[C1 / 16][4];
       {
         float acc[64];
 #pragma unroll
@@ -229,38 +257,27 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
         tc::wg_commit();
         tc::wg_wait<0>();
         stage_release(q++);
-        unsigned char* img = region + OFF_ACT12;
-#pragma unroll
-        for (int jn = 0; jn < 16; ++jn) {
-          const int k = 8 * jn + cq;
-#pragma unroll
-          for (int rr = 0; rr < 2; ++rr)
-            put_pair(img, ACT1_HALF, 2048, r0 + 8 * rr, k,
-                     fmaxf(fmaf(acc[4 * jn + 2 * rr], inv1, __ldg(sh1 + k)), 0.f),
-                     fmaxf(fmaf(acc[4 * jn + 2 * rr + 1], inv1, __ldg(sh1 + k + 1)), 0.f));
-        }
-        publish();
+        to_frags(acc, C1 / 16, inv1, sh1, a1_hi, a1_lo);
       }
 
-      // ---- layer 2: D2[64 x 256] = act1[64 x 128] * W2^T, four K slabs of 32 ----
+      // ---- layer 2: D2[64 x 256] = act1[64 x 128] * W2^T, four K slabs of 32, A from registers ----
+      uint32_t a2_hi[C2 / 16][4], a2_lo[C2 / 16][4];
       {
         float acc[128];
 #pragma unroll
         for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-#pragma unroll 1
+#pragma unroll
         for (int kc = 0; kc < L2_STAGES; ++kc) {
           const uint32_t sb = stage_wait();
           tc::wg_fence();
 #pragma unroll
           for (int ks = 0; ks < 2; ++ks) {
-            const uint32_t ka = act12_a + (kc * 4 + ks * 2) * 128;
-            const uint64_t ah = tc::smem_desc(ka, 128, 2048),
-                           al = tc::smem_desc(ka + ACT1_HALF, 128, 2048),
-                           bh = tc::smem_desc(sb + ks * 256, 128, 512),
+            const int kk = kc * 2 + ks;
+            const uint64_t bh = tc::smem_desc(sb + ks * 256, 128, 512),
                            bl = tc::smem_desc(sb + L2_STAGE_BYTES / 2 + ks * 256, 128, 512);
-            tc::wgmma_f16_n256(acc, ah, bh, 1);
-            tc::wgmma_f16_n256(acc, al, bh, 1);
-            tc::wgmma_f16_n256(acc, ah, bl, 1);
+            tc::wgmma_f16_rs_n256(acc, a1_hi[kk], bh, 1);
+            tc::wgmma_f16_rs_n256(acc, a1_lo[kk], bh, 1);
+            tc::wgmma_f16_rs_n256(acc, a1_hi[kk], bl, 1);
           }
           tc::wg_commit();
           tc::wg_wait<1>();
@@ -269,20 +286,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
         }
         tc::wg_wait<0>();
         stage_release(q - 1);
-        // act2 overwrites act1, including rows other warps' wgmmas read: wait_group only covers
-        // the executing warp's own groups, so every warp of the warpgroup must be past it first
-        tc::named_sync(1 + wg, 128);
-        unsigned char* img = region + OFF_ACT12;
-#pragma unroll
-        for (int jn = 0; jn < 32; ++jn) {
-          const int k = 8 * jn + cq;
-#pragma unroll
-          for (int rr = 0; rr < 2; ++rr)
-            put_pair(img, ACT2_HALF, 4096, r0 + 8 * rr, k,
-                     fmaxf(fmaf(acc[4 * jn + 2 * rr], inv2, __ldg(sh2 + k)), 0.f),
-                     fmaxf(fmaf(acc[4 * jn + 2 * rr + 1], inv2, __ldg(sh2 + k + 1)), 0.f));
-        }
-        publish();
+        to_frags(acc, C2 / 16, inv2, sh2, a2_hi, a2_lo);
       }
 
       // ---- layer 3: D3[64 x 384] = cat(act0, act2)[64 x 320] * W3^T, 4 chunks of N=96; bare ----
@@ -301,22 +305,27 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
         float acc[48];
 #pragma unroll
         for (int i = 0; i < 48; ++i) acc[i] = 0.f;
-#pragma unroll 1
+        // K slab 0 = act0 (shared memory), slabs 1-4 = act2 K blocks 4(kc-1) .. 4(kc-1)+3 (registers)
+#pragma unroll
         for (int kc = 0; kc < L3_KSTAGES; ++kc) {
           const uint32_t sb = stage_wait();
-          // 16-channel K groups: stage 0 = act0, stages 1-4 = act2 quarters
-          const uint32_t a0 = kc == 0 ? act0_a : act12_a + (kc - 1) * 8 * 128;
-          const uint32_t sbo = kc == 0 ? 1024 : 4096, ahalf = kc == 0 ? ACT0_HALF : ACT2_HALF;
           tc::wg_fence();
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t ah = tc::smem_desc(a0 + ks * 256, 128, sbo),
-                           al = tc::smem_desc(a0 + ahalf + ks * 256, 128, sbo),
-                           bh = tc::smem_desc(sb + ks * 256, 128, 1024),
+            const uint64_t bh = tc::smem_desc(sb + ks * 256, 128, 1024),
                            bl = tc::smem_desc(sb + L3_STAGE_BYTES / 2 + ks * 256, 128, 1024);
-            tc::wgmma_f16_n96(acc, ah, bh, 1);
-            tc::wgmma_f16_n96(acc, al, bh, 1);
-            tc::wgmma_f16_n96(acc, ah, bl, 1);
+            if (kc == 0) {
+              const uint64_t ah = tc::smem_desc(act0_a + ks * 256, 128, 1024),
+                             al = tc::smem_desc(act0_a + ACT0_HALF + ks * 256, 128, 1024);
+              tc::wgmma_f16_n96(acc, ah, bh, 1);
+              tc::wgmma_f16_n96(acc, al, bh, 1);
+              tc::wgmma_f16_n96(acc, ah, bl, 1);
+            } else {
+              const int kk = 4 * (kc - 1) + ks;
+              tc::wgmma_f16_rs_n96(acc, a2_hi[kk], bh, 1);
+              tc::wgmma_f16_rs_n96(acc, a2_lo[kk], bh, 1);
+              tc::wgmma_f16_rs_n96(acc, a2_hi[kk], bl, 1);
+            }
           }
           tc::wg_commit();
           tc::wg_wait<1>();
@@ -334,11 +343,11 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
             if (j >= P) continue;
             float* o = out + (static_cast<size_t>(b) * C3 + cbase) * P + j;
 #pragma unroll
-            for (int jn = 0; jn < 12; ++jn)
+            for (int jn = 0; jn < 12; ++jn, o += 8 * static_cast<size_t>(P))
 #pragma unroll
               for (int e = 0; e < 2; ++e)
-                o[static_cast<size_t>(8 * jn + e) * P] =
-                    fmaf(acc[4 * jn + 2 * rr + e], inv3, __ldg(sh3 + cbase + 8 * jn + e));
+                o[e * static_cast<size_t>(P)] =
+                    fmaf(acc[4 * jn + 2 * rr + e], inv3, sh3[cbase + 8 * jn + e]);
           }
         } else {
           // per-node max over the warp's 16 rows, one pass per run of equal node ids
@@ -350,22 +359,29 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
             const bool in0 = nd[0] == node, in1 = nd[1] == node;
             rem0 &= ~__ballot_sync(FULL, in0);
             rem1 &= ~__ballot_sync(FULL, in1);
-            int32_t* kb = pool.keys + (static_cast<size_t>(b) * C3 + cbase) * pool.M + node;
+            // the 24 columns' shuffle chains interleaved, then lanes 0-3 issue the reductions;
+            // the key pointer is stepped, not indexed: 24 precomputed 64-bit column offsets would
+            // not fit next to act2
+            float mx[24];
 #pragma unroll
-            for (int jn = 0; jn < 12; ++jn)
+            for (int c = 0; c < 24; ++c)
+              mx[c] = fmaxf(in0 ? acc[4 * (c >> 1) + (c & 1)] : -INFINITY,
+                            in1 ? acc[4 * (c >> 1) + 2 + (c & 1)] : -INFINITY);
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                float mx = fmaxf(in0 ? acc[4 * jn + e] : -INFINITY, in1 ? acc[4 * jn + 2 + e] : -INFINITY);
-                mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 4));
-                mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 8));
-                mx = fmaxf(mx, __shfl_xor_sync(FULL, mx, 16));
-                if (lane < 4) {
-                  const int co = 8 * jn + e;
-                  const int bits = __float_as_int(fmaf(mx, inv3, __ldg(sh3 + cbase + co)));
+            for (int d = 4; d <= 16; d <<= 1)
+#pragma unroll
+              for (int c = 0; c < 24; ++c) mx[c] = fmaxf(mx[c], __shfl_xor_sync(FULL, mx[c], d));
+            if (lane < 4) {
+              int32_t* kb = pool.keys + (static_cast<size_t>(b) * C3 + cbase) * pool.M + node;
+#pragma unroll
+              for (int jn = 0; jn < 12; ++jn, kb += 8 * static_cast<size_t>(pool.M))
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int bits = __float_as_int(fmaf(mx[2 * jn + e], inv3, sh3[cbase + 8 * jn + e]));
                   const int key = bits ^ ((bits >> 31) & 0x7fffffff);   // order-preserving float -> int
-                  atomicMax(kb + static_cast<size_t>(co) * pool.M, key);
+                  atomicMax(kb + e * static_cast<size_t>(pool.M), key);
                 }
-              }
+            }
           }
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
@@ -375,7 +391,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
               for (int e = 0; e < 2; ++e)
                 pool.p0[static_cast<size_t>(b) * C3 + cbase + 8 * jn + e] =
-                    fmaf(acc[4 * jn + 2 * rr + e], inv3, __ldg(sh3 + cbase + 8 * jn + e));
+                    fmaf(acc[4 * jn + 2 * rr + e], inv3, sh3[cbase + 8 * jn + e]);
           }
         }
       }

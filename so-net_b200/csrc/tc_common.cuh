@@ -43,6 +43,15 @@ __device__ __forceinline__ void fence_proxy_async() {
 __device__ __forceinline__ void named_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// per-thread register budget of the executing warpgroup (all its warps must execute it)
+template <int N>
+__device__ __forceinline__ void regs_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void regs_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 // ---- conversions -----------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
