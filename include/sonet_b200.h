@@ -420,6 +420,23 @@ int sonet_pointwise_tc_forward(const float* x0, int C0, const float* x1, int C1,
                                int relu, const float* addend, const int32_t* gidx, int G,
                                float* out, sonet_stream_t stream);
 
+/* ---- KNNModule (3+C -> 512 -> 512, BN + ReLU, max over K) on wgmma, csrc/knn_tc.cu -----------
+ * Layer 1 is split by linearity: Y = W1f x [B,512,M] (the C feature columns, computed once per
+ * node by sonet_pointwise_tc_forward without shift or ReLU) is gathered per neighbour row and added
+ * to W1d dec (the 3 coordinate columns, fp32). One kernel then runs layer 2 on wgmma and the max
+ * over the K neighbours; neither h1 nor h2 is written.
+ *   blob_bytes / pack (host pointers): W2 [512,512] folded fp32 -> blob_host, *inv_scale.
+ *   forward (device pointers): coord [B,3,M], center [B,3,M] (as sonet_knn_assemble*_f32 writes
+ *     it), idx [B,M,Kstride] int64 (first K columns), Y [B,512,M], w1 [512][4] = {W1d[c,0..2],
+ *     shift1[c]} (16-byte aligned), shift2 [512] -> out [B,512,M] = knn_feature_1.
+ *     2 <= K <= 16, M <= 65535. Error envelope of layer 2 as sonet_pointwise_tc_forward. */
+long long sonet_knn_mlp_tc_blob_bytes(void);
+int sonet_knn_mlp_tc_pack(const float* W2, void* blob_host, float* inv_scale);
+int sonet_knn_mlp_tc_forward(const float* coord, const float* center, const int64_t* idx, int B,
+                             int M, int K, int Kstride, const float* Y, const float* w1,
+                             const void* blob, float inv_scale, const float* shift2, float* out,
+                             sonet_stream_t stream);
+
 /* ---- diagnostics -------------------------------------------------------------------------------
  * One 128 x N x K bf16 GEMM on wgmma (fp32 accumulate in registers), D = bf16(A) * bf16(Bm)^T.
  * A [128,K], Bm [N,K], D [128,N] fp32 row-major device pointers. mode 0: A from shared memory
@@ -446,6 +463,13 @@ int sonet_debug_pointresnet_tc_pool_timeline(const float* x_sorted, int Cin, int
                                              const int32_t* node_sorted, const int32_t* pos0, int M,
                                              int32_t* pool_keys, float* p0, long long* timeline64,
                                              sonet_stream_t stream);
+/* sonet_knn_mlp_tc_forward with clock64() stamps of CTA 0 in timeline64[128] (device): [126] kernel
+ * start, [127] kernel end. */
+int sonet_debug_knn_mlp_tc_timeline(const float* coord, const float* center, const int64_t* idx,
+                                    int B, int M, int K, int Kstride, const float* Y,
+                                    const float* w1, const void* blob, float inv_scale,
+                                    const float* shift2, float* out, long long* timeline64,
+                                    sonet_stream_t stream);
 int sonet_debug_tc_probe(const float* A, const float* Bm, int N, int K, int mode, int layout,
                          int swap_fields, float* D, sonet_stream_t stream);
 

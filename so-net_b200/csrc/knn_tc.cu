@@ -1,0 +1,336 @@
+// knn_tc.cu — the encoder's KNN module (models/layers.py:299-367: gather the K neighbour nodes,
+// decentre, 1x1 conv 387 -> 512 -> 512 with BN + ReLU, max over the K neighbours) as ONE wgmma
+// kernel for sm_90a, after a per-node GEMM for the feature part of layer 1.
+//
+// Layer 1 is linear in its input [dec; f(nbr)], so W1 [dec; f(nbr)] = W1d dec + (W1f f)(nbr): the
+// 384 feature channels are the same vector for every row that gathers node nbr. The caller computes
+// Y = W1f x once per NODE ([B,512,M], the generic wgmma layer without shift or ReLU, 9x fewer rows
+// than per (node, neighbour) row at som_k = 9). This kernel then runs, per row (node m, neighbour j):
+//
+//   * layer-1 epilogue on CUDA cores: h1 = relu(W1d . dec + Y[b,:,nbr] + shift1) in fp32, with
+//     dec = coord[b,:,nbr] - center[b,:,m] (the same __fsub_rn as knn_assemble). Each thread builds
+//     its part of the register A operand of m64k16 (2 rows x 8 channels, fp16 hi/lo) right before
+//     the wgmmas of that K block; h1 never exists in memory. The Y loads of block kk+2 are issued
+//     while block kk's wgmmas run;
+//   * layer 2 (512 -> 512) on wgmma with the fp16 hi/lo 3-product split, fp32 accumulators, in two
+//     N halves of 256 (128 accumulators per thread); the A operand is rebuilt for the second half;
+//   * max over the K neighbours on the RAW accumulators: y = relu(fmaf(raw, inv2 > 0, shift2)) is
+//     monotone in raw, so max_rows(y) == relu(fmaf(max_rows(raw), inv2, shift2)) bit for bit (the
+//     argument of the POOL epilogue of pointmlp_tc.cu). Every row reduces into per-node shared-memory
+//     keys, which the warpgroup converts and stores as knn_feature_1 [B,512,M]. h2 is never written.
+//     (A segmented shuffle reduction in front of the atomics spilled the accumulators.)
+//
+// Rows: a warpgroup owns a BLOCK of floor(64/K) whole consecutive nodes of the flattened (cloud,
+// node) sequence (7 nodes = 63 rows at K = 9), so no node is split across warpgroups or CTAs and no
+// global atomics are needed. A CTA tile is two blocks (one per consumer warpgroup) against one pass
+// of the 1 MB layer-2 weight stream: 32 stages of [256 out x 32 k] hi|lo, 32 KB each, through a
+// 4-slot ring (cp.async.bulk + mbarrier) fed by one producer thread. Warp roles and the register
+// hand-over (setmaxnreg 240 / 24) follow pointmlp_tc.cu.
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+
+#include "tc_common.cuh"
+
+namespace sonet {
+
+namespace kt {
+constexpr int C1 = 512, C2 = 512;        // hidden and output widths (KNNModule (512, 512))
+constexpr int NH = 256, NPASS = C2 / NH; // out channels per pass
+constexpr int KT = 32;                   // K extent of one weight stage
+constexpr int KSTAGES = C1 / KT;         // 16 stages per pass
+constexpr int STAGES_PER_TILE = NPASS * KSTAGES;
+constexpr int STAGE_BYTES = NH * KT * 2 * 2;          // hi + lo, 32 KB
+constexpr int BLOB_BYTES = STAGES_PER_TILE * STAGE_BYTES;   // 1 MB
+constexpr int NSLOT = 4;
+constexpr int MAX_K = 16, MIN_K = 2;
+constexpr int MAX_NPB = 64 / MIN_K;      // nodes per block
+constexpr int KEY_LD = NH + 8;           // padded key row: leaders of adjacent nodes hit other banks
+constexpr int NUM_THREADS = 384;
+constexpr int CONSUMER_REGS = 240, PRODUCER_REGS = 24;
+constexpr int OFF_RING = 0;
+constexpr int OFF_W1 = OFF_RING + NSLOT * STAGE_BYTES;          // float4 {w1d[0..2], shift1} x C1
+constexpr int OFF_SH2 = OFF_W1 + C1 * 16;                       // shift2 [C2]
+constexpr int OFF_KEYS = OFF_SH2 + C2 * 4;                      // [2 wg][MAX_NPB][KEY_LD] int
+constexpr int OFF_BAR = OFF_KEYS + 2 * MAX_NPB * KEY_LD * 4;
+constexpr int SMEM_BYTES = OFF_BAR + 2 * NSLOT * 8;
+}  // namespace kt
+
+struct KnnArgs {
+  const float* coord;     // [B,3,M]
+  const float* center;    // [B,3,M]
+  const int64_t* idx;     // [B,M,Kstride]
+  const float* Y;         // [B,C1,M]
+  const float* w1;        // [C1][4] {W1d[c,0..2], shift1[c]}
+  const float* shift2;    // [C2]
+  float inv2;
+  int B, M, K, Kstride;
+  int npb, nblocks;
+  float* out;             // [B,C2,M]
+};
+
+__global__ void __launch_bounds__(kt::NUM_THREADS, 1)
+    knn_mlp_tc_kernel(const unsigned char* __restrict__ blob, KnnArgs a, long long* __restrict__ dbg) {
+  using namespace kt;
+  extern __shared__ __align__(1024) unsigned char smem[];
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
+  uint64_t* empty = full + NSLOT;
+  const float4* w1s = reinterpret_cast<const float4*>(smem + OFF_W1);
+  const float* sh2 = reinterpret_cast<const float*>(smem + OFF_SH2);
+
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[64 + 62] = clock64();
+  const int num_tiles = (a.nblocks + 1) / 2;
+  const int my_tiles = (static_cast<int>(blockIdx.x) < num_tiles)
+                           ? (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+
+  for (int i = threadIdx.x; i < C1 * 4; i += NUM_THREADS)
+    reinterpret_cast<float*>(smem + OFF_W1)[i] = __ldg(a.w1 + i);
+  for (int i = threadIdx.x; i < C2; i += NUM_THREADS)
+    reinterpret_cast<float*>(smem + OFF_SH2)[i] = __ldg(a.shift2 + i);
+  for (int i = threadIdx.x; i < 2 * MAX_NPB * KEY_LD; i += NUM_THREADS)
+    reinterpret_cast<int*>(smem + OFF_KEYS)[i] = POOL_KEY_INIT;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NSLOT; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);   // one arrival per consumer warp
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // =========================== TMA producer ===========================
+    tc::regs_dec<PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
+      uint32_t q = 0;
+#pragma unroll 1
+      for (int t = 0; t < my_tiles; ++t) {
+#pragma unroll 1
+        for (int s = 0; s < STAGES_PER_TILE; ++s, ++q) {
+          const uint32_t slot = q % NSLOT, use = q / NSLOT;
+          if (use > 0) tc::mbar_wait_relaxed(&empty[slot], (use - 1) & 1, 300 + s);
+          mbar_arrive_expect_tx(&full[slot], STAGE_BYTES);
+          bulk_g2s(smem + OFF_RING + slot * STAGE_BYTES, blob + static_cast<size_t>(s) * STAGE_BYTES,
+                   STAGE_BYTES, &full[slot]);
+        }
+      }
+    }
+  } else {
+    // =========================== consumer warpgroups ===========================
+    tc::regs_inc<CONSUMER_REGS>();
+    constexpr unsigned FULL = 0xffffffffu;
+    const int wg = warp >> 2;
+    const int tw = threadIdx.x & 127;
+    const uint32_t ring_a = smem_u32(smem + OFF_RING);
+    int* keys = reinterpret_cast<int*>(smem + OFF_KEYS) + wg * MAX_NPB * KEY_LD;
+    // accumulator fragment: rows r0 = 16*(warp%4) + lane/4 and r0 + 8 of the warpgroup's 64,
+    // columns 8j + 2*(lane%4) + {0,1} (registers 4j+{0,1} for r0, 4j+{2,3} for r0 + 8)
+    const int r0 = 16 * (warp & 3) + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    const int rows_pb = a.npb * a.K;
+    const long long nodes = static_cast<long long>(a.B) * a.M;
+    uint32_t q = 0;
+
+    auto stage_wait = [&]() -> uint32_t {
+      const uint32_t slot = q % NSLOT;
+      tc::mbar_wait_bounded(&full[slot], (q / NSLOT) & 1, 3);
+      return ring_a + slot * STAGE_BYTES;
+    };
+    auto stage_release = [&](uint32_t qq) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[qq % NSLOT]);
+    };
+
+#pragma unroll 1
+    for (int t = 0; t < my_tiles; ++t) {
+      const int block = 2 * (blockIdx.x + t * gridDim.x) + wg;
+      const long long gnode0 = static_cast<long long>(block) * a.npb;
+      // this thread's two rows: block-local node (-1 = padding), Y column base, decentred coords
+      int ln[2];
+      const float* yrow[2];
+      float dec[2][3];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int lr = r0 + 8 * rr;
+        const long long g = gnode0 + lr / a.K;
+        ln[rr] = -1;
+        yrow[rr] = a.Y;
+        dec[rr][0] = dec[rr][1] = dec[rr][2] = 0.f;
+        if (block < a.nblocks && lr < rows_pb && g < nodes) {
+          const int b = static_cast<int>(g / a.M), m = static_cast<int>(g - static_cast<long long>(b) * a.M);
+          const int j = lr - (lr / a.K) * a.K;
+          const long long w = a.idx[(static_cast<size_t>(b) * a.M + m) * a.Kstride + j];
+          const int nbr = static_cast<int>(w < 0 ? 0 : (w > a.M - 1 ? a.M - 1 : w));
+          ln[rr] = lr / a.K;
+          yrow[rr] = a.Y + static_cast<size_t>(b) * C1 * a.M + nbr;
+#pragma unroll
+          for (int c = 0; c < 3; ++c)
+            dec[rr][c] = __fsub_rn(__ldg(a.coord + (static_cast<size_t>(b) * 3 + c) * a.M + nbr),
+                                   __ldg(a.center + (static_cast<size_t>(b) * 3 + c) * a.M + m));
+        }
+      }
+      // Y values of K block kk: word i of the A fragment = row i&1, channels 16kk + 8(i>>1) + cq + {0,1}
+      auto load_y = [&](int kk, float (&yv)[8]) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            yv[2 * i + e] = __ldg(yrow[i & 1] + static_cast<size_t>(16 * kk + 8 * (i >> 1) + cq + e) * a.M);
+      };
+      auto build = [&](int kk, const float (&yv)[8], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          float h[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float4 w = w1s[16 * kk + 8 * (i >> 1) + cq + e];
+            const float* d = dec[i & 1];
+            float v = yv[2 * i + e] + w.w;
+            v = fmaf(w.x, d[0], v);
+            v = fmaf(w.y, d[1], v);
+            v = fmaf(w.z, d[2], v);
+            h[e] = fmaxf(v, 0.f);
+          }
+          tc::split2_f16(h[0], h[1], hi[i], lo[i]);
+        }
+      };
+
+#pragma unroll 1
+      for (int pass = 0; pass < NPASS; ++pass) {
+        float acc[128];
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        uint32_t fh[2][4], fl[2][4];
+        float yv[8];
+        load_y(0, yv);
+        build(0, yv, fh[0], fl[0]);
+        load_y(1, yv);
+#pragma unroll 1
+        for (int st = 0; st < KSTAGES; ++st) {
+          const uint32_t sb = stage_wait();
+#pragma unroll
+          for (int ks = 0; ks < 2; ++ks) {
+            const int kk = 2 * st + ks;
+            const uint64_t bh = tc::smem_desc(sb + ks * 256, 128, 512),
+                           bl = tc::smem_desc(sb + STAGE_BYTES / 2 + ks * 256, 128, 512);
+            tc::wg_fence();
+            tc::wgmma_f16_rs_n256(acc, fh[ks], bh, 1);
+            tc::wgmma_f16_rs_n256(acc, fl[ks], bh, 1);
+            tc::wgmma_f16_rs_n256(acc, fh[ks], bl, 1);
+            tc::wg_commit();
+            // K block kk-1 has retired: its fragment buffer is free, and so is its stage if it
+            // was the stage's second block
+            tc::wg_wait<1>();
+            if (ks == 0 && st > 0) stage_release(q - 1);
+            if (kk + 1 < 2 * KSTAGES) {
+              build(kk + 1, yv, fh[ks ^ 1], fl[ks ^ 1]);
+              if (kk + 2 < 2 * KSTAGES) load_y(kk + 2, yv);
+            }
+          }
+          ++q;
+        }
+        tc::wg_wait<0>();
+        stage_release(q - 1);
+
+        // ---- max over each node's rows: every thread reduces its raw accumulators into the
+        // node's shared-memory keys (order-preserving ints); rows of one node share an address ----
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          if (ln[rr] < 0) continue;
+          int* kr = keys + ln[rr] * KEY_LD + cq;
+#pragma unroll
+          for (int jn = 0; jn < 32; ++jn)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int bits = __float_as_int(acc[4 * jn + 2 * rr + e]);
+              atomicMax(kr + 8 * jn + e, bits ^ ((bits >> 31) & 0x7fffffff));
+            }
+        }
+        tc::named_sync(1 + wg, 128);
+        // keys -> knn_feature_1[b, NH*pass + c, m] for the block's nodes; reset for the next pass
+        for (int i = tw; i < a.npb * NH; i += 128) {
+          const int c = i / a.npb, l = i - c * a.npb;
+          const long long g = gnode0 + l;
+          int* kp = keys + l * KEY_LD + c;
+          if (block < a.nblocks && g < nodes) {
+            const int b = static_cast<int>(g / a.M), m = static_cast<int>(g - static_cast<long long>(b) * a.M);
+            const int key = *kp;
+            const float raw = __int_as_float(key ^ ((key >> 31) & 0x7fffffff));
+            const int co = NH * pass + c;
+            a.out[(static_cast<size_t>(b) * C2 + co) * a.M + m] = fmaxf(fmaf(raw, a.inv2, sh2[co]), 0.f);
+          }
+          *kp = POOL_KEY_INIT;
+        }
+        tc::named_sync(1 + wg, 128);
+      }
+    }
+  }
+  __syncthreads();
+  if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[64 + 63] = clock64();
+}
+
+}  // namespace sonet
+
+extern "C" long long sonet_knn_mlp_tc_blob_bytes(void) { return sonet::kt::BLOB_BYTES; }
+
+extern "C" int sonet_knn_mlp_tc_pack(const float* W2, void* blob_host, float* inv_scale) {
+  using namespace sonet;
+  using namespace sonet::kt;
+  SONET_REQUIRE(W2 && blob_host && inv_scale, "knn_mlp_tc_pack: null pointer");
+  unsigned char* blob = static_cast<unsigned char*>(blob_host);
+  const float s = pow2_scale(W2, static_cast<size_t>(C2) * C1);
+  size_t off = 0;
+  for (int p = 0; p < NPASS; ++p)
+    for (int ks = 0; ks < KSTAGES; ++ks) {
+      pack_tile(W2, s, C1, NH * p, NH, KT * ks, KT, blob + off, blob + off + STAGE_BYTES / 2);
+      off += STAGE_BYTES;
+    }
+  *inv_scale = 1.f / s;
+  return SONET_OK;
+}
+
+static int launch_knn_mlp_tc(const float* coord, const float* center, const int64_t* idx, int B, int M,
+                             int K, int Kstride, const float* Y, const float* w1, const void* blob,
+                             float inv2, const float* shift2, float* out, long long* dbg,
+                             sonet_stream_t stream) {
+  using namespace sonet;
+  using namespace sonet::kt;
+  SONET_REQUIRE(B >= 0 && M >= 1 && Kstride >= K, "knn_mlp_tc: bad dimension");
+  SONET_REQUIRE(K >= MIN_K && K <= MAX_K, "knn_mlp_tc: K=%d out of range [%d,%d]", K, MIN_K, MAX_K);
+  SONET_REQUIRE(M <= 65535, "knn_mlp_tc: M=%d too large", M);
+  if (B == 0) return SONET_OK;
+  SONET_REQUIRE(coord && center && idx && Y && w1 && blob && shift2 && out, "knn_mlp_tc: null pointer");
+  SONET_REQUIRE(aligned16(blob) && aligned16(w1), "knn_mlp_tc: blob and w1 must be 16-byte aligned");
+  SONET_REQUIRE(inv2 > 0.f, "knn_mlp_tc: inv_scale must be positive");
+  KnnArgs a{coord, center, idx, Y, w1, shift2, inv2, B, M, K, Kstride, 64 / K, 0, out};
+  const long long nodes = static_cast<long long>(B) * M;
+  const long long nblocks = (nodes + a.npb - 1) / a.npb;
+  SONET_REQUIRE(nblocks < (1LL << 30), "knn_mlp_tc: too many nodes");
+  a.nblocks = static_cast<int>(nblocks);
+  SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "knn_mlp_tc: needs %d B of shared memory", SMEM_BYTES);
+  const int grid = static_cast<int>(std::min<long long>((nblocks + 1) / 2, sm_count()));
+  cudaFuncSetAttribute(knn_mlp_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+  knn_mlp_tc_kernel<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
+      static_cast<const unsigned char*>(blob), a, dbg);
+  return check_launch("knn_mlp_tc");
+}
+
+extern "C" int sonet_knn_mlp_tc_forward(const float* coord, const float* center, const int64_t* idx,
+                                        int B, int M, int K, int Kstride, const float* Y,
+                                        const float* w1, const void* blob, float inv_scale,
+                                        const float* shift2, float* out, sonet_stream_t stream) {
+  return launch_knn_mlp_tc(coord, center, idx, B, M, K, Kstride, Y, w1, blob, inv_scale, shift2, out,
+                           nullptr, stream);
+}
+
+extern "C" int sonet_debug_knn_mlp_tc_timeline(const float* coord, const float* center,
+                                               const int64_t* idx, int B, int M, int K, int Kstride,
+                                               const float* Y, const float* w1, const void* blob,
+                                               float inv_scale, const float* shift2, float* out,
+                                               long long* timeline64, sonet_stream_t stream) {
+  return launch_knn_mlp_tc(coord, center, idx, B, M, K, Kstride, Y, w1, blob, inv_scale, shift2, out,
+                           timeline64, stream);
+}

@@ -404,33 +404,6 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
   if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[64 + 63] = clock64();
 }
 
-// ---- host-side packing -------------------------------------------------------------------------------
-// fp16 hi/lo images of scale * W[rows r0..r0+nr) x [k0..k0+kt) (row stride ld), K-major no-swizzle:
-// element (r,k) at (r/8)*SBO + (k/8)*128 + (r%8)*16 + (k%8)*2 with SBO = kt*16.
-static void pack_tile(const float* W, float scale, int ld, int r0, int nr, int k0, int kt,
-                      unsigned char* hi, unsigned char* lo) {
-  const uint32_t sbo = static_cast<uint32_t>(kt) * 16;
-  for (int r = 0; r < nr; ++r)
-    for (int k = 0; k < kt; ++k) {
-      const float w = W[static_cast<size_t>(r0 + r) * ld + k0 + k] * scale;  // exact (power of 2)
-      const __half h = __float2half_rn(w);
-      const __half l = __float2half_rn(w - __half2float(h));
-      const uint32_t off = (r >> 3) * sbo + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2;
-      std::memcpy(hi + off, &h, 2);
-      std::memcpy(lo + off, &l, 2);
-    }
-}
-// power of two that brings max|W| into [256, 512): keeps the lo parts normal fp16 numbers and the
-// hi parts far from the 65504 overflow; undone exactly by the epilogue's multiply.
-static float pow2_scale(const float* W, size_t n) {
-  float m = 0.f;
-  for (size_t i = 0; i < n; ++i) m = std::max(m, std::fabs(W[i]));
-  if (!(m > 0.f) || !std::isfinite(m)) return 1.f;
-  int e;
-  std::frexp(m, &e);  // m = f * 2^e, f in [0.5, 1)
-  return std::ldexp(1.f, 9 - e);
-}
-
 }  // namespace sonet
 
 extern "C" int sonet_pointresnet_tc_blob_bytes(void) { return sonet::pm::BLOB_BYTES; }

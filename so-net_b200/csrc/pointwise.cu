@@ -448,11 +448,13 @@ __global__ void __launch_bounds__(256)
       ctr = cb[c * M + m];
     }
     center[(static_cast<size_t>(b) * 3 + c) * M + m] = ctr;
+    if (x_aug == nullptr) continue;
     for (int j = 0; j < K; ++j) {
       int id = clamp_idx(ib[m * Kstride + j], M);
       ob[static_cast<size_t>(c) * MK + m * K + j] = __fsub_rn(cb[c * M + id], ctr);
     }
   }
+  if (x_aug == nullptr) return;   // center only (the fused KNN MLP decentres on its own)
   // features: thread per (c, m, j); 32-bit index arithmetic (the launcher checks C*M*K < 2^31 — the
   // 64-bit division and modulo per element were what this loop spent its time on)
   const uint32_t total = static_cast<uint32_t>(C) * MK;
@@ -476,6 +478,29 @@ __device__ __forceinline__ bool sonet_aligned16_ptr(const void* p) {
   return (reinterpret_cast<uintptr_t>(p) & 15u) == 0;
 }
 constexpr int KA_MAX_MK = 2304;  // M*K positions cached per CTA
+
+// center [b,3,M] and, when ob is not null, the decentred coordinates = channels 0-2 of x_aug:
+// thread per (c, m)
+__device__ void knn_pool_center(const float* __restrict__ coord, int b, int M, int K, int center_type,
+                                const uint16_t* sid, float* __restrict__ center, float* __restrict__ ob) {
+  const float* cb = coord + static_cast<size_t>(b) * 3 * M;
+  const int MK = M * K;
+  for (int t = threadIdx.x; t < 3 * M; t += blockDim.x) {
+    const int c = t / M, m = t - c * M;
+    float ctr;
+    if (center_type == 0) {  // 'avg': torch.mean over K = sum / K
+      float s = 0.f;
+      for (int j = 0; j < K; ++j) s += cb[c * M + sid[m * K + j]];
+      ctr = __fdiv_rn(s, static_cast<float>(K));
+    } else {
+      ctr = cb[c * M + m];
+    }
+    center[(static_cast<size_t>(b) * 3 + c) * M + m] = ctr;
+    if (ob == nullptr) continue;
+    for (int j = 0; j < K; ++j)
+      ob[static_cast<size_t>(c) * MK + m * K + j] = __fsub_rn(cb[c * M + sid[m * K + j]], ctr);
+  }
+}
 
 __global__ void __launch_bounds__(256)
     knn_assemble_pool_kernel(const float* __restrict__ coord, int32_t* __restrict__ keys,
@@ -502,6 +527,13 @@ __global__ void __launch_bounds__(256)
     masked_max[g] = v;
     vals[cl * M + m] = v;
   }
+  if (x_aug == nullptr) {   // the fused KNN MLP gathers and decentres on its own
+    if (blockIdx.x == 0) {
+      __syncthreads();         // sid
+      knn_pool_center(coord, b, M, K, center_type, sid, center, nullptr);
+    }
+    return;
+  }
   __syncthreads();
   float* ob = x_aug + static_cast<size_t>(b) * (3 + C) * MK;
   if ((MK & 3) == 0 && sonet_aligned16_ptr(ob)) {
@@ -525,23 +557,7 @@ __global__ void __launch_bounds__(256)
       for (int mj = threadIdx.x; mj < MK; mj += blockDim.x) orow[mj] = vrow[sid[mj]];
     }
   }
-  if (blockIdx.x == 0) {   // coordinates: thread per (c, m)
-    const float* cb = coord + static_cast<size_t>(b) * 3 * M;
-    for (int t = threadIdx.x; t < 3 * M; t += blockDim.x) {
-      const int c = t / M, m = t - c * M;
-      float ctr;
-      if (center_type == 0) {  // 'avg': torch.mean over K = sum / K
-        float s = 0.f;
-        for (int j = 0; j < K; ++j) s += cb[c * M + sid[m * K + j]];
-        ctr = __fdiv_rn(s, static_cast<float>(K));
-      } else {
-        ctr = cb[c * M + m];
-      }
-      center[(static_cast<size_t>(b) * 3 + c) * M + m] = ctr;
-      for (int j = 0; j < K; ++j)
-        ob[static_cast<size_t>(c) * MK + m * K + j] = __fsub_rn(cb[c * M + sid[m * K + j]], ctr);
-    }
-  }
+  if (blockIdx.x == 0) knn_pool_center(coord, b, M, K, center_type, sid, center, ob);
 }
 
 // exact K-NN among the M nodes (models/layers.py:334-337): thread per (b, m).
@@ -750,8 +766,8 @@ extern "C" int sonet_knn_assemble_f32(const float* coord, const float* feat, con
   SONET_REQUIRE(center_type == 0 || center_type == 1, "knn_assemble: center_type must be 0|1");
   SONET_REQUIRE(B <= 65535, "knn_assemble: B=%d exceeds grid limit", B);
   if (B == 0) return SONET_OK;
-  SONET_REQUIRE(coord && (feat || C == 0) && idx && center && x_aug, "knn_assemble: null pointer");
-  const long long per_b = static_cast<long long>(C + 3) * M * K;
+  SONET_REQUIRE(coord && (feat || C == 0 || !x_aug) && idx && center, "knn_assemble: null pointer");
+  const long long per_b = x_aug ? static_cast<long long>(C + 3) * M * K : 3LL * M;
   SONET_REQUIRE(per_b < (1LL << 31), "knn_assemble: C*M*K = %lld exceeds the 32-bit index range", per_b);
   dim3 grid(static_cast<unsigned>(std::max<long long>(1, std::min<long long>((per_b + 255) / 256, 64))), B);
   knn_assemble_kernel<<<grid, 256, 0, as_stream(stream)>>>(coord, feat, idx, C, M, K, Kstride,
@@ -771,7 +787,7 @@ extern "C" int sonet_knn_assemble_pool_f32(const float* coord, int32_t* pool_key
                 "knn_assemble_pool: M=%d, K=%d exceed the per-CTA cache (finalize the pool and use "
                 "sonet_knn_assemble_f32)", M, K);
   if (B == 0) return SONET_OK;
-  SONET_REQUIRE(coord && pool_keys && p0 && idx && masked_max && center && x_aug,
+  SONET_REQUIRE(coord && pool_keys && p0 && idx && masked_max && center,
                 "knn_assemble_pool: null pointer");
   dim3 grid(static_cast<unsigned>((C + KA_CPB - 1) / KA_CPB), B);
   knn_assemble_pool_kernel<<<grid, 256, 0, as_stream(stream)>>>(

@@ -105,6 +105,13 @@ _SIGNATURES = {
     "sonet_pointwise_tc_forward": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                    ctypes.c_float, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                    c_int, c_void_p, c_void_p],
+    "sonet_knn_mlp_tc_blob_bytes": [],
+    "sonet_knn_mlp_tc_pack": [c_void_p, c_void_p, c_void_p],
+    "sonet_knn_mlp_tc_forward": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                 c_void_p, c_void_p, ctypes.c_float, c_void_p, c_void_p, c_void_p],
+    "sonet_debug_knn_mlp_tc_timeline": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                        c_void_p, c_void_p, c_void_p, ctypes.c_float, c_void_p,
+                                        c_void_p, c_void_p, c_void_p],
     "sonet_debug_pointresnet_tc_timeline": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_void_p],
     "sonet_debug_pointwise_tc_timeline": [c_void_p, c_int, c_int, c_int, c_void_p, ctypes.c_float,
@@ -120,6 +127,7 @@ _SIGNATURES = {
 }
 _RESTYPE = {"sonet_last_error_string": ctypes.c_char_p, "sonet_version": ctypes.c_char_p,
             "sonet_pointwise_tc_blob_bytes": ctypes.c_longlong,
+            "sonet_knn_mlp_tc_blob_bytes": ctypes.c_longlong,
             "sonet_som_group_smem_bytes": ctypes.c_longlong,
             "sonet_seg_loss_scratch_bytes": ctypes.c_longlong,
             "sonet_wgrad_kpad": ctypes.c_longlong, "sonet_wgrad_blob_bytes": ctypes.c_longlong,

@@ -492,6 +492,42 @@ class KNNModule(nn.Module):
                 and all(l._fast_eligible() for l in self.layers)
                 and (precomputed_knn_I is None or precomputed_knn_I.is_cuda))
 
+    # ---- fused wgmma path (csrc/knn_tc.cu) ----------------------------------------------------
+    def _tc_fused(self, K, M):
+        """Two BN/ReLU layers 3+C -> 512 -> 512 (the encoder's), 2 <= K <= 16, M*K <= 2304."""
+        ls = self.layers
+        return (os.environ.get("SONET_TC", "1") != "0" and len(ls) == 2
+                and ls[0].conv.in_channels >= 3 + 32
+                and all(l.conv.out_channels == 512 and l.activation == 'relu' for l in ls)
+                and 2 <= K <= 16 and M * K <= 2304)
+
+    def _tc_params(self):
+        """Layer 1 split by linearity into the per-node GEMM of its feature columns (a generic
+        wgmma blob) and (W1d | shift1) [512,4]; layer 2 as the fused kernel's weight stream.
+        Re-packed only when a parameter changes."""
+        folded = [l._folded.get(l._conv_weight2d(), l.conv.bias,
+                                l.norm if l.normalization == 'batch' else None, transpose=False)
+                  for l in self.layers]
+        key = tuple(l._folded.version for l in self.layers) + \
+            tuple(w.data_ptr() for w, _ in folded)
+        if getattr(self, "_tc_key", None) != key:
+            (w1, s1), (w2, s2) = folded
+            dev = w1.device
+            yblob, yinv = ops.pointwise_tc_pack(w1[:, 3:])
+            blob2, inv2 = ops.knn_mlp_tc_pack(w2)
+            self._tc_pack = dict(yblob=yblob.to(dev), yinv=yinv,
+                                 w1=torch.cat((w1[:, :3], s1[:, None]), dim=1).contiguous(),
+                                 blob2=blob2.to(dev), inv2=inv2, shift2=s2.contiguous())
+            self._tc_key = key
+        return self._tc_pack
+
+    def _tc_forward(self, coord, center, knn_I, K, x):
+        """x [B,C,M] -> knn_feature [B,512,M]: Y = W1f x once per node, then one fused launch."""
+        pk = self._tc_params()
+        y = ops.pointwise_layer_tc(x, pk["yblob"], pk["yinv"], None, 512, False)
+        return ops.knn_mlp_tc(coord, center, knn_I, K, y, pk["w1"], pk["blob2"], pk["inv2"],
+                              pk["shift2"])
+
     def forward_pooled(self, coordinate, pool, precomputed_knn_I, K, center_type, epoch=None,
                        owner=None):
         """forward() for the fused-pool path: `pool` = (keys [B,C,M] i32, p0 [B,C]) as left by
@@ -509,6 +545,10 @@ class KNNModule(nn.Module):
             knn_I = precomputed_knn_I.contiguous()
         else:
             knn_I = ops.node_knn(coord, K)
+        if self._tc_fused(K, M):
+            center, _, masked_max = ops.knn_assemble_pool(coord, keys, p0, knn_I, K, center_type,
+                                                          owner=owner, want_x_aug=False)
+            return center, self._tc_forward(coord, center, knn_I, K, masked_max), masked_max
         center, h, masked_max = ops.knn_assemble_pool(coord, keys, p0, knn_I, K, center_type,
                                                       owner=owner)
         for layer in self.layers:
@@ -527,6 +567,10 @@ class KNNModule(nn.Module):
             else:
                 knn_I = ops.node_knn(coord, K)
             B, C, M = x.shape
+            if self._tc_fused(K, M):
+                center, _ = ops.knn_assemble(coord, x.contiguous(), knn_I, K, center_type,
+                                             want_x_aug=False)
+                return center, self._tc_forward(coord, center, knn_I, K, x.contiguous())
             center, h = ops.knn_assemble(coord, x.contiguous(), knn_I, K, center_type)
             for layer in self.layers:
                 h = layer.forward_points(h)                     # [B, C', M*K]

@@ -242,8 +242,8 @@ def knn_gather(src, idx, K=None):
     return out
 
 
-def knn_assemble(coord, feat, idx, K, center_type):
-    """-> (center [B,3,M], x_aug [B,3+C,M*K])."""
+def knn_assemble(coord, feat, idx, K, center_type, want_x_aug=True):
+    """-> (center [B,3,M], x_aug [B,3+C,M*K], or None with want_x_aug=False)."""
     _chk(coord, "coordinate", torch.float32)
     _chk(feat, "x", torch.float32)
     _chk(idx, "knn_I", torch.int64)
@@ -252,7 +252,8 @@ def knn_assemble(coord, feat, idx, K, center_type):
     ct = {"avg": 0, "center": 1}[center_type]
     with torch.cuda.device(feat.device):
         center = torch.empty((B, 3, M), dtype=torch.float32, device=feat.device)
-        x_aug = torch.empty((B, 3 + C, M * K), dtype=torch.float32, device=feat.device)
+        x_aug = torch.empty((B, 3 + C, M * K), dtype=torch.float32, device=feat.device) \
+            if want_x_aug else None
         _call("sonet_knn_assemble_f32", _C.ptr(coord), _C.ptr(feat), _C.ptr(idx), B, C, M, int(K),
               Kstride, ct, _C.ptr(center), _C.ptr(x_aug), _stream(feat))
     return center, x_aug
@@ -467,6 +468,45 @@ def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=N
     return out
 
 
+def knn_mlp_tc_pack(W2):
+    """W2 [512,512] folded fp32 (any device) -> (blob uint8 CPU tensor, inv_scale float): the
+    layer-2 weight stream of knn_mlp_tc."""
+    import ctypes
+    lib = _C.lib()
+    Wc = W2.detach().to("cpu", torch.float32).contiguous()
+    if tuple(Wc.shape) != (512, 512):
+        raise RuntimeError("knn_mlp_tc_pack: expected W2 [512,512], got %s" % (tuple(Wc.shape),))
+    blob = torch.zeros(int(lib.sonet_knn_mlp_tc_blob_bytes()), dtype=torch.uint8)
+    inv = ctypes.c_float(0.0)
+    _C.check(lib.sonet_knn_mlp_tc_pack(Wc.data_ptr(), blob.data_ptr(), ctypes.addressof(inv)),
+             "sonet_knn_mlp_tc_pack")
+    return blob, float(inv.value)
+
+
+def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2):
+    """The KNN module's layer 1 (from the per-node Y = W1f x [B,512,M]) + layer 2 + max over the
+    K neighbours in one wgmma kernel. coord, center [B,3,M]; idx [B,M,K'] i64; w1 [512,4] =
+    (W1d | shift1); shift2 [512] -> knn_feature_1 [B,512,M]."""
+    _chk(coord, "coordinate", torch.float32)
+    _chk(center, "center", torch.float32)
+    _chk(idx, "knn_I", torch.int64)
+    _chk(Y, "Y", torch.float32)
+    _chk(w1, "w1", torch.float32)
+    _chk(blob, "blob", torch.uint8)
+    _chk(shift2, "shift2", torch.float32)
+    B, _, M = coord.shape
+    if tuple(Y.shape) != (B, 512, M) or tuple(w1.shape) != (512, 4) or shift2.numel() != 512 \
+            or tuple(idx.shape[:2]) != (B, M):
+        raise RuntimeError("knn_mlp_tc: unexpected shapes coord %s Y %s w1 %s idx %s"
+                           % (tuple(coord.shape), tuple(Y.shape), tuple(w1.shape), tuple(idx.shape)))
+    with torch.cuda.device(coord.device):
+        out = torch.empty((B, 512, M), dtype=torch.float32, device=coord.device)
+        _call("sonet_knn_mlp_tc_forward", _C.ptr(coord), _C.ptr(center), _C.ptr(idx), B, M, int(K),
+              idx.shape[2], _C.ptr(Y), _C.ptr(w1), _C.ptr(blob), float(inv_scale), _C.ptr(shift2),
+              _C.ptr(out), _stream(coord))
+    return out
+
+
 def som_sort_decenter(x, sn, cluster_mean, min_idx_i32, count, k):
     """-> (x_sorted [B,3(+3),kN], node_sorted [B,kN] i32, pos0 [B] i32): the stacked copies grouped
     by node, decentred (models/networks.py:168-172) — input of pointresnet_tc_pool."""
@@ -574,9 +614,9 @@ def pool_finalize(keys, p0, owner=None):
     return out
 
 
-def knn_assemble_pool(coord, keys, p0, idx, K, center_type, owner=None):
+def knn_assemble_pool(coord, keys, p0, idx, K, center_type, owner=None, want_x_aug=True):
     """knn_assemble reading the per-node maxima from the pool keys (pool_finalize folded in).
-    -> (center [B,3,M], x_aug [B,3+C,M*K], masked_max [B,C,M])."""
+    -> (center [B,3,M], x_aug [B,3+C,M*K] or None with want_x_aug=False, masked_max [B,C,M])."""
     _chk(coord, "coordinate", torch.float32)
     _chk(keys, "pool_keys", torch.int32)
     _chk(p0, "p0", torch.float32)
@@ -587,7 +627,8 @@ def knn_assemble_pool(coord, keys, p0, idx, K, center_type, owner=None):
     dev = keys.device
     with torch.cuda.device(dev):
         center = torch.empty((B, 3, M), dtype=torch.float32, device=dev)
-        x_aug = torch.empty((B, 3 + C, M * K), dtype=torch.float32, device=dev)
+        x_aug = torch.empty((B, 3 + C, M * K), dtype=torch.float32, device=dev) \
+            if want_x_aug else None
         mm = torch.empty((B, C, M), dtype=torch.float32, device=dev)
         _call("sonet_knn_assemble_pool_f32", _C.ptr(coord), _C.ptr(keys), _C.ptr(p0), _C.ptr(idx), B,
               C, M, int(K), Kstride, ct, _C.ptr(mm), _C.ptr(center), _C.ptr(x_aug), _stream(keys))
