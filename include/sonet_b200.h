@@ -419,6 +419,13 @@ int sonet_pointwise_tc_forward(const float* x0, int C0, const float* x1, int C1,
                                const void* blob, float inv_scale, const float* shift, int Cout,
                                int relu, const float* addend, const int32_t* gidx, int G,
                                float* out, sonet_stream_t stream);
+/* sonet_pointwise_tc_forward storing the point-major transpose: out [B,P,Cout], out[b,p,co] = the
+ * value sonet_pointwise_tc_forward writes at [b,co,p], bit for bit. Consumers that gather whole
+ * rows (the KNN module's per-node Y) read them as contiguous vectors. */
+int sonet_pointwise_tc_forward_rows(const float* x0, int C0, const float* x1, int C1, int B, int P,
+                                    const void* blob, float inv_scale, const float* shift, int Cout,
+                                    int relu, const float* addend, const int32_t* gidx, int G,
+                                    float* out, sonet_stream_t stream);
 
 /* ---- KNNModule (3+C -> 512 -> 512, BN + ReLU, max over K) on wgmma, csrc/knn_tc.cu -----------
  * Layer 1 is split by linearity: Y = W1f x [B,512,M] (the C feature columns, computed once per
@@ -427,14 +434,18 @@ int sonet_pointwise_tc_forward(const float* x0, int C0, const float* x1, int C1,
  * over the K neighbours; neither h1 nor h2 is written.
  *   blob_bytes / pack (host pointers): W2 [512,512] folded fp32 -> blob_host, *inv_scale.
  *   forward (device pointers): coord [B,3,M], center [B,3,M] (as sonet_knn_assemble*_f32 writes
- *     it), idx [B,M,Kstride] int64 (first K columns), Y [B,512,M], w1 [512][4] = {W1d[c,0..2],
- *     shift1[c]} (16-byte aligned), shift2 [512] -> out [B,512,M] = knn_feature_1.
+ *     it), idx [B,M,Kstride] int64 (first K columns), Y with element (b, c, n) at
+ *     Y[b*512*M + c*y_cstride + n*y_nstride]: channel-major [B,512,M] (y_cstride = M,
+ *     y_nstride = 1) or node-major [B,M,512] (1, 512; 8-byte aligned, read as float2 pairs, the
+ *     faster layout), w1 [512][4] = {W1d[c,0..2], shift1[c]} (16-byte aligned), shift2 [512]
+ *     -> out [B,512,M] = knn_feature_1. Both Y layouts give bit-identical results.
  *     2 <= K <= 16, M <= 65535. Error envelope of layer 2 as sonet_pointwise_tc_forward. */
 long long sonet_knn_mlp_tc_blob_bytes(void);
 int sonet_knn_mlp_tc_pack(const float* W2, void* blob_host, float* inv_scale);
 int sonet_knn_mlp_tc_forward(const float* coord, const float* center, const int64_t* idx, int B,
-                             int M, int K, int Kstride, const float* Y, const float* w1,
-                             const void* blob, float inv_scale, const float* shift2, float* out,
+                             int M, int K, int Kstride, const float* Y, long long y_cstride,
+                             long long y_nstride, const float* w1, const void* blob,
+                             float inv_scale, const float* shift2, float* out,
                              sonet_stream_t stream);
 
 /* ---- diagnostics -------------------------------------------------------------------------------
@@ -463,13 +474,15 @@ int sonet_debug_pointresnet_tc_pool_timeline(const float* x_sorted, int Cin, int
                                              const int32_t* node_sorted, const int32_t* pos0, int M,
                                              int32_t* pool_keys, float* p0, long long* timeline64,
                                              sonet_stream_t stream);
-/* sonet_knn_mlp_tc_forward with clock64() stamps of CTA 0 in timeline64[128] (device): [126] kernel
- * start, [127] kernel end. */
+/* sonet_knn_mlp_tc_forward with clock64() stamps of CTA 0 in timeline128[128] (device): [126]
+ * kernel start, [127] kernel end, and per consumer warpgroup w and work item i < 15 of the CTA
+ * [64 w + 4 i + phase]: phase 0 item start, 1 first wgmma issued, 2 last wgmma retired, 3 neighbour
+ * max and store done. */
 int sonet_debug_knn_mlp_tc_timeline(const float* coord, const float* center, const int64_t* idx,
                                     int B, int M, int K, int Kstride, const float* Y,
-                                    const float* w1, const void* blob, float inv_scale,
-                                    const float* shift2, float* out, long long* timeline64,
-                                    sonet_stream_t stream);
+                                    long long y_cstride, long long y_nstride, const float* w1,
+                                    const void* blob, float inv_scale, const float* shift2,
+                                    float* out, long long* timeline128, sonet_stream_t stream);
 int sonet_debug_tc_probe(const float* A, const float* Bm, int N, int K, int mode, int layout,
                          int swap_fields, float* D, sonet_stream_t stream);
 

@@ -20,7 +20,9 @@
 //   * producer warp: streams the pre-packed fp16 hi/lo weight images (cp.async.bulk + mbarrier)
 //     through a 4-stage ring shared by both warpgroups;
 //   * epilogue in registers: fused scale/shift (+ gathered addend) + ReLU; eight lanes of a warp
-//     hold eight consecutive points of one channel, so every store fills 32-byte sectors.
+//     hold eight consecutive points of one channel, so every store fills 32-byte sectors. The
+//     point-major store mode (out [B,P,Cout]) writes each thread's column pair as one float2: four
+//     lanes fill one 32-byte sector of a row.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -74,6 +76,7 @@ struct Dims {
   long long blob_gstride;   // bytes between the weight blobs of consecutive groups
   long long out_gstride;    // floats between the outputs of consecutive groups (0 when scattering)
   long long out_sstride;    // floats between the partial sums of consecutive K splits
+  int rows_out;             // 1: out is point-major [B, P, Cout] (single group, no split or scatter)
 };
 struct Item {
   int g, tile, nt, sub, kc0;
@@ -294,6 +297,31 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
           const int g = min(max(__ldg(gidx + static_cast<long long>(im.g) * rows + R), 0), d.G - 1);
           arow = addend + static_cast<size_t>(b) * d.Cout * d.G + g;
         }
+        if (d.rows_out) {
+          // point-major: out[R, co], columns (co, co+1) as one float2 when both exist and Cout is
+          // even (8-byte aligned); same values as the channel-major store
+          float* o = out + static_cast<size_t>(R) * d.Cout;
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            if (8 * j >= ns) break;
+            const int co = col0 + 8 * j;
+            float y[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              y[e] = fmaf(acc[4 * j + 2 * rr + e], inv_w,
+                          (shift != nullptr && co + e < d.Cout) ? __ldg(shift + co + e) : 0.f);
+              if (arow != nullptr && co + e < d.Cout) y[e] += __ldg(arow + static_cast<size_t>(co + e) * d.G);
+              y[e] = fmaxf(y[e], floor_v);
+            }
+            if (co + 1 < d.Cout && (d.Cout & 1) == 0)
+              *reinterpret_cast<float2*>(o + co) = make_float2(y[0], y[1]);
+            else
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                if (co + e < d.Cout) o[co + e] = y[e];
+          }
+          continue;
+        }
         float* o = out + obase + static_cast<size_t>(b) * d.Cout * d.P_out + po;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
@@ -396,8 +424,8 @@ extern "C" int sonet_pointwise_tc_pack_groups(const float* W, int G, int Cout, i
   return SONET_OK;
 }
 
-struct TcExt {   // grouped / split-K / scatter launch options (defaults = the plain layer)
-  int groups = 1, splits = 1, scat_w = 0, P_out = 0, conv_w = 0;
+struct TcExt {   // grouped / split-K / scatter / point-major launch options (defaults = the plain layer)
+  int groups = 1, splits = 1, scat_w = 0, P_out = 0, conv_w = 0, rows_out = 0;
   const float* inv_ptr = nullptr;
   const float* act_ptr = nullptr;
   long long blob_gstride = 0, out_gstride = 0, out_sstride = 0;
@@ -443,6 +471,10 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   d.blob_gstride = ext.blob_gstride;
   d.out_gstride = ext.out_gstride;
   d.out_sstride = ext.out_sstride;
+  d.rows_out = ext.rows_out;
+  SONET_REQUIRE(!ext.rows_out || (ext.groups == 1 && ext.splits == 1 && ext.scat_w == 0 &&
+                                  ext.conv_w == 0),
+                "pointwise_tc: the point-major store needs one group, no split and no scatter");
   const long long rows = static_cast<long long>(B) * P;
   d.row_tiles = static_cast<int>((rows + TILE - 1) / TILE);
   const long long items = static_cast<long long>(d.row_tiles) * d.ntiles * ext.groups * ext.splits;
@@ -462,6 +494,17 @@ extern "C" int sonet_pointwise_tc_forward(const float* x0, int C0, const float* 
                                           float* out, sonet_stream_t stream) {
   return launch_pointwise_tc(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
                              out, nullptr, stream);
+}
+
+extern "C" int sonet_pointwise_tc_forward_rows(const float* x0, int C0, const float* x1, int C1,
+                                               int B, int P, const void* blob, float inv_scale,
+                                               const float* shift, int Cout, int relu,
+                                               const float* addend, const int32_t* gidx, int G,
+                                               float* out, sonet_stream_t stream) {
+  TcExt e;
+  e.rows_out = 1;
+  return launch_pointwise_tc(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
+                             out, nullptr, stream, e);
 }
 
 namespace sonet {

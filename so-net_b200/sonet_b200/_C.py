@@ -107,11 +107,16 @@ _SIGNATURES = {
                                    c_int, c_void_p, c_void_p],
     "sonet_knn_mlp_tc_blob_bytes": [],
     "sonet_knn_mlp_tc_pack": [c_void_p, c_void_p, c_void_p],
+    "sonet_pointwise_tc_forward_rows": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
+                                        ctypes.c_float, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                        c_int, c_void_p, c_void_p],
     "sonet_knn_mlp_tc_forward": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
-                                 c_void_p, c_void_p, ctypes.c_float, c_void_p, c_void_p, c_void_p],
+                                 ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p,
+                                 ctypes.c_float, c_void_p, c_void_p, c_void_p],
     "sonet_debug_knn_mlp_tc_timeline": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
-                                        c_void_p, c_void_p, c_void_p, ctypes.c_float, c_void_p,
-                                        c_void_p, c_void_p, c_void_p],
+                                        c_void_p, ctypes.c_longlong, ctypes.c_longlong, c_void_p,
+                                        c_void_p, ctypes.c_float, c_void_p, c_void_p, c_void_p,
+                                        c_void_p],
     "sonet_debug_pointresnet_tc_timeline": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                             c_void_p, c_void_p, c_void_p],
     "sonet_debug_pointwise_tc_timeline": [c_void_p, c_int, c_int, c_int, c_void_p, ctypes.c_float,

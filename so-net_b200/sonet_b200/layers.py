@@ -522,11 +522,12 @@ class KNNModule(nn.Module):
         return self._tc_pack
 
     def _tc_forward(self, coord, center, knn_I, K, x):
-        """x [B,C,M] -> knn_feature [B,512,M]: Y = W1f x once per node, then one fused launch."""
+        """x [B,C,M] -> knn_feature [B,512,M]: Y = W1f x once per node, stored node-major so the
+        fused kernel gathers each neighbour's channels as contiguous pairs, then one fused launch."""
         pk = self._tc_params()
-        y = ops.pointwise_layer_tc(x, pk["yblob"], pk["yinv"], None, 512, False)
-        return ops.knn_mlp_tc(coord, center, knn_I, K, y, pk["w1"], pk["blob2"], pk["inv2"],
-                              pk["shift2"])
+        y = ops.pointwise_layer_tc(x, pk["yblob"], pk["yinv"], None, 512, False, rows=True)
+        return ops.knn_mlp_tc(coord, center, knn_I, K, y.transpose(1, 2), pk["w1"], pk["blob2"],
+                              pk["inv2"], pk["shift2"])
 
     def forward_pooled(self, coordinate, pool, precomputed_knn_I, K, center_type, epoch=None,
                        owner=None):

@@ -449,8 +449,10 @@ def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, group
     return out
 
 
-def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=None, gidx=None):
-    """wgmma variant of pointwise_layer: x0 [B,C0,P] (+ x1) -> [B,cout,P]."""
+def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=None, gidx=None,
+                       rows=False):
+    """wgmma variant of pointwise_layer: x0 [B,C0,P] (+ x1) -> [B,cout,P], or with rows=True the
+    same values point-major, [B,P,cout]."""
     _chk(x0, "x0", torch.float32)
     _chk(x1, "x1", torch.float32, optional=True)
     _chk(blob, "blob", torch.uint8)
@@ -461,10 +463,16 @@ def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=N
     C1 = 0 if x1 is None else x1.shape[1]
     G = 0 if addend is None else addend.shape[2]
     with torch.cuda.device(x0.device):
-        out = torch.empty((B, cout, P), dtype=torch.float32, device=x0.device)
-        _call("sonet_pointwise_tc_forward", _C.ptr(x0), C0, _C.ptr(x1), C1, B, P, _C.ptr(blob),
-              float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)), _C.ptr(addend),
-              _C.ptr(gidx), G, _C.ptr(out), _stream(x0))
+        if rows:
+            out = torch.empty((B, P, cout), dtype=torch.float32, device=x0.device)
+            _call("sonet_pointwise_tc_forward_rows", _C.ptr(x0), C0, _C.ptr(x1), C1, B, P,
+                  _C.ptr(blob), float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)),
+                  _C.ptr(addend), _C.ptr(gidx), G, _C.ptr(out), _stream(x0))
+        else:
+            out = torch.empty((B, cout, P), dtype=torch.float32, device=x0.device)
+            _call("sonet_pointwise_tc_forward", _C.ptr(x0), C0, _C.ptr(x1), C1, B, P, _C.ptr(blob),
+                  float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)), _C.ptr(addend),
+                  _C.ptr(gidx), G, _C.ptr(out), _stream(x0))
     return out
 
 
@@ -486,11 +494,16 @@ def knn_mlp_tc_pack(W2):
 def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2):
     """The KNN module's layer 1 (from the per-node Y = W1f x [B,512,M]) + layer 2 + max over the
     K neighbours in one wgmma kernel. coord, center [B,3,M]; idx [B,M,K'] i64; w1 [512,4] =
-    (W1d | shift1); shift2 [512] -> knn_feature_1 [B,512,M]."""
+    (W1d | shift1); shift2 [512] -> knn_feature_1 [B,512,M]. Y is [B,512,M] either contiguous or
+    the channel-fastest view y.transpose(1, 2) of a contiguous [B,M,512] (pointwise_layer_tc(...,
+    rows=True)); the kernel reads the latter as float2 pairs, with bit-identical results."""
     _chk(coord, "coordinate", torch.float32)
     _chk(center, "center", torch.float32)
     _chk(idx, "knn_I", torch.int64)
-    _chk(Y, "Y", torch.float32)
+    if Y.dim() == 3 and not Y.is_contiguous() and Y.transpose(1, 2).is_contiguous():
+        _chk(Y.transpose(1, 2), "Y", torch.float32)
+    else:
+        _chk(Y, "Y", torch.float32)
     _chk(w1, "w1", torch.float32)
     _chk(blob, "blob", torch.uint8)
     _chk(shift2, "shift2", torch.float32)
@@ -502,8 +515,8 @@ def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2):
     with torch.cuda.device(coord.device):
         out = torch.empty((B, 512, M), dtype=torch.float32, device=coord.device)
         _call("sonet_knn_mlp_tc_forward", _C.ptr(coord), _C.ptr(center), _C.ptr(idx), B, M, int(K),
-              idx.shape[2], _C.ptr(Y), _C.ptr(w1), _C.ptr(blob), float(inv_scale), _C.ptr(shift2),
-              _C.ptr(out), _stream(coord))
+              idx.shape[2], _C.ptr(Y), Y.stride(1), Y.stride(2), _C.ptr(w1), _C.ptr(blob),
+              float(inv_scale), _C.ptr(shift2), _C.ptr(out), _stream(coord))
     return out
 
 
