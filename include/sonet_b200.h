@@ -464,11 +464,17 @@ int sonet_debug_pointresnet_tc_timeline(const float* x, int Cin, int B, int P, c
 int sonet_debug_pointwise_tc_timeline(const float* x0, int C0, int B, int P, const void* blob,
                                       float inv_scale, int Cout, float* out, long long* timeline128,
                                       sonet_stream_t stream);
-/* Cycles for `iters` back-to-back M=64 x N x 16 fp16 wgmmas issued by one warpgroup (N = 64, 96,
- * 128 or 256), A and B from shared memory (no-swizzle K-major, 8-row-group stride `sbo`); mode must
- * be 0. */
+/* Cycles for `iters` back-to-back M=64 x N x 16 fp16 wgmmas issued by one warpgroup, B from shared
+ * memory (no-swizzle K-major, 8-row-group stride `sbo`). mode 0: A from shared memory too, N = 64,
+ * 96, 128 or 256; mode 1: A from registers, N = 96, 128 or 256. */
 int sonet_debug_tc_mma_rate(int mode, int N, int sbo, int iters, long long* cycles,
                             sonet_stream_t stream);
+/* sonet_pointresnet_tc_pool_forward with clock64() stamps of CTA 0 in timeline64[128] (device):
+ * [126] kernel start, [127] kernel end, and per consumer warpgroup w and tile t < 6 of the CTA
+ * [64 w + 10 t + phase]: phase 0 tile start, 1 act0 written, 2 layer 1 retired, 3 layer-2 epilogue
+ * done, 4 + 2c layer-3 chunk c's last wgmma retired, 5 + 2c its pool epilogue done (c = 0..2).
+ * [64 w + 60]: cycles warp 4w spent blocked on weight stages over all its tiles. Other slots are
+ * not written. */
 int sonet_debug_pointresnet_tc_pool_timeline(const float* x_sorted, int Cin, int B, int P,
                                              const void* blob, const float* fparams,
                                              const int32_t* node_sorted, const int32_t* pos0, int M,

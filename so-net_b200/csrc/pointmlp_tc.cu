@@ -24,8 +24,13 @@
 //     pre-scaled per layer by a power of two (undone exactly in the epilogue FMA) so their lo
 //     halves stay normal fp16 numbers; activations saturate at the fp16 range (65504) in the conversion;
 //   * weights (B operand, K-major no-swizzle core-matrix images packed once by the host) stream
-//     L2 -> shared memory through a 5-slot ring (cp.async.bulk + mbarrier), 25 stages per tile:
-//     layer 1 (N=128), four layer-2 K slabs (N=256), 4 chunks x 5 K slabs of layer 3 (N=96).
+//     L2 -> shared memory through a 5-slot ring (cp.async.bulk + mbarrier), 20 stages per tile:
+//     layer 1 (N=128), four layer-2 K slabs (N=256), 3 chunks x 5 K slabs of layer 3 (N=128).
+//     The blob keeps layer 3 as 96-row chunks; the producer assembles each 128-row stage from two
+//     of them with four bulk copies (an 8-row band of an image is one contiguous 1 KB range).
+//     N=128 chunks instead of 96 cut the drains and pool epilogues per tile from 4 to 3 and keep
+//     the tensor pipe busier while a single warpgroup issues (measured on an H100 80GB HBM3 from
+//     registers: 115 cycles per m64n128k16 against the ideal 64, 99 per m64n96k16 against 48).
 //     Every consumer warp releases a slot as soon as the wgmmas that read it have retired;
 //   * shared memory: 2 x 16 KB act0 images + 5 x 32 KB weight slots + W0 and the four shift
 //     vectors = 197 KB (a sixth slot would not leave room for the shifts);
@@ -39,9 +44,11 @@
 //     With the earlier column-at-a-time pool epilogue, at 700 W, both took 1.81-1.83 ms. With the
 //     one below, at 400 W, ping-pong took ~3 % fewer SM cycles but ran at a lower clock, for < 1 %
 //     more clouds/s. That does not pay for the turn protocol, so free drift stays;
-//   * the pool epilogue runs the shuffle reductions of all 24 columns interleaved before lanes 0-3
-//     issue the atomics: one column at a time, each a chain of 3 dependent shuffles behind its own
-//     branch, it was latency-bound and cost ~25 % of the kernel's cycles.
+//   * the pool epilogue reduces the 8 lanes that share a thread's columns by reduce-scatter (28
+//     shuffles for 32 columns, where a butterfly per column takes 96), and every lane then issues
+//     the atomics of its 4 finished columns. At cfg-2 on an H100 80GB HBM3 (400 W) a chunk's
+//     epilogue takes ~1.9 k cycles, as the 24-column butterfly of the N=96 chunks did; the
+//     butterfly over 32 columns took ~3.2 k.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -57,12 +64,18 @@ constexpr int TILE = 128;                                            // points p
 constexpr int SLOT_BYTES = 32768, NSLOT = 5;
 constexpr int W1_BYTES = 2 * C1 * C0 * 2;                            // hi + lo images, 32 KB
 constexpr int L2_STAGES = 4, L2_KT = 32;                             // [256 rows x 32 k] per stage
-constexpr int L3_CHUNKS = 4, L3_N = 96, L3_KSTAGES = 5, L3_KT = 64;  // [96 rows x 64 k] per stage
+constexpr int L3_KSTAGES = 5, L3_KT = 64;                            // K slabs of layer 3
 constexpr int L2_STAGE_BYTES = C2 * L2_KT * 2 * 2;                   // 32768
-constexpr int L3_STAGE_BYTES = L3_N * L3_KT * 2 * 2;                 // 24576
-constexpr int STAGES_PER_TILE = 1 + L2_STAGES + L3_CHUNKS * L3_KSTAGES;  // 25
-constexpr int BLOB_BYTES =
-    W1_BYTES + L2_STAGES * L2_STAGE_BYTES + L3_CHUNKS * L3_KSTAGES * L3_STAGE_BYTES;  // 655360
+// layer 3 in the blob: 4 chunks of 96 rows x 5 K slabs, each stage [96 rows x 64 k] hi | lo
+constexpr int L3B_CHUNKS = 4, L3B_N = 96;
+constexpr int L3B_HALF = L3B_N * L3_KT * 2;                          // 12288
+constexpr int L3B_OFF = W1_BYTES + L2_STAGES * L2_STAGE_BYTES;
+constexpr int BLOB_BYTES = L3B_OFF + L3B_CHUNKS * L3_KSTAGES * 2 * L3B_HALF;  // 655360
+// layer 3 in shared memory: 3 chunks of 128 rows, each stage [128 rows x 64 k] hi | lo
+constexpr int L3_CHUNKS = 3, L3_N = 128;
+constexpr int L3_HALF = L3_N * L3_KT * 2;                            // 16384
+constexpr int L3_ROW = L3_KT * 2;   // bytes per row of an image: an 8-row band is 1 KB contiguous
+constexpr int STAGES_PER_TILE = 1 + L2_STAGES + L3_CHUNKS * L3_KSTAGES;  // 20
 constexpr int NFP = C0 * 6 + C0 + C1 + C2 + C3 + 4;   // W0 | shift0..3 | 1/wscale1..3 (floats)
 // warpgroups 0-1 consume (64 points each), warpgroup 2 produces; registers per thread after the
 // hand-over: 2 * 128 * 240 + 128 * 24 = 64512, the launch's 168 x 384
@@ -77,11 +90,17 @@ constexpr int NFP_SMEM = C0 * 6 + C0 + C1 + C2 + C3;
 constexpr int OFF_FP = OFF_RING + NSLOT * SLOT_BYTES;
 constexpr int OFF_BAR = OFF_FP + NFP_SMEM * 4;
 constexpr int NBAR = 2 * NSLOT;
-constexpr int SMEM_BYTES = OFF_BAR + NBAR * 8;         // 201552 (the opt-in limit is 232448)
+constexpr int OFF_TLW = OFF_BAR + NBAR * 8;            // [2] blocked cycles (debug timeline)
+constexpr int SMEM_BYTES = OFF_TLW + 2 * 8;            // 201568 (the opt-in limit is 232448)
+// debug timeline of CTA 0, per consumer warpgroup w: [64 w + TL_PHASES t + phase] for its tiles
+// t < TL_TILES, [64 w + TL_WAIT] the cycles warp 4w spent blocked on `full` over all its tiles
+constexpr int TL_PHASES = 4 + 2 * L3_CHUNKS, TL_TILES = 60 / TL_PHASES, TL_WAIT = 60;
 
-__host__ __device__ constexpr int stage_bytes(int s) {
-  return s == 0 ? W1_BYTES : (s <= L2_STAGES ? L2_STAGE_BYTES : L3_STAGE_BYTES);
-}
+// every stage fills exactly one slot
+static_assert(W1_BYTES == SLOT_BYTES && L2_STAGE_BYTES == SLOT_BYTES && 2 * L3_HALF == SLOT_BYTES,
+              "one weight stage per slot");
+static_assert(L3_CHUNKS * L3_N == C3 && L3B_CHUNKS * L3B_N == C3 && L3B_N < L3_N && L3_N <= 2 * L3B_N,
+              "a shared-memory chunk spans exactly two blob chunks");
 }  // namespace pm
 
 // POOL variant (the classifier / auto-encoder path): the input rows are the stacked copies SORTED
@@ -102,7 +121,8 @@ struct PoolArgs {
   int M;
 };
 
-template <bool POOL>
+// DBG: the debug entry points' build, which also stamps the phase timeline of CTA 0
+template <bool POOL, bool DBG>
 __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     pointresnet_tc_kernel(const float* __restrict__ x_in, int Cin, int B, int P,
                           const unsigned char* __restrict__ blob, const float* __restrict__ fparams,
@@ -138,15 +158,28 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
       uint32_t q = 0;
 #pragma unroll 1
       for (int t = 0; t < my_tiles; ++t) {
-        uint32_t off = 0;
 #pragma unroll 1
         for (int s = 0; s < STAGES_PER_TILE; ++s, ++q) {
           const uint32_t slot = q % NSLOT, use = q / NSLOT;
           if (use > 0) tc::mbar_wait_relaxed(&empty[slot], (use - 1) & 1, 100 + s);
-          const uint32_t bytes = stage_bytes(s);
-          mbar_arrive_expect_tx(&full[slot], bytes);
-          bulk_g2s(smem + OFF_RING + slot * SLOT_BYTES, blob + off, bytes, &full[slot]);
-          off += bytes;
+          unsigned char* dst = smem + OFF_RING + slot * SLOT_BYTES;
+          mbar_arrive_expect_tx(&full[slot], SLOT_BYTES);
+          if (s <= L2_STAGES) {   // layer 1, then layer 2's K slabs: one blob stage each
+            bulk_g2s(dst, blob + static_cast<uint32_t>(s) * SLOT_BYTES, SLOT_BYTES, &full[slot]);
+          } else {
+            // layer-3 stage (nc, kc) = rows [128 nc, 128 nc + 128) of K slab kc: the tail of blob
+            // chunk oc from row r, then the head of chunk oc + 1, in the hi and the lo image
+            const int nc = (s - 1 - L2_STAGES) / L3_KSTAGES, kc = (s - 1 - L2_STAGES) % L3_KSTAGES;
+            const int oc = L3_N * nc / L3B_N, r = L3_N * nc - L3B_N * oc;
+            const uint32_t na = (L3B_N - r) * L3_ROW;
+            const unsigned char* src = blob + L3B_OFF + (oc * L3_KSTAGES + kc) * 2 * L3B_HALF + r * L3_ROW;
+            const unsigned char* src1 = blob + L3B_OFF + ((oc + 1) * L3_KSTAGES + kc) * 2 * L3B_HALF;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              bulk_g2s(dst + h * L3_HALF, src + h * L3B_HALF, na, &full[slot]);
+              bulk_g2s(dst + h * L3_HALF + na, src1 + h * L3B_HALF, L3_HALF - na, &full[slot]);
+            }
+          }
         }
       }
     }
@@ -169,10 +202,25 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     const int r0 = 16 * (warp & 3) + (lane >> 2);
     const int cq = 2 * (lane & 3);
     uint32_t q = 0;   // weight stages consumed
+    // clock64 stamps (debug entry points only): phase 0 tile start, 1 act0 written, 2 layer 1
+    // retired, 3 layer-2 epilogue done, 4 + 2c layer-3 chunk c's last wgmma retired, 5 + 2c its
+    // epilogue done
+    // (pool variant only: next to the plain variant's stores the pointer would spill)
+    long long* stamp = (POOL && DBG && blockIdx.x == 0 && tw == 0) ? dbg + 64 * wg : nullptr;
+    int t = 0;
+    // blocked cycles add up in shared memory: a register next to act2 spills, a global
+    // read-modify-write puts an L2 round trip behind every stage
+    long long* full_wait = reinterpret_cast<long long*>(smem + OFF_TLW) + wg;
+    if (stamp != nullptr) *full_wait = 0;
+    auto mark = [&](int phase) {
+      if (stamp != nullptr && t < TL_TILES) stamp[TL_PHASES * t + phase] = clock64();
+    };
 
     auto stage_wait = [&]() -> uint32_t {
       const uint32_t slot = q % NSLOT;
+      const long long w0 = stamp != nullptr ? clock64() : 0;
       tc::mbar_wait_bounded(&full[slot], (q / NSLOT) & 1, 1);
+      if (stamp != nullptr) *full_wait += clock64() - w0;
       return ring_a + slot * SLOT_BYTES;
     };
     auto stage_release = [&](uint32_t qq) {
@@ -197,10 +245,11 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     };
 
 #pragma unroll 1
-    for (int t = 0; t < my_tiles; ++t) {
+    for (; t < my_tiles; ++t) {
       const int tile = blockIdx.x + t * gridDim.x;
       const int b = tile / tiles_per_cloud;
       const int jbase = (tile - b * tiles_per_cloud) * TILE + wg * 64;   // first point of this warpgroup
+      mark(0);
 
       // ---- layer 0 on CUDA cores: point m, channels [32 half, 32 half + 32) ----
       {
@@ -234,6 +283,19 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
         // act0 writes of this warpgroup -> its wgmmas
         tc::fence_proxy_async();
         tc::named_sync(1 + wg, 128);
+        mark(1);
+      }
+
+      // this thread's rows in the layer-3 epilogue (loaded here, where few registers are live)
+      int nd[2] = {-1, -1};
+      bool is_p0[2] = {false, false};
+      const bool valid0 = jbase + r0 < P, valid1 = jbase + r0 + 8 < P;
+      if (POOL) {
+        const int p0row = __ldg(pool.pos0 + b);
+        if (valid0) nd[0] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0);
+        if (valid1) nd[1] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0 + 8);
+        is_p0[0] = valid0 && jbase + r0 == p0row;
+        is_p0[1] = valid1 && jbase + r0 + 8 == p0row;
       }
 
       // ---- layer 1: D1[64 x 128] = act0[64 x 64] * W1^T, A from shared memory ----
@@ -256,6 +318,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
         }
         tc::wg_commit();
         tc::wg_wait<0>();
+        mark(2);
         stage_release(q++);
         to_frags(acc, C1 / 16, inv1, sh1, a1_hi, a1_lo);
       }
@@ -287,24 +350,15 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
         tc::wg_wait<0>();
         stage_release(q - 1);
         to_frags(acc, C2 / 16, inv2, sh2, a2_hi, a2_lo);
+        mark(3);
       }
 
-      // ---- layer 3: D3[64 x 384] = cat(act0, act2)[64 x 320] * W3^T, 4 chunks of N=96; bare ----
-      int nd[2] = {-1, -1};
-      bool is_p0[2] = {false, false};
-      const bool valid0 = jbase + r0 < P, valid1 = jbase + r0 + 8 < P;
-      if (POOL) {
-        const int p0row = __ldg(pool.pos0 + b);
-        if (valid0) nd[0] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0);
-        if (valid1) nd[1] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0 + 8);
-        is_p0[0] = valid0 && jbase + r0 == p0row;
-        is_p0[1] = valid1 && jbase + r0 + 8 == p0row;
-      }
+      // ---- layer 3: D3[64 x 384] = cat(act0, act2)[64 x 320] * W3^T, 3 chunks of N=128; bare ----
 #pragma unroll 1
       for (int nc = 0; nc < L3_CHUNKS; ++nc) {
-        float acc[48];
+        float acc[64];
 #pragma unroll
-        for (int i = 0; i < 48; ++i) acc[i] = 0.f;
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
         // K slab 0 = act0 (shared memory), slabs 1-4 = act2 K blocks 4(kc-1) .. 4(kc-1)+3 (registers)
 #pragma unroll
         for (int kc = 0; kc < L3_KSTAGES; ++kc) {
@@ -313,18 +367,18 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {
             const uint64_t bh = tc::smem_desc(sb + ks * 256, 128, 1024),
-                           bl = tc::smem_desc(sb + L3_STAGE_BYTES / 2 + ks * 256, 128, 1024);
+                           bl = tc::smem_desc(sb + L3_HALF + ks * 256, 128, 1024);
             if (kc == 0) {
               const uint64_t ah = tc::smem_desc(act0_a + ks * 256, 128, 1024),
                              al = tc::smem_desc(act0_a + ACT0_HALF + ks * 256, 128, 1024);
-              tc::wgmma_f16_n96(acc, ah, bh, 1);
-              tc::wgmma_f16_n96(acc, al, bh, 1);
-              tc::wgmma_f16_n96(acc, ah, bl, 1);
+              tc::wgmma_f16_n128(acc, ah, bh, 1);
+              tc::wgmma_f16_n128(acc, al, bh, 1);
+              tc::wgmma_f16_n128(acc, ah, bl, 1);
             } else {
               const int kk = 4 * (kc - 1) + ks;
-              tc::wgmma_f16_rs_n96(acc, a2_hi[kk], bh, 1);
-              tc::wgmma_f16_rs_n96(acc, a2_lo[kk], bh, 1);
-              tc::wgmma_f16_rs_n96(acc, a2_hi[kk], bl, 1);
+              tc::wgmma_f16_rs_n128(acc, a2_hi[kk], bh, 1);
+              tc::wgmma_f16_rs_n128(acc, a2_lo[kk], bh, 1);
+              tc::wgmma_f16_rs_n128(acc, a2_hi[kk], bl, 1);
             }
           }
           tc::wg_commit();
@@ -333,6 +387,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
           ++q;
         }
         tc::wg_wait<0>();
+        mark(4 + 2 * nc);
         stage_release(q - 1);
 
         const int cbase = L3_N * nc + cq;
@@ -343,7 +398,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
             if (j >= P) continue;
             float* o = out + (static_cast<size_t>(b) * C3 + cbase) * P + j;
 #pragma unroll
-            for (int jn = 0; jn < 12; ++jn, o += 8 * static_cast<size_t>(P))
+            for (int jn = 0; jn < 16; ++jn, o += 8 * static_cast<size_t>(P))
 #pragma unroll
               for (int e = 0; e < 2; ++e)
                 o[e * static_cast<size_t>(P)] =
@@ -359,46 +414,58 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
             const bool in0 = nd[0] == node, in1 = nd[1] == node;
             rem0 &= ~__ballot_sync(FULL, in0);
             rem1 &= ~__ballot_sync(FULL, in1);
-            // the 24 columns' shuffle chains interleaved, then lanes 0-3 issue the reductions;
-            // the key pointer is stepped, not indexed: 24 precomputed 64-bit column offsets would
-            // not fit next to act2
-            float mx[24];
+            // reduce-scatter over the 8 lanes that hold the same 32 columns (lane xor 16, 8, 4):
+            // each step keeps half of the columns and takes the partner's maxima of that half, so
+            // the 32 columns cost 16 + 8 + 4 shuffles (a full butterfly per column costs 96) and
+            // every lane ends with 4 finished columns, slots base .. base + 3 of the thread's 32
+            // (slot s = column 8 (s / 2) + s % 2 + cq of the chunk)
+            const bool b2 = lane & 16, b1 = lane & 8, b0 = lane & 4;
+            float r1[16];
 #pragma unroll
-            for (int c = 0; c < 24; ++c)
-              mx[c] = fmaxf(in0 ? acc[4 * (c >> 1) + (c & 1)] : -INFINITY,
-                            in1 ? acc[4 * (c >> 1) + 2 + (c & 1)] : -INFINITY);
+            for (int c = 0; c < 16; ++c) {
+              const int s = c, u = c + 16;
+              const float vs = fmaxf(in0 ? acc[4 * (s >> 1) + (s & 1)] : -INFINITY,
+                                     in1 ? acc[4 * (s >> 1) + 2 + (s & 1)] : -INFINITY);
+              const float vu = fmaxf(in0 ? acc[4 * (u >> 1) + (u & 1)] : -INFINITY,
+                                     in1 ? acc[4 * (u >> 1) + 2 + (u & 1)] : -INFINITY);
+              r1[c] = fmaxf(b2 ? vu : vs, __shfl_xor_sync(FULL, b2 ? vs : vu, 16));
+            }
+            float r2[8];
 #pragma unroll
-            for (int d = 4; d <= 16; d <<= 1)
+            for (int c = 0; c < 8; ++c)
+              r2[c] = fmaxf(b1 ? r1[c + 8] : r1[c], __shfl_xor_sync(FULL, b1 ? r1[c] : r1[c + 8], 8));
+            float r3[4];
 #pragma unroll
-              for (int c = 0; c < 24; ++c) mx[c] = fmaxf(mx[c], __shfl_xor_sync(FULL, mx[c], d));
-            if (lane < 4) {
-              int32_t* kb = pool.keys + (static_cast<size_t>(b) * C3 + cbase) * pool.M + node;
+            for (int c = 0; c < 4; ++c)
+              r3[c] = fmaxf(b0 ? r2[c + 4] : r2[c], __shfl_xor_sync(FULL, b0 ? r2[c] : r2[c + 4], 4));
+            const int col = cbase + 8 * ((16 * b2 + 8 * b1 + 4 * b0) >> 1);   // slot base's column
+            int32_t* kb = pool.keys + (static_cast<size_t>(b) * C3 + col) * pool.M + node;
 #pragma unroll
-              for (int jn = 0; jn < 12; ++jn, kb += 8 * static_cast<size_t>(pool.M))
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const int bits = __float_as_int(fmaf(mx[2 * jn + e], inv3, sh3[cbase + 8 * jn + e]));
-                  const int key = bits ^ ((bits >> 31) & 0x7fffffff);   // order-preserving float -> int
-                  atomicMax(kb + e * static_cast<size_t>(pool.M), key);
-                }
+            for (int i = 0; i < 4; ++i) {
+              const int dc = 8 * (i >> 1) + (i & 1);
+              const int bits = __float_as_int(fmaf(r3[i], inv3, sh3[col + dc]));
+              const int key = bits ^ ((bits >> 31) & 0x7fffffff);   // order-preserving float -> int
+              atomicMax(kb + dc * static_cast<size_t>(pool.M), key);
             }
           }
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
             if (!is_p0[rr]) continue;   // rare: one row per cloud
 #pragma unroll
-            for (int jn = 0; jn < 12; ++jn)
+            for (int jn = 0; jn < 16; ++jn)
 #pragma unroll
               for (int e = 0; e < 2; ++e)
                 pool.p0[static_cast<size_t>(b) * C3 + cbase + 8 * jn + e] =
                     fmaf(acc[4 * jn + 2 * rr + e], inv3, sh3[cbase + 8 * jn + e]);
           }
         }
+        mark(5 + 2 * nc);
       }
       // the next tile's layer 0 overwrites act0, which this tile's layer-3 wgmmas read: all are
       // complete (wait_group 0 above); the other warps of the warpgroup must be past them too
       tc::named_sync(1 + wg, 128);
     }
+    if (stamp != nullptr) stamp[TL_WAIT] = *full_wait;
   }
   __syncthreads();
   if (dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0) dbg[64 + 63] = clock64();
@@ -433,11 +500,10 @@ extern "C" int sonet_pointresnet_tc_pack(const float* W0, int Cin, const float* 
     off += L2_STAGE_BYTES;
   }
   // layer 3: four 96-row chunks x five K slabs [96 rows x 64 k]
-  for (int nc = 0; nc < L3_CHUNKS; ++nc)
+  for (int nc = 0; nc < L3B_CHUNKS; ++nc)
     for (int kc = 0; kc < L3_KSTAGES; ++kc) {
-      pack_tile(W3, s3, K3, L3_N * nc, L3_N, L3_KT * kc, L3_KT, blob + off,
-                blob + off + L3_STAGE_BYTES / 2);
-      off += L3_STAGE_BYTES;
+      pack_tile(W3, s3, K3, L3B_N * nc, L3B_N, L3_KT * kc, L3_KT, blob + off, blob + off + L3B_HALF);
+      off += 2 * L3B_HALF;
     }
   if (off != static_cast<size_t>(BLOB_BYTES)) SONET_FAIL(SONET_ERR_BAD_ARG, "pack: size mismatch");
   float* f = fparams_host;
@@ -472,7 +538,8 @@ static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const vo
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "pointresnet_tc: needs %d B of shared memory",
                 SMEM_BYTES);
   const int grid = static_cast<int>(std::min<long long>(tiles, sm_count()));
-  auto kern = pool ? pointresnet_tc_kernel<true> : pointresnet_tc_kernel<false>;
+  auto kern = pool ? (dbg ? pointresnet_tc_kernel<true, true> : pointresnet_tc_kernel<true, false>)
+                   : (dbg ? pointresnet_tc_kernel<false, true> : pointresnet_tc_kernel<false, false>);
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   PoolArgs pa = pool ? *pool : PoolArgs{nullptr, nullptr, nullptr, nullptr, 0};
   kern<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(

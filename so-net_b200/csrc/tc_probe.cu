@@ -111,10 +111,10 @@ extern "C" int sonet_debug_tc_probe(const float* A, const float* Bm, int N, int 
   return check_launch("tc_probe");
 }
 
-// ---- MMA rate microbenchmark: `iters` back-to-back M=64 x N x 16 fp16 wgmmas (A and B in shared
-// memory) of one warpgroup ----------------------------------------------------------------------------
+// ---- MMA rate microbenchmark: `iters` back-to-back M=64 x N x 16 fp16 wgmmas of one warpgroup, B in
+// shared memory, A in shared memory (RS = false) or in registers (RS = true) ----------------------
 namespace sonet {
-template <int N>
+template <int N, bool RS>
 __global__ void __launch_bounds__(128, 1)
     tc_rate_kernel(uint32_t sbo, int iters, long long* __restrict__ cycles) {
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -126,10 +126,14 @@ __global__ void __launch_bounds__(128, 1)
   float acc[N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  const uint32_t a[4] = {0x3c003c00u, 0x3c003c00u, 0x3c003c00u, 0x3c003c00u};   // fp16 1.0 pairs
   const long long t0 = clock64();
   tc::wg_fence();
   for (int i = 0; i < iters; ++i) {
-    if constexpr (N == 64) tc::wgmma_f16_n64(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
+    if constexpr (RS && N == 96) tc::wgmma_f16_rs_n96(acc, a, bd + (i & 3) * 16, 1);
+    else if constexpr (RS && N == 128) tc::wgmma_f16_rs_n128(acc, a, bd + (i & 3) * 16, 1);
+    else if constexpr (RS) tc::wgmma_f16_rs_n256(acc, a, bd + (i & 3) * 16, 1);
+    else if constexpr (N == 64) tc::wgmma_f16_n64(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
     else if constexpr (N == 96) tc::wgmma_f16_n96(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
     else if constexpr (N == 128) tc::wgmma_f16_n128(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
     else tc::wgmma_f16_n256(acc, ad + (i & 3) * 16, bd + (i & 3) * 16, 1);
@@ -150,10 +154,13 @@ __global__ void __launch_bounds__(128, 1)
 extern "C" int sonet_debug_tc_mma_rate(int mode, int N, int sbo, int iters, long long* cycles,
                                        sonet_stream_t stream) {
   using namespace sonet;
-  SONET_REQUIRE(mode == 0 && (N == 64 || N == 96 || N == 128 || N == 256) && cycles,
-                "tc_mma_rate: mode 0 with N in {64, 96, 128, 256}");
-  auto kern = N == 64 ? tc_rate_kernel<64> : N == 96 ? tc_rate_kernel<96>
-            : N == 128 ? tc_rate_kernel<128> : tc_rate_kernel<256>;
+  SONET_REQUIRE(cycles && ((mode == 0 && (N == 64 || N == 96 || N == 128 || N == 256)) ||
+                           (mode == 1 && (N == 96 || N == 128 || N == 256))),
+                "tc_mma_rate: mode 0 with N in {64, 96, 128, 256} or mode 1 with N in {96, 128, 256}");
+  auto kern = mode == 1 ? (N == 96 ? tc_rate_kernel<96, true> : N == 128 ? tc_rate_kernel<128, true>
+                                                                       : tc_rate_kernel<256, true>)
+            : N == 64 ? tc_rate_kernel<64, false> : N == 96 ? tc_rate_kernel<96, false>
+            : N == 128 ? tc_rate_kernel<128, false> : tc_rate_kernel<256, false>;
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
   kern<<<1, 128, 64 * 1024, as_stream(stream)>>>(static_cast<uint32_t>(sbo), iters, cycles);
   return check_launch("tc_mma_rate");
