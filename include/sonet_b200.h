@@ -326,7 +326,7 @@ int sonet_chamfer_f32(const float* pred, const float* gt, int B, int Mp, int N, 
  * layers 1-2's outputs in registers as the next layer's wgmma A operand; fp32 parity comes from a
  * 3-product fp16 hi/lo split (see csrc/pointmlp_tc.cu).
  *   pack (host pointers): W0 [64,Cin], W1 [128,64], W2 [256,128], W3 [384,320] row-major with the
- *     eval BatchNorm scale already folded in; shift0..3 = folded bias/BN shift. Writes the bf16
+ *     eval BatchNorm scale already folded in; shift0..3 = folded bias/BN shift. Writes the fp16 hi/lo
  *     K-major core-matrix images streamed by the kernel into blob_host
  *     (sonet_pointresnet_tc_blob_bytes() bytes) and the fp32 side parameters into fparams_host
  *     (sonet_pointresnet_tc_fparam_count() floats).

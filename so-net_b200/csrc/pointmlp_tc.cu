@@ -26,8 +26,7 @@
 //   * weights (B operand, K-major no-swizzle core-matrix images packed once by the host) stream
 //     L2 -> shared memory through a 5-slot ring (cp.async.bulk + mbarrier), 20 stages per tile:
 //     layer 1 (N=128), four layer-2 K slabs (N=256), 3 chunks x 5 K slabs of layer 3 (N=128).
-//     The blob keeps layer 3 as 96-row chunks; the producer assembles each 128-row stage from two
-//     of them with four bulk copies (an 8-row band of an image is one contiguous 1 KB range).
+//     The blob is these 20 stages of 32 KB in that order, so each stage is one bulk copy.
 //     N=128 chunks instead of 96 cut the drains and pool epilogues per tile from 4 to 3 and keep
 //     the tensor pipe busier while a single warpgroup issues (measured on an H100 80GB HBM3 from
 //     registers: 115 cycles per m64n128k16 against the ideal 64, 99 per m64n96k16 against 48).
@@ -66,16 +65,11 @@ constexpr int W1_BYTES = 2 * C1 * C0 * 2;                            // hi + lo 
 constexpr int L2_STAGES = 4, L2_KT = 32;                             // [256 rows x 32 k] per stage
 constexpr int L3_KSTAGES = 5, L3_KT = 64;                            // K slabs of layer 3
 constexpr int L2_STAGE_BYTES = C2 * L2_KT * 2 * 2;                   // 32768
-// layer 3 in the blob: 4 chunks of 96 rows x 5 K slabs, each stage [96 rows x 64 k] hi | lo
-constexpr int L3B_CHUNKS = 4, L3B_N = 96;
-constexpr int L3B_HALF = L3B_N * L3_KT * 2;                          // 12288
-constexpr int L3B_OFF = W1_BYTES + L2_STAGES * L2_STAGE_BYTES;
-constexpr int BLOB_BYTES = L3B_OFF + L3B_CHUNKS * L3_KSTAGES * 2 * L3B_HALF;  // 655360
-// layer 3 in shared memory: 3 chunks of 128 rows, each stage [128 rows x 64 k] hi | lo
+// layer 3: 3 chunks of 128 rows x 5 K slabs, each stage [128 rows x 64 k] hi | lo
 constexpr int L3_CHUNKS = 3, L3_N = 128;
 constexpr int L3_HALF = L3_N * L3_KT * 2;                            // 16384
-constexpr int L3_ROW = L3_KT * 2;   // bytes per row of an image: an 8-row band is 1 KB contiguous
 constexpr int STAGES_PER_TILE = 1 + L2_STAGES + L3_CHUNKS * L3_KSTAGES;  // 20
+constexpr int BLOB_BYTES = STAGES_PER_TILE * SLOT_BYTES;             // 655360
 constexpr int NFP = C0 * 6 + C0 + C1 + C2 + C3 + 4;   // W0 | shift0..3 | 1/wscale1..3 (floats)
 // warpgroups 0-1 consume (64 points each), warpgroup 2 produces; registers per thread after the
 // hand-over: 2 * 128 * 240 + 128 * 24 = 64512, the launch's 168 x 384
@@ -99,8 +93,6 @@ constexpr int TL_PHASES = 4 + 2 * L3_CHUNKS, TL_TILES = 60 / TL_PHASES, TL_WAIT 
 // every stage fills exactly one slot
 static_assert(W1_BYTES == SLOT_BYTES && L2_STAGE_BYTES == SLOT_BYTES && 2 * L3_HALF == SLOT_BYTES,
               "one weight stage per slot");
-static_assert(L3_CHUNKS * L3_N == C3 && L3B_CHUNKS * L3B_N == C3 && L3B_N < L3_N && L3_N <= 2 * L3B_N,
-              "a shared-memory chunk spans exactly two blob chunks");
 }  // namespace pm
 
 // POOL variant (the classifier / auto-encoder path): the input rows are the stacked copies SORTED
@@ -164,22 +156,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
           if (use > 0) tc::mbar_wait_relaxed(&empty[slot], (use - 1) & 1, 100 + s);
           unsigned char* dst = smem + OFF_RING + slot * SLOT_BYTES;
           mbar_arrive_expect_tx(&full[slot], SLOT_BYTES);
-          if (s <= L2_STAGES) {   // layer 1, then layer 2's K slabs: one blob stage each
-            bulk_g2s(dst, blob + static_cast<uint32_t>(s) * SLOT_BYTES, SLOT_BYTES, &full[slot]);
-          } else {
-            // layer-3 stage (nc, kc) = rows [128 nc, 128 nc + 128) of K slab kc: the tail of blob
-            // chunk oc from row r, then the head of chunk oc + 1, in the hi and the lo image
-            const int nc = (s - 1 - L2_STAGES) / L3_KSTAGES, kc = (s - 1 - L2_STAGES) % L3_KSTAGES;
-            const int oc = L3_N * nc / L3B_N, r = L3_N * nc - L3B_N * oc;
-            const uint32_t na = (L3B_N - r) * L3_ROW;
-            const unsigned char* src = blob + L3B_OFF + (oc * L3_KSTAGES + kc) * 2 * L3B_HALF + r * L3_ROW;
-            const unsigned char* src1 = blob + L3B_OFF + ((oc + 1) * L3_KSTAGES + kc) * 2 * L3B_HALF;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              bulk_g2s(dst + h * L3_HALF, src + h * L3B_HALF, na, &full[slot]);
-              bulk_g2s(dst + h * L3_HALF + na, src1 + h * L3B_HALF, L3_HALF - na, &full[slot]);
-            }
-          }
+          bulk_g2s(dst, blob + static_cast<uint32_t>(s) * SLOT_BYTES, SLOT_BYTES, &full[slot]);
         }
       }
     }
@@ -499,11 +476,11 @@ extern "C" int sonet_pointresnet_tc_pack(const float* W0, int Cin, const float* 
     pack_tile(W2, s2, C1, 0, C2, L2_KT * kc, L2_KT, blob + off, blob + off + L2_STAGE_BYTES / 2);
     off += L2_STAGE_BYTES;
   }
-  // layer 3: four 96-row chunks x five K slabs [96 rows x 64 k]
-  for (int nc = 0; nc < L3B_CHUNKS; ++nc)
+  // layer 3: three 128-row chunks x five K slabs [128 rows x 64 k]
+  for (int nc = 0; nc < L3_CHUNKS; ++nc)
     for (int kc = 0; kc < L3_KSTAGES; ++kc) {
-      pack_tile(W3, s3, K3, L3B_N * nc, L3B_N, L3_KT * kc, L3_KT, blob + off, blob + off + L3B_HALF);
-      off += 2 * L3B_HALF;
+      pack_tile(W3, s3, K3, L3_N * nc, L3_N, L3_KT * kc, L3_KT, blob + off, blob + off + L3_HALF);
+      off += 2 * L3_HALF;
     }
   if (off != static_cast<size_t>(BLOB_BYTES)) SONET_FAIL(SONET_ERR_BAD_ARG, "pack: size mismatch");
   float* f = fparams_host;

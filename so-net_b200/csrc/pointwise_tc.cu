@@ -32,12 +32,11 @@
 
 namespace sonet {
 namespace pwt {
-constexpr int TILE = 128, KCH = 64, NT = 256;   // NT: out-channel width of one weight-blob tile
+// the weight blob's n-tile width NT, K chunk KCH and stage K extent WK: tc::wblob
+constexpr int TILE = 128, KCH = tc::wblob::KCH, NT = tc::wblob::NT, WK = tc::wblob::WK;
 constexpr int NSUB = 128;                       // out channels per item (two per blob tile)
-constexpr int WK = 32;                          // K extent of one weight stage in the blob
 constexpr int A_HALF = TILE * KCH * 2;          // one fp16 image of an activation chunk, 16 KB
 constexpr int A_BYTES = 2 * A_HALF;             // hi + lo
-constexpr int W_BYTES = 2 * NT * KCH * 2;       // hi + lo weight images of one (blob tile, 64-k chunk)
 constexpr int WIMG = NSUB * WK * 2;             // one [128 x 32] fp16 weight image, 8 KB
 constexpr int WS_BYTES = 4 * WIMG;              // one chunk in shared memory: [half][hi|lo], 32 KB
 constexpr int NSTAGE = 2;                       // A ring
@@ -95,12 +94,8 @@ __device__ __forceinline__ Item decode_item(const Dims& d, int item) {
   r.kc0 = sp * d.kpi;
   return r;
 }
-__host__ __device__ inline int ntile_width(int Cout, int nt) {
-  const int cpad = (Cout + 63) / 64 * 64;
-  return min(NT, cpad - nt * NT);
-}
-__host__ __device__ inline int item_width(int Cout, int nt, int sub) {
-  return min(NSUB, ntile_width(Cout, nt) - sub * NSUB);
+__device__ inline int item_width(int Cout, int nt, int sub) {
+  return min(NSUB, tc::wblob::tile_width(Cout, nt) - sub * NSUB);
 }
 }  // namespace pwt
 
@@ -138,13 +133,11 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
       uint32_t q = 0;
       for (int it = 0; it < my_items; ++it) {
         const Item im = decode_item(d, blockIdx.x + it * gridDim.x);
-        const int nw = ntile_width(d.Cout, im.nt);
+        const int nw = tc::wblob::tile_width(d.Cout, im.nt);
         const int ns = item_width(d.Cout, im.nt, im.sub);
-        // blob: tile nt starts after nt full-width tiles; a 64-k chunk = two [nw x 32] stages, each
-        // a hi image then a lo image; this item's rows are [128 sub, 128 sub + ns) of each image
-        const size_t off0 = static_cast<size_t>(im.g) * d.blob_gstride +
-                            static_cast<size_t>(im.nt) * d.kchunks * W_BYTES;
-        const uint32_t stage = static_cast<uint32_t>(nw) * WK * 4;
+        // this item's rows are [128 sub, 128 sub + ns) of each image of n-tile nt
+        const unsigned char* rows = blob + static_cast<size_t>(im.g) * d.blob_gstride +
+                                    static_cast<size_t>(im.sub) * NSUB * WK * 2;
         const uint32_t bytes = static_cast<uint32_t>(ns) * WK * 2;
         for (int kc = im.kc0; kc < im.kc0 + d.kpi; ++kc, ++q) {
           const int halves = (d.cin_pad - kc * KCH > WK) ? 2 : 1;   // the consumers agree
@@ -153,8 +146,7 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
           mbar_arrive_expect_tx(&full_w[slot], 2 * halves * bytes);
           unsigned char* dst = smem + OFF_W + slot * WS_BYTES;
           for (int hh = 0; hh < halves; ++hh) {
-            const unsigned char* src = blob + off0 + (static_cast<size_t>(kc) * 2 + hh) * stage +
-                                       static_cast<size_t>(im.sub) * NSUB * WK * 2;
+            const unsigned char* src = rows + tc::wblob::stage_off(d.Cout, d.kchunks, im.nt, kc, hh);
             bulk_g2s(dst + (2 * hh) * WIMG, src, bytes, &full_w[slot]);
             bulk_g2s(dst + (2 * hh + 1) * WIMG, src + static_cast<size_t>(nw) * WK * 2, bytes,
                      &full_w[slot]);
@@ -345,67 +337,8 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
 }  // namespace sonet
 
 extern "C" long long sonet_pointwise_tc_blob_bytes(int Cout, int Cin) {
-  using namespace sonet::pwt;
   if (Cout < 1 || Cin < 1) return -1;
-  const int cpad = (Cout + 63) / 64 * 64;
-  const int kch = ((Cin + 15) / 16 * 16 + KCH - 1) / KCH;
-  return static_cast<long long>(cpad) * kch * KCH * 4;
-}
-
-static float tc_weight_scale(const float* W, size_t n) {
-  float mx = 0.f;
-  for (size_t i = 0; i < n; ++i) mx = std::max(mx, std::fabs(W[i]));
-  float scale = 1.f;
-  if (mx > 0.f && std::isfinite(mx)) {
-    int e;
-    std::frexp(mx, &e);
-    scale = std::ldexp(1.f, 9 - e);   // max|scale*W| in [256, 512)
-  }
-  return scale;
-}
-
-static void tc_pack_matrix(const float* W, int Cout, int Cin, unsigned char* blob, float scale) {
-  using namespace sonet::pwt;
-  const long long bytes = sonet_pointwise_tc_blob_bytes(Cout, Cin);
-  std::memset(blob, 0, static_cast<size_t>(bytes));
-  const int cpad = (Cout + 63) / 64 * 64;
-  const int kch = ((Cin + 15) / 16 * 16 + KCH - 1) / KCH;
-  const int ntiles = (cpad + NT - 1) / NT;
-  size_t off = 0;
-  for (int nt = 0; nt < ntiles; ++nt) {
-    const int nw = std::min(NT, cpad - nt * NT);
-    for (int kc = 0; kc < kch; ++kc) {
-      for (int hh = 0; hh < 2; ++hh) {   // one shared-memory weight stage = [nw x 32] hi | lo images
-        unsigned char* hi = blob + off;
-        unsigned char* lo = hi + static_cast<size_t>(nw) * WK * 2;
-        for (int r = 0; r < nw; ++r) {
-          const int co = nt * NT + r;
-          if (co >= Cout) continue;
-          for (int k = 0; k < WK; ++k) {
-            const int ci = kc * KCH + hh * WK + k;
-            if (ci >= Cin) continue;
-            const float w = W[static_cast<size_t>(co) * Cin + ci] * scale;
-            const __half h = __float2half_rn(w);
-            const __half l = __float2half_rn(w - __half2float(h));
-            const uint32_t o = (r >> 3) * 512 + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2;
-            std::memcpy(hi + o, &h, 2);
-            std::memcpy(lo + o, &l, 2);
-          }
-        }
-        off += static_cast<size_t>(nw) * WK * 4;
-      }
-    }
-  }
-}
-
-extern "C" int sonet_pointwise_tc_pack(const float* W, int Cout, int Cin, void* blob_host,
-                                       float* inv_scale) {
-  using namespace sonet;
-  SONET_REQUIRE(W && blob_host && inv_scale && Cout >= 1 && Cin >= 1, "pointwise_tc_pack: bad args");
-  const float scale = tc_weight_scale(W, static_cast<size_t>(Cout) * Cin);
-  *inv_scale = 1.f / scale;
-  tc_pack_matrix(W, Cout, Cin, static_cast<unsigned char*>(blob_host), scale);
-  return SONET_OK;
+  return sonet::tc::wblob::bytes(Cout, Cin);
 }
 
 // G matrices [G, Cout, Cin] packed back to back (sonet_pointwise_tc_blob_bytes each) with ONE
@@ -414,14 +347,28 @@ extern "C" int sonet_pointwise_tc_pack_groups(const float* W, int G, int Cout, i
                                               void* blob_host, float* inv_scale) {
   using namespace sonet;
   SONET_REQUIRE(W && blob_host && inv_scale && G >= 1 && Cout >= 1 && Cin >= 1,
-                "pointwise_tc_pack_groups: bad args");
+                "pointwise_tc_pack: bad args");
   const size_t per = static_cast<size_t>(Cout) * Cin;
-  const float scale = tc_weight_scale(W, per * G);
+  const float scale = pow2_scale(W, per * G);
   *inv_scale = 1.f / scale;
-  const long long bytes = sonet_pointwise_tc_blob_bytes(Cout, Cin);
+  const long long bytes = tc::wblob::bytes(Cout, Cin);
+  const int kch = tc::wblob::kchunks(Cin);
+  unsigned char* blob = static_cast<unsigned char*>(blob_host);
+  std::memset(blob, 0, static_cast<size_t>(bytes) * G);
   for (int g = 0; g < G; ++g)
-    tc_pack_matrix(W + g * per, Cout, Cin, static_cast<unsigned char*>(blob_host) + g * bytes, scale);
+    for (int n = 0; n < Cout; ++n)
+      for (int k = 0; k < Cin; ++k) {
+        long long hi, lo;
+        tc::wblob::elem_off(Cout, kch, n, k, hi, lo);
+        tc::put_weight(blob + g * bytes + hi, blob + g * bytes + lo,
+                       W[g * per + static_cast<size_t>(n) * Cin + k] * scale);
+      }
   return SONET_OK;
+}
+
+extern "C" int sonet_pointwise_tc_pack(const float* W, int Cout, int Cin, void* blob_host,
+                                       float* inv_scale) {
+  return sonet_pointwise_tc_pack_groups(W, 1, Cout, Cin, blob_host, inv_scale);
 }
 
 struct TcExt {   // grouped / split-K / scatter / point-major launch options (defaults = the plain layer)

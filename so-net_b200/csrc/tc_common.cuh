@@ -5,6 +5,7 @@
 // (128 contiguous bytes, row r at +16*r).
 #pragma once
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
 #include <cstring>
 
@@ -138,33 +139,78 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity
   asm volatile("trap;");
 }
 
+// ---- weight blobs ----------------------------------------------------------------------------------
+// Every kernel reads its weights (the B operand) from blobs packed by the host or, in train mode, by
+// the device; both packers use the definitions below.
+//
+// Byte offset of element (r, k) in one fp16 image with K extent kt, K-major without swizzle:
+// SBO = kt * 16, LBO = 128.
+__host__ __device__ inline uint32_t img_off(int r, int k, int kt) {
+  return static_cast<uint32_t>((r >> 3) * kt * 16 + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2);
+}
+// Writes the hi/lo split of one pre-scaled weight, h = rn16(w), l = rn16(w - h). Unlike the
+// activations' split2_f16 it does not saturate: a pre-scaled weight is below 512.
+__host__ __device__ inline void put_weight(unsigned char* hi, unsigned char* lo, float w) {
+  const __half h = __float2half_rn(w);
+  const __half l = __float2half_rn(w - __half2float(h));
+  *reinterpret_cast<__half*>(hi) = h;
+  *reinterpret_cast<__half*>(lo) = l;
+}
+// The pre-scale of a matrix with max|W| = absmax: the power of two that brings max|W| into
+// [256, 512), so the lo parts stay normal fp16 numbers and the hi parts far from the 65504
+// overflow; the epilogue's multiply undoes it exactly. 1 for an all-zero or non-finite matrix.
+// The exponent is capped at max_exp.
+__host__ __device__ inline float pow2_scale(float absmax, int max_exp = 1 << 30) {
+  if (!(absmax > 0.f && absmax <= FLT_MAX)) return 1.f;
+  int e;
+  frexpf(absmax, &e);  // absmax = f * 2^e, f in [0.5, 1)
+  return ldexpf(1.f, min(9 - e, max_exp));
+}
+
+// The generic layer's blob (csrc/pointwise_tc.cu) of a logical [N x K] matrix. N is padded to 64
+// and cut into n-tiles of up to 256 rows; K is padded to 16 and cut into 64-k chunks. A chunk is
+// two [nw x 32] stages (k 0..31, then 32..63), each a hi image then a lo image, where nw is the
+// tile's width. Tiles, chunks and stages follow each other without gaps; padding is zero.
+namespace wblob {
+constexpr int NT = 256, KCH = 64, WK = 32;
+__host__ __device__ inline int npad(int N) { return (N + 63) / 64 * 64; }
+__host__ __device__ inline int kchunks(long long K) {
+  return static_cast<int>(((K + 15) / 16 * 16 + KCH - 1) / KCH);
+}
+__host__ __device__ inline long long bytes(int N, long long K) {
+  return static_cast<long long>(npad(N)) * kchunks(K) * KCH * 4;
+}
+// rows of n-tile nt
+__host__ __device__ inline int tile_width(int N, int nt) { return min(NT, npad(N) - nt * NT); }
+// stage hh of chunk kc of n-tile nt; kch = kchunks(K)
+__host__ __device__ inline long long stage_off(int N, int kch, int nt, int kc, int hh) {
+  return static_cast<long long>(nt) * NT * kch * KCH * 4 +
+         (static_cast<long long>(kc) * 2 + hh) * tile_width(N, nt) * WK * 4;
+}
+// hi and lo images of element (n, k)
+__host__ __device__ inline void elem_off(int N, int kch, int n, int k, long long& hi, long long& lo) {
+  const int nt = n / NT;
+  hi = stage_off(N, kch, nt, k / KCH, (k / WK) & 1) + img_off(n - nt * NT, k % WK, WK);
+  lo = hi + tile_width(N, nt) * WK * 2;
+}
+}  // namespace wblob
 }  // namespace tc
 
 // ---- host-side packing -------------------------------------------------------------------------------
-// fp16 hi/lo images of scale * W[rows r0..r0+nr) x [k0..k0+kt) (row stride ld), K-major no-swizzle:
-// element (r,k) at (r/8)*SBO + (k/8)*128 + (r%8)*16 + (k%8)*2 with SBO = kt*16.
+// hi/lo images of scale * W[rows r0..r0+nr) x [k0..k0+kt) (row stride ld) with K extent kt
 inline void pack_tile(const float* W, float scale, int ld, int r0, int nr, int k0, int kt,
                       unsigned char* hi, unsigned char* lo) {
-  const uint32_t sbo = static_cast<uint32_t>(kt) * 16;
   for (int r = 0; r < nr; ++r)
     for (int k = 0; k < kt; ++k) {
-      const float w = W[static_cast<size_t>(r0 + r) * ld + k0 + k] * scale;  // exact (power of 2)
-      const __half h = __float2half_rn(w);
-      const __half l = __float2half_rn(w - __half2float(h));
-      const uint32_t off = (r >> 3) * sbo + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2;
-      std::memcpy(hi + off, &h, 2);
-      std::memcpy(lo + off, &l, 2);
+      const uint32_t off = tc::img_off(r, k, kt);
+      tc::put_weight(hi + off, lo + off, W[static_cast<size_t>(r0 + r) * ld + k0 + k] * scale);
     }
 }
-// power of two that brings max|W| into [256, 512): keeps the lo parts normal fp16 numbers and the
-// hi parts far from the 65504 overflow; undone exactly by the epilogue's multiply.
+// tc::pow2_scale of the n floats at W
 inline float pow2_scale(const float* W, size_t n) {
   float m = 0.f;
   for (size_t i = 0; i < n; ++i) m = std::max(m, std::fabs(W[i]));
-  if (!(m > 0.f) || !std::isfinite(m)) return 1.f;
-  int e;
-  std::frexp(m, &e);  // m = f * 2^e, f in [0.5, 1)
-  return std::ldexp(1.f, 9 - e);
+  return tc::pow2_scale(m);
 }
 
 }  // namespace sonet

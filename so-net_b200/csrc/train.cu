@@ -16,15 +16,14 @@
 //   tc_pack_device               fp32 weights -> wgmma hi/lo blob ON THE DEVICE (weights change
 //                                every optimizer step; the eval path packs on the host once), also
 //                                transposed: the dgrad GEMM dx = W^T dy runs on the same generic
-//                                wgmma layer kernel as the forward (csrc/pointwise_tc.cu)
+//                                wgmma layer kernel as the forward (csrc/pointwise_tc.cu); and the
+//                                activations x as the weight operand of the wgrad GEMM
 //
 // All reductions are two-stage with fp64 partial sums in a fixed order: bit-reproducible.
 #include <algorithm>
 #include <cmath>
 
-#include <cuda_fp16.h>
-
-#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace sonet {
 
@@ -180,47 +179,40 @@ __global__ void __launch_bounds__(256)
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) atomicMax(out_bits, __float_as_uint(m));   // non-negative floats
 }
-// scale2[0] = power-of-two pre-scale with max|scale*W| in [256,512), scale2[1] = 1/scale
+// scale2[0] = the power-of-two pre-scale of the tensor (tc::pow2_scale), scale2[1] = 1/scale
 __global__ void scale_from_absmax_kernel(const unsigned* __restrict__ bits, float* __restrict__ scale2) {
-  const float mx = __uint_as_float(*bits);
-  float sc = 1.f;
-  if (mx > 0.f && isfinite(mx)) {
-    int e;
-    frexpf(mx, &e);
-    sc = ldexpf(1.f, 9 - e);
-  }
+  const float sc = tc::pow2_scale(__uint_as_float(*bits));
   scale2[0] = sc;
   scale2[1] = 1.f / sc;
 }
-// blob layout of csrc/pointwise_tc.cu (tc_pack_matrix): n-tiles of <= 256 rows, 64-channel K chunks,
-// two [nw x 32] stages per chunk, hi image then lo image, 8x16-byte core matrices.
+// Packs the logical matrix Wl [N][K] times scale2[0] into the generic layer's blob (tc::wblob) with
+// kch K chunks, zero-padded. Wl[n][k] = src[n * sn + (k / kp) * sb + (k % kp) * sk]:
+//   W [N][K]:                     sn = K, sk = 1, kp = K, sb = 0
+//   W^T, of W [K][N]:             sn = 1, sk = N, kp = K, sb = 0
+//   x [B][N][P] with k = (b, p):  sn = P, sk = 1, kp = P, sb = N * P
+// Consecutive threads take consecutive k of one row n: the reads are coalesced unless sk > 1.
 __global__ void __launch_bounds__(256)
-    tc_pack_device_kernel(const float* __restrict__ W, int Cout, int Cin, int transpose,
-                          const float* __restrict__ scale2, unsigned char* __restrict__ blob,
-                          int cpad, int kch) {
-  // logical matrix Wl[n][k], n < Nl, k < Kl: Wl = W (Nl=Cout,Kl=Cin) or W^T (Nl=Cin,Kl=Cout)
-  const int Nl = transpose ? Cin : Cout, Kl = transpose ? Cout : Cin;
-  const long long total = static_cast<long long>(cpad) * kch * 64;
+    tc_pack_device_kernel(const float* __restrict__ src, int N, int K, long long sn, long long sk,
+                          int kp, long long sb, const float* __restrict__ scale2,
+                          unsigned char* __restrict__ blob, int kch) {
+  const int kext = kch * tc::wblob::KCH;
+  const long long total = static_cast<long long>(tc::wblob::npad(N)) * kext;
   const float sc = scale2[0];
   for (long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
        t += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int k = static_cast<int>(t % (kch * 64));
-    const int n = static_cast<int>(t / (kch * 64));
-    const int nt = n / 256, r = n - nt * 256;
-    const int nw = min(256, cpad - nt * 256);
-    const int kc = k >> 6, hh = (k >> 5) & 1, kk = k & 31;
+    const int n = static_cast<int>(t / kext), k = static_cast<int>(t - static_cast<long long>(n) * kext);
     float w = 0.f;
-    if (n < Nl && k < Kl) w = (transpose ? W[static_cast<size_t>(k) * Cin + n]
-                                         : W[static_cast<size_t>(n) * Cin + k]) * sc;
-    const __half h = __float2half_rn(w);
-    const __half l = __float2half_rn(w - __half2float(h));
-    // tile nt starts after nt full-width tiles: nt * 256 rows * kch chunks * 64 k * 4 B
-    const size_t stage = static_cast<size_t>(nt) * 256 * kch * 64 * 4 +
-                         (static_cast<size_t>(kc) * 2 + hh) * nw * 32 * 4;
-    const uint32_t o = (r >> 3) * 512 + (kk >> 3) * 128 + (r & 7) * 16 + (kk & 7) * 2;
-    *reinterpret_cast<__half*>(blob + stage + o) = h;
-    *reinterpret_cast<__half*>(blob + stage + static_cast<size_t>(nw) * 32 * 2 + o) = l;
+    if (n < N && k < K) w = src[n * sn + (k / kp) * sb + (k % kp) * sk] * sc;
+    long long hi, lo;
+    tc::wblob::elem_off(N, kch, n, k, hi, lo);
+    tc::put_weight(blob + hi, blob + lo, w);
   }
+}
+static void launch_tc_pack(const float* src, int N, int K, long long sn, long long sk, int kp,
+                           long long sb, const float* scale2, void* blob, int kch, cudaStream_t st) {
+  const long long total = static_cast<long long>(tc::wblob::npad(N)) * kch * tc::wblob::KCH;
+  tc_pack_device_kernel<<<static_cast<unsigned>(std::min<long long>((total + 255) / 256, 16384)), 256, 0,
+                          st>>>(src, N, K, sn, sk, kp, sb, scale2, static_cast<unsigned char*>(blob), kch);
 }
 
 // ---- wgrad helpers ------------------------------------------------------------------------------------
@@ -244,12 +236,7 @@ __global__ void __launch_bounds__(256)
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < 8; ++w) m = fmaxf(m, wm[w]);
-    float sc = 1.f;
-    if (m > 0.f && isfinite(m)) {
-      int e;
-      frexpf(m, &e);
-      sc = ldexpf(1.f, min(9 - e, 126));   // 2^126: 1/sc stays a normal float
-    }
+    const float sc = tc::pow2_scale(m, 126);   // 2^126: 1/sc stays a normal float
     cscale[c] = sc;
     cscale[C + c] = 1.f / sc;
   }
@@ -280,40 +267,6 @@ __global__ void __launch_bounds__(256)
        i += static_cast<long long>(gridDim.x) * blockDim.x)
     dWT[i] *= inv_c[i % Cout];
 }
-// x [B][Cin][P] as the "weight" matrix Wl[n = ci][k = b*P + p] of the wgrad GEMM, packed into the
-// wgmma blob layout (see tc_pack_device_kernel); K padded with zeros up to kch*64.
-__global__ void __launch_bounds__(256)
-    tc_pack_points_kernel(const float* __restrict__ x, int B, int Cin, int P,
-                          const float* __restrict__ scale2, unsigned char* __restrict__ blob, int cpad,
-                          int kch) {
-  const long long K = static_cast<long long>(B) * P;
-  const long long total = static_cast<long long>(cpad) * kch * 64;
-  const float sc = scale2[0];
-  for (long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
-       t += static_cast<long long>(gridDim.x) * blockDim.x) {
-    // consecutive threads -> consecutive k of one row n: coalesced reads of x along p
-    const long long k = t % (static_cast<long long>(kch) * 64);
-    const int n = static_cast<int>(t / (static_cast<long long>(kch) * 64));
-    const int nt = n / 256, r = n - nt * 256;
-    const int nw = min(256, cpad - nt * 256);
-    const long long kc = k >> 6;
-    const int hh = static_cast<int>((k >> 5) & 1), kk = static_cast<int>(k & 31);
-    float w = 0.f;
-    if (n < Cin && k < K) {
-      const long long b = k / P;
-      const int p = static_cast<int>(k - b * P);
-      w = x[(static_cast<size_t>(b) * Cin + n) * P + p] * sc;
-    }
-    const __half h = __float2half_rn(w);
-    const __half l = __float2half_rn(w - __half2float(h));
-    const size_t stage = static_cast<size_t>(nt) * 256 * kch * 64 * 4 +
-                         (static_cast<size_t>(kc) * 2 + hh) * nw * 32 * 4;
-    const uint32_t o = (r >> 3) * 512 + (kk >> 3) * 128 + (r & 7) * 16 + (kk & 7) * 2;
-    *reinterpret_cast<__half*>(blob + stage + o) = h;
-    *reinterpret_cast<__half*>(blob + stage + static_cast<size_t>(nw) * 32 * 2 + o) = l;
-  }
-}
-
 }  // namespace sonet
 
 static int bn_splits(int B, int C) {
@@ -389,13 +342,10 @@ extern "C" int sonet_pointwise_tc_pack_device(const float* W, int Cout, int Cin,
   absmax_kernel<<<static_cast<unsigned>(std::min<long long>((n + 255) / 256, 1024)), 256, 0, st>>>(
       W, n, scratch_bits);
   scale_from_absmax_kernel<<<1, 1, 0, st>>>(scratch_bits, scale2);
-  const int Nl = transpose ? Cin : Cout, Kl = transpose ? Cout : Cin;
-  const int cpad = (Nl + 63) / 64 * 64;
-  const int kch = ((Kl + 15) / 16 * 16 + 63) / 64;
-  const long long total = static_cast<long long>(cpad) * kch * 64;
-  tc_pack_device_kernel<<<static_cast<unsigned>(std::min<long long>((total + 255) / 256, 4096)), 256, 0,
-                          st>>>(W, Cout, Cin, transpose, scale2, static_cast<unsigned char*>(blob),
-                                cpad, kch);
+  if (transpose)   // W^T [Cin][Cout]
+    launch_tc_pack(W, Cin, Cout, 1, Cin, Cout, 0, scale2, blob, tc::wblob::kchunks(Cout), st);
+  else
+    launch_tc_pack(W, Cout, Cin, Cin, 1, Cin, 0, scale2, blob, tc::wblob::kchunks(Cin), st);
   return check_launch("pointwise_tc_pack_device");
 }
 
@@ -431,8 +381,7 @@ extern "C" long long sonet_wgrad_kpad(int B, int P, int splits) {
   return (K + q - 1) / q * q;
 }
 extern "C" long long sonet_wgrad_blob_bytes(int Cin, long long Kpad) {
-  const long long cpad = (Cin + 63) / 64 * 64;
-  return cpad * Kpad * 4;
+  return sonet::tc::wblob::bytes(Cin, Kpad);
 }
 extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Cout, int Cin, int P,
                                   int splits, float* dyT, void* blob, float* part, float* small,
@@ -455,11 +404,9 @@ extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Co
   if (Kpad > K)   // zero rows of the padded tail (the matching weight columns are packed as zeros too)
     cudaMemsetAsync(dyT + K * Cout, 0, sizeof(float) * static_cast<size_t>(Kpad - K) * Cout, st);
   transpose_scale_kernel<<<dim3((P + 31) / 32, (Cout + 31) / 32, B), 256, 0, st>>>(dy, Cout, P, s_dy, dyT);
-  const int cpad = (Cin + 63) / 64 * 64;
-  const int kch = static_cast<int>(Kpad / 64);
-  const long long total = static_cast<long long>(cpad) * Kpad;
-  tc_pack_points_kernel<<<static_cast<unsigned>(std::min<long long>((total + 255) / 256, 16384)), 256, 0,
-                          st>>>(x, B, Cin, P, s_x, static_cast<unsigned char*>(blob), cpad, kch);
+  // x as the weight matrix [Cin][k = (b, p)], zero-padded up to Kpad
+  launch_tc_pack(x, Cin, static_cast<int>(K), P, 1, P, static_cast<long long>(Cin) * P, s_x, blob,
+                 tc::wblob::kchunks(Kpad), st);
   rc = check_launch("wgrad_tc(prepare)");
   if (rc) return rc;
   // activations: dyT viewed as [B'=1][C'=Kpad][P'=Cout] (already scaled: no act pre-scale needed);
