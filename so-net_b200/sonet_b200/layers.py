@@ -12,6 +12,7 @@ compose differentiable PyTorch ops on the GPU exactly as the reference does — 
 training path, not a CPU fallback. Non-default options ('instance' norm, elu/swish/leakyrelu)
 always take the PyTorch path.
 """
+import itertools
 import math
 import os
 
@@ -87,26 +88,50 @@ def _make_act(activation):
     return None
 
 
-class _FoldedParams:
-    """Eval-mode conv/linear + BatchNorm folded into (weights, shift), re-packed only when a
+def tc_enabled():
+    """True unless SONET_TC=0, which routes every layer to the exact-fp32 CUDA-core kernels.
+    Read at call time, so a change applies from the next forward on."""
+    return os.environ.get("SONET_TC", "1") != "0"
+
+
+_stamps = itertools.count(1)
+
+
+class _Cache:
+    """A value derived from module parameters, rebuilt by get() when its key (never None)
+    changes. Values derived from this one key on `version`, a stamp of the current value unique
+    across all caches, so such a key also changes when a source layer is swapped for another."""
+    _key = _value = version = None
+
+    def clear(self):
+        self._key = self._value = self.version = None
+
+    def get(self, key, build):
+        if key != self._key:
+            self._value = build()
+            self._key, self.version = key, next(_stamps)
+        return self._value
+
+
+class _FoldedParams(_Cache):
+    """Eval-mode conv/linear + BatchNorm folded into (weights, shift), re-folded only when a
     parameter or running statistic changes (tracked through tensor version counters).
 
       y = gamma * (W x + bias - mean) / sqrt(var + eps) + beta  =  (s*W) x + ((bias-mean)*s + beta)
+
+    get() takes the fold's sources instead of a key and builder: it derives both from them.
     """
 
     def __init__(self):
-        self._key = None
-        self.version = 0    # bumped on every re-fold (lets dependants cache derived packings)
-        self.w = None       # [Cout, Cin] with the BN scale folded in
-        self.wt = None      # [Cin, Cout] (the point-wise kernel wants K-major slabs)
-        self.shift = None   # [Cout]
+        self._wt = _Cache()     # [Cin, Cout] (the point-wise kernel wants K-major slabs)
 
     def get(self, weight2d, bias, norm, transpose):
         srcs = [weight2d, bias]
         if norm is not None:
             srcs += [norm.weight, norm.bias, norm.running_mean, norm.running_var]
         key = tuple((t.data_ptr(), t._version, t.device) for t in srcs if t is not None)
-        if key != self._key:
+
+        def build():
             with torch.no_grad():
                 w = weight2d.detach().float()
                 shift = bias.detach().float() if bias is not None else \
@@ -115,32 +140,25 @@ class _FoldedParams:
                     s = norm.weight.detach() / torch.sqrt(norm.running_var.detach() + norm.eps)
                     shift = (shift - norm.running_mean.detach()) * s + norm.bias.detach()
                     w = w * s[:, None]
-                self.w = w.contiguous()          # [Cout, Cin]
-                self.wt = None                   # [Cin, Cout], built on first use
-                self.shift = shift.contiguous()
-            self._key = key
-            self.version += 1
+                return w.contiguous(), shift.contiguous()      # [Cout, Cin], [Cout]
+        w, shift = super().get(key, build)
         if not transpose:
-            return self.w, self.shift
-        if self.wt is None:
-            self.wt = self.w.t().contiguous()
-        return self.wt, self.shift
+            return w, shift
+        return self._wt.get(self.version, lambda: w.t().contiguous()), shift
 
 
 def invalidate(module):
     """Drop every derived weight cache (BN-folded weights, wgmma packings) below `module`.
 
-    The caches are keyed on (data_ptr, tensor._version) of the parameters and BN statistics, which
-    optimizer steps, load_state_dict() and in-place tensor ops all bump. Writes through `.data`
+    The BN fold is keyed on (data_ptr, tensor._version, device) of the parameters and BN
+    statistics, which optimizer steps, load_state_dict() and in-place tensor ops all bump; the
+    packings derived from a fold are keyed on its version. Writes through `.data`
     (`p.data.mul_(..)`, `w.data.copy_(..)` — an idiom of the reference code base,
     e.g. models/networks.py:366) do NOT bump the version counter: call this after such edits."""
     for m in module.modules():
-        f = getattr(m, "_folded", None)
-        if isinstance(f, _FoldedParams):
-            f._key = None
-        for attr in ("_tc_key", "_l1_key"):
-            if hasattr(m, attr):
-                setattr(m, attr, None)
+        for v in vars(m).values():
+            if isinstance(v, _Cache):
+                v.clear()
 
 
 class MyLinear(nn.Module):
@@ -171,15 +189,18 @@ class MyLinear(nn.Module):
             nn.init.ones_(self.norm.weight)
             nn.init.zeros_(self.norm.bias)
 
+    def folded(self, transpose=False):
+        """Eval-mode (w [Cout,Cin] or with transpose [Cin,Cout], shift [Cout]), BN folded in."""
+        return self._folded.get(self.linear.weight, self.linear.bias,
+                                self.norm if self.normalization == 'batch' else None, transpose)
+
     def _fast(self, x):
         return (_fast_ok(self, x) and x.dim() == 2
                 and self.normalization in (None, 'batch') and self.activation in (None, 'relu'))
 
     def forward(self, x, epoch=None):
         if self._fast(x):
-            w, shift = self._folded.get(self.linear.weight, self.linear.bias,
-                                        self.norm if self.normalization == 'batch' else None,
-                                        transpose=False)
+            w, shift = self.folded()
             return ops.linear(x.contiguous(), w, None, shift, self.activation == 'relu')
         x = self.linear(x)
         if self.normalization == 'batch':
@@ -194,9 +215,28 @@ class MyLinear(nn.Module):
 class _PointwiseConvBase(nn.Module):
     """Shared eval fast path of the 1x1 conv layers: y = act(BN(conv1x1(cat(x0, x1))))."""
 
+    def __init__(self):
+        super().__init__()
+        self._folded = _FoldedParams()
+        self._tc = _Cache()
+
     def _conv_weight2d(self):
         w = self.conv.weight
-        return w.view(w.shape[0], w.shape[1])
+        return w.view(w.shape[0], -1)
+
+    def folded(self, transpose=False):
+        """Eval-mode (w [Cout,Cin*kh*kw] or its transpose, shift [Cout]), BN folded in."""
+        return self._folded.get(self._conv_weight2d(), self.conv.bias,
+                                self.norm if self.normalization == 'batch' else None, transpose)
+
+    def _tc_params(self):
+        """(blob, inv_scale, shift) of the folded weight for the wgmma kernel, on its device."""
+        w, shift = self.folded()
+
+        def build():
+            blob, inv = ops.pointwise_tc_pack(w)
+            return blob.to(w.device), inv, shift
+        return self._tc.get(self._folded.version, build)
 
     def _fast_eligible(self):
         ks = self.conv.kernel_size
@@ -214,7 +254,6 @@ class _PointwiseConvBase(nn.Module):
         """x0 [B,C0,P] (+ x1 [B,C1,P] virtually concatenated on channels) -> [B,Cout,P].
         Dense layers run on wgmma (csrc/pointwise_tc.cu, fp16 hi/lo split); thin ones on the
         exact-fp32 CUDA-core kernel (csrc/pointwise.cu)."""
-        norm = self.norm if self.normalization == 'batch' else None
         cin = x0.shape[1] + (0 if x1 is None else x1.shape[1])
         cout = self.conv.out_channels
         rows = x0.shape[0] * x0.shape[2]
@@ -222,18 +261,11 @@ class _PointwiseConvBase(nn.Module):
         # tiles; thin OUTPUTS (the 128 -> 3 ConvToPC heads) qualify too — the layer is then a
         # streaming read of the activations into the tensor-core kernel instead of the
         # register-tiled fp32 kernel
-        if cin >= 32 and rows >= 256 and os.environ.get("SONET_TC", "1") != "0":
-            w, shift = self._folded.get(self._conv_weight2d(), self.conv.bias, norm,
-                                        transpose=False)
-            key = (self._folded.version, w.data_ptr())
-            if getattr(self, "_tc_key", None) != key:
-                blob, inv = ops.pointwise_tc_pack(w)
-                self._tc_pack = (blob.to(w.device), inv)
-                self._tc_key = key
-            blob, inv = self._tc_pack
+        if cin >= 32 and rows >= 256 and tc_enabled():
+            blob, inv, shift = self._tc_params()
             return ops.pointwise_layer_tc(x0, blob, inv, shift, cout, self.activation == 'relu',
                                           x1=x1, addend=addend, gidx=gidx)
-        w, shift = self._folded.get(self._conv_weight2d(), self.conv.bias, norm, transpose=True)
+        w, shift = self.folded(transpose=True)
         return ops.pointwise_layer(x0, w, None, shift, self.activation == 'relu', x1=x1,
                                    addend=addend, gidx=gidx)
 
@@ -257,7 +289,6 @@ class MyConv2d(_PointwiseConvBase):
         act = _make_act(activation)
         if act is not None:
             self.act = act
-        self._folded = _FoldedParams()
         self.weight_init()
 
     def weight_init(self):
@@ -317,8 +348,7 @@ class UpConv(nn.Module):
         self.up_sample = nn.Upsample(scale_factor=2)
         self.conv = MyConv2d(in_channels, out_channels, kernel_size=3, stride=1, padding=1,
                              bias=True, activation=activation, normalization=normalization)
-        self._tc_key = None
-        self._tc_pack = None
+        self._tc = _Cache()
         self._scratch = {}
         self.weight_init()
 
@@ -336,51 +366,38 @@ class UpConv(nn.Module):
                 and c.stride == (1, 1) and c.padding == (1, 1) and c.dilation == (1, 1)
                 and c.groups == 1 and c.out_channels >= 64 and c.in_channels >= 16
                 and self.normalization in (None, 'batch') and self.activation in (None, 'relu')
-                and os.environ.get("SONET_TC", "1") != "0")
+                and tc_enabled())
 
     def _packed(self):
-        """BN-folded, parity-combined weights as wgmma blobs; re-packed when a source tensor
-        changes. Wg[g=(py,px)][co][(a,c)*Cin + ci] = sum of the 3x3 taps (dy,dx) that read low-res
+        """BN-folded, parity-combined weights as wgmma blobs; re-packed when the fold changes.
+        Wg[g=(py,px)][co][(a,c)*Cin + ci] = sum of the 3x3 taps (dy,dx) that read low-res
         neighbour (a,c) for output parity (py,px): rows {0}|{1,2} (py=0) or {0,1}|{2} (py=1)."""
-        c = self.conv.conv
-        norm = self.conv.norm if self.normalization == 'batch' else None
-        srcs = [c.weight, c.bias]
-        if norm is not None:
-            srcs += [norm.weight, norm.bias, norm.running_mean, norm.running_var]
-        key = tuple((t.data_ptr(), t._version, t.device) for t in srcs if t is not None)
-        if key != self._tc_key:
-            with torch.no_grad():
-                w = c.weight.detach().float()                              # [Cout,Cin,3,3]
-                shift = c.bias.detach().float() if c.bias is not None else \
-                    torch.zeros(w.shape[0], device=w.device)
-                if norm is not None:
-                    sc = norm.weight.detach() / torch.sqrt(norm.running_var.detach() + norm.eps)
-                    shift = (shift - norm.running_mean.detach()) * sc + norm.bias.detach()
-                    w = w * sc[:, None, None, None]
-                sets = (((0,), (1, 2)), ((0, 1), (2,)))                    # [parity][tap] -> kernel rows
-                Cout, Cin = w.shape[0], w.shape[1]
-                Wg = torch.zeros(4, Cout, 4, Cin, device=w.device)
-                for py in range(2):
-                    for px in range(2):
-                        for a in range(2):
-                            for cc in range(2):
-                                acc = 0
-                                for dy in sets[py][a]:
-                                    for dx in sets[px][cc]:
-                                        acc = acc + w[:, :, dy, dx]
-                                Wg[py * 2 + px, :, a * 2 + cc, :] = acc
-                blob4, per4, inv4 = ops.pointwise_tc_pack_groups(Wg.view(4, Cout, 4 * Cin))
-                # 1x1 input: only the tap that lands on the single pixel survives -> one dense
-                # layer Cin -> 4*Cout (output channel co*4 + py*2 + px)
-                W1 = torch.stack([Wg[g, :, (1 - (g >> 1)) * 2 + (1 - (g & 1)), :] for g in range(4)],
-                                 dim=1).reshape(1, Cout * 4, Cin)
-                blob1, per1, inv1 = ops.pointwise_tc_pack_groups(W1)
-                dev = w.device
-                self._tc_pack = dict(blob4=blob4.to(dev), per4=per4, inv4=inv4, blob1=blob1.to(dev),
-                                     per1=per1, inv1=inv1, shift=shift.contiguous(),
-                                     shift1=shift.repeat_interleave(4).contiguous())
-            self._tc_key = key
-        return self._tc_pack
+        w, shift = self.conv.folded()                                      # [Cout,Cin*9]
+
+        def build():
+            Cout, Cin = self.conv.conv.out_channels, self.conv.conv.in_channels
+            w4 = w.view(Cout, Cin, 3, 3)
+            sets = (((0,), (1, 2)), ((0, 1), (2,)))    # [parity][tap] -> kernel rows
+            Wg = torch.zeros(4, Cout, 4, Cin, device=w.device)
+            for py in range(2):
+                for px in range(2):
+                    for a in range(2):
+                        for cc in range(2):
+                            acc = 0
+                            for dy in sets[py][a]:
+                                for dx in sets[px][cc]:
+                                    acc = acc + w4[:, :, dy, dx]
+                            Wg[py * 2 + px, :, a * 2 + cc, :] = acc
+            blob4, per4, inv4 = ops.pointwise_tc_pack_groups(Wg.view(4, Cout, 4 * Cin))
+            # 1x1 input: only the tap that lands on the single pixel survives -> one dense
+            # layer Cin -> 4*Cout (output channel co*4 + py*2 + px)
+            W1 = torch.stack([Wg[g, :, (1 - (g >> 1)) * 2 + (1 - (g & 1)), :] for g in range(4)],
+                             dim=1).reshape(1, Cout * 4, Cin)
+            blob1, per1, inv1 = ops.pointwise_tc_pack_groups(W1)
+            return dict(blob4=blob4.to(w.device), per4=per4, inv4=inv4, blob1=blob1.to(w.device),
+                        per1=per1, inv1=inv1, shift=shift,
+                        shift1=shift.repeat_interleave(4).contiguous())
+        return self._tc.get(self.conv._folded.version, build)
 
     def _scratch_for(self, n, dev):
         buf = self._scratch.get(dev)
@@ -439,7 +456,6 @@ class EquivariantLayer(_PointwiseConvBase):
         act = _make_act(activation)
         if act is not None:
             self.act = act
-        self._folded = _FoldedParams()
         self.weight_init()
 
     def weight_init(self):
@@ -486,6 +502,7 @@ class KNNModule(nn.Module):
                                         bn_momentum_decay_step=bn_momentum_decay_step,
                                         bn_momentum_decay=bn_momentum_decay))
             prev = c_out
+        self._tc = _Cache()
 
     def _fast(self, coordinate, x, precomputed_knn_I, center_type):
         return (_fast_ok(self, coordinate, x) and center_type in ('avg', 'center')
@@ -496,7 +513,7 @@ class KNNModule(nn.Module):
     def _tc_fused(self, K, M):
         """Two BN/ReLU layers 3+C -> 512 -> 512 (the encoder's), 2 <= K <= 16, M*K <= 2304."""
         ls = self.layers
-        return (os.environ.get("SONET_TC", "1") != "0" and len(ls) == 2
+        return (tc_enabled() and len(ls) == 2
                 and ls[0].conv.in_channels >= 3 + 32
                 and all(l.conv.out_channels == 512 and l.activation == 'relu' for l in ls)
                 and 2 <= K <= 16 and M * K <= 2304)
@@ -504,22 +521,16 @@ class KNNModule(nn.Module):
     def _tc_params(self):
         """Layer 1 split by linearity into the per-node GEMM of its feature columns (a generic
         wgmma blob) and (W1d | shift1) [512,4]; layer 2 as the fused kernel's weight stream.
-        Re-packed only when a parameter changes."""
-        folded = [l._folded.get(l._conv_weight2d(), l.conv.bias,
-                                l.norm if l.normalization == 'batch' else None, transpose=False)
-                  for l in self.layers]
-        key = tuple(l._folded.version for l in self.layers) + \
-            tuple(w.data_ptr() for w, _ in folded)
-        if getattr(self, "_tc_key", None) != key:
-            (w1, s1), (w2, s2) = folded
-            dev = w1.device
+        Re-packed only when a fold changes."""
+        (w1, s1), (w2, s2) = [l.folded() for l in self.layers]
+
+        def build():
             yblob, yinv = ops.pointwise_tc_pack(w1[:, 3:])
             blob2, inv2 = ops.knn_mlp_tc_pack(w2)
-            self._tc_pack = dict(yblob=yblob.to(dev), yinv=yinv,
-                                 w1=torch.cat((w1[:, :3], s1[:, None]), dim=1).contiguous(),
-                                 blob2=blob2.to(dev), inv2=inv2, shift2=s2.contiguous())
-            self._tc_key = key
-        return self._tc_pack
+            return dict(yblob=yblob.to(w1.device), yinv=yinv,
+                        w1=torch.cat((w1[:, :3], s1[:, None]), dim=1).contiguous(),
+                        blob2=blob2.to(w1.device), inv2=inv2, shift2=s2)
+        return self._tc.get(tuple(l._folded.version for l in self.layers), build)
 
     def _tc_forward(self, coord, center, knn_I, K, x):
         """x [B,C,M] -> knn_feature [B,512,M]: Y = W1f x once per node, stored node-major so the
@@ -651,10 +662,11 @@ class PointResNet(nn.Module):
         self.layers = _chain(in_channels, out_channels_list, activation, normalization, momentum,
                              bn_momentum_decay_step, bn_momentum_decay,
                              last_extra_in=out_channels_list[0])
+        self._tc = _Cache()
 
     # ---- fused wgmma path (csrc/pointmlp_tc.cu): the encoder's first PointResNet -------------
     def _tc_eligible(self, cin, x1):
-        if x1 is not None or os.environ.get("SONET_TC", "1") == "0":
+        if x1 is not None or not tc_enabled():
             return False
         if list(self.out_channels_list) != [64, 128, 256, 384] or cin > 6:
             return False
@@ -663,19 +675,13 @@ class PointResNet(nn.Module):
                 and ls[3].normalization is None and ls[3].activation is None)
 
     def _tc_params(self):
-        """(blob, fparams) on the weights' device, re-packed only when a parameter changes."""
-        folded = [l._folded.get(l._conv_weight2d(), l.conv.bias,
-                                l.norm if l.normalization == 'batch' else None, transpose=False)
-                  for l in self.layers]
-        key = tuple(l._folded.version for l in self.layers) + \
-            tuple(w.data_ptr() for w, _ in folded)
-        if getattr(self, "_tc_key", None) != key:
-            dev = folded[0][0].device
-            blob, fpar = ops.pointresnet_tc_pack([w for w, _ in folded], [s for _, s in folded],
-                                                 folded[0][0].shape[1])
-            self._tc_pack = (blob.to(dev), fpar.to(dev))
-            self._tc_key = key
-        return self._tc_pack
+        """(blob, fparams) on the weights' device, re-packed only when a fold changes."""
+        ws, shifts = zip(*[l.folded() for l in self.layers])
+
+        def build():
+            blob, fpar = ops.pointresnet_tc_pack(ws, shifts, ws[0].shape[1])
+            return blob.to(ws[0].device), fpar.to(ws[0].device)
+        return self._tc.get(tuple(l._folded.version for l in self.layers), build)
 
     def forward(self, x, epoch=None, x1=None):
         """x [B,C,P]; x1: optional second tensor virtually concatenated to x (eval fast path)."""

@@ -12,14 +12,13 @@ remain available as lazily materialised attributes for callers that read them
 (models/segmenter.py:90).
 """
 import math
-import os
 
 import torch
 import torch.nn as nn
 
 from . import ops, som, train_ops
 from .layers import (EquivariantLayer, KNNModule, MyConv2d, MyLinear, PointNet, PointResNet,
-                     UpConv, _fast_ok, _pick_splits)
+                     UpConv, _Cache, _fast_ok, _pick_splits, tc_enabled)
 
 
 def _bn_kwargs(opt):
@@ -281,8 +280,7 @@ class Segmenter(nn.Module):
         self.layer4 = EquivariantLayer(256, 128, activation=act, normalization=norm)
         self.drop4 = nn.Dropout(p=self.opt.dropout)
         self.layer5 = EquivariantLayer(128, self.opt.classes, activation=None, normalization=None)
-        self._l1_key = None
-        self._l1_pack = None
+        self._l1 = _Cache()
 
     def _onehot(self, label, B, device):
         onehot = torch.zeros(B, 16, dtype=torch.float32, device=device)
@@ -336,11 +334,9 @@ class Segmenter(nn.Module):
 
     def _pack_layer1(self, n_pt_a, n_onehot, n_pp, n_node):
         """Split the folded layer-1 weight (transposed [Cin,1024]) by input-channel role."""
-        l1 = self.layer1
-        w, shift = l1._folded.get(l1._conv_weight2d(), l1.conv.bias,
-                                  l1.norm if l1.normalization == 'batch' else None, transpose=True)
-        key = (w.data_ptr(), n_pt_a, n_onehot, n_pp, n_node)
-        if key != self._l1_key:
+        w, shift = self.layer1.folded(transpose=True)
+
+        def build():
             o0 = n_pt_a
             o1 = o0 + n_onehot
             o2 = o1 + n_pp
@@ -350,15 +346,12 @@ class Segmenter(nn.Module):
             # per-cloud inputs (one-hot label | global feature): a [B,1040]x[1040,1024] fp32 GEMM
             # whose result enters the node-level GEMM as a broadcast addend
             w_cloud = torch.cat((w[o0:o1], w[o3:]), dim=0).t().contiguous()   # [1024, 1040]
-            tc = None
-            if os.environ.get("SONET_TC", "1") != "0":      # wgmma images of both halves
-                bp, ip = ops.pointwise_tc_pack(w_point.t().contiguous())
-                # node-level GEMM: one launch of the grouped entry (K split to fill the SMs)
-                bn, pern, inn = ops.pointwise_tc_pack_groups(w_node.t().contiguous().unsqueeze(0))
-                tc = (bp.to(w.device), ip, bn.to(w.device), pern, inn)
-            self._l1_pack = (w_point, w_node, w_cloud, tc)
-            self._l1_key = key
-        return self._l1_pack + (shift,)
+            bp, ip = ops.pointwise_tc_pack(w_point.t().contiguous())
+            # node-level GEMM: one launch of the grouped entry (K split to fill the SMs)
+            bn, pern, inn = ops.pointwise_tc_pack_groups(w_node.t().contiguous().unsqueeze(0))
+            tc = (bp.to(w.device), ip, bn.to(w.device), pern, inn)
+            return w_point, w_node, w_cloud, tc, shift
+        return self._l1.get((self.layer1._folded.version, n_pt_a, n_onehot, n_pp, n_node), build)
 
     def forward_nodes(self, x_decentered, x, centers, sn, label, first_pn_out, node_first, node_knn,
                       node_final, feature, min_idx_i32):
@@ -395,7 +388,7 @@ class Segmenter(nn.Module):
         cloud = torch.cat((self._onehot(label, B, x.device), feature), dim=1)   # [B,1040]
         cloud_add = ops.linear(cloud.contiguous(), w_cloud, None, None, False).unsqueeze(2)  # [B,1024,1]
         relu1 = self.layer1.activation == 'relu'
-        if tc is not None:
+        if tc_enabled():
             bp, ip, bn, pern, inn = tc
             cout = w_point.shape[1]
             # [B,1920,M] -> [B,1024,M]: 16 row tiles x 4 column tiles would leave the GPU to 64

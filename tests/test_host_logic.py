@@ -48,7 +48,7 @@ def test_bn_folding_matches_eval_batchnorm():
     layer = layers.EquivariantLayer(7, 5, 'relu', 'batch')
     layer.load_state_dict(synth.synth_state_dict(layer, seed=3))
     layer.eval()
-    wt, shift = layer._folded.get(layer._conv_weight2d(), layer.conv.bias, layer.norm, True)
+    wt, shift = layer.folded(transpose=True)
     assert wt.shape == (7, 5)
     x = torch.randn(2, 7, 11)
     with torch.no_grad():
@@ -58,7 +58,7 @@ def test_bn_folding_matches_eval_batchnorm():
     # re-packs when a parameter changes in place
     with torch.no_grad():
         layer.norm.running_mean.add_(1.0)
-    wt2, shift2 = layer._folded.get(layer._conv_weight2d(), layer.conv.bias, layer.norm, True)
+    wt2, shift2 = layer.folded(transpose=True)
     assert not torch.equal(shift, shift2)
 
 
