@@ -303,6 +303,26 @@ long long sonet_seg_loss_scratch_bytes(int B, int N);
 int sonet_seg_loss_f32(const float* score, const long long* target, int B, int C, int N,
                        int size_average, void* scratch, float* loss, sonet_stream_t stream);
 
+/* Part-segmentation IoU (models/losses.py:73-189 compute_iou_np_array / compute_iou, called by
+ * part-seg/train.py:95). score [B,C,N] f32, seg [B,N] int64, label [B] int64; part table in CSR
+ * form: category k owns part_ids[part_offsets[k] .. part_offsets[k+1]) (int32, table order), each
+ * category 1..256 parts, every id in [0,C). pred = argmax over C (lowest class on ties, first NaN
+ * wins); per part p of label[b]'s category, I = #(seg==p && pred==p), U = #(seg==p || pred==p),
+ * iou = U ? I / (U + 0.0001) : 1.0 in double; iou_shape[b] [B] f64 = left-to-right sum / parts.
+ * pred [B,N] int64 and correct [B] int32 (= #(pred == seg)) are nullable. Deterministic.
+ * Device pointers; the table is not validated on the device: a label outside [0,num_categories)
+ * yields iou_shape[b] = NaN. */
+int sonet_seg_iou_f32(const float* score, const long long* seg, const long long* label, int B, int C,
+                      int N, const int32_t* part_offsets, const int32_t* part_ids, int num_categories,
+                      double* iou_shape, long long* pred, int32_t* correct, sonet_stream_t stream);
+/* The same over host pointers, shapes split over at most thread_num threads (fewer for small
+ * batches: at least 2^20 score elements per thread). Validates the table and every
+ * label: a label outside the table returns SONET_ERR_BAD_ARG. */
+int sonet_seg_iou_cpu_f32(const float* score, const long long* seg, const long long* label, int B,
+                          int C, int N, const int32_t* part_offsets, const int32_t* part_ids,
+                          int num_categories, double* iou_shape, long long* pred, int32_t* correct,
+                          int thread_num);
+
 /* ---- a-11: Chamfer distance ------------------------------------------------------------------------
  * Replaces ChamferLoss.forward (models/losses.py:237-290) including the Faiss IndexFlatL2
  * k=1 searches (losses.py:209-235) — exact brute force, direct differences, lowest index on ties.

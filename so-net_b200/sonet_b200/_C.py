@@ -80,6 +80,10 @@ _SIGNATURES = {
     "sonet_seg_loss_scratch_bytes": [c_int, c_int],
     "sonet_seg_loss_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                            c_void_p],
+    "sonet_seg_iou_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                          c_int, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sonet_seg_iou_cpu_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                              c_int, c_void_p, c_void_p, c_void_p, c_int],
     "sonet_chamfer_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sonet_pointresnet_tc_blob_bytes": [],

@@ -1,15 +1,26 @@
-"""ChamferLoss with the reference's API (models/losses.py:17-27, 192-296) on one fused CUDA path.
+"""The reference's models/losses.py API on our kernels.
 
-The reference builds two Faiss IndexFlatL2 per cloud and round-trips through host numpy
-(losses.py:247-276). Here both nearest-neighbour searches of the whole batch, the
-sqrt(d^2 + 1e-8) terms and all means run on the device in four launches (csrc/chamfer.cu).
-No Faiss dependency.
+ChamferLoss (losses.py:17-27, 192-296): the reference builds two Faiss IndexFlatL2 per cloud and
+round-trips through host numpy (losses.py:247-276). Here both nearest-neighbour searches of the
+whole batch, the sqrt(d^2 + 1e-8) terms and all means run on the device in four launches
+(csrc/chamfer.cu). No Faiss dependency.
+
+compute_iou_np_array / compute_iou (losses.py:73-189), the part-segmentation metric of
+part-seg/train.py:95: one kernel for CUDA tensors, the same arithmetic in C++ for host tensors
+(csrc/seg_iou.cu); PartSegIoU accumulates it over an evaluation loop without a sync per batch.
 """
+import json
+import os
+from collections import OrderedDict
+
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import ops
+from . import _C, ops
+
+SHAPENET_PART_TABLE = ops.SHAPENET_PART_TABLE
 
 
 def robust_norm(var):
@@ -76,3 +87,112 @@ class ChamferLoss(nn.Module):
 
     def __call__(self, predict_pc, gt_pc):
         return self.forward(predict_pc, gt_pc)
+
+
+def _seg_iou(score, seg, label, table=None, want_correct=False):
+    """Per-shape IoU [B] float64 (and correct-point counts [B] int32) on score's device: the sm_90a
+    kernel for CUDA scores (no sync; a label outside the table gives NaN), the library's host entry
+    for CPU scores (a label outside the table raises)."""
+    if score.dtype != torch.float32:
+        raise RuntimeError("seg_iou: score must be float32 (got %s)" % score.dtype)
+    score = score.detach().contiguous()
+    seg = seg.detach().to(score.device, torch.int64).contiguous()
+    label = label.detach().to(score.device, torch.int64).contiguous()
+    if score.is_cuda:
+        iou, _, correct = ops.seg_iou(score, seg, label, table, want_correct=want_correct)
+        return iou, correct
+    B, C, N = ops._seg_iou_args(score, seg, label)
+    offsets, ids, K = ops.part_table_csr(table, C, score.device)
+    iou = torch.empty((B,), dtype=torch.float64)
+    correct = torch.empty((B,), dtype=torch.int32) if want_correct else None
+    _C.check(_C.lib().sonet_seg_iou_cpu_f32(score.data_ptr(), seg.data_ptr(), label.data_ptr(), B, C,
+                                            N, offsets.data_ptr(), ids.data_ptr(), K, iou.data_ptr(),
+                                            None, _C.ptr(correct), torch.get_num_threads()),
+             "sonet_seg_iou_cpu_f32")
+    return iou, correct
+
+
+def _host_iou(iou):
+    out = iou.cpu().numpy()
+    if np.isnan(out).any():
+        raise RuntimeError("seg_iou: label outside the part table (cloud %d)"
+                           % int(np.flatnonzero(np.isnan(out))[0]))
+    return out
+
+
+def compute_iou_np_array(score, seg, label, visualizer, opt, input_pc):
+    """score [B,C,N] float32, seg [B,N], label [B] (integer) -> per-shape IoU, float64 numpy [B]
+    (models/losses.py:73-116): for each part of the shape's ShapeNetPart category, I / (U + 1e-4)
+    of the predicted (argmax over C) and ground-truth point sets, or 1.0 if the part is absent
+    from both; their mean. Bit-equal to the reference. CUDA scores run one kernel, host scores the
+    library's C++ entry. visualizer, opt and input_pc are accepted and ignored, as in the reference.
+    Unlike the reference, whose list indexing wraps negative labels, a label outside [0, 16) raises
+    RuntimeError."""
+    return _host_iou(_seg_iou(score, seg, label)[0])
+
+
+def compute_iou(score, seg, label, visualizer, opt, input_pc):
+    """Mean over the batch of compute_iou_np_array (models/losses.py:119-189), as np.float64."""
+    return compute_iou_np_array(score, seg, label, visualizer, opt, input_pc).mean()
+
+
+def visualize_pc_seg(score, seg, label, visualizer, opt, input_pc, batch_num):
+    """Show one cloud coloured by predicted and by ground-truth part (models/losses.py:46-70):
+    score [C,N], seg [N], input_pc [3,N]; colours from <opt.dataroot>/part_color_mapping.json
+    (RGB in [0,1], scaled to int 0..255); ground-truth part 49 is drawn as (1,1,1). label and
+    batch_num are unused, as in the reference."""
+    xyz = input_pc.detach().cpu().numpy().transpose()                        # N x 3
+    predicted = torch.max(score.detach().cpu(), dim=0)[1].numpy()
+    gt = seg.detach().cpu().numpy()
+    with open(os.path.join(opt.dataroot, "part_color_mapping.json")) as f:
+        colors = np.fabs(np.asarray(json.load(f)) * 255).astype(int)
+    gt_colors = colors[gt]
+    gt_colors[gt == 49] = 1
+    visualizer.display_current_results(OrderedDict([("pc_colored_predicted", [xyz, colors[predicted]]),
+                                                    ("pc_colored_gt", [xyz, gt_colors])]), 1, 1)
+
+
+class PartSegIoU:
+    """Part-segmentation metrics over an evaluation loop, without a host sync per batch.
+
+        meter = PartSegIoU()
+        for batch in loader:
+            ...; meter.update(model.score_segmenter, model.input_seg, model.input_label)
+        r = meter.compute()
+
+    update() runs the seg_iou kernel (the host entry for CPU tensors) and keeps the per-shape IoUs,
+    categories and correct-point counts on the scores' device. compute() copies them once and
+    returns, all computed in float64 numpy in a fixed order (the same batches in the same order give
+    the same bits):
+      instance_miou  mean IoU over all shapes (what part-seg/train.py accumulates in test_iou)
+      category_miou  {category: mean IoU of its shapes} for every category seen
+      class_miou     mean of category_miou over the categories seen, in ascending order
+      accuracy       correct points / all points
+    table: category -> part ids (default: the 16 ShapeNetPart categories)."""
+
+    def __init__(self, table=None):
+        self.table = table
+        self.reset()
+
+    def reset(self):
+        self._iou, self._label, self._correct = [], [], []
+        self._points = 0
+
+    def update(self, score, seg, label):
+        iou, correct = _seg_iou(score, seg, label, self.table, want_correct=True)
+        self._iou.append(iou)
+        self._label.append(label.detach().to(iou.device, torch.int64, copy=True))
+        self._correct.append(correct)
+        self._points += seg.numel()
+
+    def compute(self):
+        if not self._iou:
+            raise RuntimeError("PartSegIoU.compute() before any update()")
+        iou = _host_iou(torch.cat(self._iou))
+        label = torch.cat(self._label).cpu().numpy()
+        correct = torch.cat(self._correct).cpu().numpy().astype(np.int64)
+        cats = np.unique(label)
+        per_cat = OrderedDict((int(c), iou[label == c].mean()) for c in cats)
+        return dict(instance_miou=iou.mean(), category_miou=per_cat,
+                    class_miou=np.asarray(list(per_cat.values())).mean(),
+                    accuracy=correct.sum() / float(self._points))

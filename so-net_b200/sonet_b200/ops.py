@@ -311,6 +311,71 @@ def seg_loss(score, target, size_average=True):
     return loss
 
 
+# ShapeNetPart: category -> its part ids, in the reference's order (models/losses.py:74-91)
+SHAPENET_PART_TABLE = ((0, 1, 2, 3), (4, 5), (6, 7), (8, 9, 10, 11), (12, 13, 14, 15), (16, 17, 18),
+                       (19, 20, 21), (22, 23), (24, 25, 26, 27), (28, 29), (30, 31, 32, 33, 34, 35),
+                       (36, 37), (38, 39, 40), (41, 42, 43), (44, 45, 46), (47, 48, 49))
+SEG_IOU_MAX_PARTS = 256
+_PART_TABLES = {}
+
+
+def part_table_csr(table, C, device):
+    """Validated (offsets [K+1], ids) int32 tensors of a category -> part ids table on `device`,
+    uploaded once per (table, device) and cached: later calls neither copy nor allocate."""
+    table = SHAPENET_PART_TABLE if table is None else tuple(tuple(int(p) for p in parts)
+                                                            for parts in table)
+    key = (table, C, str(device))
+    hit = _PART_TABLES.get(key)
+    if hit is None:
+        if not table:
+            raise RuntimeError("seg_iou: the part table has no category")
+        for k, parts in enumerate(table):
+            if not 1 <= len(parts) <= SEG_IOU_MAX_PARTS:
+                raise RuntimeError("seg_iou: category %d has %d parts (1..%d allowed)"
+                                   % (k, len(parts), SEG_IOU_MAX_PARTS))
+            if any(not 0 <= p < C for p in parts):
+                raise RuntimeError("seg_iou: category %d has a part id outside [0, C=%d)" % (k, C))
+        offsets = [0]
+        for parts in table:
+            offsets.append(offsets[-1] + len(parts))
+        ids = [p for parts in table for p in parts]
+        hit = (torch.tensor(offsets, dtype=torch.int32, device=device),
+               torch.tensor(ids, dtype=torch.int32, device=device), len(table))
+        _PART_TABLES[key] = hit
+    return hit
+
+
+def _seg_iou_args(score, seg, label):
+    if score.dim() != 3 or tuple(seg.shape) != (score.shape[0], score.shape[2]) \
+            or tuple(label.shape) != (score.shape[0],):
+        raise RuntimeError("seg_iou: expected score [B,C,N], seg [B,N], label [B], got %s, %s, %s"
+                           % (tuple(score.shape), tuple(seg.shape), tuple(label.shape)))
+    return score.shape
+
+
+def seg_iou(score, seg, label, table=None, want_pred=False, want_correct=False):
+    """Part-segmentation IoU of every cloud (models/losses.py:73-116) in one launch, no sync.
+    score [B,C,N] f32, seg [B,N] int64, label [B] int64 (CUDA, contiguous); table: category ->
+    part ids (default SHAPENET_PART_TABLE). Returns (iou_shape [B] f64, pred [B,N] int64 or None,
+    correct [B] int32 or None). A label outside the table gives iou_shape[b] = NaN (the device
+    cannot raise without a sync). The table is uploaded on its first use per device, so a call
+    captured in a CUDA graph needs one call with that table before the capture."""
+    _chk(score, "score", torch.float32)
+    _chk(seg, "seg", torch.int64)
+    _chk(label, "label", torch.int64)
+    B, C, N = _seg_iou_args(score, seg, label)
+    dev = score.device
+    with torch.cuda.device(dev):
+        offsets, ids, K = part_table_csr(table, C, dev)
+        iou = torch.empty((B,), dtype=torch.float64, device=dev)
+        pred = torch.empty((B, N), dtype=torch.int64, device=dev) if want_pred else None
+        correct = torch.empty((B,), dtype=torch.int32, device=dev) if want_correct else None
+        _call("sonet_seg_iou_f32", _C.ptr(score), _C.ptr(seg), _C.ptr(label), B, C, N,
+              _C.ptr(offsets), _C.ptr(ids), K, _C.ptr(iou), _C.ptr(pred), _C.ptr(correct),
+              _stream(score))
+    return iou, pred, correct
+
+
 def chamfer(pred, gt, want_idx=False):
     """pred [B,3,Mp], gt [B,3,N] -> dict(loss [3], fwd_arr [B], bwd_arr [B], elem_fwd, elem_bwd,
     idx_fwd?, idx_bwd?)."""
