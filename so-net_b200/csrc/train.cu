@@ -29,8 +29,14 @@ namespace sonet {
 
 constexpr int BN_THREADS = 256;
 
-// stage 1: CTA (c, s) sums the clouds b = s, s+S, ... of channel c. want_gx: sums of g and g*xhat
-// for the backward (g = dy * [gamma*xhat + beta > 0] when relu), else sums of x and x*x.
+// stage 1: CTA (c, s) sums the clouds b = s, s+S, ... of channel c. BWD: sums of g and g*xhat
+// (g = dy * [gamma*xhat + beta > 0] when relu), else sums of d and d*d with d = x - x[0,c,0].
+//
+// The forward sums are shifted by a pivot, the channel's first element, and taken in fp64 term by
+// term. var = E[d^2] - E[d]^2 then cancels only by 1 + (mean - pivot)^2 / var, a few units for any
+// pivot drawn from the channel, where E[x^2] - mean^2 would cancel by (mean/std)^2: with fp32 sums
+// that is a relative error of ~(mean/std)^2 * 2^-24 in var, 1e-2 at mean/std = 1e3 (channels behind
+// a large bias, near-dead inputs). d is exact in fp64, d*d too, and a constant channel gives var = 0.
 template <bool BWD>
 __global__ void __launch_bounds__(BN_THREADS)
     bn_partial_kernel(const float* __restrict__ x, const float* __restrict__ dy,
@@ -40,35 +46,40 @@ __global__ void __launch_bounds__(BN_THREADS)
   const int c = blockIdx.x, s = blockIdx.y;
   double a0 = 0.0, a1 = 0.0;
   float mu = 0.f, is = 1.f, ga = 1.f, be = 0.f;
+  double pivot = 0.0;
   if (BWD) {
     mu = mean[c];
     is = invstd[c];
     ga = gamma ? gamma[c] : 1.f;
     be = beta ? beta[c] : 0.f;
+  } else {
+    pivot = x[static_cast<size_t>(c) * P];
   }
   for (int b = s; b < B; b += S) {
     const float* xr = x + (static_cast<size_t>(b) * C + c) * P;
-    const float* gr = BWD ? dy + (static_cast<size_t>(b) * C + c) * P : nullptr;
-    float f0 = 0.f, f1 = 0.f;            // fp32 within one row chunk, fp64 across
-    int cnt = 0;
-    for (int p = threadIdx.x; p < P; p += BN_THREADS) {
-      const float v = xr[p];
-      if (BWD) {
-        const float xh = (v - mu) * is;
+    if (BWD) {
+      const float* gr = dy + (static_cast<size_t>(b) * C + c) * P;
+      float f0 = 0.f, f1 = 0.f;          // fp32 within one row chunk, fp64 across
+      int cnt = 0;
+      for (int p = threadIdx.x; p < P; p += BN_THREADS) {
+        const float xh = (xr[p] - mu) * is;
         float g = gr[p];
         if (relu && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
         f0 += g;
         f1 = fmaf(g, xh, f1);
-      } else {
-        f0 += v;
-        f1 = fmaf(v, v, f1);
+        if (++cnt == 64) {               // flush to fp64 every 64 terms
+          a0 += f0; a1 += f1; f0 = f1 = 0.f; cnt = 0;
+        }
       }
-      if (++cnt == 64) {                 // flush to fp64 every 64 terms
-        a0 += f0; a1 += f1; f0 = f1 = 0.f; cnt = 0;
+      a0 += f0;
+      a1 += f1;
+    } else {
+      for (int p = threadIdx.x; p < P; p += BN_THREADS) {
+        const double d = static_cast<double>(xr[p]) - pivot;
+        a0 += d;
+        a1 = fma(d, d, a1);
       }
     }
-    a0 += f0;
-    a1 += f1;
   }
   __shared__ double r0[BN_THREADS], r1[BN_THREADS];
   r0[threadIdx.x] = a0;
@@ -87,9 +98,10 @@ __global__ void __launch_bounds__(BN_THREADS)
   }
 }
 
-__global__ void bn_stats_final_kernel(const double* __restrict__ partial, int C, int S, double n,
-                                      float eps, float* __restrict__ mean,
-                                      float* __restrict__ var, float* __restrict__ invstd) {
+__global__ void bn_stats_final_kernel(const double* __restrict__ partial, const float* __restrict__ x,
+                                      int C, int P, int S, double n, float eps,
+                                      float* __restrict__ mean, float* __restrict__ var,
+                                      float* __restrict__ invstd) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   double s0 = 0.0, s1 = 0.0;
@@ -97,10 +109,10 @@ __global__ void bn_stats_final_kernel(const double* __restrict__ partial, int C,
     s0 += partial[(static_cast<size_t>(c) * S + s) * 2];
     s1 += partial[(static_cast<size_t>(c) * S + s) * 2 + 1];
   }
-  const double m = s0 / n;
-  double v = s1 / n - m * m;
+  const double md = s0 / n;                                        // mean - pivot
+  double v = s1 / n - md * md;
   if (v < 0.0) v = 0.0;
-  mean[c] = static_cast<float>(m);
+  mean[c] = static_cast<float>(static_cast<double>(x[static_cast<size_t>(c) * P]) + md);
   var[c] = static_cast<float>(v);                                  // biased (F.batch_norm normalises with it)
   invstd[c] = static_cast<float>(1.0 / sqrt(v + static_cast<double>(eps)));
 }
@@ -287,8 +299,8 @@ extern "C" int sonet_bn_train_forward_f32(const float* x, const float* gamma, co
   const int S = bn_splits(B, C);
   bn_partial_kernel<false><<<dim3(C, S), BN_THREADS, 0, st>>>(x, nullptr, nullptr, nullptr, nullptr,
                                                              nullptr, B, C, P, 0, S, partial);
-  bn_stats_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(partial, C, S, static_cast<double>(B) * P, eps,
-                                                        save_mean, save_var, save_invstd);
+  bn_stats_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(partial, x, C, P, S, static_cast<double>(B) * P,
+                                                        eps, save_mean, save_var, save_invstd);
   bn_apply_kernel<<<dim3((P + 1023) / 1024, C, B), 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta,
                                                                C, P, relu, y);
   return check_launch("bn_train_forward");

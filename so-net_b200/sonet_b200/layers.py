@@ -312,10 +312,10 @@ class MyConv2d(_PointwiseConvBase):
                 x.contiguous().view(B, C, H * W), self._conv_weight2d(), self.conv.bias,
                 self.norm if self.normalization == 'batch' else None, self.activation == 'relu', epoch)
             return y.view(B, y.shape[1], H, W)
-        # PyTorch/cuDNN path (3x3 decoder convs, training): strict fp32 — cuDNN's default TF32
-        # convolution is ~1e-3 relative, outside the 1e-4 parity bar of the reference's fp32 math
-        with torch.backends.cudnn.flags(enabled=True, allow_tf32=False):
-            x = self.conv(x)
+        # PyTorch/cuDNN path (3x3 decoder convs, training): strict fp32 in the forward and the
+        # backward — cuDNN's default TF32 convolution is ~1e-3 relative, outside the 1e-4 parity
+        # bar of the reference's fp32 math
+        x = train_ops.conv_strict(self.conv, x)
         if self.normalization == 'batch':
             x = self.norm(x, epoch)
         elif self.normalization is not None:

@@ -200,18 +200,61 @@ class IndexMaxGather(torch.autograd.Function):
         return gd, None, None
 
 
+def _cudnn_strict_fp32():
+    c = torch.backends.cudnn
+    return c.flags(enabled=True, benchmark=c.benchmark, deterministic=c.deterministic,
+                   allow_tf32=False)
+
+
+class ConvStrict(torch.autograd.Function):
+    """F.conv1d / F.conv2d (zero padding) with cuDNN's TF32 off in the forward AND the backward,
+    whatever torch.backends.cudnn.allow_tf32 says. PyTorch's own backward reads the global flag
+    when backward() runs, outside any context the forward was called in; TF32 (~5e-4 per product)
+    is far outside the 1e-4 parity bar of the reference's fp32 math."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, stride, padding, dilation, groups):
+        with _cudnn_strict_fp32():
+            y = torch.ops.aten.convolution(x, weight, bias, stride, padding, dilation, False,
+                                           [0] * len(stride), groups)
+        ctx.save_for_backward(x, weight)
+        ctx.conf = (None if bias is None else [bias.shape[0]], stride, padding, dilation, groups)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        bias_sizes, stride, padding, dilation, groups = ctx.conf
+        need = ctx.needs_input_grad
+        with _cudnn_strict_fp32():
+            dx, dw, db = torch.ops.aten.convolution_backward(
+                dy.contiguous(), x, weight, bias_sizes, stride, padding, dilation, False,
+                [0] * len(stride), groups, [need[0], need[1], bias_sizes is not None and need[2]])
+        return dx, dw, db, None, None, None, None
+
+
+def conv_strict(conv, x):
+    """conv (nn.Conv1d / nn.Conv2d, zero padding) applied to x through ConvStrict."""
+    return ConvStrict.apply(x, conv.weight, conv.bias, list(conv.stride), list(conv.padding),
+                            list(conv.dilation), conv.groups)
+
+
 def conv_bn_act_train(x3, weight2d, bias, norm, relu, epoch=None):
     """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (wgmma when dense
-    enough) -> batch-stat BN (+ running-stat update with the reference's momentum schedule,
-    models/layers.py:57-65) -> ReLU."""
+    enough, else strict-fp32 cuDNN) -> batch-stat BN (+ running-stat update with the reference's
+    momentum schedule, models/layers.py:57-65; like F.batch_norm, num_batches_tracked is left
+    alone) -> ReLU."""
     B, Cin, P = x3.shape
     Cout = weight2d.shape[0]
     if tc_eligible(Cin, Cout, B * P):
         y0 = ConvTC.apply(x3, weight2d, bias)
     else:
-        y0 = torch.nn.functional.conv1d(x3, weight2d.unsqueeze(2), bias)
+        y0 = ConvStrict.apply(x3, weight2d.unsqueeze(2), bias, [1], [0], [1], 1)
     if norm is None:
         return torch.relu(y0) if relu else y0
+    if B * P == 1:     # F.batch_norm's check: a batch statistic of one value is undefined
+        raise ValueError("Expected more than 1 value per channel when training, got input size "
+                         "{}".format(y0.size()))
     step = norm.momentum_decay_step
     if epoch is not None and epoch >= 1 and step is not None and step > 0:
         norm.momentum = max(norm.momentum_original * (norm.momentum_decay ** (epoch // step)), 0.01)
@@ -220,7 +263,5 @@ def conv_bn_act_train(x3, weight2d, bias, norm, relu, epoch=None):
         n = B * P
         m = norm.momentum
         norm.running_mean.mul_(1 - m).add_(mean, alpha=m)
-        norm.running_var.mul_(1 - m).add_(var * (n / max(n - 1, 1)), alpha=m)
-        if norm.num_batches_tracked is not None:
-            norm.num_batches_tracked += 1
+        norm.running_var.mul_(1 - m).add_(var * (n / (n - 1)), alpha=m)
     return y

@@ -115,10 +115,16 @@ def test_index_max_gather_backward_vs_torch_gather(oracle_mod):
     assert float(got[:, :, 0].abs().sum()) > 0              # the empty nodes' gradient landed on point 0
 
 
+CLASSIFIER_STEP_GRAD_TOL = 1e-4
+
+
 def test_classifier_training_step_kernels_vs_torch_composition():
-    """One optimize() step from identical weights with the train kernels ON and OFF: same loss,
-    same gradients (1e-3 of each tensor's scale: the wgmma GEMMs carry ~1e-5 per layer),
-    same running statistics."""
+    """One optimize() step from identical weights with the train kernels ON (under PyTorch's
+    default precision flags: cuDNN TF32 on, cuBLAS TF32 off) and OFF (strict fp32): same loss,
+    same gradients to CLASSIFIER_STEP_GRAD_TOL of each tensor's scale, same running statistics in
+    every BN layer. Measured on one H100 80GB HBM3 (700 W power limit): the largest gradient error
+    was 2.9e-5 (first_pointnet.layers.0.norm.weight); the tolerance is 3.5x that. TF32 in the kernel
+    arm's thin layers shows as 2e-4 to 5e-4 (test_gpu_train_parity.py)."""
     from helpers import build_states
     from sonet_b200 import classifier, synth, train_ops
     opt = synth.make_opt("classifier", batch_size=8, input_pc_num=512, device=DEV)
@@ -126,13 +132,13 @@ def test_classifier_training_step_kernels_vs_torch_composition():
     st = build_states("classifier", opt, seed=81)
     inp = synth.synth_inputs(8, 512, seed=81)
     res = {}
-    # the PyTorch composition must be a strict-fp32 baseline: cuDNN/cuBLAS default to TF32
-    # (~1e-3), which is coarser than the kernels under test
+    # the PyTorch composition must be a strict-fp32 baseline: cuDNN defaults to TF32 (~1e-3),
+    # which is coarser than the kernels under test; the kernel arm must not depend on the flag
     tf32 = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
-    torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     for flag in (True, False):
         train_ops.ENABLED = flag
+        torch.backends.cudnn.allow_tf32 = flag
         try:
             m = classifier.Model(opt)
             m.encoder.load_state_dict(st["encoder"])
@@ -150,15 +156,17 @@ def test_classifier_training_step_kernels_vs_torch_composition():
                 loss=loss.detach().clone(),
                 grads={n: p.grad.detach().clone() for n, p in m.encoder.named_parameters()
                        if p.grad is not None},
-                rm=m.encoder.first_pointnet.layers[1].norm.running_mean.clone(),
-                rv=m.encoder.first_pointnet.layers[1].norm.running_var.clone())
+                stats={n: b.detach().clone() for n, b in m.encoder.named_buffers()
+                       if n.endswith(("running_mean", "running_var"))})
         finally:
             train_ops.ENABLED = True
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
+            torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
     close(res[True]["loss"], res[False]["loss"], "loss", 1e-4)
-    close(res[True]["rm"], res[False]["rm"], "running_mean", 1e-5)
-    close(res[True]["rv"], res[False]["rv"], "running_var", 1e-5)
+    assert set(res[True]["stats"]) == set(res[False]["stats"]) and len(res[True]["stats"]) >= 12
+    for n, ref in res[False]["stats"].items():
+        close(res[True]["stats"][n], ref, n, 1e-5)
     assert set(res[True]["grads"]) == set(res[False]["grads"]) and len(res[True]["grads"]) > 20
+    worst = (0.0, None)
     for n, gref in res[False]["grads"].items():
         got = res[True]["grads"][n]
         wname = n.rsplit(".", 1)[0] + ".weight"
@@ -171,4 +179,8 @@ def test_classifier_training_step_kernels_vs_torch_composition():
             if float(gref.abs().max()) < 1e-3 * wscale:
                 assert float(got.abs().max()) < 1e-3 * wscale, n
                 continue
-        close(got, gref, "grad " + n, 2e-3)
+        err = float((got - gref).abs().max()) / float(gref.abs().max().clamp(min=1e-12))
+        worst = max(worst, (err, n))
+        close(got, gref, "grad " + n, CLASSIFIER_STEP_GRAD_TOL)
+    print("\n[train-step] kernels (default flags) vs strict-fp32 composition: worst grad %.2e (%s)"
+          % worst)
