@@ -468,6 +468,45 @@ int sonet_knn_mlp_tc_forward(const float* coord, const float* center, const int6
                              float inv_scale, const float* shift2, float* out,
                              sonet_stream_t stream);
 
+/* ---- opt-in fp16 mode of the eval wgmma entries (SONET_TC=fp16, INTEGRATION.md) ----------------
+ * Each takes the arguments and the blob of the entry without the suffix, and runs every wgmma
+ * GEMM as ONE fp16 product per MAC instead of the hi/lo split's three:
+ *   y = (sum_k rn16sat(x_k) * rn16(s * w_k)) / s, accumulated in fp32,
+ * where s is the blob's power-of-two pre-scale, rn16sat(x) the round-to-nearest fp16 of x saturated
+ * at +-65504 (the split's hi word) and rn16(s * w) the hi image already in the blob. Everything
+ * outside the GEMMs is unchanged: layer 0 of the PointResNet and layer 1's coordinate part of the
+ * KNN module stay fp32 on CUDA cores, and so do all epilogues (shift, ReLU, addends, maxima,
+ * scatter). Per output the rounding of both operands costs up to ~2^-10 * sum_k |w_k x_k|
+ * (2^-11 each); against the rounded operands the GEMM is exact up to fp32 accumulation. Same
+ * properties as the split entries: no allocation, no host synchronisation, deterministic, CUDA
+ * graph capturable. */
+int sonet_pointresnet_tc_forward_f16(const float* x, int Cin, int B, int P, const void* blob,
+                                     const float* fparams, float* out, sonet_stream_t stream);
+int sonet_pointresnet_tc_pool_forward_f16(const float* x_sorted, int Cin, int B, int P,
+                                          const void* blob, const float* fparams,
+                                          const int32_t* node_sorted, const int32_t* pos0, int M,
+                                          int32_t* pool_keys, float* p0, sonet_stream_t stream);
+int sonet_pointwise_tc_forward_f16(const float* x0, int C0, const float* x1, int C1, int B, int P,
+                                   const void* blob, float inv_scale, const float* shift, int Cout,
+                                   int relu, const float* addend, const int32_t* gidx, int G,
+                                   float* out, sonet_stream_t stream);
+int sonet_pointwise_tc_forward_rows_f16(const float* x0, int C0, const float* x1, int C1, int B,
+                                        int P, const void* blob, float inv_scale,
+                                        const float* shift, int Cout, int relu,
+                                        const float* addend, const int32_t* gidx, int G, float* out,
+                                        sonet_stream_t stream);
+int sonet_pointwise_tc_grouped_forward_f16(const float* x, int C, int B, int P, const void* blob,
+                                           long long blob_gstride, float inv_scale,
+                                           const float* shift, int Cout, int relu, int groups,
+                                           int splits, int scat_w, int conv_w, int P_out,
+                                           long long out_gstride, float* out, float* scratch,
+                                           sonet_stream_t stream);
+int sonet_knn_mlp_tc_forward_f16(const float* coord, const float* center, const int64_t* idx,
+                                 int B, int M, int K, int Kstride, const float* Y,
+                                 long long y_cstride, long long y_nstride, const float* w1,
+                                 const void* blob, float inv_scale, const float* shift2, float* out,
+                                 sonet_stream_t stream);
+
 /* ---- diagnostics -------------------------------------------------------------------------------
  * One 128 x N x K bf16 GEMM on wgmma (fp32 accumulate in registers), D = bf16(A) * bf16(Bm)^T.
  * A [128,K], Bm [N,K], D [128,N] fp32 row-major device pointers. mode 0: A from shared memory

@@ -81,7 +81,9 @@ struct KnnArgs {
 };
 
 // YVEC: Y is node-major (y_cs == 1), so channels (c, c+1) of a row are one float2.
-template <bool YVEC>
+// NPROD: fp16 products per MAC in layer 2, 3 (the hi/lo split) or 1 (hi only, the opt-in fp16 mode:
+// the A fragments carry no lo words and the producer copies the hi half of each stage)
+template <bool YVEC, int NPROD>
 __global__ void __launch_bounds__(kt::NUM_THREADS, 1)
     knn_mlp_tc_kernel(const unsigned char* __restrict__ blob, KnnArgs a, long long* __restrict__ dbg) {
   using namespace kt;
@@ -127,9 +129,10 @@ __global__ void __launch_bounds__(kt::NUM_THREADS, 1)
         for (int s = 0; s < KSTAGES; ++s, ++q) {
           const uint32_t slot = q % NSLOT, use = q / NSLOT;
           if (use > 0) tc::mbar_wait_relaxed(&empty[slot], (use - 1) & 1, 300 + s);
-          mbar_arrive_expect_tx(&full[slot], STAGE_BYTES);
+          constexpr uint32_t bytes = NPROD == 3 ? STAGE_BYTES : STAGE_BYTES / 2;   // [hi | lo]
+          mbar_arrive_expect_tx(&full[slot], bytes);
           bulk_g2s(smem + OFF_RING + slot * STAGE_BYTES,
-                   blob + static_cast<size_t>(KSTAGES * pass + s) * STAGE_BYTES, STAGE_BYTES,
+                   blob + static_cast<size_t>(KSTAGES * pass + s) * STAGE_BYTES, bytes,
                    &full[slot]);
         }
       }
@@ -226,7 +229,7 @@ __global__ void __launch_bounds__(kt::NUM_THREADS, 1)
             v = fmaf(w.z, d[2], v);
             h[e] = fmaxf(v, 0.f);
           }
-          tc::split2_f16(h[0], h[1], hi[i], lo[i]);
+          tc::split_words<NPROD>(h[0], h[1], hi[i], lo[i]);
         }
       };
 
@@ -250,8 +253,10 @@ __global__ void __launch_bounds__(kt::NUM_THREADS, 1)
                          bl = tc::smem_desc(sb + STAGE_BYTES / 2 + ks * 256, 128, 512);
           tc::wg_fence();
           tc::wgmma_f16_rs_n256(acc, fh[ks], bh, 1);
-          tc::wgmma_f16_rs_n256(acc, fl[ks], bh, 1);
-          tc::wgmma_f16_rs_n256(acc, fh[ks], bl, 1);
+          if (NPROD == 3) {
+            tc::wgmma_f16_rs_n256(acc, fl[ks], bh, 1);
+            tc::wgmma_f16_rs_n256(acc, fh[ks], bl, 1);
+          }
           tc::wg_commit();
           if (kk == 0 && stamp != nullptr && it < 15) stamp[4 * it + 1] = clock64();
           // K block kk-1 has retired: its fragment buffer is free, and so is its stage if it
@@ -337,7 +342,7 @@ extern "C" int sonet_knn_mlp_tc_pack(const float* W2, void* blob_host, float* in
 static int launch_knn_mlp_tc(const float* coord, const float* center, const int64_t* idx, int B, int M,
                              int K, int Kstride, const float* Y, long long y_cs, long long y_ns,
                              const float* w1, const void* blob, float inv2, const float* shift2,
-                             float* out, long long* dbg, sonet_stream_t stream) {
+                             float* out, long long* dbg, sonet_stream_t stream, bool f16 = false) {
   using namespace sonet;
   using namespace sonet::kt;
   SONET_REQUIRE(B >= 0 && M >= 1 && Kstride >= K, "knn_mlp_tc: bad dimension");
@@ -361,7 +366,8 @@ static int launch_knn_mlp_tc(const float* coord, const float* center, const int6
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "knn_mlp_tc: needs %d B of shared memory", SMEM_BYTES);
   const long long items = 2 * ((nblocks + 1) / 2);   // (tile, pass) pairs
   const int grid = static_cast<int>(std::min<long long>(items, sm_count()));
-  auto kernel = y_cs == 1 ? knn_mlp_tc_kernel<true> : knn_mlp_tc_kernel<false>;
+  auto kernel = f16 ? (y_cs == 1 ? knn_mlp_tc_kernel<true, 1> : knn_mlp_tc_kernel<false, 1>)
+                    : (y_cs == 1 ? knn_mlp_tc_kernel<true, 3> : knn_mlp_tc_kernel<false, 3>);
   cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   kernel<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(static_cast<const unsigned char*>(blob),
                                                                a, dbg);
@@ -375,6 +381,16 @@ extern "C" int sonet_knn_mlp_tc_forward(const float* coord, const float* center,
                                         float* out, sonet_stream_t stream) {
   return launch_knn_mlp_tc(coord, center, idx, B, M, K, Kstride, Y, y_cstride, y_nstride, w1, blob,
                            inv_scale, shift2, out, nullptr, stream);
+}
+
+// the opt-in fp16 mode: one product hi(x)*hi(w) per MAC in layer 2, same blob and arguments
+extern "C" int sonet_knn_mlp_tc_forward_f16(const float* coord, const float* center, const int64_t* idx,
+                                            int B, int M, int K, int Kstride, const float* Y,
+                                            long long y_cstride, long long y_nstride, const float* w1,
+                                            const void* blob, float inv_scale, const float* shift2,
+                                            float* out, sonet_stream_t stream) {
+  return launch_knn_mlp_tc(coord, center, idx, B, M, K, Kstride, Y, y_cstride, y_nstride, w1, blob,
+                           inv_scale, shift2, out, nullptr, stream, true);
 }
 
 extern "C" int sonet_debug_knn_mlp_tc_timeline(const float* coord, const float* center,

@@ -113,8 +113,10 @@ struct PoolArgs {
   int M;
 };
 
-// DBG: the debug entry points' build, which also stamps the phase timeline of CTA 0
-template <bool POOL, bool DBG>
+// DBG: the debug entry points' build, which also stamps the phase timeline of CTA 0.
+// NPROD: fp16 products per MAC, 3 (the hi/lo split) or 1 (hi only, the opt-in fp16 mode: act0
+// has no lo image, act1 / act2 no lo fragments, and the producer copies the hi half of each stage)
+template <bool POOL, bool DBG, int NPROD>
 __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     pointresnet_tc_kernel(const float* __restrict__ x_in, int Cin, int B, int P,
                           const unsigned char* __restrict__ blob, const float* __restrict__ fparams,
@@ -155,8 +157,10 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
           const uint32_t slot = q % NSLOT, use = q / NSLOT;
           if (use > 0) tc::mbar_wait_relaxed(&empty[slot], (use - 1) & 1, 100 + s);
           unsigned char* dst = smem + OFF_RING + slot * SLOT_BYTES;
-          mbar_arrive_expect_tx(&full[slot], SLOT_BYTES);
-          bulk_g2s(dst, blob + static_cast<uint32_t>(s) * SLOT_BYTES, SLOT_BYTES, &full[slot]);
+          // every stage is [hi | lo], 16 KB each
+          constexpr uint32_t bytes = NPROD == 3 ? SLOT_BYTES : SLOT_BYTES / 2;
+          mbar_arrive_expect_tx(&full[slot], bytes);
+          bulk_g2s(dst, blob + static_cast<uint32_t>(s) * SLOT_BYTES, bytes, &full[slot]);
         }
       }
     }
@@ -215,9 +219,9 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int k = 16 * kk + 8 * (i >> 1);
-          tc::split2_f16(fmaxf(fmaf(acc[8 * kk + 2 * i], inv, shq[k]), 0.f),
-                         fmaxf(fmaf(acc[8 * kk + 2 * i + 1], inv, shq[k + 1]), 0.f),
-                         hi[kk][i], lo[kk][i]);
+          tc::split_words<NPROD>(fmaxf(fmaf(acc[8 * kk + 2 * i], inv, shq[k]), 0.f),
+                                 fmaxf(fmaf(acc[8 * kk + 2 * i + 1], inv, shq[k + 1]), 0.f),
+                                 hi[kk][i], lo[kk][i]);
         }
     };
 
@@ -251,11 +255,12 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
               for (int c = 0; c < 6; ++c) a = fmaf(fps[ch * 6 + c], xv[c], a);
               y[e] = fmaxf(a, 0.f);
             }
-            tc::split2_f16(y[0], y[1], hi[jj], lo[jj]);
+            tc::split_words<NPROD>(y[0], y[1], hi[jj], lo[jj]);
           }
           const int oct = half * 4 + o;
           *reinterpret_cast<uint4*>(a_hi + oct * 128) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-          *reinterpret_cast<uint4*>(a_hi + ACT0_HALF + oct * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+          if (NPROD == 3)
+            *reinterpret_cast<uint4*>(a_hi + ACT0_HALF + oct * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
         }
         // act0 writes of this warpgroup -> its wgmmas
         tc::fence_proxy_async();
@@ -290,8 +295,10 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
                          bh = tc::smem_desc(sb + ks * 256, 128, 1024),
                          bl = tc::smem_desc(sb + W1_BYTES / 2 + ks * 256, 128, 1024);
           tc::wgmma_f16_n128(acc, ah, bh, 1);
-          tc::wgmma_f16_n128(acc, al, bh, 1);
-          tc::wgmma_f16_n128(acc, ah, bl, 1);
+          if (NPROD == 3) {
+            tc::wgmma_f16_n128(acc, al, bh, 1);
+            tc::wgmma_f16_n128(acc, ah, bl, 1);
+          }
         }
         tc::wg_commit();
         tc::wg_wait<0>();
@@ -316,8 +323,10 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
             const uint64_t bh = tc::smem_desc(sb + ks * 256, 128, 512),
                            bl = tc::smem_desc(sb + L2_STAGE_BYTES / 2 + ks * 256, 128, 512);
             tc::wgmma_f16_rs_n256(acc, a1_hi[kk], bh, 1);
-            tc::wgmma_f16_rs_n256(acc, a1_lo[kk], bh, 1);
-            tc::wgmma_f16_rs_n256(acc, a1_hi[kk], bl, 1);
+            if (NPROD == 3) {
+              tc::wgmma_f16_rs_n256(acc, a1_lo[kk], bh, 1);
+              tc::wgmma_f16_rs_n256(acc, a1_hi[kk], bl, 1);
+            }
           }
           tc::wg_commit();
           tc::wg_wait<1>();
@@ -349,13 +358,17 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
               const uint64_t ah = tc::smem_desc(act0_a + ks * 256, 128, 1024),
                              al = tc::smem_desc(act0_a + ACT0_HALF + ks * 256, 128, 1024);
               tc::wgmma_f16_n128(acc, ah, bh, 1);
-              tc::wgmma_f16_n128(acc, al, bh, 1);
-              tc::wgmma_f16_n128(acc, ah, bl, 1);
+              if (NPROD == 3) {
+                tc::wgmma_f16_n128(acc, al, bh, 1);
+                tc::wgmma_f16_n128(acc, ah, bl, 1);
+              }
             } else {
               const int kk = 4 * (kc - 1) + ks;
               tc::wgmma_f16_rs_n128(acc, a2_hi[kk], bh, 1);
-              tc::wgmma_f16_rs_n128(acc, a2_lo[kk], bh, 1);
-              tc::wgmma_f16_rs_n128(acc, a2_hi[kk], bl, 1);
+              if (NPROD == 3) {
+                tc::wgmma_f16_rs_n128(acc, a2_lo[kk], bh, 1);
+                tc::wgmma_f16_rs_n128(acc, a2_hi[kk], bl, 1);
+              }
             }
           }
           tc::wg_commit();
@@ -500,7 +513,7 @@ extern "C" int sonet_pointresnet_tc_pack(const float* W0, int Cin, const float* 
 
 static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const void* blob,
                                  const float* fparams, float* out, long long* dbg,
-                                 const sonet::PoolArgs* pool, sonet_stream_t stream) {
+                                 const sonet::PoolArgs* pool, sonet_stream_t stream, bool f16 = false) {
   using namespace sonet;
   using namespace sonet::pm;
   SONET_REQUIRE(B >= 0 && P >= 0, "pointresnet_tc: negative dimension");
@@ -515,8 +528,10 @@ static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const vo
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "pointresnet_tc: needs %d B of shared memory",
                 SMEM_BYTES);
   const int grid = static_cast<int>(std::min<long long>(tiles, sm_count()));
-  auto kern = pool ? (dbg ? pointresnet_tc_kernel<true, true> : pointresnet_tc_kernel<true, false>)
-                   : (dbg ? pointresnet_tc_kernel<false, true> : pointresnet_tc_kernel<false, false>);
+  SONET_REQUIRE(!(f16 && dbg), "pointresnet_tc: the debug timeline has no fp16 build");
+  auto kern = f16 ? (pool ? pointresnet_tc_kernel<true, false, 1> : pointresnet_tc_kernel<false, false, 1>)
+            : pool ? (dbg ? pointresnet_tc_kernel<true, true, 3> : pointresnet_tc_kernel<true, false, 3>)
+                   : (dbg ? pointresnet_tc_kernel<false, true, 3> : pointresnet_tc_kernel<false, false, 3>);
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   PoolArgs pa = pool ? *pool : PoolArgs{nullptr, nullptr, nullptr, nullptr, 0};
   kern<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
@@ -537,6 +552,22 @@ extern "C" int sonet_pointresnet_tc_pool_forward(const float* x_sorted, int Cin,
                                                  sonet_stream_t stream) {
   sonet::PoolArgs pa{node_sorted, pos0, pool_keys, p0, M};
   return launch_pointresnet_tc(x_sorted, Cin, B, P, blob, fparams, nullptr, nullptr, &pa, stream);
+}
+
+// the opt-in fp16 mode of the two entries above: one product hi(x)*hi(w) per MAC, same blob
+extern "C" int sonet_pointresnet_tc_forward_f16(const float* x, int Cin, int B, int P, const void* blob,
+                                                const float* fparams, float* out,
+                                                sonet_stream_t stream) {
+  return launch_pointresnet_tc(x, Cin, B, P, blob, fparams, out, nullptr, nullptr, stream, true);
+}
+
+extern "C" int sonet_pointresnet_tc_pool_forward_f16(const float* x_sorted, int Cin, int B, int P,
+                                                     const void* blob, const float* fparams,
+                                                     const int32_t* node_sorted, const int32_t* pos0,
+                                                     int M, int32_t* pool_keys, float* p0,
+                                                     sonet_stream_t stream) {
+  sonet::PoolArgs pa{node_sorted, pos0, pool_keys, p0, M};
+  return launch_pointresnet_tc(x_sorted, Cin, B, P, blob, fparams, nullptr, nullptr, &pa, stream, true);
 }
 
 extern "C" int sonet_debug_pointresnet_tc_pool_timeline(const float* x_sorted, int Cin, int B, int P,

@@ -16,7 +16,8 @@
 //     fp16 hi/lo and writes the K-major no-swizzle A images with one 128-bit shared store per 8
 //     channels (conflict free), then issues 3 wgmma per 16-channel K step (hi*hi + lo*hi + hi*lo)
 //     with fp32 accumulators in registers (64 per thread at N = 128). A 2-slot A ring: a slot is
-//     rewritten once wgmma.wait_group shows the chunk that read it complete;
+//     rewritten once wgmma.wait_group shows the chunk that read it complete. The opt-in fp16
+//     mode (the `_f16` entries, NPROD = 1) writes only the hi image and issues hi*hi alone;
 //   * producer warp: streams the pre-packed fp16 hi/lo weight images (cp.async.bulk + mbarrier)
 //     through a 4-stage ring shared by both warpgroups;
 //   * epilogue in registers: fused scale/shift (+ gathered addend) + ReLU; eight lanes of a warp
@@ -99,6 +100,9 @@ __device__ inline int item_width(int Cout, int nt, int sub) {
 }
 }  // namespace pwt
 
+// NPROD: fp16 products per MAC, 3 (hi/lo split, the default) or 1 (hi only, the opt-in fp16 mode:
+// the lo A image is never written and the producer copies only the hi image of each stage)
+template <int NPROD>
 __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
     pointwise_tc_kernel(const float* __restrict__ x0, const float* __restrict__ x1,
                         const unsigned char* __restrict__ blob, const float* __restrict__ shift,
@@ -143,13 +147,14 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
           const int halves = (d.cin_pad - kc * KCH > WK) ? 2 : 1;   // the consumers agree
           const uint32_t slot = q % NSTAGE_W, use = q / NSTAGE_W;
           if (use > 0) tc::mbar_wait_relaxed(&empty_w[slot], (use - 1) & 1, 200);
-          mbar_arrive_expect_tx(&full_w[slot], 2 * halves * bytes);
+          mbar_arrive_expect_tx(&full_w[slot], (NPROD == 3 ? 2 : 1) * halves * bytes);
           unsigned char* dst = smem + OFF_W + slot * WS_BYTES;
           for (int hh = 0; hh < halves; ++hh) {
             const unsigned char* src = rows + tc::wblob::stage_off(d.Cout, d.kchunks, im.nt, kc, hh);
             bulk_g2s(dst + (2 * hh) * WIMG, src, bytes, &full_w[slot]);
-            bulk_g2s(dst + (2 * hh + 1) * WIMG, src + static_cast<size_t>(nw) * WK * 2, bytes,
-                     &full_w[slot]);
+            if (NPROD == 3)
+              bulk_g2s(dst + (2 * hh + 1) * WIMG, src + static_cast<size_t>(nw) * WK * 2, bytes,
+                       &full_w[slot]);
           }
         }
       }
@@ -221,10 +226,12 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
         for (int o = 0; o < 4; ++o) {
           uint32_t hi[4], lo[4];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) tc::split2_f16(v[o * 8 + 2 * j], v[o * 8 + 2 * j + 1], hi[j], lo[j]);
+          for (int j = 0; j < 4; ++j)
+            tc::split_words<NPROD>(v[o * 8 + 2 * j], v[o * 8 + 2 * j + 1], hi[j], lo[j]);
           const int oct = half * 4 + o;
           *reinterpret_cast<uint4*>(a_hi + oct * 128) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-          *reinterpret_cast<uint4*>(a_hi + A_HALF + oct * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+          if (NPROD == 3)
+            *reinterpret_cast<uint4*>(a_hi + A_HALF + oct * 128) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
         }
         tc::fence_proxy_async();
         tc::named_sync(1 + wg, 128);         // the warpgroup's 64 rows are written
@@ -241,13 +248,17 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
           const uint64_t bh = tc::smem_desc(wb, 128, 512), bl = tc::smem_desc(wb + WIMG, 128, 512);
           if (ns == NSUB) {
             tc::wgmma_f16_n128(acc, ah, bh, 1);
-            tc::wgmma_f16_n128(acc, al, bh, 1);
-            tc::wgmma_f16_n128(acc, ah, bl, 1);
+            if (NPROD == 3) {
+              tc::wgmma_f16_n128(acc, al, bh, 1);
+              tc::wgmma_f16_n128(acc, ah, bl, 1);
+            }
           } else {
             float (&a32)[32] = *reinterpret_cast<float (*)[32]>(acc);
             tc::wgmma_f16_n64(a32, ah, bh, 1);
-            tc::wgmma_f16_n64(a32, al, bh, 1);
-            tc::wgmma_f16_n64(a32, ah, bl, 1);
+            if (NPROD == 3) {
+              tc::wgmma_f16_n64(a32, al, bh, 1);
+              tc::wgmma_f16_n64(a32, ah, bl, 1);
+            }
           }
         }
         tc::wg_commit();
@@ -373,6 +384,7 @@ extern "C" int sonet_pointwise_tc_pack(const float* W, int Cout, int Cin, void* 
 
 struct TcExt {   // grouped / split-K / scatter / point-major launch options (defaults = the plain layer)
   int groups = 1, splits = 1, scat_w = 0, P_out = 0, conv_w = 0, rows_out = 0;
+  int nprod = 3;   // fp16 products per MAC: 3 (hi/lo split) or 1 (the opt-in fp16 mode)
   const float* inv_ptr = nullptr;
   const float* act_ptr = nullptr;
   long long blob_gstride = 0, out_gstride = 0, out_sstride = 0;
@@ -427,11 +439,20 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   const long long items = static_cast<long long>(d.row_tiles) * d.ntiles * ext.groups * ext.splits;
   SONET_REQUIRE(items < (1LL << 31), "pointwise_tc: too many tiles");
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "pointwise_tc: needs %d B of shared memory", SMEM_BYTES);
-  cudaFuncSetAttribute(pointwise_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+  SONET_REQUIRE(ext.nprod == 3 || (ext.nprod == 1 && !ext.act_ptr && !ext.inv_ptr),
+                "pointwise_tc: the one-product mode is eval-only");
+  auto kern = ext.nprod == 1 ? pointwise_tc_kernel<1> : pointwise_tc_kernel<3>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   const int grid = static_cast<int>(std::min<long long>(items, sm_count()));
-  pointwise_tc_kernel<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
+  kern<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
       x0, x1, static_cast<const unsigned char*>(blob), shift, addend, gidx, out, d, dbg);
   return check_launch("pointwise_tc");
+}
+
+static TcExt with_nprod(int nprod) {
+  TcExt e;
+  e.nprod = nprod;
+  return e;
 }
 
 extern "C" int sonet_pointwise_tc_forward(const float* x0, int C0, const float* x1, int C1, int B,
@@ -443,15 +464,42 @@ extern "C" int sonet_pointwise_tc_forward(const float* x0, int C0, const float* 
                              out, nullptr, stream);
 }
 
+// the opt-in fp16 mode: one product hi(x)*hi(w) per MAC, same blob and arguments
+extern "C" int sonet_pointwise_tc_forward_f16(const float* x0, int C0, const float* x1, int C1, int B,
+                                              int P, const void* blob, float inv_scale,
+                                              const float* shift, int Cout, int relu,
+                                              const float* addend, const int32_t* gidx, int G,
+                                              float* out, sonet_stream_t stream) {
+  return launch_pointwise_tc(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
+                             out, nullptr, stream, with_nprod(1));
+}
+
+static int pointwise_tc_rows(const float* x0, int C0, const float* x1, int C1, int B, int P,
+                             const void* blob, float inv_scale, const float* shift, int Cout, int relu,
+                             const float* addend, const int32_t* gidx, int G, float* out,
+                             sonet_stream_t stream, int nprod) {
+  TcExt e = with_nprod(nprod);
+  e.rows_out = 1;
+  return launch_pointwise_tc(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
+                             out, nullptr, stream, e);
+}
+
 extern "C" int sonet_pointwise_tc_forward_rows(const float* x0, int C0, const float* x1, int C1,
                                                int B, int P, const void* blob, float inv_scale,
                                                const float* shift, int Cout, int relu,
                                                const float* addend, const int32_t* gidx, int G,
                                                float* out, sonet_stream_t stream) {
-  TcExt e;
-  e.rows_out = 1;
-  return launch_pointwise_tc(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
-                             out, nullptr, stream, e);
+  return pointwise_tc_rows(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
+                           out, stream, 3);
+}
+
+extern "C" int sonet_pointwise_tc_forward_rows_f16(const float* x0, int C0, const float* x1, int C1,
+                                                   int B, int P, const void* blob, float inv_scale,
+                                                   const float* shift, int Cout, int relu,
+                                                   const float* addend, const int32_t* gidx, int G,
+                                                   float* out, sonet_stream_t stream) {
+  return pointwise_tc_rows(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
+                           out, stream, 1);
 }
 
 namespace sonet {
@@ -502,13 +550,11 @@ static void launch_splitk_reduce(const float* part, int G, int S, int B, int Cou
 }
 }  // namespace sonet
 
-extern "C" int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, int P,
-                                                  const void* blob, long long blob_gstride,
-                                                  float inv_scale, const float* shift, int Cout,
-                                                  int relu, int groups, int splits, int scat_w,
-                                                  int conv_w, int P_out, long long out_gstride,
-                                                  float* out, float* scratch,
-                                                  sonet_stream_t stream) {
+static int pointwise_tc_grouped(const float* x, int C, int B, int P, const void* blob,
+                                long long blob_gstride, float inv_scale, const float* shift, int Cout,
+                                int relu, int groups, int splits, int scat_w, int conv_w, int P_out,
+                                long long out_gstride, float* out, float* scratch,
+                                sonet_stream_t stream, int nprod) {
   using namespace sonet;
   SONET_REQUIRE(groups >= 1 && splits >= 1 && scat_w >= 0, "pointwise_tc_grouped: bad group/split");
   SONET_REQUIRE(scat_w == 0 || (groups == 4 && P % scat_w == 0 && P_out == 4 * P && out_gstride == 0),
@@ -517,7 +563,7 @@ extern "C" int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, 
   if (B == 0 || P == 0) return SONET_OK;
   if (P_out <= 0) P_out = P;
   SONET_REQUIRE(conv_w == 0 || conv_w == scat_w, "pointwise_tc_grouped: conv_w must equal scat_w");
-  TcExt e;
+  TcExt e = with_nprod(nprod);
   e.groups = groups;
   e.splits = splits;
   e.blob_gstride = blob_gstride;
@@ -538,6 +584,28 @@ extern "C" int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, 
   launch_splitk_reduce(scratch, groups, splits, B, Cout, P, shift, relu, scat_w, P_out, out_gstride, out,
                        as_stream(stream));
   return check_launch("splitk_reduce");
+}
+
+extern "C" int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, int P,
+                                                  const void* blob, long long blob_gstride,
+                                                  float inv_scale, const float* shift, int Cout,
+                                                  int relu, int groups, int splits, int scat_w,
+                                                  int conv_w, int P_out, long long out_gstride,
+                                                  float* out, float* scratch,
+                                                  sonet_stream_t stream) {
+  return pointwise_tc_grouped(x, C, B, P, blob, blob_gstride, inv_scale, shift, Cout, relu, groups,
+                              splits, scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 3);
+}
+
+extern "C" int sonet_pointwise_tc_grouped_forward_f16(const float* x, int C, int B, int P,
+                                                      const void* blob, long long blob_gstride,
+                                                      float inv_scale, const float* shift, int Cout,
+                                                      int relu, int groups, int splits, int scat_w,
+                                                      int conv_w, int P_out, long long out_gstride,
+                                                      float* out, float* scratch,
+                                                      sonet_stream_t stream) {
+  return pointwise_tc_grouped(x, C, B, P, blob, blob_gstride, inv_scale, shift, Cout, relu, groups,
+                              splits, scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 1);
 }
 
 // Train-mode variant: the weight blob was packed on the device this step

@@ -91,6 +91,18 @@ __device__ __forceinline__ void split2_f16(float a, float b, uint32_t& hi, uint3
   const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
   lo = pack_f16x2_sat(a - hf.x, b - hf.y);
 }
+// The A-operand words of one product count: NPROD = 3 is split2_f16; NPROD = 1 (the opt-in fp16
+// mode, x*w ~= hi(x)*hi(w)) writes only the hi word, the same bits split2_f16 writes, and leaves
+// lo untouched. In that mode the kernels issue one wgmma per K step and read only the hi image of
+// each weight stage: |err| ~ 2^-11 * sum_k |w_k x_k| instead of the split's 4e-6.
+template <int NPROD>
+__device__ __forceinline__ void split_words(float a, float b, uint32_t& hi, uint32_t& lo) {
+  static_assert(NPROD == 1 || NPROD == 3, "one or three fp16 products");
+  if constexpr (NPROD == 3)
+    split2_f16(a, b, hi, lo);
+  else
+    hi = pack_f16x2_sat(a, b);
+}
 
 // Spin on the barrier phase; a protocol bug traps (instead of hanging the GPU) after 2^24 failed
 // try_waits.

@@ -134,6 +134,12 @@ _SIGNATURES = {
     "sonet_last_error_string": [],
     "sonet_version": [],
 }
+# the opt-in fp16 mode: one entry per eval wgmma entry, same arguments
+for _name in ("sonet_pointresnet_tc_forward", "sonet_pointresnet_tc_pool_forward",
+              "sonet_pointwise_tc_forward", "sonet_pointwise_tc_forward_rows",
+              "sonet_pointwise_tc_grouped_forward", "sonet_knn_mlp_tc_forward"):
+    _SIGNATURES[_name + "_f16"] = _SIGNATURES[_name]
+F16_ENTRIES = tuple(n for n in _SIGNATURES if n.endswith("_f16"))
 _RESTYPE = {"sonet_last_error_string": ctypes.c_char_p, "sonet_version": ctypes.c_char_p,
             "sonet_pointwise_tc_blob_bytes": ctypes.c_longlong,
             "sonet_knn_mlp_tc_blob_bytes": ctypes.c_longlong,

@@ -15,7 +15,7 @@ re-bound to the replayed graph's buffers on every replay.
 """
 import torch
 
-from . import ops
+from . import layers, ops
 
 
 class _InputSet:
@@ -98,7 +98,6 @@ class GraphedModel:
     def invalidate(self):
         """Forget folded/packed weights and captured graphs (call after editing parameters
         through `.data`, which does not bump tensor versions — see layers.invalidate)."""
-        from . import layers
         for m in self._state_modules():
             layers.invalidate(m)
         self._graphs = {}
@@ -116,8 +115,11 @@ class GraphedModel:
         ver = 0
         for t in self._state_tensors:
             ver += t._version
+        # the precision mode picks the kernels a forward launches: a graph captured in one mode
+        # must not replay in another
         return (tuple(tuple(t.shape) for t in s.t.values()), ver,
-                getattr(self.encoder, "fuse_pool", None), getattr(self.encoder, "_fpo_demand", None))
+                getattr(self.encoder, "fuse_pool", None), getattr(self.encoder, "_fpo_demand", None),
+                layers.tc_mode())
 
     def _resolve(self, path):
         obj = self

@@ -88,10 +88,29 @@ def _make_act(activation):
     return None
 
 
+def tc_mode():
+    """The eval-mode precision of the tensor-core layers, from SONET_TC, read at call time so a
+    change applies from the next forward on (a captured CUDA graph is re-captured):
+      "fp32"  SONET_TC=0: every layer on the exact-fp32 CUDA-core kernels;
+      "fp16"  SONET_TC=fp16: every wgmma GEMM as one fp16 product per MAC (the `_f16` entries);
+      "split" anything else, unset and 1 included: the fp16 hi/lo 3-product split (default).
+    Train mode ignores it. No other module reads the variable."""
+    v = os.environ.get("SONET_TC", "1")
+    if v == "0":
+        return "fp32"
+    if v == "fp16":
+        return "fp16"
+    return "split"
+
+
 def tc_enabled():
-    """True unless SONET_TC=0, which routes every layer to the exact-fp32 CUDA-core kernels.
-    Read at call time, so a change applies from the next forward on."""
-    return os.environ.get("SONET_TC", "1") != "0"
+    """True unless SONET_TC=0, which routes every layer to the exact-fp32 CUDA-core kernels."""
+    return tc_mode() != "fp32"
+
+
+def tc_f16():
+    """True under SONET_TC=fp16: the eval wgmma launches take their one-product `_f16` entries."""
+    return tc_mode() == "fp16"
 
 
 _stamps = itertools.count(1)
@@ -264,7 +283,7 @@ class _PointwiseConvBase(nn.Module):
         if cin >= 32 and rows >= 256 and tc_enabled():
             blob, inv, shift = self._tc_params()
             return ops.pointwise_layer_tc(x0, blob, inv, shift, cout, self.activation == 'relu',
-                                          x1=x1, addend=addend, gidx=gidx)
+                                          x1=x1, addend=addend, gidx=gidx, f16=tc_f16())
         w, shift = self.folded(transpose=True)
         return ops.pointwise_layer(x0, w, None, shift, self.activation == 'relu', x1=x1,
                                    addend=addend, gidx=gidx)
@@ -409,6 +428,7 @@ class UpConv(nn.Module):
         if not self._fast(x):
             return self.conv(self.up_sample(x))
         pk = self._packed()
+        f16 = tc_f16()
         B, Cin, H, W = x.shape
         Cout = self.conv.conv.out_channels
         relu = self.activation == 'relu'
@@ -419,7 +439,7 @@ class UpConv(nn.Module):
             scratch = self._scratch_for(splits * B * 4 * Cout, x.device) if splits > 1 else None
             y = ops.pointwise_tc_grouped(x.view(B, Cin, 1), pk["blob1"], pk["per1"], pk["inv1"],
                                          pk["shift1"], 4 * Cout, relu, groups=1, splits=splits,
-                                         scratch=scratch)
+                                         scratch=scratch, f16=f16)
             return y.view(B, Cout, 2, 2)
         P = H * W
         kch = (4 * Cin + 63) // 64
@@ -431,7 +451,7 @@ class UpConv(nn.Module):
         xin = ops.upconv_hshift(x) if conv else ops.upconv_im2col(x)      # [3B,Cin,HW] | [4B,4Cin,HW]
         y = ops.pointwise_tc_grouped(xin, pk["blob4"], pk["per4"], pk["inv4"], pk["shift"], Cout,
                                      relu, groups=4, splits=splits, scat_w=W, scratch=scratch,
-                                     conv=conv)
+                                     conv=conv, f16=f16)
         return y.view(B, Cout, 2 * H, 2 * W)
 
 
@@ -536,9 +556,10 @@ class KNNModule(nn.Module):
         """x [B,C,M] -> knn_feature [B,512,M]: Y = W1f x once per node, stored node-major so the
         fused kernel gathers each neighbour's channels as contiguous pairs, then one fused launch."""
         pk = self._tc_params()
-        y = ops.pointwise_layer_tc(x, pk["yblob"], pk["yinv"], None, 512, False, rows=True)
+        f16 = tc_f16()
+        y = ops.pointwise_layer_tc(x, pk["yblob"], pk["yinv"], None, 512, False, rows=True, f16=f16)
         return ops.knn_mlp_tc(coord, center, knn_I, K, y.transpose(1, 2), pk["w1"], pk["blob2"],
-                              pk["inv2"], pk["shift2"])
+                              pk["inv2"], pk["shift2"], f16=f16)
 
     def forward_pooled(self, coordinate, pool, precomputed_knn_I, K, center_type, epoch=None,
                        owner=None):
@@ -690,7 +711,7 @@ class PointResNet(nn.Module):
         if first.fast(x) and x.dim() == 3 and all(l.fast(x) for l in self.layers) \
                 and self._tc_eligible(x.shape[1], x1):
             blob, fpar = self._tc_params()
-            return ops.pointresnet_tc(x.contiguous(), blob, fpar)
+            return ops.pointresnet_tc(x.contiguous(), blob, fpar, f16=tc_f16())
         if first.fast(x) and x.dim() == 3 and all(l.fast(x) for l in self.layers):
             layer0_out = first.forward_points(x.contiguous(),
                                               None if x1 is None else x1.contiguous())

@@ -18,7 +18,7 @@ import torch.nn as nn
 
 from . import ops, som, train_ops
 from .layers import (EquivariantLayer, KNNModule, MyConv2d, MyLinear, PointNet, PointResNet,
-                     UpConv, _Cache, _fast_ok, _pick_splits, tc_enabled)
+                     UpConv, _Cache, _fast_ok, _pick_splits, tc_enabled, tc_f16)
 
 
 def _bn_kwargs(opt):
@@ -183,7 +183,7 @@ class Encoder(nn.Module):
                 xs, ns, p0 = ops.som_sort_decenter(xd, snd, self.som_node, idx32, a["count"], k)
             blob, fpar = fpn._tc_params()
             pooled = ops.pointresnet_tc_pool(xs, blob, fpar, ns, p0, M, finalize=False,
-                                             owner=self._pool_keys)
+                                             owner=self._pool_keys, f16=tc_f16())
             done = None
             if opt.som_k >= 2:   # pool_finalize folds into the KNN module's input assembly
                 done = self.knnlayer.forward_pooled(self.som_node, pooled, node_knn_I, opt.som_k,
@@ -389,6 +389,7 @@ class Segmenter(nn.Module):
         cloud_add = ops.linear(cloud.contiguous(), w_cloud, None, None, False).unsqueeze(2)  # [B,1024,1]
         relu1 = self.layer1.activation == 'relu'
         if tc_enabled():
+            f16 = tc_f16()
             bp, ip, bn, pern, inn = tc
             cout = w_point.shape[1]
             # [B,1920,M] -> [B,1024,M]: 16 row tiles x 4 column tiles would leave the GPU to 64
@@ -397,10 +398,10 @@ class Segmenter(nn.Module):
             kch = (node_in.shape[1] + 63) // 64
             splits = _pick_splits(kch, ((B * M + 127) // 128) * ((cout + 255) // 256))
             addend = ops.pointwise_tc_grouped(node_in, bn, pern, inn, None, cout, False, groups=1,
-                                              splits=splits) + cloud_add            # [B,1024,M]
+                                              splits=splits, f16=f16) + cloud_add   # [B,1024,M]
             out1 = ops.pointwise_layer_tc(pt, bp, ip, shift, cout, relu1,
                                           x1=first_pn_out.contiguous(), addend=addend,
-                                          gidx=min_idx_i32)
+                                          gidx=min_idx_i32, f16=f16)
         else:
             node_a = torch.cat((node_first, node_knn), dim=1).contiguous()
             addend = ops.pointwise_layer(node_a, w_node, None, None, False,

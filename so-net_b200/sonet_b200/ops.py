@@ -32,6 +32,12 @@ def _stream(t):
     return torch.cuda.current_stream(t.device).cuda_stream
 
 
+def _entry(name, f16):
+    """The C-ABI entry of an eval wgmma launch: `name`, or with f16 its one-product `_f16` twin
+    (same arguments; include/sonet_b200.h)."""
+    return name + "_f16" if f16 else name
+
+
 def _call(name, *args, kernels=None):
     global LAUNCHES, KERNEL_LAUNCHES
     LAUNCHES += 1
@@ -420,16 +426,17 @@ def pointresnet_tc_pack(W, shifts, cin):
     return blob, fparams
 
 
-def pointresnet_tc(x, blob, fparams):
-    """x [B,Cin<=6,P] f32 -> [B,384,P]: the fused wgmma first PointResNet."""
+def pointresnet_tc(x, blob, fparams, f16=False):
+    """x [B,Cin<=6,P] f32 -> [B,384,P]: the fused wgmma first PointResNet (f16: one fp16 product
+    per MAC instead of the hi/lo split's three)."""
     _chk(x, "x", torch.float32)
     _chk(blob, "blob", torch.uint8)
     _chk(fparams, "fparams", torch.float32)
     B, Cin, P = x.shape
     with torch.cuda.device(x.device):
         out = torch.empty((B, 384, P), dtype=torch.float32, device=x.device)
-        _call("sonet_pointresnet_tc_forward", _C.ptr(x), Cin, B, P, _C.ptr(blob), _C.ptr(fparams),
-              _C.ptr(out), _stream(x))
+        _call(_entry("sonet_pointresnet_tc_forward", f16), _C.ptr(x), Cin, B, P, _C.ptr(blob),
+              _C.ptr(fparams), _C.ptr(out), _stream(x))
     return out
 
 
@@ -485,10 +492,11 @@ def upconv_hshift(x):
 
 
 def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, groups, splits=1,
-                         scat_w=0, out=None, scratch=None, conv=False):
+                         scat_w=0, out=None, scratch=None, conv=False, f16=False):
     """Grouped wgmma layer: x [G*B, C, P], G weight blobs -> out. scat_w = W > 0: the four groups
     are the output parities of an up-convolution over [H, W] maps, interleaved into
-    out [B, cout, 4*P]; otherwise out [G*B, cout, P]. splits > 1: K split through `scratch`."""
+    out [B, cout, 4*P]; otherwise out [G*B, cout, P]. splits > 1: K split through `scratch`.
+    f16: one fp16 product per MAC instead of the hi/lo split's three."""
     _chk(x, "x", torch.float32)
     _chk(blob, "blob", torch.uint8)
     _chk(shift, "shift", torch.float32, optional=True)
@@ -506,7 +514,8 @@ def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, group
                 out = torch.empty((GB, cout, P), dtype=torch.float32, device=dev)
         if splits > 1 and scratch is None:
             scratch = torch.empty((groups * splits * B * cout * P,), dtype=torch.float32, device=dev)
-        _call("sonet_pointwise_tc_grouped_forward", _C.ptr(x), C, B, P, _C.ptr(blob), int(per_bytes),
+        _call(_entry("sonet_pointwise_tc_grouped_forward", f16), _C.ptr(x), C, B, P, _C.ptr(blob),
+              int(per_bytes),
               float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)), int(groups), int(splits),
               int(scat_w), int(scat_w) if conv else 0, int(P_out), int(gstride), _C.ptr(out),
               _C.ptr(scratch), _stream(x),
@@ -515,9 +524,10 @@ def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, group
 
 
 def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=None, gidx=None,
-                       rows=False):
+                       rows=False, f16=False):
     """wgmma variant of pointwise_layer: x0 [B,C0,P] (+ x1) -> [B,cout,P], or with rows=True the
-    same values point-major, [B,P,cout]."""
+    same values point-major, [B,P,cout]. f16: one fp16 product per MAC instead of the hi/lo
+    split's three."""
     _chk(x0, "x0", torch.float32)
     _chk(x1, "x1", torch.float32, optional=True)
     _chk(blob, "blob", torch.uint8)
@@ -530,12 +540,13 @@ def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=N
     with torch.cuda.device(x0.device):
         if rows:
             out = torch.empty((B, P, cout), dtype=torch.float32, device=x0.device)
-            _call("sonet_pointwise_tc_forward_rows", _C.ptr(x0), C0, _C.ptr(x1), C1, B, P,
+            _call(_entry("sonet_pointwise_tc_forward_rows", f16), _C.ptr(x0), C0, _C.ptr(x1), C1, B, P,
                   _C.ptr(blob), float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)),
                   _C.ptr(addend), _C.ptr(gidx), G, _C.ptr(out), _stream(x0))
         else:
             out = torch.empty((B, cout, P), dtype=torch.float32, device=x0.device)
-            _call("sonet_pointwise_tc_forward", _C.ptr(x0), C0, _C.ptr(x1), C1, B, P, _C.ptr(blob),
+            _call(_entry("sonet_pointwise_tc_forward", f16), _C.ptr(x0), C0, _C.ptr(x1), C1, B, P,
+                  _C.ptr(blob),
                   float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)), _C.ptr(addend),
                   _C.ptr(gidx), G, _C.ptr(out), _stream(x0))
     return out
@@ -556,12 +567,13 @@ def knn_mlp_tc_pack(W2):
     return blob, float(inv.value)
 
 
-def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2):
+def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2, f16=False):
     """The KNN module's layer 1 (from the per-node Y = W1f x [B,512,M]) + layer 2 + max over the
     K neighbours in one wgmma kernel. coord, center [B,3,M]; idx [B,M,K'] i64; w1 [512,4] =
     (W1d | shift1); shift2 [512] -> knn_feature_1 [B,512,M]. Y is [B,512,M] either contiguous or
     the channel-fastest view y.transpose(1, 2) of a contiguous [B,M,512] (pointwise_layer_tc(...,
-    rows=True)); the kernel reads the latter as float2 pairs, with bit-identical results."""
+    rows=True)); the kernel reads the latter as float2 pairs, with bit-identical results.
+    f16: layer 2 as one fp16 product per MAC instead of the hi/lo split's three."""
     _chk(coord, "coordinate", torch.float32)
     _chk(center, "center", torch.float32)
     _chk(idx, "knn_I", torch.int64)
@@ -579,8 +591,8 @@ def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2):
                            % (tuple(coord.shape), tuple(Y.shape), tuple(w1.shape), tuple(idx.shape)))
     with torch.cuda.device(coord.device):
         out = torch.empty((B, 512, M), dtype=torch.float32, device=coord.device)
-        _call("sonet_knn_mlp_tc_forward", _C.ptr(coord), _C.ptr(center), _C.ptr(idx), B, M, int(K),
-              idx.shape[2], _C.ptr(Y), Y.stride(1), Y.stride(2), _C.ptr(w1), _C.ptr(blob),
+        _call(_entry("sonet_knn_mlp_tc_forward", f16), _C.ptr(coord), _C.ptr(center), _C.ptr(idx), B,
+              M, int(K), idx.shape[2], _C.ptr(Y), Y.stride(1), Y.stride(2), _C.ptr(w1), _C.ptr(blob),
               float(inv_scale), _C.ptr(shift2), _C.ptr(out), _stream(coord))
     return out
 
@@ -714,9 +726,11 @@ def knn_assemble_pool(coord, keys, p0, idx, K, center_type, owner=None, want_x_a
     return center, x_aug, mm
 
 
-def pointresnet_tc_pool(x_sorted, blob, fparams, node_sorted, pos0, M, finalize=True, owner=None):
+def pointresnet_tc_pool(x_sorted, blob, fparams, node_sorted, pos0, M, finalize=True, owner=None,
+                        f16=False):
     """Fused wgmma PointResNet + per-node max: -> first_pn_out_masked_max [B,384,M], or with
-    finalize=False the raw (keys [B,384,M] i32, p0 [B,384]) for knn_assemble_pool / pool_finalize."""
+    finalize=False the raw (keys [B,384,M] i32, p0 [B,384]) for knn_assemble_pool / pool_finalize.
+    f16: one fp16 product per MAC instead of the hi/lo split's three."""
     _chk(x_sorted, "x_sorted", torch.float32)
     _chk(blob, "blob", torch.uint8)
     _chk(fparams, "fparams", torch.float32)
@@ -727,7 +741,8 @@ def pointresnet_tc_pool(x_sorted, blob, fparams, node_sorted, pos0, M, finalize=
     with torch.cuda.device(dev):
         keys = (owner or _DEFAULT_POOL_KEYS).acquire(dev, B, M, _stream(x_sorted))
         p0 = torch.empty((B, 384), dtype=torch.float32, device=dev)
-        _call("sonet_pointresnet_tc_pool_forward", _C.ptr(x_sorted), Cin, B, P, _C.ptr(blob),
+        _call(_entry("sonet_pointresnet_tc_pool_forward", f16), _C.ptr(x_sorted), Cin, B, P,
+              _C.ptr(blob),
               _C.ptr(fparams), _C.ptr(node_sorted), _C.ptr(pos0), int(M), _C.ptr(keys), _C.ptr(p0),
               _stream(x_sorted))
     if not finalize:
