@@ -323,6 +323,35 @@ int sonet_seg_iou_cpu_f32(const float* score, const long long* seg, const long l
                           int num_categories, double* iou_shape, long long* pred, int32_t* correct,
                           int thread_num);
 
+/* SHREC'16 same-label retrieval ranking (shrec16/test.py:64-99). feature [Q,D] f32; label_in [Q]
+ * int64, or NULL for the row argmax (lowest index on ties, first NaN wins). For each query q, the
+ * items p with label p == label q (q included) ranked by d = float(sqrt(sum_j double(f_q[j] -
+ * f_p[j])^2)) (fp32 differences, fp64 sum in index order), ascending, ties by ascending p, NaN last;
+ * at most k of them. Outputs [Q,k]: idx int64 (p, -1 past count), dist f32 (NaN past count);
+ * count [Q] int32 = min(group size, k), or -1 when the label is outside [0,L) (that item is nobody's
+ * candidate); label_out [Q] int64 (nullable). Limits: 1 <= D <= 1024, 1 <= k <= 4096,
+ * 1 <= L <= 4096, Q*k < 2^31. Deterministic. The device entry takes
+ * sonet_retrieval_scratch_bytes(Q, D, L, k) bytes of 256-byte aligned device scratch, makes no
+ * allocation and no host synchronisation; it returns -1 (bad arguments) from the size query. */
+long long sonet_retrieval_scratch_bytes(int Q, int D, int L, int k);
+int sonet_retrieval_rank_f32(const float* feature, const long long* label_in, int Q, int D, int L,
+                             int k, void* scratch, long long scratch_bytes, long long* idx,
+                             float* dist, int32_t* count, long long* label_out,
+                             sonet_stream_t stream);
+/* The same over host pointers, bit for bit, queries split over at most thread_num threads. */
+int sonet_retrieval_rank_cpu_f32(const float* feature, const long long* label_in, int Q, int D, int L,
+                                 int k, long long* idx, float* dist, int32_t* count,
+                                 long long* label_out, int thread_num);
+/* The bytes np.savetxt(f, rows, fmt='%06d %f') writes for each query's float64 rows
+ * (ids[idx[q,i]], dist[q,i]), i < count[q]; host pointers, no file I/O. out == NULL: size query,
+ * writes offsets [Q+1] (query q's text is out[offsets[q] .. offsets[q+1])) and returns the total.
+ * Otherwise formats into out at those offsets (which must come from the size query) and returns
+ * the total. Ids pass through double as numpy's float64 rows do; NaN prints "nan". Returns -1 when
+ * a count is outside [0,k] or an idx outside [0,Q). */
+long long sonet_retrieval_format_cpu(const long long* ids, const long long* idx, const float* dist,
+                                     const int32_t* count, int Q, int k, long long* offsets,
+                                     char* out, int thread_num);
+
 /* ---- a-11: Chamfer distance ------------------------------------------------------------------------
  * Replaces ChamferLoss.forward (models/losses.py:237-290) including the Faiss IndexFlatL2
  * k=1 searches (losses.py:209-235) — exact brute force, direct differences, lowest index on ties.

@@ -84,6 +84,14 @@ _SIGNATURES = {
                           c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "sonet_seg_iou_cpu_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                               c_int, c_void_p, c_void_p, c_void_p, c_int],
+    "sonet_retrieval_scratch_bytes": [c_int, c_int, c_int, c_int],
+    "sonet_retrieval_rank_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                 ctypes.c_longlong, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p],
+    "sonet_retrieval_rank_cpu_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_int],
+    "sonet_retrieval_format_cpu": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                   c_void_p, c_int],
     "sonet_chamfer_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sonet_pointresnet_tc_blob_bytes": [],
@@ -145,6 +153,8 @@ _RESTYPE = {"sonet_last_error_string": ctypes.c_char_p, "sonet_version": ctypes.
             "sonet_knn_mlp_tc_blob_bytes": ctypes.c_longlong,
             "sonet_som_group_smem_bytes": ctypes.c_longlong,
             "sonet_seg_loss_scratch_bytes": ctypes.c_longlong,
+            "sonet_retrieval_scratch_bytes": ctypes.c_longlong,
+            "sonet_retrieval_format_cpu": ctypes.c_longlong,
             "sonet_wgrad_kpad": ctypes.c_longlong, "sonet_wgrad_blob_bytes": ctypes.c_longlong,
             "sonet_wgrad_small_floats": ctypes.c_longlong}
 

@@ -5,6 +5,8 @@ device and the current torch stream. Inputs must be CUDA, contiguous, of the sta
 same checks the reference plugin does with CHECK_INPUT (models/index_max_ext/index_max.cpp:119-121),
 raised as RuntimeError. Nothing here falls back to PyTorch or the CPU.
 """
+import ctypes
+
 import torch
 
 from . import _C
@@ -380,6 +382,91 @@ def seg_iou(score, seg, label, table=None, want_pred=False, want_correct=False):
               _C.ptr(offsets), _C.ptr(ids), K, _C.ptr(iou), _C.ptr(pred), _C.ptr(correct),
               _stream(score))
     return iou, pred, correct
+
+
+RETRIEVAL_MAX_D = 1024
+RETRIEVAL_MAX_K = 4096
+RETRIEVAL_MAX_L = 4096
+
+
+def retrieval_rank(feature, label=None, num_labels=None, k=1000, threads=None):
+    """Same-label retrieval ranking (shrec16/test.py:64-99) of every item, no sync.
+
+    feature [Q,D] f32; label [Q] int64 on the same device, or None for the row argmax (lowest
+    index on ties, the first NaN wins); num_labels L (default D): labels live in [0, L). For each
+    query q, the items p with the same label (q included) sorted by the fp32 distance
+    ||f_q - f_p||_2 (fp32 differences summed in fp64), ties by ascending p, NaN last, at most k.
+    Returns (idx [Q,k] int64, dist [Q,k] f32, count [Q] int32, label [Q] int64) on the features'
+    device: slots past count[q] hold -1 / NaN, and count[q] = -1 flags a label outside [0, L).
+    CUDA tensors run the sm_90a kernels; CPU tensors run the host entry (bit-identical), over
+    `threads` threads (default torch.get_num_threads())."""
+    if not isinstance(feature, torch.Tensor) or feature.dtype != torch.float32 or feature.dim() != 2:
+        raise RuntimeError("retrieval_rank: feature must be a [Q,D] float32 tensor")
+    if not feature.is_contiguous():
+        raise RuntimeError("feature must be contiguous")
+    Q, D = feature.shape
+    L = D if num_labels is None else int(num_labels)
+    k = int(k)
+    if not 1 <= D <= RETRIEVAL_MAX_D:
+        raise RuntimeError("retrieval_rank: D=%d outside [1, %d]" % (D, RETRIEVAL_MAX_D))
+    if not 1 <= k <= RETRIEVAL_MAX_K:
+        raise RuntimeError("retrieval_rank: k=%d outside [1, %d]" % (k, RETRIEVAL_MAX_K))
+    if not 1 <= L <= RETRIEVAL_MAX_L:
+        raise RuntimeError("retrieval_rank: num_labels=%d outside [1, %d]" % (L, RETRIEVAL_MAX_L))
+    if Q * k >= 1 << 31:
+        raise RuntimeError("retrieval_rank: Q*k=%d must be < 2^31" % (Q * k))
+    if label is not None:
+        if label.dtype != torch.int64 or tuple(label.shape) != (Q,) or label.device != feature.device:
+            raise RuntimeError("retrieval_rank: label must be int64 [Q=%d] on %s" % (Q, feature.device))
+        if not label.is_contiguous():
+            raise RuntimeError("label must be contiguous")
+    dev = feature.device
+    idx = torch.empty((Q, k), dtype=torch.int64, device=dev)
+    dist = torch.empty((Q, k), dtype=torch.float32, device=dev)
+    count = torch.empty((Q,), dtype=torch.int32, device=dev)
+    label_out = torch.empty((Q,), dtype=torch.int64, device=dev) if label is None else label
+    out_ptr = _C.ptr(label_out) if label is None else None
+    if not feature.is_cuda:
+        nt = torch.get_num_threads() if threads is None else int(threads)
+        _C.check(_C.lib().sonet_retrieval_rank_cpu_f32(
+            feature.data_ptr(), _C.ptr(label), Q, D, L, k, idx.data_ptr(), dist.data_ptr(),
+            count.data_ptr(), out_ptr, nt), "sonet_retrieval_rank_cpu_f32")
+        return idx, dist, count, label_out
+    with torch.cuda.device(dev):
+        nbytes = int(_C.lib().sonet_retrieval_scratch_bytes(Q, D, L, k))
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        _call("sonet_retrieval_rank_f32", _C.ptr(feature), _C.ptr(label), Q, D, L, k, _C.ptr(scratch),
+              nbytes, _C.ptr(idx), _C.ptr(dist), _C.ptr(count), out_ptr, _stream(feature), kernels=4)
+    return idx, dist, count, label_out
+
+
+def retrieval_format(ids, idx, dist, count, threads=None):
+    """Host bytes of np.savetxt(f, rows, fmt='%06d %f') per query, for the rows
+    (ids[idx[q,i]], dist[q,i]), i < count[q], of a retrieval_rank result (CPU tensors).
+    Returns (text bytes, offsets [Q+1] int64): query q's file is text[offsets[q]:offsets[q+1]]."""
+    Q, k = idx.shape
+    for t, name, dt in ((ids, "ids", torch.int64), (idx, "idx", torch.int64),
+                        (dist, "dist", torch.float32), (count, "count", torch.int32)):
+        if t.is_cuda or t.dtype != dt or not t.is_contiguous():
+            raise RuntimeError("retrieval_format: %s must be a contiguous CPU %s tensor" % (name, dt))
+    if tuple(ids.shape) != (Q,) or tuple(dist.shape) != (Q, k) or tuple(count.shape) != (Q,):
+        raise RuntimeError("retrieval_format: expected ids [Q], idx/dist [Q,k], count [Q]")
+    nt = torch.get_num_threads() if threads is None else int(threads)
+    lib = _C.lib()
+    offsets = torch.empty((Q + 1,), dtype=torch.int64)
+    args = (ids.data_ptr(), idx.data_ptr(), dist.data_ptr(), count.data_ptr(), Q, k,
+            offsets.data_ptr())
+    total = lib.sonet_retrieval_format_cpu(*args, None, nt)
+    if total < 0:
+        raise RuntimeError("retrieval_format failed: %s" % _C.last_error())
+    if total == 0:
+        return b"", offsets
+    buf = bytearray(total)
+    cbuf = (ctypes.c_char * total).from_buffer(buf)
+    if lib.sonet_retrieval_format_cpu(*args, ctypes.addressof(cbuf), nt) != total:
+        raise RuntimeError("retrieval_format failed: %s" % _C.last_error())
+    del cbuf
+    return bytes(buf), offsets
 
 
 def chamfer(pred, gt, want_idx=False):
