@@ -209,11 +209,13 @@ int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Cout, int Cin
  * som.py:209-212) or [B,3,M] (node_init_batched = 1; a single batch_update on the current nodes);
  * weights [T,M,M] f32: weights[t][m][j] = get_weighting_matrix(sigma_t)[m] at grid cell j
  * (som.py:232-235); lr [T] f32. node_out [B,3,M] (may alias a batched node_init).
- * last_idx (nullable) [B,N] i32 = the assignment computed in the last iteration.
+ * last_idx (nullable) [B,N] i32 = the assignment computed in the last iteration; with T = 0 the
+ * assignment against node_init (the arithmetic of iteration 1), and node_out = node_init.
  * Numerics: distances bit-equal to ((x-node)**2).sum(1), first minimal node on ties
  * (torch.min); sums accumulated in fp64 in a fixed order and rounded once (the reference's
  * cascade torch.sum is ~1 ulp accurate; plain fp32 accumulation diverges through assignment
- * flips); mean = sum / (count + 1e-5f); node += sum_m ((mean_m - node_j) * occupied_m) * W[m][j] * lr.
+ * flips); mean = sum / (count + 1e-5f); node += sum_m ((mean_m - node_j) * occupied_m) * W[m][j] * lr,
+ * that sum over m carried exactly (fp64 TwoSum) and rounded once to the nearest fp32.
  * M <= 256; N up to ~17k points with the cloud resident in shared memory (larger N re-reads x
  * through L2; N <= ~220k). */
 int sonet_som_train(const float* x, const float* node_init, int node_init_batched,

@@ -219,20 +219,31 @@ def som_cloud(rs, B, N):
     return np.ascontiguousarray(x, dtype=np.float32)
 
 
+# SOM training fixtures: (file, grid side, clouds, points, cloud seed). The reference's scripts
+# default to an 8x8 grid; the others cover the library's range of square grids (3x3 .. 16x16).
+SOM_TRAIN_CASES = (("som_train", 8, 3, 700, 17), ("som_train_m9", 3, 2, 700, 18),
+                   ("som_train_m121", 11, 2, 700, 19), ("som_train_m256", 16, 2, 700, 20))
+
+
 def gen_som_train(ref):
     """§8f-4: BatchSOM.optimize / batch_update of the reference (util/som.py:295-366) on seeded
-    clouds; pins the oracle restatement bit-exactly against it."""
-    rs = np.random.RandomState(17)
-    B, N = 3, 700
+    clouds, one fixture per grid size of SOM_TRAIN_CASES; pins the oracle restatement
+    bit-exactly against it at every size."""
+    for tag, rows, B, N, seed in SOM_TRAIN_CASES:
+        gen_som_train_grid(ref, tag, rows, B, N, seed)
+
+
+def gen_som_train_grid(ref, tag, rows, B, N, seed):
+    rs = np.random.RandomState(seed)
     x = torch.from_numpy(som_cloud(rs, B, N))
-    som = ref.som.BatchSOM(8, 8, 3, 0, B)
+    som = ref.som.BatchSOM(rows, rows, 3, 0, B)
     out = dict(x=x.numpy(), node_init_value=som.node_init_value.numpy().copy())
     som.node_init(B)
     som.batch_update(x, 0.5, 0.4)                       # one step from the potential-field start
     out["node_after_1"] = som.node.numpy().copy()
     som.batch_update(x, 0.31, 0.22)                     # a second one with a narrower neighbourhood
     out["node_after_2"] = som.node.numpy().copy()
-    init_w = oracle.som_init_weighting_matrix(8, 8)
+    init_w = oracle.som_init_weighting_matrix(rows, rows)
     assert torch.equal(init_w, som.init_weighting_matrix)
     n0 = som.node_init_value.unsqueeze(0).expand(B, -1, -1).contiguous()
     n1, _ = oracle.som_batch_update(n0, x, init_w, 0.5, 0.4)
@@ -241,10 +252,10 @@ def gen_som_train(ref):
     assert torch.equal(n2, torch.from_numpy(out["node_after_2"]))
     som.optimize(x)
     out["node_optimized"] = som.node.numpy().copy()
-    o = oracle.som_optimize(x, som.node_init_value, 8, 8)
+    o = oracle.som_optimize(x, som.node_init_value, rows, rows)
     assert torch.equal(o, som.node), "oracle som_optimize != reference"
-    np.savez_compressed(os.path.join(GOLDEN, "som_train.npz"), **out)
-    print("som_train.npz: reference BatchSOM == oracle restatement (bit-exact)")
+    np.savez_compressed(os.path.join(GOLDEN, tag + ".npz"), **out)
+    print("%s.npz: reference BatchSOM == oracle restatement (bit-exact)" % tag)
 
 
 def gen_augment(ref):

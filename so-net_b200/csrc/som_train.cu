@@ -19,7 +19,8 @@
 //      with the reference to 1.2e-7. mean = sum / (count + 1e-5f) in fp32.
 //   3. node update (:325-347): delta[c][j] = sum_m ((mean[c][m] - node[c][j]) * occupied[m])
 //      * W_t[m][j] * lr_t, products rounded to fp32 in the reference's order, summed over m
-//      (fp64 accumulate, one fp32 rounding); node += delta.
+//      (fp64 TwoSum accumulate, one fp32 rounding of the exact sum: exact_sum_to_float); node +=
+//      delta.
 // W_t (the neighbourhood weighting matrix of get_weighting_matrix, :232-235) and lr_t are inputs:
 // the host computes the schedule with the reference's own expressions.
 //
@@ -34,6 +35,20 @@ namespace sonet {
 constexpr int ST_THREADS = 1024;
 constexpr int ST_WARPS = ST_THREADS / 32;
 constexpr int ST_MAX_M = 256;
+
+// fp32 nearest to hi + lo (an fp64 TwoSum accumulation: hi the running sum, lo its exact rounding
+// errors). A plain (float)hi rounds twice: when two comparable terms sum exactly onto an fp32
+// midpoint and a far smaller neighbourhood-tail term (W ~ 1e-21) decides the side, fp64 has
+// dropped that term and ties-to-even may pick the wrong side. Rounding hi + lo to odd in fp64
+// first keeps the sticky information, and odd-then-nearest with 53 >= 24 + 2 bits is one rounding.
+__device__ __forceinline__ float exact_sum_to_float(double hi, double lo) {
+  const double s = hi + lo, bb = s - hi;
+  const double e = (hi - (s - bb)) + (lo - bb);           // s + e == hi + lo
+  double r = s;
+  if (e != 0.0 && (__double_as_longlong(s) & 1) == 0)   // inexact and even: step toward the rest
+    r = nextafter(s, e > 0.0 ? HUGE_VAL : -HUGE_VAL);
+  return __double2float_rn(r);
+}
 
 // smem: nodes as float4 [M] | mean float [3][M] + occupied [M] | W_t [M][M] (optional) |
 //       x [3][N] (optional) | idx u8 [N]
@@ -76,14 +91,8 @@ __global__ void __launch_bounds__(ST_THREADS, 1)
   const float* xs = x_in_smem ? sx : xg;
   __syncthreads();
 
-  for (int t = 0; t < T; ++t) {
-    // this iteration's neighbourhood weights: issued now, consumed in step 3 — the 64 dependent-
-    // latency L2 reads per thread of the first version cost more than the assignment
-    if (w_in_smem) {
-      const float* Wg = weights + static_cast<size_t>(t) * M * M;
-      for (int i = tid; i < M * M; i += ST_THREADS) sw[i] = __ldg(Wg + i);
-    }
-    // ---- 1. assignment ----------------------------------------------------------------------
+  // ---- 1. assignment of every point to its nearest node (sidx) ---------------------------------
+  auto assign = [&]() {
     for (int n0 = tid; n0 < N; n0 += 2 * ST_THREADS) {
       const int n1 = n0 + ST_THREADS;
       const bool two = n1 < N;
@@ -108,6 +117,16 @@ __global__ void __launch_bounds__(ST_THREADS, 1)
       sidx[n0] = static_cast<unsigned char>(ia);
       if (two) sidx[n1] = static_cast<unsigned char>(ib);
     }
+  };
+
+  for (int t = 0; t < T; ++t) {
+    // this iteration's neighbourhood weights: issued now, consumed in step 3 — the 64 dependent-
+    // latency L2 reads per thread of the first version cost more than the assignment
+    if (w_in_smem) {
+      const float* Wg = weights + static_cast<size_t>(t) * M * M;
+      for (int i = tid; i < M * M; i += ST_THREADS) sw[i] = __ldg(Wg + i);
+    }
+    assign();
     __syncthreads();
 
     // ---- 2. per-node count / sums: warp per node, lanes stride the points, fixed order. The
@@ -166,13 +185,16 @@ __global__ void __launch_bounds__(ST_THREADS, 1)
       const int c = tid / M, j = tid - c * M;
       const float4 q = snode[j];
       const float nj = c == 0 ? q.x : (c == 1 ? q.y : q.z);
-      double acc = 0.0;
+      double hi = 0.0, lo = 0.0;
       for (int m = 0; m < M; ++m) {
         const float diff = __fmul_rn(__fsub_rn(smean[c * M + m], nj), socc[m]);
-        const float term = __fmul_rn(__fmul_rn(diff, W[static_cast<size_t>(m) * M + j]), lrt);
-        acc += static_cast<double>(term);
+        const double term =
+            static_cast<double>(__fmul_rn(__fmul_rn(diff, W[static_cast<size_t>(m) * M + j]), lrt));
+        const double s = hi + term, bb = s - hi;
+        lo += (hi - (s - bb)) + (term - bb);
+        hi = s;
       }
-      newv = __fadd_rn(nj, static_cast<float>(acc));
+      newv = __fadd_rn(nj, exact_sum_to_float(hi, lo));
     }
     __syncthreads();   // every thread has read the old nodes
     if (upd) {
@@ -190,8 +212,15 @@ __global__ void __launch_bounds__(ST_THREADS, 1)
     const int c = i / M, j = i - c * M;
     no[i] = reinterpret_cast<const float*>(snode + j)[c];
   }
-  if (idx_out != nullptr)   // assignment of the LAST iteration (w.r.t. the nodes before its update)
+  if (idx_out != nullptr) {
+    // assignment of the LAST iteration (w.r.t. the nodes before its update); with T = 0 the
+    // assignment against the initial nodes, by the same arithmetic as iteration 1
+    if (T == 0) {
+      assign();
+      __syncthreads();
+    }
     for (int n = tid; n < N; n += ST_THREADS) idx_out[static_cast<size_t>(b) * N + n] = sidx[n];
+  }
 }
 
 }  // namespace sonet

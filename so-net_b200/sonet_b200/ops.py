@@ -113,7 +113,8 @@ def som_mask(min_idx_i32, M):
 def som_train(x, node_init, weights, lr, want_idx=False):
     """T batch-SOM iterations in one launch (util/som.py:295-366). x [B,3,N]; node_init [3,M]
     (shared) or [B,3,M]; weights [T,M,M]; lr [T] -> node [B,3,M] (and the last assignment
-    [B,N] i32)."""
+    [B,N] i32: the one computed in iteration T, against the nodes before its update; with T = 0
+    the assignment against node_init, and the nodes pass through unchanged)."""
     _chk(x, "x", torch.float32)
     _chk(node_init, "node_init", torch.float32)
     _chk(weights, "weights", torch.float32)
