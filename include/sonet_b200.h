@@ -29,6 +29,13 @@ extern "C" {
 
 typedef void* sonet_stream_t; /* cudaStream_t */
 
+/* Activation codes. Entries with an `int relu` argument read it as one of these (0 and 1 keep
+ * their old meaning); any other value fails with SONET_ERR_BAD_ARG before a CUDA call.
+ * ELU is nn.ELU(alpha=1): x > 0 ? x : expm1(x), computed in fp32 in every precision mode. */
+#define SONET_ACT_NONE 0
+#define SONET_ACT_RELU 1
+#define SONET_ACT_ELU 2
+
 /* ---- library ------------------------------------------------------------------------------ */
 const char* sonet_last_error_string(void);
 /* "sonet_b200 <version> sm_90a" */
@@ -116,7 +123,7 @@ int sonet_comm_destroy(void* comm);
 
 /* ---- f-1: the auto-encoder's up-convolution decoder -------------------------------------------
  * Replaces UpConv.forward (models/layers.py:214-240; DecoderConv, models/networks.py:394-431):
- * nearest x2 up-sampling + 3x3 convolution (pad 1) + eval BatchNorm + ReLU, computed as four
+ * nearest x2 up-sampling + 3x3 convolution (pad 1) + eval BatchNorm + ReLU / ELU, computed as four
  * parity GEMMs over the LOW-resolution map with K = 4*Cin (the 3x3 taps that coincide after
  * up-sampling are pre-summed by the host into four [Cout, 4*Cin] matrices, tap-major K).
  *   sonet_upconv_im2col_f32: in [B,Cin,H,W] -> xcol [4][B][4*Cin][H*W]: group g = py*2+px, tap
@@ -157,8 +164,9 @@ int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, int P, cons
  *     y = act(gamma*(x-mean)*invstd + beta) in one elementwise pass. partial: scratch of
  *     sonet_bn_partial_slots(B,C) doubles. (The running-statistics update with the reference's
  *     momentum schedule stays on the host side: two [C] vector ops.)
- *   sonet_bn_train_backward_f32: dy, x (the BN input) -> dx, dgamma, dbeta; with relu the gate is
- *     recomputed from x (gamma*xhat+beta > 0), so the forward output need not be kept.
+ *   sonet_bn_train_backward_f32: dy, x (the BN input) -> dx, dgamma, dbeta; the activation's
+ *     derivative is recomputed from x at z = gamma*xhat+beta (ReLU: [z > 0]; ELU: z > 0 ? 1 : exp(z)),
+ *     so the forward output need not be kept. relu: activation code (SONET_ACT_*) in both.
  *   sonet_index_max_backward_f32: grad_data [B,C,N] = 0; grad_data[b,c,idx[b,c,k]] += grad_out[b,c,k]
  *     (k ascending, one thread per (b,c): deterministic also when empty nodes all gather point 0).
  *   sonet_pointwise_tc_pack_device: fp32 W [Cout,Cin] on the DEVICE -> wgmma blob (optionally of
@@ -250,7 +258,7 @@ int sonet_augment_f32(const float* pc, const float* sn, const float* som, int B,
  * Wt [C0+C1, Cout] row-major = the conv weight TRANSPOSED (so that a K-slab of weights is
  * contiguous along Cout), packed once by the host; scale/shift [Cout] hold conv bias and
  * eval-mode BatchNorm folded by the host (scale nullable = 1; the host may also fold scale into
- * Wt). relu: 0/1.
+ * Wt). relu: activation code (SONET_ACT_NONE / _RELU / _ELU).
  * addend (nullable) [B,Cout,G] with gidx [B,P] i32 in [0,G): per-point gathered additive term,
  * used by the decomposed segmenter layer-1 (per-node and per-cloud channels, SURVEY §8a-10).
  * out [B,Cout,P]. (KNNModule's max over K, layers.py:365, is sonet_rowmax_f32 on the result.) */
@@ -459,7 +467,8 @@ int sonet_pool_finalize(int32_t* keys, const float* p0, int B, int C, int M, flo
  *   pack (host pointers): W [Cout,Cin] row-major fp32 with the BN scale folded in -> blob_host,
  *     *inv_scale = 1 / (power-of-two pre-scale applied to the weights).
  *   forward (device pointers): as sonet_pointwise_layer_f32 with (blob, inv_scale) instead of
- *     (Wt, scale).
+ *     (Wt, scale); relu is the activation code, here and in the _rows, _grouped, _dev and _f16
+ *     entries (ELU in fp32 after the GEMM, in every precision mode).
  *   Range: each activation is split into fp16 hi/lo halves that each saturate at 65504, so an
  *   input with |x| >= 131008 acts as +-131008 (the output stays finite); past 65504 precision
  *   drops to ~2^-12 of the term. Error envelope (csrc/tc_common.cuh), per output:
@@ -536,6 +545,29 @@ int sonet_knn_mlp_tc_forward_f16(const float* coord, const float* center, const 
                                  int B, int M, int K, int Kstride, const float* Y,
                                  long long y_cstride, long long y_nstride, const float* w1,
                                  const void* blob, float inv_scale, const float* shift2, float* out,
+                                 sonet_stream_t stream);
+
+/* ---- explicit activation of the fused kernels ---------------------------------------------------
+ * sonet_pointresnet_tc_forward / _pool_forward and sonet_knn_mlp_tc_forward hard-code ReLU (they
+ * equal these entries with act = SONET_ACT_RELU, f16 = 0). These take the activation of the hidden
+ * layers (the PointResNet's layers 0-2, both KNN layers): act = SONET_ACT_RELU or SONET_ACT_ELU
+ * (anything else, SONET_ACT_NONE included, fails with SONET_ERR_BAD_ARG), and f16 != 0 selects the
+ * one-product fp16 mode of the `_f16` entries. Otherwise the arguments, blobs and properties of the
+ * entries without the suffix. ELU runs in fp32 in both modes. The PointResNet's per-node pool acts
+ * on the bare layer 3 (unaffected), and the KNN kernel's max over the neighbours on the raw
+ * accumulators stays exact: ELU is non-decreasing like ReLU (csrc/knn_tc.cu). */
+int sonet_pointresnet_tc_forward_act(const float* x, int Cin, int B, int P, const void* blob,
+                                     const float* fparams, int act, int f16, float* out,
+                                     sonet_stream_t stream);
+int sonet_pointresnet_tc_pool_forward_act(const float* x_sorted, int Cin, int B, int P,
+                                          const void* blob, const float* fparams,
+                                          const int32_t* node_sorted, const int32_t* pos0, int M,
+                                          int act, int f16, int32_t* pool_keys, float* p0,
+                                          sonet_stream_t stream);
+int sonet_knn_mlp_tc_forward_act(const float* coord, const float* center, const int64_t* idx, int B,
+                                 int M, int K, int Kstride, const float* Y, long long y_cstride,
+                                 long long y_nstride, const float* w1, const void* blob,
+                                 float inv_scale, const float* shift2, int act, int f16, float* out,
                                  sonet_stream_t stream);
 
 /* ---- diagnostics -------------------------------------------------------------------------------

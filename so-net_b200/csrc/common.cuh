@@ -32,6 +32,24 @@ int max_smem_optin();     // cached max opt-in dynamic shared memory per block
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+// Activation code argument (SONET_ACT_*): validated before any CUDA call.
+#define SONET_REQUIRE_ACT(act, what)                                                       \
+  SONET_REQUIRE((act) == SONET_ACT_NONE || (act) == SONET_ACT_RELU || (act) == SONET_ACT_ELU, \
+                "%s: activation code %d is not SONET_ACT_NONE (0), _RELU (1) or _ELU (2)", what, \
+                static_cast<int>(act))
+
+// ---- activations ------------------------------------------------------------------------------
+// ELU with alpha = 1 (nn.ELU(alpha=1.0), models/layers.py:136-137), in fp32 in every mode. expm1f,
+// not __expf(x) - 1: near 0 the difference loses the relative precision of the small result.
+__device__ __forceinline__ float elu1(float v) { return v > 0.f ? v : expm1f(v); }
+// The compile-time activation of the kernels that hard-code it (ACT = SONET_ACT_RELU or _ELU).
+template <int ACT>
+__device__ __forceinline__ float act_fn(float v) {
+  if constexpr (ACT == SONET_ACT_ELU) return elu1(v);
+  else if constexpr (ACT == SONET_ACT_RELU) return fmaxf(v, 0.f);
+  else return v;
+}
+
 // ---- device helpers ---------------------------------------------------------------------------
 // Running per-node maxima of the fused pool (csrc/pointmlp_tc.cu) are order-preserving int keys.
 constexpr int POOL_KEY_INIT = static_cast<int>(0x80000000u);  // below the key of every float

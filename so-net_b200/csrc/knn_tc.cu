@@ -9,7 +9,7 @@
 // mode; a channel-major [B,512,M] Y is accepted too (scalar loads, same results). This kernel then
 // runs, per row (node m, neighbour j):
 //
-//   * layer-1 epilogue on CUDA cores: h1 = relu(W1d . dec + Y[b,:,nbr] + shift1) in fp32, with
+//   * layer-1 epilogue on CUDA cores: h1 = act(W1d . dec + Y[b,:,nbr] + shift1) in fp32 (ReLU or ELU), with
 //     dec = coord[b,:,nbr] - center[b,:,m] (the same __fsub_rn as knn_assemble). Each thread builds
 //     its part of the register A operand of m64k16 (2 rows x 8 channels, fp16 hi/lo) right before
 //     the wgmmas of that K block; h1 never exists in memory. From a node-major Y a thread loads its
@@ -18,9 +18,12 @@
 //     kk+1 just read (double-buffered), so each load has two blocks of wgmmas to land;
 //   * layer 2 (512 -> 512) on wgmma with the fp16 hi/lo 3-product split, fp32 accumulators, in two
 //     N halves of 256 (passes; 128 accumulators per thread); each pass builds its own A operand;
-//   * max over the K neighbours on the RAW accumulators: y = relu(fmaf(raw, inv2 > 0, shift2)) is
-//     monotone in raw, so max_rows(y) == relu(fmaf(max_rows(raw), inv2, shift2)) bit for bit (the
-//     argument of the POOL epilogue of pointmlp_tc.cu). Every row reduces into per-node shared-memory
+//   * max over the K neighbours on the RAW accumulators: y = act(fmaf(raw, inv2 > 0, shift2)) is
+//     monotone (non-decreasing) in raw for both activations the kernel is built for: fmaf by a
+//     positive constant and a round-to-nearest are, ReLU is, and so is ELU — x for x > 0, and
+//     expm1f, non-decreasing in x, maps x <= 0 into (-1, 0], below every positive output. So
+//     max_rows(y) == act(fmaf(max_rows(raw), inv2, shift2)) bit for bit (the argument of the POOL
+//     epilogue of pointmlp_tc.cu). A non-monotone activation (swish) would break this. Every row reduces into per-node shared-memory
 //     keys, which the warpgroup converts and stores as knn_feature_1 [B,512,M]. h2 is never written.
 //     (A segmented shuffle reduction in front of the atomics spilled the accumulators; a
 //     __match_any_sync + __reduce_max_sync one made the epilogue ~10x slower, as redux.sync with
@@ -82,8 +85,9 @@ struct KnnArgs {
 
 // YVEC: Y is node-major (y_cs == 1), so channels (c, c+1) of a row are one float2.
 // NPROD: fp16 products per MAC in layer 2, 3 (the hi/lo split) or 1 (hi only, the opt-in fp16 mode:
-// the A fragments carry no lo words and the producer copies the hi half of each stage)
-template <bool YVEC, int NPROD>
+// the A fragments carry no lo words and the producer copies the hi half of each stage).
+// ACT: the activation of both layers, SONET_ACT_RELU or SONET_ACT_ELU.
+template <bool YVEC, int NPROD, int ACT>
 __global__ void __launch_bounds__(kt::NUM_THREADS, 1)
     knn_mlp_tc_kernel(const unsigned char* __restrict__ blob, KnnArgs a, long long* __restrict__ dbg) {
   using namespace kt;
@@ -227,7 +231,7 @@ __global__ void __launch_bounds__(kt::NUM_THREADS, 1)
             v = fmaf(w.x, d[0], v);
             v = fmaf(w.y, d[1], v);
             v = fmaf(w.z, d[2], v);
-            h[e] = fmaxf(v, 0.f);
+            h[e] = act_fn<ACT>(v);
           }
           tc::split_words<NPROD>(h[0], h[1], hi[i], lo[i]);
         }
@@ -307,7 +311,7 @@ __global__ void __launch_bounds__(kt::NUM_THREADS, 1)
           const int key = *kp;
           const float raw = __int_as_float(key ^ ((key >> 31) & 0x7fffffff));
           const int co = NH * pass + c;
-          a.out[(static_cast<size_t>(b) * C2 + co) * a.M + m] = fmaxf(fmaf(raw, a.inv2, sh2[co]), 0.f);
+          a.out[(static_cast<size_t>(b) * C2 + co) * a.M + m] = act_fn<ACT>(fmaf(raw, a.inv2, sh2[co]));
         }
         *kp = POOL_KEY_INIT;
       }
@@ -342,9 +346,12 @@ extern "C" int sonet_knn_mlp_tc_pack(const float* W2, void* blob_host, float* in
 static int launch_knn_mlp_tc(const float* coord, const float* center, const int64_t* idx, int B, int M,
                              int K, int Kstride, const float* Y, long long y_cs, long long y_ns,
                              const float* w1, const void* blob, float inv2, const float* shift2,
-                             float* out, long long* dbg, sonet_stream_t stream, bool f16 = false) {
+                             float* out, long long* dbg, sonet_stream_t stream, bool f16 = false,
+                             int act = SONET_ACT_RELU) {
   using namespace sonet;
   using namespace sonet::kt;
+  SONET_REQUIRE(act == SONET_ACT_RELU || act == SONET_ACT_ELU,
+                "knn_mlp_tc: activation code %d is not SONET_ACT_RELU (1) or _ELU (2)", act);
   SONET_REQUIRE(B >= 0 && M >= 1 && Kstride >= K, "knn_mlp_tc: bad dimension");
   SONET_REQUIRE(K >= MIN_K && K <= MAX_K, "knn_mlp_tc: K=%d out of range [%d,%d]", K, MIN_K, MAX_K);
   SONET_REQUIRE(M <= 65535, "knn_mlp_tc: M=%d too large", M);
@@ -366,8 +373,12 @@ static int launch_knn_mlp_tc(const float* coord, const float* center, const int6
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "knn_mlp_tc: needs %d B of shared memory", SMEM_BYTES);
   const long long items = 2 * ((nblocks + 1) / 2);   // (tile, pass) pairs
   const int grid = static_cast<int>(std::min<long long>(items, sm_count()));
-  auto kernel = f16 ? (y_cs == 1 ? knn_mlp_tc_kernel<true, 1> : knn_mlp_tc_kernel<false, 1>)
-                    : (y_cs == 1 ? knn_mlp_tc_kernel<true, 3> : knn_mlp_tc_kernel<false, 3>);
+  constexpr int R = SONET_ACT_RELU, E = SONET_ACT_ELU;
+  auto kernel =
+      act == E ? (f16 ? (y_cs == 1 ? knn_mlp_tc_kernel<true, 1, E> : knn_mlp_tc_kernel<false, 1, E>)
+                      : (y_cs == 1 ? knn_mlp_tc_kernel<true, 3, E> : knn_mlp_tc_kernel<false, 3, E>))
+               : f16 ? (y_cs == 1 ? knn_mlp_tc_kernel<true, 1, R> : knn_mlp_tc_kernel<false, 1, R>)
+                     : (y_cs == 1 ? knn_mlp_tc_kernel<true, 3, R> : knn_mlp_tc_kernel<false, 3, R>);
   cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   kernel<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(static_cast<const unsigned char*>(blob),
                                                                a, dbg);
@@ -391,6 +402,17 @@ extern "C" int sonet_knn_mlp_tc_forward_f16(const float* coord, const float* cen
                                             float* out, sonet_stream_t stream) {
   return launch_knn_mlp_tc(coord, center, idx, B, M, K, Kstride, Y, y_cstride, y_nstride, w1, blob,
                            inv_scale, shift2, out, nullptr, stream, true);
+}
+
+// explicit activation of both layers (SONET_ACT_RELU or SONET_ACT_ELU) and precision (f16 = 1: layer
+// 2 as the one-product mode)
+extern "C" int sonet_knn_mlp_tc_forward_act(const float* coord, const float* center, const int64_t* idx,
+                                            int B, int M, int K, int Kstride, const float* Y,
+                                            long long y_cstride, long long y_nstride, const float* w1,
+                                            const void* blob, float inv_scale, const float* shift2,
+                                            int act, int f16, float* out, sonet_stream_t stream) {
+  return launch_knn_mlp_tc(coord, center, idx, B, M, K, Kstride, Y, y_cstride, y_nstride, w1, blob,
+                           inv_scale, shift2, out, nullptr, stream, f16 != 0, act);
 }
 
 extern "C" int sonet_debug_knn_mlp_tc_timeline(const float* coord, const float* center,

@@ -14,7 +14,7 @@
 //     16 KB of shared memory: layer 1 and layer 3's skip slab read it as a shared-memory A operand;
 //   * layers 1-3 are wgmma f16 with fp32 accumulators in registers. A wgmma accumulator fragment
 //     (m64nN) has the layout of the register A fragment of m64k16, so the epilogues of layers 1
-//     and 2 (folded-BN shift, ReLU, fp16 hi/lo split) leave act1 / act2 in registers as the A
+//     and 2 (folded-BN shift, ReLU or ELU, fp16 hi/lo split) leave act1 / act2 in registers as the A
 //     operand of the next layer (64 / 128 registers per thread). No shared-memory image, fence or
 //     barrier separates the layers, the tensor cores read only weights from shared memory in
 //     layers 2-3, and activations never touch HBM;
@@ -115,8 +115,11 @@ struct PoolArgs {
 
 // DBG: the debug entry points' build, which also stamps the phase timeline of CTA 0.
 // NPROD: fp16 products per MAC, 3 (the hi/lo split) or 1 (hi only, the opt-in fp16 mode: act0
-// has no lo image, act1 / act2 no lo fragments, and the producer copies the hi half of each stage)
-template <bool POOL, bool DBG, int NPROD>
+// has no lo image, act1 / act2 no lo fragments, and the producer copies the hi half of each stage).
+// ACT: the activation of layers 0-2, SONET_ACT_RELU or SONET_ACT_ELU. Nothing downstream assumes
+// it is non-negative: the hi/lo split of an ELU output in [-1, inf) saturates exactly as a ReLU
+// output's does, and the pool, its -1000 sentinel and its keys act on the bare layer 3.
+template <bool POOL, bool DBG, int NPROD, int ACT>
 __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     pointresnet_tc_kernel(const float* __restrict__ x_in, int Cin, int B, int P,
                           const unsigned char* __restrict__ blob, const float* __restrict__ fparams,
@@ -219,8 +222,8 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const int k = 16 * kk + 8 * (i >> 1);
-          tc::split_words<NPROD>(fmaxf(fmaf(acc[8 * kk + 2 * i], inv, shq[k]), 0.f),
-                                 fmaxf(fmaf(acc[8 * kk + 2 * i + 1], inv, shq[k + 1]), 0.f),
+          tc::split_words<NPROD>(act_fn<ACT>(fmaf(acc[8 * kk + 2 * i], inv, shq[k])),
+                                 act_fn<ACT>(fmaf(acc[8 * kk + 2 * i + 1], inv, shq[k + 1])),
                                  hi[kk][i], lo[kk][i]);
         }
     };
@@ -253,7 +256,7 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
               float a = fps[C0 * 6 + ch];
 #pragma unroll
               for (int c = 0; c < 6; ++c) a = fmaf(fps[ch * 6 + c], xv[c], a);
-              y[e] = fmaxf(a, 0.f);
+              y[e] = act_fn<ACT>(a);
             }
             tc::split_words<NPROD>(y[0], y[1], hi[jj], lo[jj]);
           }
@@ -513,9 +516,12 @@ extern "C" int sonet_pointresnet_tc_pack(const float* W0, int Cin, const float* 
 
 static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const void* blob,
                                  const float* fparams, float* out, long long* dbg,
-                                 const sonet::PoolArgs* pool, sonet_stream_t stream, bool f16 = false) {
+                                 const sonet::PoolArgs* pool, sonet_stream_t stream, bool f16 = false,
+                                 int act = SONET_ACT_RELU) {
   using namespace sonet;
   using namespace sonet::pm;
+  SONET_REQUIRE(act == SONET_ACT_RELU || act == SONET_ACT_ELU,
+                "pointresnet_tc: activation code %d is not SONET_ACT_RELU (1) or _ELU (2)", act);
   SONET_REQUIRE(B >= 0 && P >= 0, "pointresnet_tc: negative dimension");
   SONET_REQUIRE(Cin >= 1 && Cin <= 6, "pointresnet_tc: Cin=%d out of range [1,6]", Cin);
   if (B == 0 || P == 0) return SONET_OK;
@@ -529,9 +535,14 @@ static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const vo
                 SMEM_BYTES);
   const int grid = static_cast<int>(std::min<long long>(tiles, sm_count()));
   SONET_REQUIRE(!(f16 && dbg), "pointresnet_tc: the debug timeline has no fp16 build");
-  auto kern = f16 ? (pool ? pointresnet_tc_kernel<true, false, 1> : pointresnet_tc_kernel<false, false, 1>)
-            : pool ? (dbg ? pointresnet_tc_kernel<true, true, 3> : pointresnet_tc_kernel<true, false, 3>)
-                   : (dbg ? pointresnet_tc_kernel<false, true, 3> : pointresnet_tc_kernel<false, false, 3>);
+  SONET_REQUIRE(!(act != SONET_ACT_RELU && dbg), "pointresnet_tc: the debug timeline has no ELU build");
+  constexpr int R = SONET_ACT_RELU, E = SONET_ACT_ELU;
+  auto kern =
+      act == E ? (f16 ? (pool ? pointresnet_tc_kernel<true, false, 1, E> : pointresnet_tc_kernel<false, false, 1, E>)
+                      : (pool ? pointresnet_tc_kernel<true, false, 3, E> : pointresnet_tc_kernel<false, false, 3, E>))
+      : f16 ? (pool ? pointresnet_tc_kernel<true, false, 1, R> : pointresnet_tc_kernel<false, false, 1, R>)
+      : pool ? (dbg ? pointresnet_tc_kernel<true, true, 3, R> : pointresnet_tc_kernel<true, false, 3, R>)
+             : (dbg ? pointresnet_tc_kernel<false, true, 3, R> : pointresnet_tc_kernel<false, false, 3, R>);
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   PoolArgs pa = pool ? *pool : PoolArgs{nullptr, nullptr, nullptr, nullptr, 0};
   kern<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
@@ -568,6 +579,23 @@ extern "C" int sonet_pointresnet_tc_pool_forward_f16(const float* x_sorted, int 
                                                      sonet_stream_t stream) {
   sonet::PoolArgs pa{node_sorted, pos0, pool_keys, p0, M};
   return launch_pointresnet_tc(x_sorted, Cin, B, P, blob, fparams, nullptr, nullptr, &pa, stream, true);
+}
+
+// explicit activation (SONET_ACT_RELU or SONET_ACT_ELU) and precision (f16 = 1: the one-product mode)
+extern "C" int sonet_pointresnet_tc_forward_act(const float* x, int Cin, int B, int P, const void* blob,
+                                                const float* fparams, int act, int f16, float* out,
+                                                sonet_stream_t stream) {
+  return launch_pointresnet_tc(x, Cin, B, P, blob, fparams, out, nullptr, nullptr, stream, f16 != 0, act);
+}
+
+extern "C" int sonet_pointresnet_tc_pool_forward_act(const float* x_sorted, int Cin, int B, int P,
+                                                     const void* blob, const float* fparams,
+                                                     const int32_t* node_sorted, const int32_t* pos0,
+                                                     int M, int act, int f16, int32_t* pool_keys,
+                                                     float* p0, sonet_stream_t stream) {
+  sonet::PoolArgs pa{node_sorted, pos0, pool_keys, p0, M};
+  return launch_pointresnet_tc(x_sorted, Cin, B, P, blob, fparams, nullptr, nullptr, &pa, stream, f16 != 0,
+                               act);
 }
 
 extern "C" int sonet_debug_pointresnet_tc_pool_timeline(const float* x_sorted, int Cin, int B, int P,

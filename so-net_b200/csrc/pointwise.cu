@@ -20,7 +20,8 @@ namespace sonet {
 
 constexpr int PW_BK = 8;
 
-template <int BM, int BN, int TM, int TN, bool VECP>
+// ELU: the ELU epilogue instead of relu ? ReLU : identity (relu is ignored)
+template <int BM, int BN, int TM, int TN, bool VECP, bool ELU>
 __global__ void __launch_bounds__(256, 2)
     pointwise_kernel(const float* __restrict__ x0, int C0, const float* __restrict__ x1, int C1,
                      int P, const float* __restrict__ Wt, const float* __restrict__ scale,
@@ -170,7 +171,7 @@ __global__ void __launch_bounds__(256, 2)
       for (int j = 0; j < 4; ++j) {
         float t = fmaf(acc[i][s * 4 + j], sc, sh);
         if (arow) t += __ldg(arow + gcol[s * 4 + j]);
-        v[j] = relu ? fmaxf(t, 0.f) : t;
+        v[j] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
       }
       if (VECP) {
         if (p < P) *reinterpret_cast<float4*>(orow + p) = make_float4(v[0], v[1], v[2], v[3]);
@@ -186,17 +187,28 @@ __global__ void __launch_bounds__(256, 2)
 template <int BM, int BN, int TM, int TN>
 static void launch_pointwise(bool vecp, dim3 grid, cudaStream_t st, const float* x0, int C0,
                              const float* x1, int C1, int P, const float* Wt, const float* scale,
-                             const float* shift, int Cout, int relu, const float* addend,
+                             const float* shift, int Cout, int act, const float* addend,
                              const int32_t* gidx, int G, float* out) {
-  if (vecp)
-    pointwise_kernel<BM, BN, TM, TN, true><<<grid, 256, 0, st>>>(
+  const int relu = act == SONET_ACT_RELU;
+  if (act == SONET_ACT_ELU) {
+    if (vecp)
+      pointwise_kernel<BM, BN, TM, TN, true, true><<<grid, 256, 0, st>>>(
+          x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
+    else
+      pointwise_kernel<BM, BN, TM, TN, false, true><<<grid, 256, 0, st>>>(
+          x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
+  } else if (vecp) {
+    pointwise_kernel<BM, BN, TM, TN, true, false><<<grid, 256, 0, st>>>(
         x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
-  else
-    pointwise_kernel<BM, BN, TM, TN, false><<<grid, 256, 0, st>>>(
+  } else {
+    pointwise_kernel<BM, BN, TM, TN, false, false><<<grid, 256, 0, st>>>(
         x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
+  }
 }
 
 // ---- MyLinear: out[b,co] = act(scale*(W[co,:].x[b,:]) + shift): warp per output element -----------
+// (ELU in all three MyLinear kernels: the ELU epilogue, relu ignored)
+template <bool ELU>
 __global__ void __launch_bounds__(256)
     linear_kernel(const float* __restrict__ x, int B, int Cin, const float* __restrict__ W,
                   const float* __restrict__ scale, const float* __restrict__ shift, int Cout,
@@ -214,7 +226,7 @@ __global__ void __launch_bounds__(256)
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) {
     float t = fmaf(s, scale ? scale[co] : 1.f, shift ? shift[co] : 0.f);
-    out[warp_id] = relu ? fmaxf(t, 0.f) : t;
+    out[warp_id] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
   }
 }
 
@@ -224,7 +236,7 @@ __global__ void __launch_bounds__(256)
 // each warp takes clouds warp, warp+8, ... two at a time (one LDS.128 of weights feeds two clouds'
 // FMAs), lanes stride the K axis in float4, and a butterfly reduces the 2*CT sums. Weight traffic:
 // once; activation traffic: (Cout/CT) x B x Cin from L2. Requires Cin % 4 == 0 and 16-byte aligned rows.
-template <int CT>
+template <int CT, bool ELU>
 __global__ void __launch_bounds__(256)
     linear_block_kernel(const float* __restrict__ x, int B, int Cin, const float* __restrict__ W,
                         const float* __restrict__ scale, const float* __restrict__ shift, int Cout,
@@ -276,7 +288,7 @@ __global__ void __launch_bounds__(256)
       const int co = co0 + c;
       if (co < Cout && (h == 0 || two)) {
         const float t = fmaf(v, scale ? __ldg(scale + co) : 1.f, shift ? __ldg(shift + co) : 0.f);
-        out[static_cast<size_t>(b0 + h) * Cout + co] = relu ? fmaxf(t, 0.f) : t;
+        out[static_cast<size_t>(b0 + h) * Cout + co] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
       }
     }
   }
@@ -292,6 +304,7 @@ __global__ void __launch_bounds__(256)
 // only (four interleaved partial sums, k ascending): results do not depend on the batch composition.
 constexpr int LT_B = 16, LT_C = 16, LT_STAGES = 4;
 
+template <bool ELU>
 __global__ void __launch_bounds__(256)
     linear_tile_kernel(const float* __restrict__ x, int B, int Cin, const float* __restrict__ W,
                        const float* __restrict__ scale, const float* __restrict__ shift, int Cout,
@@ -344,7 +357,7 @@ __global__ void __launch_bounds__(256)
   if (b < B && co < Cout) {
     const float v = (acc.x + acc.y) + (acc.z + acc.w);
     const float t = fmaf(v, scale ? __ldg(scale + co) : 1.f, shift ? __ldg(shift + co) : 0.f);
-    out[static_cast<size_t>(b) * Cout + co] = relu ? fmaxf(t, 0.f) : t;
+    out[static_cast<size_t>(b) * Cout + co] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
   }
 }
 
@@ -661,6 +674,7 @@ extern "C" int sonet_pointwise_layer_f32(const float* x0, int C0, const float* x
                                          const float* addend, const int32_t* gidx, int G,
                                          float* out, sonet_stream_t stream) {
   using namespace sonet;
+  SONET_REQUIRE_ACT(relu, "pointwise");
   SONET_REQUIRE(B >= 0 && P >= 0 && C0 >= 1 && C1 >= 0 && Cout >= 1, "pointwise: bad dimension");
   SONET_REQUIRE(B <= 65535, "pointwise: B=%d exceeds grid limit", B);
   if (B == 0 || P == 0) return SONET_OK;
@@ -684,21 +698,17 @@ extern "C" int sonet_pointwise_layer_f32(const float* x0, int C0, const float* x
   return check_launch("pointwise_layer");
 }
 
-extern "C" int sonet_linear_f32(const float* x, int B, int Cin, const float* W, const float* scale,
-                                const float* shift, int Cout, int relu, float* out,
-                                sonet_stream_t stream) {
-  using namespace sonet;
-  SONET_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1, "linear: bad dimension");
-  if (B == 0) return SONET_OK;
-  SONET_REQUIRE(x && W && out, "linear: null pointer");
-  cudaStream_t st = as_stream(stream);
+namespace sonet {
+template <bool ELU>
+static int launch_linear(const float* x, int B, int Cin, const float* W, const float* scale,
+                         const float* shift, int Cout, int relu, float* out, cudaStream_t st) {
   const size_t tile_smem = static_cast<size_t>(LT_B + LT_C) * (Cin / 4 + 1) * sizeof(float4);
   if (Cin % 4 == 0 && aligned16(x) && aligned16(W) && tile_smem <= static_cast<size_t>(max_smem_optin())) {
-    cudaFuncSetAttribute(linear_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaFuncSetAttribute(linear_tile_kernel<ELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          static_cast<int>(tile_smem));
     dim3 grid((Cout + LT_C - 1) / LT_C, (B + LT_B - 1) / LT_B);
     if (grid.y <= 65535) {
-      linear_tile_kernel<<<grid, 256, tile_smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
+      linear_tile_kernel<ELU><<<grid, 256, tile_smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
       return check_launch("linear");
     }
   }
@@ -712,18 +722,32 @@ extern "C" int sonet_linear_f32(const float* x, int B, int Cin, const float* W, 
     if (smem <= 48 * 1024) {
       const int grid = (Cout + ct - 1) / ct;
       if (ct == 4)
-        linear_block_kernel<4><<<grid, 256, smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
+        linear_block_kernel<4, ELU><<<grid, 256, smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
       else if (ct == 2)
-        linear_block_kernel<2><<<grid, 256, smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
+        linear_block_kernel<2, ELU><<<grid, 256, smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
       else
-        linear_block_kernel<1><<<grid, 256, smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
+        linear_block_kernel<1, ELU><<<grid, 256, smem, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
       return check_launch("linear");
     }
   }
   const long long total = static_cast<long long>(B) * Cout;
   const int grid = static_cast<int>((total * 32 + 255) / 256);
-  linear_kernel<<<grid, 256, 0, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
+  linear_kernel<ELU><<<grid, 256, 0, st>>>(x, B, Cin, W, scale, shift, Cout, relu, out);
   return check_launch("linear");
+}
+}  // namespace sonet
+
+extern "C" int sonet_linear_f32(const float* x, int B, int Cin, const float* W, const float* scale,
+                                const float* shift, int Cout, int relu, float* out,
+                                sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(relu, "linear");
+  SONET_REQUIRE(B >= 0 && Cin >= 1 && Cout >= 1, "linear: bad dimension");
+  if (B == 0) return SONET_OK;
+  SONET_REQUIRE(x && W && out, "linear: null pointer");
+  if (relu == SONET_ACT_ELU)
+    return launch_linear<true>(x, B, Cin, W, scale, shift, Cout, 0, out, as_stream(stream));
+  return launch_linear<false>(x, B, Cin, W, scale, shift, Cout, relu, out, as_stream(stream));
 }
 
 extern "C" int sonet_rowmax_f32(const float* in, int R, int L, float* out, sonet_stream_t stream) {

@@ -20,7 +20,8 @@
 //     mode (the `_f16` entries, NPROD = 1) writes only the hi image and issues hi*hi alone;
 //   * producer warp: streams the pre-packed fp16 hi/lo weight images (cp.async.bulk + mbarrier)
 //     through a 4-stage ring shared by both warpgroups;
-//   * epilogue in registers: fused scale/shift (+ gathered addend) + ReLU; eight lanes of a warp
+//   * epilogue in registers: fused scale/shift (+ gathered addend) + ReLU (one max against 0 or
+//     -inf, so ReLU and no activation share a kernel) or, in the ELU build, ELU; eight lanes of a warp
 //     hold eight consecutive points of one channel, so every store fills 32-byte sectors. The
 //     point-major store mode (out [B,P,Cout]) writes each thread's column pair as one float2: four
 //     lanes fill one 32-byte sector of a row.
@@ -101,8 +102,9 @@ __device__ inline int item_width(int Cout, int nt, int sub) {
 }  // namespace pwt
 
 // NPROD: fp16 products per MAC, 3 (hi/lo split, the default) or 1 (hi only, the opt-in fp16 mode:
-// the lo A image is never written and the producer copies only the hi image of each stage)
-template <int NPROD>
+// the lo A image is never written and the producer copies only the hi image of each stage).
+// ELU: the epilogue applies ELU instead of the max against floor_v (d.relu is ignored)
+template <int NPROD, bool ELU>
 __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
     pointwise_tc_kernel(const float* __restrict__ x0, const float* __restrict__ x1,
                         const unsigned char* __restrict__ blob, const float* __restrict__ shift,
@@ -314,7 +316,7 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
               y[e] = fmaf(acc[4 * j + 2 * rr + e], inv_w,
                           (shift != nullptr && co + e < d.Cout) ? __ldg(shift + co + e) : 0.f);
               if (arow != nullptr && co + e < d.Cout) y[e] += __ldg(arow + static_cast<size_t>(co + e) * d.G);
-              y[e] = fmaxf(y[e], floor_v);
+              y[e] = ELU ? elu1(y[e]) : fmaxf(y[e], floor_v);
             }
             if (co + 1 < d.Cout && (d.Cout & 1) == 0)
               *reinterpret_cast<float2*>(o + co) = make_float2(y[0], y[1]);
@@ -335,7 +337,7 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
             if (co < d.Cout) {
               float y = fmaf(acc[4 * j + 2 * rr + e], inv_w, shift != nullptr ? __ldg(shift + co) : 0.f);
               if (arow != nullptr) y += __ldg(arow + static_cast<size_t>(co) * d.G);
-              o[static_cast<size_t>(co) * d.P_out] = fmaxf(y, floor_v);
+              o[static_cast<size_t>(co) * d.P_out] = ELU ? elu1(y) : fmaxf(y, floor_v);
             }
           }
         }
@@ -390,6 +392,7 @@ struct TcExt {   // grouped / split-K / scatter / point-major launch options (de
   long long blob_gstride = 0, out_gstride = 0, out_sstride = 0;
 };
 
+// relu: activation code (SONET_ACT_*), validated by the entry points
 static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1, int B,
                                           int P, const void* blob, float inv_scale,
                                           const float* shift, int Cout, int relu,
@@ -406,7 +409,7 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   SONET_REQUIRE(!addend || (gidx && G >= 1), "pointwise_tc: addend needs gidx and G");
   SONET_REQUIRE(aligned16(blob), "pointwise_tc: weight blob must be 16-byte aligned");
   Dims d;
-  d.C0 = C0; d.C1 = C1; d.B = B; d.P = P; d.Cout = Cout; d.relu = relu; d.G = G;
+  d.C0 = C0; d.C1 = C1; d.B = B; d.P = P; d.Cout = Cout; d.relu = relu == SONET_ACT_RELU; d.G = G;
   d.conv_w = ext.conv_w;
   d.cpt = 1;
   if (ext.conv_w > 0) {
@@ -441,7 +444,8 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "pointwise_tc: needs %d B of shared memory", SMEM_BYTES);
   SONET_REQUIRE(ext.nprod == 3 || (ext.nprod == 1 && !ext.act_ptr && !ext.inv_ptr),
                 "pointwise_tc: the one-product mode is eval-only");
-  auto kern = ext.nprod == 1 ? pointwise_tc_kernel<1> : pointwise_tc_kernel<3>;
+  auto kern = relu == SONET_ACT_ELU ? (ext.nprod == 1 ? pointwise_tc_kernel<1, true> : pointwise_tc_kernel<3, true>)
+                                    : (ext.nprod == 1 ? pointwise_tc_kernel<1, false> : pointwise_tc_kernel<3, false>);
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   const int grid = static_cast<int>(std::min<long long>(items, sm_count()));
   kern<<<grid, NUM_THREADS, SMEM_BYTES, as_stream(stream)>>>(
@@ -460,6 +464,7 @@ extern "C" int sonet_pointwise_tc_forward(const float* x0, int C0, const float* 
                                           const float* shift, int Cout, int relu,
                                           const float* addend, const int32_t* gidx, int G,
                                           float* out, sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward");
   return launch_pointwise_tc(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
                              out, nullptr, stream);
 }
@@ -470,6 +475,7 @@ extern "C" int sonet_pointwise_tc_forward_f16(const float* x0, int C0, const flo
                                               const float* shift, int Cout, int relu,
                                               const float* addend, const int32_t* gidx, int G,
                                               float* out, sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward_f16");
   return launch_pointwise_tc(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
                              out, nullptr, stream, with_nprod(1));
 }
@@ -489,6 +495,7 @@ extern "C" int sonet_pointwise_tc_forward_rows(const float* x0, int C0, const fl
                                                const float* shift, int Cout, int relu,
                                                const float* addend, const int32_t* gidx, int G,
                                                float* out, sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward_rows");
   return pointwise_tc_rows(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
                            out, stream, 3);
 }
@@ -498,16 +505,17 @@ extern "C" int sonet_pointwise_tc_forward_rows_f16(const float* x0, int C0, cons
                                                    const float* shift, int Cout, int relu,
                                                    const float* addend, const int32_t* gidx, int G,
                                                    float* out, sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward_rows_f16");
   return pointwise_tc_rows(x0, C0, x1, C1, B, P, blob, inv_scale, shift, Cout, relu, addend, gidx, G,
                            out, stream, 1);
 }
 
 namespace sonet {
 // partial [G][S][B][Cout][P] (raw K-split sums) -> out: sum over S in ascending order (fixed ->
-// deterministic), + shift, ReLU, and the up-convolution parity scatter.
+// deterministic), + shift, ReLU (or, in the ELU build, ELU), and the up-convolution parity scatter.
 // IT = uint32_t when every index fits 32 bits (always, in practice): the three divisions per element
 // were 64-bit ones, and the kernel was bound by them (17 us for 2.1 M outputs), not by its 40 MB.
-template <typename IT>
+template <typename IT, bool ELU>
 __global__ void __launch_bounds__(256)
     splitk_reduce_kernel(const float* __restrict__ part, int G, int S, int B, int Cout, int P,
                          const float* __restrict__ shift, int relu, int scat_w, int P_out,
@@ -526,7 +534,8 @@ __global__ void __launch_bounds__(256)
     float acc = src[0];
     for (int s = 1; s < S; ++s) acc += src[static_cast<size_t>(s) * per_split];
     if (shift != nullptr) acc += __ldg(shift + co);
-    if (relu) acc = fmaxf(acc, 0.f);
+    if (ELU) acc = elu1(acc);
+    else if (relu) acc = fmaxf(acc, 0.f);
     int po = p;
     if (scat_w > 0) {
       const int i = p / scat_w, j = p - i * scat_w;
@@ -536,17 +545,30 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-static void launch_splitk_reduce(const float* part, int G, int S, int B, int Cout, int P,
-                                 const float* shift, int relu, int scat_w, int P_out,
-                                 long long out_gstride, float* out, cudaStream_t st) {
+template <bool ELU>
+static void launch_splitk_reduce_act(const float* part, int G, int S, int B, int Cout, int P,
+                                     const float* shift, int relu, int scat_w, int P_out,
+                                     long long out_gstride, float* out, cudaStream_t st) {
   const long long total = static_cast<long long>(B) * Cout * P * G;
   const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 8LL * sm_count()));
   if (total * std::max(S, 1) < (1LL << 32))
-    splitk_reduce_kernel<uint32_t><<<grid, 256, 0, st>>>(part, G, S, B, Cout, P, shift, relu, scat_w,
-                                                          P_out, out_gstride, out);
+    splitk_reduce_kernel<uint32_t, ELU><<<grid, 256, 0, st>>>(part, G, S, B, Cout, P, shift, relu,
+                                                               scat_w, P_out, out_gstride, out);
   else
-    splitk_reduce_kernel<unsigned long long><<<grid, 256, 0, st>>>(part, G, S, B, Cout, P, shift, relu,
-                                                                    scat_w, P_out, out_gstride, out);
+    splitk_reduce_kernel<unsigned long long, ELU><<<grid, 256, 0, st>>>(part, G, S, B, Cout, P, shift,
+                                                                         relu, scat_w, P_out,
+                                                                         out_gstride, out);
+}
+
+// act: activation code (SONET_ACT_*)
+static void launch_splitk_reduce(const float* part, int G, int S, int B, int Cout, int P,
+                                 const float* shift, int act, int scat_w, int P_out,
+                                 long long out_gstride, float* out, cudaStream_t st) {
+  if (act == SONET_ACT_ELU)
+    launch_splitk_reduce_act<true>(part, G, S, B, Cout, P, shift, 0, scat_w, P_out, out_gstride, out, st);
+  else
+    launch_splitk_reduce_act<false>(part, G, S, B, Cout, P, shift, act == SONET_ACT_RELU, scat_w, P_out,
+                                    out_gstride, out, st);
 }
 }  // namespace sonet
 
@@ -593,6 +615,7 @@ extern "C" int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, 
                                                   int conv_w, int P_out, long long out_gstride,
                                                   float* out, float* scratch,
                                                   sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_grouped_forward");
   return pointwise_tc_grouped(x, C, B, P, blob, blob_gstride, inv_scale, shift, Cout, relu, groups,
                               splits, scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 3);
 }
@@ -604,6 +627,7 @@ extern "C" int sonet_pointwise_tc_grouped_forward_f16(const float* x, int C, int
                                                       int conv_w, int P_out, long long out_gstride,
                                                       float* out, float* scratch,
                                                       sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_grouped_forward_f16");
   return pointwise_tc_grouped(x, C, B, P, blob, blob_gstride, inv_scale, shift, Cout, relu, groups,
                               splits, scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 1);
 }
@@ -615,6 +639,7 @@ extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, in
                                               const float* shift, int Cout, int relu, int splits,
                                               float* out, float* scratch, sonet_stream_t stream) {
   using namespace sonet;
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward_dev");
   SONET_REQUIRE(inv_scale_dev != nullptr, "pointwise_tc_forward_dev: null inv_scale pointer");
   SONET_REQUIRE(splits >= 1 && (splits == 1 || scratch != nullptr),
                 "pointwise_tc_forward_dev: split-K needs scratch");

@@ -1,14 +1,15 @@
 // train.cu — train-mode kernels of the point-wise layers (SURVEY.md §8f-2) for sm_90a.
 //
 // The reference trains through EquivariantLayer = Conv1d(k=1) -> MyBatchNorm1d (batch statistics,
-// models/layers.py:22-70) -> ReLU, and back-propagates through the per-node pool as the backward
+// models/layers.py:22-70) -> ReLU (or ELU), and back-propagates through the per-node pool as the backward
 // of a gather (models/networks.py:185). PyTorch runs that as conv + batch_norm + relu (+ three
 // backward kernels each) and a zero-fill + scatter for the gather. Here:
 //
 //   bn_stats / bn_apply          batch statistics of x[B,C,P] per channel, then
-//                                y = relu(gamma * (x - mean) * invstd + beta) in ONE elementwise pass
-//   bn_backward (2 launches)     per-channel sums of g and g*xhat (g = dy gated by the ReLU of the
-//                                recomputed output), then dx = gamma*invstd*(g - mean(g) -
+//                                y = act(gamma * (x - mean) * invstd + beta) in ONE elementwise pass
+//   bn_backward (2 launches)     per-channel sums of g and g*xhat (g = dy times the activation's
+//                                derivative at the recomputed BN output z: [z > 0] for ReLU,
+//                                z > 0 ? 1 : exp(z) for ELU), then dx = gamma*invstd*(g - mean(g) -
 //                                xhat*mean(g*xhat)); dgamma, dbeta fall out of the sums
 //   index_max_backward           grad of first_pn_out through the masked gather: zero-fill +
 //                                scatter-add of grad[b,c,k] at idx[b,c,k] (duplicates — every empty
@@ -30,14 +31,18 @@ namespace sonet {
 constexpr int BN_THREADS = 256;
 
 // stage 1: CTA (c, s) sums the clouds b = s, s+S, ... of channel c. BWD: sums of g and g*xhat
-// (g = dy * [gamma*xhat + beta > 0] when relu), else sums of d and d*d with d = x - x[0,c,0].
+// (g = dy * [gamma*xhat + beta > 0] when relu, g = dy * act_grad(gamma*xhat + beta) in the ELU
+// build), else sums of d and d*d with d = x - x[0,c,0].
 //
 // The forward sums are shifted by a pivot, the channel's first element, and taken in fp64 term by
 // term. var = E[d^2] - E[d]^2 then cancels only by 1 + (mean - pivot)^2 / var, a few units for any
 // pivot drawn from the channel, where E[x^2] - mean^2 would cancel by (mean/std)^2: with fp32 sums
 // that is a relative error of ~(mean/std)^2 * 2^-24 in var, 1e-2 at mean/std = 1e3 (channels behind
 // a large bias, near-dead inputs). d is exact in fp64, d*d too, and a constant channel gives var = 0.
-template <bool BWD>
+// d elu(z) / dz, from the BN output z (alpha = 1: exp(z) = elu(z) + 1 below 0)
+__device__ __forceinline__ float elu_grad(float z) { return z > 0.f ? 1.f : expf(z); }
+
+template <bool BWD, bool ELU>
 __global__ void __launch_bounds__(BN_THREADS)
     bn_partial_kernel(const float* __restrict__ x, const float* __restrict__ dy,
                       const float* __restrict__ mean, const float* __restrict__ invstd,
@@ -64,7 +69,8 @@ __global__ void __launch_bounds__(BN_THREADS)
       for (int p = threadIdx.x; p < P; p += BN_THREADS) {
         const float xh = (xr[p] - mu) * is;
         float g = gr[p];
-        if (relu && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
+        if (ELU) g *= elu_grad(fmaf(ga, xh, be));
+        else if (relu && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
         f0 += g;
         f1 = fmaf(g, xh, f1);
         if (++cnt == 64) {               // flush to fp64 every 64 terms
@@ -131,6 +137,7 @@ __global__ void bn_bwd_final_kernel(const double* __restrict__ partial, int C, i
 }
 
 // y = act(gamma*(x-mean)*invstd + beta); grid (ceil(P/1024), C, B)
+template <bool ELU>
 __global__ void __launch_bounds__(256)
     bn_apply_kernel(const float* __restrict__ x, const float* __restrict__ mean,
                     const float* __restrict__ invstd, const float* __restrict__ gamma,
@@ -141,11 +148,12 @@ __global__ void __launch_bounds__(256)
   for (int p = blockIdx.x * 1024 + threadIdx.x; p < min(P, (static_cast<int>(blockIdx.x) + 1) * 1024);
        p += 256) {
     const float v = fmaf(ga, (x[o + p] - mu) * is, be);
-    y[o + p] = relu ? fmaxf(v, 0.f) : v;
+    y[o + p] = ELU ? elu1(v) : (relu ? fmaxf(v, 0.f) : v);
   }
 }
 
 // dx = gamma*invstd*(g - dbeta/n - xhat*dgamma/n)
+template <bool ELU>
 __global__ void __launch_bounds__(256)
     bn_bwd_apply_kernel(const float* __restrict__ dy, const float* __restrict__ x,
                         const float* __restrict__ mean, const float* __restrict__ invstd,
@@ -160,7 +168,8 @@ __global__ void __launch_bounds__(256)
        p += 256) {
     const float xh = (x[o + p] - mu) * is;
     float g = dy[o + p];
-    if (relu && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
+    if (ELU) g *= elu_grad(fmaf(ga, xh, be));
+    else if (relu && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
     dx[o + p] = ga * is * (g - k0 - xh * k1);
   }
 }
@@ -293,16 +302,20 @@ extern "C" int sonet_bn_train_forward_f32(const float* x, const float* gamma, co
                                           float* y, float* save_mean, float* save_var,
                                           float* save_invstd, sonet_stream_t stream) {
   using namespace sonet;
+  SONET_REQUIRE_ACT(relu, "bn_train_forward");
   SONET_REQUIRE(B >= 1 && C >= 1 && P >= 1 && B <= 65535 && C <= 65535, "bn_train_forward: bad dims");
   SONET_REQUIRE(x && partial && y && save_mean && save_var && save_invstd, "bn_train_forward: null pointer");
   cudaStream_t st = as_stream(stream);
   const int S = bn_splits(B, C);
-  bn_partial_kernel<false><<<dim3(C, S), BN_THREADS, 0, st>>>(x, nullptr, nullptr, nullptr, nullptr,
-                                                             nullptr, B, C, P, 0, S, partial);
+  bn_partial_kernel<false, false><<<dim3(C, S), BN_THREADS, 0, st>>>(x, nullptr, nullptr, nullptr, nullptr,
+                                                                    nullptr, B, C, P, 0, S, partial);
   bn_stats_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(partial, x, C, P, S, static_cast<double>(B) * P,
                                                         eps, save_mean, save_var, save_invstd);
-  bn_apply_kernel<<<dim3((P + 1023) / 1024, C, B), 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta,
-                                                               C, P, relu, y);
+  const dim3 grid((P + 1023) / 1024, C, B);
+  if (relu == SONET_ACT_ELU)
+    bn_apply_kernel<true><<<grid, 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta, C, P, 0, y);
+  else
+    bn_apply_kernel<false><<<grid, 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta, C, P, relu, y);
   return check_launch("bn_train_forward");
 }
 
@@ -312,17 +325,28 @@ extern "C" int sonet_bn_train_backward_f32(const float* dy, const float* x, cons
                                            double* partial, float* dx, float* dgamma, float* dbeta,
                                            sonet_stream_t stream) {
   using namespace sonet;
+  SONET_REQUIRE_ACT(relu, "bn_train_backward");
   SONET_REQUIRE(B >= 1 && C >= 1 && P >= 1 && B <= 65535 && C <= 65535, "bn_train_backward: bad dims");
   SONET_REQUIRE(dy && x && mean && invstd && partial && dx && dgamma && dbeta,
                 "bn_train_backward: null pointer");
   cudaStream_t st = as_stream(stream);
   const int S = bn_splits(B, C);
-  bn_partial_kernel<true><<<dim3(C, S), BN_THREADS, 0, st>>>(x, dy, mean, invstd, gamma, beta, B, C, P,
-                                                            relu, S, partial);
+  const bool elu = relu == SONET_ACT_ELU;
+  if (elu)
+    bn_partial_kernel<true, true><<<dim3(C, S), BN_THREADS, 0, st>>>(x, dy, mean, invstd, gamma, beta, B, C,
+                                                                    P, 0, S, partial);
+  else
+    bn_partial_kernel<true, false><<<dim3(C, S), BN_THREADS, 0, st>>>(x, dy, mean, invstd, gamma, beta, B,
+                                                                     C, P, relu, S, partial);
   bn_bwd_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(partial, C, S, dgamma, dbeta);
-  bn_bwd_apply_kernel<<<dim3((P + 1023) / 1024, C, B), 256, 0, st>>>(
-      dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P, relu,
-      static_cast<float>(1.0 / (static_cast<double>(B) * P)), dx);
+  const dim3 grid((P + 1023) / 1024, C, B);
+  const float inv_n = static_cast<float>(1.0 / (static_cast<double>(B) * P));
+  if (elu)
+    bn_bwd_apply_kernel<true><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
+                                                    0, inv_n, dx);
+  else
+    bn_bwd_apply_kernel<false><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
+                                                     relu, inv_n, dx);
   return check_launch("bn_train_backward");
 }
 

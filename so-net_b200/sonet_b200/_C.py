@@ -148,6 +148,18 @@ for _name in ("sonet_pointresnet_tc_forward", "sonet_pointresnet_tc_pool_forward
               "sonet_pointwise_tc_grouped_forward", "sonet_knn_mlp_tc_forward"):
     _SIGNATURES[_name + "_f16"] = _SIGNATURES[_name]
 F16_ENTRIES = tuple(n for n in _SIGNATURES if n.endswith("_f16"))
+# explicit activation code (SONET_ACT_RELU / _ELU) and precision (f16 flag) of the fused kernels
+_SIGNATURES["sonet_pointresnet_tc_forward_act"] = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                   c_int, c_int, c_void_p, c_void_p]
+_SIGNATURES["sonet_pointresnet_tc_pool_forward_act"] = [c_void_p, c_int, c_int, c_int, c_void_p,
+                                                        c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                                        c_int, c_void_p, c_void_p, c_void_p]
+_SIGNATURES["sonet_knn_mlp_tc_forward_act"] = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                               c_void_p, ctypes.c_longlong, ctypes.c_longlong,
+                                               c_void_p, c_void_p, ctypes.c_float, c_void_p, c_int,
+                                               c_int, c_void_p, c_void_p]
+ACT_ENTRIES = ("sonet_pointresnet_tc_forward_act", "sonet_pointresnet_tc_pool_forward_act",
+               "sonet_knn_mlp_tc_forward_act")
 _RESTYPE = {"sonet_last_error_string": ctypes.c_char_p, "sonet_version": ctypes.c_char_p,
             "sonet_pointwise_tc_blob_bytes": ctypes.c_longlong,
             "sonet_knn_mlp_tc_blob_bytes": ctypes.c_longlong,

@@ -112,14 +112,17 @@ class GraphedModel:
         if not hasattr(self, "_state_tensors"):
             self._state_tensors = [t for m in self._state_modules()
                                    for t in list(m.parameters()) + list(m.buffers())]
+        if not hasattr(self, "_act_modules"):
+            self._act_modules = [m for sm in self._state_modules() for m in sm.modules()
+                                 if hasattr(m, "activation")]
         ver = 0
         for t in self._state_tensors:
             ver += t._version
-        # the precision mode picks the kernels a forward launches: a graph captured in one mode
-        # must not replay in another
+        # the precision mode and the layers' activations pick the kernels a forward launches: a
+        # graph captured for one must not replay for another (activation is a plain attribute)
         return (tuple(tuple(t.shape) for t in s.t.values()), ver,
                 getattr(self.encoder, "fuse_pool", None), getattr(self.encoder, "_fpo_demand", None),
-                layers.tc_mode())
+                layers.tc_mode(), tuple(m.activation for m in self._act_modules))
 
     def _resolve(self, path):
         obj = self

@@ -9,8 +9,9 @@ therefore returns tensors without grad_fn: calling backward() on them fails loud
 require grad") instead of silently dropping parameter gradients. In train() mode, when an input
 requires grad (saliency / adversarial use in eval mode), or when EVAL_AUTOGRAD is set, the layers
 compose differentiable PyTorch ops on the GPU exactly as the reference does — the reference's own
-training path, not a CPU fallback. Non-default options ('instance' norm, elu/swish/leakyrelu)
-always take the PyTorch path.
+training path, not a CPU fallback. Both activations of the reference's options (relu, elu) run on
+the kernels, as does no activation; 'instance' norm, swish and leakyrelu always take the PyTorch
+path.
 """
 import itertools
 import math
@@ -74,6 +75,10 @@ class MyBatchNorm2d(_MomentumDecayBatchNorm):
     def _check_input_dim(self, input):
         if input.dim() != 4:
             raise ValueError('expected 4D input (got {}D input)'.format(input.dim()))
+
+
+# activations with a kernel epilogue (ops.act_code); others compose PyTorch ops
+KERNEL_ACTIVATIONS = (None, 'relu', 'elu')
 
 
 def _make_act(activation):
@@ -215,12 +220,12 @@ class MyLinear(nn.Module):
 
     def _fast(self, x):
         return (_fast_ok(self, x) and x.dim() == 2
-                and self.normalization in (None, 'batch') and self.activation in (None, 'relu'))
+                and self.normalization in (None, 'batch') and self.activation in KERNEL_ACTIVATIONS)
 
     def forward(self, x, epoch=None):
         if self._fast(x):
             w, shift = self.folded()
-            return ops.linear(x.contiguous(), w, None, shift, self.activation == 'relu')
+            return ops.linear(x.contiguous(), w, None, shift, self.activation)
         x = self.linear(x)
         if self.normalization == 'batch':
             x = self.norm(x, epoch)
@@ -261,10 +266,10 @@ class _PointwiseConvBase(nn.Module):
         ks = self.conv.kernel_size
         return (all(k == 1 for k in ks) and all(s == 1 for s in self.conv.stride)
                 and all(p == 0 for p in self.conv.padding)
-                and self.normalization in (None, 'batch') and self.activation in (None, 'relu'))
+                and self.normalization in (None, 'batch') and self.activation in KERNEL_ACTIVATIONS)
 
     def _train_kernels(self, x):
-        """train() mode on CUDA fp32 with the default norm/activation: the sm_90a train kernels
+        """train() mode on CUDA fp32 with a kernel norm/activation: the sm_90a train kernels
         (train_ops) instead of the PyTorch composition."""
         return (train_ops.ENABLED and self.training and torch.is_grad_enabled() and x.is_cuda
                 and x.dtype == torch.float32 and self._fast_eligible())
@@ -282,10 +287,10 @@ class _PointwiseConvBase(nn.Module):
         # register-tiled fp32 kernel
         if cin >= 32 and rows >= 256 and tc_enabled():
             blob, inv, shift = self._tc_params()
-            return ops.pointwise_layer_tc(x0, blob, inv, shift, cout, self.activation == 'relu',
+            return ops.pointwise_layer_tc(x0, blob, inv, shift, cout, self.activation,
                                           x1=x1, addend=addend, gidx=gidx, f16=tc_f16())
         w, shift = self.folded(transpose=True)
-        return ops.pointwise_layer(x0, w, None, shift, self.activation == 'relu', x1=x1,
+        return ops.pointwise_layer(x0, w, None, shift, self.activation, x1=x1,
                                    addend=addend, gidx=gidx)
 
 
@@ -329,7 +334,7 @@ class MyConv2d(_PointwiseConvBase):
             B, C, H, W = x.shape
             y = train_ops.conv_bn_act_train(
                 x.contiguous().view(B, C, H * W), self._conv_weight2d(), self.conv.bias,
-                self.norm if self.normalization == 'batch' else None, self.activation == 'relu', epoch)
+                self.norm if self.normalization == 'batch' else None, self.activation, epoch)
             return y.view(B, y.shape[1], H, W)
         # PyTorch/cuDNN path (3x3 decoder convs, training): strict fp32 in the forward and the
         # backward — cuDNN's default TF32 convolution is ~1e-3 relative, outside the 1e-4 parity
@@ -384,7 +389,7 @@ class UpConv(nn.Module):
         return (_fast_ok(self, x) and x.dim() == 4 and c.kernel_size == (3, 3)
                 and c.stride == (1, 1) and c.padding == (1, 1) and c.dilation == (1, 1)
                 and c.groups == 1 and c.out_channels >= 64 and c.in_channels >= 16
-                and self.normalization in (None, 'batch') and self.activation in (None, 'relu')
+                and self.normalization in (None, 'batch') and self.activation in KERNEL_ACTIVATIONS
                 and tc_enabled())
 
     def _packed(self):
@@ -431,14 +436,14 @@ class UpConv(nn.Module):
         f16 = tc_f16()
         B, Cin, H, W = x.shape
         Cout = self.conv.conv.out_channels
-        relu = self.activation == 'relu'
+        act = self.activation
         x = x.contiguous()
         if H == 1 and W == 1:
             kch = (Cin + 63) // 64
             splits = _pick_splits(kch, ((B + 127) // 128) * ((4 * Cout + 255) // 256))
             scratch = self._scratch_for(splits * B * 4 * Cout, x.device) if splits > 1 else None
             y = ops.pointwise_tc_grouped(x.view(B, Cin, 1), pk["blob1"], pk["per1"], pk["inv1"],
-                                         pk["shift1"], 4 * Cout, relu, groups=1, splits=splits,
+                                         pk["shift1"], 4 * Cout, act, groups=1, splits=splits,
                                          scratch=scratch, f16=f16)
             return y.view(B, Cout, 2, 2)
         P = H * W
@@ -450,7 +455,7 @@ class UpConv(nn.Module):
         conv = P % 64 == 0 and Cin % 64 == 0 and os.environ.get("SONET_UPCONV_IM2COL", "0") != "1"
         xin = ops.upconv_hshift(x) if conv else ops.upconv_im2col(x)      # [3B,Cin,HW] | [4B,4Cin,HW]
         y = ops.pointwise_tc_grouped(xin, pk["blob4"], pk["per4"], pk["inv4"], pk["shift"], Cout,
-                                     relu, groups=4, splits=splits, scat_w=W, scratch=scratch,
+                                     act, groups=4, splits=splits, scat_w=W, scratch=scratch,
                                      conv=conv, f16=f16)
         return y.view(B, Cout, 2 * H, 2 * W)
 
@@ -496,7 +501,7 @@ class EquivariantLayer(_PointwiseConvBase):
         if self._train_kernels(x) and x.dim() == 3:
             return train_ops.conv_bn_act_train(
                 x, self._conv_weight2d(), self.conv.bias,
-                self.norm if self.normalization == 'batch' else None, self.activation == 'relu', epoch)
+                self.norm if self.normalization == 'batch' else None, self.activation, epoch)
         y = self.conv(x)
         if self.normalization == 'batch':
             y = self.norm(y, epoch)
@@ -531,11 +536,13 @@ class KNNModule(nn.Module):
 
     # ---- fused wgmma path (csrc/knn_tc.cu) ----------------------------------------------------
     def _tc_fused(self, K, M):
-        """Two BN/ReLU layers 3+C -> 512 -> 512 (the encoder's), 2 <= K <= 16, M*K <= 2304."""
+        """Two BN/ReLU or BN/ELU layers 3+C -> 512 -> 512 (the encoder's), 2 <= K <= 16,
+        M*K <= 2304."""
         ls = self.layers
         return (tc_enabled() and len(ls) == 2
                 and ls[0].conv.in_channels >= 3 + 32
-                and all(l.conv.out_channels == 512 and l.activation == 'relu' for l in ls)
+                and all(l.conv.out_channels == 512 for l in ls)
+                and ls[0].activation in ('relu', 'elu') and ls[1].activation == ls[0].activation
                 and 2 <= K <= 16 and M * K <= 2304)
 
     def _tc_params(self):
@@ -559,7 +566,7 @@ class KNNModule(nn.Module):
         f16 = tc_f16()
         y = ops.pointwise_layer_tc(x, pk["yblob"], pk["yinv"], None, 512, False, rows=True, f16=f16)
         return ops.knn_mlp_tc(coord, center, knn_I, K, y.transpose(1, 2), pk["w1"], pk["blob2"],
-                              pk["inv2"], pk["shift2"], f16=f16)
+                              pk["inv2"], pk["shift2"], f16=f16, act=self.layers[0].activation)
 
     def forward_pooled(self, coordinate, pool, precomputed_knn_I, K, center_type, epoch=None,
                        owner=None):
@@ -692,7 +699,9 @@ class PointResNet(nn.Module):
         if list(self.out_channels_list) != [64, 128, 256, 384] or cin > 6:
             return False
         ls = self.layers
-        return (all(l.normalization == 'batch' and l.activation == 'relu' for l in ls[:3])
+        return (all(l.normalization == 'batch' for l in ls[:3])
+                and ls[0].activation in ('relu', 'elu')
+                and all(l.activation == ls[0].activation for l in ls[:3])
                 and ls[3].normalization is None and ls[3].activation is None)
 
     def _tc_params(self):
@@ -711,7 +720,8 @@ class PointResNet(nn.Module):
         if first.fast(x) and x.dim() == 3 and all(l.fast(x) for l in self.layers) \
                 and self._tc_eligible(x.shape[1], x1):
             blob, fpar = self._tc_params()
-            return ops.pointresnet_tc(x.contiguous(), blob, fpar, f16=tc_f16())
+            return ops.pointresnet_tc(x.contiguous(), blob, fpar, f16=tc_f16(),
+                                      act=self.layers[0].activation)
         if first.fast(x) and x.dim() == 3 and all(l.fast(x) for l in self.layers):
             layer0_out = first.forward_points(x.contiguous(),
                                               None if x1 is None else x1.contiguous())

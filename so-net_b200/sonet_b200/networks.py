@@ -183,7 +183,8 @@ class Encoder(nn.Module):
                 xs, ns, p0 = ops.som_sort_decenter(xd, snd, self.som_node, idx32, a["count"], k)
             blob, fpar = fpn._tc_params()
             pooled = ops.pointresnet_tc_pool(xs, blob, fpar, ns, p0, M, finalize=False,
-                                             owner=self._pool_keys, f16=tc_f16())
+                                             owner=self._pool_keys, f16=tc_f16(),
+                                             act=fpn.layers[0].activation)
             done = None
             if opt.som_k >= 2:   # pool_finalize folds into the KNN module's input assembly
                 done = self.knnlayer.forward_pooled(self.som_node, pooled, node_knn_I, opt.som_k,
@@ -387,7 +388,7 @@ class Segmenter(nn.Module):
             node_first.shape[1] + node_knn.shape[1] + node_final.shape[1])
         cloud = torch.cat((self._onehot(label, B, x.device), feature), dim=1)   # [B,1040]
         cloud_add = ops.linear(cloud.contiguous(), w_cloud, None, None, False).unsqueeze(2)  # [B,1024,1]
-        relu1 = self.layer1.activation == 'relu'
+        act1 = self.layer1.activation
         if tc_enabled():
             f16 = tc_f16()
             bp, ip, bn, pern, inn = tc
@@ -399,7 +400,7 @@ class Segmenter(nn.Module):
             splits = _pick_splits(kch, ((B * M + 127) // 128) * ((cout + 255) // 256))
             addend = ops.pointwise_tc_grouped(node_in, bn, pern, inn, None, cout, False, groups=1,
                                               splits=splits, f16=f16) + cloud_add   # [B,1024,M]
-            out1 = ops.pointwise_layer_tc(pt, bp, ip, shift, cout, relu1,
+            out1 = ops.pointwise_layer_tc(pt, bp, ip, shift, cout, act1,
                                           x1=first_pn_out.contiguous(), addend=addend,
                                           gidx=min_idx_i32, f16=f16)
         else:
@@ -407,7 +408,7 @@ class Segmenter(nn.Module):
             addend = ops.pointwise_layer(node_a, w_node, None, None, False,
                                          x1=node_final.contiguous(), addend=cloud_add,
                                          gidx=self._zero_idx(B, M, x.device))
-            out1 = ops.pointwise_layer(pt, w_point, None, shift, relu1,
+            out1 = ops.pointwise_layer(pt, w_point, None, shift, act1,
                                        x1=first_pn_out.contiguous(), addend=addend,
                                        gidx=min_idx_i32)
         out = self.layer3(self.layer2(out1))

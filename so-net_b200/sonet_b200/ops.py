@@ -34,6 +34,23 @@ def _stream(t):
     return torch.cuda.current_stream(t.device).cuda_stream
 
 
+# activation codes of the C-ABI (SONET_ACT_*, include/sonet_b200.h)
+ACT_NONE, ACT_RELU, ACT_ELU = 0, 1, 2
+_ACT_NAMES = {None: ACT_NONE, "relu": ACT_RELU, "elu": ACT_ELU}
+
+
+def act_code(act):
+    """An activation as its C-ABI code: a layer's activation name (None, 'relu', 'elu'), a bool
+    (False / True = none / ReLU, the old flag) or a code, which the library validates."""
+    if isinstance(act, bool):
+        return int(act)
+    if act is None or isinstance(act, str):
+        if act not in _ACT_NAMES:
+            raise RuntimeError("activation %r has no kernel (None, 'relu' or 'elu')" % (act,))
+        return _ACT_NAMES[act]
+    return int(act)
+
+
 def _entry(name, f16):
     """The C-ABI entry of an eval wgmma launch: `name`, or with f16 its one-product `_f16` twin
     (same arguments; include/sonet_b200.h)."""
@@ -186,8 +203,9 @@ def som_decenter(x, sn, cluster_mean, min_idx_i32, k, want_centers=False):
     return x_aug, centers
 
 
-def pointwise_layer(x0, Wt, scale, shift, relu, x1=None, addend=None, gidx=None, out=None):
-    """x0 [B,C0,P] (+ x1 [B,C1,P]) -> [B,Cout,P]; Wt [C0+C1,Cout] transposed folded weights."""
+def pointwise_layer(x0, Wt, scale, shift, act, x1=None, addend=None, gidx=None, out=None):
+    """x0 [B,C0,P] (+ x1 [B,C1,P]) -> [B,Cout,P]; Wt [C0+C1,Cout] transposed folded weights;
+    act: activation (act_code)."""
     _chk(x0, "x0", torch.float32)
     _chk(x1, "x1", torch.float32, optional=True)
     _chk(Wt, "Wt", torch.float32)
@@ -206,13 +224,13 @@ def pointwise_layer(x0, Wt, scale, shift, relu, x1=None, addend=None, gidx=None,
         if out is None:
             out = torch.empty((B, Cout, P), dtype=torch.float32, device=x0.device)
         _call("sonet_pointwise_layer_f32", _C.ptr(x0), C0, _C.ptr(x1), C1, B, P, _C.ptr(Wt),
-              _C.ptr(scale), _C.ptr(shift), Cout, int(bool(relu)), _C.ptr(addend), _C.ptr(gidx), G,
+              _C.ptr(scale), _C.ptr(shift), Cout, act_code(act), _C.ptr(addend), _C.ptr(gidx), G,
               _C.ptr(out), _stream(x0))
     return out
 
 
-def linear(x, W, scale, shift, relu):
-    """x [B,Cin], W [Cout,Cin] -> [B,Cout]."""
+def linear(x, W, scale, shift, act):
+    """x [B,Cin], W [Cout,Cin] -> [B,Cout]; act: activation (act_code)."""
     _chk(x, "x", torch.float32)
     _chk(W, "W", torch.float32)
     _chk(scale, "scale", torch.float32, optional=True)
@@ -222,7 +240,7 @@ def linear(x, W, scale, shift, relu):
     with torch.cuda.device(x.device):
         out = torch.empty((B, Cout), dtype=torch.float32, device=x.device)
         _call("sonet_linear_f32", _C.ptr(x), B, Cin, _C.ptr(W), _C.ptr(scale), _C.ptr(shift),
-              Cout, int(bool(relu)), _C.ptr(out), _stream(x))
+              Cout, act_code(act), _C.ptr(out), _stream(x))
     return out
 
 
@@ -514,17 +532,23 @@ def pointresnet_tc_pack(W, shifts, cin):
     return blob, fparams
 
 
-def pointresnet_tc(x, blob, fparams, f16=False):
+def pointresnet_tc(x, blob, fparams, f16=False, act=ACT_RELU):
     """x [B,Cin<=6,P] f32 -> [B,384,P]: the fused wgmma first PointResNet (f16: one fp16 product
-    per MAC instead of the hi/lo split's three)."""
+    per MAC instead of the hi/lo split's three; act: the activation of layers 0-2, 'relu' or
+    'elu')."""
+    act = act_code(act)
     _chk(x, "x", torch.float32)
     _chk(blob, "blob", torch.uint8)
     _chk(fparams, "fparams", torch.float32)
     B, Cin, P = x.shape
     with torch.cuda.device(x.device):
         out = torch.empty((B, 384, P), dtype=torch.float32, device=x.device)
-        _call(_entry("sonet_pointresnet_tc_forward", f16), _C.ptr(x), Cin, B, P, _C.ptr(blob),
-              _C.ptr(fparams), _C.ptr(out), _stream(x))
+        if act == ACT_RELU:
+            _call(_entry("sonet_pointresnet_tc_forward", f16), _C.ptr(x), Cin, B, P, _C.ptr(blob),
+                  _C.ptr(fparams), _C.ptr(out), _stream(x))
+        else:
+            _call("sonet_pointresnet_tc_forward_act", _C.ptr(x), Cin, B, P, _C.ptr(blob),
+                  _C.ptr(fparams), act, int(bool(f16)), _C.ptr(out), _stream(x))
     return out
 
 
@@ -579,11 +603,12 @@ def upconv_hshift(x):
     return out
 
 
-def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, groups, splits=1,
+def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, act, groups, splits=1,
                          scat_w=0, out=None, scratch=None, conv=False, f16=False):
     """Grouped wgmma layer: x [G*B, C, P], G weight blobs -> out. scat_w = W > 0: the four groups
     are the output parities of an up-convolution over [H, W] maps, interleaved into
     out [B, cout, 4*P]; otherwise out [G*B, cout, P]. splits > 1: K split through `scratch`.
+    act: activation (act_code).
     f16: one fp16 product per MAC instead of the hi/lo split's three."""
     _chk(x, "x", torch.float32)
     _chk(blob, "blob", torch.uint8)
@@ -604,18 +629,18 @@ def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, relu, group
             scratch = torch.empty((groups * splits * B * cout * P,), dtype=torch.float32, device=dev)
         _call(_entry("sonet_pointwise_tc_grouped_forward", f16), _C.ptr(x), C, B, P, _C.ptr(blob),
               int(per_bytes),
-              float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)), int(groups), int(splits),
+              float(inv_scale), _C.ptr(shift), int(cout), act_code(act), int(groups), int(splits),
               int(scat_w), int(scat_w) if conv else 0, int(P_out), int(gstride), _C.ptr(out),
               _C.ptr(scratch), _stream(x),
               kernels=2 if splits > 1 else 1)
     return out
 
 
-def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=None, gidx=None,
+def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, act, x1=None, addend=None, gidx=None,
                        rows=False, f16=False):
     """wgmma variant of pointwise_layer: x0 [B,C0,P] (+ x1) -> [B,cout,P], or with rows=True the
-    same values point-major, [B,P,cout]. f16: one fp16 product per MAC instead of the hi/lo
-    split's three."""
+    same values point-major, [B,P,cout]. act: activation (act_code). f16: one fp16 product per MAC
+    instead of the hi/lo split's three."""
     _chk(x0, "x0", torch.float32)
     _chk(x1, "x1", torch.float32, optional=True)
     _chk(blob, "blob", torch.uint8)
@@ -629,13 +654,13 @@ def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, relu, x1=None, addend=N
         if rows:
             out = torch.empty((B, P, cout), dtype=torch.float32, device=x0.device)
             _call(_entry("sonet_pointwise_tc_forward_rows", f16), _C.ptr(x0), C0, _C.ptr(x1), C1, B, P,
-                  _C.ptr(blob), float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)),
+                  _C.ptr(blob), float(inv_scale), _C.ptr(shift), int(cout), act_code(act),
                   _C.ptr(addend), _C.ptr(gidx), G, _C.ptr(out), _stream(x0))
         else:
             out = torch.empty((B, cout, P), dtype=torch.float32, device=x0.device)
             _call(_entry("sonet_pointwise_tc_forward", f16), _C.ptr(x0), C0, _C.ptr(x1), C1, B, P,
                   _C.ptr(blob),
-                  float(inv_scale), _C.ptr(shift), int(cout), int(bool(relu)), _C.ptr(addend),
+                  float(inv_scale), _C.ptr(shift), int(cout), act_code(act), _C.ptr(addend),
                   _C.ptr(gidx), G, _C.ptr(out), _stream(x0))
     return out
 
@@ -655,13 +680,15 @@ def knn_mlp_tc_pack(W2):
     return blob, float(inv.value)
 
 
-def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2, f16=False):
+def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2, f16=False, act=ACT_RELU):
     """The KNN module's layer 1 (from the per-node Y = W1f x [B,512,M]) + layer 2 + max over the
     K neighbours in one wgmma kernel. coord, center [B,3,M]; idx [B,M,K'] i64; w1 [512,4] =
     (W1d | shift1); shift2 [512] -> knn_feature_1 [B,512,M]. Y is [B,512,M] either contiguous or
     the channel-fastest view y.transpose(1, 2) of a contiguous [B,M,512] (pointwise_layer_tc(...,
     rows=True)); the kernel reads the latter as float2 pairs, with bit-identical results.
-    f16: layer 2 as one fp16 product per MAC instead of the hi/lo split's three."""
+    f16: layer 2 as one fp16 product per MAC instead of the hi/lo split's three. act: the
+    activation of both layers, 'relu' or 'elu'."""
+    act = act_code(act)
     _chk(coord, "coordinate", torch.float32)
     _chk(center, "center", torch.float32)
     _chk(idx, "knn_I", torch.int64)
@@ -679,9 +706,14 @@ def knn_mlp_tc(coord, center, idx, K, Y, w1, blob, inv_scale, shift2, f16=False)
                            % (tuple(coord.shape), tuple(Y.shape), tuple(w1.shape), tuple(idx.shape)))
     with torch.cuda.device(coord.device):
         out = torch.empty((B, 512, M), dtype=torch.float32, device=coord.device)
-        _call(_entry("sonet_knn_mlp_tc_forward", f16), _C.ptr(coord), _C.ptr(center), _C.ptr(idx), B,
-              M, int(K), idx.shape[2], _C.ptr(Y), Y.stride(1), Y.stride(2), _C.ptr(w1), _C.ptr(blob),
-              float(inv_scale), _C.ptr(shift2), _C.ptr(out), _stream(coord))
+        if act == ACT_RELU:
+            _call(_entry("sonet_knn_mlp_tc_forward", f16), _C.ptr(coord), _C.ptr(center), _C.ptr(idx),
+                  B, M, int(K), idx.shape[2], _C.ptr(Y), Y.stride(1), Y.stride(2), _C.ptr(w1),
+                  _C.ptr(blob), float(inv_scale), _C.ptr(shift2), _C.ptr(out), _stream(coord))
+        else:
+            _call("sonet_knn_mlp_tc_forward_act", _C.ptr(coord), _C.ptr(center), _C.ptr(idx), B, M,
+                  int(K), idx.shape[2], _C.ptr(Y), Y.stride(1), Y.stride(2), _C.ptr(w1), _C.ptr(blob),
+                  float(inv_scale), _C.ptr(shift2), act, int(bool(f16)), _C.ptr(out), _stream(coord))
     return out
 
 
@@ -815,10 +847,12 @@ def knn_assemble_pool(coord, keys, p0, idx, K, center_type, owner=None, want_x_a
 
 
 def pointresnet_tc_pool(x_sorted, blob, fparams, node_sorted, pos0, M, finalize=True, owner=None,
-                        f16=False):
+                        f16=False, act=ACT_RELU):
     """Fused wgmma PointResNet + per-node max: -> first_pn_out_masked_max [B,384,M], or with
     finalize=False the raw (keys [B,384,M] i32, p0 [B,384]) for knn_assemble_pool / pool_finalize.
-    f16: one fp16 product per MAC instead of the hi/lo split's three."""
+    f16: one fp16 product per MAC instead of the hi/lo split's three. act: the activation of
+    layers 0-2, 'relu' or 'elu'."""
+    act = act_code(act)
     _chk(x_sorted, "x_sorted", torch.float32)
     _chk(blob, "blob", torch.uint8)
     _chk(fparams, "fparams", torch.float32)
@@ -829,10 +863,15 @@ def pointresnet_tc_pool(x_sorted, blob, fparams, node_sorted, pos0, M, finalize=
     with torch.cuda.device(dev):
         keys = (owner or _DEFAULT_POOL_KEYS).acquire(dev, B, M, _stream(x_sorted))
         p0 = torch.empty((B, 384), dtype=torch.float32, device=dev)
-        _call(_entry("sonet_pointresnet_tc_pool_forward", f16), _C.ptr(x_sorted), Cin, B, P,
-              _C.ptr(blob),
-              _C.ptr(fparams), _C.ptr(node_sorted), _C.ptr(pos0), int(M), _C.ptr(keys), _C.ptr(p0),
-              _stream(x_sorted))
+        if act == ACT_RELU:
+            _call(_entry("sonet_pointresnet_tc_pool_forward", f16), _C.ptr(x_sorted), Cin, B, P,
+                  _C.ptr(blob),
+                  _C.ptr(fparams), _C.ptr(node_sorted), _C.ptr(pos0), int(M), _C.ptr(keys),
+                  _C.ptr(p0), _stream(x_sorted))
+        else:
+            _call("sonet_pointresnet_tc_pool_forward_act", _C.ptr(x_sorted), Cin, B, P, _C.ptr(blob),
+                  _C.ptr(fparams), _C.ptr(node_sorted), _C.ptr(pos0), int(M), act, int(bool(f16)),
+                  _C.ptr(keys), _C.ptr(p0), _stream(x_sorted))
     if not finalize:
         return keys, p0
     return pool_finalize(keys, p0, owner)

@@ -1,12 +1,12 @@
 """Train-mode building blocks on the sm_90a kernels (SURVEY.md §8f-2, csrc/train.cu): autograd
 Functions that the layer classes use in train() mode instead of the PyTorch composition
-conv1d -> batch_norm(training=True) -> relu and gather (models/layers.py:22-70, 282-296;
+conv1d -> batch_norm(training=True) -> relu / elu and gather (models/layers.py:22-70, 282-296;
 models/networks.py:185).
 
     ConvTC        y = W x + b, dx = W^T dy AND dW = dy x^T on the generic wgmma layer kernel
                   (weights / activations packed on the device each step; gradients pre-scaled by a
                   power of two before the fp16 hi/lo split)
-    BNActTrain    batch-statistics BatchNorm + ReLU, forward and backward, fused elementwise passes
+    BNActTrain    batch-statistics BatchNorm + ReLU / ELU / none, forward and backward, fused elementwise passes
                   and two-stage deterministic reductions
     IndexMaxGather  first_pn_out_masked_max = first_pn_out.gather(2, idx * mask_row_max) with the
                   arg-max kernel in the forward and a deterministic scatter in the backward
@@ -14,6 +14,7 @@ models/networks.py:185).
 ENABLED = False switches every layer back to the PyTorch composition (the tests compare the two).
 """
 import torch
+import torch.nn.functional as F
 
 from . import _C, ops
 
@@ -30,7 +31,7 @@ def _scratch(dev, n, dtype, cache={}):
 
 class BNActTrain(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, gamma, beta, eps, relu):
+    def forward(ctx, x, gamma, beta, eps, act):
         x = x.contiguous()
         B, C, P = x.shape
         dev = x.device
@@ -41,10 +42,10 @@ class BNActTrain(torch.autograd.Function):
             invstd = torch.empty(C, dtype=torch.float32, device=dev)
             part = _scratch(dev, _C.lib().sonet_bn_partial_slots(B, C), torch.float64)
             ops._call("sonet_bn_train_forward_f32", _C.ptr(x), _C.ptr(gamma), _C.ptr(beta), B, C, P,
-                      float(eps), int(bool(relu)), _C.ptr(part), _C.ptr(y), _C.ptr(mean), _C.ptr(var),
+                      float(eps), ops.act_code(act), _C.ptr(part), _C.ptr(y), _C.ptr(mean), _C.ptr(var),
                       _C.ptr(invstd), ops._stream(x), kernels=3)
         ctx.save_for_backward(x, mean, invstd, gamma, beta)
-        ctx.relu = bool(relu)
+        ctx.act = ops.act_code(act)
         ctx.mark_non_differentiable(mean, var)
         return y, mean, var
 
@@ -60,7 +61,7 @@ class BNActTrain(torch.autograd.Function):
             dbeta = torch.empty(C, dtype=torch.float32, device=dev)
             part = _scratch(dev, _C.lib().sonet_bn_partial_slots(B, C), torch.float64)
             ops._call("sonet_bn_train_backward_f32", _C.ptr(dy), _C.ptr(x), _C.ptr(mean),
-                      _C.ptr(invstd), _C.ptr(gamma), _C.ptr(beta), B, C, P, int(ctx.relu),
+                      _C.ptr(invstd), _C.ptr(gamma), _C.ptr(beta), B, C, P, ctx.act,
                       _C.ptr(part), _C.ptr(dx), _C.ptr(dgamma), _C.ptr(dbeta), ops._stream(x),
                       kernels=3)
         return dx, dgamma, dbeta, None, None
@@ -239,11 +240,11 @@ def conv_strict(conv, x):
                             list(conv.dilation), conv.groups)
 
 
-def conv_bn_act_train(x3, weight2d, bias, norm, relu, epoch=None):
+def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None):
     """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (wgmma when dense
     enough, else strict-fp32 cuDNN) -> batch-stat BN (+ running-stat update with the reference's
     momentum schedule, models/layers.py:57-65; like F.batch_norm, num_batches_tracked is left
-    alone) -> ReLU."""
+    alone) -> act: the layer's activation (None, 'relu' or 'elu'; a bool means ReLU or none)."""
     B, Cin, P = x3.shape
     Cout = weight2d.shape[0]
     if tc_eligible(Cin, Cout, B * P):
@@ -251,14 +252,17 @@ def conv_bn_act_train(x3, weight2d, bias, norm, relu, epoch=None):
     else:
         y0 = ConvStrict.apply(x3, weight2d.unsqueeze(2), bias, [1], [0], [1], 1)
     if norm is None:
-        return torch.relu(y0) if relu else y0
+        code = ops.act_code(act)
+        if code == ops.ACT_ELU:
+            return F.elu(y0)
+        return torch.relu(y0) if code == ops.ACT_RELU else y0
     if B * P == 1:     # F.batch_norm's check: a batch statistic of one value is undefined
         raise ValueError("Expected more than 1 value per channel when training, got input size "
                          "{}".format(y0.size()))
     step = norm.momentum_decay_step
     if epoch is not None and epoch >= 1 and step is not None and step > 0:
         norm.momentum = max(norm.momentum_original * (norm.momentum_decay ** (epoch // step)), 0.01)
-    y, mean, var = BNActTrain.apply(y0, norm.weight, norm.bias, norm.eps, relu)
+    y, mean, var = BNActTrain.apply(y0, norm.weight, norm.bias, norm.eps, act)
     with torch.no_grad():
         n = B * P
         m = norm.momentum

@@ -1,0 +1,558 @@
+"""-m gpu: models built with the reference's `--activation elu` on the sm_90a kernels.
+
+  (a) every ELU fixture the reference produced (tools/make_golden_act.py) through every route:
+      fused pool, unfused, SONET_TC=0 (exact-fp32 kernels) at |a-b| <= 1e-4 * max(|b|, 1) with
+      k-sets and counts exact, and SONET_TC=fp16 at 3.5e-3 of max|golden|. Each case asserts from
+      ops.PROFILE that the kernels ran at the ELU code and never at ReLU, and that no PyTorch
+      ELU or convolution ran (these models took the PyTorch path before the kernels had ELU);
+  (b) each kernel entry at act = ELU against fp64, inputs centred so that >= 30% of the
+      pre-activations are negative; the KNN kernel's max-before-activation bit for bit;
+  (c) train mode: BN-train forward / backward with ELU against fp64, one optimize() step with the
+      train kernels on vs off;
+  (d) CUDA graphs: models of different activation never replay each other's graph."""
+import contextlib
+import copy
+import math
+
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+from helpers import (assert_close, assert_golden, build_states, check_encoder_against_golden,
+                     golden, golden_case, sampled, to_ref_slot_order)
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda:0"
+ELU, RELU = 2, 1
+HEAD = {"classifier": "classifier", "segmenter": "segmenter", "autoencoder": "decoder"}
+FIXTURES = [("classifier", "elu_classifier_b2_n256"),
+            ("classifier", "elu_classifier_b2_n200_emptynodes"),
+            ("classifier", "elu_classifier_b2_n256_somk0"),
+            ("segmenter", "elu_segmenter_b2_n128"),
+            ("autoencoder", "elu_autoencoder_b2_n256")]
+# the activation argument's position in each entry's argument list
+ACT_ARG = {"sonet_pointwise_tc_forward": 10, "sonet_pointwise_tc_forward_f16": 10,
+           "sonet_pointwise_tc_forward_rows": 10, "sonet_pointwise_tc_forward_rows_f16": 10,
+           "sonet_pointwise_tc_grouped_forward": 9, "sonet_pointwise_tc_grouped_forward_f16": 9,
+           "sonet_pointwise_layer_f32": 10, "sonet_linear_f32": 7,
+           "sonet_pointresnet_tc_forward_act": 6, "sonet_pointresnet_tc_pool_forward_act": 9,
+           "sonet_knn_mlp_tc_forward_act": 14}
+RELU_ONLY = ("sonet_pointresnet_tc_forward", "sonet_pointresnet_tc_pool_forward",
+             "sonet_knn_mlp_tc_forward", "sonet_pointresnet_tc_forward_f16",
+             "sonet_pointresnet_tc_pool_forward_f16", "sonet_knn_mlp_tc_forward_f16")
+FP16_REL = 3.5e-3
+# The final outputs of the two deepest heads miss 1e-4 by a hair: measured on an H100 80GB HBM3,
+# score_segmenter 1.01e-4 (wgmma routes) and the auto-encoder's predicted_pc 1.11e-4 (SONET_TC=0,
+# where the 3x3 up-convolutions run on strict-fp32 cuDNN). The encoder's attributes, every other
+# head and the other routes hold 1e-4.
+HEAD_TOL = {"score_segmenter": 2e-4, "predicted_pc": 2e-4}
+
+
+def _model(task, opt, st):
+    from sonet_b200 import autoencoder, classifier, segmenter
+    gopt = copy.copy(opt)
+    gopt.device, gopt.gpu_id = torch.device(DEV), 0
+    mod = {"classifier": classifier, "segmenter": segmenter, "autoencoder": autoencoder}[task]
+    m = mod.Model(gopt)
+    m.encoder.load_state_dict(st["encoder"])
+    getattr(m, HEAD[task]).load_state_dict(st["head"])
+    return m
+
+
+def _set_input(m, task, inp):
+    if task == "segmenter":
+        seg = torch.zeros(inp["pc"].shape[0], inp["pc"].shape[2], dtype=torch.int64)
+        m.set_input(inp["pc"], inp["sn"], inp["label"], seg, inp["node"], inp["node_knn_I"])
+    else:
+        m.set_input(inp["pc"], inp["sn"], inp["label"], inp["node"], inp["node_knn_I"])
+
+
+@contextlib.contextmanager
+def _torch_calls(monkeypatch):
+    """Counts PyTorch ELU modules, F.elu and convolutions run while the block executes."""
+    from sonet_b200 import train_ops
+    n = {"elu": 0, "conv": 0}
+
+    def counted(key, fn):
+        def f(*a, **k):
+            n[key] += 1
+            return fn(*a, **k)
+        return f
+    monkeypatch.setattr(torch.nn.ELU, "forward", counted("elu", torch.nn.ELU.forward))
+    monkeypatch.setattr(F, "elu", counted("elu", F.elu))
+    for cls in (torch.nn.Conv1d, torch.nn.Conv2d, torch.nn.Linear):
+        monkeypatch.setattr(cls, "forward", counted("conv", cls.forward))
+    monkeypatch.setattr(train_ops, "conv_strict", counted("conv", train_ops.conv_strict))
+    yield n
+
+
+def _run(m, task, inp, monkeypatch):
+    from sonet_b200 import ops
+    _set_input(m, task, inp)
+    ops.PROFILE = []
+    try:
+        with _torch_calls(monkeypatch) as n:
+            m.test_model()
+            torch.cuda.synchronize()
+        return [(name, args) for name, _, _, args in ops.PROFILE], n
+    finally:
+        ops.PROFILE = None
+
+
+def _assert_elu_route(calls, n, route, task):
+    names = {c for c, _ in calls}
+    acts = {(c, a[ACT_ARG[c]]) for c, a in calls if c in ACT_ARG}
+    assert not names & set(RELU_ONLY), "a ReLU-only entry ran: %s" % sorted(names & set(RELU_ONLY))
+    assert all(a != RELU for _, a in acts), "a launch at the ReLU code: %s" % sorted(acts)
+    elu_calls = {c for c, a in acts if a == ELU}
+    if route == "fp32":
+        assert not [c for c in names if "_tc_" in c], sorted(names)
+        assert "sonet_pointwise_layer_f32" in elu_calls
+    elif route == "fused":
+        assert "sonet_pointresnet_tc_pool_forward_act" in elu_calls, sorted(elu_calls)
+    else:
+        assert "sonet_pointresnet_tc_forward_act" in elu_calls, sorted(elu_calls)
+        assert "sonet_pointresnet_tc_pool_forward_act" not in names
+    # the point-wise layers at ELU: on wgmma, or below two 128-row tiles on the fp32 kernel
+    assert any(c.startswith(("sonet_pointwise_tc_", "sonet_pointwise_layer_f32"))
+               for c in elu_calls), sorted(elu_calls)
+    assert "sonet_linear_f32" in elu_calls or task == "segmenter", sorted(elu_calls)
+    # SONET_TC=0 runs the auto-encoder's 3x3 up-convolutions on cuDNN, ReLU models included
+    if not (route == "fp32" and task == "autoencoder"):
+        assert n == {"elu": 0, "conv": 0}, "PyTorch ran: %s" % n
+
+
+def _check_fp16(g, name, t):
+    ref = torch.from_numpy(g[name]).double()
+    got = sampled(g, name, t).double()
+    err = float((got - ref).abs().max())
+    assert err <= FP16_REL * float(ref.abs().max()), "%s: %.3e > %.1e of max|golden| %.3e" % (
+        name, err, FP16_REL, float(ref.abs().max()))
+
+
+@pytest.mark.parametrize("route", ["fused", "unfused", "fp32", "fp16"])
+@pytest.mark.parametrize("task,name", FIXTURES)
+def test_elu_models_vs_reference_golden(monkeypatch, task, name, route):
+    g = golden(name)
+    opt, inp, seed = golden_case(g, task)
+    assert opt.activation == "elu"
+    if route == "fp32":
+        monkeypatch.setenv("SONET_TC", "0")
+    elif route == "fp16":
+        monkeypatch.setenv("SONET_TC", "fp16")
+    m = _model(task, opt, build_states(task, opt, seed))
+    m.encoder.fuse_pool = route != "unfused"      # unfused: first_pn_out materialised
+    calls, n = _run(m, task, inp, monkeypatch)
+    _assert_elu_route(calls, n, "fused" if route == "fp16" else route, task)
+    enc = m.encoder
+    outs = {"classifier": ["score"], "segmenter": ["score_segmenter"],
+            "autoencoder": ["predicted_pc", "conv_pc4"]}[task]
+    head = {o: (getattr(m, o) if hasattr(m, o) else getattr(m.decoder, o)) for o in outs}
+    if route == "fp16":
+        for nm in ("first_pn_out_masked_max", "final_pn_out", "feature"):
+            _check_fp16(g, nm, getattr(enc, nm))
+        for nm, t in head.items():
+            _check_fp16(g, nm, t)
+        return
+    check_encoder_against_golden(g, enc, opt)
+    for nm, t in head.items():
+        assert_golden(g, nm, t, HEAD_TOL.get(nm, 1e-4))
+    if task == "segmenter":
+        assert_golden(g, "centers", to_ref_slot_order(enc.centers, enc.min_idx, g, opt.k))
+    if task == "autoencoder":
+        assert_close(m.loss_chamfer, g["loss_chamfer"], "loss_chamfer")
+
+
+# ---- (b) per kernel against fp64 -----------------------------------------------------------------
+def _elu64(z):
+    return torch.where(z > 0, z, torch.expm1(z))
+
+
+def _centred(shape, seed, scale=1.0):
+    g = torch.Generator().manual_seed(seed)
+    return ((torch.rand(*shape, generator=g) * 2 - 1) * scale).to(DEV)
+
+
+def _neg_share(z):
+    share = float((z < 0).double().mean())
+    assert share >= 0.3, "only %.2f of the pre-activations are negative" % share
+    return share
+
+
+def _assert_fp64(got, z, mag, rel, what):
+    """got against elu(z) (fp64), per element within rel * (sum_k |w_k x_k| + |shift|)."""
+    y = _elu64(z)
+    err = (got.detach().double() - y).abs()
+    u = float((err / (rel * mag + 1e-30)).max())
+    assert u <= 1.0, "%s: error %.3g x the bar" % (what, u)
+
+
+# tile remainders of the generic layer (test_gpu_tc_envelope.py's shapes): rows around 128,
+# Cout around 64 / 128 / 256, Cin off the 16 / 64 grid, a second source
+TC_SHAPES = [(1, 35, 0, 129, 64), (3, 100, 0, 333, 72), (2, 64, 35, 255, 200), (2, 387, 0, 130, 512)]
+
+
+@pytest.mark.parametrize("f16", [False, True])
+@pytest.mark.parametrize("rows", [False, True])
+@pytest.mark.parametrize("shape", TC_SHAPES)
+def test_generic_layer_elu(shape, rows, f16):
+    from sonet_b200 import ops
+    B, C0, C1, P, Cout = shape
+    W = _centred((Cout, C0 + C1), 1 + C0, 1 / math.sqrt(C0 + C1))
+    sh = _centred((Cout,), 2 + Cout, 0.3) - 0.2
+    x0 = _centred((B, C0, P), 3 + P)
+    x1 = _centred((B, C1, P), 4 + P) if C1 else None
+    blob, inv = ops.pointwise_tc_pack(W)
+    out = ops.pointwise_layer_tc(x0, blob.to(DEV), inv, sh, Cout, "elu", x1=x1, rows=rows, f16=f16)
+    if rows:
+        out = out.transpose(1, 2)
+    x = x0 if x1 is None else torch.cat((x0, x1), 1)
+    z = torch.einsum("oc,bcp->bop", W.double(), x.double()) + sh.double()[None, :, None]
+    mag = torch.einsum("oc,bcp->bop", W.double().abs(), x.double().abs()) + sh.double().abs()[None, :, None]
+    _neg_share(z)
+    _assert_fp64(out, z, mag, 2e-3 if f16 else 1e-5, "layer %s rows=%s f16=%s" % (shape, rows, f16))
+    # the fp32 kernel at the same shape
+    wt = W.t().contiguous()
+    out32 = ops.pointwise_layer(x0, wt, None, sh, "elu", x1=x1)
+    _assert_fp64(out32, z, mag, 1e-6, "fp32 layer %s" % (shape,))
+
+
+@pytest.mark.parametrize("splits", [1, 2])
+def test_grouped_layer_elu(splits):
+    """The grouped launch and, with splits > 1, the split-K reduce kernel's ELU epilogue."""
+    from sonet_b200 import ops
+    G, B, C, P, Cout = 2, 2, 256, 200, 128
+    W = _centred((G, Cout, C), 11, 1 / math.sqrt(C))
+    sh = _centred((Cout,), 12, 0.3) - 0.2
+    x = _centred((G * B, C, P), 13)
+    blob, per, inv = ops.pointwise_tc_pack_groups(W)
+    out = ops.pointwise_tc_grouped(x, blob.to(DEV), per, inv, sh, Cout, "elu", groups=G,
+                                   splits=splits)
+    xg = x.double().view(G, B, C, P)
+    z = torch.einsum("goc,gbcp->gbop", W.double(), xg) + sh.double()[None, None, :, None]
+    mag = torch.einsum("goc,gbcp->gbop", W.double().abs(), xg.abs()) + sh.double().abs()[None, None, :, None]
+    _neg_share(z)
+    _assert_fp64(out.view(G, B, Cout, P), z, mag, 1e-5, "grouped splits=%d" % splits)
+
+
+@pytest.mark.parametrize("hw", [1, 4, 8])
+def test_upconv_elu(hw):
+    """UpConv's parity GEMMs with ELU (hw = 1: the 1x1-input dense layer; 8: the im2col-free
+    conv mode) against the fp64 composition upsample -> conv -> BN -> ELU."""
+    from sonet_b200 import layers, ops
+    Cin, Cout, B = 64, 64, 2
+    torch.manual_seed(hw)
+    up = layers.UpConv(Cin, Cout, activation="elu", normalization="batch")
+    with torch.no_grad():
+        bn = up.conv.norm
+        bn.running_mean.normal_(0, 0.5)
+        bn.running_var.uniform_(0.5, 2.0)
+        bn.weight.uniform_(0.5, 1.5)
+        bn.bias.normal_(0, 0.3)
+    up = up.to(DEV).eval()
+    x = _centred((B, Cin, hw, hw), 21 + hw)
+    ops.PROFILE = []
+    try:
+        with torch.no_grad():
+            got = up(x)
+        names = [n for n, _, _, _ in ops.PROFILE]
+    finally:
+        ops.PROFILE = None
+    assert any(n.startswith("sonet_pointwise_tc_grouped_forward") for n in names), names
+    c = up.conv.conv
+    xu = F.interpolate(x.double(), scale_factor=2, mode="nearest")
+    z = F.conv2d(xu, c.weight.double(), c.bias.double(), padding=1)
+    s = bn.weight.double() / torch.sqrt(bn.running_var.double() + bn.eps)
+    z = (z - bn.running_mean.double()[None, :, None, None]) * s[None, :, None, None] + bn.bias.double()[None, :, None, None]
+    mag = F.conv2d(xu.abs(), c.weight.double().abs(), c.bias.double().abs(), padding=1)
+    mag = mag * s.abs()[None, :, None, None] + (bn.running_mean.double().abs() * s.abs() + bn.bias.double().abs())[None, :, None, None]
+    _neg_share(z)
+    _assert_fp64(got, z, mag.detach(), 1e-5, "UpConv %dx%d" % (hw, hw))
+
+
+def test_linear_elu():
+    from sonet_b200 import ops
+    for B, Cin, Cout in ((3, 64, 40), (70, 1024, 512), (5, 33, 17)):
+        W = _centred((Cout, Cin), Cin, 1 / math.sqrt(Cin))
+        sh = _centred((Cout,), Cout, 0.3) - 0.2
+        x = _centred((B, Cin), B)
+        out = ops.linear(x, W, None, sh, "elu")
+        z = x.double() @ W.double().t() + sh.double()
+        mag = x.double().abs() @ W.double().abs().t() + sh.double().abs()
+        _neg_share(z)
+        _assert_fp64(out, z, mag, 1e-6, "linear %d %d %d" % (B, Cin, Cout))
+
+
+def _pointresnet(seed):
+    from sonet_b200 import layers
+    torch.manual_seed(seed)
+    pr = layers.PointResNet(6, [64, 128, 256, 384], "elu", "batch")
+    with torch.no_grad():
+        for l in pr.layers[:3]:
+            l.conv.bias.normal_(0, 0.1)
+            l.norm.running_mean.normal_(0, 0.3)
+            l.norm.running_var.uniform_(0.5, 2.0)
+            l.norm.weight.uniform_(0.5, 1.5)
+            l.norm.bias.normal_(-0.3, 0.3)          # centred below 0: many negative pre-activations
+    return pr.to(DEV).eval()
+
+
+def _pointresnet64(pr, x):
+    """fp64 forward of the fused PointResNet; returns (out, bar magnitude, pre-activations)."""
+    h, mag, zs = x.double(), x.double().abs(), []
+    outs = []
+    for i, l in enumerate(pr.layers):
+        w, s = l.folded()
+        inp, im = (h, mag) if i < 3 else (torch.cat((outs[0][0], h), 1), torch.cat((outs[0][1], mag), 1))
+        z = torch.einsum("oc,bcp->bop", w.double(), inp) + s.double()[None, :, None]
+        m = torch.einsum("oc,bcp->bop", w.double().abs(), im) + s.double().abs()[None, :, None]
+        if i < 3:
+            zs.append(z)
+            h, mag = _elu64(z), m
+            outs.append((h, m))
+        else:
+            h, mag = z, m
+    return h, mag, torch.cat([z.flatten() for z in zs])
+
+
+@pytest.mark.parametrize("f16", [False, True])
+@pytest.mark.parametrize("P", [128, 333])
+def test_pointresnet_elu_plain_and_pool(P, f16):
+    from sonet_b200 import ops
+    pr = _pointresnet(P)
+    B, M = 2, 16
+    x = _centred((B, 6, P), P + 1)
+    blob, fpar = pr._tc_params()
+    out = ops.pointresnet_tc(x, blob, fpar, f16=f16, act="elu")
+    y, mag, zs = _pointresnet64(pr, x)
+    _neg_share(zs)
+    err = (out.double() - y).abs()
+    rel = 1e-2 if f16 else 2e-5
+    u = float((err / (rel * mag + 1e-6)).max())
+    assert u <= 1.0, "PointResNet P=%d f16=%s: %.3g x the bar" % (P, f16, u)
+    # pool: node-sorted rows -> per-node maxima == the max over the plain kernel's rows
+    node = torch.sort(torch.randint(0, M, (B, P), generator=torch.Generator().manual_seed(P)), 1)[0]
+    node = node.to(torch.int32).to(DEV).contiguous()
+    pos0 = torch.zeros(B, dtype=torch.int32, device=DEV)
+    pooled = ops.pointresnet_tc_pool(x, blob, fpar, node, pos0, M, f16=f16, act="elu")
+    want = torch.full((B, 384, M), -float("inf"), device=DEV, dtype=torch.float64)
+    want = want.scatter_reduce(2, node.long().unsqueeze(1).expand(B, 384, P), out.double(), "amax")
+    filled = torch.isfinite(want) & (want > -1000)
+    want = torch.where(filled, want, out[:, :, :1].double().expand(B, 384, M))
+    assert torch.equal(pooled.double(), want), "pool != per-node max of the plain kernel"
+
+
+@pytest.mark.parametrize("f16", [False, True])
+@pytest.mark.parametrize("K", [2, 9])
+def test_knn_kernel_max_before_elu_bit_exact(K, f16):
+    """The fused KNN kernel applies ELU once to the max over the raw layer-2 accumulators. Its
+    output must equal max over neighbours j of elu(layer 2 of row (m, j)), each row computed by
+    the same kernel alone (both neighbour slots = j: the max of two equal rows is that row)."""
+    from sonet_b200 import layers, ops
+    torch.manual_seed(K)
+    mod = layers.KNNModule(3 + 384, (512, 512), "elu", "batch")
+    with torch.no_grad():
+        for l in mod.layers:
+            l.conv.bias.normal_(0, 0.1)
+            l.norm.running_mean.normal_(0, 0.3)
+            l.norm.running_var.uniform_(0.5, 2.0)
+            l.norm.weight.uniform_(0.5, 1.5)
+            l.norm.bias.normal_(-0.3, 0.3)
+    mod = mod.to(DEV).eval()
+    B, M = 2, 64
+    coord = _centred((B, 3, M), 5)
+    x = _centred((B, 384, M), 6)
+    d = ((coord.unsqueeze(3) - coord.unsqueeze(2)) ** 2).sum(1)
+    knn_I = torch.topk(d, k=K, dim=2, largest=False, sorted=True)[1].contiguous()
+    pk = mod._tc_params()
+    y = ops.pointwise_layer_tc(x, pk["yblob"], pk["yinv"], None, 512, None, rows=True, f16=f16)
+    run = lambda idx: ops.knn_mlp_tc(coord, coord, idx, K if idx is knn_I else 2,  # noqa: E731
+                                     y.transpose(1, 2), pk["w1"], pk["blob2"], pk["inv2"],
+                                     pk["shift2"], f16=f16, act="elu")
+    full = run(knn_I)
+    per_row = [run(knn_I[:, :, j:j + 1].expand(B, M, 2).contiguous()) for j in range(K)]
+    want = torch.stack(per_row, 0).max(0)[0]
+    assert torch.equal(full, want), "max-before-ELU differs from ELU-then-max"
+    assert float((torch.stack(per_row) < 0).double().mean()) >= 0.3
+    # and the module routes its ELU layers through this kernel
+    ops.PROFILE = []
+    try:
+        with torch.no_grad():
+            _, feat = mod(coord, x, knn_I, K, "center")
+        names = [n for n, _, _, _ in ops.PROFILE]
+    finally:
+        ops.PROFILE = None
+    assert "sonet_knn_mlp_tc_forward_act" in names and "sonet_knn_mlp_tc_forward" not in names, names
+
+
+# ---- (c) train mode --------------------------------------------------------------------------------
+EPS = 1e-5
+
+
+@pytest.mark.parametrize("B,C,P", [(1, 1, 5), (4, 64, 512), (2, 300, 77), (32, 3, 1024)])
+def test_bn_train_elu_vs_fp64(B, C, P):
+    from sonet_b200 import train_ops
+    x = (_centred((B, C, P), B * C + P) * 3 + _centred((1, C, 1), C, 2.0)).contiguous()
+    gamma = (torch.rand(C, device=DEV) + 0.5)
+    beta = _centred((C,), 7, 0.5)
+    w = _centred((B, C, P), 8)
+    xg, gg, bg = (t.clone().requires_grad_(True) for t in (x, gamma, beta))
+    y, mean, var = train_ops.BNActTrain.apply(xg, gg, bg, EPS, "elu")
+    y.backward(w)
+    x64, g64, b64 = (t.double().requires_grad_(True) for t in (x, gamma, beta))
+    z = F.batch_norm(x64, None, None, g64, b64, True, 0.0, EPS)
+    y64 = F.elu(z)
+    y64.backward(w.double())
+    if B * P > 1:
+        _neg_share(z.detach())
+    for got, ref, nm in ((y, y64, "y"), (xg.grad, x64.grad, "dx"), (gg.grad, g64.grad, "dgamma"),
+                         (bg.grad, b64.grad, "dbeta")):
+        ref = ref.detach()
+        scale = float(ref.abs().max()) + 1e-30
+        err = float((got.double() - ref).abs().max())
+        assert err <= 1e-4 * scale, "%s: %.3e of %.3e" % (nm, err, scale)
+
+
+@contextlib.contextmanager
+def train_kernels(on):
+    from sonet_b200 import train_ops
+    prev = train_ops.ENABLED
+    train_ops.ENABLED = on
+    try:
+        yield
+    finally:
+        train_ops.ENABLED = prev
+
+
+@contextlib.contextmanager
+def precision_flags(cudnn_tf32, matmul_tf32=False):
+    prev = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
+    torch.backends.cudnn.allow_tf32 = cudnn_tf32
+    torch.backends.cuda.matmul.allow_tf32 = matmul_tf32
+    try:
+        yield
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+
+
+def _analytically_zero(grads, name):
+    w = name[:-4] + "weight"
+    return (name.endswith(".bias") and w in grads
+            and float(grads[name].abs().max()) < 1e-3 * float(grads[w].abs().max()))
+
+
+def _wrapper_step(task, enabled):
+    from sonet_b200 import autoencoder, classifier, segmenter, synth
+    B, N = 4, 512
+    opt = synth.make_opt(task, batch_size=B, input_pc_num=N, device=DEV, activation="elu")
+    opt.device = torch.device(DEV)
+    st = build_states(task, opt, seed=29)
+    inp = synth.synth_inputs(B, N, seed=29)
+    mod = {"classifier": classifier, "segmenter": segmenter, "autoencoder": autoencoder}[task]
+    head = HEAD[task]
+    with train_kernels(enabled), precision_flags(cudnn_tf32=enabled):
+        m = mod.Model(opt)
+        m.encoder.load_state_dict(st["encoder"])
+        getattr(m, head).load_state_dict(st["head"])
+        if task == "segmenter":
+            seg = torch.from_numpy(np.random.RandomState(29).randint(0, 50, size=(B, N)))
+            m.set_input(inp["pc"], inp["sn"], inp["label"], seg, inp["node"], inp["node_knn_I"])
+        else:
+            m.set_input(inp["pc"], inp["sn"], inp["label"], inp["node"], inp["node_knn_I"])
+        torch.manual_seed(0)
+        m.optimize(epoch=2)
+    mods = (m.encoder, getattr(m, head))
+    state = {"%d.%s" % (i, k): v.detach().clone() for i, mm in enumerate(mods)
+             for k, v in mm.state_dict().items()}
+    grads = {"%d.%s" % (i, k): p.grad.detach().clone() for i, mm in enumerate(mods)
+             for k, p in mm.named_parameters() if p.grad is not None}
+    before = {"%d.%s" % (i, k): v for i, sd in enumerate((st["encoder"], st["head"]))
+              for k, v in sd.items()}
+    return state, grads, before, opt.lr
+
+
+def _adam_first_step_dir(g):
+    return g / (g.abs() + 1e-8)
+
+
+STEP_GRAD_TOL = 1e-4
+
+
+@pytest.mark.parametrize("task", ["classifier", "segmenter", "autoencoder"])
+def test_elu_optimize_step_kernels_on_vs_off(task):
+    """One optimize() of an ELU model, train kernels on vs the PyTorch composition: the criteria
+    of test_gpu_train_parity.py's kernels-on-vs-off step test."""
+    from sonet_b200 import ops
+    ops.PROFILE = []
+    try:
+        on, g_on, before, lr = _wrapper_step(task, True)
+        bn_acts = [a[7] for n, _, _, a in ops.PROFILE if n == "sonet_bn_train_forward_f32"]
+    finally:
+        ops.PROFILE = None
+    assert bn_acts and set(bn_acts) == {ELU}, bn_acts
+    off, g_off, _, _ = _wrapper_step(task, False)
+    assert set(on) == set(off)
+    for k, ref in off.items():
+        got = on[k]
+        if k.endswith("num_batches_tracked"):
+            assert torch.equal(got, ref), k
+        elif k.endswith(("running_mean", "running_var")):
+            err = float((got - ref).abs().max() / ref.abs().max().clamp(min=1e-30))
+            assert err <= 1e-4, "%s: %.3e" % (k, err)
+        else:
+            if k not in g_off:
+                assert torch.equal(got, ref), k
+                continue
+            g = g_off[k].double()
+            if _analytically_zero(g_off, k):
+                slack = 2 * lr * torch.ones_like(g)
+            else:
+                eps_g = STEP_GRAD_TOL * g.abs().max()
+                d0 = _adam_first_step_dir(g)
+                slack = lr * torch.maximum((_adam_first_step_dir(g + eps_g) - d0).abs(),
+                                           (_adam_first_step_dir(g - eps_g) - d0).abs())
+            p0 = before[k].to(DEV).double()
+            bar = 1e-6 * p0.abs().max() + slack
+            diff = (got.double() - ref.double()).abs()
+            assert bool((diff <= 1e-6 * p0.abs().max() + 2 * lr).all()), k
+            if task == "autoencoder":
+                continue
+            firm = g.abs() >= 1e-2 * g.abs().max()
+            bad = firm & (diff > bar)
+            assert int(bad.sum()) <= max(4, 1e-4 * g.numel()), "%s: %d elements over the bar" % (
+                k, int(bad.sum()))
+
+
+# ---- (d) CUDA graphs ---------------------------------------------------------------------------------
+def test_cuda_graph_never_replays_across_activations():
+    """Two classifiers of different activation with graphs enabled, run alternately, each match
+    their own reference fixture; and flipping one model's activation re-captures its graph."""
+    models = {}
+    for name in ("classifier_b2_n256", "elu_classifier_b2_n256"):
+        g = golden(name)
+        opt, inp, seed = golden_case(g, "classifier")
+        m = _model("classifier", opt, build_states("classifier", opt, seed))
+        m.enable_cuda_graph(True)
+        models[name] = (g, m, inp)
+    for _ in range(2):
+        for name, (g, m, inp) in models.items():
+            _set_input(m, "classifier", inp)
+            m.test_model()
+            torch.cuda.synchronize()
+            assert_golden(g, "score", m.score)
+    # the same instance, its activation switched to the other model's: no stale replay
+    g_r, m_e, inp = models["elu_classifier_b2_n256"][0], models["elu_classifier_b2_n256"][1], \
+        models["elu_classifier_b2_n256"][2]
+    _set_input(m_e, "classifier", inp)
+    m_e.test_model()
+    torch.cuda.synchronize()
+    elu_score = m_e.score.clone()
+    for mod in list(m_e.encoder.modules()) + list(m_e.classifier.modules()):
+        if getattr(mod, "activation", None) == "elu":
+            mod.activation = "relu"
+    _set_input(m_e, "classifier", inp)
+    m_e.test_model()
+    torch.cuda.synchronize()
+    assert_golden(models["classifier_b2_n256"][0], "score", m_e.score)
+    assert not torch.equal(elu_score, m_e.score)
