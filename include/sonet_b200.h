@@ -194,6 +194,30 @@ int sonet_bn_train_backward_f32(const float* dy, const float* x, const float* me
                                 float* dbeta, sonet_stream_t stream);
 int sonet_index_max_backward_f32(const float* grad_out, const int32_t* idx, int B, int C, int N, int K,
                                  float* grad_data, sonet_stream_t stream);
+/* Instance normalisation, nn.InstanceNorm1d/2d(C, affine=True) with track_running_stats=False
+ * (models/layers.py:133, 179, 257): eval and train compute the same forward. For each
+ * row r = b*C + c of z [B,C,P] (P = points, neighbour slots or pixels), the biased mean and
+ * variance of the row, then y = act(gamma[c]*(z - mean)*invstd + beta[c]), invstd = 1/sqrt(var+eps).
+ * Statistics are exact two-pass (mean, then sum (z-mean)^2) in fp64 in a fixed order:
+ * bit-reproducible; a constant row gives y = act(beta) exactly. gamma, beta nullable (identity);
+ * act: SONET_ACT_*. reduce folds a reduction of the activated rows into the same pass:
+ *   SONET_REDUCE_NONE       out [B,C,P], may alias z; k unused
+ *   SONET_REDUCE_KCOPY_MEAN out [B,C,P/k], the mean over k stacked copies, copy j of point n at
+ *                           j*(P/k) + n, summed in the reference's order (models/networks.py:331-336):
+ *                           0.5*(a+b), (1/3)*((a+b)+c)
+ *   SONET_REDUCE_GROUP_MAX  out [B,C,P/k], the max over consecutive groups of k (the KNN module's
+ *                           max over neighbours, models/layers.py:365)
+ * save_mean, save_invstd (nullable together) [B,C]: the row statistics sonet_bn_train_backward_f32
+ * takes on the [1, B*C, P] view, which is the instance-norm backward of every row.
+ * One read of z and one write of out for rows of P <= 16384 (staged on chip); longer rows read z
+ * again. Fails with SONET_ERR_BAD_ARG before any CUDA call for P < 2 (PyTorch: "Expected more than
+ * 1 spatial element"), an unknown act or reduce code, or P not divisible by k. */
+#define SONET_REDUCE_NONE 0
+#define SONET_REDUCE_KCOPY_MEAN 1
+#define SONET_REDUCE_GROUP_MAX 2
+int sonet_instance_norm_f32(const float* z, const float* gamma, const float* beta, int B, int C, int P,
+                            float eps, int act, int reduce, int k, float* out, float* save_mean,
+                            float* save_invstd, sonet_stream_t stream);
 int sonet_pointwise_tc_pack_device(const float* W, int Cout, int Cin, int transpose, void* blob,
                                    float* scale2, unsigned* scratch_bits, sonet_stream_t stream);
 int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, int P, const void* blob,

@@ -11,6 +11,10 @@
 //                                derivative at the recomputed BN output z: [z > 0] for ReLU,
 //                                z > 0 ? 1 : exp(z) for ELU), then dx = gamma*invstd*(g - mean(g) -
 //                                xhat*mean(g*xhat)); dgamma, dbeta fall out of the sums
+//   instance_norm (1 launch)     per-row statistics of z[B,C,P] (InstanceNorm, eval and train
+//                                alike) and y = act(gamma*(z-mean)*invstd + beta), optionally reduced
+//                                to the k-copy mean or the max over groups of K; its backward is
+//                                bn_backward on the [1, B*C, P] view
 //   index_max_backward           grad of first_pn_out through the masked gather: zero-fill +
 //                                scatter-add of grad[b,c,k] at idx[b,c,k] (duplicates — every empty
 //                                node gathers point 0 — are added by ONE thread in ascending k)
@@ -172,6 +176,179 @@ __global__ void __launch_bounds__(256)
     else if (relu && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
     dx[o + p] = ga * is * (g - k0 - xh * k1);
   }
+}
+
+// ---- instance normalisation (nn.InstanceNorm1d/2d, affine, no running statistics) -----------------
+// Row r = b*C + c of z [B,C,P] is normalised by its own biased statistics: y = act(gamma_c * (z -
+// mean_r) * invstd_r + beta_c). The row is staged on chip once; the statistics are exact two-pass
+// (mean, then sum (z - mean)^2) with fp64 accumulation, every thread summing its strided elements in
+// ascending order and the partial sums combined by a fixed butterfly / warp order: bit-reproducible.
+// A constant row gives var = 0, z - mean = 0 and y = act(beta) exactly. The output pass can fold the
+// k-copy mean (copy j of point n at j*N + n, summed (a+b)+c in fp32 and scaled like kcopy_mean_kernel)
+// or the max over consecutive groups of K (after the activation, fmaxf like the rowmax kernels).
+constexpr int IN_THREADS = 256;
+constexpr int IN_WARP_ROW_MAX = 1024;      // rows up to this length: a warp per row, 8 rows per CTA
+constexpr int IN_ROW_SMEM_MAX = 16384;     // longer rows up to this length: a CTA per row, staged
+                                           // in 64 KB of shared memory; beyond it z is read again
+
+__device__ __forceinline__ double in_warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);   // same bits in all lanes
+  return v;
+}
+
+// thread t of nt writes its share of the output row o from the row s (shared or global memory)
+template <int ACT, int RED>
+__device__ __forceinline__ void in_write_row(const float* s, int P, int k, float mu, float is, float ga,
+                                             float be, float* o, int t, int nt) {
+  if constexpr (RED == SONET_REDUCE_NONE) {
+    for (int p = t; p < P; p += nt) o[p] = act_fn<ACT>(fmaf(ga, (s[p] - mu) * is, be));
+  } else if constexpr (RED == SONET_REDUCE_KCOPY_MEAN) {
+    const int N = P / k;
+    const float w = (k == 2) ? 0.5f : (k == 3 ? (1.0f / 3.0f) : __fdiv_rn(1.0f, (float)k));
+    for (int n = t; n < N; n += nt) {
+      float acc = act_fn<ACT>(fmaf(ga, (s[n] - mu) * is, be));
+      for (int j = 1; j < k; ++j)
+        acc = __fadd_rn(acc, act_fn<ACT>(fmaf(ga, (s[j * N + n] - mu) * is, be)));
+      o[n] = __fmul_rn(w, acc);
+    }
+  } else {
+    const int G = P / k;
+    for (int g = t; g < G; g += nt) {
+      const float* q = s + static_cast<size_t>(g) * k;
+      float m = act_fn<ACT>(fmaf(ga, (q[0] - mu) * is, be));
+      for (int j = 1; j < k; ++j) m = fmaxf(m, act_fn<ACT>(fmaf(ga, (q[j] - mu) * is, be)));
+      o[g] = m;
+    }
+  }
+}
+
+__device__ __forceinline__ long long in_out_len(int P, int k, int red) {
+  return red == SONET_REDUCE_NONE ? P : P / k;
+}
+
+// rows with P <= IN_WARP_ROW_MAX: warp w of the CTA owns row 8*blockIdx.x + w, staged in srow[w]
+template <int ACT, int RED>
+__global__ void __launch_bounds__(IN_THREADS)
+    instance_norm_warp_kernel(const float* z, const float* __restrict__ gamma,
+                              const float* __restrict__ beta, long long R, int C, int P, float eps,
+                              int k, float* out, float* __restrict__ save_mean,
+                              float* __restrict__ save_invstd) {
+  extern __shared__ float in_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long r = static_cast<long long>(blockIdx.x) * (IN_THREADS / 32) + warp;
+  if (r >= R) return;                                   // warp-uniform; no CTA barrier below
+  float* s = in_smem + static_cast<size_t>(warp) * P;
+  const float* zr = z + r * P;
+  double a = 0.0;
+  for (int p = lane; p < P; p += 32) {
+    const float v = zr[p];
+    s[p] = v;
+    a += v;
+  }
+  const double mean = in_warp_sum(a) / P;
+  double q = 0.0;
+  for (int p = lane; p < P; p += 32) {                  // the lane's own elements: no sync needed
+    const double d = static_cast<double>(s[p]) - mean;
+    q = fma(d, d, q);
+  }
+  const double var = in_warp_sum(q) / P;
+  const float mu = static_cast<float>(mean);
+  const float is = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+  const int c = static_cast<int>(r % C);
+  if (lane == 0 && save_mean) {
+    save_mean[r] = mu;
+    save_invstd[r] = is;
+  }
+  __syncwarp();
+  in_write_row<ACT, RED>(s, P, k, mu, is, gamma ? gamma[c] : 1.f, beta ? beta[c] : 0.f,
+                         out + r * in_out_len(P, k, RED), lane, 32);
+}
+
+__device__ __forceinline__ double in_block_sum(double v, double* red) {
+  v = in_warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+#pragma unroll
+  for (int w = 0; w < IN_THREADS / 32; ++w) s += red[w];
+  __syncthreads();                                      // red is reused by the next sum
+  return s;
+}
+
+// longer rows: CTA blockIdx.x owns row r; STAGED keeps it in shared memory, else z is re-read
+template <int ACT, int RED, bool STAGED>
+__global__ void __launch_bounds__(IN_THREADS)
+    instance_norm_row_kernel(const float* z, const float* __restrict__ gamma,
+                             const float* __restrict__ beta, int C, int P, float eps, int k,
+                             float* out, float* __restrict__ save_mean,
+                             float* __restrict__ save_invstd) {
+  extern __shared__ float in_smem[];
+  __shared__ double red[IN_THREADS / 32];
+  const long long r = blockIdx.x;
+  const float* zr = z + r * P;
+  double a = 0.0;
+  for (int p = threadIdx.x; p < P; p += IN_THREADS) {
+    const float v = zr[p];
+    if (STAGED) in_smem[p] = v;
+    a += v;
+  }
+  const double mean = in_block_sum(a, red) / P;
+  double q = 0.0;
+  for (int p = threadIdx.x; p < P; p += IN_THREADS) {
+    const double d = static_cast<double>(STAGED ? in_smem[p] : zr[p]) - mean;
+    q = fma(d, d, q);
+  }
+  const double var = in_block_sum(q, red) / P;          // its barriers also publish in_smem
+  const float mu = static_cast<float>(mean);
+  const float is = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+  const int c = static_cast<int>(r % C);
+  if (threadIdx.x == 0 && save_mean) {
+    save_mean[r] = mu;
+    save_invstd[r] = is;
+  }
+  // without a reduction out may alias z: each element is read and written by the same thread,
+  // after every thread's statistics reads (the barriers above)
+  in_write_row<ACT, RED>(STAGED ? in_smem : zr, P, k, mu, is, gamma ? gamma[c] : 1.f,
+                         beta ? beta[c] : 0.f, out + r * in_out_len(P, k, RED), threadIdx.x,
+                         IN_THREADS);
+}
+
+template <int ACT, int RED>
+static void launch_instance_norm(const float* z, const float* gamma, const float* beta, long long R,
+                                 int C, int P, float eps, int k, float* out, float* save_mean,
+                                 float* save_invstd, cudaStream_t st) {
+  if (P <= IN_WARP_ROW_MAX) {
+    const int rows = IN_THREADS / 32;
+    instance_norm_warp_kernel<ACT, RED>
+        <<<static_cast<unsigned>((R + rows - 1) / rows), IN_THREADS, sizeof(float) * rows * P, st>>>(
+            z, gamma, beta, R, C, P, eps, k, out, save_mean, save_invstd);
+  } else if (P <= IN_ROW_SMEM_MAX) {
+    const int smem = static_cast<int>(sizeof(float)) * P;
+    cudaFuncSetAttribute(instance_norm_row_kernel<ACT, RED, true>,
+                         cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    instance_norm_row_kernel<ACT, RED, true><<<static_cast<unsigned>(R), IN_THREADS, smem, st>>>(
+        z, gamma, beta, C, P, eps, k, out, save_mean, save_invstd);
+  } else {
+    instance_norm_row_kernel<ACT, RED, false><<<static_cast<unsigned>(R), IN_THREADS, 0, st>>>(
+        z, gamma, beta, C, P, eps, k, out, save_mean, save_invstd);
+  }
+}
+
+template <int ACT>
+static void launch_instance_norm_red(int reduce, const float* z, const float* gamma,
+                                     const float* beta, long long R, int C, int P, float eps, int k,
+                                     float* out, float* save_mean, float* save_invstd,
+                                     cudaStream_t st) {
+  if (reduce == SONET_REDUCE_KCOPY_MEAN)
+    launch_instance_norm<ACT, SONET_REDUCE_KCOPY_MEAN>(z, gamma, beta, R, C, P, eps, k, out, save_mean,
+                                                       save_invstd, st);
+  else if (reduce == SONET_REDUCE_GROUP_MAX)
+    launch_instance_norm<ACT, SONET_REDUCE_GROUP_MAX>(z, gamma, beta, R, C, P, eps, k, out, save_mean,
+                                                      save_invstd, st);
+  else
+    launch_instance_norm<ACT, SONET_REDUCE_NONE>(z, gamma, beta, R, C, P, eps, k, out, save_mean,
+                                                 save_invstd, st);
 }
 
 // grad_data[b,c,idx[b,c,k]] += grad_out[b,c,k], k ascending, one thread per (b,c) row
@@ -348,6 +525,39 @@ extern "C" int sonet_bn_train_backward_f32(const float* dy, const float* x, cons
     bn_bwd_apply_kernel<false><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
                                                      relu, inv_n, dx);
   return check_launch("bn_train_backward");
+}
+
+extern "C" int sonet_instance_norm_f32(const float* z, const float* gamma, const float* beta, int B,
+                                       int C, int P, float eps, int act, int reduce, int k, float* out,
+                                       float* save_mean, float* save_invstd, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(act, "instance_norm");
+  SONET_REQUIRE(reduce == SONET_REDUCE_NONE || reduce == SONET_REDUCE_KCOPY_MEAN ||
+                    reduce == SONET_REDUCE_GROUP_MAX,
+                "instance_norm: reduction code %d is not SONET_REDUCE_NONE (0), _KCOPY_MEAN (1) or "
+                "_GROUP_MAX (2)", reduce);
+  SONET_REQUIRE(B >= 1 && C >= 1, "instance_norm: bad dims B=%d C=%d", B, C);
+  SONET_REQUIRE(P >= 2, "instance_norm: Expected more than 1 spatial element (got P=%d)", P);
+  SONET_REQUIRE(reduce == SONET_REDUCE_NONE || (k >= 1 && P % k == 0),
+                "instance_norm: P=%d is not divisible by the %s k=%d", P,
+                reduce == SONET_REDUCE_KCOPY_MEAN ? "copy count" : "group size", k);
+  SONET_REQUIRE(z && out, "instance_norm: null pointer");
+  SONET_REQUIRE((save_mean == nullptr) == (save_invstd == nullptr),
+                "instance_norm: save_mean and save_invstd are given together or not at all");
+  SONET_REQUIRE(reduce == SONET_REDUCE_NONE || out != z, "instance_norm: a reduced output cannot alias z");
+  const long long R = static_cast<long long>(B) * C;
+  SONET_REQUIRE(R < (1LL << 31), "instance_norm: too many rows");
+  cudaStream_t st = as_stream(stream);
+  if (act == SONET_ACT_ELU)
+    launch_instance_norm_red<SONET_ACT_ELU>(reduce, z, gamma, beta, R, C, P, eps, k, out, save_mean,
+                                            save_invstd, st);
+  else if (act == SONET_ACT_RELU)
+    launch_instance_norm_red<SONET_ACT_RELU>(reduce, z, gamma, beta, R, C, P, eps, k, out, save_mean,
+                                             save_invstd, st);
+  else
+    launch_instance_norm_red<SONET_ACT_NONE>(reduce, z, gamma, beta, R, C, P, eps, k, out, save_mean,
+                                             save_invstd, st);
+  return check_launch("instance_norm");
 }
 
 extern "C" int sonet_index_max_backward_f32(const float* grad_out, const int32_t* idx, int B, int C,

@@ -40,6 +40,8 @@ _SIGNATURES = {
                                     c_void_p],
     "sonet_index_max_backward_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
                                      c_void_p],
+    "sonet_instance_norm_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_float,
+                                c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "sonet_pointwise_tc_pack_device": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                        c_void_p],
     "sonet_pointwise_tc_forward_dev": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,

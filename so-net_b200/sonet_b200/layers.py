@@ -10,8 +10,16 @@ require grad") instead of silently dropping parameter gradients. In train() mode
 requires grad (saliency / adversarial use in eval mode), or when EVAL_AUTOGRAD is set, the layers
 compose differentiable PyTorch ops on the GPU exactly as the reference does — the reference's own
 training path, not a CPU fallback. Both activations of the reference's options (relu, elu) run on
-the kernels, as does no activation; 'instance' norm, swish and leakyrelu always take the PyTorch
-path.
+the kernels, as does no activation; swish and leakyrelu always take the PyTorch path.
+
+Both normalizations of the reference's options (batch, instance) run on the kernels too. BatchNorm
+folds into the layer's GEMM in eval mode. Instance norm (track_running_stats=False: eval and train
+compute the same forward) needs each row's statistics over all its points first: an instance layer
+runs its GEMM with the conv bias and no activation, then ops.instance_norm applies the per-row
+statistics, gamma, beta and the activation in one pass, fused with the KNN module's max over
+neighbours or the segmenter's k-copy mean where those follow. MyLinear with instance norm keeps the
+PyTorch path: on a [B, C] input nn.InstanceNorm1d raises in the reference, and so it does here. The
+fused first-PointResNet and KNN kernels are BatchNorm-only; instance models take the per-layer chain.
 """
 import itertools
 import math
@@ -79,6 +87,17 @@ class MyBatchNorm2d(_MomentumDecayBatchNorm):
 
 # activations with a kernel epilogue (ops.act_code); others compose PyTorch ops
 KERNEL_ACTIVATIONS = (None, 'relu', 'elu')
+# normalizations with a kernel: BatchNorm folded into the GEMM, instance norm by ops.instance_norm
+KERNEL_NORMALIZATIONS = (None, 'batch', 'instance')
+
+
+def _norm_on_kernels(normalization, norm):
+    """A layer's normalization runs on the kernels: None, BatchNorm, or instance norm without
+    running statistics (the reference's nn.InstanceNorm*d default; with running statistics eval
+    mode would normalise by those instead)."""
+    if normalization not in KERNEL_NORMALIZATIONS:
+        return False
+    return normalization != 'instance' or not norm.track_running_stats
 
 
 def _make_act(activation):
@@ -219,8 +238,10 @@ class MyLinear(nn.Module):
                                 self.norm if self.normalization == 'batch' else None, transpose)
 
     def _fast(self, x):
+        # instance norm stays PyTorch: on [B, C] the reference's nn.InstanceNorm1d raises
         return (_fast_ok(self, x) and x.dim() == 2
-                and self.normalization in (None, 'batch') and self.activation in KERNEL_ACTIVATIONS)
+                and self.normalization in KERNEL_NORMALIZATIONS and self.normalization != 'instance'
+                and self.activation in KERNEL_ACTIVATIONS)
 
     def forward(self, x, epoch=None):
         if self._fast(x):
@@ -266,18 +287,39 @@ class _PointwiseConvBase(nn.Module):
         ks = self.conv.kernel_size
         return (all(k == 1 for k in ks) and all(s == 1 for s in self.conv.stride)
                 and all(p == 0 for p in self.conv.padding)
-                and self.normalization in (None, 'batch') and self.activation in KERNEL_ACTIVATIONS)
+                and _norm_on_kernels(self.normalization, getattr(self, "norm", None))
+                and self.activation in KERNEL_ACTIVATIONS)
 
     def _train_kernels(self, x):
         """train() mode on CUDA fp32 with a kernel norm/activation: the sm_90a train kernels
-        (train_ops) instead of the PyTorch composition."""
+        (train_ops) instead of the PyTorch composition. Instance norm also needs its affine
+        parameters (the reference's layers always have them)."""
         return (train_ops.ENABLED and self.training and torch.is_grad_enabled() and x.is_cuda
-                and x.dtype == torch.float32 and self._fast_eligible())
+                and x.dtype == torch.float32 and self._fast_eligible()
+                and (self.normalization != 'instance' or self.norm.affine))
 
-    def forward_points(self, x0, x1=None, addend=None, gidx=None):
+    def _train_norm(self):
+        """The norm module train_ops.conv_bn_act_train applies (None: no normalization)."""
+        return self.norm if self.normalization in ('batch', 'instance') else None
+
+    def instance_norm(self, z, kcopy=None, group_max=None):
+        """This layer's instance norm + activation on its pre-norm output z [B,Cout,P] (in place
+        without a reduction; kcopy / group_max as ops.instance_norm)."""
+        n = self.norm
+        return ops.instance_norm(z, n.weight, n.bias, n.eps, self.activation, kcopy=kcopy,
+                                 group_max=group_max,
+                                 out=z if kcopy is None and group_max is None else None)
+
+    def forward_points(self, x0, x1=None, addend=None, gidx=None, kcopy=None, group_max=None):
         """x0 [B,C0,P] (+ x1 [B,C1,P] virtually concatenated on channels) -> [B,Cout,P].
         Dense layers run on wgmma (csrc/pointwise_tc.cu, fp16 hi/lo split); thin ones on the
-        exact-fp32 CUDA-core kernel (csrc/pointwise.cu)."""
+        exact-fp32 CUDA-core kernel (csrc/pointwise.cu). An instance-norm layer writes the GEMM's
+        z (conv bias, no activation) and normalises it with ops.instance_norm, which can also
+        reduce the result (kcopy / group_max: instance layers only)."""
+        inst = self.normalization == 'instance'
+        if not inst and (kcopy is not None or group_max is not None):
+            raise RuntimeError("forward_points: kcopy / group_max are fused into instance norm only")
+        act = None if inst else self.activation
         cin = x0.shape[1] + (0 if x1 is None else x1.shape[1])
         cout = self.conv.out_channels
         rows = x0.shape[0] * x0.shape[2]
@@ -287,11 +329,12 @@ class _PointwiseConvBase(nn.Module):
         # register-tiled fp32 kernel
         if cin >= 32 and rows >= 256 and tc_enabled():
             blob, inv, shift = self._tc_params()
-            return ops.pointwise_layer_tc(x0, blob, inv, shift, cout, self.activation,
-                                          x1=x1, addend=addend, gidx=gidx, f16=tc_f16())
-        w, shift = self.folded(transpose=True)
-        return ops.pointwise_layer(x0, w, None, shift, self.activation, x1=x1,
-                                   addend=addend, gidx=gidx)
+            z = ops.pointwise_layer_tc(x0, blob, inv, shift, cout, act,
+                                       x1=x1, addend=addend, gidx=gidx, f16=tc_f16())
+        else:
+            w, shift = self.folded(transpose=True)
+            z = ops.pointwise_layer(x0, w, None, shift, act, x1=x1, addend=addend, gidx=gidx)
+        return self.instance_norm(z, kcopy, group_max) if inst else z
 
 
 class MyConv2d(_PointwiseConvBase):
@@ -334,7 +377,7 @@ class MyConv2d(_PointwiseConvBase):
             B, C, H, W = x.shape
             y = train_ops.conv_bn_act_train(
                 x.contiguous().view(B, C, H * W), self._conv_weight2d(), self.conv.bias,
-                self.norm if self.normalization == 'batch' else None, self.activation, epoch)
+                self._train_norm(), self.activation, epoch)
             return y.view(B, y.shape[1], H, W)
         # PyTorch/cuDNN path (3x3 decoder convs, training): strict fp32 in the forward and the
         # backward — cuDNN's default TF32 convolution is ~1e-3 relative, outside the 1e-4 parity
@@ -389,8 +432,8 @@ class UpConv(nn.Module):
         return (_fast_ok(self, x) and x.dim() == 4 and c.kernel_size == (3, 3)
                 and c.stride == (1, 1) and c.padding == (1, 1) and c.dilation == (1, 1)
                 and c.groups == 1 and c.out_channels >= 64 and c.in_channels >= 16
-                and self.normalization in (None, 'batch') and self.activation in KERNEL_ACTIVATIONS
-                and tc_enabled())
+                and _norm_on_kernels(self.normalization, getattr(self.conv, "norm", None))
+                and self.activation in KERNEL_ACTIVATIONS and tc_enabled())
 
     def _packed(self):
         """BN-folded, parity-combined weights as wgmma blobs; re-packed when the fold changes.
@@ -436,7 +479,10 @@ class UpConv(nn.Module):
         f16 = tc_f16()
         B, Cin, H, W = x.shape
         Cout = self.conv.conv.out_channels
-        act = self.activation
+        # instance norm: the parity GEMMs write z (conv bias, no activation), then each [2H x 2W]
+        # map is normalised
+        inst = self.normalization == 'instance'
+        act = None if inst else self.activation
         x = x.contiguous()
         if H == 1 and W == 1:
             kch = (Cin + 63) // 64
@@ -445,6 +491,8 @@ class UpConv(nn.Module):
             y = ops.pointwise_tc_grouped(x.view(B, Cin, 1), pk["blob1"], pk["per1"], pk["inv1"],
                                          pk["shift1"], 4 * Cout, act, groups=1, splits=splits,
                                          scratch=scratch, f16=f16)
+            if inst:     # output channel co*4 + py*2 + px: [B, Cout, 4] rows of the 2x2 maps
+                y = self.conv.instance_norm(y.view(B, Cout, 4))
             return y.view(B, Cout, 2, 2)
         P = H * W
         kch = (4 * Cin + 63) // 64
@@ -457,6 +505,8 @@ class UpConv(nn.Module):
         y = ops.pointwise_tc_grouped(xin, pk["blob4"], pk["per4"], pk["inv4"], pk["shift"], Cout,
                                      act, groups=4, splits=splits, scat_w=W, scratch=scratch,
                                      conv=conv, f16=f16)
+        if inst:
+            y = self.conv.instance_norm(y)                                  # [B, Cout, 4HW]
         return y.view(B, Cout, 2 * H, 2 * W)
 
 
@@ -500,8 +550,8 @@ class EquivariantLayer(_PointwiseConvBase):
             return self.forward_points(x.contiguous())
         if self._train_kernels(x) and x.dim() == 3:
             return train_ops.conv_bn_act_train(
-                x, self._conv_weight2d(), self.conv.bias,
-                self.norm if self.normalization == 'batch' else None, self.activation, epoch)
+                x, self._conv_weight2d(), self.conv.bias, self._train_norm(), self.activation,
+                epoch)
         y = self.conv(x)
         if self.normalization == 'batch':
             y = self.norm(y, epoch)
@@ -542,6 +592,7 @@ class KNNModule(nn.Module):
         return (tc_enabled() and len(ls) == 2
                 and ls[0].conv.in_channels >= 3 + 32
                 and all(l.conv.out_channels == 512 for l in ls)
+                and all(l.normalization in (None, 'batch') for l in ls)   # folds into the GEMMs
                 and ls[0].activation in ('relu', 'elu') and ls[1].activation == ls[0].activation
                 and 2 <= K <= 16 and M * K <= 2304)
 
@@ -591,10 +642,18 @@ class KNNModule(nn.Module):
             return center, self._tc_forward(coord, center, knn_I, K, masked_max), masked_max
         center, h, masked_max = ops.knn_assemble_pool(coord, keys, p0, knn_I, K, center_type,
                                                       owner=owner)
-        for layer in self.layers:
-            h = layer.forward_points(h)
-        feature = ops.rowmax(h.view(B, h.shape[1], M, K))
-        return center, feature, masked_max
+        return center, self._layers_max(h, B, M, K), masked_max
+
+    def _layers_max(self, h, B, M, K):
+        """The 1x1-conv stack on x_aug [B,3+C,M*K] and the max over each node's K neighbours.
+        An instance-norm last layer takes the max inside its normalisation pass."""
+        last = self.layers[-1]
+        for layer in self.layers[:-1]:
+            h = layer.forward_points(h)                     # [B, C', M*K]
+        if last.normalization == 'instance':
+            return last.forward_points(h, group_max=K)
+        h = last.forward_points(h)
+        return ops.rowmax(h.view(B, h.shape[1], M, K))      # max over K
 
     def forward(self, coordinate, x, precomputed_knn_I, K, center_type, epoch=None):
         """coordinate [B,3,M], x [B,C,M], precomputed_knn_I [B,M,K'] -> (center [B,3,M],
@@ -612,10 +671,7 @@ class KNNModule(nn.Module):
                                              want_x_aug=False)
                 return center, self._tc_forward(coord, center, knn_I, K, x.contiguous())
             center, h = ops.knn_assemble(coord, x.contiguous(), knn_I, K, center_type)
-            for layer in self.layers:
-                h = layer.forward_points(h)                     # [B, C', M*K]
-            feature = ops.rowmax(h.view(B, h.shape[1], M, K))   # max over K
-            return center, feature
+            return center, self._layers_max(h, B, M, K)
 
         coordinate_tensor = coordinate.data
         if precomputed_knn_I is not None:

@@ -288,8 +288,13 @@ class Segmenter(nn.Module):
         onehot.scatter_(1, label.unsqueeze(1), 1)
         return onehot
 
-    def _tail(self, layer3_out, k, N):
-        """k-copy average + layer4/5 (models/networks.py:331-341)."""
+    def _tail(self, layer2_out, k, N):
+        """layer3 + k-copy average + layer4/5 (models/networks.py:326-341). An instance-norm
+        layer 3 takes the k-copy mean inside its normalisation pass."""
+        if (self.layer3.normalization == 'instance' and k in (2, 3) and layer2_out.dim() == 3
+                and self.layer3.fast(layer2_out) and self.layer4.fast(layer2_out)):
+            return self._tail_avg(self.layer3.forward_points(layer2_out.contiguous(), kcopy=k))
+        layer3_out = self.layer3(layer2_out)
         fast = self.layer4.fast(layer3_out)
         if fast and k in (2, 3):
             avg = ops.kcopy_mean(layer3_out.contiguous(), k)
@@ -300,6 +305,9 @@ class Segmenter(nn.Module):
                 avg = 0.5 * (parts[0] + parts[1])
             elif k == 3:
                 avg = (1.0 / 3.0) * (parts[0] + parts[1] + parts[2])
+        return self._tail_avg(avg)
+
+    def _tail_avg(self, avg):
         out4 = self.layer4(avg)
         if self.opt.dropout > 0.1:
             out4 = self.drop4(out4)
@@ -323,8 +331,7 @@ class Segmenter(nn.Module):
             parts.append(feature_max_knn_feature_1)
         parts += [feature_max_final_pn_out, feature.unsqueeze(2).expand(B, self.feature_num, kN)]
         layer1_in = torch.cat(parts, dim=1)
-        out = self.layer3(self.layer2(self.layer1(layer1_in)))
-        return self._tail(out, k, self.opt.input_pc_num)
+        return self._tail(self.layer2(self.layer1(layer1_in)), k, self.opt.input_pc_num)
 
     # ---- fast entry: node-level features + assignment, no per-point gathers ----------------
     def _zero_idx(self, B, M, dev):
@@ -388,7 +395,9 @@ class Segmenter(nn.Module):
             node_first.shape[1] + node_knn.shape[1] + node_final.shape[1])
         cloud = torch.cat((self._onehot(label, B, x.device), feature), dim=1)   # [B,1040]
         cloud_add = ops.linear(cloud.contiguous(), w_cloud, None, None, False).unsqueeze(2)  # [B,1024,1]
-        act1 = self.layer1.activation
+        # the split is linear up to the pre-norm z: an instance-norm layer 1 normalises it after
+        inst1 = self.layer1.normalization == 'instance'
+        act1 = None if inst1 else self.layer1.activation
         if tc_enabled():
             f16 = tc_f16()
             bp, ip, bn, pern, inn = tc
@@ -411,8 +420,9 @@ class Segmenter(nn.Module):
             out1 = ops.pointwise_layer(pt, w_point, None, shift, act1,
                                        x1=first_pn_out.contiguous(), addend=addend,
                                        gidx=min_idx_i32)
-        out = self.layer3(self.layer2(out1))
-        return self._tail(out, k, N)
+        if inst1:
+            out1 = self.layer1.instance_norm(out1)
+        return self._tail(self.layer2(out1), k, N)
 
 
 class DecoderLinear(nn.Module):

@@ -319,6 +319,47 @@ def kcopy_mean(t, k):
     return out
 
 
+# reduction codes of sonet_instance_norm_f32 (SONET_REDUCE_*, include/sonet_b200.h)
+REDUCE_NONE, REDUCE_KCOPY_MEAN, REDUCE_GROUP_MAX = 0, 1, 2
+
+
+def instance_norm(z, gamma, beta, eps, act, kcopy=None, group_max=None, save_stats=False, out=None):
+    """Instance norm + activation of z [B,C,P] per row (b, c): act(gamma*(z-mean)*invstd + beta)
+    with the row's biased statistics (nn.InstanceNorm1d/2d, affine, no running statistics).
+    gamma, beta [C] or None (identity); act: activation (act_code). kcopy=k: the mean over the k
+    stacked copies, out [B,C,P/k]; group_max=K: the max over consecutive groups of K, out
+    [B,C,P/K]. out: the output tensor (may be z itself without a reduction). save_stats: also
+    return the row statistics (mean, invstd), each [B,C]."""
+    _chk(z, "z", torch.float32)
+    _chk(gamma, "gamma", torch.float32, optional=True)
+    _chk(beta, "beta", torch.float32, optional=True)
+    if z.dim() != 3:
+        raise RuntimeError("instance_norm: expected z [B,C,P], got %s" % (tuple(z.shape),))
+    if kcopy is not None and group_max is not None:
+        raise RuntimeError("instance_norm: kcopy and group_max exclude each other")
+    B, C, P = z.shape
+    reduce, k = REDUCE_NONE, 1
+    if kcopy is not None:
+        reduce, k = REDUCE_KCOPY_MEAN, int(kcopy)
+    elif group_max is not None:
+        reduce, k = REDUCE_GROUP_MAX, int(group_max)
+    dev = z.device
+    _chk(out, "out", torch.float32, optional=True)
+    if out is not None and out.numel() != B * C * (P // max(k, 1)):
+        raise RuntimeError("instance_norm: out has %d elements, expected %d"
+                           % (out.numel(), B * C * (P // max(k, 1))))
+    with torch.cuda.device(dev):
+        if out is None:
+            out = torch.empty((B, C, P // max(k, 1)), dtype=torch.float32, device=dev)
+        mean = invstd = None
+        if save_stats:
+            mean = torch.empty((B, C), dtype=torch.float32, device=dev)
+            invstd = torch.empty((B, C), dtype=torch.float32, device=dev)
+        _call("sonet_instance_norm_f32", _C.ptr(z), _C.ptr(gamma), _C.ptr(beta), B, C, P, float(eps),
+              act_code(act), reduce, k, _C.ptr(out), _C.ptr(mean), _C.ptr(invstd), _stream(z))
+    return (out, mean, invstd) if save_stats else out
+
+
 def seg_loss(score, target, size_average=True):
     """score [B,C,N] f32, target [B,N] int64 -> scalar loss tensor (mean/sum of the per-point NLL
     of log_softmax over the class axis, models/losses.py:30-43)."""

@@ -8,6 +8,8 @@ models/networks.py:185).
                   power of two before the fp16 hi/lo split)
     BNActTrain    batch-statistics BatchNorm + ReLU / ELU / none, forward and backward, fused elementwise passes
                   and two-stage deterministic reductions
+    InstanceNormActTrain  instance norm + ReLU / ELU / none: the instance-norm kernel forward, the
+                  BN backward on the [1, B*C, P] view
     IndexMaxGather  first_pn_out_masked_max = first_pn_out.gather(2, idx * mask_row_max) with the
                   arg-max kernel in the forward and a deterministic scatter in the backward
 
@@ -15,6 +17,7 @@ ENABLED = False switches every layer back to the PyTorch composition (the tests 
 """
 import torch
 import torch.nn.functional as F
+from torch.nn.modules.instancenorm import _InstanceNorm
 
 from . import _C, ops
 
@@ -65,6 +68,46 @@ class BNActTrain(torch.autograd.Function):
                       _C.ptr(part), _C.ptr(dx), _C.ptr(dgamma), _C.ptr(dbeta), ops._stream(x),
                       kernels=3)
         return dx, dgamma, dbeta, None, None
+
+
+class InstanceNormActTrain(torch.autograd.Function):
+    """Instance norm (affine, no running statistics) + ReLU / ELU / none of z [B,C,P]. Forward:
+    the instance-norm kernel, keeping each row's mean and invstd. Backward: the BN-train backward
+    on the [1, B*C, P] view, whose per-channel statistics are exactly the per-row ones, with gamma
+    and beta expanded to [B*C]; dgamma and dbeta are then summed over the clouds in fp64."""
+
+    @staticmethod
+    def forward(ctx, z, gamma, beta, eps, act):
+        z = z.contiguous()
+        y, mean, invstd = ops.instance_norm(z, gamma.detach(), beta.detach(), eps, act,
+                                            save_stats=True)
+        ctx.save_for_backward(z, mean, invstd, gamma, beta)
+        ctx.act = ops.act_code(act)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        z, mean, invstd, gamma, beta = ctx.saved_tensors
+        dy = dy.contiguous()
+        B, C, P = z.shape
+        dev = z.device
+        # the kernel's grid holds at most 65535 channels: whole clouds per call
+        cb = max(1, 65535 // C)
+        with torch.cuda.device(dev):
+            dz = torch.empty_like(z)
+            g_rows = gamma.detach().repeat(cb).contiguous()
+            b_rows = beta.detach().repeat(cb).contiguous()
+            dgamma = torch.empty((B, C), dtype=torch.float32, device=dev)
+            dbeta = torch.empty((B, C), dtype=torch.float32, device=dev)
+            part = _scratch(dev, _C.lib().sonet_bn_partial_slots(1, cb * C), torch.float64)
+            for b0 in range(0, B, cb):
+                n = min(cb, B - b0)
+                ops._call("sonet_bn_train_backward_f32", _C.ptr(dy[b0:b0 + n]), _C.ptr(z[b0:b0 + n]),
+                          _C.ptr(mean[b0:b0 + n]), _C.ptr(invstd[b0:b0 + n]), _C.ptr(g_rows),
+                          _C.ptr(b_rows), 1, n * C, P, ctx.act, _C.ptr(part), _C.ptr(dz[b0:b0 + n]),
+                          _C.ptr(dgamma[b0:b0 + n]), _C.ptr(dbeta[b0:b0 + n]), ops._stream(z),
+                          kernels=3)
+        return (dz, dgamma.double().sum(0).float(), dbeta.double().sum(0).float(), None, None)
 
 
 def _pack_device(W, transpose):
@@ -244,13 +287,23 @@ def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None):
     """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (wgmma when dense
     enough, else strict-fp32 cuDNN) -> batch-stat BN (+ running-stat update with the reference's
     momentum schedule, models/layers.py:57-65; like F.batch_norm, num_batches_tracked is left
-    alone) -> act: the layer's activation (None, 'relu' or 'elu'; a bool means ReLU or none)."""
+    alone) or instance norm (affine, no running statistics: nothing to update) -> act: the
+    layer's activation (None, 'relu' or 'elu'; a bool means ReLU or none)."""
     B, Cin, P = x3.shape
     Cout = weight2d.shape[0]
+    instance = isinstance(norm, _InstanceNorm)
+    if instance and not (norm.affine and not norm.track_running_stats):
+        raise RuntimeError("conv_bn_act_train: instance norm needs affine=True and "
+                           "track_running_stats=False")
+    if instance and P < 2:   # F.instance_norm's check
+        raise ValueError("Expected more than 1 spatial element when training, got input size "
+                         "{}".format(torch.Size((B, Cout, P))))
     if tc_eligible(Cin, Cout, B * P):
         y0 = ConvTC.apply(x3, weight2d, bias)
     else:
         y0 = ConvStrict.apply(x3, weight2d.unsqueeze(2), bias, [1], [0], [1], 1)
+    if instance:
+        return InstanceNormActTrain.apply(y0, norm.weight, norm.bias, norm.eps, act)
     if norm is None:
         code = ops.act_code(act)
         if code == ops.ACT_ELU:
