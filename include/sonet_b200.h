@@ -233,6 +233,46 @@ int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Cout, int Cin
                        float* dyT, void* blob, float* part, float* small, float* dWT,
                        sonet_stream_t stream);
 
+/* ---- f-2 (decoder): train-mode up-convolution -----------------------------------------------------
+ * UpConv in train() mode (models/layers.py:214-240): nearest x2 up-sampling + 3x3 conv (pad 1) as the
+ * four parity GEMMs of f-1, with weights folded and packed on the device every step, and its
+ * backward. For input x [B,Cin,H,W], output z [B,Cout,2H,2W] and upstream gradient dz:
+ *   forward  z = sonet_pointwise_tc_grouped_forward_dev(Wg, x) + b (conv bias, no activation)
+ *   dgrad    dx[b,ci,i,j] = sum_{g,t,co} Wg[g][co][t*Cin+ci] dz[b,co,2(i-oy)+py,2(j-ox)+px],
+ *            oy = a-1+py, ox = c-1+px: ONE GEMM with K = 16*Cout, the dgrad matrix times the
+ *            operand D of sonet_upconv_dgrad_im2col_f32 (sonet_pointwise_tc_forward_dev)
+ *   wgrad    dWg[g] = sum_{b,p} dz_g xcol_g^T per parity (sonet_wgrad_tc_f32; dz_g = dz[:,:,py::2,
+ *            px::2], xcol_g = group g of sonet_upconv_im2col_f32), then dW by the adjoint fold.
+ * Every entry validates its arguments (SONET_ERR_BAD_ARG before any CUDA call), allocates nothing,
+ * does not synchronise and uses no atomics: two identical calls give identical bits.
+ *   sonet_upconv_fold_weights_f32: adjoint = 0: W [Cout,Cin,3,3] -> out = Wg [4][Cout][4*Cin]
+ *     (Wg[g][co][t*Cin+ci] = sum of the taps that (g, t) collects, rows then columns ascending)
+ *     and/or out_dgrad = the dgrad matrix [Cin][16*Cout], element (ci, (g*4+t)*Cout+co) =
+ *     Wg[g][co][t*Cin+ci] (either may be null, not both). adjoint = 1: in = dWT [4][4*Cin][Cout] (the
+ *     per-parity wgrad results in sonet_wgrad_tc_f32's layout) -> out = dW [Cout,Cin,3,3], each tap
+ *     the sum of its one entry per parity in ascending parity order; out_dgrad must be null.
+ *   sonet_upconv_dgrad_im2col_f32: dz [B,Cout,2H,2W] -> D [B][16*Cout][H*W], row (g*4+t)*Cout+co,
+ *     point i*W+j = dz[b,co,2(i-oy)+py,2(j-ox)+px] (0 outside the map). Row (g, t0 = (1-py)*2 +
+ *     (1-px), co) is the parity plane dz_g.
+ *   sonet_pointwise_tc_pack_groups_device: the device twin of sonet_pointwise_tc_pack_groups (same
+ *     blobs and pre-scale): W [G][Cout][Cin] on the device -> G consecutive blobs, scale2 = (s, 1/s)
+ *     of the one power-of-two pre-scale of all G matrices; scratch: SONET_ABSMAX_SLOTS floats.
+ *   sonet_pointwise_tc_grouped_forward_dev: sonet_pointwise_tc_grouped_forward with its inverse
+ *     pre-scale read from device memory (inv_scale_dev, e.g. scale2 + 1 of the pack above). */
+#define SONET_ABSMAX_SLOTS 256
+int sonet_upconv_fold_weights_f32(const float* in, int Cout, int Cin, int adjoint, float* out,
+                                  float* out_dgrad, sonet_stream_t stream);
+int sonet_upconv_dgrad_im2col_f32(const float* dz, int B, int Cout, int H, int W, float* d,
+                                  sonet_stream_t stream);
+int sonet_pointwise_tc_pack_groups_device(const float* W, int G, int Cout, int Cin, void* blob,
+                                          float* scale2, float* scratch, sonet_stream_t stream);
+int sonet_pointwise_tc_grouped_forward_dev(const float* x, int C, int B, int P, const void* blob,
+                                           long long blob_gstride, const float* inv_scale_dev,
+                                           const float* shift, int Cout, int relu, int groups,
+                                           int splits, int scat_w, int conv_w, int P_out,
+                                           long long out_gstride, float* out, float* scratch,
+                                           sonet_stream_t stream);
+
 /* ---- f-4: batch-SOM training --------------------------------------------------------------------
  * Replaces BatchSOM.batch_update / BatchSOM.optimize (util/som.py:295-366): T iterations of
  * {nearest-node assignment, per-node mean, neighbourhood-weighted node update} per cloud, in ONE

@@ -576,7 +576,7 @@ static int pointwise_tc_grouped(const float* x, int C, int B, int P, const void*
                                 long long blob_gstride, float inv_scale, const float* shift, int Cout,
                                 int relu, int groups, int splits, int scat_w, int conv_w, int P_out,
                                 long long out_gstride, float* out, float* scratch,
-                                sonet_stream_t stream, int nprod) {
+                                sonet_stream_t stream, int nprod, const float* inv_ptr = nullptr) {
   using namespace sonet;
   SONET_REQUIRE(groups >= 1 && splits >= 1 && scat_w >= 0, "pointwise_tc_grouped: bad group/split");
   SONET_REQUIRE(scat_w == 0 || (groups == 4 && P % scat_w == 0 && P_out == 4 * P && out_gstride == 0),
@@ -586,6 +586,7 @@ static int pointwise_tc_grouped(const float* x, int C, int B, int P, const void*
   if (P_out <= 0) P_out = P;
   SONET_REQUIRE(conv_w == 0 || conv_w == scat_w, "pointwise_tc_grouped: conv_w must equal scat_w");
   TcExt e = with_nprod(nprod);
+  e.inv_ptr = inv_ptr;
   e.groups = groups;
   e.splits = splits;
   e.blob_gstride = blob_gstride;
@@ -630,6 +631,22 @@ extern "C" int sonet_pointwise_tc_grouped_forward_f16(const float* x, int C, int
   SONET_REQUIRE_ACT(relu, "pointwise_tc_grouped_forward_f16");
   return pointwise_tc_grouped(x, C, B, P, blob, blob_gstride, inv_scale, shift, Cout, relu, groups,
                               splits, scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 1);
+}
+
+// Train-mode grouped launch (the up-convolution's parity GEMMs): the blobs were packed on the device
+// this step (sonet_pointwise_tc_pack_groups_device) and their common 1/pre-scale is read from device
+// memory; everything else as sonet_pointwise_tc_grouped_forward.
+extern "C" int sonet_pointwise_tc_grouped_forward_dev(const float* x, int C, int B, int P,
+                                                      const void* blob, long long blob_gstride,
+                                                      const float* inv_scale_dev, const float* shift,
+                                                      int Cout, int relu, int groups, int splits,
+                                                      int scat_w, int conv_w, int P_out,
+                                                      long long out_gstride, float* out, float* scratch,
+                                                      sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_grouped_forward_dev");
+  SONET_REQUIRE(inv_scale_dev != nullptr, "pointwise_tc_grouped_forward_dev: null inv_scale pointer");
+  return pointwise_tc_grouped(x, C, B, P, blob, blob_gstride, 1.f, shift, Cout, relu, groups, splits,
+                              scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 3, inv_scale_dev);
 }
 
 // Train-mode variant: the weight blob was packed on the device this step

@@ -413,6 +413,36 @@ static void launch_tc_pack(const float* src, int N, int K, long long sn, long lo
                           st>>>(src, N, K, sn, sk, kp, sb, scale2, static_cast<unsigned char*>(blob), kch);
 }
 
+// absmax without atomics: CTA b writes the max of its grid-stride share to partial[b], then one
+// thread takes the max of the partials in ascending order and forms the scale like
+// scale_from_absmax_kernel (the max of a set is order-free; this keeps the entry graph-capturable
+// without a memset and free of atomics)
+constexpr int ABSMAX_SLOTS = 256;
+__global__ void __launch_bounds__(256)
+    absmax_partial_kernel(const float* __restrict__ w, long long n, float* __restrict__ partial) {
+  float m = 0.f;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    m = fmaxf(m, fabsf(w[i]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  __shared__ float wm[8];
+  if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < 8; ++k) m = fmaxf(m, wm[k]);
+    partial[blockIdx.x] = m;
+  }
+}
+__global__ void scale_from_partials_kernel(const float* __restrict__ partial, int nb,
+                                           float* __restrict__ scale2) {
+  float m = 0.f;
+  for (int b = 0; b < nb; ++b) m = fmaxf(m, partial[b]);
+  const float sc = tc::pow2_scale(m);
+  scale2[0] = sc;
+  scale2[1] = 1.f / sc;
+}
+
 // ---- wgrad helpers ------------------------------------------------------------------------------------
 // Per-channel power-of-two pre-scale of dy [B][C][P]: cscale[c] = s_c with max_{b,p} |s_c dy[b,c,p]|
 // in [256,512) (1 for an all-zero or non-finite channel), cscale[C + c] = 1/s_c. Gradients of one
@@ -593,6 +623,30 @@ extern "C" int sonet_pointwise_tc_pack_device(const float* W, int Cout, int Cin,
   else
     launch_tc_pack(W, Cout, Cin, Cin, 1, Cin, 0, scale2, blob, tc::wblob::kchunks(Cin), st);
   return check_launch("pointwise_tc_pack_device");
+}
+
+// G matrices [G][Cout][Cin] on the device -> G consecutive blobs (sonet_pointwise_tc_blob_bytes each)
+// with ONE power-of-two pre-scale, computed on the device: the same bytes and scale as the host's
+// sonet_pointwise_tc_pack_groups. scratch: SONET_ABSMAX_SLOTS floats.
+extern "C" int sonet_pointwise_tc_pack_groups_device(const float* W, int G, int Cout, int Cin, void* blob,
+                                                     float* scale2, float* scratch,
+                                                     sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE(G >= 1 && Cout >= 1 && Cin >= 1, "pointwise_tc_pack_groups_device: bad dimension "
+                "G=%d Cout=%d Cin=%d", G, Cout, Cin);
+  SONET_REQUIRE(W && blob && scale2 && scratch, "pointwise_tc_pack_groups_device: null pointer");
+  SONET_REQUIRE(aligned16(blob), "pointwise_tc_pack_groups_device: blob must be 16-byte aligned");
+  static_assert(ABSMAX_SLOTS == SONET_ABSMAX_SLOTS, "scratch size of the header");
+  cudaStream_t st = as_stream(stream);
+  const long long per = static_cast<long long>(Cout) * Cin, n = per * G;
+  const int nb = static_cast<int>(std::min<long long>((n + 255) / 256, ABSMAX_SLOTS));
+  absmax_partial_kernel<<<nb, 256, 0, st>>>(W, n, scratch);
+  scale_from_partials_kernel<<<1, 1, 0, st>>>(scratch, nb, scale2);
+  const long long bytes = tc::wblob::bytes(Cout, Cin);
+  for (int g = 0; g < G; ++g)
+    launch_tc_pack(W + g * per, Cout, Cin, Cin, 1, Cin, 0, scale2, static_cast<unsigned char*>(blob) + g * bytes,
+                   tc::wblob::kchunks(Cin), st);
+  return check_launch("pointwise_tc_pack_groups_device");
 }
 
 // power-of-two scale of a device tensor: scale2[0] = s with max|s*t| in [256,512), scale2[1] = 1/s

@@ -52,6 +52,14 @@ _SIGNATURES = {
     "sonet_wgrad_small_floats": [c_int],
     "sonet_wgrad_tc_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                            c_void_p, c_void_p, c_void_p, c_void_p],
+    "sonet_upconv_fold_weights_f32": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "sonet_upconv_dgrad_im2col_f32": [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "sonet_pointwise_tc_pack_groups_device": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                              c_void_p, c_void_p],
+    "sonet_pointwise_tc_grouped_forward_dev": [c_void_p, c_int, c_int, c_int, c_void_p,
+                                               ctypes.c_longlong, c_void_p, c_void_p, c_int, c_int,
+                                               c_int, c_int, c_int, c_int, c_int, ctypes.c_longlong,
+                                               c_void_p, c_void_p, c_void_p],
     "sonet_comm_nccl_version": [],
     "sonet_comm_unique_id": [c_void_p],
     "sonet_comm_init": [c_void_p, c_int, c_int, c_void_p],

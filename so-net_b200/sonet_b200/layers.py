@@ -243,10 +243,21 @@ class MyLinear(nn.Module):
                 and self.normalization in KERNEL_NORMALIZATIONS and self.normalization != 'instance'
                 and self.activation in KERNEL_ACTIVATIONS)
 
+    def _train_kernels(self, x):
+        # instance norm keeps the PyTorch path here too (nn.InstanceNorm1d raises on [B, C])
+        return (train_ops.ENABLED and self.training and torch.is_grad_enabled() and x.is_cuda
+                and x.dtype == torch.float32 and x.dim() == 2
+                and self.normalization in (None, 'batch') and self.activation in KERNEL_ACTIVATIONS)
+
     def forward(self, x, epoch=None):
         if self._fast(x):
             w, shift = self.folded()
             return ops.linear(x.contiguous(), w, None, shift, self.activation)
+        if self._train_kernels(x):
+            y = train_ops.LinearStrict.apply(x, self.linear.weight, self.linear.bias)
+            norm = self.norm if self.normalization == 'batch' else None
+            return train_ops.norm_act_train(y.unsqueeze(2), norm, self.activation, epoch,
+                                            size=y.shape).squeeze(2)
         x = self.linear(x)
         if self.normalization == 'batch':
             x = self.norm(x, epoch)
@@ -392,15 +403,6 @@ class MyConv2d(_PointwiseConvBase):
         return x
 
 
-def _pick_splits(kchunks, base_items, target=120, cap=32):
-    """K split of a grouped wgmma launch: the smallest power of two dividing the number of
-    64-channel K chunks that brings the item count to ~one wave of SMs."""
-    s = 1
-    while s * 2 <= cap and kchunks % (s * 2) == 0 and base_items * s < target:
-        s *= 2
-    return s
-
-
 class UpConv(nn.Module):
     """Nearest x2 upsample + 3x3 conv + BN + act (models/layers.py:214-240), the decoder's
     building block. Eval fast path (SURVEY.md §8f-1): four parity GEMMs over the LOW-resolution
@@ -426,14 +428,28 @@ class UpConv(nn.Module):
         if c.bias is not None:
             nn.init.constant_(c.bias, 0.001)
 
-    # ---- eval fast path --------------------------------------------------------------------------
-    def _fast(self, x):
+    def _kernel_eligible(self, x):
+        """The parity-GEMM kernels apply: a 4-D input, 3x3 / stride 1 / pad 1 / dilation 1, one
+        group, Cin >= 16, Cout >= 64, and a norm and activation the kernels have."""
         c = self.conv.conv
-        return (_fast_ok(self, x) and x.dim() == 4 and c.kernel_size == (3, 3)
+        return (x.dim() == 4 and c.kernel_size == (3, 3)
                 and c.stride == (1, 1) and c.padding == (1, 1) and c.dilation == (1, 1)
                 and c.groups == 1 and c.out_channels >= 64 and c.in_channels >= 16
                 and _norm_on_kernels(self.normalization, getattr(self.conv, "norm", None))
-                and self.activation in KERNEL_ACTIVATIONS and tc_enabled())
+                and self.activation in KERNEL_ACTIVATIONS)
+
+    # ---- eval fast path --------------------------------------------------------------------------
+    def _fast(self, x):
+        return _fast_ok(self, x) and self._kernel_eligible(x) and tc_enabled()
+
+    def _train_kernels(self, x):
+        """train() mode on CUDA fp32, input maps of at least train_ops.UPCONV_MIN_HW pixels: the
+        parity GEMMs' forward, dgrad and wgrad (train_ops.upconv_train), then the shared norm /
+        activation kernels. SONET_TC is ignored."""
+        return (train_ops.ENABLED and self.training and torch.is_grad_enabled() and x.is_cuda
+                and x.dtype == torch.float32 and self._kernel_eligible(x)
+                and x.shape[2] * x.shape[3] >= train_ops.UPCONV_MIN_HW
+                and (self.normalization != 'instance' or self.conv.norm.affine))
 
     def _packed(self):
         """BN-folded, parity-combined weights as wgmma blobs; re-packed when the fold changes.
@@ -474,6 +490,13 @@ class UpConv(nn.Module):
 
     def forward(self, x):
         if not self._fast(x):
+            if self._train_kernels(x):
+                c = self.conv.conv
+                z = train_ops.upconv_train(x, c.weight, c.bias)           # [B, Cout, 2H, 2W]
+                B, Cout, H2, W2 = z.shape
+                y = train_ops.norm_act_train(z.view(B, Cout, H2 * W2), self.conv._train_norm(),
+                                             self.activation)
+                return y.view(B, Cout, H2, W2)
             return self.conv(self.up_sample(x))
         pk = self._packed()
         f16 = tc_f16()
@@ -486,7 +509,7 @@ class UpConv(nn.Module):
         x = x.contiguous()
         if H == 1 and W == 1:
             kch = (Cin + 63) // 64
-            splits = _pick_splits(kch, ((B + 127) // 128) * ((4 * Cout + 255) // 256))
+            splits = ops.pick_splits(kch, ((B + 127) // 128) * ((4 * Cout + 255) // 256))
             scratch = self._scratch_for(splits * B * 4 * Cout, x.device) if splits > 1 else None
             y = ops.pointwise_tc_grouped(x.view(B, Cin, 1), pk["blob1"], pk["per1"], pk["inv1"],
                                          pk["shift1"], 4 * Cout, act, groups=1, splits=splits,
@@ -496,11 +519,11 @@ class UpConv(nn.Module):
             return y.view(B, Cout, 2, 2)
         P = H * W
         kch = (4 * Cin + 63) // 64
-        splits = _pick_splits(kch, 4 * ((B * P + 127) // 128) * ((Cout + 255) // 256))
+        splits = ops.pick_splits(kch, 4 * ((B * P + 127) // 128) * ((Cout + 255) // 256))
         scratch = self._scratch_for(4 * splits * B * Cout * P, x.device) if splits > 1 else None
         # H*W % 64 == 0 and Cin % 64 == 0: no im2col — three horizontally shifted copies, the
         # vertical shifts are point-coordinate offsets inside the GEMM (3x the input instead of 16x)
-        conv = P % 64 == 0 and Cin % 64 == 0 and os.environ.get("SONET_UPCONV_IM2COL", "0") != "1"
+        conv = ops.upconv_conv_mode(Cin, H, W)
         xin = ops.upconv_hshift(x) if conv else ops.upconv_im2col(x)      # [3B,Cin,HW] | [4B,4Cin,HW]
         y = ops.pointwise_tc_grouped(xin, pk["blob4"], pk["per4"], pk["inv4"], pk["shift"], Cout,
                                      act, groups=4, splits=splits, scat_w=W, scratch=scratch,

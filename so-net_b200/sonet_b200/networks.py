@@ -18,7 +18,7 @@ import torch.nn as nn
 
 from . import ops, som, train_ops
 from .layers import (EquivariantLayer, KNNModule, MyConv2d, MyLinear, PointNet, PointResNet,
-                     UpConv, _Cache, _fast_ok, _pick_splits, tc_enabled, tc_f16)
+                     UpConv, _Cache, _fast_ok, tc_enabled, tc_f16)
 
 
 def _bn_kwargs(opt):
@@ -406,7 +406,7 @@ class Segmenter(nn.Module):
             # CTAs that each walk all 30 K chunks; the K split brings it to one wave
             node_in = torch.cat((node_first, node_knn, node_final), dim=1).contiguous()
             kch = (node_in.shape[1] + 63) // 64
-            splits = _pick_splits(kch, ((B * M + 127) // 128) * ((cout + 255) // 256))
+            splits = ops.pick_splits(kch, ((B * M + 127) // 128) * ((cout + 255) // 256))
             addend = ops.pointwise_tc_grouped(node_in, bn, pern, inn, None, cout, False, groups=1,
                                               splits=splits, f16=f16) + cloud_add   # [B,1024,M]
             out1 = ops.pointwise_layer_tc(pt, bp, ip, shift, cout, act1,

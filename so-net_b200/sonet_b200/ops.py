@@ -6,6 +6,7 @@ same checks the reference plugin does with CHECK_INPUT (models/index_max_ext/ind
 raised as RuntimeError. Nothing here falls back to PyTorch or the CPU.
 """
 import ctypes
+import os
 
 import torch
 
@@ -633,6 +634,12 @@ def upconv_im2col(x):
     return xcol
 
 
+def upconv_conv_mode(Cin, H, W):
+    """The parity GEMMs of an up-convolution read the three horizontal shifts (upconv_hshift)
+    instead of the 16x im2col: H*W % 64 == 0 and Cin % 64 == 0, unless SONET_UPCONV_IM2COL=1."""
+    return (H * W) % 64 == 0 and Cin % 64 == 0 and os.environ.get("SONET_UPCONV_IM2COL", "0") != "1"
+
+
 def upconv_hshift(x):
     """x [B,Cin,H,W] -> [3*B, Cin, H*W]: the input shifted horizontally by -1, 0, +1 (zeros at the
     row ends) — the operand of the im2col-free up-convolution (csrc/upconv.cu)."""
@@ -642,6 +649,15 @@ def upconv_hshift(x):
         out = torch.empty((3 * B, Cin, H * W), dtype=torch.float32, device=x.device)
         _call("sonet_upconv_hshift_f32", _C.ptr(x), B, Cin, H, W, _C.ptr(out), _stream(x))
     return out
+
+
+def pick_splits(kchunks, base_items, target=120, cap=32):
+    """K split of a wgmma launch: the smallest power of two dividing the number of 64-channel
+    K chunks that brings the item count to ~one wave of SMs."""
+    s = 1
+    while s * 2 <= cap and kchunks % (s * 2) == 0 and base_items * s < target:
+        s *= 2
+    return s
 
 
 def pointwise_tc_grouped(x, blob, per_bytes, inv_scale, shift, cout, act, groups, splits=1,

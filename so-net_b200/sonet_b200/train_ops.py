@@ -10,11 +10,18 @@ models/networks.py:185).
                   and two-stage deterministic reductions
     InstanceNormActTrain  instance norm + ReLU / ELU / none: the instance-norm kernel forward, the
                   BN backward on the [1, B*C, P] view
+    UpConvTC      nearest x2 up-sampling + 3x3 conv (pad 1) as four parity GEMMs over the
+                  low-resolution map (csrc/upconv.cu): forward, dgrad (one GEMM with K = 16*Cout over
+                  the gathered gradient D) and wgrad (one GEMM per parity) on the wgmma layer kernel
+    LinearStrict  x W^T + b on cuBLAS with TF32 off in the forward and the backward (MyLinear)
     IndexMaxGather  first_pn_out_masked_max = first_pn_out.gather(2, idx * mask_row_max) with the
                   arg-max kernel in the forward and a deterministic scatter in the backward
 
-ENABLED = False switches every layer back to the PyTorch composition (the tests compare the two).
+norm_act_train is the norm / activation half every train-mode layer shares. ENABLED = False
+switches every layer back to the PyTorch composition (the tests compare the two).
 """
+import contextlib
+
 import torch
 import torch.nn.functional as F
 from torch.nn.modules.instancenorm import _InstanceNorm
@@ -206,12 +213,8 @@ class ConvTC(torch.autograd.Function):
             if W.shape[0] % 64 == 0 and W.shape[1] >= 16 and WGRAD_TC:
                 dW = wgrad_tc(dy, x)
             else:                                                    # thin layers: cuBLAS fp32
-                prev = torch.backends.cuda.matmul.allow_tf32
-                torch.backends.cuda.matmul.allow_tf32 = False
-                try:
+                with _cublas_strict_fp32():
                     dW = torch.einsum("bop,bip->oi", dy, x)
-                finally:
-                    torch.backends.cuda.matmul.allow_tf32 = prev
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = dy.sum(dim=(0, 2))
         return dx, dW, db
@@ -283,25 +286,60 @@ def conv_strict(conv, x):
                             list(conv.dilation), conv.groups)
 
 
-def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None):
-    """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (wgmma when dense
-    enough, else strict-fp32 cuDNN) -> batch-stat BN (+ running-stat update with the reference's
-    momentum schedule, models/layers.py:57-65; like F.batch_norm, num_batches_tracked is left
-    alone) or instance norm (affine, no running statistics: nothing to update) -> act: the
-    layer's activation (None, 'relu' or 'elu'; a bool means ReLU or none)."""
-    B, Cin, P = x3.shape
-    Cout = weight2d.shape[0]
+@contextlib.contextmanager
+def _cublas_strict_fp32():
+    """cuBLAS fp32 GEMMs without TF32 for the duration, whatever the global flag says."""
+    prev = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        yield
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev
+
+
+class LinearStrict(torch.autograd.Function):
+    """x [B,Cin] W^T + b on cuBLAS with TF32 off in the forward AND the backward (the global flag
+    is read when backward() runs, outside any context the forward was called in)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        with _cublas_strict_fp32():
+            y = torch.addmm(bias, x, weight.t()) if bias is not None else x @ weight.t()
+        ctx.save_for_backward(x, weight)
+        ctx.has_bias = bias is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        dx = dW = db = None
+        with _cublas_strict_fp32():
+            if need[0]:
+                dx = dy @ weight
+            if need[1]:
+                dW = dy.t() @ x
+        if ctx.has_bias and need[2]:
+            db = dy.sum(0)
+        return dx, dW, db
+
+
+def norm_act_train(y0, norm, act, epoch=None, size=None):
+    """The norm / activation half of every train-mode layer on its pre-norm output y0 [B,C,P]:
+    batch-stat BN (+ running-stat update with the reference's momentum schedule,
+    models/layers.py:57-65; like F.batch_norm, num_batches_tracked is left alone) or instance norm
+    (affine, no running statistics: nothing to update) or none -> act: the layer's activation
+    (None, 'relu' or 'elu'; a bool means ReLU or none). size: the layer output's shape as the
+    reference sees it, for the messages of F.batch_norm's and F.instance_norm's ValueErrors."""
+    B, C, P = y0.shape
+    size = y0.size() if size is None else torch.Size(size)
     instance = isinstance(norm, _InstanceNorm)
     if instance and not (norm.affine and not norm.track_running_stats):
-        raise RuntimeError("conv_bn_act_train: instance norm needs affine=True and "
+        raise RuntimeError("norm_act_train: instance norm needs affine=True and "
                            "track_running_stats=False")
     if instance and P < 2:   # F.instance_norm's check
         raise ValueError("Expected more than 1 spatial element when training, got input size "
-                         "{}".format(torch.Size((B, Cout, P))))
-    if tc_eligible(Cin, Cout, B * P):
-        y0 = ConvTC.apply(x3, weight2d, bias)
-    else:
-        y0 = ConvStrict.apply(x3, weight2d.unsqueeze(2), bias, [1], [0], [1], 1)
+                         "{}".format(size))
     if instance:
         return InstanceNormActTrain.apply(y0, norm.weight, norm.bias, norm.eps, act)
     if norm is None:
@@ -311,7 +349,7 @@ def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None):
         return torch.relu(y0) if code == ops.ACT_RELU else y0
     if B * P == 1:     # F.batch_norm's check: a batch statistic of one value is undefined
         raise ValueError("Expected more than 1 value per channel when training, got input size "
-                         "{}".format(y0.size()))
+                         "{}".format(size))
     step = norm.momentum_decay_step
     if epoch is not None and epoch >= 1 and step is not None and step > 0:
         norm.momentum = max(norm.momentum_original * (norm.momentum_decay ** (epoch // step)), 0.01)
@@ -322,3 +360,161 @@ def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None):
         norm.running_mean.mul_(1 - m).add_(mean, alpha=m)
         norm.running_var.mul_(1 - m).add_(var * (n / (n - 1)), alpha=m)
     return y
+
+
+def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None):
+    """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (wgmma when dense
+    enough, else strict-fp32 cuDNN) -> norm_act_train."""
+    B, Cin, P = x3.shape
+    Cout = weight2d.shape[0]
+    if tc_eligible(Cin, Cout, B * P):
+        y0 = ConvTC.apply(x3, weight2d, bias)
+    else:
+        y0 = ConvStrict.apply(x3, weight2d.unsqueeze(2), bias, [1], [0], [1], 1)
+    return norm_act_train(y0, norm, act, epoch)
+
+
+# ---- the up-convolution (csrc/upconv.cu) -----------------------------------------------------------
+def _fold(src, Cout, Cin, adjoint, out, out_dgrad=None):
+    ops._call("sonet_upconv_fold_weights_f32", _C.ptr(src), Cout, Cin, int(adjoint), _C.ptr(out),
+              _C.ptr(out_dgrad), ops._stream(src), kernels=(out is not None) + (out_dgrad is not None))
+
+
+def _pack_groups_device(Wg):
+    """Wg [G,Cout,Cin] (device) -> (G consecutive blobs, scale2) with one common pre-scale."""
+    G, Cout, Cin = Wg.shape
+    dev = Wg.device
+    per = int(_C.lib().sonet_pointwise_tc_blob_bytes(Cout, Cin))
+    with torch.cuda.device(dev):
+        blob = torch.empty(per * G, dtype=torch.uint8, device=dev)
+        scale2 = torch.empty(2, dtype=torch.float32, device=dev)
+        part = torch.empty(256, dtype=torch.float32, device=dev)     # SONET_ABSMAX_SLOTS
+        ops._call("sonet_pointwise_tc_pack_groups_device", _C.ptr(Wg), G, Cout, Cin, _C.ptr(blob),
+                  _C.ptr(scale2), _C.ptr(part), ops._stream(Wg), kernels=2 + G)
+    return blob, per, scale2
+
+
+# Longest K extent, in 64-channel chunks, that one wgmma accumulator of the up-convolution's forward
+# and dgrad GEMMs sums before the fixed-order fp32 split-K reduce takes over. The tensor cores' fp32
+# accumulation loses precision with the length of one accumulation chain: the row error of deconv6's
+# dx from fp64 grew about linearly with it (one H100 80GB HBM3, 700 W, B = 16: 1.1e-5 at 32 chunks,
+# 1.5e-6 at 4; cuDNN strict fp32 4.6e-7). The extra split costs deconv6's forward + backward at
+# B = 32 3.31 ms instead of 2.98.
+UPCONV_MAX_KPI = 4
+
+
+def _upconv_splits(kchunks, base_items):
+    """K split of an up-convolution GEMM: ops.pick_splits' choice, raised to the smallest divisor of
+    kchunks that keeps every accumulator within UPCONV_MAX_KPI chunks."""
+    s = ops.pick_splits(kchunks, base_items)
+    if kchunks // s <= UPCONV_MAX_KPI:
+        return s
+    return min(d for d in range(s, kchunks + 1) if kchunks % d == 0 and kchunks // d <= UPCONV_MAX_KPI)
+
+
+class UpConvTC(torch.autograd.Function):
+    """x [B,Cin,H,W] (H*W > 1), W [Cout,Cin,3,3], b [Cout] -> z = conv3x3(upsample2(x)) + b
+    [B,Cout,2H,2W] as four parity GEMMs (Wg = the taps that coincide after up-sampling, summed).
+      forward  z = grouped parity GEMMs (Wg, x) + b, Wg folded and packed on the device
+      dgrad    dx = Wd D: D [B][16*Cout][H*W] = dz gathered at each (parity, tap, co)'s offset
+      wgrad    dWg[g] = dz_g xcol_g^T per parity (xcol recomputed from x), dW = adjoint fold"""
+
+    @staticmethod
+    def forward(ctx, x, W, b):
+        x = x.contiguous()
+        Wc = W.contiguous()
+        B, Cin, H, Wd = x.shape
+        Cout = Wc.shape[0]
+        P = H * Wd
+        dev = x.device
+        with torch.cuda.device(dev):
+            Wg = torch.empty((4, Cout, 4 * Cin), dtype=torch.float32, device=dev)
+            _fold(Wc, Cout, Cin, False, Wg)
+            blob, per, scale2 = _pack_groups_device(Wg)
+            conv = ops.upconv_conv_mode(Cin, H, Wd)
+            xin = ops.upconv_hshift(x) if conv else ops.upconv_im2col(x)
+            splits = _upconv_splits((4 * Cin + 63) // 64, 4 * ((B * P + 127) // 128) * ((Cout + 255) // 256))
+            z = torch.empty((B, Cout, 4 * P), dtype=torch.float32, device=dev)
+            scratch = (torch.empty(4 * splits * B * Cout * P, dtype=torch.float32, device=dev)
+                       if splits > 1 else None)
+            ops._call("sonet_pointwise_tc_grouped_forward_dev", _C.ptr(xin), xin.shape[1], B, P,
+                      _C.ptr(blob),
+                      per, _C.ptr(scale2[1:]), _C.ptr(None if b is None else b.contiguous()), Cout,
+                      ops.ACT_NONE, 4, splits, Wd, Wd if conv else 0, 4 * P, 0, _C.ptr(z),
+                      _C.ptr(scratch), ops._stream(x), kernels=2 if splits > 1 else 1)
+        ctx.save_for_backward(x, Wc)
+        ctx.has_bias = b is not None
+        return z.view(B, Cout, 2 * H, 2 * Wd)
+
+    @staticmethod
+    def backward(ctx, dz):
+        x, W = ctx.saved_tensors
+        dz = dz.contiguous()
+        B, Cin, H, Wd = x.shape
+        Cout = W.shape[0]
+        P = H * Wd
+        dev = x.device
+        dx = dW = db = None
+        with torch.cuda.device(dev):
+            if ctx.needs_input_grad[0]:
+                Wdg = torch.empty((Cin, 16 * Cout), dtype=torch.float32, device=dev)
+                _fold(W, Cout, Cin, False, None, Wdg)
+                blob, scale2 = _pack_device(Wdg, False)
+                D = torch.empty((B, 16 * Cout, P), dtype=torch.float32, device=dev)
+                ops._call("sonet_upconv_dgrad_im2col_f32", _C.ptr(dz), B, Cout, H, Wd, _C.ptr(D),
+                          ops._stream(dz))
+                s_dz = _absmax_scale(dz)            # max|D| = max|dz|: D holds every dz element
+                splits = _upconv_splits((16 * Cout + 63) // 64,
+                                        ((B * P + 127) // 128) * (((Cin + 63) // 64 * 64 + 127) // 128))
+                dx = torch.empty((B, Cin, P), dtype=torch.float32, device=dev)
+                scratch = (torch.empty(splits * B * Cin * P, dtype=torch.float32, device=dev)
+                           if splits > 1 else None)
+                ops._call("sonet_pointwise_tc_forward_dev", _C.ptr(D), 16 * Cout, B, P, _C.ptr(blob),
+                          _C.ptr(scale2[1:] * s_dz[1:]), _C.ptr(s_dz[:1]), None, Cin, 0, splits,
+                          _C.ptr(dx), _C.ptr(scratch), ops._stream(dz),
+                          kernels=2 if splits > 1 else 1)
+                dx = dx.view(B, Cin, H, Wd)
+            if ctx.needs_input_grad[1]:
+                # the four parity planes of dz, copied once: [4][B][Cout][H*W]
+                dzg = dz.view(B, Cout, H, 2, Wd, 2).permute(3, 5, 0, 1, 2, 4).reshape(4, B, Cout, P)
+                xcol = ops.upconv_im2col(x).view(4, B, 4 * Cin, P)
+                if Cout % 64 == 0 and WGRAD_TC:
+                    dWT = torch.stack([wgrad_tc(dzg[g], xcol[g]).t() for g in range(4)])
+                else:
+                    with _cublas_strict_fp32():
+                        dWT = torch.einsum("gbkp,gbop->gko", xcol, dzg)
+                dW = torch.empty_like(W)
+                _fold(dWT.contiguous(), Cout, Cin, True, dW)
+            if ctx.has_bias and ctx.needs_input_grad[2]:
+                db = dz.sum(dim=(0, 2, 3))
+        return dx, dW, db
+
+
+# Smallest input map (H*W) whose train-mode up-convolution runs on the parity GEMMs; smaller maps
+# keep the strict-fp32 cuDNN composition. Measured with tools/ae_train_bench.py on one H100 80GB HBM3
+# (700 W power limit), B = 32, forward + backward of each DecoderConv stage: kernels vs cuDNN
+# 1.33/1.12 ms (1x1 input), 1.67/0.79 (2x2), 1.47/0.74 (4x4), 1.29/0.70 (8x8), 1.57/1.44 and
+# 1.45/1.58 in two runs (16x16), 3.31/8.00 (32x32): below 32x32 the fixed cost of the per-step fold,
+# packs and four wgrad calls (tools/ae_train_bench.py breaks it down) outweighs the GEMMs.
+UPCONV_MIN_HW = 1024
+
+
+def upconv_train(x, weight, bias):
+    """Train-mode nearest x2 up-sampling + 3x3 conv (pad 1) of x [B,Cin,H,W] -> [B,Cout,2H,2W],
+    before the norm. A 1x1 input is the dense layer Cin -> 4*Cout whose weight holds, per output
+    parity, the sum of the taps that land on the single pixel (rows / columns {1,2} for parity 0,
+    {0,1} for parity 1); larger maps run UpConvTC."""
+    B, Cin, H, Wd = x.shape
+    Cout = weight.shape[0]
+    if H * Wd > 1:
+        return UpConvTC.apply(x, weight, bias)
+    taps = ((1, 2), (0, 1))
+    W1 = torch.stack([weight[:, :, taps[py][0]:taps[py][1] + 1, taps[px][0]:taps[px][1] + 1].sum((2, 3))
+                      for py in range(2) for px in range(2)], dim=1).reshape(4 * Cout, Cin)
+    b1 = None if bias is None else bias.repeat_interleave(4)
+    x3 = x.reshape(B, Cin, 1)
+    if tc_eligible(Cin, 4 * Cout, B):
+        y0 = ConvTC.apply(x3, W1, b1)
+    else:
+        y0 = ConvStrict.apply(x3, W1.unsqueeze(2), b1, [1], [0], [1], 1)
+    return y0.view(B, Cout, 2, 2)      # output channel co*4 + py*2 + px
