@@ -436,6 +436,9 @@ long long sonet_retrieval_format_cpu(const long long* ids, const long long* idx,
  *     (forward_loss_element / backward_loss_element, losses.py:281, 286)
  *   loss_fwd_arr, loss_bwd_arr [B] f32: per-cloud means of the above
  *   loss [3] f32: {forward_loss, backward_loss, forward_loss + backward_loss} (means over B).
+ * A point with no finite nearest neighbour (its minimum squared distance over non-NaN candidates
+ * is +inf, or it has no non-NaN candidate) gets index 0 and the element of the pair (point, other
+ * cloud's point 0): NaN if either has a NaN, +inf on overflow. Indices are always in range.
  * All reductions run in a fixed order (bit-reproducible). */
 int sonet_chamfer_f32(const float* pred, const float* gt, int B, int Mp, int N, int32_t* idx_fwd,
                       int32_t* idx_bwd, float* elem_fwd, float* elem_bwd, float* loss_fwd_arr,

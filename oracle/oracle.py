@@ -337,27 +337,54 @@ def segmenter_forward(st, opt, enc, x, sn, label):
 # ---- Chamfer -------------------------------------------------------------------------------------------
 def nn_search(query, db):
     """faiss.IndexFlatL2 k=1 (models/losses.py:209-235) as exact brute force.
-    query [3,Q], db [3,D] -> idx [Q] int32."""
+    query [3,Q], db [3,D] -> (idx [Q] int32, dist2 [Q] float32).
+
+    dist2 is the fp32 squared distance of the selected pair, ((dx*dx + dy*dy) + dz*dz) with every
+    op rounded separately: the scan's minimum, or, for a query no candidate beats +inf for (index
+    0, every distance NaN or +inf), the distance to db point 0 (NaN or +inf)."""
     query = query.contiguous().float()
     db = db.contiguous().float()
     Q, D = query.shape[1], db.shape[1]
     idx = torch.zeros(Q, dtype=torch.int32)
-    clib().oracle_nn_search(_p(query), Q, _p(db), D, _p(idx), None)
-    return idx
+    dist2 = torch.zeros(Q, dtype=torch.float32)
+    clib().oracle_nn_search(_p(query), Q, _p(db), D, _p(idx), _p(dist2))
+    none = torch.isinf(dist2)
+    if bool(none.any()):
+        dist2[none] = pair_dist2(query[:, none], db[:, :1].expand(3, int(none.sum())))
+    return idx, dist2
+
+
+def pair_dist2(a, b):
+    """fp32 ((dx*dx + dy*dy) + dz*dz) of a [3,P] and b [3,P] point by point, every op rounded
+    separately (numpy float32 ops are correctly rounded and never contracted)."""
+    with np.errstate(all="ignore"):     # NaN and overflow are part of what is checked
+        d = a.numpy().astype(np.float32) - b.numpy().astype(np.float32)
+        return torch.from_numpy((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2])
+
+
+def chamfer_elem(dist2):
+    """The kernel's per-point term sqrt(dist2 + 1e-8) in fp32, each op correctly rounded."""
+    d = dist2.numpy().astype(np.float32)
+    with np.errstate(all="ignore"):
+        return torch.from_numpy(np.sqrt(d + np.float32(1e-8)))
 
 
 def chamfer(predict_pc, gt_pc):
     """ChamferLoss.forward, models/losses.py:237-290. -> dict(loss, forward_loss, backward_loss,
-    forward_loss_array, backward_loss_array, loss_array, idx_fwd, idx_bwd)."""
+    forward_loss_array, backward_loss_array, loss_array, idx_fwd, idx_bwd, dist2_fwd, dist2_bwd);
+    dist2_* [B,P] are nn_search's fp32 squared distances of the selected pairs."""
     B = predict_pc.shape[0]
-    sel_gt, sel_pr, i_f, i_b = [], [], [], []
+    sel_gt, sel_pr, i_f, i_b, d_f, d_b = [], [], [], [], [], []
     for i in range(B):                                                      # losses.py:260-276
-        fi = nn_search(predict_pc[i], gt_pc[i]).long()
-        bi = nn_search(gt_pc[i], predict_pc[i]).long()
+        fi, df = nn_search(predict_pc[i], gt_pc[i])
+        bi, db = nn_search(gt_pc[i], predict_pc[i])
+        fi, bi = fi.long(), bi.long()
         sel_gt.append(gt_pc[i].index_select(1, fi))
         sel_pr.append(predict_pc[i].index_select(1, bi))
         i_f.append(fi)
         i_b.append(bi)
+        d_f.append(df)
+        d_b.append(db)
     sel_gt = torch.stack(sel_gt).unsqueeze(1)                               # B,1,3,M
     sel_pr = torch.stack(sel_pr).unsqueeze(1)
     rn = lambda v: ((v ** 2).sum(dim=2) + 1e-8).sqrt()                      # noqa: E731  :17-27
@@ -366,7 +393,8 @@ def chamfer(predict_pc, gt_pc):
     fa, ba = f_el.mean(dim=1).mean(dim=1), b_el.mean(dim=1).mean(dim=1)
     return dict(loss=f_el.mean() + b_el.mean(), forward_loss=f_el.mean(),
                 backward_loss=b_el.mean(), forward_loss_array=fa, backward_loss_array=ba,
-                loss_array=fa + ba, idx_fwd=torch.stack(i_f), idx_bwd=torch.stack(i_b))
+                loss_array=fa + ba, idx_fwd=torch.stack(i_f), idx_bwd=torch.stack(i_b),
+                dist2_fwd=torch.stack(d_f), dist2_bwd=torch.stack(d_b))
 
 
 def split_state(state, prefix):

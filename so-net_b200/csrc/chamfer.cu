@@ -23,6 +23,15 @@
 //   chamfer_cloud/final   sqrt(d + 1e-8) in place, fixed-order tree sums -> per-cloud means and the
 //       three scalar losses (deterministic, independent of batch sharding).
 // Bound: FP32 ALU / issue (arithmetic intensity >> 100 flop/B): 8 FP + 2 FMNMX + ~0.4 per pair.
+//
+// Points with no finite nearest neighbour follow the oracle's scan, which starts from (+inf,
+// index 0) and only moves on a strictly smaller distance: a point whose minimum squared distance
+// over its non-NaN candidates is +inf (every candidate overflows), or that has no non-NaN
+// candidate (a NaN coordinate in the point, or in every point of the other cloud), gets index 0
+// and the element sqrt(d(point, other cloud's point 0) + 1e-8) in the usual arithmetic — NaN if
+// either point has a NaN, +inf on overflow. fminf drops NaN, so these are exactly the points
+// whose key is +inf after the value pass; chamfer_cloud_kernel rewrites them. The tile padding
+// is NaN: a padded row or column is never anyone's minimum and never matches in the arg-min pass.
 #include <algorithm>
 
 #include "common.cuh"
@@ -33,7 +42,8 @@ constexpr int CH_WARPS = 4;            // warps per CTA, each with its own 256-c
 constexpr int CH_RN = 8;               // gt points per lane
 constexpr int CH_COLS = 32 * CH_RN;    // 256 columns per warp
 constexpr int CH_TM = 128;             // pred points per CTA tile (256: 5.4 CTAs per SM, 80 us; see r02 summary)
-constexpr float CH_FAR = 1.0e30f;      // padding coordinate: (x - 1e30)^2 overflows to +inf
+constexpr unsigned CH_PAD = 0x7fffffffu;  // padding coordinate (NaN bits): ignored by fminf, == nothing
+constexpr unsigned CH_INF = 0x7f800000u;  // +inf bits: the key of a point with no finite neighbour
 
 // row_key [B,Mp] / col_key [B,N]: running minima as float bit patterns (init 0xFFFFFFFF).
 // IDX pass: row_key/col_key hold the FINAL minima; row_idx/col_idx (init INT_MAX-like) receive the
@@ -56,8 +66,9 @@ __global__ void __launch_bounds__(CH_WARPS * 32)
   const int rows = min(CH_TM, Mp - m0);
   for (int i = threadIdx.x; i < CH_TM; i += CH_WARPS * 32) {
     const int m = m0 + i;
-    const float rx = (m < Mp) ? pb[m] : CH_FAR, ry = (m < Mp) ? pb[Mp + m] : CH_FAR,
-                rz = (m < Mp) ? pb[2 * Mp + m] : CH_FAR;
+    const float pad = __uint_as_float(CH_PAD);
+    const float rx = (m < Mp) ? pb[m] : pad, ry = (m < Mp) ? pb[Mp + m] : pad,
+                rz = (m < Mp) ? pb[2 * Mp + m] : pad;
     srow[i][0] = make_float2(rx, rx);
     srow[i][1] = make_float2(ry, ry);
     srow[i][2] = make_float2(rz, rz);
@@ -77,8 +88,8 @@ __global__ void __launch_bounds__(CH_WARPS * 32)
   for (int j = 0; j < CH_RN; ++j) {
     const int n = n0 + j * 32 + lane;
     const bool ok = n < N;
-    const float vx = ok ? -gb[n] : CH_FAR, vy = ok ? -gb[N + n] : CH_FAR,
-                vz = ok ? -gb[2 * N + n] : CH_FAR;
+    const float pad = __uint_as_float(CH_PAD);
+    const float vx = ok ? -gb[n] : pad, vy = ok ? -gb[N + n] : pad, vz = ok ? -gb[2 * N + n] : pad;
     if (j & 1) {
       ngx[j >> 1].y = vx; ngy[j >> 1].y = vy; ngz[j >> 1].y = vz;
     } else {
@@ -180,19 +191,34 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 
 // grid = (B, 2): keys (min squared distances) of one direction of one cloud -> sqrt(d + 1e-8) in
 // place and their mean. 1024 threads, fixed order: thread-strided partial sums, xor-shuffle tree
-// inside each warp, then a fixed 32-term tree over the warps.
+// inside each warp, then a fixed 32-term tree over the warps. A key of +inf (no finite nearest
+// neighbour, see the header) becomes the distance to the other cloud's point 0, and its index 0
+// when indices are asked for: (p - g)^2 == (g - p)^2, so both directions compute pred - gt.
 constexpr int CC_THREADS = 1024;
 __global__ void __launch_bounds__(CC_THREADS)
-    chamfer_cloud_kernel(float* __restrict__ elem_fwd, int Mp, float* __restrict__ elem_bwd, int N,
+    chamfer_cloud_kernel(const float* __restrict__ pred, const float* __restrict__ gt,
+                         float* __restrict__ elem_fwd, int Mp, float* __restrict__ elem_bwd, int N,
+                         int* __restrict__ idx_fwd, int* __restrict__ idx_bwd,
                          float* __restrict__ fwd_arr, float* __restrict__ bwd_arr) {
   __shared__ float wsum[CC_THREADS / 32];
   const int b = blockIdx.x;
   const bool fwd = blockIdx.y == 0;
   const int P = fwd ? Mp : N;
   float* e = (fwd ? elem_fwd : elem_bwd) + static_cast<size_t>(b) * P;
+  int* idx = fwd ? idx_fwd : idx_bwd;
+  const float* pb = pred + static_cast<size_t>(b) * 3 * Mp;
+  const float* gb = gt + static_cast<size_t>(b) * 3 * N;
   float s = 0.f;
   for (int i = threadIdx.x; i < P; i += CC_THREADS) {
-    const float v = __fsqrt_rn(__fadd_rn(e[i], 1e-8f));
+    float d = e[i];
+    if (__float_as_uint(d) == CH_INF) {
+      const int m = fwd ? i : 0, n = fwd ? 0 : i;
+      const float dx = __fsub_rn(pb[m], gb[n]), dy = __fsub_rn(pb[Mp + m], gb[N + n]),
+                  dz = __fsub_rn(pb[2 * Mp + m], gb[2 * N + n]);
+      d = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+      if (idx) idx[static_cast<size_t>(b) * P + i] = 0;
+    }
+    const float v = __fsqrt_rn(__fadd_rn(d, 1e-8f));
     e[i] = v;
     s += v;
   }
@@ -259,7 +285,8 @@ extern "C" int sonet_chamfer_f32(const float* pred, const float* gt, int B, int 
     rc = check_launch("chamfer(arg-min)");
     if (rc) return rc;
   }
-  chamfer_cloud_kernel<<<dim3(B, 2), CC_THREADS, 0, st>>>(elem_fwd, Mp, elem_bwd, N, loss_fwd_arr, loss_bwd_arr);
+  chamfer_cloud_kernel<<<dim3(B, 2), CC_THREADS, 0, st>>>(pred, gt, elem_fwd, Mp, elem_bwd, N, idx_fwd,
+                                                          idx_bwd, loss_fwd_arr, loss_bwd_arr);
   chamfer_final_kernel<<<1, 256, 0, st>>>(loss_fwd_arr, loss_bwd_arr, B, loss);
   return check_launch("chamfer");
 }

@@ -58,7 +58,13 @@ class ChamferLoss(nn.Module):
 
     def forward(self, predict_pc, gt_pc):
         """predict_pc [B,3,M], gt_pc [B,3,N] (CUDA) -> scalar loss; also sets forward_loss,
-        backward_loss, forward_loss_array, backward_loss_array, loss_array (losses.py:281-289)."""
+        backward_loss, forward_loss_array, backward_loss_array, loss_array (losses.py:281-289).
+
+        Nearest neighbours are exact, lowest index on ties. A point with no finite nearest
+        neighbour (every candidate's squared distance is NaN or overflows to +inf) is paired with
+        the other cloud's point 0, as a brute-force scan from (+inf, index 0) would: its term is
+        NaN if either point has a NaN coordinate, +inf on overflow. So non-finite inputs give a
+        NaN or inf loss, in training as in evaluation, and nn_idx_fwd / nn_idx_bwd stay in range."""
         if not predict_pc.is_cuda:
             raise RuntimeError("sonet_b200.ChamferLoss runs on CUDA tensors only (no CPU fallback)")
         need_grad = torch.is_grad_enabled() and (predict_pc.requires_grad or gt_pc.requires_grad)

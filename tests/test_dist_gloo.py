@@ -33,7 +33,9 @@ def _worker(rank, world, port, total, q):
 
     out = sdist.ShardedForward(fwd)(inputs, total)
     if rank == 0:
-        q.put(out)
+        # by value: a tensor would cross the queue as a file descriptor that its sender hands out
+        # on request, and this process may have exited before the parent asks for it
+        q.put(out.numpy())
     dist.barrier()
     dist.destroy_process_group()
 
@@ -45,7 +47,7 @@ def _run(total):
     procs = [ctx.Process(target=_worker, args=(r, 2, port, total, q)) for r in range(2)]
     for p in procs:
         p.start()
-    out = q.get(timeout=120)
+    out = torch.from_numpy(q.get(timeout=120))
     for p in procs:
         p.join(timeout=120)
         assert p.exitcode == 0
