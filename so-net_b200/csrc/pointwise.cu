@@ -20,11 +20,20 @@ namespace sonet {
 
 constexpr int PW_BK = 8;
 
-// ELU: the ELU epilogue instead of relu ? ReLU : identity (relu is ignored)
+// max(a, b) that is NaN when either operand is NaN, as PyTorch's relu and max are (fmaxf returns
+// the other operand). One FMNMX.NAN; for every non-NaN input the same bits as fmaxf.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// ELU: the ELU epilogue instead of relu ? ReLU : identity (relu is ignored).
+// wvec: Cout % 4 == 0 and Wt 16-byte aligned -> 128-bit weight loads.
 template <int BM, int BN, int TM, int TN, bool VECP, bool ELU>
 __global__ void __launch_bounds__(256, 2)
     pointwise_kernel(const float* __restrict__ x0, int C0, const float* __restrict__ x1, int C1,
-                     int P, const float* __restrict__ Wt, const float* __restrict__ scale,
+                     int P, const float* __restrict__ Wt, int wvec, const float* __restrict__ scale,
                      const float* __restrict__ shift, int Cout, int relu,
                      const float* __restrict__ addend, const int32_t* __restrict__ gidx, int G,
                      float* __restrict__ out) {
@@ -40,7 +49,6 @@ __global__ void __launch_bounds__(256, 2)
   const int b = blockIdx.z;
   const int co0 = blockIdx.y * BM, p0 = blockIdx.x * BN;
   const int Cin = C0 + C1;
-  const bool wvec = (Cout % 4 == 0);
 
   float acc[TM][TN];
 #pragma unroll
@@ -171,7 +179,7 @@ __global__ void __launch_bounds__(256, 2)
       for (int j = 0; j < 4; ++j) {
         float t = fmaf(acc[i][s * 4 + j], sc, sh);
         if (arow) t += __ldg(arow + gcol[s * 4 + j]);
-        v[j] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
+        v[j] = ELU ? elu1(t) : (relu ? fmax_nan(t, 0.f) : t);
       }
       if (VECP) {
         if (p < P) *reinterpret_cast<float4*>(orow + p) = make_float4(v[0], v[1], v[2], v[3]);
@@ -186,23 +194,23 @@ __global__ void __launch_bounds__(256, 2)
 
 template <int BM, int BN, int TM, int TN>
 static void launch_pointwise(bool vecp, dim3 grid, cudaStream_t st, const float* x0, int C0,
-                             const float* x1, int C1, int P, const float* Wt, const float* scale,
-                             const float* shift, int Cout, int act, const float* addend,
-                             const int32_t* gidx, int G, float* out) {
+                             const float* x1, int C1, int P, const float* Wt, int wvec,
+                             const float* scale, const float* shift, int Cout, int act,
+                             const float* addend, const int32_t* gidx, int G, float* out) {
   const int relu = act == SONET_ACT_RELU;
   if (act == SONET_ACT_ELU) {
     if (vecp)
       pointwise_kernel<BM, BN, TM, TN, true, true><<<grid, 256, 0, st>>>(
-          x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
+          x0, C0, x1, C1, P, Wt, wvec, scale, shift, Cout, relu, addend, gidx, G, out);
     else
       pointwise_kernel<BM, BN, TM, TN, false, true><<<grid, 256, 0, st>>>(
-          x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
+          x0, C0, x1, C1, P, Wt, wvec, scale, shift, Cout, relu, addend, gidx, G, out);
   } else if (vecp) {
     pointwise_kernel<BM, BN, TM, TN, true, false><<<grid, 256, 0, st>>>(
-        x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
+        x0, C0, x1, C1, P, Wt, wvec, scale, shift, Cout, relu, addend, gidx, G, out);
   } else {
     pointwise_kernel<BM, BN, TM, TN, false, false><<<grid, 256, 0, st>>>(
-        x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu, addend, gidx, G, out);
+        x0, C0, x1, C1, P, Wt, wvec, scale, shift, Cout, relu, addend, gidx, G, out);
   }
 }
 
@@ -226,7 +234,7 @@ __global__ void __launch_bounds__(256)
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) {
     float t = fmaf(s, scale ? scale[co] : 1.f, shift ? shift[co] : 0.f);
-    out[warp_id] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
+    out[warp_id] = ELU ? elu1(t) : (relu ? fmax_nan(t, 0.f) : t);
   }
 }
 
@@ -288,7 +296,7 @@ __global__ void __launch_bounds__(256)
       const int co = co0 + c;
       if (co < Cout && (h == 0 || two)) {
         const float t = fmaf(v, scale ? __ldg(scale + co) : 1.f, shift ? __ldg(shift + co) : 0.f);
-        out[static_cast<size_t>(b0 + h) * Cout + co] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
+        out[static_cast<size_t>(b0 + h) * Cout + co] = ELU ? elu1(t) : (relu ? fmax_nan(t, 0.f) : t);
       }
     }
   }
@@ -357,7 +365,7 @@ __global__ void __launch_bounds__(256)
   if (b < B && co < Cout) {
     const float v = (acc.x + acc.y) + (acc.z + acc.w);
     const float t = fmaf(v, scale ? __ldg(scale + co) : 1.f, shift ? __ldg(shift + co) : 0.f);
-    out[static_cast<size_t>(b) * Cout + co] = ELU ? elu1(t) : (relu ? fmaxf(t, 0.f) : t);
+    out[static_cast<size_t>(b) * Cout + co] = ELU ? elu1(t) : (relu ? fmax_nan(t, 0.f) : t);
   }
 }
 
@@ -376,14 +384,14 @@ __global__ void __launch_bounds__(256)
     const long long r = row0 + static_cast<long long>(u) * rpw;
     if (r < R) {
       const float4 v = __ldg(in + r * G + (lane - sub * G));
-      m[u] = fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w));
+      m[u] = fmax_nan(fmax_nan(v.x, v.y), fmax_nan(v.z, v.w));
     } else {
       m[u] = -__int_as_float(0x7f800000);
     }
   }
 #pragma unroll
   for (int u = 0; u < 4; ++u) {
-    for (int o = G >> 1; o > 0; o >>= 1) m[u] = fmaxf(m[u], __shfl_xor_sync(0xffffffffu, m[u], o));
+    for (int o = G >> 1; o > 0; o >>= 1) m[u] = fmax_nan(m[u], __shfl_xor_sync(0xffffffffu, m[u], o));
     const long long r = row0 + static_cast<long long>(u) * rpw;
     if (lane == sub * G && r < R) out[r] = m[u];
   }
@@ -397,7 +405,7 @@ __global__ void __launch_bounds__(256)
   if (r >= R) return;
   const float* p = in + r * L;
   float m = p[0];
-  for (int i = 1; i < L; ++i) m = fmaxf(m, p[i]);
+  for (int i = 1; i < L; ++i) m = fmax_nan(m, p[i]);
   out[r] = m;
 }
 __global__ void __launch_bounds__(256)
@@ -407,9 +415,9 @@ __global__ void __launch_bounds__(256)
   if (r >= R) return;
   const float* p = in + r * L;
   float m = -__int_as_float(0x7f800000);
-  for (int i = lane; i < L; i += 32) m = fmaxf(m, p[i]);
+  for (int i = lane; i < L; i += 32) m = fmax_nan(m, p[i]);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  for (int o = 16; o > 0; o >>= 1) m = fmax_nan(m, __shfl_xor_sync(0xffffffffu, m, o));
   if (lane == 0) out[r] = m;
 }
 
@@ -681,19 +689,20 @@ extern "C" int sonet_pointwise_layer_f32(const float* x0, int C0, const float* x
   SONET_REQUIRE(x0 && Wt && out, "pointwise: null pointer");
   SONET_REQUIRE(C1 == 0 || x1 != nullptr, "pointwise: x1 null with C1=%d", C1);
   SONET_REQUIRE(!addend || (gidx && G >= 1), "pointwise: addend needs gidx and G");
-  const bool vecp = (P % 4 == 0) && aligned16(x0) && aligned16(out) && (C1 == 0 || aligned16(x1)) &&
-                    aligned16(Wt);
+  // 128-bit loads: of the activation rows and the output (vecp), of the weight rows (wvec)
+  const bool vecp = (P % 4 == 0) && aligned16(x0) && aligned16(out) && (C1 == 0 || aligned16(x1));
+  const int wvec = (Cout % 4 == 0) && aligned16(Wt);
   cudaStream_t st = as_stream(stream);
   if (P >= 1024 && Cout >= 128) {
     dim3 grid((P + 127) / 128, (Cout + 127) / 128, B);
     SONET_REQUIRE(grid.y <= 65535, "pointwise: Cout too large");
-    launch_pointwise<128, 128, 8, 8>(vecp, grid, st, x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu,
-                                     addend, gidx, G, out);
+    launch_pointwise<128, 128, 8, 8>(vecp, grid, st, x0, C0, x1, C1, P, Wt, wvec, scale, shift, Cout,
+                                     relu, addend, gidx, G, out);
   } else {
     dim3 grid((P + 63) / 64, (Cout + 63) / 64, B);
     SONET_REQUIRE(grid.y <= 65535, "pointwise: Cout too large");
-    launch_pointwise<64, 64, 4, 4>(vecp, grid, st, x0, C0, x1, C1, P, Wt, scale, shift, Cout, relu,
-                                   addend, gidx, G, out);
+    launch_pointwise<64, 64, 4, 4>(vecp, grid, st, x0, C0, x1, C1, P, Wt, wvec, scale, shift, Cout,
+                                   relu, addend, gidx, G, out);
   }
   return check_launch("pointwise_layer");
 }

@@ -206,7 +206,9 @@ def test_linear_rowmax_kcopy():
     assert torch.equal(ops.linear(xb[:3].contiguous(), W.to(DEV), None, shift.to(DEV), False), full[:3])
     assert_close(full.cpu(), F.linear(xb.cpu(), W) + shift, "linear B=67", 2e-5)
     assert torch.equal(ops.linear(xb[66:].contiguous(), W.to(DEV), None, shift.to(DEV), False), full[66:])
-    # channel tiles of 4 / 2 / 1, ragged Cout and B, folded scale, and the unaligned fallback
+    # the tiled kernel with ragged Cout and B and a folded scale, the blocked kernel with one
+    # channel per block (Cin 12288) and the warp-per-output kernel (Cin % 4 != 0);
+    # test_gpu_fp32_envelope.py reaches every branch of the launcher on purpose
     for B_, cin, cout in ((64, 1024, 512), (64, 512, 256), (33, 1040, 1024), (7, 256, 41), (1, 64, 3),
                           (5, 1030, 17), (4, 12288, 8)):
         x = torch.from_numpy(rs.normal(size=(B_, cin)).astype(np.float32))
