@@ -45,13 +45,15 @@ const char* sonet_version(void);
  * Replaces index_max.forward_cuda / forward_cuda_shared_mem
  *   (models/index_max_ext/index_max.cpp:132-148, index_max_cuda.cu:10-100; called at
  *   models/networks.py:181-185).
- * data [B,C,N] f32, index [B,N] i32 with values in [0,K) (validated only in debug builds; an
- * out-of-range value is clamped, never a wild write), out_idx [B,C,K] i32:
+ * data [B,C,N] f32, index [B,N] i32 with values in [0,K). The values are not validated: an id
+ * outside [0,K) is read as min((unsigned)id, K-1), so a negative or too large id counts as node
+ * K-1 and is never a wild write. A NaN in data is never an arg-max (strict '>').
+ * out_idx [B,C,K] i32:
  *   out_idx[b,c,k] = lowest n with index[b,n]==k maximising data[b,c,n], provided that maximum
  *   is > -1000.0f; otherwise 0 (empty node, or all values <= -1000: the reference's sentinel).
  * out_val (nullable) [B,C,K] f32 = data[b,c,out_idx[b,c,k]]  — i.e. the masked gather of
  *   models/networks.py:185 (first_pn_out_masked_max) fused into the pool.
- * K <= 256 on the CUDA path. */
+ * K <= 256 on the CUDA path. N == 0 writes zeros to both outputs (data and index may be null). */
 int sonet_index_max_f32(const float* data, const int32_t* index, int B, int C, int N, int K,
                         int32_t* out_idx, float* out_val, sonet_stream_t stream);
 

@@ -67,14 +67,6 @@ __device__ __forceinline__ float4 ldg_stream_f4(const float4* p) {
                : "l"(p));
   return r;
 }
-// same, asking L2 to fetch the whole 256-byte neighbourhood from DRAM (sequential row streams)
-__device__ __forceinline__ float4 ldg_stream256_f4(const float4* p) {
-  float4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::256B.v4.f32 {%0,%1,%2,%3}, [%4];"
-               : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w)
-               : "l"(p));
-  return r;
-}
 __device__ __forceinline__ float ldg_stream_f1(const float* p) {
   float r;
   asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(r) : "l"(p));

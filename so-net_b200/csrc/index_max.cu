@@ -4,6 +4,10 @@
 // index_max_cuda.cu:10-26): for data[B,C,N], index[B,N] in [0,K):
 //   max_idx[b,c,k] = first n (ascending) with index[b,n]==k that attains the maximum of
 //   data[b,c,n] over that node, if the maximum is > -1000.0f; else 0.
+// A NaN never passes the strict '>', so it is never an arg-max; -inf never beats the sentinel.
+// index values outside [0,K) are not an error: every table access goes through
+// min(unsigned(index), K-1) (im_update, im_update4), so a negative or too large id counts as node
+// K-1 and never writes outside the warp's table.
 //
 // Design (HBM-bound: 4 B/element must stream at close to the HBM bandwidth):
 //   * persistent grid, one CTA per SM; a work item is (b, group of NW channels); warp w of the CTA
@@ -18,7 +22,6 @@
 //   * the masked gather that follows in the model (models/networks.py:185) is fused: the max
 //     value (or data[b,c,0] for empty nodes, as idx*mask_row_max gathers point 0) is emitted too.
 #include <algorithm>
-#include <cstdlib>
 #include <thread>
 #include <vector>
 
@@ -101,7 +104,7 @@ __device__ __forceinline__ void im_reduce_row(float* tval, IdxT* tidx, int lane,
 }
 
 // VEC path: N % 4 == 0 and 16B-aligned bases. blockDim = (NW + 1) * 32; warp NW is the producer.
-template <typename IdxT, bool L2HINT>
+template <typename IdxT>
 __global__ void __launch_bounds__((IM_MAX_WARPS + 1) * 32, 1)
     index_max_vec_kernel(const float* __restrict__ data, const int32_t* __restrict__ index, int B,
                          int C, int N, int K, int NW, int32_t* __restrict__ out_idx,
@@ -186,7 +189,7 @@ __global__ void __launch_bounds__((IM_MAX_WARPS + 1) * 32, 1)
 #pragma unroll
       for (int u = 0; u < IM_UNROLL; ++u) {
         const int v = u * 32 + lane;
-        if (v < nvec_row) nxt[u] = L2HINT ? ldg_stream256_f4(row4 + v) : ldg_stream_f4(row4 + v);
+        if (v < nvec_row) nxt[u] = ldg_stream_f4(row4 + v);
       }
     }
     for (int ch = 0; ch < nch; ++ch) {
@@ -202,7 +205,7 @@ __global__ void __launch_bounds__((IM_MAX_WARPS + 1) * 32, 1)
 #pragma unroll
             for (int u = 0; u < IM_UNROLL; ++u) {
               const int v = (g + 1) * GV + u * 32 + lane;
-              if (v < nvec_row) nxt[u] = L2HINT ? ldg_stream256_f4(row4 + v) : ldg_stream_f4(row4 + v);
+              if (v < nvec_row) nxt[u] = ldg_stream_f4(row4 + v);
             }
           }
 #pragma unroll
@@ -293,12 +296,7 @@ static int launch_index_max(const float* data, const int32_t* index, int B, int 
   const size_t smem = fixed + NW * per_warp;
   const int sms = sm_count();
   if (vec) {
-    // SONET_IM_L2HINT=1: 256-byte L2 prefetch qualifier on the row loads (experiment switch)
-    static const bool hint = [] {
-      const char* e = getenv("SONET_IM_L2HINT");
-      return e != nullptr && e[0] == '1';
-    }();
-    auto kern = hint ? index_max_vec_kernel<IdxT, true> : index_max_vec_kernel<IdxT, false>;
+    auto kern = index_max_vec_kernel<IdxT>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     const int groups = (C + NW - 1) / NW;
     const long long items = static_cast<long long>(B) * groups;
@@ -323,7 +321,8 @@ extern "C" int sonet_index_max_f32(const float* data, const int32_t* index, int 
   SONET_REQUIRE(B >= 0 && C >= 0 && N >= 0, "index_max: negative dimension");
   SONET_REQUIRE(K >= 1 && K <= 256, "index_max: K=%d out of range [1,256]", K);
   if (B == 0 || C == 0) return SONET_OK;
-  SONET_REQUIRE(data && index && out_idx, "index_max: null pointer");
+  // N == 0: data and index have no elements, and an empty tensor's pointer may be null
+  SONET_REQUIRE(out_idx && (N == 0 || (data && index)), "index_max: null pointer");
   cudaStream_t st = as_stream(stream);
   if (N == 0) {  // every node empty: idx 0; there is no point 0 to gather -> val 0
     cudaMemsetAsync(out_idx, 0, sizeof(int32_t) * static_cast<size_t>(B) * C * K, st);

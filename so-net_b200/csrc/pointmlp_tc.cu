@@ -105,6 +105,11 @@ static_assert(W1_BYTES == SLOT_BYTES && L2_STAGE_BYTES == SLOT_BYTES && 2 * L3_H
 // max_rows(y) == fmaf(max_rows(raw), ...) bit for bit. models/index_max_ext semantics (max must be
 // > -1000, else the feature of copy 0) are restored when the keys are read
 // (knn_assemble_pool_kernel / pool_finalize_kernel). first_pn_out is never written.
+// The result does not depend on the order of the rows: the run loop takes the node ids of a warp's
+// 16 rows in any arrangement (sorting only makes one pass per warp the common case, and the order
+// inside a node is whatever som_sort left). A NaN row never becomes a node's maximum, as in
+// index_max: fmaxf drops it next to any other row, and a run of NaN rows only is keyed as -inf.
+// Required: node_sorted[b,j] < M (a negative id skips the row), 0 <= pos0[b] < P.
 struct PoolArgs {
   const int32_t* node_sorted;  // [B,P] node id of each sorted row
   const int32_t* pos0;         // [B] sorted row of stacked copy 0
@@ -436,7 +441,9 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const int dc = 8 * (i >> 1) + (i & 1);
-              const int bits = __float_as_int(fmaf(r3[i], inv3, sh3[col + dc]));
+              // fmaxf(NaN, -inf) = -inf: a run whose 16 rows are all NaN in this column must not
+              // leave a NaN key, which would order above +inf and displace the node's finite maximum
+              const int bits = __float_as_int(fmaxf(fmaf(r3[i], inv3, sh3[col + dc]), -INFINITY));
               const int key = bits ^ ((bits >> 31) & 0x7fffffff);   // order-preserving float -> int
               atomicMax(kb + dc * static_cast<size_t>(pool.M), key);
             }

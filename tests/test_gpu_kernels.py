@@ -22,6 +22,8 @@ def _rand_case(rs, B, C, N, K, ties=True, empty=True):
 
 
 # ---- index_max --------------------------------------------------------------------------------
+# golden vectors, eight shapes and one full-size property test; test_gpu_pool_envelope.py reaches every
+# branch of the launcher, the -1000 sentinel and non-finite values on purpose
 def test_index_max_golden_reference_binary():
     from sonet_b200 import index_max
     g = golden("index_max")
