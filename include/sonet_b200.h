@@ -556,6 +556,26 @@ int sonet_pointwise_tc_forward_rows(const float* x0, int C0, const float* x1, in
                                     int relu, const float* addend, const int32_t* gidx, int G,
                                     float* out, sonet_stream_t stream);
 
+/* ---- the point-wise layer at node-level row counts, csrc/nodegemm_tc.cu ------------------------
+ * The same layer, bit for bit, with the activations pre-split into fp16 hi/lo operand images in
+ * global memory so that both wgmma operands arrive by bulk copy (the encoder's final PointNet:
+ * two layers over B*M rows, where the generic kernel's per-chunk conversion dominates).
+ *   image_bytes(rows, C, f16): size of the images of a [rows x C] activation matrix (16-byte
+ *     aligned device memory); f16 != 0: the hi image only, for the one-product fp16 mode.
+ *   split_pack (device pointers): cat(x0 [B,C0,P], x1 [B,C1,P] or NULL) -> img.
+ *   forward (device pointers): img (of B*P rows x Cin) x the blob of sonet_pointwise_tc_pack
+ *     -> act(inv_scale * GEMM + shift), written either as out [B,Cout,P] fp32 (img_out NULL), the
+ *     values sonet_pointwise_tc_forward writes, or as img_out (out NULL), the images split_pack
+ *     would build from that tensor: the next layer's input. act is the activation code; f16 must
+ *     be the value the images were built with (then: the values of sonet_pointwise_tc_forward_f16).
+ *   No allocation, no host synchronisation, deterministic, CUDA graph capturable. */
+long long sonet_nodegemm_image_bytes(long long rows, int C, int f16);
+int sonet_nodegemm_split_pack(const float* x0, int C0, const float* x1, int C1, int B, int P,
+                              int f16, void* img, sonet_stream_t stream);
+int sonet_nodegemm_tc_forward(const void* img, int Cin, int B, int P, const void* blob,
+                              float inv_scale, const float* shift, int Cout, int act, int f16,
+                              void* img_out, float* out, sonet_stream_t stream);
+
 /* ---- KNNModule (3+C -> 512 -> 512, BN + ReLU, max over K) on wgmma, csrc/knn_tc.cu -----------
  * Layer 1 is split by linearity: Y = W1f x [B,512,M] (the C feature columns, computed once per
  * node by sonet_pointwise_tc_forward without shift or ReLU) is gathered per neighbour row and added

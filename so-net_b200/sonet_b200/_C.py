@@ -127,6 +127,11 @@ _SIGNATURES = {
     "sonet_pointwise_tc_forward": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                    ctypes.c_float, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                    c_int, c_void_p, c_void_p],
+    "sonet_nodegemm_image_bytes": [ctypes.c_longlong, c_int, c_int],
+    "sonet_nodegemm_split_pack": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                  c_void_p],
+    "sonet_nodegemm_tc_forward": [c_void_p, c_int, c_int, c_int, c_void_p, ctypes.c_float, c_void_p,
+                                  c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "sonet_knn_mlp_tc_blob_bytes": [],
     "sonet_knn_mlp_tc_pack": [c_void_p, c_void_p, c_void_p],
     "sonet_pointwise_tc_forward_rows": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
@@ -173,6 +178,7 @@ ACT_ENTRIES = ("sonet_pointresnet_tc_forward_act", "sonet_pointresnet_tc_pool_fo
 _RESTYPE = {"sonet_last_error_string": ctypes.c_char_p, "sonet_version": ctypes.c_char_p,
             "sonet_pointwise_tc_blob_bytes": ctypes.c_longlong,
             "sonet_knn_mlp_tc_blob_bytes": ctypes.c_longlong,
+            "sonet_nodegemm_image_bytes": ctypes.c_longlong,
             "sonet_som_group_smem_bytes": ctypes.c_longlong,
             "sonet_seg_loss_scratch_bytes": ctypes.c_longlong,
             "sonet_retrieval_scratch_bytes": ctypes.c_longlong,

@@ -742,15 +742,36 @@ class PointNet(nn.Module):
         super().__init__()
         self.layers = _chain(in_channels, out_channels_list, activation, normalization, momentum,
                              bn_momentum_decay_step, bn_momentum_decay)
+        self._node_images = ops.NodeImages()
 
     def forward(self, x, epoch=None):
         for layer in self.layers:
             x = layer(x, epoch)
         return x
 
+    def _node_route(self, x0, x1):
+        """The eval fast path runs on ops.nodegemm_pointnet: two layers, both dense enough for
+        wgmma (forward_points' rule), BatchNorm + ReLU / ELU then the bare last layer, over at
+        most ops.NODEGEMM_MAX_ROWS rows (the encoder's node-level final PointNet)."""
+        if len(self.layers) != 2 or x0.dim() != 3 or not tc_enabled():
+            return False
+        l1, l2 = self.layers
+        rows = x0.shape[0] * x0.shape[2]
+        return (l1.fast(x0, x1) and l2.fast(x0)
+                and l1.normalization == 'batch' and l1.activation in ('relu', 'elu')
+                and l2.normalization is None and l2.activation is None
+                and x0.shape[1] + x1.shape[1] >= 32 and l1.conv.out_channels >= 32
+                and 256 <= rows <= ops.NODEGEMM_MAX_ROWS)
+
     def forward_pair(self, x0, x1, epoch=None):
         """forward(torch.cat((x0, x1), dim=1)) without materialising the concat in eval mode."""
         first = self.layers[0]
+        if self._node_route(x0, x1):
+            l1, l2 = self.layers
+            return ops.nodegemm_pointnet(x0.contiguous(), x1.contiguous(), l1._tc_params(),
+                                         l1.conv.out_channels, l1.activation, l2._tc_params(),
+                                         l2.conv.out_channels, f16=tc_f16(),
+                                         owner=self._node_images)
         if first.fast(x0, x1):
             x = first.forward_points(x0.contiguous(), x1.contiguous())
             for layer in self.layers[1:]:

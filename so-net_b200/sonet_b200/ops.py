@@ -722,6 +722,61 @@ def pointwise_layer_tc(x0, blob, inv_scale, shift, cout, act, x1=None, addend=No
     return out
 
 
+# Row count up to which a two-layer PointNet takes nodegemm_pointnet. Below it the generic layer's
+# per-chunk activation conversion dominates its items; the segmenter's 49 k-row layers amortise it.
+NODEGEMM_MAX_ROWS = 16384
+
+
+class NodeImages:
+    """Per-owner (one per PointNet), per-(device, size, stream) buffers of nodegemm_pointnet's fp16
+    operand images. They are static, so no forward allocates them and a captured CUDA graph
+    replays on the buffers it was captured with."""
+
+    def __init__(self):
+        self._bufs = {}
+
+    def get(self, dev, which, nbytes, stream):
+        kk = (dev, which, int(nbytes), int(stream))
+        buf = self._bufs.get(kk)
+        if buf is None:
+            buf = self._bufs[kk] = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+        return buf
+
+
+_DEFAULT_NODE_IMAGES = NodeImages()   # for direct ops.nodegemm_pointnet callers (tests, tools)
+
+
+def nodegemm_pointnet(x0, x1, params1, cout1, act, params2, cout2, f16=False, owner=None):
+    """act(layer 1) then the bare layer 2 over cat(x0 [B,C0,P], x1 [B,C1,P] or None) -> [B,cout2,P]
+    on the node-level wgmma GEMM (csrc/nodegemm_tc.cu), bit-identical to two pointwise_layer_tc
+    calls. params1 / params2: (blob, inv_scale, shift) of the layers, as pointwise_tc_pack makes
+    them. The input is split into fp16 operand images once; layer 1 writes its output as layer 2's
+    images. f16: one fp16 product per MAC instead of the hi/lo split's three."""
+    _chk(x0, "x0", torch.float32)
+    _chk(x1, "x1", torch.float32, optional=True)
+    for blob, _, shift in (params1, params2):
+        _chk(blob, "blob", torch.uint8)
+        _chk(shift, "shift", torch.float32, optional=True)
+    B, C0, P = x0.shape
+    C1 = 0 if x1 is None else x1.shape[1]
+    dev, f16, stream = x0.device, int(bool(f16)), _stream(x0)
+    lib = _C.lib()
+    with torch.cuda.device(dev):
+        imgs = owner or _DEFAULT_NODE_IMAGES
+        img0 = imgs.get(dev, 0, lib.sonet_nodegemm_image_bytes(B * P, C0 + C1, f16), stream)
+        img1 = imgs.get(dev, 1, lib.sonet_nodegemm_image_bytes(B * P, int(cout1), f16), stream)
+        out = torch.empty((B, cout2, P), dtype=torch.float32, device=dev)
+        _call("sonet_nodegemm_split_pack", _C.ptr(x0), C0, _C.ptr(x1), C1, B, P, f16, _C.ptr(img0),
+              stream)
+        _call("sonet_nodegemm_tc_forward", _C.ptr(img0), C0 + C1, B, P, _C.ptr(params1[0]),
+              float(params1[1]), _C.ptr(params1[2]), int(cout1), act_code(act), f16, _C.ptr(img1),
+              None, stream)
+        _call("sonet_nodegemm_tc_forward", _C.ptr(img1), int(cout1), B, P, _C.ptr(params2[0]),
+              float(params2[1]), _C.ptr(params2[2]), int(cout2), ACT_NONE, f16, None, _C.ptr(out),
+              stream)
+    return out
+
+
 def knn_mlp_tc_pack(W2):
     """W2 [512,512] folded fp32 (any device) -> (blob uint8 CPU tensor, inv_scale float): the
     layer-2 weight stream of knn_mlp_tc."""
