@@ -28,6 +28,12 @@
 //     (A segmented shuffle reduction in front of the atomics spilled the accumulators; a
 //     __match_any_sync + __reduce_max_sync one made the epilogue ~10x slower, as redux.sync with
 //     lane-dependent masks serialises.)
+//   * non-finite inputs: layer 1's ReLU maps a NaN to 0. Under ELU a NaN h1 makes its whole layer-2
+//     row NaN; the wgmma returns that NaN with the sign bit clear (for NaN inputs of either sign),
+//     so its key lies above +inf's and the node is NaN in every channel, as rowmax gives. +-inf
+//     saturates in the split like any |h1| >= 131008 (-inf: h1 = 0 or -1). Ids are clamped to
+//     [0, M-1]; padding rows read node 0 of cloud 0 and never reach a key
+//     (tests/test_gpu_knn_envelope.py).
 //
 // Rows: a warpgroup owns a BLOCK of floor(64/K) whole consecutive nodes of the flattened (cloud,
 // node) sequence (7 nodes = 63 rows at K = 9), so no node is split across warpgroups or CTAs and no
