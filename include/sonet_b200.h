@@ -315,6 +315,31 @@ int sonet_augment_f32(const float* pc, const float* sn, const float* som, int B,
                       const double* noise_sn, const double* noise_som, unsigned long long seed,
                       float* pc_out, float* sn_out, float* som_out, sonet_stream_t stream);
 
+/* ---- f-3: the loader's random choice of points, from a dataset in device memory ----------------
+ * Replaces the head of the loaders' __getitem__ for a whole batch: np.random.choice(P, N,
+ * replace=False) (data/modelnet_shrec_loader.py:198,212; rule SUBSET) and the ShapeNet rule
+ * (data/shapenet_loader.py:142-154; rule FILL: N < P as SUBSET, else the whole cloud in source
+ * order followed by N-P uniform draws with replacement, so N == P is the cloud in order).
+ * data [sum P, 6] f32 point-major (xyz | normal), offsets [S+1] i64 (cloud s is rows
+ * offsets[s]..offsets[s+1]), labels [sum P] i32 (nullable, with seg_out), cloud_ids [B] i64: all
+ * device pointers. Outputs pc_out, sn_out [B,3,N] and seg_out [B,N] i64 (the part labels).
+ * indices [B,N] i32 (DEVICE, nullable): the source positions within each cloud, e.g. the loader's
+ * own numpy draws (reproduces it bit for bit); values outside [0,P) are clamped to [0,P-1]. When
+ * NULL, the kernel draws them from Philox4x32-10 keyed by (seed, batch position, point): SUBSET is
+ * the distribution of permutation(P)[:N], the FILL draws are unbiased (Lemire). A cloud id outside
+ * [0,S) is clamped; a cloud longer than max_P is read as its first max_P points; an empty cloud
+ * gives zeros. SUBSET with P < N is outside the contract (the caller checks the counts): such a
+ * cloud is filled as by FILL. Fails with SONET_ERR_BAD_ARG before any CUDA call for an unknown
+ * rule, N < 1, B outside [0,65535], S < 1, max_P < 1, max_P > SONET_SAMPLE_MAX_P without indices,
+ * labels/seg_out not both null or both given, or a null data/offsets/cloud_ids/pc_out/sn_out. */
+#define SONET_SAMPLE_SUBSET 0
+#define SONET_SAMPLE_FILL 1
+#define SONET_SAMPLE_MAX_P 65536
+int sonet_sample_points_f32(const float* data, const int64_t* offsets, int S, const int32_t* labels,
+                            const int64_t* cloud_ids, int B, int N, int max_P, int rule,
+                            const int32_t* indices, unsigned long long seed, float* pc_out,
+                            float* sn_out, int64_t* seg_out, sonet_stream_t stream);
+
 /* ---- a-4/a-5/a-8/a-9/a-10: point-wise shared MLP layer (1x1 conv + folded BN + ReLU) ---------
  * Replaces EquivariantLayer.forward / MyConv2d(1x1).forward in eval mode
  * (models/layers.py:203-210, 282-296): out[b,co,p] = act(scale[co]*sum_ci W[co,ci]*X[b,ci,p] +

@@ -18,24 +18,10 @@
 // (Philox4x32-10 + Box-Muller, keyed by seed / cloud / array / point) for production loaders,
 // where shipping 11 doubles per point from the host would cost more than the augmentation.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace sonet {
 
-// ---- Philox4x32-10 (Salmon et al., SC'11): counter-based, no state to store -----------------------
-__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-  const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-  const uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-  const uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
-  c[0] = n0; c[1] = lo1; c[2] = n2; c[3] = lo0;
-}
-__device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    philox_round(c, k0, k1);
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-}
 // three standard normals for (seed, cloud, array, point)
 __device__ __forceinline__ void normal3(unsigned long long seed, uint32_t cloud, uint32_t array,
                                         uint32_t point, double (&g)[3]) {

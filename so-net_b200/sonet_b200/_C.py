@@ -71,6 +71,9 @@ _SIGNATURES = {
                           c_void_p, c_void_p, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                           ctypes.c_double, ctypes.c_double, ctypes.c_double, c_void_p, c_void_p,
                           c_void_p, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sonet_sample_points_f32": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                c_int, c_void_p, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p,
+                                c_void_p],
     "sonet_som_decenter": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                            c_void_p, c_void_p, c_void_p],
     "sonet_pointwise_layer_f32": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,

@@ -13,6 +13,9 @@ from a numpy RandomState with the loader's own expressions, in the loader's orde
 jitter draws are generated inside the kernel (Philox4x32-10, keyed by seed/cloud/array/point) —
 or, with `host_noise=True`, drawn from the same RandomState in the loader's order and shipped to
 the device, which reproduces the reference pipeline bit for bit (what the parity tests use).
+
+`DeviceDataset` adds the head of the loaders' __getitem__, the random choice of each cloud's points
+(csrc/sample_points.cu), for batches drawn from a dataset kept in device memory.
 """
 import numpy as np
 import torch
@@ -112,3 +115,134 @@ def prepare_batch(pc, sn, som, opt, train, rng=None, seed=0, host_noise=False):
                         host_noise=host_noise)
         pc, sn, som = augment_batch(pc, sn, som, p, seed=seed)
     return pc, sn, som, som_knn(som, opt.som_k, opt.node_num)
+
+
+def _draw_choice(rng, P, N, rule):
+    """The loaders' choice of source points for one item, from `rng`: choice(P, N, replace=False)
+    (modelnet_shrec_loader.py:198,212) or the ShapeNet rule (shapenet_loader.py:142-154)."""
+    if rule == ops.SAMPLE_FILL and N >= P:
+        return np.concatenate([np.arange(P), rng.choice(P, N - P, replace=True)])
+    return rng.choice(P, N, replace=False)
+
+
+def draw_batch_host(rng, counts, N, M, rule, train, **flags):
+    """Every draw of a batch from `rng` in the loader's per-item order: item b's choice of points,
+    then (train) item b's augmentation draws, then item b+1. -> (source indices [B,N] int32,
+    draw_params-style dict with host noise, or None when not training)."""
+    B = len(counts)
+    sel = np.empty((B, N), dtype=np.int32)
+    items = []
+    for b in range(B):
+        sel[b] = _draw_choice(rng, int(counts[b]), N, rule)
+        if train:
+            items.append(draw_params(rng, 1, N, M, host_noise=True, **flags))
+    if not train:
+        return sel, None
+    cat = lambda k: None if items[0][k] is None else np.concatenate(  # noqa: E731
+        [it[k] for it in items])
+    params = dict((k, cat(k)) for k in ("rot1", "rot2", "scale", "shift"))
+    params["noise"] = [np.concatenate([it["noise"][a] for it in items]) for a in range(3)]
+    return sel, params
+
+
+class DeviceDataset:
+    """A whole dataset in device memory, drawn from batch by batch: the loaders' complete
+    __getitem__ (random point choice, augmentation, SOM-node kNN) plus the collation, on the device.
+
+    points: list of [P_i, 6] arrays (xyz | normal, the column order of the ModelNet .npy files and of
+    pc / sn in the npz files); labels: [S] class ids; som_nodes: list of [M, 3]; seg: list of [P_i]
+    part labels (ShapeNet) or None. Everything is uploaded once, as fp32 (int32 part labels).
+
+    A float64 source (SHREC's np.loadtxt data) is rounded to fp32 here, once. The loader instead adds
+    its jitter and applies the rotations and scale in float64 before its one rounding, so in train
+    mode an output value can differ from the loader's by the input rounding carried through
+    (at most 2^-24 * scale * |v|, v the point's or node's 3-vector) plus one fp32 ulp of the result.
+    Test-mode outputs are the loader's bits."""
+
+    def __init__(self, points, labels, som_nodes, seg=None, device="cuda"):
+        S = len(points)
+        if S == 0 or len(labels) != S or len(som_nodes) != S or (seg is not None and len(seg) != S):
+            raise ValueError("DeviceDataset: points, labels, som_nodes (and seg) need one entry per "
+                             "cloud, at least one")
+        counts = np.array([np.shape(p)[0] for p in points], dtype=np.int64)
+        for i, p in enumerate(points):
+            if np.ndim(p) != 2 or np.shape(p)[1] != 6:
+                raise ValueError("DeviceDataset: cloud %d has shape %s, expected [P, 6]"
+                                 % (i, np.shape(p)))
+        if (counts == 0).any():
+            raise ValueError("DeviceDataset: cloud %d is empty" % int(np.flatnonzero(counts == 0)[0]))
+        M = np.shape(som_nodes[0])[0]
+        if any(np.shape(s) != (M, 3) for s in som_nodes):
+            raise ValueError("DeviceDataset: every som_nodes entry must be [M, 3] with one M")
+        if seg is not None and any(np.shape(s) != (c,) for s, c in zip(seg, counts)):
+            raise ValueError("DeviceDataset: seg[i] must be [P_i]")
+        self.device = torch.device(device)
+        self.counts = counts
+        self.max_P = int(counts.max())
+        self.node_num = M
+        offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+        host = np.concatenate([np.asarray(p, dtype=np.float32) for p in points])
+        self.data = torch.from_numpy(host).to(self.device)
+        self.offsets = torch.from_numpy(offsets).to(self.device)
+        self.labels = torch.from_numpy(np.asarray(labels, dtype=np.int64).reshape(S)).to(self.device)
+        nodes = np.stack([np.asarray(s, dtype=np.float32).T for s in som_nodes])
+        self.som_nodes = torch.from_numpy(np.ascontiguousarray(nodes)).to(self.device)
+        self.seg = None if seg is None else torch.from_numpy(
+            np.concatenate([np.asarray(s, dtype=np.int32) for s in seg])).to(self.device)
+
+    def __len__(self):
+        return len(self.counts)
+
+    def batch(self, index, opt, train, rng=None, seed=0, host_noise=False):
+        """The collated batch of the loader `opt.dataset` selects (autoencoder/train.py:25-36) for
+        the clouds `index`, ready for Model.set_input(*...):
+          modelnet / shrec: (pc, sn, label, som_node, som_knn_I)        N distinct points per cloud
+          shapenet:         (pc, sn, label, seg, som_node, som_knn_I)   the ShapeNet fill rule
+        with N = opt.input_pc_num; train=True adds the loader's augmentation (prepare_batch's).
+        host_noise=True draws everything from `rng` in the loader's per-item order (the choice of
+        item b, then item b's augmentation, then item b+1) and reproduces the loader bit for bit;
+        host_noise=False draws the choice and the jitter in the kernels (keyed by `seed`) and only
+        the per-cloud scalars from `rng`."""
+        if opt.dataset in ("modelnet", "shrec"):
+            rule = ops.SAMPLE_SUBSET
+        elif opt.dataset == "shapenet":
+            rule = ops.SAMPLE_FILL
+            if self.seg is None:
+                raise ValueError("DeviceDataset: the shapenet batch needs seg")
+        else:
+            raise ValueError("DeviceDataset: unknown dataset %r" % (opt.dataset,))
+        ids = np.asarray(index, dtype=np.int64).reshape(-1)
+        S = len(self.counts)
+        if ((ids < 0) | (ids >= S)).any():
+            raise IndexError("DeviceDataset: cloud index out of range [0, %d)" % S)
+        B, N, M = len(ids), int(opt.input_pc_num), self.node_num
+        P = self.counts[ids]
+        if rule == ops.SAMPLE_SUBSET and (P < N).any():
+            raise ValueError("Cannot take a larger sample than population when 'replace=False' "
+                             "(cloud %d has %d points, N=%d)" % (ids[P < N][0], P[P < N][0], N))
+        rng = rng if rng is not None else np.random
+        # the ShapeNet loader neither rotates nor shifts (shapenet_loader.py:157-180)
+        flags = dict(rot_horizontal=bool(getattr(opt, "rot_horizontal", False)),
+                     rot_perturbation=bool(getattr(opt, "rot_perturbation", False)),
+                     translation_perturbation=bool(getattr(opt, "translation_perturbation", False)))
+        if rule == ops.SAMPLE_FILL:
+            flags = dict.fromkeys(flags, False)
+        params = None
+        indices = None
+        if host_noise:
+            sel, params = draw_batch_host(rng, P, N, M, rule, train, **flags)
+            indices = torch.from_numpy(sel).to(self.device)
+        elif train:
+            params = draw_params(rng, B, N, M, host_noise=False, **flags)
+        cid = torch.from_numpy(ids).to(self.device)
+        pc, sn, seg = ops.sample_points(self.data, self.offsets, cid, N, rule, int(P.max()),
+                                        labels=self.seg if rule == ops.SAMPLE_FILL else None,
+                                        indices=indices, seed=seed)
+        som = self.som_nodes.index_select(0, cid)
+        if train:
+            pc, sn, som = augment_batch(pc, sn, som, params, seed=seed)
+        knn = som_knn(som, opt.som_k, M)
+        label = self.labels.index_select(0, cid)
+        if rule == ops.SAMPLE_FILL:
+            return pc, sn, label, seg, som, knn
+        return pc, sn, label, som, knn

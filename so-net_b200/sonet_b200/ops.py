@@ -185,6 +185,41 @@ def augment(pc, sn, som, rot1=None, rot2=None, scale=None, shift=None, jitter_pc
     return po, so, mo
 
 
+# point-selection rules of the C-ABI (SONET_SAMPLE_*, include/sonet_b200.h)
+SAMPLE_SUBSET, SAMPLE_FILL = 0, 1
+SAMPLE_MAX_P = 65536      # largest cloud of the in-kernel draws
+
+
+def sample_points(data, offsets, cloud_ids, N, rule, max_P, labels=None, indices=None, seed=0):
+    """The loaders' random choice of N points per cloud (csrc/sample_points.cu) from a ragged
+    dataset on the device: data [sum P, 6] f32, offsets [S+1] i64, cloud_ids [B] i64, labels
+    [sum P] i32 or None; indices [B,N] i32 (given source positions) or None (in-kernel draws keyed
+    by `seed`). -> (pc [B,3,N], sn [B,3,N], seg [B,N] i64 or None)."""
+    _chk(data, "data", torch.float32)
+    _chk(offsets, "offsets", torch.int64)
+    _chk(cloud_ids, "cloud_ids", torch.int64)
+    _chk(labels, "labels", torch.int32, optional=True)
+    _chk(indices, "indices", torch.int32, optional=True)
+    if data.dim() != 2 or data.shape[1] != 6 or offsets.dim() != 1 or cloud_ids.dim() != 1:
+        raise RuntimeError("sample_points: expected data [sum P, 6], offsets [S+1], cloud_ids [B]; "
+                           "got %s %s %s" % (tuple(data.shape), tuple(offsets.shape),
+                                             tuple(cloud_ids.shape)))
+    B, N = cloud_ids.shape[0], int(N)
+    if labels is not None and labels.shape != (data.shape[0],):
+        raise RuntimeError("sample_points: labels must have shape (%d,)" % data.shape[0])
+    if indices is not None and tuple(indices.shape) != (B, N):
+        raise RuntimeError("sample_points: indices must have shape %s" % ((B, N),))
+    dev = data.device
+    with torch.cuda.device(dev):
+        pc = torch.empty((B, 3, N), dtype=torch.float32, device=dev)
+        sn = torch.empty((B, 3, N), dtype=torch.float32, device=dev)
+        seg = torch.empty((B, N), dtype=torch.int64, device=dev) if labels is not None else None
+        _call("sonet_sample_points_f32", _C.ptr(data), _C.ptr(offsets), offsets.shape[0] - 1,
+              _C.ptr(labels), _C.ptr(cloud_ids), B, N, int(max_P), int(rule), _C.ptr(indices),
+              int(seed) & (2 ** 64 - 1), _C.ptr(pc), _C.ptr(sn), _C.ptr(seg), _stream(data))
+    return pc, sn, seg
+
+
 def som_decenter(x, sn, cluster_mean, min_idx_i32, k, want_centers=False):
     """-> (x_aug [B,3(+3),kN], centers [B,3,kN] or None)."""
     _chk(x, "x", torch.float32)
