@@ -36,7 +36,9 @@ def _stream(t):
 
 
 # activation codes of the C-ABI (SONET_ACT_*, include/sonet_b200.h)
-ACT_NONE, ACT_RELU, ACT_ELU = 0, 1, 2
+ACT_NONE = _C.CONSTANTS["SONET_ACT_NONE"]
+ACT_RELU = _C.CONSTANTS["SONET_ACT_RELU"]
+ACT_ELU = _C.CONSTANTS["SONET_ACT_ELU"]
 _ACT_NAMES = {None: ACT_NONE, "relu": ACT_RELU, "elu": ACT_ELU}
 
 
@@ -186,8 +188,9 @@ def augment(pc, sn, som, rot1=None, rot2=None, scale=None, shift=None, jitter_pc
 
 
 # point-selection rules of the C-ABI (SONET_SAMPLE_*, include/sonet_b200.h)
-SAMPLE_SUBSET, SAMPLE_FILL = 0, 1
-SAMPLE_MAX_P = 65536      # largest cloud of the in-kernel draws
+SAMPLE_SUBSET = _C.CONSTANTS["SONET_SAMPLE_SUBSET"]
+SAMPLE_FILL = _C.CONSTANTS["SONET_SAMPLE_FILL"]
+SAMPLE_MAX_P = _C.CONSTANTS["SONET_SAMPLE_MAX_P"]      # largest cloud of the in-kernel draws
 
 
 def sample_points(data, offsets, cloud_ids, N, rule, max_P, labels=None, indices=None, seed=0):
@@ -356,7 +359,9 @@ def kcopy_mean(t, k):
 
 
 # reduction codes of sonet_instance_norm_f32 (SONET_REDUCE_*, include/sonet_b200.h)
-REDUCE_NONE, REDUCE_KCOPY_MEAN, REDUCE_GROUP_MAX = 0, 1, 2
+REDUCE_NONE = _C.CONSTANTS["SONET_REDUCE_NONE"]
+REDUCE_KCOPY_MEAN = _C.CONSTANTS["SONET_REDUCE_KCOPY_MEAN"]
+REDUCE_GROUP_MAX = _C.CONSTANTS["SONET_REDUCE_GROUP_MAX"]
 
 
 def instance_norm(z, gamma, beta, eps, act, kcopy=None, group_max=None, save_stats=False, out=None):
@@ -888,7 +893,9 @@ def som_sort_decenter(x, sn, cluster_mean, min_idx_i32, count, k):
 
 _MAX_SMEM = {}
 # sonet_som_group_mode results (include/sonet_b200.h)
-SOM_GROUP_NONE, SOM_GROUP_UNSTAGED, SOM_GROUP_STAGED = 0, 1, 2
+SOM_GROUP_NONE = _C.CONSTANTS["SONET_SOM_GROUP_NONE"]
+SOM_GROUP_UNSTAGED = _C.CONSTANTS["SONET_SOM_GROUP_UNSTAGED"]
+SOM_GROUP_STAGED = _C.CONSTANTS["SONET_SOM_GROUP_STAGED"]
 
 
 def som_group_mode(N, M, k, with_sn, dev):

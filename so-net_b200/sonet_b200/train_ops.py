@@ -388,7 +388,7 @@ def _pack_groups_device(Wg):
     with torch.cuda.device(dev):
         blob = torch.empty(per * G, dtype=torch.uint8, device=dev)
         scale2 = torch.empty(2, dtype=torch.float32, device=dev)
-        part = torch.empty(256, dtype=torch.float32, device=dev)     # SONET_ABSMAX_SLOTS
+        part = torch.empty(_C.CONSTANTS["SONET_ABSMAX_SLOTS"], dtype=torch.float32, device=dev)
         ops._call("sonet_pointwise_tc_pack_groups_device", _C.ptr(Wg), G, Cout, Cin, _C.ptr(blob),
                   _C.ptr(scale2), _C.ptr(part), ops._stream(Wg), kernels=2 + G)
     return blob, per, scale2

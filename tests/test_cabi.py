@@ -157,37 +157,97 @@ def test_every_wrapper_call_names_a_bound_symbol_with_the_right_arity():
     assert len(seen) >= 25, sorted(seen)
 
 
+def _header_text():
+    text = open(os.path.join(ROOT, "include", "sonet_b200.h")).read()
+    return re.sub(r"/\*.*?\*/", " ", text, flags=re.S)          # strip comments
+
+
+def _header_prototypes():
+    """name -> (return type, parameter list) of every prototype in include/sonet_b200.h: this
+    test's own reading of the header, independent of the binding's parser."""
+    protos = {}
+    for ret, name, params in re.findall(r"^[ \t]*(\w[\w \t*]*?)\s*\b(sonet_\w+)\s*\(([^;{]*?)\)\s*;",
+                                        _header_text(), flags=re.M):
+        params = " ".join(params.split())
+        protos[name] = (" ".join(ret.split()),
+                        [] if params in ("", "void") else [q.strip() for q in params.split(",")])
+    return protos
+
+
+def _machine_type(name, q):
+    """The ctypes type a C declaration `q` (a parameter, or a return type) passes as."""
+    if re.fullmatch(r"const char\s*\*", q):
+        return ctypes.c_char_p
+    if "*" in q or "sonet_stream_t" in q:
+        return ctypes.c_void_p
+    if "unsigned long long" in q:
+        return ctypes.c_ulonglong
+    if "long long" in q:
+        return ctypes.c_longlong
+    if re.match(r"(const\s+)?double\b", q):
+        return ctypes.c_double
+    if re.match(r"(const\s+)?float\b", q):
+        return ctypes.c_float
+    assert re.match(r"(const\s+)?int\b", q), "%s: unhandled type %r" % (name, q)
+    return ctypes.c_int
+
+
 def test_ctypes_arity_matches_the_header_prototypes():
     """The ctypes argtypes of every symbol have as many entries as its prototype in
     include/sonet_b200.h has parameters (a mismatch corrupts the call frame silently)."""
-    import ctypes
-    import os
-    import re
-
     from sonet_b200 import _C
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    text = open(os.path.join(root, "include", "sonet_b200.h")).read()
-    text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)          # strip comments
-    protos = dict(re.findall(r"\b(sonet_\w+)\s*\(([^;{]*?)\)\s*;", text, flags=re.S))
-    assert set(protos) == set(_C._SIGNATURES)
-    for name, params in protos.items():
-        params = " ".join(params.split())
-        plist = [] if params in ("", "void") else [q.strip() for q in params.split(",")]
+    protos = _header_prototypes()
+    assert set(protos) == set(_C._SIGNATURES) == set(declared_symbols())
+    for name, (_, plist) in protos.items():
         sig = _C._SIGNATURES[name]
         assert len(plist) == len(sig), "%s: header %d parameters, ctypes %d" % (name, len(plist),
                                                                               len(sig))
         for q, ct in zip(plist, sig):           # and the same machine type, parameter by parameter
-            if "*" in q or "sonet_stream_t" in q:
-                want = ctypes.c_void_p
-            elif "unsigned long long" in q:
-                want = ctypes.c_ulonglong
-            elif "long long" in q:
-                want = ctypes.c_longlong
-            elif re.match(r"(const\s+)?double\b", q):
-                want = ctypes.c_double
-            elif re.match(r"(const\s+)?float\b", q):
-                want = ctypes.c_float
-            else:
-                assert re.match(r"(const\s+)?int\b", q), "%s: unhandled parameter type %r" % (name, q)
-                want = ctypes.c_int
+            want = _machine_type(name, q)
             assert ct is want, "%s: parameter %r is bound as %s" % (name, q, ct.__name__)
+
+
+def test_ctypes_restypes_match_the_header_prototypes(lib_built):
+    """Every bound entry returns the type its prototype declares: a `long long` size query read
+    as a C int would come back truncated, a `const char*` as a number."""
+    from sonet_b200 import _C
+    lib = _C.lib()
+    for name, (ret, _) in _header_prototypes().items():
+        restype = getattr(lib, name).restype
+        assert restype is _machine_type(name, ret), "%s: returns %r, bound as %s" % (
+            name, ret, restype.__name__)
+    assert lib.sonet_wgrad_kpad(1 << 16, 1 << 16, 1) == 1 << 32         # not truncated to 32 bits
+
+
+def test_header_constants():
+    """Every `#define SONET_<NAME> <int>` of the header is in _C.CONSTANTS with its value, and the
+    Python names of the codes ops.py passes to the library hold the header's values."""
+    from sonet_b200 import _C, ops
+    defines = re.findall(r"^\s*#define\s+(SONET_\w+)\s+\(?\s*(-?\d+)\s*\)?\s*$", _header_text(),
+                         flags=re.M)
+    want = {n: int(v) for n, v in defines}
+    assert len(want) >= 17 and want["SONET_ERR_BAD_ARG"] == -1
+    assert _C.CONSTANTS == want
+    for group, names in (("ACT", ("NONE", "RELU", "ELU")), ("SAMPLE", ("SUBSET", "FILL", "MAX_P")),
+                         ("REDUCE", ("NONE", "KCOPY_MEAN", "GROUP_MAX")),
+                         ("SOM_GROUP", ("NONE", "UNSTAGED", "STAGED"))):
+        for n in names:
+            assert getattr(ops, "%s_%s" % (group, n)) == want["SONET_%s_%s" % (group, n)], (group, n)
+
+
+def test_binding_parser_refuses_unknown_types():
+    """The binding's header parser binds only types with an exact ctypes twin: anything else
+    raises naming the entry and the parameter; `(void)` and `()` take no arguments."""
+    from sonet_b200 import _C
+    with pytest.raises(RuntimeError, match=r"sonet_x: parameter 'size_t n'"):
+        _C.parse_header("int sonet_x(const float* a,\n            size_t n, sonet_stream_t s);")
+    with pytest.raises(RuntimeError, match=r"sonet_y: return type 'unsigned'"):
+        _C.parse_header("unsigned sonet_y(int n);")
+    sigs, res, consts = _C.parse_header(
+        "typedef void* sonet_stream_t; /* sonet_w(x) */\n#define SONET_A (-4)\n#define SONET_B 7\n"
+        "long long sonet_v(void);\nint sonet_u();\nconst char* sonet_t(unsigned long long s,\n"
+        "                  double d, float f, int** p);\n")
+    assert sigs == {"sonet_v": [], "sonet_u": [],
+                    "sonet_t": [ctypes.c_ulonglong, ctypes.c_double, ctypes.c_float, ctypes.c_void_p]}
+    assert res == {"sonet_v": ctypes.c_longlong, "sonet_u": ctypes.c_int, "sonet_t": ctypes.c_char_p}
+    assert consts == {"SONET_A": -4, "SONET_B": 7}
