@@ -340,6 +340,44 @@ int sonet_sample_points_f32(const float* data, const int64_t* offsets, int S, co
                             const int32_t* indices, unsigned long long seed, float* pc_out,
                             float* sn_out, int64_t* seg_out, sonet_stream_t stream);
 
+/* ---- area-weighted surface sampling of triangle meshes (data/sampler_matlab/sampler.m) ---------
+ * B meshes as ragged device arrays: verts [total_V, 3] f64 with v_off [B+1] i64 (mesh b's vertices
+ * are rows v_off[b]..v_off[b+1]), faces [total_F, 3] i32 with f_off [B+1] i64 (vertex indices local
+ * to the mesh; outside [0, V) they are clamped to [0, V-1]), mesh_ids [B] i64. Output out [B*N, 6]
+ * f32, point-major xyz | normal, mesh b owning rows b*N .. b*N+N-1; face_out [B*N] i32 (nullable):
+ * the mesh-local face of each point; area_out [B] f64 (nullable): each mesh's total area.
+ * Arithmetic is float64, explicitly rounded (no FMA), rounded to f32 once:
+ *   e1 = b - a, e2 = c - a, n = cross(e1, e2), |n| = sqrt((nx*nx + ny*ny) + nz*nz),
+ *   area = 0.5 * |n|, normal = n / |n|; weight = area, or 0 when the area is 0 or not finite.
+ * CDF: every sum sequential from +0, blocked by SONET_MESH_RUN faces per run and SONET_MESH_TILE
+ * faces per tile (both starting at face 0 of the mesh): run[f] = inclusive sum of the weights of
+ * f's run up to f; roff = sum of the totals of the preceding runs of f's tile; toff = sum of the
+ * totals of the preceding tiles; cdf[f] = toff + (roff + run[f]); total = cdf[F-1].
+ * Per sample with draws (r, u, v) in [0,1): t = r * total, face = the first f with cdf[f] > t,
+ * clamped to the last face of positive weight; if u + v > 1 then u = 1-u, v = 1-v; the point is
+ * (a + u*e1) + v*e2, uniform on the triangle (sampler.m:35's a + u*b + v*c is not a point of the
+ * triangle and is not reproduced). draws [B*N, 3] f64 (DEVICE, nullable) are given (r, u, v);
+ * when NULL, Philox4x32-10 keyed by (seed, mesh_ids[b], sample) draws 53-bit uniforms, so a mesh's
+ * points do not depend on the batch it is sampled in.
+ * area_out[b] is the total, or NaN when a face's area is not finite (or the mesh exceeds 2^31-1
+ * faces or vertices); a mesh whose total is 0 or not finite writes NaN rows (face_out -1) and does
+ * not affect the other meshes. The entry takes sonet_mesh_sample_scratch_bytes(B, total_F) bytes
+ * of 256-byte aligned device scratch (the f64 CDF and per-tile and per-mesh state), allocates
+ * nothing, does not synchronise, and is deterministic. Fails with SONET_ERR_BAD_ARG before any
+ * CUDA call for B < 0, N outside [1, SONET_MESH_MAX_N], total_F or total_V outside [0, 2^40], a null
+ * v_off/f_off/mesh_ids/scratch/out, null verts (faces) with total_V (total_F) > 0, or too small or
+ * misaligned a scratch; B = 0 then returns without a launch. The size query returns -1 for bad
+ * arguments. */
+#define SONET_MESH_RUN 8
+#define SONET_MESH_TILE 2048
+#define SONET_MESH_MAX_N 16777216
+long long sonet_mesh_sample_scratch_bytes(int B, long long total_F);
+int sonet_mesh_sample_f32(const double* verts, const int64_t* v_off, long long total_V,
+                          const int32_t* faces, const int64_t* f_off, long long total_F,
+                          const int64_t* mesh_ids, int B, int N, const double* draws,
+                          unsigned long long seed, void* scratch, long long scratch_bytes, float* out,
+                          int32_t* face_out, double* area_out, sonet_stream_t stream);
+
 /* ---- a-4/a-5/a-8/a-9/a-10: point-wise shared MLP layer (1x1 conv + folded BN + ReLU) ---------
  * Replaces EquivariantLayer.forward / MyConv2d(1x1).forward in eval mode
  * (models/layers.py:203-210, 282-296): out[b,co,p] = act(scale[co]*sum_ci W[co,ci]*X[b,ci,p] +

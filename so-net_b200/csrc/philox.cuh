@@ -1,7 +1,8 @@
 // philox.cuh — the library's one counter-based generator: Philox4x32-10 (Salmon et al., SC'11).
 // No state to store: the 128-bit counter names the draw, the 64-bit seed is the key. Used by the
-// in-kernel jitter of augment.cu and the in-kernel point selection of sample_points.cu, which keep
-// their streams apart through a stream tag in counter word 2 (augment: 0..2, sample_points: 3..4).
+// in-kernel jitter of augment.cu, the in-kernel point selection of sample_points.cu and the surface
+// draws of mesh_sample.cu, which keep their streams apart through a stream tag in counter word 2
+// (augment: 0..2, sample_points: 3..4, mesh_sample: 5..6).
 #pragma once
 #include <stdint.h>
 

@@ -190,6 +190,25 @@ class DeviceDataset:
         self.seg = None if seg is None else torch.from_numpy(
             np.concatenate([np.asarray(s, dtype=np.int32) for s in seg])).to(self.device)
 
+    @classmethod
+    def from_device(cls, data, offsets, labels, som_nodes):
+        """A dataset from tensors already in device memory (meshes.build_dataset's), without a host
+        round trip: data [sum P, 6] f32, offsets [S+1] i64, labels [S] i64, som_nodes [S, 3, M]
+        f32, all on one device; no part labels. counts are read back once (S integers)."""
+        ds = cls.__new__(cls)
+        ds.device = data.device
+        ds.counts = np.diff(offsets.cpu().numpy()).astype(np.int64)
+        if len(ds.counts) == 0 or (ds.counts <= 0).any():
+            raise ValueError("DeviceDataset: every cloud needs at least one point")
+        ds.max_P = int(ds.counts.max())
+        ds.node_num = som_nodes.shape[2]
+        ds.data = data.float().contiguous()
+        ds.offsets = offsets.contiguous()
+        ds.labels = labels.to(data.device, torch.int64).contiguous()
+        ds.som_nodes = som_nodes.float().contiguous()
+        ds.seg = None
+        return ds
+
     def __len__(self):
         return len(self.counts)
 

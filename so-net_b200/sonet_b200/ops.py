@@ -223,6 +223,47 @@ def sample_points(data, offsets, cloud_ids, N, rule, max_P, labels=None, indices
     return pc, sn, seg
 
 
+MESH_MAX_N = _C.CONSTANTS["SONET_MESH_MAX_N"]      # largest sample count per mesh
+
+
+def mesh_sample(verts, v_off, faces, f_off, mesh_ids, N, draws=None, seed=0, want_faces=False,
+                want_area=False):
+    """Area-weighted surface sampling of B meshes (csrc/mesh_sample.cu): verts [sum V, 3] f64 with
+    v_off [B+1] i64, faces [sum F, 3] i32 (mesh-local vertex indices) with f_off [B+1] i64,
+    mesh_ids [B] i64 (the key of the in-kernel draws); draws [B*N, 3] f64 (r, u, v) or None.
+    -> (out [B*N, 6] f32 xyz | normal, face [B*N] i32 or None, area [B] f64 or None); a mesh
+    with no face of positive finite area gets NaN rows."""
+    _chk(verts, "verts", torch.float64)
+    _chk(v_off, "v_off", torch.int64)
+    _chk(faces, "faces", torch.int32)
+    _chk(f_off, "f_off", torch.int64)
+    _chk(mesh_ids, "mesh_ids", torch.int64)
+    _chk(draws, "draws", torch.float64, optional=True)
+    B, N = mesh_ids.shape[0] if mesh_ids.dim() == 1 else -1, int(N)
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3 \
+            or B < 0 or tuple(v_off.shape) != (B + 1,) or tuple(f_off.shape) != (B + 1,):
+        raise RuntimeError("mesh_sample: expected verts [V,3], faces [F,3], mesh_ids [B], v_off and "
+                           "f_off [B+1]; got %s %s %s %s %s" % (
+                               tuple(verts.shape), tuple(faces.shape), tuple(mesh_ids.shape),
+                               tuple(v_off.shape), tuple(f_off.shape)))
+    if draws is not None and tuple(draws.shape) != (B * N, 3):
+        raise RuntimeError("mesh_sample: draws must have shape %s" % ((B * N, 3),))
+    dev = mesh_ids.device
+    total_F = faces.shape[0]
+    with torch.cuda.device(dev):
+        nbytes = int(_C.lib().sonet_mesh_sample_scratch_bytes(B, total_F))
+        _C.check(0 if nbytes >= 0 else nbytes, "sonet_mesh_sample_scratch_bytes")
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        out = torch.empty((B * N, 6), dtype=torch.float32, device=dev)
+        face = torch.empty((B * N,), dtype=torch.int32, device=dev) if want_faces else None
+        area = torch.empty((B,), dtype=torch.float64, device=dev) if want_area else None
+        _call("sonet_mesh_sample_f32", _C.ptr(verts), _C.ptr(v_off), verts.shape[0], _C.ptr(faces),
+              _C.ptr(f_off), total_F, _C.ptr(mesh_ids), B, N, _C.ptr(draws),
+              int(seed) & (2 ** 64 - 1), _C.ptr(scratch), nbytes, _C.ptr(out), _C.ptr(face),
+              _C.ptr(area), _stream(mesh_ids), kernels=4)
+    return out, face, area
+
+
 def som_decenter(x, sn, cluster_mean, min_idx_i32, k, want_centers=False):
     """-> (x_aug [B,3(+3),kN], centers [B,3,kN] or None)."""
     _chk(x, "x", torch.float32)

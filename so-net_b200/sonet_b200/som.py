@@ -194,3 +194,70 @@ class BatchSOM():
         a = ops.som_assign(x.detach().contiguous(), self.node.contiguous(), 1, want_stats=False)
         self.last_assignment = a
         return ops.som_mask(a["min_idx_i32"], M).float(), a["row_max"].float()
+
+
+class SOM():
+    """The single-cloud SOM of util/som.py:17-173, the one data/build_som/save_som.ipynb trains per
+    shape: node [dim, M], node_init(), query(x), batch_update(x, iteration) and optimize(x) for a
+    cloud x [dim, N]. It is a BatchSOM with one cloud, so every call runs the sm_90a SOM kernels
+    and optimize() equals BatchSOM.optimize of the same cloud bit for bit. The nodes live on
+    cuda:gpu_id; gpu_id < 0 (the reference's CPU mode) or a bool (the notebook passes True) selects
+    the current CUDA device, since there is no CPU path. Only dim = 3 has kernels."""
+
+    def __init__(self, rows=4, cols=4, dim=3, gpu_id=-1):
+        if dim != 3:
+            raise RuntimeError("sonet_b200.SOM: dim=%d has no kernel (3 only)" % dim)
+        if isinstance(gpu_id, bool) or gpu_id is None or gpu_id < 0:
+            gpu_id = torch.cuda.current_device() if torch.cuda.is_available() else 0
+        self._batch = BatchSOM(rows, cols, dim, gpu_id, 1)
+        self.rows, self.cols, self.dim, self.node_num = rows, cols, dim, rows * cols
+        self.sigma = self._batch.sigma
+        self.learning_rate = self._batch.learning_rate
+        self.max_iteration = self._batch.max_iteration
+        self.gpu_id = gpu_id
+        self.device = self._batch.device
+        self.node_idx_list = torch.arange(self.node_num, dtype=torch.float32, device=self.device)
+        self.node_init()
+
+    @property
+    def node(self):
+        """[dim, M] float32 (a view of the one cloud's nodes)."""
+        return self._batch.node[0]
+
+    @property
+    def node_init_value(self):
+        return self._batch.node_init_value
+
+    @property
+    def init_weighting_matrix(self):
+        return self._batch.init_weighting_matrix
+
+    def node_init(self):
+        self._batch.node_init(1)
+
+    def get_weighting_matrix(self, sigma):
+        return self._batch.get_weighting_matrix(sigma)
+
+    def idx2multi(self, i):
+        return self._batch.idx2multi(i)
+
+    def _cloud(self, x):
+        if x.dim() != 2 or x.size(0) != self.dim:
+            raise RuntimeError("sonet_b200.SOM: x must be [%d, N], got %s" % (self.dim, tuple(x.shape)))
+        return x.to(self.device, torch.float32).unsqueeze(0)
+
+    def query(self, x):
+        """util/som.py:78-100: (mask [N, M] float, mask_row_max [M] float)."""
+        mask, row_max = self._batch.query(self._cloud(x))
+        return mask[0], row_max[0]
+
+    def batch_update(self, x, iteration):
+        """One iteration at the rates of util/som.py:102-110."""
+        decay = 1 + 2 * iteration / self.max_iteration
+        self._batch.batch_size = 1
+        self._batch.batch_update(self._cloud(x), self.learning_rate / decay, self.sigma / decay)
+
+    def optimize(self, x):
+        """util/som.py:168-173: potential-field start, max_iteration/3 iterations at the initial
+        rates, then max_iteration decaying ones, in one kernel launch."""
+        self._batch.optimize(self._cloud(x))
