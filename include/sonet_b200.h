@@ -194,6 +194,39 @@ int sonet_bn_train_backward_f32(const float* dy, const float* x, const float* me
                                 const float* invstd, const float* gamma, const float* beta, int B,
                                 int C, int P, int relu, double* partial, float* dx, float* dgamma,
                                 float* dbeta, sonet_stream_t stream);
+/* Synchronised BatchNorm for data-parallel training: the batch statistics of a global batch of Bg
+ * clouds sharded over ranks, bit-identical at every sharding. The existing entries above sum strided
+ * groups of clouds whose stride depends on B and the SM count; these route every sum through
+ * per-cloud records instead, which depend on nothing but the cloud's own values.
+ *   sonet_bn_cloud_partials_f32: one fp64 record per (b, c) of x [B,C,P], in a fixed order inside the
+ *     cloud (P == 1: a thread per record; P <= 1024: a warp; longer: a 256-thread CTA).
+ *       backward == 0: rec [B,C,SONET_BN_REC_FWD] = {pivot = x[b,c,0], sum d, sum d*d}, d = x - pivot;
+ *         dy, mean, invstd, gamma, beta unused (may be null).
+ *       backward != 0: rec [B,C,SONET_BN_REC_BWD] = {sum g, sum g*xhat}, g and xhat as in
+ *         sonet_bn_train_backward_f32 (dy, x, mean, invstd required; gamma, beta nullable).
+ *   sonet_bn_sync_forward_f32: rec [Bg,C,3], the records of all Bg clouds in global order, folded in
+ *     ascending cloud order onto cloud 0's pivot p (S1 = sum_b sum d_b + P (p_b - p),
+ *     S2 = sum_b sum d_b^2 + 2 (p_b - p) sum d_b + P (p_b - p)^2) into the biased mean / var /
+ *     invstd over n = Bg*P values, then y = act(gamma*(x-mean)*invstd + beta) of the local x [B,C,P].
+ *   sonet_bn_sync_backward_f32: rec [Bg,C,2] in global order -> dbeta = sum g, dgamma = sum g*xhat
+ *     (ascending clouds: the same on every rank) and dx of the local x with 1/n = 1/(Bg*P).
+ * act: SONET_ACT_*. Fail with SONET_ERR_BAD_ARG before any CUDA call for a null pointer, B, C or Bg
+ * outside [1, 65535], B > Bg, P < 1 or an unknown activation code. No allocation, no atomics, no
+ * host synchronisation. */
+#define SONET_BN_REC_FWD 3
+#define SONET_BN_REC_BWD 2
+int sonet_bn_cloud_partials_f32(const float* x, const float* dy, const float* mean,
+                                const float* invstd, const float* gamma, const float* beta, int B,
+                                int C, int P, int act, int backward, double* rec,
+                                sonet_stream_t stream);
+int sonet_bn_sync_forward_f32(const double* rec, const float* x, const float* gamma,
+                              const float* beta, int Bg, int B, int C, int P, float eps, int act,
+                              float* y, float* mean, float* var, float* invstd,
+                              sonet_stream_t stream);
+int sonet_bn_sync_backward_f32(const double* rec, const float* dy, const float* x, const float* mean,
+                               const float* invstd, const float* gamma, const float* beta, int Bg,
+                               int B, int C, int P, int act, float* dx, float* dgamma, float* dbeta,
+                               sonet_stream_t stream);
 int sonet_index_max_backward_f32(const float* grad_out, const int32_t* idx, int B, int C, int N, int K,
                                  float* grad_data, sonet_stream_t stream);
 /* Instance normalisation, nn.InstanceNorm1d/2d(C, affine=True) with track_running_stats=False

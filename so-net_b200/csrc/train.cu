@@ -495,6 +495,164 @@ __global__ void __launch_bounds__(256)
        i += static_cast<long long>(gridDim.x) * blockDim.x)
     dWT[i] *= inv_c[i % Cout];
 }
+
+// ---- per-cloud BatchNorm records (synchronised BN of data-parallel training) -------------------------
+// Row r = b*C + c of x [B,C,P] gets one fp64 record whose value depends on that row alone: the row's
+// elements are summed in a fixed order chosen from P only (never from B, C or the SM count), so the
+// records of a cloud are the same bits whichever shard it lands in. Forward: {pivot = x[r,0], sum d,
+// sum d*d}, d = x - pivot exact in fp64 (the cancellation argument of bn_partial_kernel). Backward:
+// {sum g, sum g*xhat}, g as in bn_partial_kernel, each term accumulated in fp64.
+constexpr int BNC_WARP_P = 1024;           // rows up to this length: a warp per row, else a CTA
+
+template <bool BWD, int ACT>
+struct BncRow {
+  const float *xr, *gr;
+  float mu, is, ga, be;
+  double pivot;
+  __device__ __forceinline__ BncRow(const float* x, const float* dy, const float* mean,
+                                    const float* invstd, const float* gamma, const float* beta,
+                                    long long r, int C, int P) {
+    const int c = static_cast<int>(r % C);
+    xr = x + r * P;
+    gr = BWD ? dy + r * P : nullptr;
+    mu = BWD ? mean[c] : 0.f;
+    is = BWD ? invstd[c] : 1.f;
+    ga = BWD && gamma ? gamma[c] : 1.f;
+    be = BWD && beta ? beta[c] : 0.f;
+    pivot = BWD ? 0.0 : static_cast<double>(xr[0]);
+  }
+  __device__ __forceinline__ void add(int p, double& a0, double& a1) const {
+    if (BWD) {
+      const float xh = (xr[p] - mu) * is;
+      float g = gr[p];
+      if (ACT == SONET_ACT_ELU) g *= elu_grad(fmaf(ga, xh, be));
+      else if (ACT == SONET_ACT_RELU && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
+      a0 += static_cast<double>(g);
+      a1 = fma(static_cast<double>(g), static_cast<double>(xh), a1);
+    } else {
+      const double d = static_cast<double>(xr[p]) - pivot;
+      a0 += d;
+      a1 = fma(d, d, a1);
+    }
+  }
+  __device__ __forceinline__ void store(double* rec, long long r, double a0, double a1) const {
+    if (BWD) {
+      rec[r * SONET_BN_REC_BWD] = a0;
+      rec[r * SONET_BN_REC_BWD + 1] = a1;
+    } else {
+      rec[r * SONET_BN_REC_FWD] = pivot;
+      rec[r * SONET_BN_REC_FWD + 1] = a0;
+      rec[r * SONET_BN_REC_FWD + 2] = a1;
+    }
+  }
+};
+
+// P == 1 (MyLinear's [B,C,1] view): a thread per row, consecutive threads on consecutive channels
+template <bool BWD, int ACT>
+__global__ void __launch_bounds__(256)
+    bn_cloud_point_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                          const float* __restrict__ mean, const float* __restrict__ invstd,
+                          const float* __restrict__ gamma, const float* __restrict__ beta, long long R,
+                          int C, double* __restrict__ rec) {
+  const long long r = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, 1);
+  double a0 = 0.0, a1 = 0.0;
+  row.add(0, a0, a1);
+  row.store(rec, r, a0, a1);
+}
+
+// 1 < P <= BNC_WARP_P: warp w of the CTA owns row 8*blockIdx.x + w; lanes take p = lane, lane+32, ...
+template <bool BWD, int ACT>
+__global__ void __launch_bounds__(256)
+    bn_cloud_warp_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                         const float* __restrict__ mean, const float* __restrict__ invstd,
+                         const float* __restrict__ gamma, const float* __restrict__ beta, long long R,
+                         int C, int P, double* __restrict__ rec) {
+  const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (r >= R) return;                                   // warp-uniform
+  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, P);
+  double a0 = 0.0, a1 = 0.0;
+  for (int p = lane; p < P; p += 32) row.add(p, a0, a1);
+  a0 = in_warp_sum(a0);
+  a1 = in_warp_sum(a1);
+  if (lane == 0) row.store(rec, r, a0, a1);
+}
+
+// P > BNC_WARP_P: CTA blockIdx.x owns row r; thread t takes p = t, t+256, ..., then the warp
+// butterfly and the 8 warp sums in ascending order
+template <bool BWD, int ACT>
+__global__ void __launch_bounds__(256)
+    bn_cloud_cta_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                        const float* __restrict__ mean, const float* __restrict__ invstd,
+                        const float* __restrict__ gamma, const float* __restrict__ beta, int C, int P,
+                        double* __restrict__ rec) {
+  static_assert(IN_THREADS == 256, "in_block_sum sums 8 warps");
+  __shared__ double red[IN_THREADS / 32];
+  const long long r = blockIdx.x;
+  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, P);
+  double a0 = 0.0, a1 = 0.0;
+  for (int p = threadIdx.x; p < P; p += IN_THREADS) row.add(p, a0, a1);
+  a0 = in_block_sum(a0, red);
+  a1 = in_block_sum(a1, red);
+  if (threadIdx.x == 0) row.store(rec, r, a0, a1);
+}
+
+template <bool BWD, int ACT>
+static void launch_bn_cloud(const float* x, const float* dy, const float* mean, const float* invstd,
+                            const float* gamma, const float* beta, long long R, int C, int P,
+                            double* rec, cudaStream_t st) {
+  if (P == 1)
+    bn_cloud_point_kernel<BWD, ACT><<<static_cast<unsigned>((R + 255) / 256), 256, 0, st>>>(
+        x, dy, mean, invstd, gamma, beta, R, C, rec);
+  else if (P <= BNC_WARP_P)
+    bn_cloud_warp_kernel<BWD, ACT><<<static_cast<unsigned>((R + 7) / 8), 256, 0, st>>>(
+        x, dy, mean, invstd, gamma, beta, R, C, P, rec);
+  else
+    bn_cloud_cta_kernel<BWD, ACT><<<static_cast<unsigned>(R), IN_THREADS, 0, st>>>(
+        x, dy, mean, invstd, gamma, beta, C, P, rec);
+}
+
+// the forward records of Bg clouds, ascending, onto cloud 0's pivot; then bn_stats_final_kernel's
+// statistics. Shifting record b by s = p_b - p (exact: both are fp32 values) is the identity
+// sum (x - p) = sum d_b + P s, sum (x - p)^2 = sum d_b^2 + 2 s sum d_b + P s^2.
+__global__ void bn_sync_stats_kernel(const double* __restrict__ rec, int Bg, int C, int P, float eps,
+                                     float* __restrict__ mean, float* __restrict__ var,
+                                     float* __restrict__ invstd) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const double p = rec[static_cast<size_t>(c) * SONET_BN_REC_FWD];
+  const double nb = static_cast<double>(P);
+  double s1 = 0.0, s2 = 0.0;
+  for (int b = 0; b < Bg; ++b) {
+    const double* q = rec + (static_cast<size_t>(b) * C + c) * SONET_BN_REC_FWD;
+    const double s = q[0] - p;
+    s1 += q[1] + nb * s;
+    s2 += q[2] + 2.0 * s * q[1] + nb * s * s;
+  }
+  const double n = static_cast<double>(Bg) * P;
+  const double md = s1 / n;                                        // mean - pivot
+  double v = s2 / n - md * md;
+  if (v < 0.0) v = 0.0;
+  mean[c] = static_cast<float>(p + md);
+  var[c] = static_cast<float>(v);
+  invstd[c] = static_cast<float>(1.0 / sqrt(v + static_cast<double>(eps)));
+}
+
+__global__ void bn_sync_bwd_final_kernel(const double* __restrict__ rec, int Bg, int C,
+                                         float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double s0 = 0.0, s1 = 0.0;
+  for (int b = 0; b < Bg; ++b) {
+    const double* q = rec + (static_cast<size_t>(b) * C + c) * SONET_BN_REC_BWD;
+    s0 += q[0];
+    s1 += q[1];
+  }
+  dbeta[c] = static_cast<float>(s0);
+  dgamma[c] = static_cast<float>(s1);
+}
 }  // namespace sonet
 
 static int bn_splits(int B, int C) {
@@ -555,6 +713,71 @@ extern "C" int sonet_bn_train_backward_f32(const float* dy, const float* x, cons
     bn_bwd_apply_kernel<false><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
                                                      relu, inv_n, dx);
   return check_launch("bn_train_backward");
+}
+
+extern "C" int sonet_bn_cloud_partials_f32(const float* x, const float* dy, const float* mean,
+                                           const float* invstd, const float* gamma, const float* beta,
+                                           int B, int C, int P, int act, int backward, double* rec,
+                                           sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(act, "bn_cloud_partials");
+  SONET_REQUIRE(B >= 1 && C >= 1 && P >= 1 && B <= 65535 && C <= 65535,
+                "bn_cloud_partials: bad dims B=%d C=%d P=%d", B, C, P);
+  SONET_REQUIRE(x && rec && (!backward || (dy && mean && invstd)), "bn_cloud_partials: null pointer");
+  const long long R = static_cast<long long>(B) * C;
+  SONET_REQUIRE(R < (1LL << 31), "bn_cloud_partials: too many rows B*C=%lld", R);
+  cudaStream_t st = as_stream(stream);
+  if (!backward)
+    launch_bn_cloud<false, SONET_ACT_NONE>(x, nullptr, nullptr, nullptr, nullptr, nullptr, R, C, P, rec, st);
+  else if (act == SONET_ACT_ELU)
+    launch_bn_cloud<true, SONET_ACT_ELU>(x, dy, mean, invstd, gamma, beta, R, C, P, rec, st);
+  else if (act == SONET_ACT_RELU)
+    launch_bn_cloud<true, SONET_ACT_RELU>(x, dy, mean, invstd, gamma, beta, R, C, P, rec, st);
+  else
+    launch_bn_cloud<true, SONET_ACT_NONE>(x, dy, mean, invstd, gamma, beta, R, C, P, rec, st);
+  return check_launch("bn_cloud_partials");
+}
+
+extern "C" int sonet_bn_sync_forward_f32(const double* rec, const float* x, const float* gamma,
+                                         const float* beta, int Bg, int B, int C, int P, float eps,
+                                         int act, float* y, float* mean, float* var, float* invstd,
+                                         sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(act, "bn_sync_forward");
+  SONET_REQUIRE(B >= 1 && C >= 1 && P >= 1 && Bg >= B && Bg <= 65535 && C <= 65535,
+                "bn_sync_forward: bad dims Bg=%d B=%d C=%d P=%d", Bg, B, C, P);
+  SONET_REQUIRE(rec && x && y && mean && var && invstd, "bn_sync_forward: null pointer");
+  cudaStream_t st = as_stream(stream);
+  bn_sync_stats_kernel<<<(C + 127) / 128, 128, 0, st>>>(rec, Bg, C, P, eps, mean, var, invstd);
+  const dim3 grid((P + 1023) / 1024, C, B);
+  if (act == SONET_ACT_ELU)
+    bn_apply_kernel<true><<<grid, 256, 0, st>>>(x, mean, invstd, gamma, beta, C, P, 0, y);
+  else
+    bn_apply_kernel<false><<<grid, 256, 0, st>>>(x, mean, invstd, gamma, beta, C, P, act, y);
+  return check_launch("bn_sync_forward");
+}
+
+extern "C" int sonet_bn_sync_backward_f32(const double* rec, const float* dy, const float* x,
+                                          const float* mean, const float* invstd, const float* gamma,
+                                          const float* beta, int Bg, int B, int C, int P, int act,
+                                          float* dx, float* dgamma, float* dbeta, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(act, "bn_sync_backward");
+  SONET_REQUIRE(B >= 1 && C >= 1 && P >= 1 && Bg >= B && Bg <= 65535 && C <= 65535,
+                "bn_sync_backward: bad dims Bg=%d B=%d C=%d P=%d", Bg, B, C, P);
+  SONET_REQUIRE(rec && dy && x && mean && invstd && dx && dgamma && dbeta,
+                "bn_sync_backward: null pointer");
+  cudaStream_t st = as_stream(stream);
+  bn_sync_bwd_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(rec, Bg, C, dgamma, dbeta);
+  const dim3 grid((P + 1023) / 1024, C, B);
+  const float inv_n = static_cast<float>(1.0 / (static_cast<double>(Bg) * P));
+  if (act == SONET_ACT_ELU)
+    bn_bwd_apply_kernel<true><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
+                                                    0, inv_n, dx);
+  else
+    bn_bwd_apply_kernel<false><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
+                                                     act, inv_n, dx);
+  return check_launch("bn_sync_backward");
 }
 
 extern "C" int sonet_instance_norm_f32(const float* z, const float* gamma, const float* beta, int B,

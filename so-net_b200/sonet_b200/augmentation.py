@@ -212,7 +212,7 @@ class DeviceDataset:
     def __len__(self):
         return len(self.counts)
 
-    def batch(self, index, opt, train, rng=None, seed=0, host_noise=False):
+    def batch(self, index, opt, train, rng=None, seed=0, host_noise=False, shard=None):
         """The collated batch of the loader `opt.dataset` selects (autoencoder/train.py:25-36) for
         the clouds `index`, ready for Model.set_input(*...):
           modelnet / shrec: (pc, sn, label, som_node, som_knn_I)        N distinct points per cloud
@@ -221,7 +221,15 @@ class DeviceDataset:
         host_noise=True draws everything from `rng` in the loader's per-item order (the choice of
         item b, then item b's augmentation, then item b+1) and reproduces the loader bit for bit;
         host_noise=False draws the choice and the jitter in the kernels (keyed by `seed`) and only
-        the per-cloud scalars from `rng`."""
+        the per-cloud scalars from `rng`.
+        shard=(rank, world): rows shard_bounds(len(index), rank, world) of the batch the same call
+        returns without it (dist.DataParallelTraining's shard). The whole batch is drawn and sliced,
+        so every rank must pass the same index, seed and identically seeded `rng`."""
+        if shard is not None:
+            from .dist import shard_bounds
+            lo, hi = shard_bounds(len(np.asarray(index).reshape(-1)), *shard)
+            full = self.batch(index, opt, train, rng=rng, seed=seed, host_noise=host_noise)
+            return tuple(t[lo:hi] for t in full)
         if opt.dataset in ("modelnet", "shrec"):
             rule = ops.SAMPLE_SUBSET
         elif opt.dataset == "shapenet":

@@ -69,6 +69,11 @@ class _MomentumDecayBatchNorm(_BatchNorm):
         if epoch is not None and epoch >= 1 and step is not None and step > 0:
             self.momentum = max(self.momentum_original * (self.momentum_decay ** (epoch // step)),
                                 0.01)
+        if self.training and train_ops.EXCHANGE is not None:
+            # data-parallel training synchronises the BatchNorms on the train kernels only; this
+            # one would normalise each rank's shard by its own statistics
+            raise RuntimeError("a data-parallel train step reached a BatchNorm outside the train "
+                               "kernels (train_ops.norm_act_train)")
         return F.batch_norm(input, self.running_mean, self.running_var, self.weight, self.bias,
                             self.training, self.momentum, self.eps)
 
@@ -379,6 +384,15 @@ class MyConv2d(_PointwiseConvBase):
             nn.init.ones_(self.norm.weight)
             nn.init.zeros_(self.norm.bias)
 
+    def _sync_norm(self, x):
+        """A train step under data-parallel training (train_ops.EXCHANGE installed) of a layer the
+        train kernels do not cover (the decoder's 3x3 convolutions below train_ops.UPCONV_MIN_HW):
+        its BatchNorm and activation still run on train_ops.norm_act_train, which synchronises the
+        statistics over the ranks. Single-process training keeps the PyTorch composition."""
+        return (train_ops.EXCHANGE is not None and self.normalization == 'batch' and self.training
+                and torch.is_grad_enabled() and x.is_cuda and x.dtype == torch.float32
+                and x.dim() == 4 and self.activation in KERNEL_ACTIVATIONS)
+
     def forward(self, x, epoch=None):
         if _fast_ok(self, x) and x.dim() == 4 and self._fast_eligible():
             B, C, H, W = x.shape
@@ -394,6 +408,10 @@ class MyConv2d(_PointwiseConvBase):
         # backward — cuDNN's default TF32 convolution is ~1e-3 relative, outside the 1e-4 parity
         # bar of the reference's fp32 math
         x = train_ops.conv_strict(self.conv, x)
+        if self._sync_norm(x):
+            B, C, H, W = x.shape
+            y = train_ops.norm_act_train(x.reshape(B, C, H * W), self.norm, self.activation, epoch)
+            return y.view(B, C, H, W)
         if self.normalization == 'batch':
             x = self.norm(x, epoch)
         elif self.normalization is not None:

@@ -7,7 +7,8 @@ models/networks.py:185).
                   (weights / activations packed on the device each step; gradients pre-scaled by a
                   power of two before the fp16 hi/lo split)
     BNActTrain    batch-statistics BatchNorm + ReLU / ELU / none, forward and backward, fused elementwise passes
-                  and two-stage deterministic reductions
+                  and two-stage deterministic reductions; with EXCHANGE installed (data-parallel
+                  training) the per-cloud route, synchronised over the ranks
     InstanceNormActTrain  instance norm + ReLU / ELU / none: the instance-norm kernel forward, the
                   BN backward on the [1, B*C, P] view
     UpConvTC      nearest x2 up-sampling + 3x3 conv (pad 1) as four parity GEMMs over the
@@ -39,12 +40,70 @@ def _scratch(dev, n, dtype, cache={}):
     return buf
 
 
+# The BatchNorm exchange of data-parallel training (dist.DataParallelTraining), or None. While one is
+# installed, BNActTrain takes the per-cloud route: the records of the local clouds, gathered along the
+# cloud axis by EXCHANGE.gather(rec) -> [Bg, C, k] in global cloud order, then folded in that order.
+# EXCHANGE.global_rows(B) is the global batch Bg of a local batch of B clouds.
+EXCHANGE = None
+
+
+def _bn_sync_forward(x, gamma, beta, eps, act, ex):
+    B, C, P = x.shape
+    Bg = ex.global_rows(B)
+    dev = x.device
+    with torch.cuda.device(dev):
+        y = torch.empty_like(x)
+        mean = torch.empty(C, dtype=torch.float32, device=dev)
+        var = torch.empty(C, dtype=torch.float32, device=dev)
+        invstd = torch.empty(C, dtype=torch.float32, device=dev)
+        rec = torch.empty((B, C, _C.CONSTANTS["SONET_BN_REC_FWD"]), dtype=torch.float64, device=dev)
+        ops._call("sonet_bn_cloud_partials_f32", _C.ptr(x), None, None, None, None, None, B, C, P,
+                  ops.act_code(act), 0, _C.ptr(rec), ops._stream(x))
+        rec = ex.gather(rec)
+        ops._call("sonet_bn_sync_forward_f32", _C.ptr(rec), _C.ptr(x), _C.ptr(gamma), _C.ptr(beta),
+                  Bg, B, C, P, float(eps), ops.act_code(act), _C.ptr(y), _C.ptr(mean), _C.ptr(var),
+                  _C.ptr(invstd), ops._stream(x), kernels=2)
+    return y, mean, var, invstd
+
+
+def _bn_sync_backward(dy, x, mean, invstd, gamma, beta, act, ex):
+    """dy is the gradient of this rank's loss, a mean over its B clouds. The exchange works in
+    units of the global-batch loss, whose gradient here is dy * B / Bg: dgamma and dbeta come out
+    as the global gradients, the same on every rank, and dx goes back to this rank's units."""
+    B, C, P = x.shape
+    dev = x.device
+    share = B / ex.global_rows(B)
+    if share != 1.0:
+        dy = dy * share
+    with torch.cuda.device(dev):
+        dx = torch.empty_like(x)
+        dgamma = torch.empty(C, dtype=torch.float32, device=dev)
+        dbeta = torch.empty(C, dtype=torch.float32, device=dev)
+        rec = torch.empty((B, C, _C.CONSTANTS["SONET_BN_REC_BWD"]), dtype=torch.float64, device=dev)
+        ops._call("sonet_bn_cloud_partials_f32", _C.ptr(x), _C.ptr(dy), _C.ptr(mean), _C.ptr(invstd),
+                  _C.ptr(gamma), _C.ptr(beta), B, C, P, act, 1, _C.ptr(rec), ops._stream(x))
+        rec = ex.gather(rec)
+        ops._call("sonet_bn_sync_backward_f32", _C.ptr(rec), _C.ptr(dy), _C.ptr(x), _C.ptr(mean),
+                  _C.ptr(invstd), _C.ptr(gamma), _C.ptr(beta), ex.global_rows(B), B, C, P, act,
+                  _C.ptr(dx), _C.ptr(dgamma), _C.ptr(dbeta), ops._stream(x), kernels=2)
+    if share != 1.0:
+        dx.div_(share)
+    return dx, dgamma, dbeta
+
+
 class BNActTrain(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, gamma, beta, eps, act):
         x = x.contiguous()
         B, C, P = x.shape
         dev = x.device
+        ctx.exchange = EXCHANGE
+        ctx.act = ops.act_code(act)
+        if EXCHANGE is not None:
+            y, mean, var, invstd = _bn_sync_forward(x, gamma, beta, eps, act, EXCHANGE)
+            ctx.save_for_backward(x, mean, invstd, gamma, beta)
+            ctx.mark_non_differentiable(mean, var)
+            return y, mean, var
         with torch.cuda.device(dev):
             y = torch.empty_like(x)
             mean = torch.empty(C, dtype=torch.float32, device=dev)
@@ -55,7 +114,6 @@ class BNActTrain(torch.autograd.Function):
                       float(eps), ops.act_code(act), _C.ptr(part), _C.ptr(y), _C.ptr(mean), _C.ptr(var),
                       _C.ptr(invstd), ops._stream(x), kernels=3)
         ctx.save_for_backward(x, mean, invstd, gamma, beta)
-        ctx.act = ops.act_code(act)
         ctx.mark_non_differentiable(mean, var)
         return y, mean, var
 
@@ -63,6 +121,10 @@ class BNActTrain(torch.autograd.Function):
     def backward(ctx, dy, _dm, _dv):
         x, mean, invstd, gamma, beta = ctx.saved_tensors
         dy = dy.contiguous()
+        if ctx.exchange is not None:
+            dx, dgamma, dbeta = _bn_sync_backward(dy, x, mean, invstd, gamma, beta, ctx.act,
+                                                  ctx.exchange)
+            return dx, dgamma, dbeta, None, None
         B, C, P = x.shape
         dev = x.device
         with torch.cuda.device(dev):
@@ -347,7 +409,9 @@ def norm_act_train(y0, norm, act, epoch=None, size=None):
         if code == ops.ACT_ELU:
             return F.elu(y0)
         return torch.relu(y0) if code == ops.ACT_RELU else y0
-    if B * P == 1:     # F.batch_norm's check: a batch statistic of one value is undefined
+    # with a BatchNorm exchange installed the statistics are those of the global batch
+    n = (B if EXCHANGE is None else EXCHANGE.global_rows(B)) * P
+    if n == 1:         # F.batch_norm's check: a batch statistic of one value is undefined
         raise ValueError("Expected more than 1 value per channel when training, got input size "
                          "{}".format(size))
     step = norm.momentum_decay_step
@@ -355,7 +419,6 @@ def norm_act_train(y0, norm, act, epoch=None, size=None):
         norm.momentum = max(norm.momentum_original * (norm.momentum_decay ** (epoch // step)), 0.01)
     y, mean, var = BNActTrain.apply(y0, norm.weight, norm.bias, norm.eps, act)
     with torch.no_grad():
-        n = B * P
         m = norm.momentum
         norm.running_mean.mul_(1 - m).add_(mean, alpha=m)
         norm.running_var.mul_(1 - m).add_(var * (n / (n - 1)), alpha=m)
