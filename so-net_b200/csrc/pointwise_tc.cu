@@ -29,6 +29,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 
 #include "tc_common.cuh"
 
@@ -51,7 +52,9 @@ constexpr int NBAR = 2 * NSTAGE_W;
 constexpr int SMEM_BYTES = OFF_BAR + NBAR * 8;
 
 struct Dims {
-  int C0, C1, B, P, Cout, relu, G;
+  int C0, C1, B, P, Cout, G;
+  float floor_v; // the non-ELU epilogue's max: 0 (ReLU), -inf (no activation) or NaN (a raw K-split
+                 // partial: fmaxf(y, NaN) == y for every y, NaN included)
   int kchunks;   // ceil(pad16(Cin) / 64)
   int ntiles;    // out-channel items of <= 128 (each a multiple of 64)
   int cin_pad;   // Cin rounded up to 16
@@ -103,7 +106,7 @@ __device__ inline int item_width(int Cout, int nt, int sub) {
 
 // NPROD: fp16 products per MAC, 3 (hi/lo split, the default) or 1 (hi only, the opt-in fp16 mode:
 // the lo A image is never written and the producer copies only the hi image of each stage).
-// ELU: the epilogue applies ELU instead of the max against floor_v (d.relu is ignored)
+// ELU: the epilogue applies ELU instead of the max against d.floor_v
 template <int NPROD, bool ELU>
 __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
     pointwise_tc_kernel(const float* __restrict__ x0, const float* __restrict__ x1,
@@ -167,7 +170,7 @@ __global__ void __launch_bounds__(pwt::NUM_THREADS, 1)
     const int tw = threadIdx.x & 127;
     const int m = tw & 63, half = tw >> 6;    // conversion: row m, channels [32 half, 32 half + 32)
     const float act_s = d.act_ptr != nullptr ? __ldg(d.act_ptr) : 1.f;
-    const float floor_v = d.relu ? 0.f : -__int_as_float(0x7f800000);   // ReLU as one max
+    const float floor_v = d.floor_v;   // ReLU, no activation or a raw partial as one max
     const float inv_w = d.inv_ptr != nullptr ? __ldg(d.inv_ptr) : d.inv;
     const uint32_t a_base = smem_u32(smem + OFF_A) + wg * (A_HALF / 2);
     const uint32_t w_base = smem_u32(smem + OFF_W);
@@ -387,6 +390,7 @@ extern "C" int sonet_pointwise_tc_pack(const float* W, int Cout, int Cin, void* 
 struct TcExt {   // grouped / split-K / scatter / point-major launch options (defaults = the plain layer)
   int groups = 1, splits = 1, scat_w = 0, P_out = 0, conv_w = 0, rows_out = 0;
   int nprod = 3;   // fp16 products per MAC: 3 (hi/lo split) or 1 (the opt-in fp16 mode)
+  int raw = 0;     // 1: store acc * inv (+ shift) with no activation, NaN kept (K-split partials)
   const float* inv_ptr = nullptr;
   const float* act_ptr = nullptr;
   long long blob_gstride = 0, out_gstride = 0, out_sstride = 0;
@@ -409,7 +413,9 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   SONET_REQUIRE(!addend || (gidx && G >= 1), "pointwise_tc: addend needs gidx and G");
   SONET_REQUIRE(aligned16(blob), "pointwise_tc: weight blob must be 16-byte aligned");
   Dims d;
-  d.C0 = C0; d.C1 = C1; d.B = B; d.P = P; d.Cout = Cout; d.relu = relu == SONET_ACT_RELU; d.G = G;
+  d.C0 = C0; d.C1 = C1; d.B = B; d.P = P; d.Cout = Cout; d.G = G;
+  d.floor_v = ext.raw ? std::numeric_limits<float>::quiet_NaN()
+                      : (relu == SONET_ACT_RELU ? 0.f : -std::numeric_limits<float>::infinity());
   d.conv_w = ext.conv_w;
   d.cpt = 1;
   if (ext.conv_w > 0) {
@@ -512,7 +518,8 @@ extern "C" int sonet_pointwise_tc_forward_rows_f16(const float* x0, int C0, cons
 
 namespace sonet {
 // partial [G][S][B][Cout][P] (raw K-split sums) -> out: sum over S in ascending order (fixed ->
-// deterministic), + shift, ReLU (or, in the ELU build, ELU), and the up-convolution parity scatter.
+// deterministic), + shift, the activation as the main epilogue applies it (a max against 0 or
+// -inf, or in the ELU build ELU), and the up-convolution parity scatter.
 // IT = uint32_t when every index fits 32 bits (always, in practice): the three divisions per element
 // were 64-bit ones, and the kernel was bound by them (17 us for 2.1 M outputs), not by its 40 MB.
 template <typename IT, bool ELU>
@@ -534,8 +541,9 @@ __global__ void __launch_bounds__(256)
     float acc = src[0];
     for (int s = 1; s < S; ++s) acc += src[static_cast<size_t>(s) * per_split];
     if (shift != nullptr) acc += __ldg(shift + co);
-    if (ELU) acc = elu1(acc);
-    else if (relu) acc = fmaxf(acc, 0.f);
+    // the main epilogue's last step, so a split layer gives the unsplit layer's result for every
+    // input: the partials are raw, a NaN among them reaches this point as NaN
+    acc = ELU ? elu1(acc) : fmaxf(acc, relu ? 0.f : -__int_as_float(0x7f800000));
     int po = p;
     if (scat_w > 0) {
       const int i = p / scat_w, j = p - i * scat_w;
@@ -601,6 +609,7 @@ static int pointwise_tc_grouped(const float* x, int C, int B, int P, const void*
   const long long per_split = static_cast<long long>(B) * Cout * P;
   e.out_sstride = per_split;
   e.out_gstride = per_split * splits;
+  e.raw = 1;
   int rc = launch_pointwise_tc(x, C, nullptr, 0, B, P, blob, inv_scale, nullptr, Cout, 0, nullptr,
                                nullptr, 0, scratch, nullptr, stream, e);
   if (rc) return rc;
@@ -669,6 +678,7 @@ extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, in
   const long long per_split = static_cast<long long>(B) * Cout * P;
   e.splits = splits;
   e.out_sstride = per_split;
+  e.raw = 1;
   int rc = launch_pointwise_tc(x0, C0, nullptr, 0, B, P, blob, 1.f, nullptr, Cout, 0, nullptr, nullptr,
                                0, scratch, nullptr, stream, e);
   if (rc) return rc;

@@ -36,6 +36,16 @@ TC_F = 2.0 ** -24
 TC_FP32_FACTOR = 8.0
 TC_FP32_FLOOR = 0.125
 
+# Error bar of one opt-in fp16-mode GEMM output (SONET_TC=fp16: one fp16 product per MAC) against
+# the fp64 GEMM of its rounded operands:
+#     |got - y16| <= F16_C * (sum_k |W16[o,k] x16[k]| / s + |shift| + |addend|)
+# F16_C covers the fp32 accumulation inside the tensor cores, the fp32 epilogue and, with split-K,
+# the fp32 partial sums. Measured on one H100 80GB HBM3 (700 W power limit) over the kernel cases
+# of tests/test_gpu_fp16_mode.py: max err / m = 6.0e-7 (the saturated-input case; 1.2e-7 .. 5.3e-7
+# elsewhere). F16_C is 2.5x that, as TC_R is 2.5x its measurement. A leftover lo product would
+# show as ~2^-11 = 4.9e-4.
+F16_C = 1.5e-6
+
 
 def tc_reference(W, x, shift=None, addend=None, w_scale=None, parts=False):
     """fp64 y = W x (+ shift[o]) (+ addend, already gathered to [B,Cout,P]) and the error bar of
