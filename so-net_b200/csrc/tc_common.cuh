@@ -171,8 +171,9 @@ __host__ __device__ inline void put_weight(unsigned char* hi, unsigned char* lo,
 // The pre-scale of a matrix with max|W| = absmax: the power of two that brings max|W| into
 // [256, 512), so the lo parts stay normal fp16 numbers and the hi parts far from the 65504
 // overflow; the epilogue's multiply undoes it exactly. 1 for an all-zero or non-finite matrix.
-// The exponent is capped at max_exp.
-__host__ __device__ inline float pow2_scale(float absmax, int max_exp = 1 << 30) {
+// The exponent is capped at max_exp, by default 126 so that 1/scale stays a normal float: uncapped,
+// absmax < 2^-119 would give 2^128 = inf (and 1/scale = 0). Every absmax >= 2^-118 is below the cap.
+__host__ __device__ inline float pow2_scale(float absmax, int max_exp = 126) {
   if (!(absmax > 0.f && absmax <= FLT_MAX)) return 1.f;
   int e;
   frexpf(absmax, &e);  // absmax = f * 2^e, f in [0.5, 1)

@@ -377,9 +377,19 @@ __global__ void __launch_bounds__(256)
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) atomicMax(out_bits, __float_as_uint(m));   // non-negative floats
 }
-// scale2[0] = the power-of-two pre-scale of the tensor (tc::pow2_scale), scale2[1] = 1/scale
-__global__ void scale_from_absmax_kernel(const unsigned* __restrict__ bits, float* __restrict__ scale2) {
-  const float sc = tc::pow2_scale(__uint_as_float(*bits));
+// The pre-scale of a GRADIENT operand with max |g| = absmax (NaN elements do not count): tc::pow2_scale,
+// except that an infinite max gives NaN. The saturating fp16 split would turn an infinite gradient
+// into +-131008 and its results finite; a NaN scale makes them non-finite instead. Weight packs keep
+// pow2_scale's 1: an infinite weight propagates by itself (hi = inf, lo = NaN).
+__device__ inline float grad_scale(float absmax) {
+  return isinf(absmax) ? __int_as_float(0x7fffffff) : tc::pow2_scale(absmax);
+}
+// scale2[0] = the power-of-two pre-scale of the tensor (tc::pow2_scale, or grad_scale when grad),
+// scale2[1] = 1/scale
+__global__ void scale_from_absmax_kernel(const unsigned* __restrict__ bits, int grad,
+                                         float* __restrict__ scale2) {
+  const float m = __uint_as_float(*bits);
+  const float sc = grad ? grad_scale(m) : tc::pow2_scale(m);
   scale2[0] = sc;
   scale2[1] = 1.f / sc;
 }
@@ -445,7 +455,7 @@ __global__ void scale_from_partials_kernel(const float* __restrict__ partial, in
 
 // ---- wgrad helpers ------------------------------------------------------------------------------------
 // Per-channel power-of-two pre-scale of dy [B][C][P]: cscale[c] = s_c with max_{b,p} |s_c dy[b,c,p]|
-// in [256,512) (1 for an all-zero or non-finite channel), cscale[C + c] = 1/s_c. Gradients of one
+// in [256,512) (grad_scale: 1 for an all-zero channel, NaN for one holding +-inf), cscale[C + c] = 1/s_c. Gradients of one
 // layer span many decades between channels; with ONE scale per tensor the small channels' values
 // would fall into fp16's subnormal range and lose their relative precision (each row of dW is its
 // own parameter's gradient). One CTA per channel.
@@ -464,7 +474,7 @@ __global__ void __launch_bounds__(256)
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < 8; ++w) m = fmaxf(m, wm[w]);
-    const float sc = tc::pow2_scale(m, 126);   // 2^126: 1/sc stays a normal float
+    const float sc = grad_scale(m);
     cscale[c] = sc;
     cscale[C + c] = 1.f / sc;
   }
@@ -488,13 +498,19 @@ __global__ void __launch_bounds__(256)
     if (p < P && c < C) dyT[(static_cast<size_t>(b) * P + p) * C + c] = tile[tx][i];
   }
 }
-// dWT [Cin][Cout] *= 1/s_co: undoes the per-channel pre-scale of dy (exact: powers of two)
+// dWT [Cin][Cout] = the raw GEMM sum * (1/s_x) * (1/s_co): undoes x's pre-scale and each dy channel's.
+// Both factors are powers of two, so the fp64 product is exact and the result is rounded once. In
+// fp32, sum / s_x (= s_co dW) overflows where dW > FLT_MAX / s_co although dW itself is finite.
 __global__ void __launch_bounds__(256)
-    col_unscale_kernel(float* __restrict__ dWT, long long n, int Cout, const float* __restrict__ inv_c) {
+    col_unscale_kernel(float* __restrict__ dWT, long long n, int Cout, const float* __restrict__ inv_x,
+                       const float* __restrict__ inv_c) {
+  const double ix = static_cast<double>(*inv_x);
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
-    dWT[i] *= inv_c[i % Cout];
+    dWT[i] = static_cast<float>(static_cast<double>(dWT[i]) * ix * static_cast<double>(inv_c[i % Cout]));
 }
+// the GEMM's epilogue scale in the wgrad: 1, the unscale is col_unscale_kernel's
+__device__ const float kUnitScale = 1.f;
 
 // ---- per-cloud BatchNorm records (synchronised BN of data-parallel training) -------------------------
 // Row r = b*C + c of x [B,C,P] gets one fp64 record whose value depends on that row alone: the row's
@@ -840,7 +856,7 @@ extern "C" int sonet_pointwise_tc_pack_device(const float* W, int Cout, int Cin,
   cudaMemsetAsync(scratch_bits, 0, sizeof(unsigned), st);
   absmax_kernel<<<static_cast<unsigned>(std::min<long long>((n + 255) / 256, 1024)), 256, 0, st>>>(
       W, n, scratch_bits);
-  scale_from_absmax_kernel<<<1, 1, 0, st>>>(scratch_bits, scale2);
+  scale_from_absmax_kernel<<<1, 1, 0, st>>>(scratch_bits, 0, scale2);
   if (transpose)   // W^T [Cin][Cout]
     launch_tc_pack(W, Cin, Cout, 1, Cin, Cout, 0, scale2, blob, tc::wblob::kchunks(Cout), st);
   else
@@ -872,7 +888,8 @@ extern "C" int sonet_pointwise_tc_pack_groups_device(const float* W, int G, int 
   return check_launch("pointwise_tc_pack_groups_device");
 }
 
-// power-of-two scale of a device tensor: scale2[0] = s with max|s*t| in [256,512), scale2[1] = 1/s
+// power-of-two pre-scale of a gradient operand on the device: scale2[0] = s with max|s*t| in [256,512)
+// (grad_scale: NaN elements are ignored, 1 when all are zero, NaN when one is +-inf), scale2[1] = 1/s
 extern "C" int sonet_absmax_scale_f32(const float* t, long long n, float* scale2, unsigned* scratch_bits,
                                       sonet_stream_t stream) {
   using namespace sonet;
@@ -881,7 +898,7 @@ extern "C" int sonet_absmax_scale_f32(const float* t, long long n, float* scale2
   cudaMemsetAsync(scratch_bits, 0, sizeof(unsigned), st);
   absmax_kernel<<<static_cast<unsigned>(std::min<long long>((n + 255) / 256, 2048)), 256, 0, st>>>(
       t, n, scratch_bits);
-  scale_from_absmax_kernel<<<1, 1, 0, st>>>(scratch_bits, scale2);
+  scale_from_absmax_kernel<<<1, 1, 0, st>>>(scratch_bits, 1, scale2);
   return check_launch("absmax_scale");
 }
 
@@ -933,12 +950,15 @@ extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Co
   rc = check_launch("wgrad_tc(prepare)");
   if (rc) return rc;
   // activations: dyT viewed as [B'=1][C'=Kpad][P'=Cout] (already scaled: no act pre-scale needed);
-  // the epilogue undoes x's scale, col_unscale each dy channel's
-  rc = sonet_pointwise_tc_forward_dev(dyT, static_cast<int>(Kpad), 1, Cout, blob, s_x + 1, nullptr,
-                                      nullptr, Cin, 0, splits, dWT, part, stream);
+  // the GEMM writes the raw sums, col_unscale undoes x's scale and each dy channel's
+  void* unit = nullptr;
+  if (cudaGetSymbolAddress(&unit, kUnitScale) != cudaSuccess) return check_launch("wgrad_tc(unit scale)");
+  rc = sonet_pointwise_tc_forward_dev(dyT, static_cast<int>(Kpad), 1, Cout, blob,
+                                      static_cast<const float*>(unit), nullptr, nullptr, Cin, 0, splits,
+                                      dWT, part, stream);
   if (rc) return rc;
   const long long n = static_cast<long long>(Cin) * Cout;
   col_unscale_kernel<<<static_cast<unsigned>(std::min<long long>((n + 255) / 256, 2048)), 256, 0, st>>>(
-      dWT, n, Cout, s_dy + Cout);
+      dWT, n, Cout, s_x + 1, s_dy + Cout);
   return check_launch("wgrad_tc(unscale)");
 }

@@ -228,7 +228,10 @@ def wgrad_tc(dy, x):
     Cin = x.shape[1]
     lib = _C.lib()
     base = ((Cout + 127) // 128) * (((Cin + 63) // 64 * 64 + 255) // 256)
-    splits = max(1, min(64, 296 // base, (B * P + 63) // 64))
+    kch = (B * P + 63) // 64
+    splits = max(1, min(64, 296 // base, kch))
+    if -(-kch // splits) > WGRAD_MAX_KPI:
+        splits = min(64, -(-kch // WGRAD_MAX_KPI))
     Kpad = int(lib.sonet_wgrad_kpad(B, P, splits))
     dev = dy.device
     with torch.cuda.device(dev):
@@ -245,6 +248,13 @@ def wgrad_tc(dy, x):
 
 
 _WGRAD_CACHE = {}
+
+# Longest K extent, in 64-point chunks, that one wgmma accumulator of the wgrad sums (more splits
+# when the CTA count alone would allow longer ones). As with UPCONV_MAX_KPI, the tensor cores' fp32
+# accumulation loses precision with the length of one chain: the segmenter's 3356 -> 1024 layer at
+# B*P = 24576 had 2 splits of 192 chunks and a dW row error of 6.9e-5 (strict fp32 cuBLAS: 3e-6) on
+# one H100 80GB HBM3 (700 W), tests/test_gpu_train_tc_envelope.py.
+WGRAD_MAX_KPI = 32
 
 
 class ConvTC(torch.autograd.Function):

@@ -49,11 +49,12 @@ def test_pack_images_round_trip_128_row_layer3(lib_built):
 
 # ---- reference packer -----------------------------------------------------------------------------
 def ref_scale(W):
-    """Power of two s with max|s W| in [256, 512); 1 for an all-zero matrix."""
+    """Power of two s with max|s W| in [256, 512), at most 2^126 (1/s stays a normal float); 1 for
+    an all-zero matrix."""
     m = np.float32(np.abs(W).max())
     if not (m > 0 and np.isfinite(m)):
         return np.float32(1.0)
-    return np.float32(np.ldexp(1.0, 9 - int(np.frexp(m)[1])))
+    return np.float32(np.ldexp(1.0, min(9 - int(np.frexp(m)[1]), 126)))
 
 
 def ref_split(Ws):
@@ -106,6 +107,22 @@ def test_pointwise_pack_matches_reference(lib_built, cout, cin):
     blob, inv = ops.pointwise_tc_pack(torch.from_numpy(W))
     s = ref_scale(W)
     assert inv == np.float32(1.0) / s
+    assert np.array_equal(blob.numpy(), ref_pointwise_blob(W, s))
+
+
+@pytest.mark.parametrize("e", [-149, -140, -125, -120, -119, -118, -117])
+def test_pointwise_pack_scale_is_capped_for_tiny_matrices(lib_built, e):
+    """A matrix with max |W| = 2^e below 2^-118 gets the capped scale 2^126, not 2^(9 - e - 1),
+    which overflows to inf from e = -119 down; at 2^-118 and above the cap changes nothing."""
+    from sonet_b200 import ops
+    rs = np.random.RandomState(-e)
+    W = rs.normal(size=(70, 40))
+    W = (W / np.abs(W).max() * 2.0 ** e).astype(np.float32)
+    assert np.float32(np.abs(W).max()) == np.float32(2.0 ** e)
+    blob, inv = ops.pointwise_tc_pack(torch.from_numpy(W))
+    s = ref_scale(W)
+    assert s == np.float32(2.0 ** min(8 - e, 126)) and np.isfinite(s)
+    assert inv == np.float32(1.0) / s and inv >= np.finfo(np.float32).tiny
     assert np.array_equal(blob.numpy(), ref_pointwise_blob(W, s))
 
 
