@@ -308,6 +308,47 @@ int sonet_pointwise_tc_grouped_forward_dev(const float* x, int C, int B, int P, 
                                            long long out_gstride, float* out, float* scratch,
                                            sonet_stream_t stream);
 
+/* ---- opt-in fp16 mode of the train wgmma entries (SONET_TRAIN_TC=fp16, INTEGRATION.md) ----------
+ * One-product twins of the three train-mode GEMM entries: ConvTC's forward and dgrad
+ * (sonet_pointwise_tc_forward_dev), UpConvTC's forward (sonet_pointwise_tc_grouped_forward_dev) and
+ * every wgrad (sonet_wgrad_tc_f32). Each runs its GEMM as ONE fp16 product per MAC instead of the
+ * hi/lo split's three:
+ *   y = (sum_k rn16sat(s_x * x_k) * rn16(s_w * w_k)) / (s_x * s_w), accumulated in fp32,
+ * where s_w is the power-of-two pre-scale of the weight operand (of the blob packed on the device;
+ * the wgrad's own pack of x, whose operand is the saved activation) and s_x that of the activation
+ * operand (act_scale_dev; the wgrad's per-channel dy scales), each capped at 2^126 as in the split
+ * entries. rn16sat is the round-to-nearest fp16 saturated at +-65504, rn16 the hi image of the blob.
+ * With s_x from sonet_absmax_scale_f32 no operand of any fp32 magnitude saturates; values below
+ * ~2^-24 of their tensor's max become fp16 subnormals and lose relative precision. The caller's
+ * inv_scale_dev = 1/(s_x * s_w) is one fp32 value: it underflows to 0 when max|w| * max|x| is below
+ * about 2^-131 (every product then below fp32's normal range). Per output the
+ * rounding costs up to ~2^-10 * sum_k |w_k x_k|; against the rounded operands the GEMM is exact up
+ * to fp32 accumulation. NaN and +-inf follow the split entries' rules: the same saturation and
+ * epilogue, and a NaN scale (an infinite gradient) makes its outputs NaN.
+ *   sonet_pointwise_tc_forward_dev_f16: the arguments of sonet_pointwise_tc_forward_dev.
+ *   sonet_pointwise_tc_grouped_forward_dev_f16: those of sonet_pointwise_tc_grouped_forward_dev and
+ *     act_scale_dev, the activations' pre-scale (1 element of device memory, or null for none), whose
+ *     inverse the caller folds into inv_scale_dev.
+ *   sonet_wgrad_tc_f16: the arguments and scratch of sonet_wgrad_tc_f32 (sonet_wgrad_kpad,
+ *     sonet_wgrad_blob_bytes and sonet_wgrad_small_floats size it); x's blob is written as hi images
+ *     only, half the bytes, in the same layout, and dyT stays fp32 (the GEMM rounds it as it loads).
+ * Same properties as the split entries: arguments validated before any CUDA call (SONET_ERR_BAD_ARG),
+ * no allocation, no host synchronisation, deterministic, CUDA graph capturable. */
+int sonet_pointwise_tc_forward_dev_f16(const float* x0, int C0, int B, int P, const void* blob,
+                                       const float* inv_scale_dev, const float* act_scale_dev,
+                                       const float* shift, int Cout, int relu, int splits,
+                                       float* out, float* scratch, sonet_stream_t stream);
+int sonet_pointwise_tc_grouped_forward_dev_f16(const float* x, int C, int B, int P, const void* blob,
+                                               long long blob_gstride, const float* inv_scale_dev,
+                                               const float* act_scale_dev, const float* shift,
+                                               int Cout, int relu, int groups, int splits,
+                                               int scat_w, int conv_w, int P_out,
+                                               long long out_gstride, float* out, float* scratch,
+                                               sonet_stream_t stream);
+int sonet_wgrad_tc_f16(const float* dy, const float* x, int B, int Cout, int Cin, int P, int splits,
+                       float* dyT, void* blob, float* part, float* small, float* dWT,
+                       sonet_stream_t stream);
+
 /* ---- f-4: batch-SOM training --------------------------------------------------------------------
  * Replaces BatchSOM.batch_update / BatchSOM.optimize (util/som.py:295-366): T iterations of
  * {nearest-node assignment, per-node mean, neighbourhood-weighted node update} per cloud, in ONE

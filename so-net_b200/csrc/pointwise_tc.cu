@@ -448,8 +448,7 @@ static int launch_pointwise_tc(const float* x0, int C0, const float* x1, int C1,
   const long long items = static_cast<long long>(d.row_tiles) * d.ntiles * ext.groups * ext.splits;
   SONET_REQUIRE(items < (1LL << 31), "pointwise_tc: too many tiles");
   SONET_REQUIRE(SMEM_BYTES <= max_smem_optin(), "pointwise_tc: needs %d B of shared memory", SMEM_BYTES);
-  SONET_REQUIRE(ext.nprod == 3 || (ext.nprod == 1 && !ext.act_ptr && !ext.inv_ptr),
-                "pointwise_tc: the one-product mode is eval-only");
+  SONET_REQUIRE(ext.nprod == 3 || ext.nprod == 1, "pointwise_tc: %d products per MAC", ext.nprod);
   auto kern = relu == SONET_ACT_ELU ? (ext.nprod == 1 ? pointwise_tc_kernel<1, true> : pointwise_tc_kernel<3, true>)
                                     : (ext.nprod == 1 ? pointwise_tc_kernel<1, false> : pointwise_tc_kernel<3, false>);
   cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
@@ -584,7 +583,8 @@ static int pointwise_tc_grouped(const float* x, int C, int B, int P, const void*
                                 long long blob_gstride, float inv_scale, const float* shift, int Cout,
                                 int relu, int groups, int splits, int scat_w, int conv_w, int P_out,
                                 long long out_gstride, float* out, float* scratch,
-                                sonet_stream_t stream, int nprod, const float* inv_ptr = nullptr) {
+                                sonet_stream_t stream, int nprod, const float* inv_ptr = nullptr,
+                                const float* act_ptr = nullptr) {
   using namespace sonet;
   SONET_REQUIRE(groups >= 1 && splits >= 1 && scat_w >= 0, "pointwise_tc_grouped: bad group/split");
   SONET_REQUIRE(scat_w == 0 || (groups == 4 && P % scat_w == 0 && P_out == 4 * P && out_gstride == 0),
@@ -595,6 +595,7 @@ static int pointwise_tc_grouped(const float* x, int C, int B, int P, const void*
   SONET_REQUIRE(conv_w == 0 || conv_w == scat_w, "pointwise_tc_grouped: conv_w must equal scat_w");
   TcExt e = with_nprod(nprod);
   e.inv_ptr = inv_ptr;
+  e.act_ptr = act_ptr;
   e.groups = groups;
   e.splits = splits;
   e.blob_gstride = blob_gstride;
@@ -658,18 +659,34 @@ extern "C" int sonet_pointwise_tc_grouped_forward_dev(const float* x, int C, int
                               scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 3, inv_scale_dev);
 }
 
-// Train-mode variant: the weight blob was packed on the device this step
-// (sonet_pointwise_tc_pack_device) and its 1/pre-scale is read from device memory.
-extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, int P, const void* blob,
-                                              const float* inv_scale_dev, const float* act_scale_dev,
-                                              const float* shift, int Cout, int relu, int splits,
-                                              float* out, float* scratch, sonet_stream_t stream) {
+// The one-product twin (SONET_TRAIN_TC=fp16): act_scale_dev, when given, pre-scales the activations
+// before their fp16 rounding as in the split entry, so the operand keeps fp16's relative precision
+// whatever its fp32 magnitude.
+extern "C" int sonet_pointwise_tc_grouped_forward_dev_f16(const float* x, int C, int B, int P,
+                                                          const void* blob, long long blob_gstride,
+                                                          const float* inv_scale_dev,
+                                                          const float* act_scale_dev,
+                                                          const float* shift, int Cout, int relu,
+                                                          int groups, int splits, int scat_w,
+                                                          int conv_w, int P_out, long long out_gstride,
+                                                          float* out, float* scratch,
+                                                          sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_grouped_forward_dev_f16");
+  SONET_REQUIRE(inv_scale_dev != nullptr, "pointwise_tc_grouped_forward_dev_f16: null inv_scale pointer");
+  return pointwise_tc_grouped(x, C, B, P, blob, blob_gstride, 1.f, shift, Cout, relu, groups, splits,
+                              scat_w, conv_w, P_out, out_gstride, out, scratch, stream, 1, inv_scale_dev,
+                              act_scale_dev);
+}
+
+static int pointwise_tc_dev(const float* x0, int C0, int B, int P, const void* blob,
+                            const float* inv_scale_dev, const float* act_scale_dev, const float* shift,
+                            int Cout, int relu, int splits, float* out, float* scratch,
+                            sonet_stream_t stream, int nprod) {
   using namespace sonet;
-  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward_dev");
   SONET_REQUIRE(inv_scale_dev != nullptr, "pointwise_tc_forward_dev: null inv_scale pointer");
   SONET_REQUIRE(splits >= 1 && (splits == 1 || scratch != nullptr),
                 "pointwise_tc_forward_dev: split-K needs scratch");
-  TcExt e;
+  TcExt e = with_nprod(nprod);
   e.inv_ptr = inv_scale_dev;
   e.act_ptr = act_scale_dev;
   if (splits == 1)
@@ -684,6 +701,28 @@ extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, in
   if (rc) return rc;
   launch_splitk_reduce(scratch, 1, splits, B, Cout, P, shift, relu, 0, P, 0, out, as_stream(stream));
   return check_launch("splitk_reduce");
+}
+
+// Train-mode variant: the weight blob was packed on the device this step
+// (sonet_pointwise_tc_pack_device) and its 1/pre-scale is read from device memory.
+extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, int P, const void* blob,
+                                              const float* inv_scale_dev, const float* act_scale_dev,
+                                              const float* shift, int Cout, int relu, int splits,
+                                              float* out, float* scratch, sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward_dev");
+  return pointwise_tc_dev(x0, C0, B, P, blob, inv_scale_dev, act_scale_dev, shift, Cout, relu, splits,
+                          out, scratch, stream, 3);
+}
+
+// its one-product twin (SONET_TRAIN_TC=fp16): same arguments and blob, the hi images only
+extern "C" int sonet_pointwise_tc_forward_dev_f16(const float* x0, int C0, int B, int P,
+                                                  const void* blob, const float* inv_scale_dev,
+                                                  const float* act_scale_dev, const float* shift,
+                                                  int Cout, int relu, int splits, float* out,
+                                                  float* scratch, sonet_stream_t stream) {
+  SONET_REQUIRE_ACT(relu, "pointwise_tc_forward_dev_f16");
+  return pointwise_tc_dev(x0, C0, B, P, blob, inv_scale_dev, act_scale_dev, shift, Cout, relu, splits,
+                          out, scratch, stream, 1);
 }
 
 extern "C" int sonet_debug_pointwise_tc_timeline(const float* x0, int C0, int B, int P,

@@ -399,6 +399,9 @@ __global__ void scale_from_absmax_kernel(const unsigned* __restrict__ bits, int 
 //   W^T, of W [K][N]:             sn = 1, sk = N, kp = K, sb = 0
 //   x [B][N][P] with k = (b, p):  sn = P, sk = 1, kp = P, sb = N * P
 // Consecutive threads take consecutive k of one row n: the reads are coalesced unless sk > 1.
+// NPROD = 1 (the one-product wgrad) writes the hi images only, the bytes the GEMM then reads: half
+// the stores, in the same layout.
+template <int NPROD>
 __global__ void __launch_bounds__(256)
     tc_pack_device_kernel(const float* __restrict__ src, int N, int K, long long sn, long long sk,
                           int kp, long long sb, const float* __restrict__ scale2,
@@ -413,14 +416,22 @@ __global__ void __launch_bounds__(256)
     if (n < N && k < K) w = src[n * sn + (k / kp) * sb + (k % kp) * sk] * sc;
     long long hi, lo;
     tc::wblob::elem_off(N, kch, n, k, hi, lo);
-    tc::put_weight(blob + hi, blob + lo, w);
+    if (NPROD == 3)
+      tc::put_weight(blob + hi, blob + lo, w);
+    else   // put_weight's hi half
+      *reinterpret_cast<__half*>(blob + hi) = __float2half_rn(w);
   }
 }
 static void launch_tc_pack(const float* src, int N, int K, long long sn, long long sk, int kp,
-                           long long sb, const float* scale2, void* blob, int kch, cudaStream_t st) {
+                           long long sb, const float* scale2, void* blob, int kch, cudaStream_t st,
+                           int nprod = 3) {
   const long long total = static_cast<long long>(tc::wblob::npad(N)) * kch * tc::wblob::KCH;
-  tc_pack_device_kernel<<<static_cast<unsigned>(std::min<long long>((total + 255) / 256, 16384)), 256, 0,
-                          st>>>(src, N, K, sn, sk, kp, sb, scale2, static_cast<unsigned char*>(blob), kch);
+  const unsigned grid = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 16384));
+  unsigned char* b = static_cast<unsigned char*>(blob);
+  if (nprod == 1)
+    tc_pack_device_kernel<1><<<grid, 256, 0, st>>>(src, N, K, sn, sk, kp, sb, scale2, b, kch);
+  else
+    tc_pack_device_kernel<3><<<grid, 256, 0, st>>>(src, N, K, sn, sk, kp, sb, scale2, b, kch);
 }
 
 // absmax without atomics: CTA b writes the max of its grid-stride share to partial[b], then one
@@ -906,6 +917,11 @@ extern "C" int sonet_pointwise_tc_forward_dev(const float* x0, int C0, int B, in
                                               const float* inv_scale_dev, const float* act_scale_dev,
                                               const float* shift, int Cout, int relu, int splits,
                                               float* out, float* scratch, sonet_stream_t stream);
+extern "C" int sonet_pointwise_tc_forward_dev_f16(const float* x0, int C0, int B, int P,
+                                                  const void* blob, const float* inv_scale_dev,
+                                                  const float* act_scale_dev, const float* shift,
+                                                  int Cout, int relu, int splits, float* out,
+                                                  float* scratch, sonet_stream_t stream);
 
 // wgrad of a 1x1 convolution on wgmma: dW[co][ci] = sum_{b,p} dy[b,co,p] * x[b,ci,p].
 // Written as the generic layer GEMM out[rows = co][n = ci] = sum_k A[k][co] * Wl[ci][k] with the
@@ -923,9 +939,11 @@ extern "C" long long sonet_wgrad_kpad(int B, int P, int splits) {
 extern "C" long long sonet_wgrad_blob_bytes(int Cin, long long Kpad) {
   return sonet::tc::wblob::bytes(Cin, Kpad);
 }
-extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Cout, int Cin, int P,
-                                  int splits, float* dyT, void* blob, float* part, float* small,
-                                  float* dWT, sonet_stream_t stream) {
+// nprod = 1: the one-product twin. dyT keeps fp32 (the generic kernel rounds its activation operand
+// itself); x is packed as hi images only, into the same blob layout and size.
+static int wgrad_tc(const float* dy, const float* x, int B, int Cout, int Cin, int P, int splits,
+                    float* dyT, void* blob, float* part, float* small, float* dWT,
+                    sonet_stream_t stream, int nprod) {
   using namespace sonet;
   SONET_REQUIRE(dy && x && dyT && blob && part && small && dWT, "wgrad_tc: null pointer");
   SONET_REQUIRE(B >= 1 && P >= 1 && Cout >= 64 && Cout % 64 == 0 && Cin >= 1 && splits >= 1 &&
@@ -946,19 +964,32 @@ extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Co
   transpose_scale_kernel<<<dim3((P + 31) / 32, (Cout + 31) / 32, B), 256, 0, st>>>(dy, Cout, P, s_dy, dyT);
   // x as the weight matrix [Cin][k = (b, p)], zero-padded up to Kpad
   launch_tc_pack(x, Cin, static_cast<int>(K), P, 1, P, static_cast<long long>(Cin) * P, s_x, blob,
-                 tc::wblob::kchunks(Kpad), st);
+                 tc::wblob::kchunks(Kpad), st, nprod);
   rc = check_launch("wgrad_tc(prepare)");
   if (rc) return rc;
   // activations: dyT viewed as [B'=1][C'=Kpad][P'=Cout] (already scaled: no act pre-scale needed);
   // the GEMM writes the raw sums, col_unscale undoes x's scale and each dy channel's
   void* unit = nullptr;
   if (cudaGetSymbolAddress(&unit, kUnitScale) != cudaSuccess) return check_launch("wgrad_tc(unit scale)");
-  rc = sonet_pointwise_tc_forward_dev(dyT, static_cast<int>(Kpad), 1, Cout, blob,
-                                      static_cast<const float*>(unit), nullptr, nullptr, Cin, 0, splits,
-                                      dWT, part, stream);
+  rc = (nprod == 1 ? sonet_pointwise_tc_forward_dev_f16 : sonet_pointwise_tc_forward_dev)(
+      dyT, static_cast<int>(Kpad), 1, Cout, blob, static_cast<const float*>(unit), nullptr, nullptr, Cin,
+      0, splits, dWT, part, stream);
   if (rc) return rc;
   const long long n = static_cast<long long>(Cin) * Cout;
   col_unscale_kernel<<<static_cast<unsigned>(std::min<long long>((n + 255) / 256, 2048)), 256, 0, st>>>(
       dWT, n, Cout, s_x + 1, s_dy + Cout);
   return check_launch("wgrad_tc(unscale)");
+}
+
+extern "C" int sonet_wgrad_tc_f32(const float* dy, const float* x, int B, int Cout, int Cin, int P,
+                                  int splits, float* dyT, void* blob, float* part, float* small,
+                                  float* dWT, sonet_stream_t stream) {
+  return wgrad_tc(dy, x, B, Cout, Cin, P, splits, dyT, blob, part, small, dWT, stream, 3);
+}
+
+// the one-product twin (SONET_TRAIN_TC=fp16): same arguments and scratch sizes
+extern "C" int sonet_wgrad_tc_f16(const float* dy, const float* x, int B, int Cout, int Cin, int P,
+                                  int splits, float* dyT, void* blob, float* part, float* small,
+                                  float* dWT, sonet_stream_t stream) {
+  return wgrad_tc(dy, x, B, Cout, Cin, P, splits, dyT, blob, part, small, dWT, stream, 1);
 }

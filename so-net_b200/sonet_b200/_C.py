@@ -61,8 +61,11 @@ with open(HEADER_PATH) as _f:
     _SIGNATURES, _RESTYPE, CONSTANTS = parse_header(_f.read())
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
+# the one-product twins of the train-mode GEMM entries (SONET_TRAIN_TC=fp16)
+TRAIN_F16_ENTRIES = ("sonet_pointwise_tc_forward_dev_f16", "sonet_pointwise_tc_grouped_forward_dev_f16",
+                     "sonet_wgrad_tc_f16")
 # the opt-in fp16 mode's twins of the eval wgmma entries (same arguments as the split entry)
-F16_ENTRIES = tuple(n for n in _SIGNATURES if n.endswith("_f16"))
+F16_ENTRIES = tuple(n for n in _SIGNATURES if n.endswith("_f16") and n not in TRAIN_F16_ENTRIES)
 # the fused kernels with an explicit activation code (SONET_ACT_RELU / _ELU) and f16 flag
 ACT_ENTRIES = tuple(n for n in _SIGNATURES if n.endswith("_act"))
 

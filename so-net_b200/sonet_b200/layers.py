@@ -393,7 +393,9 @@ class MyConv2d(_PointwiseConvBase):
                 and torch.is_grad_enabled() and x.is_cuda and x.dtype == torch.float32
                 and x.dim() == 4 and self.activation in KERNEL_ACTIVATIONS)
 
-    def forward(self, x, epoch=None):
+    def forward(self, x, epoch=None, tf32=False):
+        """tf32: a cuDNN convolution of a train step may round to TF32 (UpConv's 3x3 convolution
+        below train_ops.UPCONV_MIN_HW under SONET_TRAIN_TC=fp16); otherwise it is strict fp32."""
         if _fast_ok(self, x) and x.dim() == 4 and self._fast_eligible():
             B, C, H, W = x.shape
             y = self.forward_points(x.contiguous().view(B, C, H * W))
@@ -407,7 +409,7 @@ class MyConv2d(_PointwiseConvBase):
         # PyTorch/cuDNN path (3x3 decoder convs, training): strict fp32 in the forward and the
         # backward — cuDNN's default TF32 convolution is ~1e-3 relative, outside the 1e-4 parity
         # bar of the reference's fp32 math
-        x = train_ops.conv_strict(self.conv, x)
+        x = train_ops.conv_tf32(self.conv, x) if tf32 else train_ops.conv_strict(self.conv, x)
         if self._sync_norm(x):
             B, C, H, W = x.shape
             y = train_ops.norm_act_train(x.reshape(B, C, H * W), self.norm, self.activation, epoch)
@@ -515,7 +517,11 @@ class UpConv(nn.Module):
                 y = train_ops.norm_act_train(z.view(B, Cout, H2 * W2), self.conv._train_norm(),
                                              self.activation)
                 return y.view(B, Cout, H2, W2)
-            return self.conv(self.up_sample(x))
+            # the decoder's maps below UPCONV_MIN_HW: SONET_TRAIN_TC=fp16 gives up fp32 parity in
+            # their cuDNN convolutions too and allows TF32, the reference's default
+            tf32 = (train_ops.ENABLED and self.training and torch.is_grad_enabled() and x.is_cuda
+                    and train_ops.train_f16())
+            return self.conv(self.up_sample(x), tf32=tf32)
         pk = self._packed()
         f16 = tc_f16()
         B, Cin, H, W = x.shape

@@ -19,9 +19,11 @@ models/networks.py:185).
                   arg-max kernel in the forward and a deterministic scatter in the backward
 
 norm_act_train is the norm / activation half every train-mode layer shares. ENABLED = False
-switches every layer back to the PyTorch composition (the tests compare the two).
+switches every layer back to the PyTorch composition (the tests compare the two). train_f16()
+(SONET_TRAIN_TC=fp16) runs ConvTC's and UpConvTC's GEMMs as one fp16 product per MAC.
 """
 import contextlib
+import os
 
 import torch
 import torch.nn.functional as F
@@ -30,6 +32,23 @@ from torch.nn.modules.instancenorm import _InstanceNorm
 from . import _C, ops
 
 ENABLED = True
+
+
+def train_f16():
+    """True under SONET_TRAIN_TC=fp16: the train-mode wgmma GEMMs (ConvTC's and UpConvTC's forward,
+    dgrad and wgrad) run as one fp16 product per MAC on the `_f16` twins of their entries, each
+    operand pre-scaled by a power of two first, and the decoder's cuDNN convolutions below
+    UPCONV_MIN_HW run with TF32 allowed. Read when a layer's forward runs, so a change applies from
+    the next train step on; its backward keeps the forward's mode. Unset or any other value: the
+    fp16 hi/lo split. Eval mode ignores it (SONET_TC is eval's switch)."""
+    return os.environ.get("SONET_TRAIN_TC") == "fp16"
+
+
+def _f16(name, f16):
+    """The C-ABI entry `name`, or with f16 its one-product twin (`_f32` becomes `_f16`)."""
+    if not f16:
+        return name
+    return (name[:-4] if name.endswith("_f32") else name) + "_f16"
 
 
 def _scratch(dev, n, dtype, cache={}):
@@ -206,14 +225,31 @@ def _absmax_scale(t):
     return scale2
 
 
-def _tc_dev(x, blob, inv, shift, cout, act_scale=None):
+def _forward_scale(x):
+    """_absmax_scale of a forward activation, except that an infinite max gives 1 instead of NaN:
+    the forward keeps the split's saturation rule (an infinite activation acts as the largest fp16)
+    instead of making its outputs NaN."""
+    return torch.nan_to_num(_absmax_scale(x), nan=1.0)
+
+
+def _forward_scales(scale2, x):
+    """(inv, act) of an fp16-mode forward with weight scales scale2 = (s_w, 1/s_w): act = s_x of
+    _forward_scale(x), inv = 1/(s_w s_x) folded into one fp32 power of two. The fold underflows to
+    0 when s_w s_x > 2^149, i.e. max|W| max|x| below about 2^-131 (both pre-scales near their 2^126
+    cap): the products, all of them then below fp32's normal range, are lost and y is the bias."""
+    s_x = _forward_scale(x)
+    return scale2[1:] * s_x[1:], s_x[:1]
+
+
+def _tc_dev(x, blob, inv, shift, cout, act_scale=None, f16=False):
     """Generic wgmma layer with a device-packed blob: inv (1-element device tensor) = the total
-    inverse pre-scale, act_scale (1-element) = activation pre-scale or None."""
+    inverse pre-scale, act_scale (1-element) = activation pre-scale or None; f16: the
+    one-product twin."""
     B, C, P = x.shape
     with torch.cuda.device(x.device):
         out = torch.empty((B, cout, P), dtype=torch.float32, device=x.device)
-        ops._call("sonet_pointwise_tc_forward_dev", _C.ptr(x), C, B, P, _C.ptr(blob), _C.ptr(inv),
-                  _C.ptr(act_scale), _C.ptr(shift), int(cout), 0, 1, _C.ptr(out), None,
+        ops._call(_f16("sonet_pointwise_tc_forward_dev", f16), _C.ptr(x), C, B, P, _C.ptr(blob),
+                  _C.ptr(inv), _C.ptr(act_scale), _C.ptr(shift), int(cout), 0, 1, _C.ptr(out), None,
                   ops._stream(x))
     return out
 
@@ -222,8 +258,9 @@ def tc_eligible(cin, cout, rows):
     return cin >= 32 and cout >= 32 and rows >= 256
 
 
-def wgrad_tc(dy, x):
-    """dW [Cout,Cin] = sum_{b,p} dy[b,:,p] x[b,:,p]^T on wgmma (csrc/train.cu: sonet_wgrad_tc_f32)."""
+def wgrad_tc(dy, x, f16=False):
+    """dW [Cout,Cin] = sum_{b,p} dy[b,:,p] x[b,:,p]^T on wgmma (csrc/train.cu: sonet_wgrad_tc_f32,
+    with f16 its one-product twin sonet_wgrad_tc_f16: same splits and scratch)."""
     B, Cout, P = dy.shape
     Cin = x.shape[1]
     lib = _C.lib()
@@ -241,9 +278,9 @@ def wgrad_tc(dy, x):
         part = _scratch(dev, splits * Cin * Cout, torch.float32, _WGRAD_CACHE.setdefault("part", {}))
         small = torch.empty(int(lib.sonet_wgrad_small_floats(Cout)), dtype=torch.float32, device=dev)
         dWT = torch.empty((Cin, Cout), dtype=torch.float32, device=dev)
-        ops._call("sonet_wgrad_tc_f32", _C.ptr(dy), _C.ptr(x), B, Cout, Cin, P, splits, _C.ptr(dyT),
-                  _C.ptr(blob), _C.ptr(part), _C.ptr(small), _C.ptr(dWT), ops._stream(dy),
-                  kernels=8 if splits > 1 else 7)
+        ops._call(_f16("sonet_wgrad_tc_f32", f16), _C.ptr(dy), _C.ptr(x), B,
+                  Cout, Cin, P, splits, _C.ptr(dyT), _C.ptr(blob), _C.ptr(part), _C.ptr(small),
+                  _C.ptr(dWT), ops._stream(dy), kernels=8 if splits > 1 else 7)
     return dWT.t()
 
 
@@ -259,16 +296,21 @@ WGRAD_MAX_KPI = 32
 
 class ConvTC(torch.autograd.Function):
     """x [B,Cin,P], W [Cout,Cin], b [Cout] or None -> W x + b. Forward, dgrad and wgrad all run on
-    the generic wgmma layer kernel (fp16 hi/lo split, fp32 accumulation)."""
+    the generic wgmma layer kernel (fp16 hi/lo split, fp32 accumulation; under train_f16() one fp16
+    product per MAC, the forward's x pre-scaled by a power of two like the dgrad's dy)."""
 
     @staticmethod
     def forward(ctx, x, W, b):
         x = x.contiguous()
         Wc = W.contiguous()
+        f16 = train_f16()
         blob, scale2 = _pack_device(Wc, False)
-        y = _tc_dev(x, blob, scale2[1:], None if b is None else b.contiguous(), Wc.shape[0])
+        shift = None if b is None else b.contiguous()
+        inv, act = _forward_scales(scale2, x) if f16 else (scale2[1:], None)
+        y = _tc_dev(x, blob, inv, shift, Wc.shape[0], act_scale=act, f16=f16)
         ctx.save_for_backward(x, Wc)
         ctx.has_bias = b is not None
+        ctx.f16 = f16
         return y
 
     @staticmethod
@@ -280,10 +322,10 @@ class ConvTC(torch.autograd.Function):
             blob, scale2 = _pack_device(W, True)                     # dgrad: dx = W^T dy
             s_dy = _absmax_scale(dy)
             inv = scale2[1:] * s_dy[1:]
-            dx = _tc_dev(dy, blob, inv, None, W.shape[1], act_scale=s_dy[:1])
+            dx = _tc_dev(dy, blob, inv, None, W.shape[1], act_scale=s_dy[:1], f16=ctx.f16)
         if ctx.needs_input_grad[1]:
             if W.shape[0] % 64 == 0 and W.shape[1] >= 16 and WGRAD_TC:
-                dW = wgrad_tc(dy, x)
+                dW = wgrad_tc(dy, x, ctx.f16)
             else:                                                    # thin layers: cuBLAS fp32
                 with _cublas_strict_fp32():
                     dW = torch.einsum("bop,bip->oi", dy, x)
@@ -319,10 +361,20 @@ class IndexMaxGather(torch.autograd.Function):
         return gd, None, None
 
 
-def _cudnn_strict_fp32():
+def _cudnn_strict_fp32(tf32=False):
     c = torch.backends.cudnn
     return c.flags(enabled=True, benchmark=c.benchmark, deterministic=c.deterministic,
-                   allow_tf32=False)
+                   allow_tf32=tf32)
+
+
+def _conv_forward(ctx, tf32, x, weight, bias, stride, padding, dilation, groups):
+    ctx.tf32 = tf32
+    with _cudnn_strict_fp32(tf32):
+        y = torch.ops.aten.convolution(x, weight, bias, stride, padding, dilation, False,
+                                       [0] * len(stride), groups)
+    ctx.save_for_backward(x, weight)
+    ctx.conf = (None if bias is None else [bias.shape[0]], stride, padding, dilation, groups)
+    return y
 
 
 class ConvStrict(torch.autograd.Function):
@@ -333,29 +385,40 @@ class ConvStrict(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, bias, stride, padding, dilation, groups):
-        with _cudnn_strict_fp32():
-            y = torch.ops.aten.convolution(x, weight, bias, stride, padding, dilation, False,
-                                           [0] * len(stride), groups)
-        ctx.save_for_backward(x, weight)
-        ctx.conf = (None if bias is None else [bias.shape[0]], stride, padding, dilation, groups)
-        return y
+        return _conv_forward(ctx, False, x, weight, bias, stride, padding, dilation, groups)
 
     @staticmethod
     def backward(ctx, dy):
         x, weight = ctx.saved_tensors
         bias_sizes, stride, padding, dilation, groups = ctx.conf
         need = ctx.needs_input_grad
-        with _cudnn_strict_fp32():
+        with _cudnn_strict_fp32(ctx.tf32):
             dx, dw, db = torch.ops.aten.convolution_backward(
                 dy.contiguous(), x, weight, bias_sizes, stride, padding, dilation, False,
                 [0] * len(stride), groups, [need[0], need[1], bias_sizes is not None and need[2]])
         return dx, dw, db, None, None, None, None
 
 
+class ConvTF32(ConvStrict):
+    """ConvStrict with TF32 allowed in the forward and the backward (the reference's default),
+    whatever the global flag says when backward() runs: the decoder's cuDNN convolutions under
+    train_f16()."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, stride, padding, dilation, groups):
+        return _conv_forward(ctx, True, x, weight, bias, stride, padding, dilation, groups)
+
+
 def conv_strict(conv, x):
     """conv (nn.Conv1d / nn.Conv2d, zero padding) applied to x through ConvStrict."""
     return ConvStrict.apply(x, conv.weight, conv.bias, list(conv.stride), list(conv.padding),
                             list(conv.dilation), conv.groups)
+
+
+def conv_tf32(conv, x):
+    """conv applied to x through ConvTF32."""
+    return ConvTF32.apply(x, conv.weight, conv.bias, list(conv.stride), list(conv.padding),
+                          list(conv.dilation), conv.groups)
 
 
 @contextlib.contextmanager
@@ -490,11 +553,14 @@ class UpConvTC(torch.autograd.Function):
     [B,Cout,2H,2W] as four parity GEMMs (Wg = the taps that coincide after up-sampling, summed).
       forward  z = grouped parity GEMMs (Wg, x) + b, Wg folded and packed on the device
       dgrad    dx = Wd D: D [B][16*Cout][H*W] = dz gathered at each (parity, tap, co)'s offset
-      wgrad    dWg[g] = dz_g xcol_g^T per parity (xcol recomputed from x), dW = adjoint fold"""
+      wgrad    dWg[g] = dz_g xcol_g^T per parity (xcol recomputed from x), dW = adjoint fold
+    Under train_f16() all three take the one-product twins, the forward's x pre-scaled by a power
+    of two (max|im2col(x)| = max|x|)."""
 
     @staticmethod
     def forward(ctx, x, W, b):
         x = x.contiguous()
+        f16 = train_f16()
         Wc = W.contiguous()
         B, Cin, H, Wd = x.shape
         Cout = Wc.shape[0]
@@ -510,13 +576,16 @@ class UpConvTC(torch.autograd.Function):
             z = torch.empty((B, Cout, 4 * P), dtype=torch.float32, device=dev)
             scratch = (torch.empty(4 * splits * B * Cout * P, dtype=torch.float32, device=dev)
                        if splits > 1 else None)
-            ops._call("sonet_pointwise_tc_grouped_forward_dev", _C.ptr(xin), xin.shape[1], B, P,
-                      _C.ptr(blob),
-                      per, _C.ptr(scale2[1:]), _C.ptr(None if b is None else b.contiguous()), Cout,
-                      ops.ACT_NONE, 4, splits, Wd, Wd if conv else 0, 4 * P, 0, _C.ptr(z),
-                      _C.ptr(scratch), ops._stream(x), kernels=2 if splits > 1 else 1)
+            shift = None if b is None else b.contiguous()
+            inv, act = _forward_scales(scale2, x) if f16 else (scale2[1:], None)
+            scales = (_C.ptr(inv), _C.ptr(act)) if f16 else (_C.ptr(inv),)   # the twin's extra argument
+            ops._call(_f16("sonet_pointwise_tc_grouped_forward_dev", f16), _C.ptr(xin), xin.shape[1], B,
+                      P, _C.ptr(blob), per, *scales, _C.ptr(shift), Cout, ops.ACT_NONE, 4, splits, Wd,
+                      Wd if conv else 0, 4 * P, 0, _C.ptr(z), _C.ptr(scratch), ops._stream(x),
+                      kernels=2 if splits > 1 else 1)
         ctx.save_for_backward(x, Wc)
         ctx.has_bias = b is not None
+        ctx.f16 = f16
         return z.view(B, Cout, 2 * H, 2 * Wd)
 
     @staticmethod
@@ -542,7 +611,8 @@ class UpConvTC(torch.autograd.Function):
                 dx = torch.empty((B, Cin, P), dtype=torch.float32, device=dev)
                 scratch = (torch.empty(splits * B * Cin * P, dtype=torch.float32, device=dev)
                            if splits > 1 else None)
-                ops._call("sonet_pointwise_tc_forward_dev", _C.ptr(D), 16 * Cout, B, P, _C.ptr(blob),
+                ops._call(_f16("sonet_pointwise_tc_forward_dev", ctx.f16), _C.ptr(D), 16 * Cout, B, P,
+                          _C.ptr(blob),
                           _C.ptr(scale2[1:] * s_dz[1:]), _C.ptr(s_dz[:1]), None, Cin, 0, splits,
                           _C.ptr(dx), _C.ptr(scratch), ops._stream(dz),
                           kernels=2 if splits > 1 else 1)
@@ -552,7 +622,7 @@ class UpConvTC(torch.autograd.Function):
                 dzg = dz.view(B, Cout, H, 2, Wd, 2).permute(3, 5, 0, 1, 2, 4).reshape(4, B, Cout, P)
                 xcol = ops.upconv_im2col(x).view(4, B, 4 * Cin, P)
                 if Cout % 64 == 0 and WGRAD_TC:
-                    dWT = torch.stack([wgrad_tc(dzg[g], xcol[g]).t() for g in range(4)])
+                    dWT = torch.stack([wgrad_tc(dzg[g], xcol[g], ctx.f16).t() for g in range(4)])
                 else:
                     with _cublas_strict_fp32():
                         dWT = torch.einsum("gbkp,gbop->gko", xcol, dzg)
