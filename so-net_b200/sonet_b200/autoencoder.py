@@ -1,7 +1,7 @@
 """autoencoder.Model — caller-facing wrapper of models/autoencoder.py:13-161 on the H100
 networks: encoder + decoder + Chamfer, all on the hand-written kernels in eval mode.
-Double-buffered asynchronous set_input and CUDA-graph replay of test_model():
-_model_base.GraphedModel."""
+Double-buffered asynchronous set_input and CUDA-graph replay of test_model() and
+optimize(): _model_base.GraphedModel."""
 import torch
 
 from . import losses, networks
@@ -23,7 +23,6 @@ class Model(GraphedModel):
         self.encoder = networks.Encoder(opt).to(dev)
         self.decoder = networks.Decoder(opt).to(dev)
         self.chamfer_criteria = losses.ChamferLoss(opt).to(dev)
-        self._optim = None
         B, N, M, K = opt.batch_size, opt.input_pc_num, opt.node_num, max(opt.som_k, 1)
         self._INPUT_SPEC = (
             ("input_pc", lambda d: torch.empty(B, 3, N, dtype=torch.float32, device=d)),
@@ -84,17 +83,17 @@ class Model(GraphedModel):
             self.forward(is_train=False)
             self._losses(train=False)
 
-    def optimize(self, epoch=None):
-        """One training step (models/autoencoder.py:70-103) on the differentiable PyTorch path."""
-        if self._optim is None:
-            self._optim = (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr,
-                                            betas=(0.9, 0.999)),
-                           torch.optim.Adam(self.decoder.parameters(), lr=self.opt.lr,
-                                            betas=(0.9, 0.999)))
+    def _make_optimizers(self):
+        return (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr, betas=(0.9, 0.999)),
+                torch.optim.Adam(self.decoder.parameters(), lr=self.opt.lr, betas=(0.9, 0.999)))
+
+    def _train_step(self, epoch, forward):
+        """One training step (models/autoencoder.py:70-103) on the differentiable PyTorch path;
+        optimize() runs it (GraphedModel.optimize)."""
         self.encoder.train()
         self.decoder.train()
         with torch.enable_grad():
-            self.forward(is_train=True, epoch=epoch)
+            forward(True, epoch)
             self.encoder.zero_grad()
             self.decoder.zero_grad()
             self._losses(train=True)

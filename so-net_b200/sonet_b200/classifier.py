@@ -2,8 +2,8 @@
 forward / test_model / optimize), built on the H100 networks. This is the public API bench.py
 times end to end: host tensors in through set_input, scores out.
 
-set_input is double-buffered and asynchronous, test_model() can replay as one CUDA graph
-(enable_cuda_graph) — see _model_base.GraphedModel.
+set_input is double-buffered and asynchronous, test_model() and optimize() can each replay as one
+CUDA graph (enable_cuda_graph, enable_train_graph) — see _model_base.GraphedModel.
 """
 import torch
 import torch.nn as nn
@@ -21,7 +21,6 @@ class Model(GraphedModel):
         self.encoder = networks.Encoder(opt).to(dev)
         self.classifier = networks.Classifier(opt).to(dev)
         self.softmax_criteria = nn.CrossEntropyLoss().to(dev)
-        self._optim = None
         B, N, M, K = opt.batch_size, opt.input_pc_num, opt.node_num, max(opt.som_k, 1)
         self._INPUT_SPEC = (
             ("input_pc", lambda d: torch.empty(B, 3, N, dtype=torch.float32, device=d)),
@@ -50,11 +49,14 @@ class Model(GraphedModel):
         """models/classifier.py:64-72."""
         self._set_input(input_pc, input_sn, input_label, input_node, input_node_knn_I)
 
-    def forward(self, is_train=False, epoch=None):
-        s = self._wait_inputs()
+    def _forward(self, is_train, epoch):
         self.feature = self.encoder(self.pc, self.sn, self.input_node, self.input_node_knn_I,
                                     is_train, epoch)
         self.score = self.classifier(self.feature, epoch)
+
+    def forward(self, is_train=False, epoch=None):
+        s = self._wait_inputs()
+        self._forward(is_train, epoch)
         self._mark_consumed(s)
 
     def test_model(self):
@@ -66,17 +68,19 @@ class Model(GraphedModel):
             self.forward(is_train=False)
             self.loss = self.softmax_criteria(self.score, self.label)
 
-    def optimize(self, epoch=None):
-        """One training step (models/classifier.py:78-99) on the differentiable PyTorch path."""
-        if self._optim is None:
-            self._optim = (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr,
-                                            betas=(0.9, 0.999), weight_decay=0),
-                           torch.optim.Adam(self.classifier.parameters(), lr=self.opt.lr,
-                                            betas=(0.9, 0.999), weight_decay=0))
+    def _make_optimizers(self):
+        return (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr,
+                                 betas=(0.9, 0.999), weight_decay=0),
+                torch.optim.Adam(self.classifier.parameters(), lr=self.opt.lr,
+                                 betas=(0.9, 0.999), weight_decay=0))
+
+    def _train_step(self, epoch, forward):
+        """One training step (models/classifier.py:78-99) on the differentiable PyTorch path;
+        optimize() runs it (GraphedModel.optimize)."""
         self.encoder.train()
         self.classifier.train()
         with torch.enable_grad():
-            self.forward(is_train=True, epoch=epoch)
+            forward(True, epoch)
             self.encoder.zero_grad()
             self.classifier.zero_grad()
             self.loss = self.softmax_criteria(self.score, self.label)

@@ -64,11 +64,16 @@ class _MomentumDecayBatchNorm(_BatchNorm):
         self.momentum_decay = momentum_decay
         self.momentum_original = self.momentum
 
-    def forward(self, input, epoch=None):
+    def momentum_at(self, epoch):
+        """The momentum a train forward at `epoch` uses: the decayed one from epoch 1 on when a
+        decay step is set, else the current one (the last epoch's, or the constructor's)."""
         step = self.momentum_decay_step
         if epoch is not None and epoch >= 1 and step is not None and step > 0:
-            self.momentum = max(self.momentum_original * (self.momentum_decay ** (epoch // step)),
-                                0.01)
+            return max(self.momentum_original * (self.momentum_decay ** (epoch // step)), 0.01)
+        return self.momentum
+
+    def forward(self, input, epoch=None):
+        self.momentum = self.momentum_at(epoch)
         if self.training and train_ops.EXCHANGE is not None:
             # data-parallel training synchronises the BatchNorms on the train kernels only; this
             # one would normalise each rank's shard by its own statistics

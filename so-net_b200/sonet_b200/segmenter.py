@@ -3,7 +3,7 @@
 forward() hands the Segmenter the node-level features and the point->node assignment directly
 (Segmenter.forward_nodes) instead of the three per-point torch.gather copies of
 models/segmenter.py:90-98. Double-buffered asynchronous set_input and CUDA-graph replay of
-test_model(): _model_base.GraphedModel.
+test_model() and optimize(): _model_base.GraphedModel.
 """
 import torch
 
@@ -22,7 +22,6 @@ class Model(GraphedModel):
         self.segmenter = networks.Segmenter(opt).to(dev)
         self.softmax_segmenter = losses.CrossEntropyLossSeg().to(dev)
         self.encoder.fuse_pool = False   # the head reads first_pn_out of every forward
-        self._optim = None
         B, N, M, K = opt.batch_size, opt.input_pc_num, opt.node_num, max(opt.som_k, 1)
         self._INPUT_SPEC = (
             ("input_pc", lambda d: torch.empty(B, 3, N, dtype=torch.float32, device=d)),
@@ -77,17 +76,19 @@ class Model(GraphedModel):
             self.forward(is_train=False)
             self._loss()
 
-    def optimize(self, epoch=None):
-        """One training step (models/segmenter.py:111-123) on the differentiable PyTorch path."""
-        if self._optim is None:
-            self._optim = (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr,
-                                            betas=(0.9, 0.999), weight_decay=0),
-                           torch.optim.Adam(self.segmenter.parameters(), lr=self.opt.lr,
-                                            betas=(0.9, 0.999), weight_decay=0))
+    def _make_optimizers(self):
+        return (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr,
+                                 betas=(0.9, 0.999), weight_decay=0),
+                torch.optim.Adam(self.segmenter.parameters(), lr=self.opt.lr,
+                                 betas=(0.9, 0.999), weight_decay=0))
+
+    def _train_step(self, epoch, forward):
+        """One training step (models/segmenter.py:111-123) on the differentiable PyTorch path;
+        optimize() runs it (GraphedModel.optimize)."""
         self.encoder.train()
         self.segmenter.train()
         with torch.enable_grad():
-            self.forward(is_train=True, epoch=epoch)
+            forward(True, epoch)
             self.encoder.zero_grad()
             self.segmenter.zero_grad()
             self.loss_segmenter = self.softmax_segmenter(self.score_segmenter, self.seg)

@@ -51,12 +51,22 @@ def _f16(name, f16):
     return (name[:-4] if name.endswith("_f32") else name) + "_f16"
 
 
-def _scratch(dev, n, dtype, cache={}):
+def _scratch(dev, n, dtype, cache=None):
+    cache = _SCRATCH if cache is None else cache
     key = (dev, dtype)
     buf = cache.get(key)
     if buf is None or buf.numel() < n:
         buf = cache[key] = torch.empty(max(n, 1), dtype=dtype, device=dev)
     return buf
+
+
+_SCRATCH = {}
+
+
+def scratch_buffers():
+    """Every scratch buffer the train ops hold now. A captured CUDA graph keeps these alive: a
+    larger step replaces a buffer in its cache, and the graph must not write into freed memory."""
+    return list(_SCRATCH.values()) + [b for c in _WGRAD_CACHE.values() for b in c.values()]
 
 
 # The BatchNorm exchange of data-parallel training (dist.DataParallelTraining), or None. While one is
@@ -487,9 +497,7 @@ def norm_act_train(y0, norm, act, epoch=None, size=None):
     if n == 1:         # F.batch_norm's check: a batch statistic of one value is undefined
         raise ValueError("Expected more than 1 value per channel when training, got input size "
                          "{}".format(size))
-    step = norm.momentum_decay_step
-    if epoch is not None and epoch >= 1 and step is not None and step > 0:
-        norm.momentum = max(norm.momentum_original * (norm.momentum_decay ** (epoch // step)), 0.01)
+    norm.momentum = norm.momentum_at(epoch)
     y, mean, var = BNActTrain.apply(y0, norm.weight, norm.bias, norm.eps, act)
     with torch.no_grad():
         m = norm.momentum
