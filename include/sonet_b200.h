@@ -535,6 +535,38 @@ int sonet_seg_iou_cpu_f32(const float* score, const long long* seg, const long l
                           int C, int N, const int32_t* part_offsets, const int32_t* part_ids,
                           int num_categories, double* iou_shape, long long* pred, int32_t* correct,
                           int thread_num);
+/* Ragged twin over every point of each shape: score [T,C] f32 point-major, seg [T] int64, label [B]
+ * int64, offsets [B+1] int64 (shape b owns points offsets[b] .. offsets[b+1]); the same argmax and
+ * per-part rule, one launch. pred [T] int64 and correct [B] int32 nullable. The device entry reads
+ * offsets on the device only: a shape whose offsets are out of order or outside [0,T] yields
+ * iou_shape[b] = NaN, as does a label outside the table. */
+int sonet_seg_iou_ragged_f32(const float* score, const long long* seg, const long long* label,
+                             const long long* offsets, int B, int C, long long T,
+                             const int32_t* part_offsets, const int32_t* part_ids, int num_categories,
+                             double* iou_shape, long long* pred, int32_t* correct, sonet_stream_t stream);
+/* The same over host pointers; validates offsets (0 .. T, non-decreasing), the table and every
+ * label: SONET_ERR_BAD_ARG otherwise. */
+int sonet_seg_iou_ragged_cpu_f32(const float* score, const long long* seg, const long long* label,
+                                 const long long* offsets, int B, int C, long long T,
+                                 const int32_t* part_offsets, const int32_t* part_ids,
+                                 int num_categories, double* iou_shape, long long* pred,
+                                 int32_t* correct, int thread_num);
+
+/* SOM assignment and decentring of one chunk of a ragged point set for the segmenter's per-point
+ * head (segmenter.Model.score_points). points [total,6] f32 (xyz | normal), offsets [B+1] int64
+ * (device; cloud b owns rows offsets[b] .. offsets[b+1]), node [B,3,M] the loader's SOM nodes,
+ * cluster_mean [B,3,M] the encoder's centres of the sampled forward. Rows [row0, row0+rows) find their
+ * k nearest nodes of their cloud with sonet_som_assign's arithmetic and tie rule and are written
+ * copy-major over k*rows_pad columns (column s*rows_pad + r: copy s of row r): gidx [k*rows_pad]
+ * int32 = b*M + node (a flat index into the node-level addend laid out [C, B*M]); x_aug
+ * [3(+3), k*rows_pad] = xyz - centre (| normal); pt [9(+3), k*rows_pad] = x_dec | xyz | centre
+ * (| normal). with_sn: 1 writes the normal channels. Columns of rows >= rows are zero, node 0.
+ * 1 <= M <= 256, 1 <= k <= min(4, M), rows <= rows_pad, row0 + rows <= total. offsets are not read
+ * on the host (the caller validates them); one launch. */
+int sonet_seg_points_assign_f32(const float* points, long long total, const long long* offsets, int B,
+                                const float* node, const float* cluster_mean, int M, int k, int with_sn,
+                                long long row0, int rows, int rows_pad, int32_t* gidx, float* x_aug,
+                                float* pt, sonet_stream_t stream);
 
 /* SHREC'16 same-label retrieval ranking (shrec16/test.py:64-99). feature [Q,D] f32; label_in [Q]
  * int64, or NULL for the row argmax (lowest index on ties, first NaN wins). For each query q, the

@@ -128,6 +128,85 @@ __global__ void __launch_bounds__(SEG_IOU_THREADS)
   }
 }
 
+// Ragged twin: score [T,C] point-major, seg [T], shape b owns points offsets[b] .. offsets[b+1]. The
+// same argmax, counters and IoU arithmetic as seg_iou_kernel, one CTA per shape; pred [T] holds the
+// argmax of every point. A shape whose offsets are not inside [0, T] and ordered gets NaN.
+__global__ void __launch_bounds__(SEG_IOU_THREADS)
+    seg_iou_ragged_kernel(const float* __restrict__ score, const long long* __restrict__ seg,
+                          const long long* __restrict__ label, const long long* __restrict__ offsets,
+                          int C, long long T, const int32_t* __restrict__ part_offsets,
+                          const int32_t* __restrict__ part_ids, int num_categories,
+                          double* __restrict__ iou_shape, long long* __restrict__ pred,
+                          int32_t* __restrict__ correct) {
+  __shared__ int s_ids[SEG_IOU_MAX_PARTS];
+  __shared__ int s_g[SEG_IOU_MAX_PARTS], s_p[SEG_IOU_MAX_PARTS], s_i[SEG_IOU_MAX_PARTS];
+  __shared__ double s_iou[SEG_IOU_MAX_PARTS];
+  __shared__ int s_correct;
+
+  const int b = blockIdx.x;
+  const long long lab = label[b];
+  long long n0 = offsets[b], n1 = offsets[b + 1];
+  const bool range_ok = n0 >= 0 && n0 <= n1 && n1 <= T;
+  if (!range_ok) n0 = n1 = 0;
+  int first = 0, np = 0;
+  if (lab >= 0 && lab < num_categories) {
+    first = part_offsets[lab];
+    np = part_offsets[lab + 1] - first;
+  }
+  const bool valid = range_ok && np >= 1 && np <= SEG_IOU_MAX_PARTS;
+  if (!valid) np = 0;
+  for (int j = threadIdx.x; j < np; j += SEG_IOU_THREADS) {
+    s_ids[j] = part_ids[first + j];
+    s_g[j] = s_p[j] = s_i[j] = 0;
+  }
+  if (threadIdx.x == 0) s_correct = 0;
+  __syncthreads();
+
+  int my_correct = 0;
+  for (long long n = n0 + threadIdx.x; n < n1; n += SEG_IOU_THREADS) {
+    const float* row = score + static_cast<size_t>(n) * C;
+    float best = __ldg(row);
+    int bi = 0;
+#pragma unroll 10
+    for (int c = 1; c < C; ++c) argmax_step(__ldg(row + c), c, best, bi);
+    const long long s = __ldg(seg + n);
+    my_correct += (s == bi);
+    if (pred != nullptr) pred[n] = bi;
+    int gs = -1, ps = -1;
+    for (int j = 0; j < np; ++j) {
+      const int id = s_ids[j];
+      if (gs < 0 && id == s) gs = j;
+      if (ps < 0 && id == bi) ps = j;
+    }
+    if (gs >= 0) atomicAdd(&s_g[gs], 1);
+    if (ps >= 0) atomicAdd(&s_p[ps], 1);
+    if (gs >= 0 && gs == ps) atomicAdd(&s_i[gs], 1);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) my_correct += __shfl_xor_sync(0xffffffffu, my_correct, o);
+  if ((threadIdx.x & 31) == 0 && my_correct != 0) atomicAdd(&s_correct, my_correct);
+  __syncthreads();
+
+  if (threadIdx.x >= 32) return;
+  const int lane = threadIdx.x;
+  for (int j = lane; j < np; j += 32) {
+    int f = 0;
+    while (s_ids[f] != s_ids[j]) ++f;
+    s_iou[j] = part_iou(s_g[f], s_p[f], s_i[f]);
+  }
+  __syncwarp();
+  if (lane == 0) {
+    if (valid) {
+      double sum = 0.0;
+      for (int j = 0; j < np; ++j) sum += s_iou[j];
+      iou_shape[b] = sum / static_cast<double>(np);
+    } else {
+      iou_shape[b] = __longlong_as_double(0x7ff8000000000000LL);
+    }
+    if (correct != nullptr) correct[b] = s_correct;
+  }
+}
+
 // ---- host entry: the same arithmetic over host pointers -----------------------------------------
 static void seg_iou_cpu_range(const float* score, const long long* seg, const long long* label, int C,
                               int N, const int32_t* part_offsets, const int32_t* part_ids,
@@ -154,6 +233,47 @@ static void seg_iou_cpu_range(const float* score, const long long* seg, const lo
       const int bi = bis[n];
       corr += (s == bi);
       if (pred != nullptr) pred[static_cast<size_t>(b) * N + n] = bi;
+      int gs = -1, ps = -1;
+      for (int j = 0; j < np; ++j) {
+        if (gs < 0 && ids[j] == s) gs = j;
+        if (ps < 0 && ids[j] == bi) ps = j;
+      }
+      if (gs >= 0) ++g[gs];
+      if (ps >= 0) ++p[ps];
+      if (gs >= 0 && gs == ps) ++i[gs];
+    }
+    double sum = 0.0;
+    for (int j = 0; j < np; ++j) {
+      int f = 0;
+      while (ids[f] != ids[j]) ++f;
+      sum += part_iou(g[f], p[f], i[f]);
+    }
+    iou_shape[b] = sum / static_cast<double>(np);
+    if (correct != nullptr) correct[b] = corr;
+  }
+}
+
+static void seg_iou_ragged_cpu_range(const float* score, const long long* seg, const long long* label,
+                                     const long long* offsets, int C, const int32_t* part_offsets,
+                                     const int32_t* part_ids, double* iou_shape, long long* pred,
+                                     int32_t* correct, int b0, int b1) {
+  std::vector<int> g, p, i;
+  for (int b = b0; b < b1; ++b) {
+    const int first = part_offsets[label[b]];
+    const int np = part_offsets[label[b] + 1] - first;
+    const int32_t* ids = part_ids + first;
+    g.assign(np, 0);
+    p.assign(np, 0);
+    i.assign(np, 0);
+    int corr = 0;
+    for (long long n = offsets[b]; n < offsets[b + 1]; ++n) {
+      const float* row = score + static_cast<size_t>(n) * C;
+      float best = row[0];
+      int bi = 0;
+      for (int c = 1; c < C; ++c) argmax_step(row[c], c, best, bi);
+      const long long s = seg[n];
+      corr += (s == bi);
+      if (pred != nullptr) pred[n] = bi;
       int gs = -1, ps = -1;
       for (int j = 0; j < np; ++j) {
         if (gs < 0 && ids[j] == s) gs = j;
@@ -226,6 +346,72 @@ extern "C" int sonet_seg_iou_cpu_f32(const float* score, const long long* seg, c
     const int b1 = static_cast<int>(static_cast<long long>(B) * (t + 1) / T);
     pool.emplace_back(seg_iou_cpu_range, score, seg, label, C, N, part_offsets, part_ids, iou_shape,
                       pred, correct, b0, b1);
+  }
+  for (auto& th : pool) th.join();
+  return SONET_OK;
+}
+
+extern "C" int sonet_seg_iou_ragged_f32(const float* score, const long long* seg, const long long* label,
+                                        const long long* offsets, int B, int C, long long T,
+                                        const int32_t* part_offsets, const int32_t* part_ids,
+                                        int num_categories, double* iou_shape, long long* pred,
+                                        int32_t* correct, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE(B >= 0 && C >= 1 && T >= 0 && num_categories >= 1, "seg_iou_ragged: bad dimension");
+  if (B == 0) return SONET_OK;
+  SONET_REQUIRE(score && seg && label && offsets && part_offsets && part_ids && iou_shape,
+                "seg_iou_ragged: null pointer");
+  seg_iou_ragged_kernel<<<B, SEG_IOU_THREADS, 0, as_stream(stream)>>>(
+      score, seg, label, offsets, C, T, part_offsets, part_ids, num_categories, iou_shape, pred,
+      correct);
+  return check_launch("seg_iou_ragged");
+}
+
+extern "C" int sonet_seg_iou_ragged_cpu_f32(const float* score, const long long* seg,
+                                            const long long* label, const long long* offsets, int B,
+                                            int C, long long T, const int32_t* part_offsets,
+                                            const int32_t* part_ids, int num_categories,
+                                            double* iou_shape, long long* pred, int32_t* correct,
+                                            int thread_num) {
+  using namespace sonet;
+  SONET_REQUIRE(B >= 0 && C >= 1 && T >= 0 && num_categories >= 1, "seg_iou_ragged_cpu: bad dimension");
+  SONET_REQUIRE(thread_num >= 1, "seg_iou_ragged_cpu: thread_num must be >= 1");
+  if (B == 0) return SONET_OK;
+  SONET_REQUIRE(score && seg && label && offsets && part_offsets && part_ids && iou_shape,
+                "seg_iou_ragged_cpu: null pointer");
+  SONET_REQUIRE(offsets[0] == 0 && offsets[B] == T,
+                "seg_iou_ragged_cpu: offsets must run from 0 to T=%lld (got %lld .. %lld)", T,
+                offsets[0], offsets[B]);
+  for (int b = 0; b < B; ++b)
+    SONET_REQUIRE(offsets[b] <= offsets[b + 1], "seg_iou_ragged_cpu: offsets decrease at shape %d", b);
+  SONET_REQUIRE(part_offsets[0] == 0, "seg_iou_ragged_cpu: part_offsets[0] must be 0");
+  for (int k = 0; k < num_categories; ++k) {
+    const int np = part_offsets[k + 1] - part_offsets[k];
+    SONET_REQUIRE(np >= 1 && np <= SEG_IOU_MAX_PARTS,
+                  "seg_iou_ragged_cpu: category %d has %d parts (1..%d allowed)", k, np,
+                  SEG_IOU_MAX_PARTS);
+  }
+  for (int j = 0; j < part_offsets[num_categories]; ++j)
+    SONET_REQUIRE(part_ids[j] >= 0 && part_ids[j] < C,
+                  "seg_iou_ragged_cpu: part id %d outside [0, C=%d)", part_ids[j], C);
+  for (int b = 0; b < B; ++b)
+    SONET_REQUIRE(label[b] >= 0 && label[b] < num_categories,
+                  "seg_iou_ragged_cpu: label[%d]=%lld outside the part table (%d categories)", b,
+                  label[b], num_categories);
+  // at least 2^20 score elements per thread, as the fixed-N entry
+  const long long work = (T * C) >> 20;
+  const int T_ = static_cast<int>(std::min<long long>({thread_num, B, std::max(work, 1LL)}));
+  if (T_ == 1) {
+    seg_iou_ragged_cpu_range(score, seg, label, offsets, C, part_offsets, part_ids, iou_shape, pred,
+                             correct, 0, B);
+    return SONET_OK;
+  }
+  std::vector<std::thread> pool;
+  for (int t = 0; t < T_; ++t) {
+    const int b0 = static_cast<int>(static_cast<long long>(B) * t / T_);
+    const int b1 = static_cast<int>(static_cast<long long>(B) * (t + 1) / T_);
+    pool.emplace_back(seg_iou_ragged_cpu_range, score, seg, label, offsets, C, part_offsets, part_ids,
+                      iou_shape, pred, correct, b0, b1);
   }
   for (auto& th : pool) th.join();
   return SONET_OK;

@@ -212,6 +212,27 @@ class DeviceDataset:
     def __len__(self):
         return len(self.counts)
 
+    def full_clouds(self, index):
+        """(points [sum P_i, 6] f32, offsets [len(index)+1] int64, seg [sum P_i] int64 or None) of
+        the clouds `index`, all their points, in index order, on the dataset's device: the ragged
+        input of segmenter.Model.score_points and losses.compute_iou_full for the batch that
+        batch(index, ...) draws. A run of consecutive clouds is a view of the resident points;
+        otherwise the rows are gathered."""
+        index = np.asarray(index, dtype=np.int64).reshape(-1)
+        if len(index) == 0 or index.min() < 0 or index.max() >= len(self.counts):
+            raise ValueError("full_clouds: index must name clouds in [0, %d)" % len(self.counts))
+        counts = self.counts[index]
+        offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)) \
+            .to(self.device)
+        starts = np.concatenate([[0], np.cumsum(self.counts)])[index]
+        if (np.diff(index) == 1).all():
+            rows = slice(int(starts[0]), int(starts[0] + counts.sum()))
+        else:
+            rows = torch.from_numpy(np.concatenate(
+                [np.arange(s, s + c) for s, c in zip(starts, counts)])).to(self.device)
+        seg = None if self.seg is None else self.seg[rows].long()
+        return self.data[rows], offsets, seg
+
     def batch(self, index, opt, train, rng=None, seed=0, host_noise=False, shard=None):
         """The collated batch of the loader `opt.dataset` selects (autoencoder/train.py:25-36) for
         the clouds `index`, ready for Model.set_input(*...):

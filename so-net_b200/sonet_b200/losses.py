@@ -142,6 +142,36 @@ def compute_iou(score, seg, label, visualizer, opt, input_pc):
     return compute_iou_np_array(score, seg, label, visualizer, opt, input_pc).mean()
 
 
+def compute_iou_full(score, seg, label, offsets, table=None):
+    """Per-shape IoU over ALL points of each shape, float64 numpy [B]: compute_iou_np_array's rule
+    (argmax over all classes, then per part of the shape's category I / (U + 0.0001), 1.0 for an
+    empty union, averaged over the parts) on ragged shapes. score [sum P_i, C] f32 (what
+    segmenter.Model.score_points returns), seg [sum P_i], label [B], offsets [B+1] int64. CUDA
+    scores run one kernel, host scores the library's C++ entry; both give the same bits. Its mean
+    is compute_iou's number at full resolution. Bad offsets or a label outside the table raise."""
+    if score.dtype != torch.float32 or score.dim() != 2:
+        raise RuntimeError("compute_iou_full: score must be float32 [T, C] (got %s %s)"
+                           % (score.dtype, tuple(score.shape)))
+    score = score.detach().contiguous()
+    seg = seg.detach().to(score.device, torch.int64).contiguous()
+    label = label.detach().to(score.device, torch.int64).contiguous()
+    ops.ragged_offsets(offsets, score.shape[0], label.shape[0])
+    offsets = offsets.detach().to(score.device).contiguous()
+    if score.is_cuda:
+        return _host_iou(ops.seg_iou_ragged(score, seg, label, offsets, table)[0])
+    if tuple(seg.shape) != (score.shape[0],):
+        raise RuntimeError("compute_iou_full: seg must be [T] (got %s)" % (tuple(seg.shape),))
+    T, C = score.shape
+    B = label.shape[0]
+    poff, ids, K = ops.part_table_csr(table, C, score.device)
+    iou = torch.empty((B,), dtype=torch.float64)
+    _C.check(_C.lib().sonet_seg_iou_ragged_cpu_f32(
+        score.data_ptr(), seg.data_ptr(), label.data_ptr(), offsets.data_ptr(), B, C, T,
+        poff.data_ptr(), ids.data_ptr(), K, iou.data_ptr(), None, None, torch.get_num_threads()),
+        "sonet_seg_iou_ragged_cpu_f32")
+    return iou.numpy()
+
+
 def visualize_pc_seg(score, seg, label, visualizer, opt, input_pc, batch_num):
     """Show one cloud coloured by predicted and by ground-truth part (models/losses.py:46-70):
     score [C,N], seg [N], input_pc [3,N]; colours from <opt.dataroot>/part_color_mapping.json

@@ -301,7 +301,9 @@ class Segmenter(nn.Module):
         else:
             parts = torch.split(layer3_out, N, dim=2)
             assert len(parts) == k
-            if k == 2:
+            if k == 1:     # one copy per point: its own layer-3 output
+                avg = parts[0]
+            elif k == 2:
                 avg = 0.5 * (parts[0] + parts[1])
             elif k == 3:
                 avg = (1.0 / 3.0) * (parts[0] + parts[1] + parts[2])
@@ -384,22 +386,29 @@ class Segmenter(nn.Module):
                                 g(node_knn), g(node_final), feature)
         B, N = x.size()[0], x.size()[2]
         k = self.opt.k
-        M = node_first.shape[2]
         use_sn = self.opt.surface_normal == True  # noqa: E712
         small = [x_decentered, torch.cat((x,) * k, dim=2), centers]
         if use_sn:
             small.append(torch.cat((sn,) * k, dim=2))
         pt = torch.cat(small, dim=1).contiguous()                       # [B,12,kN]
-        w_point, w_node, w_cloud, tc, shift = self._pack_layer1(
-            pt.shape[1], 16, first_pn_out.shape[1],
-            node_first.shape[1] + node_knn.shape[1] + node_final.shape[1])
-        cloud = torch.cat((self._onehot(label, B, x.device), feature), dim=1)   # [B,1040]
+        addend, packed = self._node_addend(pt.shape[1], first_pn_out.shape[1], node_first,
+                                           node_knn, node_final, feature, label)
+        out1 = self._layer1_points(pt, first_pn_out, addend, min_idx_i32, packed)
+        if self.layer1.normalization == 'instance':
+            out1 = self.layer1.instance_norm(out1)
+        return self._tail(self.layer2(out1), k, N)
+
+    def _node_addend(self, n_pt, n_pp, node_first, node_knn, node_final, feature, label):
+        """(addend, packed): layer 1's node- and cloud-level part [B,1024,M] (the node GEMM over
+        cat(node_first, node_knn, node_final) plus the broadcast [B,1040] cloud GEMM) and the
+        packed split weights for _layer1_points."""
+        B, M = node_first.shape[0], node_first.shape[2]
+        packed = self._pack_layer1(
+            n_pt, 16, n_pp, node_first.shape[1] + node_knn.shape[1] + node_final.shape[1])
+        w_point, w_node, w_cloud, tc, shift = packed
+        cloud = torch.cat((self._onehot(label, B, feature.device), feature), dim=1)   # [B,1040]
         cloud_add = ops.linear(cloud.contiguous(), w_cloud, None, None, False).unsqueeze(2)  # [B,1024,1]
-        # the split is linear up to the pre-norm z: an instance-norm layer 1 normalises it after
-        inst1 = self.layer1.normalization == 'instance'
-        act1 = None if inst1 else self.layer1.activation
         if tc_enabled():
-            f16 = tc_f16()
             bp, ip, bn, pern, inn = tc
             cout = w_point.shape[1]
             # [B,1920,M] -> [B,1024,M]: 16 row tiles x 4 column tiles would leave the GPU to 64
@@ -408,21 +417,36 @@ class Segmenter(nn.Module):
             kch = (node_in.shape[1] + 63) // 64
             splits = ops.pick_splits(kch, ((B * M + 127) // 128) * ((cout + 255) // 256))
             addend = ops.pointwise_tc_grouped(node_in, bn, pern, inn, None, cout, False, groups=1,
-                                              splits=splits, f16=f16) + cloud_add   # [B,1024,M]
-            out1 = ops.pointwise_layer_tc(pt, bp, ip, shift, cout, act1,
-                                          x1=first_pn_out.contiguous(), addend=addend,
-                                          gidx=min_idx_i32, f16=f16)
-        else:
-            node_a = torch.cat((node_first, node_knn), dim=1).contiguous()
-            addend = ops.pointwise_layer(node_a, w_node, None, None, False,
-                                         x1=node_final.contiguous(), addend=cloud_add,
-                                         gidx=self._zero_idx(B, M, x.device))
-            out1 = ops.pointwise_layer(pt, w_point, None, shift, act1,
-                                       x1=first_pn_out.contiguous(), addend=addend,
-                                       gidx=min_idx_i32)
-        if inst1:
-            out1 = self.layer1.instance_norm(out1)
-        return self._tail(self.layer2(out1), k, N)
+                                              splits=splits, f16=tc_f16()) + cloud_add
+            return addend, packed
+        node_a = torch.cat((node_first, node_knn), dim=1).contiguous()
+        addend = ops.pointwise_layer(node_a, w_node, None, None, False, x1=node_final.contiguous(),
+                                     addend=cloud_add, gidx=self._zero_idx(B, M, feature.device))
+        return addend, packed
+
+    def _layer1_points(self, pt, first_pn_out, addend, gidx, packed):
+        """Layer 1 over per-point rows pt [B',12,P] | first_pn_out [B',384,P], the node-level
+        addend gathered per column by gidx [B',P] (the split GEMM of forward_nodes); pre-norm z for
+        an instance-norm layer 1."""
+        w_point, _, _, tc, shift = packed
+        # the split is linear up to the pre-norm z: an instance-norm layer 1 normalises it after
+        act1 = None if self.layer1.normalization == 'instance' else self.layer1.activation
+        if tc_enabled():
+            bp, ip = tc[0], tc[1]
+            return ops.pointwise_layer_tc(pt, bp, ip, shift, w_point.shape[1], act1,
+                                          x1=first_pn_out.contiguous(), addend=addend, gidx=gidx,
+                                          f16=tc_f16())
+        return ops.pointwise_layer(pt, w_point, None, shift, act1, x1=first_pn_out.contiguous(),
+                                   addend=addend, gidx=gidx)
+
+    def forward_rows(self, pt, first_pn_out, addend_flat, gidx, k, packed):
+        """The per-point head over one chunk of ragged rows laid out as ONE batch row, copy-major
+        (csrc/seg_points.cu): pt [1,12,k*R], first_pn_out [1,384,k*R], gidx [1,k*R] flat
+        cloud*M+node ids into addend_flat [1,1024,B*M] (_node_addend's [B,1024,M] with the clouds
+        side by side; packed: its second value) -> scores [1,classes,R]. Every layer is a
+        per-column GEMM, so a row's scores do not depend on the other rows of the chunk."""
+        out1 = self._layer1_points(pt, first_pn_out, addend_flat, gidx, packed)
+        return self._tail(self.layer2(out1), k, pt.shape[2] // k)
 
 
 class DecoderLinear(nn.Module):

@@ -526,6 +526,77 @@ def seg_iou(score, seg, label, table=None, want_pred=False, want_correct=False):
     return iou, pred, correct
 
 
+def ragged_offsets(offsets, total, B=None):
+    """Host copy (numpy int64) of ragged offsets [B+1], checked: 0 first, `total` last, non-decreasing;
+    B, when given, is the expected number of shapes."""
+    if offsets.dtype != torch.int64 or offsets.dim() != 1 or offsets.numel() < 1:
+        raise RuntimeError("offsets must be a 1-D int64 tensor [B+1] (got %s %s)"
+                           % (offsets.dtype, tuple(offsets.shape)))
+    if B is not None and offsets.numel() != B + 1:
+        raise RuntimeError("offsets has %d entries, the batch needs B+1 = %d"
+                           % (offsets.numel(), B + 1))
+    off = offsets.detach().cpu().numpy()
+    if off[0] != 0 or off[-1] != total or (off[1:] < off[:-1]).any():
+        raise RuntimeError("offsets must run from 0 to %d without decreasing" % total)
+    return off
+
+
+def seg_iou_ragged(score, seg, label, offsets, table=None, want_pred=False, want_correct=False):
+    """seg_iou over every point of each shape, one launch: score [T,C] f32, seg [T] int64, label [B]
+    int64, offsets [B+1] int64 (CUDA, contiguous; shape b owns points offsets[b] .. offsets[b+1]).
+    Returns (iou_shape [B] f64, pred [T] int64 or None, correct [B] int32 or None). The offsets are
+    checked by the caller (ragged_offsets); the device marks a shape with bad offsets NaN."""
+    _chk(score, "score", torch.float32)
+    _chk(seg, "seg", torch.int64)
+    _chk(label, "label", torch.int64)
+    _chk(offsets, "offsets", torch.int64)
+    if score.dim() != 2 or tuple(seg.shape) != (score.shape[0],) or label.dim() != 1 \
+            or tuple(offsets.shape) != (label.shape[0] + 1,):
+        raise RuntimeError("seg_iou_ragged: expected score [T,C], seg [T], label [B], offsets [B+1], "
+                           "got %s, %s, %s, %s" % (tuple(score.shape), tuple(seg.shape),
+                                                   tuple(label.shape), tuple(offsets.shape)))
+    T, C = score.shape
+    B = label.shape[0]
+    dev = score.device
+    with torch.cuda.device(dev):
+        poff, ids, K = part_table_csr(table, C, dev)
+        iou = torch.empty((B,), dtype=torch.float64, device=dev)
+        pred = torch.empty((T,), dtype=torch.int64, device=dev) if want_pred else None
+        correct = torch.empty((B,), dtype=torch.int32, device=dev) if want_correct else None
+        _call("sonet_seg_iou_ragged_f32", _C.ptr(score), _C.ptr(seg), _C.ptr(label), _C.ptr(offsets),
+              B, C, T, _C.ptr(poff), _C.ptr(ids), K, _C.ptr(iou), _C.ptr(pred), _C.ptr(correct),
+              _stream(score))
+    return iou, pred, correct
+
+
+def seg_points_assign(points, offsets, node, cluster_mean, k, with_sn, row0, rows, rows_pad):
+    """Rows [row0, row0+rows) of the ragged set points [T,6] (offsets [B+1] int64, checked by the
+    caller) -> (gidx [1,k*rows_pad] int32 flat cloud*M+node ids, x_aug [1,3(+3),k*rows_pad],
+    pt [1,9(+3),k*rows_pad]), copy-major, padded with zero rows (csrc/seg_points.cu)."""
+    _chk(points, "points", torch.float32)
+    _chk(offsets, "offsets", torch.int64)
+    _chk(node, "node", torch.float32)
+    _chk(cluster_mean, "cluster_mean", torch.float32)
+    if points.dim() != 2 or points.shape[1] != 6 or node.dim() != 3 or node.shape[1] != 3 \
+            or tuple(cluster_mean.shape) != tuple(node.shape) \
+            or tuple(offsets.shape) != (node.shape[0] + 1,):
+        raise RuntimeError("seg_points_assign: expected points [T,6], offsets [B+1], node and "
+                           "cluster_mean [B,3,M], got %s, %s, %s, %s"
+                           % (tuple(points.shape), tuple(offsets.shape), tuple(node.shape),
+                              tuple(cluster_mean.shape)))
+    B, _, M = node.shape
+    cols = k * rows_pad
+    dev = points.device
+    with torch.cuda.device(dev):
+        gidx = torch.empty((1, cols), dtype=torch.int32, device=dev)
+        x_aug = torch.empty((1, 6 if with_sn else 3, cols), dtype=torch.float32, device=dev)
+        pt = torch.empty((1, 12 if with_sn else 9, cols), dtype=torch.float32, device=dev)
+        _call("sonet_seg_points_assign_f32", _C.ptr(points), points.shape[0], _C.ptr(offsets), B,
+              _C.ptr(node), _C.ptr(cluster_mean), M, int(k), int(bool(with_sn)), int(row0), int(rows),
+              int(rows_pad), _C.ptr(gidx), _C.ptr(x_aug), _C.ptr(pt), _stream(points))
+    return gidx, x_aug, pt
+
+
 RETRIEVAL_MAX_D = 1024
 RETRIEVAL_MAX_K = 4096
 RETRIEVAL_MAX_L = 4096
