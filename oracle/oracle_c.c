@@ -40,9 +40,9 @@ void oracle_index_max(const float* data, const int32_t* index, int B, int C, int
 /* util/som.py:245-253 (BatchSOM.query_topk): diff = x - node; diff_norm = (diff**2).sum(dim=1);
  * topk(k, largest=False). The sum over the 3 channels is ((d0*d0 + d1*d1) + d2*d2) in fp32
  * (SURVEY.md §8c: bit-equal to the reference expression). Slot order here: ascending distance,
- * lowest node index on exact ties (the reference's sorted=False order is implementation
- * defined -> parity is per-point set equality). Output slot-major like util/som.py:261-266:
- * min_idx[b, s*N + n]. Compile with -ffp-contract=off. */
+ * lowest node index on exact ties, +inf then NaN distances last (the reference's sorted=False
+ * order is implementation defined -> parity is per-point set equality). Output slot-major like
+ * util/som.py:261-266: min_idx[b, s*N + n]. Compile with -ffp-contract=off. */
 void oracle_som_topk(const float* x, const float* node, int B, int N, int M, int k,
                      int32_t* min_idx, float* min_dist /* nullable, same layout */) {
   for (int b = 0; b < B; ++b) {
@@ -51,9 +51,10 @@ void oracle_som_topk(const float* x, const float* node, int B, int N, int M, int
     for (int n = 0; n < N; ++n) {
       float bd[8];
       int bi[8];
+      int filled = 0;
       for (int s = 0; s < k; ++s) {
         bd[s] = INFINITY;
-        bi[s] = s;
+        bi[s] = -1;
       }
       for (int m = 0; m < M; ++m) {
         const float d0 = xb[n] - nb[m], d1 = xb[N + n] - nb[M + m], d2 = xb[2 * N + n] - nb[2 * M + m];
@@ -67,8 +68,20 @@ void oracle_som_topk(const float* x, const float* node, int B, int N, int M, int
           }
           bd[s] = d;
           bi[s] = m;
+          if (filled < k) ++filled;
         }
       }
+      /* fewer than k finite distances: then the +inf nodes, then the NaN ones, by index (the
+       * order of torch.topk / a stable sort with NaN last; a NaN point gets nodes 0..k-1) */
+      for (int pass = 0; pass < 2; ++pass)
+        for (int m = 0; m < M && filled < k; ++m) {
+          const float d0 = xb[n] - nb[m], d1 = xb[N + n] - nb[M + m], d2 = xb[2 * N + n] - nb[2 * M + m];
+          const float d = (d0 * d0 + d1 * d1) + d2 * d2;
+          if (pass == 0 ? isinf(d) && d > 0 : isnan(d)) {
+            bd[filled] = d;
+            bi[filled++] = m;
+          }
+        }
       for (int s = 0; s < k; ++s) {
         min_idx[(size_t)b * k * N + (size_t)s * N + n] = bi[s];
         if (min_dist) min_dist[(size_t)b * k * N + (size_t)s * N + n] = bd[s];

@@ -88,6 +88,36 @@ __device__ __forceinline__ float2 sqsum3_rn(float2 dx, float2 dy, float2 dz) {
   return make_float2(__fadd_rn(__fadd_rn(xx.x, yy.x), zz.x), __fadd_rn(__fadd_rn(xx.y, yy.y), zz.y));
 }
 
+// ---- register top-k of the SOM assignment ---------------------------------------------------------
+// The arg-min kernels (som.cu, seg_points.cu) insert every distance below the last slot's, starting
+// from slots (+inf, -1): a finite distance always enters, +inf and NaN never do. A point with fewer
+// than KK nodes at a finite distance (a coordinate whose square overflows for some nodes, or a point
+// that is not finite) leaves slots at -1. This fills them with the nodes at +inf, then the NaN
+// ones, each in ascending index order, so that the KK nodes stay distinct and keep the order
+// (distance, index) with NaN last: a NaN point gets nodes 0..KK-1. dist(m) must give the insertion
+// loop's value for node m. Run only when bi[KK-1] < 0, which a finite point with KK finite
+// distances never reaches.
+template <int KK, typename Dist>
+__device__ __forceinline__ void topk_fill_nonfinite(float (&bd)[KK], int (&bi)[KK], int M, Dist dist) {
+  int filled = 0;
+#pragma unroll
+  for (int s = 0; s < KK; ++s) filled += bi[s] >= 0;
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int m = 0; m < M && filled < KK; ++m) {
+      const float d = dist(m);
+      if (pass == 0 ? d == __int_as_float(0x7f800000) : d != d) {
+#pragma unroll
+        for (int s = 0; s < KK; ++s)   // register slots: no dynamic index
+          if (s == filled) {
+            bd[s] = d;
+            bi[s] = m;
+          }
+        ++filled;
+      }
+    }
+  }
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

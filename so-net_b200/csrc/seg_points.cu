@@ -11,9 +11,10 @@
 //
 // m_s is the s-th nearest of cloud b's M loader nodes with sonet_som_assign's arithmetic: distances
 // ((dx*dx + dy*dy) + dz*dz) rounded op by op with dx = x - node (add2_rn / mul2_rn in som.cu: the same
-// bits), register top-k insertion, the lowest node index on ties. cm is the cluster mean the encoder
+// bits), register top-k insertion, the lowest node index on ties, k distinct nodes even when fewer
+// than k distances are finite (common.cuh, topk_fill_nonfinite). cm is the cluster mean the encoder
 // computed on the sampled batch (Encoder.som_node). Columns of rows r >= rows are padding: zeros and
-// node 0 of cloud 0, so that a chunk keeps every layer on the same kernel route as any other.
+// node 0 of cloud 0, so that whatever reads them stays finite and in range.
 //
 // Each row finds its cloud by a binary search over offsets on the device: one launch per chunk, no
 // host round trip per cloud. offsets are not read on the host; a row outside [offsets[0], offsets[B])
@@ -67,13 +68,16 @@ __global__ void __launch_bounds__(SEGPT_THREADS)
 #pragma unroll
   for (int s = 0; s < KK; ++s) {
     bd[s] = __int_as_float(0x7f800000);  // +inf
-    bi[s] = s;
+    bi[s] = -1;                          // empty (topk_fill_nonfinite)
   }
-  for (int m = 0; m < M; ++m) {
-    // p + (-n) == p - n bit for bit: the arithmetic of som_assign_kernel's negated packed nodes
+  // p + (-n) == p - n bit for bit: the arithmetic of som_assign_kernel's negated packed nodes
+  auto dist = [&](int m) {
     const float dx = __fadd_rn(px, -__ldg(nb + m)), dy = __fadd_rn(py, -__ldg(nb + M + m)),
                 dz = __fadd_rn(pz, -__ldg(nb + 2 * M + m));
-    const float d = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+  };
+  for (int m = 0; m < M; ++m) {
+    const float d = dist(m);
     if (d < bd[KK - 1]) {  // strict: on exact ties the earlier (lower) node index stays
       bd[KK - 1] = d;
       bi[KK - 1] = m;
@@ -90,6 +94,7 @@ __global__ void __launch_bounds__(SEGPT_THREADS)
       }
     }
   }
+  if (bi[KK - 1] < 0) topk_fill_nonfinite(bd, bi, M, dist);
 
   const float* cm = cluster_mean + static_cast<size_t>(b) * 3 * M;
   const float xv[3] = {px, py, pz};

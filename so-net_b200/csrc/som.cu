@@ -8,7 +8,8 @@
 //
 //  som_assign_kernel   thread per point: 64 nodes in smem (broadcast reads), distances in the
 //                      reference's exact rounding order ((dx*dx+dy*dy)+dz*dz, no FMA), register
-//                      top-k insertion (ascending distance, lowest node index on ties).
+//                      top-k insertion (ascending distance, lowest node index on ties; k distinct
+//                      nodes even when fewer than k distances are finite: topk_fill_nonfinite).
 //  som_stats_kernel    CTA per (cloud, node): counts and coordinate sums in a fixed order
 //                      (strided per-thread partials + fixed tree) -> bit-reproducible and
 //                      independent of batch sharding; cluster_mean = sum / (count + 1e-5f).
@@ -56,7 +57,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
   for (int s = 0; s < KK; ++s) {
     bd[s] = __int_as_float(0x7f800000);  // +inf
-    bi[s] = s;
+    bi[s] = -1;                          // empty (topk_fill_nonfinite)
   }
   auto consider = [&](float d, int m) {
     if (d < bd[KK - 1]) {  // strict: on exact ties the earlier (lower) node index stays
@@ -80,6 +81,14 @@ __global__ void __launch_bounds__(256)
     const float2 d = sqsum3_rn(add2_rn(px2, snx[m2]), add2_rn(py2, sny[m2]), add2_rn(pz2, snz[m2]));
     consider(d.x, 2 * m2);
     if (2 * m2 + 1 < M) consider(d.y, 2 * m2 + 1);
+  }
+  if (bi[KK - 1] < 0) {
+    topk_fill_nonfinite(bd, bi, M, [&](int m) {
+      const float2 nx = snx[m >> 1], ny = sny[m >> 1], nz = snz[m >> 1];
+      const float dx = __fadd_rn(px, (m & 1) ? nx.y : nx.x), dy = __fadd_rn(py, (m & 1) ? ny.y : ny.x),
+                  dz = __fadd_rn(pz, (m & 1) ? nz.y : nz.x);
+      return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+    });
   }
   if (mask != nullptr) {
     // Fused dense one-hot mask (util/som.py:255-265), M % 32 == 0: the warp writes the KK rows of

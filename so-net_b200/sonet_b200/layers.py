@@ -331,19 +331,22 @@ class _PointwiseConvBase(nn.Module):
                                  group_max=group_max,
                                  out=z if kcopy is None and group_max is None else None)
 
-    def forward_points(self, x0, x1=None, addend=None, gidx=None, kcopy=None, group_max=None):
+    def forward_points(self, x0, x1=None, addend=None, gidx=None, kcopy=None, group_max=None,
+                       route_rows=None):
         """x0 [B,C0,P] (+ x1 [B,C1,P] virtually concatenated on channels) -> [B,Cout,P].
         Dense layers run on wgmma (csrc/pointwise_tc.cu, fp16 hi/lo split); thin ones on the
         exact-fp32 CUDA-core kernel (csrc/pointwise.cu). An instance-norm layer writes the GEMM's
         z (conv bias, no activation) and normalises it with ops.instance_norm, which can also
-        reduce the result (kcopy / group_max: instance layers only)."""
+        reduce the result (kcopy / group_max: instance layers only). route_rows: the row count
+        that picks the kernel instead of B*P, for a launch that must take the route of another
+        (segmenter.Model.score_points runs each layer on the route of the sampled forward)."""
         inst = self.normalization == 'instance'
         if not inst and (kcopy is not None or group_max is not None):
             raise RuntimeError("forward_points: kcopy / group_max are fused into instance norm only")
         act = None if inst else self.activation
         cin = x0.shape[1] + (0 if x1 is None else x1.shape[1])
         cout = self.conv.out_channels
-        rows = x0.shape[0] * x0.shape[2]
+        rows = x0.shape[0] * x0.shape[2] if route_rows is None else route_rows
         # wgmma eligibility: a dense enough contraction (cin >= 32) over at least two 128-row
         # tiles; thin OUTPUTS (the 128 -> 3 ConvToPC heads) qualify too — the layer is then a
         # streaming read of the activations into the tensor-core kernel instead of the
@@ -597,9 +600,10 @@ class EquivariantLayer(_PointwiseConvBase):
     def fast(self, *tensors):
         return _fast_ok(self, *tensors) and self._fast_eligible()
 
-    def forward(self, x, epoch=None):
+    def forward(self, x, epoch=None, route_rows=None):
+        """route_rows: as forward_points (eval fast path only)."""
         if self.fast(x) and x.dim() == 3:
-            return self.forward_points(x.contiguous())
+            return self.forward_points(x.contiguous(), route_rows=route_rows)
         if self._train_kernels(x) and x.dim() == 3:
             return train_ops.conv_bn_act_train(
                 x, self._conv_weight2d(), self.conv.bias, self._train_norm(), self.activation,
@@ -842,8 +846,9 @@ class PointResNet(nn.Module):
             return blob.to(ws[0].device), fpar.to(ws[0].device)
         return self._tc.get(tuple(l._folded.version for l in self.layers), build)
 
-    def forward(self, x, epoch=None, x1=None):
-        """x [B,C,P]; x1: optional second tensor virtually concatenated to x (eval fast path)."""
+    def forward(self, x, epoch=None, x1=None, route_rows=None):
+        """x [B,C,P]; x1: optional second tensor virtually concatenated to x (eval fast path);
+        route_rows: as EquivariantLayer.forward_points (the fused kernel has one route)."""
         n = len(self.out_channels_list)
         first, last = self.layers[0], self.layers[n - 1]
         if first.fast(x) and x.dim() == 3 and all(l.fast(x) for l in self.layers) \
@@ -853,11 +858,13 @@ class PointResNet(nn.Module):
                                       act=self.layers[0].activation)
         if first.fast(x) and x.dim() == 3 and all(l.fast(x) for l in self.layers):
             layer0_out = first.forward_points(x.contiguous(),
-                                              None if x1 is None else x1.contiguous())
+                                              None if x1 is None else x1.contiguous(),
+                                              route_rows=route_rows)
             x_tmp = layer0_out
             for l in range(1, n - 1):
-                x_tmp = self.layers[l].forward_points(x_tmp)
-            return last.forward_points(layer0_out, x_tmp)   # the skip-concat, never materialised
+                x_tmp = self.layers[l].forward_points(x_tmp, route_rows=route_rows)
+            # the skip-concat, never materialised
+            return last.forward_points(layer0_out, x_tmp, route_rows=route_rows)
         if x1 is not None:
             x = torch.cat((x, x1), dim=1)
         layer0_out = first(x, epoch)

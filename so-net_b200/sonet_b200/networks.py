@@ -288,13 +288,15 @@ class Segmenter(nn.Module):
         onehot.scatter_(1, label.unsqueeze(1), 1)
         return onehot
 
-    def _tail(self, layer2_out, k, N):
+    def _tail(self, layer2_out, k, N, route_rows=None):
         """layer3 + k-copy average + layer4/5 (models/networks.py:326-341). An instance-norm
-        layer 3 takes the k-copy mean inside its normalisation pass."""
+        layer 3 takes the k-copy mean inside its normalisation pass. route_rows: the point count
+        B*N whose routes layers 3-5 take (forward_rows), None for this launch's own."""
         if (self.layer3.normalization == 'instance' and k in (2, 3) and layer2_out.dim() == 3
                 and self.layer3.fast(layer2_out) and self.layer4.fast(layer2_out)):
             return self._tail_avg(self.layer3.forward_points(layer2_out.contiguous(), kcopy=k))
-        layer3_out = self.layer3(layer2_out)
+        layer3_out = self.layer3(layer2_out,
+                                 route_rows=None if route_rows is None else k * route_rows)
         fast = self.layer4.fast(layer3_out)
         if fast and k in (2, 3):
             avg = ops.kcopy_mean(layer3_out.contiguous(), k)
@@ -307,13 +309,13 @@ class Segmenter(nn.Module):
                 avg = 0.5 * (parts[0] + parts[1])
             elif k == 3:
                 avg = (1.0 / 3.0) * (parts[0] + parts[1] + parts[2])
-        return self._tail_avg(avg)
+        return self._tail_avg(avg, route_rows)
 
-    def _tail_avg(self, avg):
-        out4 = self.layer4(avg)
+    def _tail_avg(self, avg, route_rows=None):
+        out4 = self.layer4(avg, route_rows=route_rows)
         if self.opt.dropout > 0.1:
             out4 = self.drop4(out4)
-        return self.layer5(out4)
+        return self.layer5(out4, route_rows=route_rows)
 
     def forward(self, x_decentered, x, centers, sn, label, first_pn_out, feature_max_first_pn_out,
                 feature_max_knn_feature_1, feature_max_final_pn_out, feature):
@@ -439,14 +441,18 @@ class Segmenter(nn.Module):
         return ops.pointwise_layer(pt, w_point, None, shift, act1, x1=first_pn_out.contiguous(),
                                    addend=addend, gidx=gidx)
 
-    def forward_rows(self, pt, first_pn_out, addend_flat, gidx, k, packed):
+    def forward_rows(self, pt, first_pn_out, addend_flat, gidx, k, packed, route_rows):
         """The per-point head over one chunk of ragged rows laid out as ONE batch row, copy-major
         (csrc/seg_points.cu): pt [1,12,k*R], first_pn_out [1,384,k*R], gidx [1,k*R] flat
         cloud*M+node ids into addend_flat [1,1024,B*M] (_node_addend's [B,1024,M] with the clouds
         side by side; packed: its second value) -> scores [1,classes,R]. Every layer is a
-        per-column GEMM, so a row's scores do not depend on the other rows of the chunk."""
+        per-column GEMM, so a row's scores do not depend on the other rows of the chunk.
+        route_rows: the B*N points of the sampled forward. Each layer takes the kernel that
+        forward_nodes took for them (layers 2-3 over k*B*N columns, 4-5 over B*N), whatever the
+        chunk's size, so that a point's scores keep the sampled forward's bits."""
         out1 = self._layer1_points(pt, first_pn_out, addend_flat, gidx, packed)
-        return self._tail(self.layer2(out1), k, pt.shape[2] // k)
+        out2 = self.layer2(out1, route_rows=k * route_rows)
+        return self._tail(out2, k, pt.shape[2] // k, route_rows=route_rows)
 
 
 class DecoderLinear(nn.Module):

@@ -104,8 +104,8 @@ class Model(GraphedModel):
     # ---- every point of each shape -----------------------------------------------------------
     # device bytes per stacked copy of a row in one chunk: pt, x_aug, first_pn_out and layers 1-3
     _COPY_BYTES = 4 * (12 + 6 + 384 + 1024 + 512 + 256) + 4
-    # padding unit of a chunk: k * rows stays >= 256, so every layer keeps the kernel route of the
-    # sampled forward (EquivariantLayer.forward_points) whatever the chunk holds
+    # padding unit of a chunk's rows (whole wgmma row tiles). It decides no kernel route: every
+    # layer takes the route of the sampled forward (Segmenter.forward_rows)
     _ROW_QUANTUM = 256
 
     def _default_chunk_rows(self, total):
@@ -129,6 +129,8 @@ class Model(GraphedModel):
         cluster means (encoder.som_node), and run through the first PointResNet, the split layer 1
         with the node/cloud addend, layers 2-5 and the k-copy mean. Rows go in chunks of
         chunk_rows (default: a quarter of the free device memory); the chunking changes no bit.
+        Each layer runs on the kernel the sampled forward ran it on for its B*N points, so the
+        sampled points themselves get score_segmenter's bits at every batch size.
 
         Refused (RuntimeError, before any launch): train mode; instance normalisation (layer 1's
         per-row statistics would depend on the point set); som_k < 2; a batch test_model() has not
@@ -155,6 +157,7 @@ class Model(GraphedModel):
         if chunk_rows is not None and chunk_rows < 1:
             raise RuntimeError("score_points: chunk_rows must be >= 1 (got %d)" % chunk_rows)
         k = opt.k
+        BN = B * self.input_pc.shape[2]      # the sampled forward's points: the layers' routes
         use_sn = opt.surface_normal == True  # noqa: E712
         with torch.no_grad():
             points = points.contiguous()
@@ -172,7 +175,7 @@ class Model(GraphedModel):
                 R = min(chunk, T - r0)
                 gidx, x_aug, pt = ops.seg_points_assign(points, offsets, node, enc.som_node, k,
                                                         use_sn, r0, R, (R + q - 1) // q * q)
-                fpo = enc.first_pointnet(x_aug)
-                y = seg.forward_rows(pt, fpo, addend_flat, gidx, k, packed)   # [1, classes, Rp]
+                fpo = enc.first_pointnet(x_aug, route_rows=k * BN)
+                y = seg.forward_rows(pt, fpo, addend_flat, gidx, k, packed, BN)   # [1,classes,Rp]
                 score[r0:r0 + R].copy_(y[0, :, :R].t())
         return score

@@ -406,8 +406,8 @@ def test_som_assign_k4_ties(oracle_mod, M):
 
 
 def test_som_assign_nan_point_stays_in_range():
-    """A NaN point compares false against every distance, so its k slots keep their
-    initialisation bi[s] = s: indices 0..k-1, in range for everything downstream."""
+    """A NaN point compares false against every distance, so every node is a NaN one and its k
+    slots take nodes 0..k-1 in index order: in range for everything downstream."""
     from sonet_b200 import ops
     M, k, N = 121, 4, 200
     rs = np.random.RandomState(5)
