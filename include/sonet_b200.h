@@ -161,14 +161,6 @@ int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, int P, cons
  * EquivariantLayer in train() mode = Conv1d(k=1) -> MyBatchNorm1d with BATCH statistics
  * (models/layers.py:22-70, 282-296) -> ReLU, and its backward; the backward of the per-node pool
  * (the gather of models/networks.py:185).
- *   sonet_bn_train_forward_f32: x [B,C,P] -> per-channel batch mean / biased variance / invstd
- *     (two-stage, fp64 partial sums in a fixed order: bit-reproducible) and
- *     y = act(gamma*(x-mean)*invstd + beta) in one elementwise pass. partial: scratch of
- *     sonet_bn_partial_slots(B,C) doubles. (The running-statistics update with the reference's
- *     momentum schedule stays on the host side: two [C] vector ops.)
- *   sonet_bn_train_backward_f32: dy, x (the BN input) -> dx, dgamma, dbeta; the activation's
- *     derivative is recomputed from x at z = gamma*xhat+beta (ReLU: [z > 0]; ELU: z > 0 ? 1 : exp(z)),
- *     so the forward output need not be kept. relu: activation code (SONET_ACT_*) in both.
  *   sonet_index_max_backward_f32: grad_data [B,C,N] = 0; grad_data[b,c,idx[b,c,k]] += grad_out[b,c,k]
  *     (k ascending, one thread per (b,c): deterministic also when empty nodes all gather point 0).
  *   sonet_pointwise_tc_pack_device: fp32 W [Cout,Cin] on the DEVICE -> wgmma blob (optionally of
@@ -185,25 +177,19 @@ int sonet_pointwise_tc_grouped_forward(const float* x, int C, int B, int P, cons
  *     sonet_wgrad_blob_bytes(Cin,Kpad) bytes, part splits*Cin*Cout floats, small
  *     sonet_wgrad_small_floats(Cout) floats. Needs Cout % 64 == 0.
  *   sonet_absmax_scale_f32: scale2 = (s, 1/s), s the power of two with max|s*t| in [256,512). */
-int sonet_bn_partial_slots(int B, int C);
-int sonet_bn_train_forward_f32(const float* x, const float* gamma, const float* beta, int B, int C,
-                               int P, float eps, int relu, double* partial, float* y,
-                               float* save_mean, float* save_var, float* save_invstd,
-                               sonet_stream_t stream);
-int sonet_bn_train_backward_f32(const float* dy, const float* x, const float* mean,
-                                const float* invstd, const float* gamma, const float* beta, int B,
-                                int C, int P, int relu, double* partial, float* dx, float* dgamma,
-                                float* dbeta, sonet_stream_t stream);
-/* Synchronised BatchNorm for data-parallel training: the batch statistics of a global batch of Bg
- * clouds sharded over ranks, bit-identical at every sharding. The existing entries above sum strided
- * groups of clouds whose stride depends on B and the SM count; these route every sum through
- * per-cloud records instead, which depend on nothing but the cloud's own values.
+/* Train-mode BatchNorm: the batch statistics of Bg clouds, of which the caller holds B (Bg = B in
+ * one process; in data-parallel training the global batch, sharded over the ranks). Every sum goes
+ * through one record per (cloud, channel), which depends on nothing but that cloud's values, so
+ * the results are the same bits at every SM count, sharding and world size. (The running-statistics
+ * update with the reference's momentum schedule stays on the host side: two [C] vector ops.)
  *   sonet_bn_cloud_partials_f32: one fp64 record per (b, c) of x [B,C,P], in a fixed order inside the
  *     cloud (P == 1: a thread per record; P <= 1024: a warp; longer: a 256-thread CTA).
  *       backward == 0: rec [B,C,SONET_BN_REC_FWD] = {pivot = x[b,c,0], sum d, sum d*d}, d = x - pivot;
  *         dy, mean, invstd, gamma, beta unused (may be null).
- *       backward != 0: rec [B,C,SONET_BN_REC_BWD] = {sum g, sum g*xhat}, g and xhat as in
- *         sonet_bn_train_backward_f32 (dy, x, mean, invstd required; gamma, beta nullable).
+ *       backward != 0: rec [B,C,SONET_BN_REC_BWD] = {sum g, sum g*xhat}, xhat = (x-mean)*invstd,
+ *         g = dy times the activation's derivative, recomputed from x at z = gamma*xhat+beta (ReLU:
+ *         [z > 0]; ELU: z > 0 ? 1 : exp(z)), so the forward output need not be kept (dy, x, mean,
+ *         invstd required; gamma, beta nullable).
  *   sonet_bn_sync_forward_f32: rec [Bg,C,3], the records of all Bg clouds in global order, folded in
  *     ascending cloud order onto cloud 0's pivot p (S1 = sum_b sum d_b + P (p_b - p),
  *     S2 = sum_b sum d_b^2 + 2 (p_b - p) sum d_b + P (p_b - p)^2) into the biased mean / var /
@@ -242,8 +228,9 @@ int sonet_index_max_backward_f32(const float* grad_out, const int32_t* idx, int 
  *                           0.5*(a+b), (1/3)*((a+b)+c)
  *   SONET_REDUCE_GROUP_MAX  out [B,C,P/k], the max over consecutive groups of k (the KNN module's
  *                           max over neighbours, models/layers.py:365)
- * save_mean, save_invstd (nullable together) [B,C]: the row statistics sonet_bn_train_backward_f32
- * takes on the [1, B*C, P] view, which is the instance-norm backward of every row.
+ * save_mean, save_invstd (nullable together) [B,C]: the row statistics the BatchNorm backward
+ * (sonet_bn_cloud_partials_f32 with backward = 1, then sonet_bn_sync_backward_f32, both with
+ * B = Bg = 1) takes on the [1, B*C, P] view, which is the instance-norm backward of every row.
  * One read of z and one write of out for rows of P <= 16384 (staged on chip); longer rows read z
  * again. Fails with SONET_ERR_BAD_ARG before any CUDA call for P < 2 (PyTorch: "Expected more than
  * 1 spatial element"), an unknown act or reduce code, or P not divisible by k. */

@@ -5,16 +5,18 @@
 // of a gather (models/networks.py:185). PyTorch runs that as conv + batch_norm + relu (+ three
 // backward kernels each) and a zero-fill + scatter for the gather. Here:
 //
-//   bn_stats / bn_apply          batch statistics of x[B,C,P] per channel, then
-//                                y = act(gamma * (x - mean) * invstd + beta) in ONE elementwise pass
-//   bn_backward (2 launches)     per-channel sums of g and g*xhat (g = dy times the activation's
-//                                derivative at the recomputed BN output z: [z > 0] for ReLU,
-//                                z > 0 ? 1 : exp(z) for ELU), then dx = gamma*invstd*(g - mean(g) -
-//                                xhat*mean(g*xhat)); dgamma, dbeta fall out of the sums
+//   bn forward (3 launches)      one fp64 record of sums per (cloud, channel) of x[B,C,P], the
+//                                records folded in ascending cloud order into the batch statistics,
+//                                then y = act(gamma * (x - mean) * invstd + beta) in ONE elementwise pass
+//   bn backward (3 launches)     per-(cloud, channel) records of the sums of g and g*xhat (g = dy
+//                                times the activation's derivative at the recomputed BN output z:
+//                                [z > 0] for ReLU, z > 0 ? 1 : exp(z) for ELU), folded like the
+//                                forward's, then dx = gamma*invstd*(g - mean(g) - xhat*mean(g*xhat));
+//                                dgamma, dbeta fall out of the sums
 //   instance_norm (1 launch)     per-row statistics of z[B,C,P] (InstanceNorm, eval and train
 //                                alike) and y = act(gamma*(z-mean)*invstd + beta), optionally reduced
 //                                to the k-copy mean or the max over groups of K; its backward is
-//                                bn_backward on the [1, B*C, P] view
+//                                the bn backward on the [1, B*C, P] view
 //   index_max_backward           grad of first_pn_out through the masked gather: zero-fill +
 //                                scatter-add of grad[b,c,k] at idx[b,c,k] (duplicates — every empty
 //                                node gathers point 0 — are added by ONE thread in ascending k)
@@ -32,113 +34,8 @@
 
 namespace sonet {
 
-constexpr int BN_THREADS = 256;
-
-// stage 1: CTA (c, s) sums the clouds b = s, s+S, ... of channel c. BWD: sums of g and g*xhat
-// (g = dy * [gamma*xhat + beta > 0] when relu, g = dy * act_grad(gamma*xhat + beta) in the ELU
-// build), else sums of d and d*d with d = x - x[0,c,0].
-//
-// The forward sums are shifted by a pivot, the channel's first element, and taken in fp64 term by
-// term. var = E[d^2] - E[d]^2 then cancels only by 1 + (mean - pivot)^2 / var, a few units for any
-// pivot drawn from the channel, where E[x^2] - mean^2 would cancel by (mean/std)^2: with fp32 sums
-// that is a relative error of ~(mean/std)^2 * 2^-24 in var, 1e-2 at mean/std = 1e3 (channels behind
-// a large bias, near-dead inputs). d is exact in fp64, d*d too, and a constant channel gives var = 0.
 // d elu(z) / dz, from the BN output z (alpha = 1: exp(z) = elu(z) + 1 below 0)
 __device__ __forceinline__ float elu_grad(float z) { return z > 0.f ? 1.f : expf(z); }
-
-template <bool BWD, bool ELU>
-__global__ void __launch_bounds__(BN_THREADS)
-    bn_partial_kernel(const float* __restrict__ x, const float* __restrict__ dy,
-                      const float* __restrict__ mean, const float* __restrict__ invstd,
-                      const float* __restrict__ gamma, const float* __restrict__ beta, int B, int C,
-                      int P, int relu, int S, double* __restrict__ partial) {
-  const int c = blockIdx.x, s = blockIdx.y;
-  double a0 = 0.0, a1 = 0.0;
-  float mu = 0.f, is = 1.f, ga = 1.f, be = 0.f;
-  double pivot = 0.0;
-  if (BWD) {
-    mu = mean[c];
-    is = invstd[c];
-    ga = gamma ? gamma[c] : 1.f;
-    be = beta ? beta[c] : 0.f;
-  } else {
-    pivot = x[static_cast<size_t>(c) * P];
-  }
-  for (int b = s; b < B; b += S) {
-    const float* xr = x + (static_cast<size_t>(b) * C + c) * P;
-    if (BWD) {
-      const float* gr = dy + (static_cast<size_t>(b) * C + c) * P;
-      float f0 = 0.f, f1 = 0.f;          // fp32 within one row chunk, fp64 across
-      int cnt = 0;
-      for (int p = threadIdx.x; p < P; p += BN_THREADS) {
-        const float xh = (xr[p] - mu) * is;
-        float g = gr[p];
-        if (ELU) g *= elu_grad(fmaf(ga, xh, be));
-        else if (relu && !(fmaf(ga, xh, be) > 0.f)) g = 0.f;
-        f0 += g;
-        f1 = fmaf(g, xh, f1);
-        if (++cnt == 64) {               // flush to fp64 every 64 terms
-          a0 += f0; a1 += f1; f0 = f1 = 0.f; cnt = 0;
-        }
-      }
-      a0 += f0;
-      a1 += f1;
-    } else {
-      for (int p = threadIdx.x; p < P; p += BN_THREADS) {
-        const double d = static_cast<double>(xr[p]) - pivot;
-        a0 += d;
-        a1 = fma(d, d, a1);
-      }
-    }
-  }
-  __shared__ double r0[BN_THREADS], r1[BN_THREADS];
-  r0[threadIdx.x] = a0;
-  r1[threadIdx.x] = a1;
-  __syncthreads();
-  for (int w = BN_THREADS / 2; w > 0; w >>= 1) {
-    if (threadIdx.x < w) {
-      r0[threadIdx.x] += r0[threadIdx.x + w];
-      r1[threadIdx.x] += r1[threadIdx.x + w];
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    partial[(static_cast<size_t>(c) * S + s) * 2] = r0[0];
-    partial[(static_cast<size_t>(c) * S + s) * 2 + 1] = r1[0];
-  }
-}
-
-__global__ void bn_stats_final_kernel(const double* __restrict__ partial, const float* __restrict__ x,
-                                      int C, int P, int S, double n, float eps,
-                                      float* __restrict__ mean, float* __restrict__ var,
-                                      float* __restrict__ invstd) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  double s0 = 0.0, s1 = 0.0;
-  for (int s = 0; s < S; ++s) {
-    s0 += partial[(static_cast<size_t>(c) * S + s) * 2];
-    s1 += partial[(static_cast<size_t>(c) * S + s) * 2 + 1];
-  }
-  const double md = s0 / n;                                        // mean - pivot
-  double v = s1 / n - md * md;
-  if (v < 0.0) v = 0.0;
-  mean[c] = static_cast<float>(static_cast<double>(x[static_cast<size_t>(c) * P]) + md);
-  var[c] = static_cast<float>(v);                                  // biased (F.batch_norm normalises with it)
-  invstd[c] = static_cast<float>(1.0 / sqrt(v + static_cast<double>(eps)));
-}
-
-__global__ void bn_bwd_final_kernel(const double* __restrict__ partial, int C, int S,
-                                    float* __restrict__ dgamma, float* __restrict__ dbeta) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  double s0 = 0.0, s1 = 0.0;
-  for (int s = 0; s < S; ++s) {
-    s0 += partial[(static_cast<size_t>(c) * S + s) * 2];
-    s1 += partial[(static_cast<size_t>(c) * S + s) * 2 + 1];
-  }
-  dbeta[c] = static_cast<float>(s0);
-  dgamma[c] = static_cast<float>(s1);
-}
 
 // y = act(gamma*(x-mean)*invstd + beta); grid (ceil(P/1024), C, B)
 template <bool ELU>
@@ -523,12 +420,19 @@ __global__ void __launch_bounds__(256)
 // the GEMM's epilogue scale in the wgrad: 1, the unscale is col_unscale_kernel's
 __device__ const float kUnitScale = 1.f;
 
-// ---- per-cloud BatchNorm records (synchronised BN of data-parallel training) -------------------------
+// ---- train-mode BatchNorm: per-cloud records ------------------------------------------------------
 // Row r = b*C + c of x [B,C,P] gets one fp64 record whose value depends on that row alone: the row's
 // elements are summed in a fixed order chosen from P only (never from B, C or the SM count), so the
-// records of a cloud are the same bits whichever shard it lands in. Forward: {pivot = x[r,0], sum d,
-// sum d*d}, d = x - pivot exact in fp64 (the cancellation argument of bn_partial_kernel). Backward:
-// {sum g, sum g*xhat}, g as in bn_partial_kernel, each term accumulated in fp64.
+// records of a cloud are the same bits whichever batch or data-parallel shard it lands in.
+// Forward: {pivot = x[r,0], sum d, sum d*d}, d = x - pivot. Backward: {sum g, sum g*xhat}, g = dy *
+// [gamma*xhat + beta > 0] for ReLU, dy * elu_grad(gamma*xhat + beta) for ELU, dy for none. Every
+// term is accumulated in fp64.
+//
+// The forward sums are shifted by a pivot drawn from the channel. var = E[d^2] - E[d]^2 then cancels
+// only by 1 + (mean - pivot)^2 / var, a few units for any such pivot, where E[x^2] - mean^2 would
+// cancel by (mean/std)^2: with fp32 sums that is a relative error of ~(mean/std)^2 * 2^-24 in var,
+// 1e-2 at mean/std = 1e3 (channels behind a large bias, near-dead inputs). d is exact in fp64, d*d
+// too, and a constant channel gives var = 0.
 constexpr int BNC_WARP_P = 1024;           // rows up to this length: a warp per row, else a CTA
 
 template <bool BWD, int ACT>
@@ -641,8 +545,9 @@ static void launch_bn_cloud(const float* x, const float* dy, const float* mean, 
         x, dy, mean, invstd, gamma, beta, C, P, rec);
 }
 
-// the forward records of Bg clouds, ascending, onto cloud 0's pivot; then bn_stats_final_kernel's
-// statistics. Shifting record b by s = p_b - p (exact: both are fp32 values) is the identity
+// the forward records of Bg clouds, ascending, onto cloud 0's pivot p; then mean = p + E[x - p] and
+// the biased var = E[(x - p)^2] - E[x - p]^2 (F.batch_norm normalises with it). Shifting record b by
+// s = p_b - p (exact: both are fp32 values) is the identity
 // sum (x - p) = sum d_b + P s, sum (x - p)^2 = sum d_b^2 + 2 s sum d_b + P s^2.
 __global__ void bn_sync_stats_kernel(const double* __restrict__ rec, int Bg, int C, int P, float eps,
                                      float* __restrict__ mean, float* __restrict__ var,
@@ -681,66 +586,6 @@ __global__ void bn_sync_bwd_final_kernel(const double* __restrict__ rec, int Bg,
   dgamma[c] = static_cast<float>(s1);
 }
 }  // namespace sonet
-
-static int bn_splits(int B, int C) {
-  int S = std::max(1, std::min(B, (4 * sonet::sm_count() + C - 1) / C));
-  return std::min(S, 64);
-}
-
-extern "C" int sonet_bn_partial_slots(int B, int C) { return bn_splits(B, C) * C * 2; }
-
-extern "C" int sonet_bn_train_forward_f32(const float* x, const float* gamma, const float* beta,
-                                          int B, int C, int P, float eps, int relu, double* partial,
-                                          float* y, float* save_mean, float* save_var,
-                                          float* save_invstd, sonet_stream_t stream) {
-  using namespace sonet;
-  SONET_REQUIRE_ACT(relu, "bn_train_forward");
-  SONET_REQUIRE(B >= 1 && C >= 1 && P >= 1 && B <= 65535 && C <= 65535, "bn_train_forward: bad dims");
-  SONET_REQUIRE(x && partial && y && save_mean && save_var && save_invstd, "bn_train_forward: null pointer");
-  cudaStream_t st = as_stream(stream);
-  const int S = bn_splits(B, C);
-  bn_partial_kernel<false, false><<<dim3(C, S), BN_THREADS, 0, st>>>(x, nullptr, nullptr, nullptr, nullptr,
-                                                                    nullptr, B, C, P, 0, S, partial);
-  bn_stats_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(partial, x, C, P, S, static_cast<double>(B) * P,
-                                                        eps, save_mean, save_var, save_invstd);
-  const dim3 grid((P + 1023) / 1024, C, B);
-  if (relu == SONET_ACT_ELU)
-    bn_apply_kernel<true><<<grid, 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta, C, P, 0, y);
-  else
-    bn_apply_kernel<false><<<grid, 256, 0, st>>>(x, save_mean, save_invstd, gamma, beta, C, P, relu, y);
-  return check_launch("bn_train_forward");
-}
-
-extern "C" int sonet_bn_train_backward_f32(const float* dy, const float* x, const float* mean,
-                                           const float* invstd, const float* gamma,
-                                           const float* beta, int B, int C, int P, int relu,
-                                           double* partial, float* dx, float* dgamma, float* dbeta,
-                                           sonet_stream_t stream) {
-  using namespace sonet;
-  SONET_REQUIRE_ACT(relu, "bn_train_backward");
-  SONET_REQUIRE(B >= 1 && C >= 1 && P >= 1 && B <= 65535 && C <= 65535, "bn_train_backward: bad dims");
-  SONET_REQUIRE(dy && x && mean && invstd && partial && dx && dgamma && dbeta,
-                "bn_train_backward: null pointer");
-  cudaStream_t st = as_stream(stream);
-  const int S = bn_splits(B, C);
-  const bool elu = relu == SONET_ACT_ELU;
-  if (elu)
-    bn_partial_kernel<true, true><<<dim3(C, S), BN_THREADS, 0, st>>>(x, dy, mean, invstd, gamma, beta, B, C,
-                                                                    P, 0, S, partial);
-  else
-    bn_partial_kernel<true, false><<<dim3(C, S), BN_THREADS, 0, st>>>(x, dy, mean, invstd, gamma, beta, B,
-                                                                     C, P, relu, S, partial);
-  bn_bwd_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(partial, C, S, dgamma, dbeta);
-  const dim3 grid((P + 1023) / 1024, C, B);
-  const float inv_n = static_cast<float>(1.0 / (static_cast<double>(B) * P));
-  if (elu)
-    bn_bwd_apply_kernel<true><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
-                                                    0, inv_n, dx);
-  else
-    bn_bwd_apply_kernel<false><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
-                                                     relu, inv_n, dx);
-  return check_launch("bn_train_backward");
-}
 
 extern "C" int sonet_bn_cloud_partials_f32(const float* x, const float* dy, const float* mean,
                                            const float* invstd, const float* gamma, const float* beta,

@@ -272,11 +272,12 @@ class DataParallelTraining:
     process group, with the semantics of one process over the global batch:
 
       * every BatchNorm normalises by the statistics of the whole global batch and updates its
-        running statistics with the global count. Each rank writes one fp64 record per (cloud,
-        channel) (sonet_bn_cloud_partials_f32), the records are gathered along the cloud axis and
-        folded in ascending cloud order (sonet_bn_sync_forward_f32 / _backward_f32). The records
-        depend only on their cloud, so mean, var, y, dx, dgamma and dbeta are bit-identical at
-        every world size and sharding;
+        running statistics with the global count. Each rank writes the train-mode BatchNorm's one
+        fp64 record per (cloud, channel) (sonet_bn_cloud_partials_f32), as a single process does;
+        the records are gathered along the cloud axis and folded in ascending cloud order
+        (sonet_bn_sync_forward_f32 / _backward_f32). The records depend only on their cloud, so
+        mean, var, y, dx, dgamma and dbeta are bit-identical at every world size and sharding, and
+        to those of one process over the global batch;
       * before every step of an optimizer over the model's parameters, its gradients are scaled
         by B_r / Bg (every loss of the reference is a batch mean), gathered and summed in
         ascending rank order: every rank steps on the same gradient of the global-batch loss.
@@ -288,8 +289,8 @@ class DataParallelTraining:
     global batch (DeviceDataset.batch(..., shard=(rank, world))). The host RNGs (`random`,
     `np.random`: the point dropout of the reference's optimize(), the per-cloud augmentation
     scalars) must be seeded identically on every rank; nn.Dropout masks differ per rank, as they
-    do between two single-GPU runs. Without a process group the exchange is the identity and the
-    per-cloud route still runs: a one-process run is the reference for a run over G ranks.
+    do between two single-GPU runs. Without a process group the exchange is the identity: a
+    one-process run is the reference for a run over G ranks.
 
     The optimizers are hooked through torch.optim's global step pre-hook, restricted to those
     that step a parameter of the model, so optimizers the Model creates lazily in its first
@@ -363,7 +364,9 @@ class DataParallelTraining:
 
     def close(self):
         """Remove the BatchNorm exchange and the optimizer hook: train steps are single-process
-        steps again, bit for bit."""
+        steps again. Their BatchNorms give the bits they gave under the exchange at world 1, except
+        those of the decoder's 3x3 convolutions below UPCONV_MIN_HW, which return to PyTorch's
+        BatchNorm."""
         from . import train_ops
         if self._hook is not None:
             self._hook.remove()

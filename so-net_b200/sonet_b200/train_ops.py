@@ -7,10 +7,10 @@ models/networks.py:185).
                   (weights / activations packed on the device each step; gradients pre-scaled by a
                   power of two before the fp16 hi/lo split)
     BNActTrain    batch-statistics BatchNorm + ReLU / ELU / none, forward and backward, fused elementwise passes
-                  and two-stage deterministic reductions; with EXCHANGE installed (data-parallel
-                  training) the per-cloud route, synchronised over the ranks
+                  and deterministic reductions through per-cloud records, which EXCHANGE
+                  (data-parallel training) synchronises over the ranks
     InstanceNormActTrain  instance norm + ReLU / ELU / none: the instance-norm kernel forward, the
-                  BN backward on the [1, B*C, P] view
+                  BatchNorm backward on the [1, B*C, P] view
     UpConvTC      nearest x2 up-sampling + 3x3 conv (pad 1) as four parity GEMMs over the
                   low-resolution map (csrc/upconv.cu): forward, dgrad (one GEMM with K = 16*Cout over
                   the gathered gradient D) and wgrad (one GEMM per parity) on the wgmma layer kernel
@@ -51,8 +51,7 @@ def _f16(name, f16):
     return (name[:-4] if name.endswith("_f32") else name) + "_f16"
 
 
-def _scratch(dev, n, dtype, cache=None):
-    cache = _SCRATCH if cache is None else cache
+def _scratch(dev, n, dtype, cache):
     key = (dev, dtype)
     buf = cache.get(key)
     if buf is None or buf.numel() < n:
@@ -60,88 +59,76 @@ def _scratch(dev, n, dtype, cache=None):
     return buf
 
 
-_SCRATCH = {}
-
-
 def scratch_buffers():
     """Every scratch buffer the train ops hold now. A captured CUDA graph keeps these alive: a
     larger step replaces a buffer in its cache, and the graph must not write into freed memory."""
-    return list(_SCRATCH.values()) + [b for c in _WGRAD_CACHE.values() for b in c.values()]
+    return [b for c in _WGRAD_CACHE.values() for b in c.values()]
 
 
-# The BatchNorm exchange of data-parallel training (dist.DataParallelTraining), or None. While one is
-# installed, BNActTrain takes the per-cloud route: the records of the local clouds, gathered along the
-# cloud axis by EXCHANGE.gather(rec) -> [Bg, C, k] in global cloud order, then folded in that order.
-# EXCHANGE.global_rows(B) is the global batch Bg of a local batch of B clouds.
+# The BatchNorm exchange of data-parallel training (dist.DataParallelTraining), or None. BNActTrain
+# writes the records of the local clouds, gathers them along the cloud axis by exchange.gather(rec)
+# -> [Bg, C, k] in global cloud order, then folds them in that order. exchange.global_rows(B) is the
+# global batch Bg of a local batch of B clouds. With none installed BNActTrain uses _LOCAL.
 EXCHANGE = None
 
 
-def _bn_sync_forward(x, gamma, beta, eps, act, ex):
-    B, C, P = x.shape
-    Bg = ex.global_rows(B)
-    dev = x.device
-    with torch.cuda.device(dev):
-        y = torch.empty_like(x)
-        mean = torch.empty(C, dtype=torch.float32, device=dev)
-        var = torch.empty(C, dtype=torch.float32, device=dev)
-        invstd = torch.empty(C, dtype=torch.float32, device=dev)
-        rec = torch.empty((B, C, _C.CONSTANTS["SONET_BN_REC_FWD"]), dtype=torch.float64, device=dev)
-        ops._call("sonet_bn_cloud_partials_f32", _C.ptr(x), None, None, None, None, None, B, C, P,
-                  ops.act_code(act), 0, _C.ptr(rec), ops._stream(x))
-        rec = ex.gather(rec)
-        ops._call("sonet_bn_sync_forward_f32", _C.ptr(rec), _C.ptr(x), _C.ptr(gamma), _C.ptr(beta),
-                  Bg, B, C, P, float(eps), ops.act_code(act), _C.ptr(y), _C.ptr(mean), _C.ptr(var),
-                  _C.ptr(invstd), ops._stream(x), kernels=2)
-    return y, mean, var, invstd
+class _LocalExchange:
+    """One process's batch is the whole batch."""
+
+    @staticmethod
+    def global_rows(B):
+        return B
+
+    @staticmethod
+    def gather(rec):
+        return rec
 
 
-def _bn_sync_backward(dy, x, mean, invstd, gamma, beta, act, ex):
-    """dy is the gradient of this rank's loss, a mean over its B clouds. The exchange works in
-    units of the global-batch loss, whose gradient here is dy * B / Bg: dgamma and dbeta come out
-    as the global gradients, the same on every rank, and dx goes back to this rank's units."""
-    B, C, P = x.shape
-    dev = x.device
-    share = B / ex.global_rows(B)
-    if share != 1.0:
-        dy = dy * share
-    with torch.cuda.device(dev):
-        dx = torch.empty_like(x)
-        dgamma = torch.empty(C, dtype=torch.float32, device=dev)
-        dbeta = torch.empty(C, dtype=torch.float32, device=dev)
-        rec = torch.empty((B, C, _C.CONSTANTS["SONET_BN_REC_BWD"]), dtype=torch.float64, device=dev)
-        ops._call("sonet_bn_cloud_partials_f32", _C.ptr(x), _C.ptr(dy), _C.ptr(mean), _C.ptr(invstd),
-                  _C.ptr(gamma), _C.ptr(beta), B, C, P, act, 1, _C.ptr(rec), ops._stream(x))
-        rec = ex.gather(rec)
-        ops._call("sonet_bn_sync_backward_f32", _C.ptr(rec), _C.ptr(dy), _C.ptr(x), _C.ptr(mean),
-                  _C.ptr(invstd), _C.ptr(gamma), _C.ptr(beta), ex.global_rows(B), B, C, P, act,
-                  _C.ptr(dx), _C.ptr(dgamma), _C.ptr(dbeta), ops._stream(x), kernels=2)
-    if share != 1.0:
-        dx.div_(share)
-    return dx, dgamma, dbeta
+_LOCAL = _LocalExchange()
+
+
+def _exchange():
+    return _LOCAL if EXCHANGE is None else EXCHANGE
+
+
+def _bn_backward(dy, x, mean, invstd, gamma, beta, B, C, P, act, ex, dx, dgamma, dbeta):
+    """The BatchNorm backward of x [B,C,P] (contiguous, like dy and dx) into dx, dgamma, dbeta: the
+    records of the B local clouds, gathered by the exchange ex and folded over its global batch."""
+    rec = torch.empty((B, C, _C.CONSTANTS["SONET_BN_REC_BWD"]), dtype=torch.float64, device=x.device)
+    ops._call("sonet_bn_cloud_partials_f32", _C.ptr(x), _C.ptr(dy), _C.ptr(mean), _C.ptr(invstd),
+              _C.ptr(gamma), _C.ptr(beta), B, C, P, act, 1, _C.ptr(rec), ops._stream(x))
+    rec = ex.gather(rec)
+    ops._call("sonet_bn_sync_backward_f32", _C.ptr(rec), _C.ptr(dy), _C.ptr(x), _C.ptr(mean),
+              _C.ptr(invstd), _C.ptr(gamma), _C.ptr(beta), ex.global_rows(B), B, C, P, act,
+              _C.ptr(dx), _C.ptr(dgamma), _C.ptr(dbeta), ops._stream(x), kernels=2)
 
 
 class BNActTrain(torch.autograd.Function):
+    """Batch-statistics BatchNorm + activation of x [B,C,P] through the per-cloud records
+    (sonet_bn_cloud_partials_f32, then sonet_bn_sync_forward_f32 / _backward_f32). The backward's
+    dy is the gradient of this process's loss, a mean over its B clouds. The exchange works in
+    units of the global-batch loss, whose gradient here is dy * B / Bg: dgamma and dbeta come out
+    as the global gradients, the same on every rank, and dx goes back to this rank's units."""
+
     @staticmethod
     def forward(ctx, x, gamma, beta, eps, act):
         x = x.contiguous()
         B, C, P = x.shape
         dev = x.device
-        ctx.exchange = EXCHANGE
+        ex = ctx.exchange = _exchange()
         ctx.act = ops.act_code(act)
-        if EXCHANGE is not None:
-            y, mean, var, invstd = _bn_sync_forward(x, gamma, beta, eps, act, EXCHANGE)
-            ctx.save_for_backward(x, mean, invstd, gamma, beta)
-            ctx.mark_non_differentiable(mean, var)
-            return y, mean, var
         with torch.cuda.device(dev):
             y = torch.empty_like(x)
             mean = torch.empty(C, dtype=torch.float32, device=dev)
             var = torch.empty(C, dtype=torch.float32, device=dev)
             invstd = torch.empty(C, dtype=torch.float32, device=dev)
-            part = _scratch(dev, _C.lib().sonet_bn_partial_slots(B, C), torch.float64)
-            ops._call("sonet_bn_train_forward_f32", _C.ptr(x), _C.ptr(gamma), _C.ptr(beta), B, C, P,
-                      float(eps), ops.act_code(act), _C.ptr(part), _C.ptr(y), _C.ptr(mean), _C.ptr(var),
-                      _C.ptr(invstd), ops._stream(x), kernels=3)
+            rec = torch.empty((B, C, _C.CONSTANTS["SONET_BN_REC_FWD"]), dtype=torch.float64, device=dev)
+            ops._call("sonet_bn_cloud_partials_f32", _C.ptr(x), None, None, None, None, None, B, C, P,
+                      ctx.act, 0, _C.ptr(rec), ops._stream(x))
+            rec = ex.gather(rec)
+            ops._call("sonet_bn_sync_forward_f32", _C.ptr(rec), _C.ptr(x), _C.ptr(gamma), _C.ptr(beta),
+                      ex.global_rows(B), B, C, P, float(eps), ctx.act, _C.ptr(y), _C.ptr(mean),
+                      _C.ptr(var), _C.ptr(invstd), ops._stream(x), kernels=2)
         ctx.save_for_backward(x, mean, invstd, gamma, beta)
         ctx.mark_non_differentiable(mean, var)
         return y, mean, var
@@ -150,29 +137,28 @@ class BNActTrain(torch.autograd.Function):
     def backward(ctx, dy, _dm, _dv):
         x, mean, invstd, gamma, beta = ctx.saved_tensors
         dy = dy.contiguous()
-        if ctx.exchange is not None:
-            dx, dgamma, dbeta = _bn_sync_backward(dy, x, mean, invstd, gamma, beta, ctx.act,
-                                                  ctx.exchange)
-            return dx, dgamma, dbeta, None, None
         B, C, P = x.shape
         dev = x.device
+        share = B / ctx.exchange.global_rows(B)
+        if share != 1.0:
+            dy = dy * share
         with torch.cuda.device(dev):
             dx = torch.empty_like(x)
             dgamma = torch.empty(C, dtype=torch.float32, device=dev)
             dbeta = torch.empty(C, dtype=torch.float32, device=dev)
-            part = _scratch(dev, _C.lib().sonet_bn_partial_slots(B, C), torch.float64)
-            ops._call("sonet_bn_train_backward_f32", _C.ptr(dy), _C.ptr(x), _C.ptr(mean),
-                      _C.ptr(invstd), _C.ptr(gamma), _C.ptr(beta), B, C, P, ctx.act,
-                      _C.ptr(part), _C.ptr(dx), _C.ptr(dgamma), _C.ptr(dbeta), ops._stream(x),
-                      kernels=3)
+            _bn_backward(dy, x, mean, invstd, gamma, beta, B, C, P, ctx.act, ctx.exchange, dx, dgamma,
+                         dbeta)
+        if share != 1.0:
+            dx.div_(share)
         return dx, dgamma, dbeta, None, None
 
 
 class InstanceNormActTrain(torch.autograd.Function):
     """Instance norm (affine, no running statistics) + ReLU / ELU / none of z [B,C,P]. Forward:
-    the instance-norm kernel, keeping each row's mean and invstd. Backward: the BN-train backward
-    on the [1, B*C, P] view, whose per-channel statistics are exactly the per-row ones, with gamma
-    and beta expanded to [B*C]; dgamma and dbeta are then summed over the clouds in fp64."""
+    the instance-norm kernel, keeping each row's mean and invstd. Backward: the BatchNorm backward
+    of one cloud on the [1, B*C, P] view, whose per-channel statistics are exactly the per-row
+    ones, with gamma and beta expanded to [B*C]; dgamma and dbeta are then summed over the clouds
+    in fp64."""
 
     @staticmethod
     def forward(ctx, z, gamma, beta, eps, act):
@@ -189,7 +175,7 @@ class InstanceNormActTrain(torch.autograd.Function):
         dy = dy.contiguous()
         B, C, P = z.shape
         dev = z.device
-        # the kernel's grid holds at most 65535 channels: whole clouds per call
+        # the entries take at most 65535 channels: whole clouds per call
         cb = max(1, 65535 // C)
         with torch.cuda.device(dev):
             dz = torch.empty_like(z)
@@ -197,14 +183,11 @@ class InstanceNormActTrain(torch.autograd.Function):
             b_rows = beta.detach().repeat(cb).contiguous()
             dgamma = torch.empty((B, C), dtype=torch.float32, device=dev)
             dbeta = torch.empty((B, C), dtype=torch.float32, device=dev)
-            part = _scratch(dev, _C.lib().sonet_bn_partial_slots(1, cb * C), torch.float64)
             for b0 in range(0, B, cb):
                 n = min(cb, B - b0)
-                ops._call("sonet_bn_train_backward_f32", _C.ptr(dy[b0:b0 + n]), _C.ptr(z[b0:b0 + n]),
-                          _C.ptr(mean[b0:b0 + n]), _C.ptr(invstd[b0:b0 + n]), _C.ptr(g_rows),
-                          _C.ptr(b_rows), 1, n * C, P, ctx.act, _C.ptr(part), _C.ptr(dz[b0:b0 + n]),
-                          _C.ptr(dgamma[b0:b0 + n]), _C.ptr(dbeta[b0:b0 + n]), ops._stream(z),
-                          kernels=3)
+                _bn_backward(dy[b0:b0 + n], z[b0:b0 + n], mean[b0:b0 + n], invstd[b0:b0 + n], g_rows,
+                             b_rows, 1, n * C, P, ctx.act, _LOCAL, dz[b0:b0 + n], dgamma[b0:b0 + n],
+                             dbeta[b0:b0 + n])
         return (dz, dgamma.double().sum(0).float(), dbeta.double().sum(0).float(), None, None)
 
 
@@ -493,7 +476,7 @@ def norm_act_train(y0, norm, act, epoch=None, size=None):
             return F.elu(y0)
         return torch.relu(y0) if code == ops.ACT_RELU else y0
     # with a BatchNorm exchange installed the statistics are those of the global batch
-    n = (B if EXCHANGE is None else EXCHANGE.global_rows(B)) * P
+    n = _exchange().global_rows(B) * P
     if n == 1:         # F.batch_norm's check: a batch statistic of one value is undefined
         raise ValueError("Expected more than 1 value per channel when training, got input size "
                          "{}".format(size))

@@ -1,6 +1,7 @@
-"""C-ABI of the activation codes (SONET_ACT_NONE / _RELU / _ELU), without a GPU: every entry with an
-activation argument rejects an unknown code with a negative status and a message before any CUDA
-call, and the explicit-activation entries of the fused kernels are exported and bound."""
+"""C-ABI of the activation codes (SONET_ACT_NONE / _RELU / _ELU), without a GPU: every layer entry
+with an activation argument rejects an unknown code with a negative status and a message before any
+CUDA call, and the explicit-activation entries of the fused kernels are exported and bound. The
+train-mode BatchNorm entries' check is test_dp_train_host.test_rejects_unknown_activation."""
 import ctypes
 import os
 import re
@@ -14,7 +15,7 @@ ACT_ENTRIES = ("sonet_pointresnet_tc_forward_act", "sonet_pointresnet_tc_pool_fo
 
 
 def _calls(lib, act):
-    """Each entry with an activation argument, called with `act` and otherwise plausible
+    """Each layer entry with an activation argument, called with `act` and otherwise plausible
     arguments (null pointers: the activation check must come first)."""
     n = None
     return {
@@ -35,10 +36,6 @@ def _calls(lib, act):
             n, 64, 2, 64, n, 0, 1.0, n, 64, act, 1, 1, 0, 0, 64, 0, n, n, n),
         "sonet_pointwise_tc_forward_dev": lambda: lib.sonet_pointwise_tc_forward_dev(
             n, 64, 2, 64, n, n, n, n, 64, act, 1, n, n, n),
-        "sonet_bn_train_forward_f32": lambda: lib.sonet_bn_train_forward_f32(
-            n, n, n, 2, 8, 16, 1e-5, act, n, n, n, n, n, n),
-        "sonet_bn_train_backward_f32": lambda: lib.sonet_bn_train_backward_f32(
-            n, n, n, n, n, n, 2, 8, 16, act, n, n, n, n, n),
         "sonet_pointresnet_tc_forward_act": lambda: lib.sonet_pointresnet_tc_forward_act(
             n, 6, 2, 256, n, n, act, 0, n, n),
         "sonet_pointresnet_tc_pool_forward_act": lambda: lib.sonet_pointresnet_tc_pool_forward_act(
@@ -49,7 +46,7 @@ def _calls(lib, act):
 
 
 @pytest.mark.parametrize("act", [3, -1])
-def test_unknown_activation_codes_are_rejected(lib_built, act):
+def test_layer_entries_reject_unknown_activation_codes(lib_built, act):
     from sonet_b200 import _C
     lib = _C.lib()
     for name, call in _calls(lib, act).items():

@@ -477,17 +477,20 @@ def _adam_first_step_dir(g):
 
 
 STEP_GRAD_TOL = 1e-4
+# the activation code's position in the arguments of each train-mode BatchNorm entry
+BN_ACT_ARG = {"sonet_bn_cloud_partials_f32": 9, "sonet_bn_sync_forward_f32": 9,
+              "sonet_bn_sync_backward_f32": 11}
 
 
 @pytest.mark.parametrize("task", ["classifier", "segmenter", "autoencoder"])
-def test_elu_optimize_step_kernels_on_vs_off(task):
+def test_elu_optimize_step_train_kernels_vs_pytorch(task):
     """One optimize() of an ELU model, train kernels on vs the PyTorch composition: the criteria
     of test_gpu_train_parity.py's kernels-on-vs-off step test."""
     from sonet_b200 import ops
     ops.PROFILE = []
     try:
         on, g_on, before, lr = _wrapper_step(task, True)
-        bn_acts = [a[7] for n, _, _, a in ops.PROFILE if n == "sonet_bn_train_forward_f32"]
+        bn_acts = [a[BN_ACT_ARG[n]] for n, _, _, a in ops.PROFILE if n in BN_ACT_ARG]
     finally:
         ops.PROFILE = None
     assert bn_acts and set(bn_acts) == {ELU}, bn_acts

@@ -357,16 +357,18 @@ GRAD_TOL = 5e-2
 STEP_OUTLIERS = 1e-3
 
 
-def test_instance_segmenter_optimize_step_kernels_on_vs_off():
+def test_instance_segmenter_optimize_step_train_kernels_vs_pytorch():
     from sonet_b200 import ops
     ops.PROFILE = []
     try:
         loss_on, on, g_on, before, lr = _segmenter_step(True)
         names = [n for n, _, _, _ in ops.PROFILE]
+        bn_forwards = [n for n, _, _, a in ops.PROFILE if n == "sonet_bn_sync_forward_f32"
+                       or (n == "sonet_bn_cloud_partials_f32" and not a[10])]
     finally:
         ops.PROFILE = None
-    assert "sonet_instance_norm_f32" in names and "sonet_bn_train_backward_f32" in names
-    assert "sonet_bn_train_forward_f32" not in names, "a BatchNorm forward ran in an instance model"
+    assert "sonet_instance_norm_f32" in names and "sonet_bn_sync_backward_f32" in names
+    assert not bn_forwards, "a BatchNorm forward ran in an instance model"
     loss_off, off, g_off, _, _ = _segmenter_step(False)
     print("loss on %.8f off %.8f" % (loss_on, loss_off))
     assert abs(loss_on - loss_off) <= 1e-4 * max(1.0, abs(loss_off)), (loss_on, loss_off)

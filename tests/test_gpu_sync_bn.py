@@ -1,12 +1,10 @@
-"""-m gpu: the synchronised BatchNorm of data-parallel training (csrc/train.cu:
-sonet_bn_cloud_partials_f32, sonet_bn_sync_forward_f32 / _backward_f32) in one process.
+"""-m gpu: the train-mode BatchNorm's records synchronised as data-parallel training does
+(csrc/train.cu: sonet_bn_cloud_partials_f32, sonet_bn_sync_forward_f32 / _backward_f32), in one
+process. Its accuracy against fp64 is test_gpu_train_parity.test_bn_train_vs_fp64.
 
   * shard invariance: the records of every shard of a batch, concatenated in cloud order and folded
     by each shard's sync forward / backward, give torch.equal y, mean, var, invstd, dx, dgamma and
     dbeta to the unsplit call, at every shape, activation and split;
-  * accuracy: BNActTrain on the per-cloud route (a one-process exchange installed) against fp64
-    F.batch_norm with the error bars of the existing BatchNorm test (test_gpu_train_parity.py),
-    which includes channels at mean/std = 1e3 and 1e4 and constant channels; plus P = 1 at B = 2;
   * reproducibility: two identical calls give identical bits."""
 import pytest
 import torch
@@ -122,35 +120,67 @@ def test_partial_records_depend_on_their_cloud_only(act):
         assert not torch.equal(c[3], a[3])
 
 
-# ---- accuracy: the per-cloud route through BNActTrain against fp64 ------------------------------------
-@pytest.fixture
-def per_cloud_route():
-    """Install a one-process exchange (the identity, as DataParallelTraining installs without a
-    process group) whose global batch follows each call's B."""
+# ---- one route: a single process computes what data-parallel training at world 1 computes ----------
+def _one_process_and_world1(run, model, B):
+    """run() with no exchange installed, then under DataParallelTraining(model, B) without a process
+    group: every tensor it returns must be the same bits."""
+    from sonet_b200 import dist as sdist, train_ops
+    assert train_ops.EXCHANGE is None
+    alone = run()
+    with sdist.DataParallelTraining(model, B):
+        world1 = run()
+    assert train_ops.EXCHANGE is None
+    for k in alone:
+        assert torch.equal(alone[k], world1[k]), \
+            "%s differs between one process and data-parallel training at world 1" % k
+
+
+def test_layer_step_is_the_same_alone_and_at_world1():
+    """A train-mode EquivariantLayer on ConvTC (a wgmma shape: deterministic) with BatchNorm + ReLU:
+    forward, backward and running-statistics update."""
+    import copy
+    from sonet_b200 import layers, ops
+    torch.manual_seed(0)
+    base = layers.EquivariantLayer(64, 128, 'relu', 'batch').to(DEV).train()
+    g = torch.Generator(device=DEV).manual_seed(1)
+    x = torch.randn(8, 64, 1000, device=DEV, generator=g)
+    dy = torch.randn(8, 128, 1000, device=DEV, generator=g)
+    layer = copy.deepcopy(base)
+
+    def run():
+        layer.load_state_dict(base.state_dict())
+        layer.zero_grad(set_to_none=True)
+        xg = x.clone().requires_grad_(True)
+        ops.PROFILE = []
+        try:
+            y = layer(xg)
+            y.backward(dy)
+            names = {n for n, _, _, _ in ops.PROFILE}
+        finally:
+            ops.PROFILE = None
+        # the wgmma convolution and the BatchNorm kernels ran
+        assert "sonet_wgrad_tc_f32" in names and any(n.startswith("sonet_bn_") for n in names), names
+        out = dict(y=y.detach(), dx=xg.grad,
+                   running_mean=layer.norm.running_mean.clone(),
+                   running_var=layer.norm.running_var.clone())
+        out.update({"grad " + k: p.grad.clone() for k, p in layer.named_parameters()})
+        return out
+
+    _one_process_and_world1(run, layer, x.shape[0])
+
+
+BN_ROUTE_CASES = [("relu", (32, 64, 15000)), ("elu", (32, 512, 576)), ("none", (32, 1024, 1))]
+
+
+@pytest.mark.parametrize("act,shape", BN_ROUTE_CASES, ids=[c[0] for c in BN_ROUTE_CASES])
+def test_bn_is_the_same_alone_and_at_world1(act, shape):
     from sonet_b200 import train_ops
+    x, dy, gamma, beta = _case(*shape, seed=sum(shape))
 
-    class _Identity:
-        def global_rows(self, B):
-            return B
+    def run():
+        xg, gg, bg = (t.clone().requires_grad_(True) for t in (x, gamma, beta))
+        y, mean, var = train_ops.BNActTrain.apply(xg, gg, bg, 1e-5, None if act == "none" else act)
+        y.backward(dy)
+        return dict(y=y.detach(), mean=mean, var=var, dx=xg.grad, dgamma=gg.grad, dbeta=bg.grad)
 
-        def gather(self, rec):
-            return rec
-
-    prev = train_ops.EXCHANGE
-    train_ops.EXCHANGE = _Identity()
-    yield
-    train_ops.EXCHANGE = prev
-
-
-import test_gpu_train_parity as parity  # noqa: E402  (the existing BatchNorm test's bars)
-
-ACC_SHAPES = parity.BN_SHAPES + [("p1_b2", 2, 64, 1, True), ("p1_b2_linear", 2, 64, 1, False)]
-
-
-@pytest.mark.parametrize("name,B,C,P,relu", ACC_SHAPES, ids=[s[0] for s in ACC_SHAPES])
-def test_per_cloud_route_vs_fp64(per_cloud_route, name, B, C, P, relu):
-    """test_gpu_train_parity.test_bn_train_vs_fp64 (fp64 reference, its bars, bit-reproducibility,
-    var == 0 and invstd == 1/sqrt(eps) on constant channels) with BNActTrain on the per-cloud route."""
-    from sonet_b200 import train_ops
-    assert train_ops.EXCHANGE is not None
-    parity.test_bn_train_vs_fp64(name, B, C, P, relu)
+    _one_process_and_world1(run, torch.nn.Module(), shape[0])

@@ -3,7 +3,7 @@
   A. the batch-statistics BatchNorm kernels (csrc/train.cu through train_ops.BNActTrain) against
      fp64 statistics and F.batch_norm + ReLU in fp64, over channels whose |mean|/std spans 0..1e4,
      near-constant and constant channels, variances around eps, gamma = 0 and dead ReLUs, at the
-     training shapes and at every branch of the split count;
+     training shapes and at every branch of the per-cloud record kernels;
   B. every train-mode layer kind (kernels on, PyTorch's default precision flags) against the same
      module in fp64, held to 8x the error of a strict-fp32 run of the PyTorch composition; and the
      whole training step with cuDNN's TF32 flag on and off;
@@ -144,8 +144,9 @@ def _units(err, bar):
 
 BN_SHAPES = [
     # name, B, C, P, relu: the training shapes (first PointResNet at N = 5000, KNN module),
-    # B = 1 with a long odd row, P = 1, and each branch of bn_splits (S = B, S = 1 at C > 4 SMs,
-    # the 64 cap at C = 1)
+    # B = 1 with a long odd row, C = 1, and each branch of the record kernels: a thread per record
+    # (P = 1, also at B = 2), a warp (1 < P <= 1024) and a 256-thread CTA (P > 1024), with both
+    # sides of the warp / CTA edge
     ("first_pointresnet_n5000", 64, 64, 15000, True),
     ("knn_module", 64, 512, 576, True),
     ("b1_p100003", 1, 16, 100003, False),
@@ -154,6 +155,10 @@ BN_SHAPES = [
     ("c600_one_split", 3, 600, 257, False),
     ("b4_split_b", 4, 40, 3000, True),
     ("b4_split_b_linear", 4, 40, 3000, False),
+    ("p1_b2", 2, 64, 1, True),
+    ("p1_b2_linear", 2, 64, 1, False),
+    ("p1024_warp_edge", 5, 48, 1024, True),
+    ("p1025_cta_edge", 5, 48, 1025, False),
 ]
 
 

@@ -1,12 +1,13 @@
-"""Time the batch-statistics BatchNorm forward (sonet_bn_train_forward_f32: partial sums, final
-statistics, normalise + ReLU) at the training shapes, CUDA events around back-to-back calls.
+"""Time the batch-statistics BatchNorm at the training shapes, CUDA events around back-to-back
+calls: the forward (sonet_bn_cloud_partials_f32's per-cloud records, then sonet_bn_sync_forward_f32's
+fold and normalise + ReLU) and the backward (the backward records, then sonet_bn_sync_backward_f32).
 
     python tools/bn_train_bench.py [--baseline-lib other/libsonet_b200.so] [--out results.jsonl]
 
 With --baseline-lib the same call of another build of the library is timed in the same process,
 alternating with this tree's in every repetition, so that both see the same clocks and neighbours;
-both builds' statistics are compared too. Prints one JSON line per shape with medians in ms and the
-GPU's name and power limit.
+both builds' statistics are compared too. Prints one JSON line per shape and direction with medians
+in ms and the GPU's name and power limit.
 """
 import argparse
 import ctypes
@@ -27,12 +28,12 @@ from sonet_b200 import _C  # noqa: E402
 # (B, C, P): the first PointResNet's BN layers at N = 5000 (3 copies of the cloud per point) and
 # the KNN module's (64 nodes x 9 neighbours)
 SHAPES = ((64, 64, 15000), (64, 512, 576))
-FWD = "sonet_bn_train_forward_f32"
+ENTRIES = ("sonet_bn_cloud_partials_f32", "sonet_bn_sync_forward_f32", "sonet_bn_sync_backward_f32")
 
 
 def load(path):
     lib = ctypes.CDLL(os.path.abspath(path))
-    for name in (FWD, "sonet_bn_partial_slots"):
+    for name in ENTRIES:
         fn = getattr(lib, name)
         fn.argtypes = _C._SIGNATURES[name]
         fn.restype = ctypes.c_int
@@ -63,39 +64,58 @@ def main():
     for B, C, P in SHAPES:
         g = torch.Generator(device=dev).manual_seed(B + C + P)
         x = torch.randn(B, C, P, device=dev, generator=g) * 2 + torch.randn(C, 1, device=dev, generator=g)
+        dy = torch.randn(B, C, P, device=dev, generator=g)
         gamma = torch.rand(C, device=dev, generator=g) + 0.5
         beta = torch.randn(C, device=dev, generator=g) * 0.2
         out = {}
         for k, lib in libs.items():
-            part = torch.empty(lib.sonet_bn_partial_slots(B, C), dtype=torch.float64, device=dev)
-            y = torch.empty_like(x)
-            st = [torch.empty(C, device=dev) for _ in range(3)]
-            args = (x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), B, C, P, 1e-5, 1,
-                    part.data_ptr(), y.data_ptr(), *[t.data_ptr() for t in st], stream)
-            fn = getattr(lib, FWD)
-            out[k] = dict(call=lambda fn=fn, args=args: _C.check(fn(*args), FWD), y=y, stats=st)
-            out[k]["call"]()
+            rec = torch.empty(B * C * _C.CONSTANTS["SONET_BN_REC_FWD"], dtype=torch.float64, device=dev)
+            y, dx = torch.empty_like(x), torch.empty_like(x)
+            st = [torch.empty(C, device=dev) for _ in range(5)]      # mean, var, invstd, dgamma, dbeta
+            p = lambda t: t.data_ptr()
+
+            def fwd(lib=lib, rec=rec, y=y, st=st):
+                _C.check(lib.sonet_bn_cloud_partials_f32(p(x), None, None, None, None, None, B, C, P, 1,
+                                                         0, p(rec), stream), ENTRIES[0])
+                _C.check(lib.sonet_bn_sync_forward_f32(p(rec), p(x), p(gamma), p(beta), B, B, C, P, 1e-5,
+                                                       1, p(y), *[p(t) for t in st[:3]], stream),
+                         ENTRIES[1])
+
+            def bwd(lib=lib, rec=rec, dx=dx, st=st):
+                mean, _, invstd, dgamma, dbeta = st
+                _C.check(lib.sonet_bn_cloud_partials_f32(p(x), p(dy), p(mean), p(invstd), p(gamma),
+                                                         p(beta), B, C, P, 1, 1, p(rec), stream),
+                         ENTRIES[0])
+                _C.check(lib.sonet_bn_sync_backward_f32(p(rec), p(dy), p(x), p(mean), p(invstd),
+                                                        p(gamma), p(beta), B, B, C, P, 1, p(dx),
+                                                        p(dgamma), p(dbeta), stream), ENTRIES[2])
+            out[k] = dict(forward=fwd, backward=bwd, stats=st)
+            fwd()
+            bwd()
         torch.cuda.synchronize()
-        times = {k: [] for k in libs}
-        for _ in range(a.reps):
-            for k in libs:                     # alternate the builds within every repetition
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(a.inner):
-                    out[k]["call"]()
-                e1.record()
-                e1.synchronize()
-                times[k].append(e0.elapsed_time(e1) / a.inner)
-        r = dict(B=B, C=C, P=P, gpu=gpu_info(), bytes_per_call=3 * 4 * B * C * P)
-        for k in libs:
-            r[k + "_ms"] = float(np.median(times[k]))
-            r[k + "_ms_spread"] = [float(np.min(times[k])), float(np.max(times[k]))]
-        if "baseline" in out:
-            v64 = x.double().var(dim=(0, 2), unbiased=False)
+        for direction in ("forward", "backward"):
+            times = {k: [] for k in libs}
+            for _ in range(a.reps):
+                for k in libs:                     # alternate the builds within every repetition
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(a.inner):
+                        out[k][direction]()
+                    e1.record()
+                    e1.synchronize()
+                    times[k].append(e0.elapsed_time(e1) / a.inner)
+            # forward: read x twice, write y; backward: read x and dy twice, write dx
+            nbytes = (3 if direction == "forward" else 5) * 4 * B * C * P
+            r = dict(B=B, C=C, P=P, direction=direction, gpu=gpu_info(), bytes_per_call=nbytes)
             for k in libs:
-                r[k + "_var_max_rel_err"] = float(((out[k]["stats"][1].double() - v64).abs() / v64).max())
-        rows.append(r)
-        print(json.dumps(r), flush=True)
+                r[k + "_ms"] = float(np.median(times[k]))
+                r[k + "_ms_spread"] = [float(np.min(times[k])), float(np.max(times[k]))]
+            if "baseline" in out and direction == "forward":
+                v64 = x.double().var(dim=(0, 2), unbiased=False)
+                for k in libs:
+                    r[k + "_var_max_rel_err"] = float(((out[k]["stats"][1].double() - v64).abs() / v64).max())
+            rows.append(r)
+            print(json.dumps(r), flush=True)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:
