@@ -439,6 +439,57 @@ int sonet_mesh_sample_f32(const double* verts, const int64_t* v_off, long long t
                           unsigned long long seed, void* scratch, long long scratch_bytes, float* out,
                           int32_t* face_out, double* area_out, sonet_stream_t stream);
 
+/* ---- point clouds without normals: exact k-NN within each cloud, and PCA surface normals ---------
+ * Input: data [T, stride] f32 point-major (xyz in columns 0..2, stride >= 3; a DeviceDataset's
+ * [T, 6] works in place), offsets [S+1] i64 (cloud s is rows offsets[s]..offsets[s+1]), all device
+ * pointers. Every offset is clamped into [0, T] and a decreasing pair is an empty cloud, so no
+ * offsets value reads or writes out of range; a cloud's results do not depend on the other clouds.
+ *
+ * sonet_point_knn_f32: idx [T, K] i32, the cloud-local indices of each point's K nearest points of
+ * its own cloud (the point itself included), dist [T, K] f32 (nullable) their distances
+ * d = ((dx*dx + dy*dy) + dz*dz), dx = q.x - p.x etc., fp32, explicitly rounded, no FMA (the SOM
+ * assignment's and sonet_node_knn's convention). Ascending distance, lowest index first on ties;
+ * a NaN distance ranks after every other, +inf included, again by index. Every index lies in
+ * [0, P); when P < K, slots P..K-1 hold -1 and dist +inf. Brute force over each cloud's P^2 pairs.
+ *
+ * sonet_point_normals_f32: from idx [T, K] (sonet_point_knn_f32's), per point: the neighbours with
+ * an index in [0, P) give a mean and a centred covariance (divided by their count) in fp64, two
+ * passes in slot order, explicitly rounded; the eigenvector of the smallest eigenvalue (cyclic
+ * Jacobi in fp64) normalised in fp64 and rounded to f32 once is the normal, written to
+ * normals + row * normal_stride (normal_stride >= 3, e.g. data + 3 with stride 6 for data[:, 3:6]);
+ * curvature [T] (nullable) = l0 / (l0 + l1 + l2), the surface variation. A neighbourhood with fewer
+ * than 3 neighbours, a non-finite neighbour coordinate, a covariance trace that is 0 or not finite,
+ * or collinear neighbours (l1 <= 2^-40 (l0 + l1 + l2)) gives the zero vector and NaN curvature.
+ * Sign: canonically, the component of largest magnitude of the f32 normal is positive (the first
+ * such component on ties); then, with ref per orientation code, the normal flips iff
+ * dot(n, ref) < 0, computed in fp64 ((nx*rx + ny*ry) + nz*rz); a dot of 0 or NaN keeps the
+ * canonical sign:
+ *   SONET_NORMALS_CANONICAL           no ref;
+ *   SONET_NORMALS_AWAY_FROM_CENTROID  ref = p - c, c the cloud's fp64 mean: with 256 lanes, lane t
+ *                                     sums rows t, t+256, .. in order from +0, then s[i] += s[i+h]
+ *                                     for h = 128, 64, .., 1, and c = s[0] / P;
+ *   SONET_NORMALS_TOWARD_VIEWPOINT    ref = view[s] - p, view [S, 3] f32 (one point per cloud).
+ * The centroid code takes sonet_point_normals_scratch_bytes(S) bytes of 256-byte aligned device
+ * scratch (nullable with the other codes).
+ *
+ * Both entries allocate nothing, do not synchronise, are deterministic and capturable in a CUDA
+ * graph. They fail with SONET_ERR_BAD_ARG before any CUDA call for S < 0, T < 0, stride < 3, K outside
+ * [3, SONET_POINT_KNN_MAX_K], a null offsets/idx (knn) or offsets/normals (normals), null data
+ * (and idx) with T > 0, an unknown orientation code, a null view with the viewpoint code,
+ * normal_stride < 3, or a missing, too small or misaligned scratch with the centroid code; S = 0
+ * then returns without a launch. The size query returns -1 for S < 0. */
+#define SONET_POINT_KNN_MAX_K 32
+#define SONET_NORMALS_CANONICAL 0
+#define SONET_NORMALS_AWAY_FROM_CENTROID 1
+#define SONET_NORMALS_TOWARD_VIEWPOINT 2
+int sonet_point_knn_f32(const float* data, long long T, int stride, const int64_t* offsets, int S,
+                        int K, int32_t* idx, float* dist, sonet_stream_t stream);
+long long sonet_point_normals_scratch_bytes(int S);
+int sonet_point_normals_f32(const float* data, long long T, int stride, const int64_t* offsets,
+                            int S, const int32_t* idx, int K, int orient, const float* view,
+                            void* scratch, long long scratch_bytes, float* normals,
+                            int normal_stride, float* curvature, sonet_stream_t stream);
+
 /* ---- a-4/a-5/a-8/a-9/a-10: point-wise shared MLP layer (1x1 conv + folded BN + ReLU) ---------
  * Replaces EquivariantLayer.forward / MyConv2d(1x1).forward in eval mode
  * (models/layers.py:203-210, 282-296): out[b,co,p] = act(scale[co]*sum_ci W[co,ci]*X[b,ci,p] +

@@ -264,6 +264,72 @@ def mesh_sample(verts, v_off, faces, f_off, mesh_ids, N, draws=None, seed=0, wan
     return out, face, area
 
 
+POINT_KNN_MAX_K = _C.CONSTANTS["SONET_POINT_KNN_MAX_K"]
+# sign rules of the estimated normals (SONET_NORMALS_*, include/sonet_b200.h)
+NORMALS_CANONICAL = _C.CONSTANTS["SONET_NORMALS_CANONICAL"]
+NORMALS_AWAY_FROM_CENTROID = _C.CONSTANTS["SONET_NORMALS_AWAY_FROM_CENTROID"]
+NORMALS_TOWARD_VIEWPOINT = _C.CONSTANTS["SONET_NORMALS_TOWARD_VIEWPOINT"]
+
+
+def _rows_arg(data, what):
+    """(T, stride) of a point-major [T, stride] f32 tensor whose rows may be longer than xyz."""
+    _chk(data, "data", torch.float32)
+    if data.dim() != 2 or data.shape[1] < 3:
+        raise RuntimeError("%s: expected data [T, >=3], got %s" % (what, tuple(data.shape)))
+    return data.shape[0], data.shape[1]
+
+
+def point_knn(data, offsets, K, want_dist=False):
+    """Exact K nearest neighbours of every point within its own cloud (csrc/point_normals.cu):
+    data [T, stride>=3] f32 (xyz in columns 0..2), offsets [S+1] i64. -> (idx [T, K] i32
+    cloud-local, dist [T, K] f32 or None); ascending distance, lowest index on ties, NaN last."""
+    T, stride = _rows_arg(data, "point_knn")
+    _chk(offsets, "offsets", torch.int64)
+    S = offsets.shape[0] - 1
+    dev = data.device
+    with torch.cuda.device(dev):
+        idx = torch.empty((T, int(K)), dtype=torch.int32, device=dev)
+        dist = torch.empty((T, int(K)), dtype=torch.float32, device=dev) if want_dist else None
+        _call("sonet_point_knn_f32", _C.ptr(data), T, stride, _C.ptr(offsets), S, int(K),
+              _C.ptr(idx), _C.ptr(dist), _stream(data), kernels=int(S > 0))
+    return idx, dist
+
+
+def estimate_normals(data, offsets, idx, orient, view=None, out=None, want_curvature=False):
+    """PCA normals of every point from its neighbours idx [T, K] i32 (point_knn's) with the sign
+    rule `orient` (NORMALS_*); view [S, 3] f32 for NORMALS_TOWARD_VIEWPOINT. out: [T, 3] f32 whose
+    rows may be strided (e.g. data[:, 3:6]), or None for a new tensor. -> (normals, curvature [T]
+    or None); a degenerate neighbourhood gives the zero vector and NaN curvature."""
+    T, stride = _rows_arg(data, "estimate_normals")
+    _chk(offsets, "offsets", torch.int64)
+    _chk(idx, "idx", torch.int32)
+    _chk(view, "view", torch.float32, optional=True)
+    S = offsets.shape[0] - 1
+    if idx.dim() != 2 or idx.shape[0] != T:
+        raise RuntimeError("estimate_normals: idx must be [%d, K], got %s" % (T, tuple(idx.shape)))
+    if view is not None and tuple(view.shape) != (S, 3):
+        raise RuntimeError("estimate_normals: view must be [%d, 3], got %s" % (S, tuple(view.shape)))
+    dev = data.device
+    if out is not None and (not out.is_cuda or out.dtype != torch.float32 or out.dim() != 2
+                            or tuple(out.shape) != (T, 3) or out.stride(1) != 1
+                            or (T > 1 and out.stride(0) < 3)):
+        raise RuntimeError("estimate_normals: out must be a CUDA f32 [T, 3] view with unit column "
+                           "stride, got %s with strides %s" % (tuple(out.shape), out.stride()))
+    with torch.cuda.device(dev):
+        normals = torch.empty((T, 3), dtype=torch.float32, device=dev) if out is None else out
+        curv = torch.empty((T,), dtype=torch.float32, device=dev) if want_curvature else None
+        scratch, nbytes = None, 0
+        if orient == NORMALS_AWAY_FROM_CENTROID:
+            nbytes = int(_C.lib().sonet_point_normals_scratch_bytes(S))
+            _C.check(0 if nbytes >= 0 else nbytes, "sonet_point_normals_scratch_bytes")
+            scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        _call("sonet_point_normals_f32", _C.ptr(data), T, stride, _C.ptr(offsets), S, _C.ptr(idx),
+              idx.shape[1], int(orient), _C.ptr(view), _C.ptr(scratch), nbytes, _C.ptr(normals),
+              max(normals.stride(0), 3), _C.ptr(curv), _stream(data),
+              kernels=(S > 0) * (1 + (orient == NORMALS_AWAY_FROM_CENTROID)))
+    return normals, curv
+
+
 def som_decenter(x, sn, cluster_mean, min_idx_i32, k, want_centers=False):
     """-> (x_aug [B,3(+3),kN], centers [B,3,kN] or None)."""
     _chk(x, "x", torch.float32)

@@ -4,8 +4,8 @@
 
 classifier (fused wgmma + pool at N=5000, graph replay), segmenter, auto-encoder (up-conv decoder,
 grouped / split-K GEMMs, Chamfer incl. the arg-min pass), BatchSOM training, augmentation,
-query_topk with the fused mask, standalone index_max, and one training step (BN / scatter / device
-pack kernels)."""
+query_topk with the fused mask, standalone index_max, per-cloud k-NN and normal estimation, and one
+training step (BN / scatter / device pack kernels)."""
 import os
 import sys
 
@@ -67,6 +67,11 @@ print("augment", float(out[0].sum()), int(out[3].sum()))
 data = torch.randn(2, 40, 1000, device=dev, generator=g)
 index = torch.randint(0, 64, (2, 1000), device=dev, generator=g, dtype=torch.int32)
 print("index_max", int(ops.index_max(data, index, 64).sum()))
+pts = torch.rand(1500, 6, device=dev, generator=g)
+offs = torch.tensor([0, 100, 100, 1500], dtype=torch.int64, device=dev)
+nb, _ = ops.point_knn(pts, offs, 16)
+nrm, _ = ops.estimate_normals(pts, offs, nb, ops.NORMALS_AWAY_FROM_CENTROID, out=pts[:, 3:6])
+print("normals", int(nb.sum()), float(nrm.sum()))
 m, a = build("classifier", 4, 256)
 m.set_input(*a)
 m.optimize()
