@@ -606,6 +606,53 @@ int sonet_seg_points_assign_f32(const float* points, long long total, const long
                                 long long row0, int rows, int rows_pad, int32_t* gidx, float* x_aug,
                                 float* pt, sonet_stream_t stream);
 
+/* ---- whole clouds of any size: the encoder's stage before the first per-node max, ragged ---------
+ * (networks.Encoder.forward_ragged, csrc/som_ragged.cu, INTEGRATION.md "Whole clouds of any size").
+ * points [T,6] f32 (xyz | normal), offsets [B+1] int64 (device): cloud b is rows offsets[b] ..
+ * offsets[b+1], P_b points. Its k stacked copies are the columns k*offsets[b] + s*P_b + n (copy s of
+ * point n, the reference's x_stack order at N = P_b), k*T columns in all. node [B,3,M] the loader's
+ * SOM nodes. Every offset is clamped to [0,T] and a decreasing pair is an empty cloud, so no input
+ * reads or writes out of range (the results of such offsets are unspecified; callers validate them).
+ * Limits: 1 <= M <= 256, 1 <= k <= min(4, M), k*T < 2^31, B*M < 2^31; no scratch.
+ *   assign: min_idx [k*T] i32 = the cloud-local node of every copy (sonet_som_assign's arithmetic
+ *     and tie rule against node[b]), count [B,M] i32, row_max [B,M] i32 = count > 0. Two memsets and
+ *     one launch, a thread per point.
+ *   group_decenter: CTA per cloud, any P_b (the stable sort runs through global memory), T < 2^24.
+ *     cluster_mean [B,3,M] = sum / (count + 1e-5), the sums in sonet_som_group_decenter's order (a
+ *     node's copies in ascending stacked order, lane l of a warp sums copies l, l+32, ... in groups of
+ *     four, xor butterfly 16..1), so a cloud gets that entry's bits at N = P_b; x_sorted [3|6, k*T]
+ *     (row stride k*T) the decentred copies (| normals, with_sn = 1) grouped by (cloud, node),
+ *     ascending stacked order inside a node, cloud b's block at its own columns; node_sorted [k*T]
+ *     i32 = b*M + m; pos0 [B] i32 = the sorted column of cloud b's copy 0.
+ *   decenter: x_aug [3|6, k*T] = the decentred copies in stacked order (the unfused route).
+ *   sonet_pointresnet_tc_pool_ragged_forward: sonet_pointresnet_tc_pool_forward_act over x_sorted
+ *     [Cin, P] as ONE batch row (P = k*T) with node_sorted's flat ids (grouped, each < B*M): the max of
+ *     every (cloud, channel, node) goes to pool_keys [B,384,M] (sonet_pool_keys_init's value on
+ *     entry), the features of the row pos0[b] to p0 [b,384]; act = SONET_ACT_RELU or _ELU, f16 != 0
+ *     the one-product mode. sonet_pool_finalize / sonet_knn_assemble_pool_f32 read the keys as usual.
+ *   sonet_index_max_ragged_f32: data [C, ld] (ld >= k*T) in stacked column order, index the
+ *     min_idx above -> out_idx [B,C,M] i32 (cloud-local stacked column, the lowest on ties) and
+ *     out_val [B,C,M] f32 (nullable): index_max's semantics per cloud at N = k*P_b (max > -1000,
+ *     else column 0 and the value of the cloud's copy 0; NaN never a maximum). C <= 65535*16.
+ * All deterministic; no allocation, no host synchronisation. */
+int sonet_som_assign_ragged_f32(const float* points, long long T, const long long* offsets, int B,
+                                const float* node, int M, int k, int32_t* min_idx, int32_t* count,
+                                int32_t* row_max, sonet_stream_t stream);
+int sonet_som_group_decenter_ragged_f32(const float* points, long long T, const long long* offsets,
+                                        int B, int M, int k, int with_sn, const int32_t* min_idx,
+                                        float* cluster_mean, float* x_sorted, int32_t* node_sorted,
+                                        int32_t* pos0, sonet_stream_t stream);
+int sonet_som_decenter_ragged_f32(const float* points, long long T, const long long* offsets, int B,
+                                  int M, int k, int with_sn, const int32_t* min_idx,
+                                  const float* cluster_mean, float* x_aug, sonet_stream_t stream);
+int sonet_pointresnet_tc_pool_ragged_forward(const float* x_sorted, int Cin, int P, const void* blob,
+                                             const float* fparams, const int32_t* node_sorted,
+                                             const int32_t* pos0, int B, int M, int act, int f16,
+                                             int32_t* pool_keys, float* p0, sonet_stream_t stream);
+int sonet_index_max_ragged_f32(const float* data, int C, long long ld, const int32_t* index,
+                               const long long* offsets, int B, long long T, int M, int k,
+                               int32_t* out_idx, float* out_val, sonet_stream_t stream);
+
 /* SHREC'16 same-label retrieval ranking (shrec16/test.py:64-99). feature [Q,D] f32; label_in [Q]
  * int64, or NULL for the row argmax (lowest index on ties, first NaN wins). For each query q, the
  * items p with label p == label q (q included) ranked by d = float(sqrt(sum_j double(f_q[j] -

@@ -378,3 +378,88 @@ extern "C" int sonet_index_max_cpu_f32(const float* data, const int32_t* index, 
   for (auto& th : pool) th.join();
   return SONET_OK;
 }
+
+// ---- ragged clouds (networks.Encoder.forward_ragged's unfused route) ------------------------------
+// data [C, ld] holds the stacked copies of a ragged batch side by side: cloud b's k*P_b copies are the
+// columns k*offsets[b] .. k*offsets[b+1], in stacked order; index the cloud-local node of every column.
+// Per (cloud, channel, node): the first column (cloud-local, ascending) that attains the maximum if it
+// is > -1000, else column 0 and the value of the cloud's copy 0 — index_max's semantics at N = k*P_b,
+// so the values are the fused ragged pool's (csrc/pointmlp_tc.cu, RAGGED) bit for bit. A CTA owns one
+// cloud and IMR_G channels: a pass of shared-memory atomicMax over order-preserving keys finds each
+// node's maximum, a second pass of atomicMin the lowest column that holds it (+0 and -0 compare equal,
+// as under '>'); NaN and values <= -1000 never enter. Offsets are clamped to [0, T] (a decreasing
+// pair is an empty cloud) and node ids to [0, M-1], so nothing reads or writes out of range.
+namespace sonet {
+
+constexpr int IMR_G = 16, IMR_THREADS = 512;
+
+__device__ __forceinline__ int imr_key(float v) {
+  const int bits = __float_as_int(v == 0.f ? 0.f : v);
+  return bits ^ ((bits >> 31) & 0x7fffffff);
+}
+
+__global__ void __launch_bounds__(IMR_THREADS)
+    index_max_ragged_kernel(const float* __restrict__ data, int C, long long ld,
+                            const int32_t* __restrict__ index, const long long* __restrict__ offsets,
+                            long long T, int M, int k, int32_t* __restrict__ out_idx,
+                            float* __restrict__ out_val) {
+  __shared__ int skey[IMR_G * 256];
+  __shared__ int sidx[IMR_G * 256];
+  const int b = blockIdx.x, c0 = blockIdx.y * IMR_G, nc = min(IMR_G, C - c0);
+  const long long lo = min(max(__ldg(offsets + b), 0LL), T);
+  const long long hi = max(min(max(__ldg(offsets + b + 1), 0LL), T), lo);
+  const long long base = k * lo;
+  const int kP = static_cast<int>(k * (hi - lo));
+  const float* db = data + static_cast<size_t>(c0) * ld + base;
+  const int32_t* ib = index + base;
+  const unsigned mmax = static_cast<unsigned>(M - 1);
+  for (int e = threadIdx.x; e < IMR_G * M; e += IMR_THREADS) {
+    skey[e] = POOL_KEY_INIT;
+    sidx[e] = 0x7fffffff;
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < kP; j += IMR_THREADS) {
+    const int m = min(static_cast<unsigned>(__ldg(ib + j)), mmax);
+    for (int g = 0; g < nc; ++g) {
+      const float v = __ldg(db + g * ld + j);
+      if (v > IM_SENTINEL) atomicMax(&skey[g * M + m], imr_key(v));
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < kP; j += IMR_THREADS) {
+    const int m = min(static_cast<unsigned>(__ldg(ib + j)), mmax);
+    for (int g = 0; g < nc; ++g) {
+      const float v = __ldg(db + g * ld + j);
+      if (v > IM_SENTINEL && imr_key(v) == skey[g * M + m]) atomicMin(&sidx[g * M + m], j);
+    }
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < nc * M; e += IMR_THREADS) {
+    const int g = e / M, m = e - g * M;
+    const int i = sidx[g * M + m];
+    const bool hit = i != 0x7fffffff;
+    const size_t o = (static_cast<size_t>(b) * C + c0 + g) * M + m;
+    out_idx[o] = hit ? i : 0;
+    if (out_val) out_val[o] = (hit || kP > 0) ? db[g * ld + (hit ? i : 0)] : 0.f;
+  }
+}
+
+}  // namespace sonet
+
+extern "C" int sonet_index_max_ragged_f32(const float* data, int C, long long ld, const int32_t* index,
+                                          const long long* offsets, int B, long long T, int M, int k,
+                                          int32_t* out_idx, float* out_val, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE(B >= 0 && C >= 0 && T >= 0 && k >= 1 && k <= 4,
+                "index_max_ragged: bad dimension (B=%d, C=%d, T=%lld, k=%d)", B, C, T, k);
+  SONET_REQUIRE(M >= 1 && M <= 256, "index_max_ragged: M=%d out of range [1,256]", M);
+  SONET_REQUIRE(ld >= k * T && k * T < (1LL << 31),
+                "index_max_ragged: row stride %lld below the k*T=%lld columns (or too many)", ld, k * T);
+  SONET_REQUIRE((C + IMR_G - 1) / IMR_G <= 65535, "index_max_ragged: C=%d too large", C);
+  if (B == 0 || C == 0) return SONET_OK;
+  SONET_REQUIRE(offsets && out_idx && (T == 0 || (data && index)), "index_max_ragged: null pointer");
+  dim3 grid(B, (C + IMR_G - 1) / IMR_G);
+  index_max_ragged_kernel<<<grid, IMR_THREADS, 0, as_stream(stream)>>>(data, C, ld, index, offsets, T, M,
+                                                                      k, out_idx, out_val);
+  return check_launch("index_max_ragged");
+}

@@ -110,6 +110,9 @@ static_assert(W1_BYTES == SLOT_BYTES && L2_STAGE_BYTES == SLOT_BYTES && 2 * L3_H
 // inside a node is whatever som_sort left). A NaN row never becomes a node's maximum, as in
 // index_max: fmaxf drops it next to any other row, and a run of NaN rows only is keyed as -inf.
 // Required: node_sorted[b,j] < M (a negative id skips the row), 0 <= pos0[b] < P.
+// RAGGED (sonet_pointresnet_tc_pool_ragged_forward): one batch row of P sorted copies of several
+// clouds; node_sorted holds flat ids b*M + m (< B*M), grouped by them, a row is copy 0 of cloud b
+// when it is row pos0[b], and its keys and p0 go to cloud b's [384,M] and [384] slices.
 struct PoolArgs {
   const int32_t* node_sorted;  // [B,P] node id of each sorted row
   const int32_t* pos0;         // [B] sorted row of stacked copy 0
@@ -124,7 +127,7 @@ struct PoolArgs {
 // ACT: the activation of layers 0-2, SONET_ACT_RELU or SONET_ACT_ELU. Nothing downstream assumes
 // it is non-negative: the hi/lo split of an ELU output in [-1, inf) saturates exactly as a ReLU
 // output's does, and the pool, its -1000 sentinel and its keys act on the bare layer 3.
-template <bool POOL, bool DBG, int NPROD, int ACT>
+template <bool POOL, bool DBG, int NPROD, int ACT, bool RAGGED = false>
 __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
     pointresnet_tc_kernel(const float* __restrict__ x_in, int Cin, int B, int P,
                           const unsigned char* __restrict__ blob, const float* __restrict__ fparams,
@@ -284,8 +287,13 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
         const int p0row = __ldg(pool.pos0 + b);
         if (valid0) nd[0] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0);
         if (valid1) nd[1] = __ldg(pool.node_sorted + static_cast<size_t>(b) * P + jbase + r0 + 8);
-        is_p0[0] = valid0 && jbase + r0 == p0row;
-        is_p0[1] = valid1 && jbase + r0 + 8 == p0row;
+        if (RAGGED) {
+          is_p0[0] = valid0 && nd[0] >= 0 && jbase + r0 == __ldg(pool.pos0 + nd[0] / pool.M);
+          is_p0[1] = valid1 && nd[1] >= 0 && jbase + r0 + 8 == __ldg(pool.pos0 + nd[1] / pool.M);
+        } else {
+          is_p0[0] = valid0 && jbase + r0 == p0row;
+          is_p0[1] = valid1 && jbase + r0 + 8 == p0row;
+        }
       }
 
       // ---- layer 1: D1[64 x 128] = act0[64 x 64] * W1^T, A from shared memory ----
@@ -437,7 +445,8 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
             for (int c = 0; c < 4; ++c)
               r3[c] = fmaxf(b0 ? r2[c + 4] : r2[c], __shfl_xor_sync(FULL, b0 ? r2[c] : r2[c + 4], 4));
             const int col = cbase + 8 * ((16 * b2 + 8 * b1 + 4 * b0) >> 1);   // slot base's column
-            int32_t* kb = pool.keys + (static_cast<size_t>(b) * C3 + col) * pool.M + node;
+            const int kcloud = RAGGED ? node / pool.M : b, knode = RAGGED ? node - kcloud * pool.M : node;
+            int32_t* kb = pool.keys + (static_cast<size_t>(kcloud) * C3 + col) * pool.M + knode;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const int dc = 8 * (i >> 1) + (i & 1);
@@ -451,11 +460,12 @@ __global__ void __launch_bounds__(pm::NUM_THREADS, 1)
 #pragma unroll
           for (int rr = 0; rr < 2; ++rr) {
             if (!is_p0[rr]) continue;   // rare: one row per cloud
+            const int pcloud = RAGGED ? nd[rr] / pool.M : b;
 #pragma unroll
             for (int jn = 0; jn < 16; ++jn)
 #pragma unroll
               for (int e = 0; e < 2; ++e)
-                pool.p0[static_cast<size_t>(b) * C3 + cbase + 8 * jn + e] =
+                pool.p0[static_cast<size_t>(pcloud) * C3 + cbase + 8 * jn + e] =
                     fmaf(acc[4 * jn + 2 * rr + e], inv3, sh3[cbase + 8 * jn + e]);
           }
         }
@@ -524,7 +534,7 @@ extern "C" int sonet_pointresnet_tc_pack(const float* W0, int Cin, const float* 
 static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const void* blob,
                                  const float* fparams, float* out, long long* dbg,
                                  const sonet::PoolArgs* pool, sonet_stream_t stream, bool f16 = false,
-                                 int act = SONET_ACT_RELU) {
+                                 int act = SONET_ACT_RELU, bool ragged = false) {
   using namespace sonet;
   using namespace sonet::pm;
   SONET_REQUIRE(act == SONET_ACT_RELU || act == SONET_ACT_ELU,
@@ -545,7 +555,9 @@ static int launch_pointresnet_tc(const float* x, int Cin, int B, int P, const vo
   SONET_REQUIRE(!(act != SONET_ACT_RELU && dbg), "pointresnet_tc: the debug timeline has no ELU build");
   constexpr int R = SONET_ACT_RELU, E = SONET_ACT_ELU;
   auto kern =
-      act == E ? (f16 ? (pool ? pointresnet_tc_kernel<true, false, 1, E> : pointresnet_tc_kernel<false, false, 1, E>)
+      ragged ? (act == E ? (f16 ? pointresnet_tc_kernel<true, false, 1, E, true> : pointresnet_tc_kernel<true, false, 3, E, true>)
+                         : (f16 ? pointresnet_tc_kernel<true, false, 1, R, true> : pointresnet_tc_kernel<true, false, 3, R, true>))
+      : act == E ? (f16 ? (pool ? pointresnet_tc_kernel<true, false, 1, E> : pointresnet_tc_kernel<false, false, 1, E>)
                       : (pool ? pointresnet_tc_kernel<true, false, 3, E> : pointresnet_tc_kernel<false, false, 3, E>))
       : f16 ? (pool ? pointresnet_tc_kernel<true, false, 1, R> : pointresnet_tc_kernel<false, false, 1, R>)
       : pool ? (dbg ? pointresnet_tc_kernel<true, true, 3, R> : pointresnet_tc_kernel<true, false, 3, R>)
@@ -603,6 +615,20 @@ extern "C" int sonet_pointresnet_tc_pool_forward_act(const float* x_sorted, int 
   sonet::PoolArgs pa{node_sorted, pos0, pool_keys, p0, M};
   return launch_pointresnet_tc(x_sorted, Cin, B, P, blob, fparams, nullptr, nullptr, &pa, stream, f16 != 0,
                                act);
+}
+
+// the pool over the sorted copies of a ragged batch laid out as one row (PoolArgs, RAGGED)
+extern "C" int sonet_pointresnet_tc_pool_ragged_forward(const float* x_sorted, int Cin, int P,
+                                                        const void* blob, const float* fparams,
+                                                        const int32_t* node_sorted, const int32_t* pos0,
+                                                        int B, int M, int act, int f16,
+                                                        int32_t* pool_keys, float* p0,
+                                                        sonet_stream_t stream) {
+  SONET_REQUIRE(B >= 1 && M >= 1 && M <= 256 && static_cast<long long>(B) * M < (1LL << 31),
+                "pointresnet_tc_pool_ragged: bad dimension (B=%d, M=%d)", B, M);
+  sonet::PoolArgs pa{node_sorted, pos0, pool_keys, p0, M};
+  return launch_pointresnet_tc(x_sorted, Cin, 1, P, blob, fparams, nullptr, nullptr, &pa, stream, f16 != 0,
+                               act, true);
 }
 
 extern "C" int sonet_debug_pointresnet_tc_pool_timeline(const float* x_sorted, int Cin, int B, int P,

@@ -233,6 +233,18 @@ class DeviceDataset:
         seg = None if self.seg is None else self.seg[rows].long()
         return self.data[rows], offsets, seg
 
+    def full_batch(self, index, opt):
+        """(points [sum P_i, 6] f32, offsets [len(index)+1] int64, label [len(index)] int64,
+        som_node [len(index),3,M] f32, som_knn_I [len(index),M,som_k] int64) of the clouds `index`:
+        every point of each (full_clouds), with the test-mode loader's SOM nodes and their kNN and
+        no augmentation — the input of classifier.Model.score_clouds and
+        networks.Encoder.forward_ragged."""
+        points, offsets, _ = self.full_clouds(index)
+        cid = torch.from_numpy(np.asarray(index, dtype=np.int64).reshape(-1)).to(self.device)
+        som = self.som_nodes.index_select(0, cid)
+        return (points, offsets, self.labels.index_select(0, cid), som,
+                som_knn(som, opt.som_k, self.node_num))
+
     def batch(self, index, opt, train, rng=None, seed=0, host_noise=False, shard=None):
         """The collated batch of the loader `opt.dataset` selects (autoencoder/train.py:25-36) for
         the clouds `index`, ready for Model.set_input(*...):

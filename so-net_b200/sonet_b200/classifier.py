@@ -8,7 +8,7 @@ CUDA graph (enable_cuda_graph, enable_train_graph) — see _model_base.GraphedMo
 import torch
 import torch.nn as nn
 
-from . import networks
+from . import augmentation, networks
 from ._model_base import ENCODER_SNAPSHOT, GraphedModel
 
 
@@ -67,6 +67,26 @@ class Model(GraphedModel):
         with torch.no_grad():
             self.forward(is_train=False)
             self.loss = self.softmax_criteria(self.score, self.label)
+
+    def score_clouds(self, points, offsets, node, node_knn_I=None, chunk_points=None):
+        """Class scores [B, classes] of whole clouds of any size, from all of their points, in eval
+        mode: points [T,6] f32, offsets [B+1] int64, node [B,3,M] (the test-mode loader's SOM nodes,
+        DeviceDataset.full_batch), node_knn_I [B,M,som_k] int64 or None to compute it with
+        augmentation.som_knn. Encoder.forward_ragged, then the classifier head (dropout is the
+        identity in eval mode). Reads no bound input and writes no attribute of the model: score,
+        the encoder's state and a captured eval graph stay as test_model() left them. Refused before
+        any launch: train mode and Encoder.check_ragged's cases."""
+        enc, head, opt = self.encoder, self.classifier, self.opt
+        if enc.training or head.training:
+            raise RuntimeError("score_clouds: the model is in train mode; call test_model() or "
+                               "eval() first")
+        enc.check_ragged(points, offsets, node, node_knn_I, chunk_points, what="score_clouds")
+        with torch.no_grad():
+            if node_knn_I is None:
+                node_knn_I = augmentation.som_knn(node.detach().contiguous(), opt.som_k,
+                                                  node.shape[2])
+            feature = enc.forward_ragged(points, offsets, node, node_knn_I, chunk_points)
+            return head.fc3(head.fc2(head.fc1(feature)))
 
     def _make_optimizers(self):
         return (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr,

@@ -13,6 +13,7 @@ remain available as lazily materialised attributes for callers that read them
 """
 import math
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -93,6 +94,7 @@ class Encoder(nn.Module):
         self.fuse_pool = True
         self._fpo_demand = False     # set once a caller has read first_pn_out lazily (see below)
         self._pool_keys = ops.PoolKeys()
+        self._ragged_keys = ops.PoolKeys()   # forward_ragged's own: the graphed forward's stay put
 
     # ---- lazily materialised public attributes (API of models/networks.py:127, 169) -----------
     @property
@@ -238,6 +240,146 @@ class Encoder(nn.Module):
         else:
             self.feature, _ = torch.max(self.final_pn_out, dim=2, keepdim=False)
         return self.feature
+
+    # ---- whole clouds of any size ------------------------------------------------------------
+    # device bytes per stacked copy of a point in one chunk: the decentred copy, its node ids and
+    # the unfused route's four layer outputs
+    _RAGGED_COPY_BYTES = 4 * (6 + 2 + 64 + 128 + 256 + 384)
+    # som_group_decenter_ragged packs a chunk's point index into 24 bits
+    _RAGGED_MAX_POINTS = (1 << 24) - 1
+
+    def check_ragged(self, points, offsets, node, node_knn_I=None, chunk_points=None,
+                     what="forward_ragged"):
+        """The refusals of forward_ragged (RuntimeError; ValueError for an empty cloud), raised
+        before any launch. Returns the offsets as a host numpy array."""
+        opt = self.opt
+        if self.training:
+            raise RuntimeError("%s: the encoder is in train mode; call eval() first" % what)
+        if opt.normalization == 'instance':
+            raise RuntimeError("%s: --normalization instance has no ragged per-cloud statistics"
+                               % what)
+        if not all(l._fast_eligible() for l in self.first_pointnet.layers):
+            raise RuntimeError("%s: activation %r / normalization %r have no kernels"
+                               % (what, opt.activation, opt.normalization))
+        dev = self.first_pointnet.layers[0].conv.weight.device
+        if not (1 <= opt.k <= 4):
+            raise RuntimeError("%s: k=%d outside [1, 4]" % (what, opt.k))
+        for name, t, dt, dim in (("points", points, torch.float32, 2), ("node", node, torch.float32, 3),
+                                 ("offsets", offsets, torch.int64, 1),
+                                 ("node_knn_I", node_knn_I, torch.int64, 3)):
+            if t is None and name == "node_knn_I":
+                continue
+            if not isinstance(t, torch.Tensor) or t.dtype != dt or t.dim() != dim:
+                raise RuntimeError("%s: %s must be a %d-D %s tensor (got %s)" % (
+                    what, name, dim, dt, (t.dtype, tuple(t.shape)) if isinstance(t, torch.Tensor)
+                    else type(t).__name__))
+            if t.device != dev:
+                raise RuntimeError("%s: %s must be on the model's device %s (got %s)"
+                                   % (what, name, dev, t.device))
+        if points.shape[1] != 6:
+            raise RuntimeError("%s: points must be [T, 6] (got %s)" % (what, tuple(points.shape)))
+        B, M = node.shape[0], node.shape[2]
+        if node.shape[1] != 3 or B < 1:
+            raise RuntimeError("%s: node must be [B, 3, M] (got %s)" % (what, tuple(node.shape)))
+        if not (opt.k <= M <= 256):
+            raise RuntimeError("%s: M=%d nodes outside [k=%d, 256]" % (what, M, opt.k))
+        if node_knn_I is not None and (node_knn_I.shape[:2] != (B, M)
+                                       or node_knn_I.shape[2] < max(opt.som_k, 1)):
+            raise RuntimeError("%s: node_knn_I must be [%d, %d, >=%d] (got %s)"
+                               % (what, B, M, max(opt.som_k, 1), tuple(node_knn_I.shape)))
+        if chunk_points is not None and int(chunk_points) < 1:
+            raise RuntimeError("%s: chunk_points must be >= 1 (got %s)" % (what, chunk_points))
+        off = ops.ragged_offsets(offsets, points.shape[0], B)
+        counts = np.diff(off)
+        if (counts == 0).any():
+            raise ValueError("%s: cloud %d has no points" % (what, int(np.flatnonzero(counts == 0)[0])))
+        if counts.max() > self._RAGGED_MAX_POINTS:
+            raise RuntimeError("%s: cloud %d has %d points, more than %d"
+                               % (what, int(counts.argmax()), int(counts.max()),
+                                  self._RAGGED_MAX_POINTS))
+        return off
+
+    def forward_ragged(self, points, offsets, node, node_knn_I, chunk_points=None,
+                       return_nodes=False):
+        """The global feature of every cloud of a ragged batch from ALL of its points, in eval mode.
+
+        points [T,6] f32 on the model's device (xyz | normal, DeviceDataset.data's layout; the
+        normals are ignored unless surface_normal), offsets [B+1] int64 (cloud b is rows
+        offsets[b] .. offsets[b+1], P_b points), node [B,3,M] the loader's SOM nodes, node_knn_I
+        [B,M,som_k] int64. Returns feature [B,feature_num]; with return_nodes also a dict of
+        som_node, first_pn_out_masked_max, knn_center_1, knn_feature_1 (None when som_k < 2) and
+        final_pn_out, each [B,.,M].
+
+        Cloud b is the dense forward at N = P_b: its k stacked copies in the reference's x_stack
+        order, assigned with sonet_som_assign's arithmetic, cluster means summed in the group
+        route's order, the first PointResNet and index_max's per-node max (> -1000, else the cloud's
+        copy 0). From the pooled features on, the node-level stage runs on [B,.,M] as in forward().
+        Routes: the first PointResNet's from the batch's k*T columns, the node-level stage's from
+        its B*M rows. A cloud's results depend only on its own points and nodes and those routes:
+        permuting the clouds permutes the outputs bit for bit, and chunk_points (default: from the
+        free device memory) changes no bit, since chunks are whole clouds.
+
+        The encoder attributes of the last forward() (som_node, feature, ...) are left untouched.
+        Refused before any launch: check_ragged."""
+        off = self.check_ragged(points, offsets, node, node_knn_I, chunk_points)
+        opt, fpn = self.opt, self.first_pointnet
+        k, M, T = opt.k, node.shape[2], points.shape[0]
+        use_sn = opt.surface_normal == True  # noqa: E712
+        fused = fpn._tc_eligible(6 if use_sn else 3, None)
+        if chunk_points:
+            chunk = int(chunk_points)
+        else:
+            free, _ = torch.cuda.mem_get_info(points.device)
+            chunk = (free // 4) // (k * self._RAGGED_COPY_BYTES)
+        chunk = max(1, min(chunk, self._RAGGED_MAX_POINTS))
+        with torch.no_grad():
+            points = points.contiguous()
+            node = node.detach().contiguous()
+            cms, mms = [], []
+            for b0, b1 in _ragged_chunks(off, chunk):
+                o0 = int(off[b0])
+                pts = points[o0:int(off[b1])]
+                offc = (offsets[b0:b1 + 1] - o0).contiguous()
+                idx, _, _ = ops.som_assign_ragged(pts, offc, node[b0:b1], k)
+                xs, ns, p0s, cm = ops.som_group_decenter_ragged(pts, offc, idx, M, k, use_sn)
+                if fused:
+                    blob, fpar = fpn._tc_params()
+                    pooled = ops.pointresnet_tc_pool_ragged(xs, blob, fpar, ns, p0s, M,
+                                                            owner=self._ragged_keys, f16=tc_f16(),
+                                                            act=fpn.layers[0].activation)
+                    mm = ops.pool_finalize(*pooled, owner=self._ragged_keys)
+                else:
+                    x_aug = ops.som_decenter_ragged(pts, offc, idx, cm, k, use_sn)
+                    fpo = fpn(x_aug, route_rows=k * T)
+                    _, mm = ops.index_max_ragged(fpo[0], idx, offc, M, k)
+                cms.append(cm)
+                mms.append(mm)
+            som_node = cms[0] if len(cms) == 1 else torch.cat(cms)
+            masked_max = mms[0] if len(mms) == 1 else torch.cat(mms)
+            center = knn_feature = None
+            if opt.som_k >= 2:
+                center, knn_feature = self.knnlayer(som_node, masked_max, node_knn_I, opt.som_k,
+                                                    opt.som_k_type)
+                final = self.final_pointnet.forward_pair(center, knn_feature)
+            else:
+                final = self.final_pointnet(som_node, x1=masked_max)
+            feature = ops.rowmax(final)
+        if not return_nodes:
+            return feature
+        return feature, dict(som_node=som_node, first_pn_out_masked_max=masked_max,
+                             knn_center_1=center, knn_feature_1=knn_feature, final_pn_out=final)
+
+
+def _ragged_chunks(off, chunk):
+    """(b0, b1) runs of whole clouds of the host offsets `off` with at most `chunk` points each;
+    a larger cloud is a run of its own."""
+    B, b0 = len(off) - 1, 0
+    while b0 < B:
+        b1 = b0 + 1
+        while b1 < B and off[b1 + 1] - off[b0] <= chunk:
+            b1 += 1
+        yield b0, b1
+        b0 = b1
 
 
 class Classifier(nn.Module):

@@ -663,6 +663,112 @@ def seg_points_assign(points, offsets, node, cluster_mean, k, with_sn, row0, row
     return gidx, x_aug, pt
 
 
+def _ragged_args(points, offsets, what):
+    _chk(points, "points", torch.float32)
+    _chk(offsets, "offsets", torch.int64)
+    if points.dim() != 2 or points.shape[1] != 6 or offsets.dim() != 1 or offsets.numel() < 2:
+        raise RuntimeError("%s: expected points [T,6] and offsets [B+1], got %s and %s"
+                           % (what, tuple(points.shape), tuple(offsets.shape)))
+    return points.shape[0], offsets.numel() - 1
+
+
+def som_assign_ragged(points, offsets, node, k):
+    """Ragged clouds (points [T,6], offsets [B+1] checked by the caller) against their loader nodes
+    node [B,3,M] -> (min_idx [k*T] i32 cloud-local node of every stacked copy, count [B,M] i32,
+    row_max [B,M] i32) (csrc/som_ragged.cu)."""
+    T, B = _ragged_args(points, offsets, "som_assign_ragged")
+    _chk(node, "node", torch.float32)
+    if node.dim() != 3 or node.shape[0] != B or node.shape[1] != 3:
+        raise RuntimeError("som_assign_ragged: node must be [%d,3,M] (got %s)" % (B, tuple(node.shape)))
+    M = node.shape[2]
+    dev = points.device
+    with torch.cuda.device(dev):
+        idx = torch.empty((k * T,), dtype=torch.int32, device=dev)
+        count = torch.empty((B, M), dtype=torch.int32, device=dev)
+        row_max = torch.empty((B, M), dtype=torch.int32, device=dev)
+        _call("sonet_som_assign_ragged_f32", _C.ptr(points), T, _C.ptr(offsets), B, _C.ptr(node),
+              int(M), int(k), _C.ptr(idx), _C.ptr(count), _C.ptr(row_max), _stream(points),
+              kernels=1 if T else 0)
+    return idx, count, row_max
+
+
+def som_group_decenter_ragged(points, offsets, min_idx, M, k, with_sn):
+    """Cluster statistics + stable (cloud, node) sort + decentring of ragged clouds, one launch ->
+    (x_sorted [3(+3),k*T], node_sorted [k*T] i32 flat ids b*M+m, pos0 [B] i32, cluster_mean [B,3,M])."""
+    T, B = _ragged_args(points, offsets, "som_group_decenter_ragged")
+    _chk(min_idx, "min_idx", torch.int32)
+    dev = points.device
+    with torch.cuda.device(dev):
+        xs = torch.empty((6 if with_sn else 3, k * T), dtype=torch.float32, device=dev)
+        ns = torch.empty((k * T,), dtype=torch.int32, device=dev)
+        p0 = torch.empty((B,), dtype=torch.int32, device=dev)
+        cmean = torch.empty((B, 3, M), dtype=torch.float32, device=dev)
+        _call("sonet_som_group_decenter_ragged_f32", _C.ptr(points), T, _C.ptr(offsets), B, int(M),
+              int(k), int(bool(with_sn)), _C.ptr(min_idx), _C.ptr(cmean), _C.ptr(xs), _C.ptr(ns),
+              _C.ptr(p0), _stream(points))
+    return xs, ns, p0, cmean
+
+
+def som_decenter_ragged(points, offsets, min_idx, cluster_mean, k, with_sn):
+    """The decentred stacked copies of ragged clouds in stacked order -> x_aug [1,3(+3),k*T]."""
+    T, B = _ragged_args(points, offsets, "som_decenter_ragged")
+    _chk(min_idx, "min_idx", torch.int32)
+    _chk(cluster_mean, "cluster_mean", torch.float32)
+    M = cluster_mean.shape[2]
+    dev = points.device
+    with torch.cuda.device(dev):
+        x_aug = torch.empty((1, 6 if with_sn else 3, k * T), dtype=torch.float32, device=dev)
+        _call("sonet_som_decenter_ragged_f32", _C.ptr(points), T, _C.ptr(offsets), B, int(M), int(k),
+              int(bool(with_sn)), _C.ptr(min_idx), _C.ptr(cluster_mean), _C.ptr(x_aug),
+              _stream(points))
+    return x_aug
+
+
+def pointresnet_tc_pool_ragged(x_sorted, blob, fparams, node_sorted, pos0, M, owner=None, f16=False,
+                               act=ACT_RELU):
+    """pointresnet_tc_pool(finalize=False) over the sorted copies of a ragged batch, x_sorted
+    [Cin,P] with flat node ids node_sorted [P] (som_group_decenter_ragged's) -> (keys [B,384,M] i32,
+    p0 [B,384]) for pool_finalize / knn_assemble_pool."""
+    act = act_code(act)
+    _chk(x_sorted, "x_sorted", torch.float32)
+    _chk(blob, "blob", torch.uint8)
+    _chk(fparams, "fparams", torch.float32)
+    _chk(node_sorted, "node_sorted", torch.int32)
+    _chk(pos0, "pos0", torch.int32)
+    Cin, P = x_sorted.shape
+    B = pos0.shape[0]
+    dev = x_sorted.device
+    with torch.cuda.device(dev):
+        keys = (owner or _DEFAULT_POOL_KEYS).acquire(dev, B, M, _stream(x_sorted))
+        p0 = torch.empty((B, 384), dtype=torch.float32, device=dev)
+        _call("sonet_pointresnet_tc_pool_ragged_forward", _C.ptr(x_sorted), Cin, P, _C.ptr(blob),
+              _C.ptr(fparams), _C.ptr(node_sorted), _C.ptr(pos0), B, int(M), act, int(bool(f16)),
+              _C.ptr(keys), _C.ptr(p0), _stream(x_sorted))
+    return keys, p0
+
+
+def index_max_ragged(data, index, offsets, M, k):
+    """index_max per cloud of a ragged batch: data [C,k*T] f32 in stacked column order, index [k*T]
+    i32 cloud-local node ids, offsets [B+1] -> (out_idx [B,C,M] i32 cloud-local stacked column,
+    out_val [B,C,M] f32)."""
+    _chk(data, "data", torch.float32)
+    _chk(index, "index", torch.int32)
+    _chk(offsets, "offsets", torch.int64)
+    if data.dim() != 2 or index.dim() != 1 or index.shape[0] != data.shape[1] \
+            or index.shape[0] % k != 0 or offsets.dim() != 1 or offsets.numel() < 2:
+        raise RuntimeError("index_max_ragged: expected data [C,k*T], index [k*T], offsets [B+1], got "
+                           "%s, %s, %s" % (tuple(data.shape), tuple(index.shape), tuple(offsets.shape)))
+    C, cols = data.shape
+    B = offsets.numel() - 1
+    dev = data.device
+    with torch.cuda.device(dev):
+        out_idx = torch.empty((B, C, M), dtype=torch.int32, device=dev)
+        out_val = torch.empty((B, C, M), dtype=torch.float32, device=dev)
+        _call("sonet_index_max_ragged_f32", _C.ptr(data), C, cols, _C.ptr(index), _C.ptr(offsets), B,
+              cols // k, int(M), int(k), _C.ptr(out_idx), _C.ptr(out_val), _stream(data))
+    return out_idx, out_val
+
+
 RETRIEVAL_MAX_D = 1024
 RETRIEVAL_MAX_K = 4096
 RETRIEVAL_MAX_L = 4096

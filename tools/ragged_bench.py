@@ -1,0 +1,144 @@
+"""Whole clouds of any size: classifier.Model.score_clouds (networks.Encoder.forward_ragged) against
+the dense test_model() on the same clouds, and a batch of clouds of mixed sizes.
+
+    python tools/ragged_bench.py [--reps 20] [--out results.json]
+
+  A  64 clouds x 10,000 points as one ragged batch, against dense test_model() at N = 10,000 and
+     N = 5,000 on the same clouds (eager and with the eval CUDA graph).
+  B  1,024 clouds with P uniform in [2,000, 10,000]: clouds/s and points/s, and the time split
+     between assignment + sort, the first PointResNet + pool and the node-level stage (a separate
+     run with per-call CUDA events, ops.PROFILE).
+
+Times are medians of --reps warm calls, each bracketed by CUDA events. Synthetic clouds and weights
+(synth.py), the default classifier options (k = 3, 8x8 SOM, som_k = 9); SONET_TC as set.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "so-net_b200")]
+
+from sonet_b200 import augmentation, classifier, networks, ops, synth  # noqa: E402
+
+DEV = torch.device("cuda:0")
+
+
+def median_ms(fn, reps, warm=3):
+    for _ in range(warm):
+        fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        fn()
+        e1.record()
+        e1.synchronize()
+        ts.append(e0.elapsed_time(e1))
+    return float(np.median(ts)), float(np.min(ts)), float(np.max(ts))
+
+
+def model(B, N, states, graph=False):
+    opt = synth.make_opt("classifier", batch_size=B, input_pc_num=N, device=DEV)
+    m = classifier.Model(opt)
+    m.encoder.load_state_dict(states[0])
+    m.classifier.load_state_dict(states[1])
+    m.encoder.eval()
+    m.classifier.eval()
+    m.enable_cuda_graph(graph)
+    return m
+
+
+def clouds(sizes, M, seed):
+    rs = np.random.RandomState(seed)
+    pts, nodes = [], []
+    for P in sizes:
+        xyz = rs.uniform(-1, 1, size=(P, 3)).astype(np.float32)
+        n = rs.normal(size=(P, 3)).astype(np.float32)
+        n /= np.linalg.norm(n, axis=1, keepdims=True)
+        pts.append(np.concatenate([xyz, n], axis=1))
+        nodes.append(xyz[rs.choice(P, M, replace=False)].T)
+    off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    return (torch.from_numpy(np.concatenate(pts)).to(DEV), torch.from_numpy(off).to(DEV),
+            torch.from_numpy(np.ascontiguousarray(np.stack(nodes))).to(DEV))
+
+
+def stage_split(m, pts, off, node, knn):
+    """Per-stage device time of one score_clouds call from per-call CUDA events."""
+    ops.PROFILE = []
+    m.score_clouds(pts, off, node, knn)
+    torch.cuda.synchronize()
+    split = {"assign_sort": 0.0, "first_pointresnet_pool": 0.0, "node_level": 0.0}
+    for name, e0, e1, _ in ops.PROFILE:
+        ms = e0.elapsed_time(e1)
+        if "ragged" in name and "pointresnet" not in name:
+            split["assign_sort"] += ms
+        elif "pointresnet_tc_pool_ragged" in name or name == "sonet_pool_finalize":
+            split["first_pointresnet_pool"] += ms
+        else:
+            split["node_level"] += ms
+    ops.PROFILE = None
+    return split
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("ragged_bench: needs a CUDA device")
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm",
+                          "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    cpu_opt = synth.make_opt("classifier")
+    states = (synth.synth_state_dict(networks.Encoder(cpu_opt), seed=1),
+              synth.synth_state_dict(networks.Classifier(cpu_opt), seed=2))
+    res = dict(gpu=gpu, sonet_tc=os.environ.get("SONET_TC", "1"), reps=a.reps)
+
+    # ---- A: 64 x 10,000 ragged against dense N = 10,000 and N = 5,000 ----
+    B, P, M = 64, 10000, 64
+    pts, off, node = clouds([P] * B, M, seed=0)
+    knn = augmentation.som_knn(node, 9, M)
+    m = model(B, P, states)
+    res["A_ragged_64x10000_ms"] = median_ms(lambda: m.score_clouds(pts, off, node, knn), a.reps)
+    for N in (10000, 5000):
+        pc = pts.view(B, P, 6)[:, :N, :3].permute(0, 2, 1).contiguous().cpu()
+        sn = pts.view(B, P, 6)[:, :N, 3:].permute(0, 2, 1).contiguous().cpu()
+        for graph in (False, True):
+            md = model(B, N, states, graph)
+
+            def dense():
+                md.set_input(pc, sn, torch.zeros(B, dtype=torch.int64), node.cpu(), knn.cpu())
+                md.test_model()
+            # set_input's host-to-device copy is part of the dense call, as in bench.py
+            res["A_dense_N%d_%s_ms" % (N, "graph" if graph else "eager")] = median_ms(dense, a.reps)
+            del md
+    del m
+    torch.cuda.empty_cache()
+
+    # ---- B: 1,024 clouds of 2,000 - 10,000 points ----
+    rs = np.random.RandomState(5)
+    sizes = rs.randint(2000, 10001, size=1024)
+    pts, off, node = clouds(sizes, M, seed=1)
+    knn = augmentation.som_knn(node, 9, M)
+    m = model(1, 256, states)
+    t = median_ms(lambda: m.score_clouds(pts, off, node, knn), a.reps)
+    res["B_mixed_1024_ms"] = t
+    res["B_points"] = int(sizes.sum())
+    res["B_clouds_per_s"] = 1024 / (t[0] * 1e-3)
+    res["B_points_per_s"] = float(sizes.sum()) / (t[0] * 1e-3)
+    res["B_split_ms"] = stage_split(m, pts, off, node, knn)
+    print(json.dumps(res, indent=1))
+    if a.out:
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
