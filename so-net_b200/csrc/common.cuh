@@ -88,14 +88,54 @@ __device__ __forceinline__ float2 sqsum3_rn(float2 dx, float2 dy, float2 dz) {
   return make_float2(__fadd_rn(__fadd_rn(xx.x, yy.x), zz.x), __fadd_rn(__fadd_rn(xx.y, yy.y), zz.y));
 }
 
-// ---- register top-k of the SOM assignment ---------------------------------------------------------
-// The arg-min kernels (som.cu, seg_points.cu) insert every distance below the last slot's, starting
-// from slots (+inf, -1): a finite distance always enters, +inf and NaN never do. A point with fewer
-// than KK nodes at a finite distance (a coordinate whose square overflows for some nodes, or a point
-// that is not finite) leaves slots at -1. This fills them with the nodes at +inf, then the NaN
-// ones, each in ascending index order, so that the KK nodes stay distinct and keep the order
-// (distance, index) with NaN last: a NaN point gets nodes 0..KK-1. dist(m) must give the insertion
-// loop's value for node m. Run only when bi[KK-1] < 0, which a finite point with KK finite
+// ---- the SOM assignment: each point's KK nearest nodes in registers -------------------------------
+// The one rule of every kernel that assigns points to SOM nodes (som.cu, som_ragged.cu,
+// seg_points.cu), which is why their indices agree bit for bit. The distance is ((dx*dx + dy*dy) +
+// dz*dz) rounded op by op, no FMA (som_dist_rn; som.cu's packed pairs round each half the same way).
+// The slots start at (+inf, -1) and take the nodes in ascending index order; a distance enters only
+// when it is strictly below the last slot's, so on an exact tie the lower node index stays ahead,
+// and a finite distance always enters while +inf and NaN never do. Slots still empty after the last
+// node are filled by topk_fill_nonfinite.
+
+// p + (-n) == p - n bit for bit: the arithmetic of som_assign_kernel's negated packed nodes.
+__device__ __forceinline__ float som_dist_rn(float px, float py, float pz, float nx, float ny, float nz) {
+  const float dx = __fadd_rn(px, -nx), dy = __fadd_rn(py, -ny), dz = __fadd_rn(pz, -nz);
+  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+
+template <int KK>
+__device__ __forceinline__ void topk_reset(float (&bd)[KK], int (&bi)[KK]) {
+#pragma unroll
+  for (int s = 0; s < KK; ++s) {
+    bd[s] = __int_as_float(0x7f800000);  // +inf
+    bi[s] = -1;                          // empty (topk_fill_nonfinite)
+  }
+}
+
+template <int KK>
+__device__ __forceinline__ void topk_insert(float (&bd)[KK], int (&bi)[KK], float d, int m) {
+  if (d < bd[KK - 1]) {  // strict: on exact ties the earlier (lower) node index stays
+    bd[KK - 1] = d;
+    bi[KK - 1] = m;
+#pragma unroll
+    for (int s = KK - 1; s > 0; --s) {
+      if (bd[s] < bd[s - 1]) {
+        const float td = bd[s];
+        bd[s] = bd[s - 1];
+        bd[s - 1] = td;
+        const int ti = bi[s];
+        bi[s] = bi[s - 1];
+        bi[s - 1] = ti;
+      }
+    }
+  }
+}
+
+// A point with fewer than KK nodes at a finite distance (a coordinate whose square overflows for
+// some nodes, or a point that is not finite) leaves slots at -1. This fills them with the nodes at
+// +inf, then the NaN ones, each in ascending index order, so that the KK nodes stay distinct and keep
+// the order (distance, index) with NaN last: a NaN point gets nodes 0..KK-1. dist(m) must give the
+// insertion loop's value for node m. Run only when bi[KK-1] < 0, which a finite point with KK finite
 // distances never reaches.
 template <int KK, typename Dist>
 __device__ __forceinline__ void topk_fill_nonfinite(float (&bd)[KK], int (&bi)[KK], int M, Dist dist) {
@@ -116,6 +156,50 @@ __device__ __forceinline__ void topk_fill_nonfinite(float (&bd)[KK], int (&bi)[K
       }
     }
   }
+}
+
+// The KK nearest of M nodes, dist(m) the distance of node m (som_dist_rn).
+template <int KK, typename Dist>
+__device__ __forceinline__ void som_topk(int M, Dist dist, float (&bd)[KK], int (&bi)[KK]) {
+  topk_reset(bd, bi);
+  for (int m = 0; m < M; ++m) topk_insert(bd, bi, dist(m), m);
+  if (bi[KK - 1] < 0) topk_fill_nonfinite(bd, bi, M, dist);
+}
+
+// ---- ragged clouds ----------------------------------------------------------------------------------
+// Cloud b of a ragged batch of T rows is rows offsets[b] .. offsets[b+1]. Every offset is clamped
+// into [0, T] and a decreasing pair is an empty cloud, so that no offsets array makes a kernel read
+// or write out of range.
+template <typename Off>
+__device__ __forceinline__ long long ragged_offset(const Off* offsets, int b, long long T) {
+  const long long o = __ldg(offsets + b);
+  return o < 0 ? 0 : (o > T ? T : o);
+}
+
+// rows [lo, hi) of cloud b, hi >= lo
+template <typename Off>
+__device__ __forceinline__ void ragged_range(const Off* offsets, int b, long long T, long long& lo,
+                                             long long& hi) {
+  lo = ragged_offset(offsets, b, T);
+  const long long e = __ldg(offsets + b + 1);
+  hi = e < lo ? lo : (e > T ? T : e);
+}
+
+// The cloud of row g: the last b in [0, B) whose clamped offset is <= g (0 when there is none), and
+// its rows [lo, hi); g lies in no cloud unless lo <= g < hi. For a row g in [0, T), a clamped offset
+// is <= g exactly when the raw one is, so the search picks the cloud an unclamped search over the
+// raw offsets would, for any offsets array.
+template <typename Off>
+__device__ __forceinline__ int ragged_find(const Off* offsets, int B, long long T, long long g,
+                                           long long& lo, long long& hi) {
+  int a = 0, z = B - 1;
+  while (a < z) {
+    const int mid = (a + z + 1) >> 1;
+    if (ragged_offset(offsets, mid, T) <= g) a = mid;
+    else z = mid - 1;
+  }
+  ragged_range(offsets, a, T, lo, hi);
+  return a;
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

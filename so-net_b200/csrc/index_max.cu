@@ -387,8 +387,8 @@ extern "C" int sonet_index_max_cpu_f32(const float* data, const int32_t* index, 
 // so the values are the fused ragged pool's (csrc/pointmlp_tc.cu, RAGGED) bit for bit. A CTA owns one
 // cloud and IMR_G channels: a pass of shared-memory atomicMax over order-preserving keys finds each
 // node's maximum, a second pass of atomicMin the lowest column that holds it (+0 and -0 compare equal,
-// as under '>'); NaN and values <= -1000 never enter. Offsets are clamped to [0, T] (a decreasing
-// pair is an empty cloud) and node ids to [0, M-1], so nothing reads or writes out of range.
+// as under '>'); NaN and values <= -1000 never enter. Offsets are clamped as common.cuh's ragged_range
+// states and node ids to [0, M-1], so nothing reads or writes out of range.
 namespace sonet {
 
 constexpr int IMR_G = 16, IMR_THREADS = 512;
@@ -406,8 +406,8 @@ __global__ void __launch_bounds__(IMR_THREADS)
   __shared__ int skey[IMR_G * 256];
   __shared__ int sidx[IMR_G * 256];
   const int b = blockIdx.x, c0 = blockIdx.y * IMR_G, nc = min(IMR_G, C - c0);
-  const long long lo = min(max(__ldg(offsets + b), 0LL), T);
-  const long long hi = max(min(max(__ldg(offsets + b + 1), 0LL), T), lo);
+  long long lo, hi;
+  ragged_range(offsets, b, T, lo, hi);
   const long long base = k * lo;
   const int kP = static_cast<int>(k * (hi - lo));
   const float* db = data + static_cast<size_t>(c0) * ld + base;

@@ -2,7 +2,7 @@
 // normals estimated from them (sm_90a): the normals SO-Net reads, for point clouds that have none.
 //
 // Layout (include/sonet_b200.h): data [T, stride] f32 point-major with xyz in columns 0..2; cloud s
-// is rows offsets[s] .. offsets[s+1], clamped into [0, T] (a decreasing pair is an empty cloud).
+// is rows offsets[s] .. offsets[s+1], clamped as common.cuh's ragged_range states.
 //
 // k-NN: d = ((dx*dx + dy*dy) + dz*dz), dx = q.x - p.x, every operation explicitly rounded (no FMA
 // contraction), the convention of the SOM assignment and sonet_node_knn. Each thread owns one query
@@ -29,15 +29,13 @@ constexpr long long PK_MAX_CLOUD = 2147483647LL;  // cloud-local indices are int
 constexpr int PN_THREADS = 128;
 constexpr int PC_THREADS = 256;                 // centroid: one CTA per cloud, fixed reduction tree
 
-// A cloud's [begin, end) rows, clamped into [0, T]; the count is 0 for a reversed range and at most
-// 2^31-1 (the rest of a longer range is not part of the cloud).
+// A cloud's first row and row count (common.cuh's ragged_range); the count is at most 2^31-1 (the
+// rest of a longer range is not part of the cloud).
 __device__ __forceinline__ void pk_range(const int64_t* off, int s, long long T, long long& begin,
                                          int& count) {
-  long long lo = off[s], hi = off[s + 1];
-  lo = lo < 0 ? 0 : (lo > T ? T : lo);
-  hi = hi < lo ? lo : (hi > T ? T : hi);
-  begin = lo;
-  count = static_cast<int>(hi - lo > PK_MAX_CLOUD ? PK_MAX_CLOUD : hi - lo);
+  long long end;
+  ragged_range(off, s, T, begin, end);
+  count = static_cast<int>(end - begin > PK_MAX_CLOUD ? PK_MAX_CLOUD : end - begin);
 }
 
 __device__ __forceinline__ float pk_dist(float qx, float qy, float qz, float px, float py, float pz) {

@@ -9,16 +9,15 @@
 //   x_aug[c][s*rows_pad + r]   = x_c - cm[b,c,m_s] (c < 3), then the normal     (the first PointResNet's input)
 //   pt[c][s*rows_pad + r]      = x_dec | x | cm[b,:,m_s] | normal               (layer 1's per-point rows)
 //
-// m_s is the s-th nearest of cloud b's M loader nodes with sonet_som_assign's arithmetic: distances
-// ((dx*dx + dy*dy) + dz*dz) rounded op by op with dx = x - node (add2_rn / mul2_rn in som.cu: the same
-// bits), register top-k insertion, the lowest node index on ties, k distinct nodes even when fewer
-// than k distances are finite (common.cuh, topk_fill_nonfinite). cm is the cluster mean the encoder
-// computed on the sampled batch (Encoder.som_node). Columns of rows r >= rows are padding: zeros and
-// node 0 of cloud 0, so that whatever reads them stays finite and in range.
+// m_s is the s-th nearest of cloud b's M loader nodes by the SOM assignment rule of common.cuh
+// (som_topk: sonet_som_assign's bits). cm is the cluster mean the encoder computed on the sampled
+// batch (Encoder.som_node). Columns of rows r >= rows are padding: zeros and node 0 of cloud 0, so
+// that whatever reads them stays finite and in range.
 //
-// Each row finds its cloud by a binary search over offsets on the device: one launch per chunk, no
-// host round trip per cloud. offsets are not read on the host; a row outside [offsets[0], offsets[B])
-// of non-monotone offsets lands in cloud 0 or B-1 (the Python caller validates offsets once).
+// Each row finds its cloud by a binary search over offsets on the device (common.cuh, ragged_find):
+// one launch per chunk, no host round trip per cloud. offsets are not read on the host; a row outside
+// [offsets[0], offsets[B]) of non-monotone offsets lands in cloud 0 or B-1 (the Python caller
+// validates offsets once).
 #include <algorithm>
 
 #include "common.cuh"
@@ -31,8 +30,8 @@ constexpr int SEGPT_THREADS = 256;
 
 template <int KK>
 __global__ void __launch_bounds__(SEGPT_THREADS)
-    seg_points_assign_kernel(const float* __restrict__ points, const long long* __restrict__ offsets,
-                             int B, const float* __restrict__ node,
+    seg_points_assign_kernel(const float* __restrict__ points, long long total,
+                             const long long* __restrict__ offsets, int B, const float* __restrict__ node,
                              const float* __restrict__ cluster_mean, int M, int with_sn,
                              long long row0, int rows, int rows_pad, int32_t* __restrict__ gidx,
                              float* __restrict__ x_aug, float* __restrict__ pt) {
@@ -51,50 +50,16 @@ __global__ void __launch_bounds__(SEGPT_THREADS)
     return;
   }
   const long long g = row0 + r;
-  // the cloud of row g: the last b with offsets[b] <= g
-  int lo = 0, hi = B - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (__ldg(offsets + mid) <= g) lo = mid;
-    else hi = mid - 1;
-  }
-  const int b = lo;
+  long long lo, hi;   // the cloud's rows: unused, a row outside it still takes the cloud found
+  const int b = ragged_find(offsets, B, total, g, lo, hi);
   const float* p = points + static_cast<size_t>(g) * 6;
   const float px = p[0], py = p[1], pz = p[2];
   const float* nb = node + static_cast<size_t>(b) * 3 * M;
-
   float bd[KK];
   int bi[KK];
-#pragma unroll
-  for (int s = 0; s < KK; ++s) {
-    bd[s] = __int_as_float(0x7f800000);  // +inf
-    bi[s] = -1;                          // empty (topk_fill_nonfinite)
-  }
-  // p + (-n) == p - n bit for bit: the arithmetic of som_assign_kernel's negated packed nodes
-  auto dist = [&](int m) {
-    const float dx = __fadd_rn(px, -__ldg(nb + m)), dy = __fadd_rn(py, -__ldg(nb + M + m)),
-                dz = __fadd_rn(pz, -__ldg(nb + 2 * M + m));
-    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-  };
-  for (int m = 0; m < M; ++m) {
-    const float d = dist(m);
-    if (d < bd[KK - 1]) {  // strict: on exact ties the earlier (lower) node index stays
-      bd[KK - 1] = d;
-      bi[KK - 1] = m;
-#pragma unroll
-      for (int s = KK - 1; s > 0; --s) {
-        if (bd[s] < bd[s - 1]) {
-          const float td = bd[s];
-          bd[s] = bd[s - 1];
-          bd[s - 1] = td;
-          const int ti = bi[s];
-          bi[s] = bi[s - 1];
-          bi[s - 1] = ti;
-        }
-      }
-    }
-  }
-  if (bi[KK - 1] < 0) topk_fill_nonfinite(bd, bi, M, dist);
+  som_topk(M, [&](int m) {
+    return som_dist_rn(px, py, pz, __ldg(nb + m), __ldg(nb + M + m), __ldg(nb + 2 * M + m));
+  }, bd, bi);
 
   const float* cm = cluster_mean + static_cast<size_t>(b) * 3 * M;
   const float xv[3] = {px, py, pz};
@@ -146,10 +111,10 @@ extern "C" int sonet_seg_points_assign_f32(const float* points, long long total,
   const int grid = (rows_pad + SEGPT_THREADS - 1) / SEGPT_THREADS;
   cudaStream_t st = as_stream(stream);
   switch (k) {
-    case 1: seg_points_assign_kernel<1><<<grid, SEGPT_THREADS, 0, st>>>(points, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
-    case 2: seg_points_assign_kernel<2><<<grid, SEGPT_THREADS, 0, st>>>(points, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
-    case 3: seg_points_assign_kernel<3><<<grid, SEGPT_THREADS, 0, st>>>(points, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
-    default: seg_points_assign_kernel<4><<<grid, SEGPT_THREADS, 0, st>>>(points, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
+    case 1: seg_points_assign_kernel<1><<<grid, SEGPT_THREADS, 0, st>>>(points, total, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
+    case 2: seg_points_assign_kernel<2><<<grid, SEGPT_THREADS, 0, st>>>(points, total, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
+    case 3: seg_points_assign_kernel<3><<<grid, SEGPT_THREADS, 0, st>>>(points, total, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
+    default: seg_points_assign_kernel<4><<<grid, SEGPT_THREADS, 0, st>>>(points, total, offsets, B, node, cluster_mean, M, with_sn, row0, rows, rows_pad, gidx, x_aug, pt); break;
   }
   return check_launch("seg_points_assign");
 }

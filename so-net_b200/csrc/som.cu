@@ -6,10 +6,8 @@
 // (~2 GB at B=64,N=5000); here the assignment is 12 B in + 4k B out per point and the cluster
 // statistics are reduced straight from the indices.
 //
-//  som_assign_kernel   thread per point: 64 nodes in smem (broadcast reads), distances in the
-//                      reference's exact rounding order ((dx*dx+dy*dy)+dz*dz, no FMA), register
-//                      top-k insertion (ascending distance, lowest node index on ties; k distinct
-//                      nodes even when fewer than k distances are finite: topk_fill_nonfinite).
+//  som_assign_kernel   thread per point: the nodes in smem (broadcast reads), two distances per step
+//                      from packed pairs, the SOM assignment rule of common.cuh (som_topk).
 //  som_stats_kernel    CTA per (cloud, node): counts and coordinate sums in a fixed order
 //                      (strided per-thread partials + fixed tree) -> bit-reproducible and
 //                      independent of batch sharding; cluster_mean = sum / (count + 1e-5f).
@@ -52,42 +50,21 @@ __global__ void __launch_bounds__(256)
   const float px = xb[nl], py = xb[N + nl], pz = xb[2 * N + nl];
   const float2 px2 = make_float2(px, px), py2 = make_float2(py, py), pz2 = make_float2(pz, pz);
 
+  // som_topk's rule (common.cuh), with the distances of two nodes per step
   float bd[KK];
   int bi[KK];
-#pragma unroll
-  for (int s = 0; s < KK; ++s) {
-    bd[s] = __int_as_float(0x7f800000);  // +inf
-    bi[s] = -1;                          // empty (topk_fill_nonfinite)
-  }
-  auto consider = [&](float d, int m) {
-    if (d < bd[KK - 1]) {  // strict: on exact ties the earlier (lower) node index stays
-      bd[KK - 1] = d;
-      bi[KK - 1] = m;
-#pragma unroll
-      for (int s = KK - 1; s > 0; --s) {
-        if (bd[s] < bd[s - 1]) {
-          const float td = bd[s];
-          bd[s] = bd[s - 1];
-          bd[s - 1] = td;
-          const int ti = bi[s];
-          bi[s] = bi[s - 1];
-          bi[s - 1] = ti;
-        }
-      }
-    }
-  };
+  topk_reset(bd, bi);
 #pragma unroll 2
   for (int m2 = 0; m2 < MP; ++m2) {
     const float2 d = sqsum3_rn(add2_rn(px2, snx[m2]), add2_rn(py2, sny[m2]), add2_rn(pz2, snz[m2]));
-    consider(d.x, 2 * m2);
-    if (2 * m2 + 1 < M) consider(d.y, 2 * m2 + 1);
+    topk_insert(bd, bi, d.x, 2 * m2);
+    if (2 * m2 + 1 < M) topk_insert(bd, bi, d.y, 2 * m2 + 1);
   }
   if (bi[KK - 1] < 0) {
     topk_fill_nonfinite(bd, bi, M, [&](int m) {
       const float2 nx = snx[m >> 1], ny = sny[m >> 1], nz = snz[m >> 1];
-      const float dx = __fadd_rn(px, (m & 1) ? nx.y : nx.x), dy = __fadd_rn(py, (m & 1) ? ny.y : ny.x),
-                  dz = __fadd_rn(pz, (m & 1) ? nz.y : nz.x);
-      return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+      return som_dist_rn(px, py, pz, -((m & 1) ? nx.y : nx.x), -((m & 1) ? ny.y : ny.x),
+                         -((m & 1) ? nz.y : nz.x));
     });
   }
   if (mask != nullptr) {

@@ -7,10 +7,9 @@
 // cloud's block where the dense [B,k*N] layout would put it at N = P_b.
 //
 //   som_assign_ragged_kernel        thread per point: its cloud by binary search over offsets, then the
-//                                   k nearest of the cloud's M nodes with sonet_som_assign's arithmetic
-//                                   ((dx*dx + dy*dy) + dz*dz rounded op by op, no FMA) and tie rule
-//                                   (ascending distance, then lowest index; topk_fill_nonfinite).
-//                                   count [B,M] by integer atomics, row_max [B,M] = count > 0.
+//                                   k nearest of the cloud's M nodes by the SOM assignment rule of
+//                                   common.cuh (som_topk, sonet_som_assign's bits). count [B,M] by
+//                                   integer atomics, row_max [B,M] = count > 0.
 //   som_group_ragged_kernel         CTA per cloud, any size: stable counting sort of the cloud's copies
 //                                   by node through global memory (warp-private histograms over
 //                                   warp-contiguous ranges, ballot ranks), then per-node sums in
@@ -22,8 +21,8 @@
 //                                   N = P_b, also for clouds too large for that kernel's shared memory.
 //   som_decenter_ragged_kernel      the decentred copies in stacked order (the unfused route's input).
 //
-// Every offset is clamped to [0, T] and a decreasing pair is an empty cloud, so that no input reads or
-// writes out of range; the Python caller refuses such offsets before any launch.
+// Offsets are clamped as common.cuh's ragged_range states, so that no input reads or writes out of
+// range; the Python caller refuses such offsets before any launch.
 #include <algorithm>
 
 #include "common.cuh"
@@ -35,30 +34,6 @@ constexpr int RAG_MAX_K = 4;
 constexpr int RAG_THREADS = 256;
 constexpr int RGROUP_THREADS = 1024, RGROUP_WARPS = RGROUP_THREADS / 32;
 
-__device__ __forceinline__ long long rag_off(const long long* offsets, int b, long long T) {
-  return min(max(__ldg(offsets + b), 0LL), T);
-}
-
-// rows [lo, hi) of cloud b, hi >= lo
-__device__ __forceinline__ void rag_cloud(const long long* offsets, int b, long long T, long long& lo,
-                                          long long& hi) {
-  lo = rag_off(offsets, b, T);
-  hi = max(rag_off(offsets, b + 1, T), lo);
-}
-
-// the cloud of row g: the last b with offsets[b] <= g (-1 when g lies in no cloud)
-__device__ __forceinline__ int rag_find(const long long* offsets, int B, long long T, long long g,
-                                        long long& lo, long long& hi) {
-  int a = 0, z = B - 1;
-  while (a < z) {
-    const int mid = (a + z + 1) >> 1;
-    if (rag_off(offsets, mid, T) <= g) a = mid;
-    else z = mid - 1;
-  }
-  rag_cloud(offsets, a, T, lo, hi);
-  return (g >= lo && g < hi) ? a : -1;
-}
-
 template <int KK>
 __global__ void __launch_bounds__(RAG_THREADS)
     som_assign_ragged_kernel(const float* __restrict__ points, long long T,
@@ -68,8 +43,8 @@ __global__ void __launch_bounds__(RAG_THREADS)
   const long long g = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (g >= T) return;
   long long lo, hi;
-  const int b = rag_find(offsets, B, T, g, lo, hi);
-  if (b < 0) return;
+  const int b = ragged_find(offsets, B, T, g, lo, hi);
+  if (g < lo || g >= hi) return;
   const long long P = hi - lo, n = g - lo;
   const float* p = points + static_cast<size_t>(g) * 6;
   const float px = p[0], py = p[1], pz = p[2];
@@ -77,36 +52,9 @@ __global__ void __launch_bounds__(RAG_THREADS)
 
   float bd[KK];
   int bi[KK];
-#pragma unroll
-  for (int s = 0; s < KK; ++s) {
-    bd[s] = __int_as_float(0x7f800000);  // +inf
-    bi[s] = -1;                          // empty (topk_fill_nonfinite)
-  }
-  // p + (-n) == p - n bit for bit: the arithmetic of som_assign_kernel's negated packed nodes
-  auto dist = [&](int m) {
-    const float dx = __fadd_rn(px, -__ldg(nb + m)), dy = __fadd_rn(py, -__ldg(nb + M + m)),
-                dz = __fadd_rn(pz, -__ldg(nb + 2 * M + m));
-    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-  };
-  for (int m = 0; m < M; ++m) {
-    const float d = dist(m);
-    if (d < bd[KK - 1]) {  // strict: on exact ties the earlier (lower) node index stays
-      bd[KK - 1] = d;
-      bi[KK - 1] = m;
-#pragma unroll
-      for (int s = KK - 1; s > 0; --s) {
-        if (bd[s] < bd[s - 1]) {
-          const float td = bd[s];
-          bd[s] = bd[s - 1];
-          bd[s - 1] = td;
-          const int ti = bi[s];
-          bi[s] = bi[s - 1];
-          bi[s - 1] = ti;
-        }
-      }
-    }
-  }
-  if (bi[KK - 1] < 0) topk_fill_nonfinite(bd, bi, M, dist);
+  som_topk(M, [&](int m) {
+    return som_dist_rn(px, py, pz, __ldg(nb + m), __ldg(nb + M + m), __ldg(nb + 2 * M + m));
+  }, bd, bi);
   int32_t* ob = min_idx + KK * lo + n;
 #pragma unroll
   for (int s = 0; s < KK; ++s) {
@@ -128,7 +76,7 @@ __global__ void __launch_bounds__(RGROUP_THREADS)
   const int b = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   long long lo, hi;
-  rag_cloud(offsets, b, T, lo, hi);
+  ragged_range(offsets, b, T, lo, hi);
   const int P = static_cast<int>(hi - lo), kP = k * P;
   const long long base = k * lo;                   // the cloud's first column
   const int32_t* ib = min_idx + base;
@@ -263,8 +211,8 @@ __global__ void __launch_bounds__(RAG_THREADS)
   const long long g = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (g >= T) return;
   long long lo, hi;
-  const int b = rag_find(offsets, B, T, g, lo, hi);
-  if (b < 0) return;
+  const int b = ragged_find(offsets, B, T, g, lo, hi);
+  if (g < lo || g >= hi) return;
   const long long P = hi - lo;
   const float* p = points + static_cast<size_t>(g) * 6;
   const float* cmb = cluster_mean + static_cast<size_t>(b) * 3 * M;

@@ -3,22 +3,19 @@
 bit, runnable without a GPU."""
 import numpy as np
 
+from test_seg_full_envelope_host import topk_ref
+
 
 def assign(points, offsets, node, k):
     """points [T,6] f32, offsets [B+1], node [B,3,M] f32 -> (min_idx [k*T] i32 cloud-local, stacked
-    column k*offsets[b] + s*P_b + n; count [B,M] i32). Distances ((dx*dx + dy*dy) + dz*dz) in fp32,
-    rounded op by op; ascending distance, then lowest index (finite points)."""
+    column k*offsets[b] + s*P_b + n; count [B,M] i32). Each point's k nodes are topk_ref's."""
     B, _, M = node.shape
     T = points.shape[0]
     idx = np.empty(k * T, dtype=np.int32)
     count = np.zeros((B, M), dtype=np.int32)
     for b in range(B):
         lo, hi = int(offsets[b]), int(offsets[b + 1])
-        P = hi - lo
-        p = points[lo:hi, :3].astype(np.float32)
-        parts = [(p[:, c:c + 1] + (-node[b, c][None, :])).astype(np.float32) for c in range(3)]
-        d = (parts[0] * parts[0] + parts[1] * parts[1]).astype(np.float32) + parts[2] * parts[2]
-        top = np.argsort(d, axis=1, kind="stable")[:, :k]          # [P, k]
+        top = topk_ref(points[lo:hi, :3].astype(np.float32), node[b], k)   # [P, k]
         idx[k * lo:k * hi] = top.T.reshape(-1)
         np.add.at(count[b], top.reshape(-1), 1)
     return idx, count
