@@ -22,7 +22,11 @@
 //   som_decenter_ragged_kernel      the decentred copies in stacked order (the unfused route's input).
 //
 // Offsets are clamped as common.cuh's ragged_range states, so that no input reads or writes out of
-// range; the Python caller refuses such offsets before any launch.
+// range; the Python caller refuses such offsets before any launch. Offsets that decrease can leave
+// two clouds' clamped ranges overlapping: their CTAs in som_group_ragged_kernel then share columns of
+// node_sorted, which holds each CTA's packed sort entries, and one CTA can read the other's entries
+// or flat ids there. Every entry is read back clamped to the CTA's own points and nodes, so such
+// columns hold unspecified values but no access leaves the cloud's rows.
 #include <algorithm>
 
 #include "common.cuh"
@@ -156,7 +160,7 @@ __global__ void __launch_bounds__(RGROUP_THREADS)
       for (int u = 0; u < 4; ++u) {
         const int q = p + 32 * u;
         const bool ok = q < e;
-        const int n = ok ? static_cast<int>(perm[q] & 0xffffffu) : 0;
+        const int n = ok ? min(static_cast<int>(perm[q] & 0xffffffu), P - 1) : 0;
         ax[u] = ok ? pb[static_cast<size_t>(n) * 6] : 0.f;
         ay[u] = ok ? pb[static_cast<size_t>(n) * 6 + 1] : 0.f;
         az[u] = ok ? pb[static_cast<size_t>(n) * 6 + 2] : 0.f;
@@ -193,7 +197,7 @@ __global__ void __launch_bounds__(RGROUP_THREADS)
   int32_t* nb = node_sorted + base;
   for (int p = threadIdx.x; p < kP; p += RGROUP_THREADS) {
     const uint32_t e = perm[p];
-    const int n = e & 0xffffffu, nd = e >> 24;
+    const int n = min(static_cast<int>(e & 0xffffffu), P - 1), nd = min(static_cast<int>(e >> 24), M - 1);
     const float* src = pb + static_cast<size_t>(n) * 6;
 #pragma unroll
     for (int c = 0; c < 3; ++c) ob[c * ld + p] = __fsub_rn(src[c], cm[c * M + nd]);
