@@ -699,6 +699,25 @@ long long sonet_retrieval_format_cpu(const long long* ids, const long long* idx,
 int sonet_chamfer_f32(const float* pred, const float* gt, int B, int Mp, int N, int32_t* idx_fwd,
                       int32_t* idx_bwd, float* elem_fwd, float* elem_bwd, float* loss_fwd_arr,
                       float* loss_bwd_arr, float* loss, sonet_stream_t stream);
+/* The same against whole ground-truth clouds of any size (losses.chamfer_ragged, INTEGRATION.md
+ * "Whole clouds: the auto-encoder"): pred [B,3,Mp]; points [T,ld] f32 rows (xyz first, ld >= 3;
+ * DeviceDataset's [T,6]), cloud b is rows offsets[b] .. offsets[b+1] (P_b points; offsets [B+1]
+ * int64 on the device, offsets_host the same values in host memory). Outputs as sonet_chamfer_f32
+ * with the gt side ragged: idx_fwd [B,Mp] (cloud-local rows) and idx_bwd [T] (nullable, together),
+ * elem_fwd [B,Mp], elem_bwd [T], loss_fwd_arr / loss_bwd_arr [B], loss [3]. Cloud b's entries are
+ * sonet_chamfer_f32's bits for that cloud alone at N = P_b (same arithmetic, tie rule, non-finite
+ * rule and summation order); loss is the mean over clouds of the per-cloud means, so every cloud
+ * counts once in backward_loss whatever its size. tile_start: device scratch of B+1 int32, written
+ * from the host (one pageable copy on the stream) with the prefix sums of the clouds' 1024-column
+ * tiles. Refused before any launch: B < 1, Mp < 1, ld < 3, a null pointer, idx_fwd without idx_bwd
+ * or the reverse, offsets_host not running from 0 to T, an empty cloud, a cloud of 2^24 points or
+ * more. Device offsets that disagree with offsets_host are clamped into [0,T] (results unspecified,
+ * nothing out of range). Deterministic; no allocation, no host synchronisation. */
+int sonet_chamfer_ragged_f32(const float* pred, int B, int Mp, const float* points, long long T,
+                             long long ld, const long long* offsets, const long long* offsets_host,
+                             int32_t* tile_start, int32_t* idx_fwd, int32_t* idx_bwd, float* elem_fwd,
+                             float* elem_bwd, float* loss_fwd_arr, float* loss_bwd_arr, float* loss,
+                             sonet_stream_t stream);
 
 /* ---- a-5 on tensor cores: the whole first PointResNet as one wgmma kernel ----------------------
  * Replaces Encoder.first_pointnet = PointResNet(Cin,[64,128,256,384]).forward in eval mode

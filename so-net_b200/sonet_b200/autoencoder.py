@@ -4,7 +4,7 @@ Double-buffered asynchronous set_input and CUDA-graph replay of test_model() and
 optimize(): _model_base.GraphedModel."""
 import torch
 
-from . import losses, networks
+from . import augmentation, losses, networks
 from ._model_base import ENCODER_SNAPSHOT, GraphedModel
 
 
@@ -82,6 +82,53 @@ class Model(GraphedModel):
         with torch.no_grad():
             self.forward(is_train=False)
             self._losses(train=False)
+
+    def reconstruct_clouds(self, points, offsets, node, node_knn_I=None, chunk_points=None):
+        """The auto-encoder's evaluation against whole clouds of any size, in eval mode: points
+        [T,6] f32, offsets [B+1] int64 (cloud b is rows offsets[b] .. offsets[b+1]), node [B,3,M]
+        (the test-mode loader's SOM nodes, DeviceDataset.full_batch), node_knn_I [B,M,som_k] int64
+        or None to compute it with augmentation.som_knn.
+
+        Encoder.forward_ragged encodes every point of each cloud; the decoder runs once over all B
+        features, as test_model() runs it; then test_model()'s combination of Chamfer terms, each
+        measured against the WHOLE clouds (losses.chamfer_ragged): predicted_pc, conv_pc4 when
+        output_conv_pc_num > 0, conv_pc5 when it is 4096. Each cloud counts once in every term
+        whatever its size. Returns a dict: feature [B,F], predicted_pc [B,3,Mp], loss_chamfer,
+        loss_chamfer_conv4 and loss_chamfer_conv5 (None when test_model() computes no such term),
+        loss, and loss_array [B], predicted_pc's per-cloud loss. With equal-size clouds and the same
+        nodes every value is test_model()'s bits.
+
+        Reads no bound input and writes no attribute of the model, its modules or chamfer_criteria:
+        what test_model() left, and a captured eval graph, stay as they were. Refused before any
+        launch: train mode and Encoder.check_ragged's cases, --normalization instance among them
+        (instance statistics have no ragged kernels)."""
+        enc, dec, opt = self.encoder, self.decoder, self.opt
+        if enc.training or dec.training:
+            raise RuntimeError("reconstruct_clouds: the model is in train mode; call test_model() "
+                               "or eval() first")
+        enc.check_ragged(points, offsets, node, node_knn_I, chunk_points, what="reconstruct_clouds")
+        with torch.no_grad():
+            if node_knn_I is None:
+                node_knn_I = augmentation.som_knn(node.detach().contiguous(), opt.som_k,
+                                                  node.shape[2])
+            feature = enc.forward_ragged(points, offsets, node, node_knn_I, chunk_points)
+            predicted_pc, parts = dec.outputs(feature)
+            n_conv = opt.output_conv_pc_num
+            conv4 = conv5 = None
+            if n_conv > 0:
+                if n_conv == 4096:
+                    conv5 = losses.chamfer_ragged(parts["conv_pc5"], points, offsets).loss
+                conv4 = losses.chamfer_ragged(parts["conv_pc4"], points, offsets).loss
+            main = losses.chamfer_ragged(predicted_pc, points, offsets)
+            if n_conv == 1024:
+                loss = main.loss + conv4
+            elif n_conv == 4096:
+                loss = main.loss + conv5 + conv4
+            else:
+                loss = main.loss
+        return dict(feature=feature, predicted_pc=predicted_pc, loss_chamfer=main.loss,
+                    loss_chamfer_conv4=conv4, loss_chamfer_conv5=conv5, loss=loss,
+                    loss_array=main.loss_array)
 
     def _make_optimizers(self):
         return (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr, betas=(0.9, 0.999)),

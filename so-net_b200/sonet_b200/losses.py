@@ -3,7 +3,8 @@
 ChamferLoss (losses.py:17-27, 192-296): the reference builds two Faiss IndexFlatL2 per cloud and
 round-trips through host numpy (losses.py:247-276). Here both nearest-neighbour searches of the
 whole batch, the sqrt(d^2 + 1e-8) terms and all means run on the device in four launches
-(csrc/chamfer.cu). No Faiss dependency.
+(csrc/chamfer.cu). No Faiss dependency. chamfer_ragged: the same numbers against whole
+ground-truth clouds of any size, for evaluation.
 
 compute_iou_np_array / compute_iou (losses.py:73-189), the part-segmentation metric of
 part-seg/train.py:95: one kernel for CUDA tensors, the same arithmetic in C++ for host tensors
@@ -11,7 +12,7 @@ part-seg/train.py:95: one kernel for CUDA tensors, the same arithmetic in C++ fo
 """
 import json
 import os
-from collections import OrderedDict
+from collections import OrderedDict, namedtuple
 
 import numpy as np
 import torch
@@ -93,6 +94,32 @@ class ChamferLoss(nn.Module):
 
     def __call__(self, predict_pc, gt_pc):
         return self.forward(predict_pc, gt_pc)
+
+
+ChamferRagged = namedtuple("ChamferRagged", ("loss", "forward_loss", "backward_loss", "loss_array",
+                                             "fwd_arr", "bwd_arr"))
+
+
+def chamfer_ragged(predict_pc, points, offsets):
+    """ChamferLoss's evaluation numbers against whole clouds of any size: predict_pc [B,3,Mp] (CUDA)
+    against ground-truth clouds points [T,>=3] (xyz first; DeviceDataset's [T,6]), cloud b rows
+    offsets[b] .. offsets[b+1]. Returns ChamferRagged(loss, forward_loss, backward_loss, loss_array,
+    fwd_arr, bwd_arr), the values ChamferLoss.forward returns and sets in evaluation.
+
+    Cloud b's numbers are ChamferLoss's on that cloud alone, at N = P_b. forward_loss and
+    backward_loss are means over the clouds of the per-cloud means, so each cloud counts once
+    whatever its size: with equal sizes that is the reference's b_el.mean(), and with ragged sizes
+    it keeps large clouds from dominating. Evaluation only: a gradient cannot flow through it, so
+    predict_pc or points requiring one with grad mode on is refused."""
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad
+                                       for t in (predict_pc, points)):
+        raise RuntimeError("chamfer_ragged is evaluation only: no gradient flows through it "
+                           "(call it under torch.no_grad() or on detached tensors)")
+    if not isinstance(predict_pc, torch.Tensor) or not predict_pc.is_cuda:
+        raise RuntimeError("sonet_b200.chamfer_ragged runs on CUDA tensors only (no CPU fallback)")
+    r = ops.chamfer_ragged(predict_pc.detach().contiguous(), points.detach(), offsets)
+    return ChamferRagged(r["loss"][2], r["loss"][0], r["loss"][1], r["fwd_arr"] + r["bwd_arr"],
+                         r["fwd_arr"], r["bwd_arr"])
 
 
 def _seg_iou(score, seg, label, table=None, want_correct=False):

@@ -655,14 +655,19 @@ class DecoderConv(nn.Module):
         self.deconv6 = UpConv(int(f / 8), int(f / 8), activation=act, normalization=norm)
         self.conv2pc6 = ConvToPC(int(f / 8), opt)
 
-    def forward(self, x):
+    def outputs(self, x):
+        """(pc4, pc5, pc6), the point sets of the 16x16, 32x32 and 64x64 levels, without storing
+        them on the module."""
         x = x.view(-1, self.feature_num, 1, 1)
         x = self.deconv4(self.deconv3(self.deconv2(self.deconv1(x))))
-        self.pc4 = self.conv2pc4(x)
+        pc4 = self.conv2pc4(x)
         x = self.deconv5(x)
-        self.pc5 = self.conv2pc5(x)
+        pc5 = self.conv2pc5(x)
         x = self.deconv6(x)
-        self.pc6 = self.conv2pc6(x)
+        return pc4, pc5, self.conv2pc6(x)
+
+    def forward(self, x):
+        self.pc4, self.pc5, self.pc6 = self.outputs(x)
         return self.pc6
 
 
@@ -676,22 +681,42 @@ class Decoder(nn.Module):
             self.fc_decoder = DecoderLinear(opt)
         self.conv_decoder = DecoderConv(opt)
 
-    def forward(self, x):
+    def outputs(self, x):
+        """(predicted point set, parts) without storing anything on this module or its submodules:
+        parts holds linear_pc when output_fc_pc_num > 0 and conv_pc4 / conv_pc5 / conv_pc6 when
+        output_conv_pc_num > 0, the tensors forward() stores under those names."""
+        return self._outputs(x, self.conv_decoder.outputs)
+
+    def _stored_pyramid(self, x):
+        self.conv_decoder(x)
+        return self.conv_decoder.pc4, self.conv_decoder.pc5, self.conv_decoder.pc6
+
+    def _outputs(self, x, pyramid):
+        parts = {}
         if self.opt.output_fc_pc_num > 0:
-            self.linear_pc = self.fc_decoder(x)
+            parts["linear_pc"] = self.fc_decoder(x)
         if self.opt.output_conv_pc_num > 0:
-            self.conv_pc6 = self.conv_decoder(x).view(-1, 3, 4096)
-            self.conv_pc4 = self.conv_decoder.pc4.view(-1, 3, 256)
-            self.conv_pc5 = self.conv_decoder.pc5.view(-1, 3, 1024)
+            pc4, pc5, pc6 = pyramid(x)
+            parts["conv_pc6"] = pc6.view(-1, 3, 4096)
+            parts["conv_pc4"] = pc4.view(-1, 3, 256)
+            parts["conv_pc5"] = pc5.view(-1, 3, 1024)
+        out = None
         if self.opt.output_fc_pc_num == 0:
             if self.opt.output_conv_pc_num == 4096:
-                return self.conv_pc6
+                out = parts["conv_pc6"]
             elif self.opt.output_conv_pc_num == 1024:
-                return self.conv_pc5
+                out = parts["conv_pc5"]
         else:
             if self.opt.output_conv_pc_num == 4096:
-                return torch.cat([self.linear_pc, self.conv_pc6], 2)
+                out = torch.cat([parts["linear_pc"], parts["conv_pc6"]], 2)
             elif self.opt.output_conv_pc_num == 1024:
-                return torch.cat([self.linear_pc, self.conv_pc5], 2)
+                out = torch.cat([parts["linear_pc"], parts["conv_pc5"]], 2)
             else:
-                return self.linear_pc
+                out = parts["linear_pc"]
+        return out, parts
+
+    def forward(self, x):
+        out, parts = self._outputs(x, self._stored_pyramid)
+        for name, t in parts.items():
+            setattr(self, name, t)
+        return out

@@ -877,6 +877,58 @@ def chamfer(pred, gt, want_idx=False):
                 idx_bwd=idx_b)
 
 
+CHAMFER_RAGGED_MAX_POINTS = (1 << 24) - 1   # P_b must be exact as the float divisor of its mean
+
+
+def chamfer_ragged(pred, points, offsets, want_idx=False):
+    """chamfer against whole clouds: pred [B,3,Mp] f32, points [T,>=3] f32 rows (xyz first, unit
+    column stride, any row stride: DeviceDataset's [T,6]), offsets [B+1] int64 on pred's device
+    (cloud b is rows offsets[b] .. offsets[b+1]). -> chamfer's dict with the gt side ragged:
+    elem_bwd [T], idx_bwd [T] (the nearest predicted point of each gt point), idx_fwd [B,Mp]
+    cloud-local rows. Cloud b's entries are chamfer's on that cloud alone; loss is the mean over
+    clouds of the per-cloud means. Copies the offsets to the host (one synchronisation) and refuses
+    bad offsets, an empty cloud (ValueError) and a cloud of 2^24 points or more before any launch."""
+    _chk(pred, "predict_pc", torch.float32)
+    _chk(offsets, "offsets", torch.int64)
+    if not isinstance(points, torch.Tensor) or points.dtype != torch.float32 or not points.is_cuda:
+        raise RuntimeError("points must be a float32 CUDA tensor")
+    if pred.dim() != 3 or pred.shape[1] != 3 or pred.shape[0] < 1 or pred.shape[2] < 1:
+        raise RuntimeError("chamfer_ragged: predict_pc must be [B,3,Mp] with B, Mp >= 1 (got %s)"
+                           % (tuple(pred.shape),))
+    if points.dim() != 2 or points.shape[1] < 3 or points.stride(1) != 1 \
+            or (points.shape[0] > 1 and points.stride(0) < 3):
+        raise RuntimeError("chamfer_ragged: points must be [T, >=3] rows with unit column stride "
+                           "(got %s, strides %s)" % (tuple(points.shape), points.stride()))
+    if points.device != pred.device or offsets.device != pred.device:
+        raise RuntimeError("chamfer_ragged: predict_pc, points and offsets must be on one device "
+                           "(got %s, %s, %s)" % (pred.device, points.device, offsets.device))
+    B, _, Mp = pred.shape
+    T = points.shape[0]
+    off = ragged_offsets(offsets, T, B)
+    counts = off[1:] - off[:-1]
+    if (counts == 0).any():
+        raise ValueError("chamfer_ragged: cloud %d has no points" % int((counts == 0).argmax()))
+    if counts.max() > CHAMFER_RAGGED_MAX_POINTS:
+        raise RuntimeError("chamfer_ragged: cloud %d has %d points, more than %d"
+                           % (int(counts.argmax()), int(counts.max()), CHAMFER_RAGGED_MAX_POINTS))
+    dev = pred.device
+    with torch.cuda.device(dev):
+        tile_start = torch.empty((B + 1,), dtype=torch.int32, device=dev)
+        idx_f = torch.empty((B, Mp), dtype=torch.int32, device=dev) if want_idx else None
+        idx_b = torch.empty((T,), dtype=torch.int32, device=dev) if want_idx else None
+        ef = torch.empty((B, Mp), dtype=torch.float32, device=dev)
+        eb = torch.empty((T,), dtype=torch.float32, device=dev)
+        fa = torch.empty((B,), dtype=torch.float32, device=dev)
+        ba = torch.empty((B,), dtype=torch.float32, device=dev)
+        loss = torch.empty((3,), dtype=torch.float32, device=dev)
+        _call("sonet_chamfer_ragged_f32", _C.ptr(pred), B, Mp, _C.ptr(points), T,
+              points.stride(0), _C.ptr(offsets), off.ctypes.data, _C.ptr(tile_start), _C.ptr(idx_f),
+              _C.ptr(idx_b), _C.ptr(ef), _C.ptr(eb), _C.ptr(fa), _C.ptr(ba), _C.ptr(loss),
+              _stream(pred), kernels=4 if want_idx else 3)
+    return dict(loss=loss, fwd_arr=fa, bwd_arr=ba, elem_fwd=ef, elem_bwd=eb, idx_fwd=idx_f,
+                idx_bwd=idx_b)
+
+
 def pointresnet_tc_pack(W, shifts, cin):
     """Host-side packing for pointresnet_tc: W = [W0 [64,cin], W1 [128,64], W2 [256,128],
     W3 [384,320]] folded fp32 weights, shifts = 4 folded shift vectors (any device).

@@ -1,7 +1,8 @@
-"""Whole clouds of any size: classifier.Model.score_clouds (networks.Encoder.forward_ragged) against
-the dense test_model() on the same clouds, and a batch of clouds of mixed sizes.
+"""Whole clouds of any size: classifier.Model.score_clouds (networks.Encoder.forward_ragged) and
+autoencoder.Model.reconstruct_clouds against the dense test_model() on the same clouds, and a batch
+of clouds of mixed sizes.
 
-    python tools/ragged_bench.py [--reps 20] [--out results.json]
+    python tools/ragged_bench.py [--reps 20] [--task all|classifier|autoencoder] [--out results.json]
 
   A  64 clouds x 10,000 points as one ragged batch, against dense test_model() at N = 10,000 and
      N = 5,000 on the same clouds (eager and with the eval CUDA graph).
@@ -9,8 +10,14 @@ the dense test_model() on the same clouds, and a batch of clouds of mixed sizes.
      between assignment + sort, the first PointResNet + pool and the node-level stage (a separate
      run with per-call CUDA events, ops.PROFILE).
 
+  AE_A, AE_B  the same two cases for the auto-encoder (reconstruct_clouds: the ragged encoder, the
+     decoder once over all features and the Chamfer terms against the whole clouds), the dense
+     side at N = 10,000; AE_B splits the time into encoder, decoder and Chamfer (CUDA events
+     around each stage) and gives the Chamfer's pair rate.
+
 Times are medians of --reps warm calls, each bracketed by CUDA events. Synthetic clouds and weights
-(synth.py), the default classifier options (k = 3, 8x8 SOM, som_k = 9); SONET_TC as set.
+(synth.py), the default options of each task (k = 3, 8x8 SOM, som_k = 9; the auto-encoder's
+256 + 1024 output points); SONET_TC as set.
 """
 import argparse
 import json
@@ -24,7 +31,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "so-net_b200")]
 
-from sonet_b200 import augmentation, classifier, networks, ops, synth  # noqa: E402
+from sonet_b200 import augmentation, autoencoder, classifier, networks, ops, synth  # noqa: E402
 
 DEV = torch.device("cuda:0")
 
@@ -87,26 +94,112 @@ def stage_split(m, pts, off, node, knn):
     return split
 
 
+def ae_model(B, N, states, graph=False):
+    opt = synth.make_opt("autoencoder", batch_size=B, input_pc_num=N, device=DEV)
+    m = autoencoder.Model(opt)
+    m.encoder.load_state_dict(states[0])
+    m.decoder.load_state_dict(states[1])
+    m.encoder.eval()
+    m.decoder.eval()
+    m.enable_cuda_graph(graph)
+    return m
+
+
+def ae_stage_split(m, pts, off, node, knn, reps):
+    """Median device time of reconstruct_clouds' three stages, each between CUDA events: the
+    ragged encoder, the decoder, and the Chamfer terms (with their offsets checks)."""
+    from sonet_b200 import losses
+    ts = {"encoder": [], "decoder": [], "chamfer": []}
+    for i in range(reps + 3):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        with torch.no_grad():
+            ev[0].record()
+            feat = m.encoder.forward_ragged(pts, off, node, knn)
+            ev[1].record()
+            pc, parts = m.decoder.outputs(feat)
+            ev[2].record()
+            for t in (parts["conv_pc4"], pc):
+                losses.chamfer_ragged(t, pts, off)
+            ev[3].record()
+        ev[3].synchronize()
+        if i >= 3:
+            for j, k in enumerate(ts):
+                ts[k].append(ev[j].elapsed_time(ev[j + 1]))
+    return {k: float(np.median(v)) for k, v in ts.items()}
+
+
+def autoencoder_cases(res, reps):
+    cpu_opt = synth.make_opt("autoencoder")
+    states = (synth.synth_state_dict(networks.Encoder(cpu_opt), seed=1),
+              synth.synth_state_dict(networks.Decoder(cpu_opt), seed=2))
+    B, P, M = 64, 10000, 64
+    pts, off, node = clouds([P] * B, M, seed=0)
+    knn = augmentation.som_knn(node, 9, M)
+    m = ae_model(B, P, states)
+    res["AE_A_ragged_64x10000_ms"] = median_ms(lambda: m.reconstruct_clouds(pts, off, node, knn),
+                                               reps)
+    pc = pts.view(B, P, 6)[:, :, :3].permute(0, 2, 1).contiguous().cpu()
+    sn = pts.view(B, P, 6)[:, :, 3:].permute(0, 2, 1).contiguous().cpu()
+    for graph in (False, True):
+        md = ae_model(B, P, states, graph)
+
+        def dense():
+            md.set_input(pc, sn, torch.zeros(B, dtype=torch.int64), node.cpu(), knn.cpu())
+            md.test_model()
+        res["AE_A_dense_N%d_%s_ms" % (P, "graph" if graph else "eager")] = median_ms(dense, reps)
+        del md
+    del m
+    torch.cuda.empty_cache()
+
+    rs = np.random.RandomState(5)
+    sizes = rs.randint(2000, 10001, size=1024)
+    pts, off, node = clouds(sizes, M, seed=1)
+    knn = augmentation.som_knn(node, 9, M)
+    m = ae_model(1, 256, states)
+    t = median_ms(lambda: m.reconstruct_clouds(pts, off, node, knn), reps)
+    res["AE_B_mixed_1024_ms"] = t
+    res["AE_B_points"] = int(sizes.sum())
+    res["AE_B_clouds_per_s"] = 1024 / (t[0] * 1e-3)
+    split = ae_stage_split(m, pts, off, node, knn, reps)
+    res["AE_B_split_ms"] = split
+    # predicted_pc (1,280 points) and conv_pc4 (256) against every point, both directions at once
+    pairs = (1280 + 256) * float(sizes.sum())
+    res["AE_B_chamfer_pairs"] = pairs
+    res["AE_B_chamfer_pairs_per_s"] = pairs / (split["chamfer"] * 1e-3)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--task", choices=("all", "classifier", "autoencoder"), default="all")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("ragged_bench: needs a CUDA device")
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm",
                           "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = dict(gpu=gpu, sonet_tc=os.environ.get("SONET_TC", "1"), reps=a.reps)
+    if a.task in ("all", "autoencoder"):
+        autoencoder_cases(res, a.reps)
+    if a.task in ("all", "classifier"):
+        classifier_cases(res, a.reps)
+    print(json.dumps(res, indent=1))
+    if a.out:
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+def classifier_cases(res, reps):
     cpu_opt = synth.make_opt("classifier")
     states = (synth.synth_state_dict(networks.Encoder(cpu_opt), seed=1),
               synth.synth_state_dict(networks.Classifier(cpu_opt), seed=2))
-    res = dict(gpu=gpu, sonet_tc=os.environ.get("SONET_TC", "1"), reps=a.reps)
 
     # ---- A: 64 x 10,000 ragged against dense N = 10,000 and N = 5,000 ----
     B, P, M = 64, 10000, 64
     pts, off, node = clouds([P] * B, M, seed=0)
     knn = augmentation.som_knn(node, 9, M)
     m = model(B, P, states)
-    res["A_ragged_64x10000_ms"] = median_ms(lambda: m.score_clouds(pts, off, node, knn), a.reps)
+    res["A_ragged_64x10000_ms"] = median_ms(lambda: m.score_clouds(pts, off, node, knn), reps)
     for N in (10000, 5000):
         pc = pts.view(B, P, 6)[:, :N, :3].permute(0, 2, 1).contiguous().cpu()
         sn = pts.view(B, P, 6)[:, :N, 3:].permute(0, 2, 1).contiguous().cpu()
@@ -117,7 +210,7 @@ def main():
                 md.set_input(pc, sn, torch.zeros(B, dtype=torch.int64), node.cpu(), knn.cpu())
                 md.test_model()
             # set_input's host-to-device copy is part of the dense call, as in bench.py
-            res["A_dense_N%d_%s_ms" % (N, "graph" if graph else "eager")] = median_ms(dense, a.reps)
+            res["A_dense_N%d_%s_ms" % (N, "graph" if graph else "eager")] = median_ms(dense, reps)
             del md
     del m
     torch.cuda.empty_cache()
@@ -128,16 +221,12 @@ def main():
     pts, off, node = clouds(sizes, M, seed=1)
     knn = augmentation.som_knn(node, 9, M)
     m = model(1, 256, states)
-    t = median_ms(lambda: m.score_clouds(pts, off, node, knn), a.reps)
+    t = median_ms(lambda: m.score_clouds(pts, off, node, knn), reps)
     res["B_mixed_1024_ms"] = t
     res["B_points"] = int(sizes.sum())
     res["B_clouds_per_s"] = 1024 / (t[0] * 1e-3)
     res["B_points_per_s"] = float(sizes.sum()) / (t[0] * 1e-3)
     res["B_split_ms"] = stage_split(m, pts, off, node, knn)
-    print(json.dumps(res, indent=1))
-    if a.out:
-        with open(a.out, "w") as f:
-            json.dump(res, f, indent=1)
 
 
 if __name__ == "__main__":

@@ -55,6 +55,10 @@ pred = torch.rand(2, 3, 300, device=dev, generator=g)
 gt = torch.rand(2, 3, 1100, device=dev, generator=g)
 r = ops.chamfer(pred, gt, want_idx=True)
 print("chamfer idx", int(r["idx_fwd"].sum()))
+pts = torch.rand(1 + 1100 + 2500, 6, device=dev, generator=g)
+off = torch.tensor([0, 1, 1101, 3601], dtype=torch.int64, device=dev)
+r = ops.chamfer_ragged(torch.rand(3, 3, 300, device=dev, generator=g), pts, off, want_idx=True)
+print("chamfer_ragged idx", int(r["idx_fwd"].sum()), int(r["idx_bwd"].sum()))
 x = torch.rand(2, 3, 1000, device=dev, generator=g) * 2 - 1
 s = som.BatchSOM(8, 8, 3, 0, 2)
 s.optimize(x)
