@@ -490,6 +490,58 @@ int sonet_point_normals_f32(const float* data, long long T, int stride, const in
                             void* scratch, long long scratch_bytes, float* normals,
                             int normal_stride, float* curvature, sonet_stream_t stream);
 
+/* sonet_point_normals_orient_f32: makes existing normals (estimated, scanned, any) consistently
+ * oriented within each cloud by propagating their signs along a minimum spanning tree of the k-NN
+ * graph (Hoppe et al. 1992). It changes only signs, in place at normals + row * normal_stride.
+ *   Clouds: row g belongs to the cloud ragged_find (csrc/common.cuh) picks over the clamped offsets
+ *     when it lies in that cloud's clamped range, to no cloud otherwise, so every row has at most one
+ *     cloud even when offsets overlap. Rows of a cloud at a cloud-local index >= max_points are not
+ *     vertices: max_points fixes the round schedule without a host synchronisation, and callers pass
+ *     the largest cloud size.
+ *   Vertices: rows with finite xyz and a finite, non-zero normal. Edges: for each vertex u and each
+ *     entry j of idx[u, 0..K) (cloud-local, as sonet_point_knn_f32 writes) in [0, P) with j != u
+ *     whose row is a vertex of u's cloud, the undirected edge {u, j}; an edge listed from both ends
+ *     is one edge. Its dot = (nx_u*nx_v + ny_u*ny_v) + nz_u*nz_v in fp64, explicitly rounded, its
+ *     weight w = fp32(1 - |dot|) rounded once. Edges are ordered strictly by (w, min(u,v), max(u,v))
+ *     (cloud-local), so every connected component has exactly one minimum spanning tree.
+ *   Anchor: one vertex per component, the codes of sonet_point_normals_f32:
+ *     SONET_NORMALS_AWAY_FROM_CENTROID  the vertex farthest from the cloud's centroid (computed as
+ *                                       sonet_point_normals_f32 does, over every row of the clamped
+ *                                       range), ref = p - c;
+ *     SONET_NORMALS_TOWARD_VIEWPOINT    the vertex nearest view[s], ref = view[s] - p;
+ *     squared distances ((dx*dx + dy*dy) + dz*dz) in fp64, a NaN distance last, the lowest
+ *     cloud-local index on ties. The anchor flips iff dot(n, ref) < 0 in fp64 ((nx*rx + ny*ry) +
+ *     nz*rz); a dot of 0 or NaN keeps its input sign. Any other code (CANONICAL too) is refused.
+ *   Signs: a vertex is negated iff the anchor's flip XOR the parity of the dot < 0 edges on its tree
+ *     path from the anchor is 1. Output normals are exactly +-input; non-vertices are untouched.
+ *     Input signs matter only through edges whose dot is exactly 0 and anchors whose dot is 0 or NaN.
+ *     component [T] i32 (nullable): the cloud-local index of the vertex's anchor, -1 for every row
+ *     that is not a vertex.
+ * Limits: every component is anchored on its own; a k-NN graph that bridges two close sheets can
+ * carry a flip across them; no edges beyond the k-NN graph are added. max_points must be below
+ * SONET_POINT_ORIENT_MAX_POINTS = 2^24 (the pairs are packed as two 24-bit local indices), a
+ * narrower limit than sonet_point_knn_f32's.
+ * Work: one optional centroid launch, one init launch, 5 launches per round for
+ * ceil(log2(max_points)) rounds (a round after one that merged nothing exits at once), then 3.
+ * Scratch: sonet_point_normals_orient_scratch_bytes(T, S) bytes of 256-byte aligned device memory
+ * (0 for S = 0, where scratch may be null; -1 for T < 0 or S < 0). After a call its first
+ * SONET_POINT_ORIENT_MAX_ROUNDS int32 hold 1 for each round that merged components.
+ * Like the entries above it allocates nothing, does not synchronise, is deterministic and capturable
+ * in a CUDA graph; every loop is bounded (rounds by max_points, pointer jumps by max_points steps).
+ * It fails with SONET_ERR_BAD_ARG before any CUDA call for S < 0, T < 0, stride < 3,
+ * normal_stride < 3, K outside [1, SONET_POINT_KNN_MAX_K], max_points outside [0, 2^24), an
+ * unknown anchor code, null offsets or normals, null data or idx with T > 0, a null view with the
+ * viewpoint code, or a missing, too small or misaligned scratch; S = 0 then returns without a
+ * launch. */
+#define SONET_POINT_ORIENT_MAX_POINTS 16777216
+#define SONET_POINT_ORIENT_MAX_ROUNDS 24
+long long sonet_point_normals_orient_scratch_bytes(long long T, int S);
+int sonet_point_normals_orient_f32(const float* data, long long T, int stride, const int64_t* offsets,
+                                   int S, int max_points, const int32_t* idx, int K, int anchor,
+                                   const float* view, void* scratch, long long scratch_bytes,
+                                   float* normals, int normal_stride, int32_t* component,
+                                   sonet_stream_t stream);
+
 /* ---- a-4/a-5/a-8/a-9/a-10: point-wise shared MLP layer (1x1 conv + folded BN + ReLU) ---------
  * Replaces EquivariantLayer.forward / MyConv2d(1x1).forward in eval mode
  * (models/layers.py:203-210, 282-296): out[b,co,p] = act(scale[co]*sum_ci W[co,ci]*X[b,ci,p] +

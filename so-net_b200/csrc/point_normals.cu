@@ -373,6 +373,252 @@ static dim3 pk_grid(long long T, int S, int tile) {
 
 static size_t pn_scratch(int S) { return (sizeof(double) * 3 * static_cast<size_t>(S) + 255) & ~static_cast<size_t>(255); }
 
+// ---- orientation: signs propagated along each component's minimum spanning tree ------------------
+// Borůvka over the k-NN graph of every cloud at once, the parity carried through the union. Per
+// vertex, node = (root row << 1) | parity of its sign relative to the root. A round: every directed
+// entry (u -> v) across two components offers its key to both roots, first the ordered weight bits
+// (atomicMin), then the cloud-local pair (lo << 24) | hi among the entries that reach that weight;
+// every root hooks to the root at the other end of its least edge (a mutual pair keeps the lower
+// row), the hooked roots pointer-jump to their tree's root XOR-ing the parities, and every vertex
+// rebases onto it. Edges are strictly ordered, so the least edges form a forest: each component with
+// an outgoing edge merges, and ceil(log2(max_points)) rounds join every connected component. Then
+// each component takes its anchor (least distance key, then least cloud-local index) and every
+// vertex's sign is its anchor's flip XOR its parity relative to the anchor.
+constexpr int PO_THREADS = 256;
+constexpr int PO_MAX_ROUNDS = SONET_POINT_ORIENT_MAX_ROUNDS;   // ceil(log2(max_points)), max_points < 2^24
+constexpr unsigned long long PO_NONE = ~0ull;
+
+struct OrientArgs {
+  const float* data;
+  const int64_t* off;
+  const int32_t* idx;
+  const float* view;
+  const double* cen;
+  float* normals;
+  int32_t* comp;
+  int* merged;                 // [PO_MAX_ROUNDS]: round r hooked at least one root
+  int32_t* cid;                // [T] the cloud of a vertex, -1 for a non-vertex
+  unsigned long long* node;    // [T] (root row << 1) | parity relative to the root
+  unsigned long long* link;    // [T] a root's (parent row << 1) | parity within a round
+  unsigned int* bw;            // [T] a root's least ordered weight key offered this round
+  unsigned long long* be;      // [T] a root's least (lo << 24) | hi among the entries at bw
+  unsigned long long* ak;      // [T] a root's least anchor distance key
+  unsigned int* ai;            // [T] a root's least (local << 1) | flip among the vertices at ak
+  long long T;
+  int stride, nstride, S, K, max_points, anchor;
+};
+
+// The pointer jumps read links other threads are rewriting: one 64-bit word holds parent and parity,
+// so any value read is a consistent ancestor, and relaxed device-scope accesses keep them uncached.
+__device__ __forceinline__ unsigned long long po_load(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void po_store(unsigned long long* p, unsigned long long v) {
+  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ bool po_active(const int* merged, int round) {
+  return round == 0 || *reinterpret_cast<const volatile int*>(merged + round - 1) != 0;
+}
+
+// (nx_u*nx_v + ny_u*ny_v) + nz_u*nz_v in fp64, explicitly rounded
+__device__ __forceinline__ double po_dot(const float* a, const float* b) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a[0], b[0]), __dmul_rn(a[1], b[1])), __dmul_rn(a[2], b[2]));
+}
+
+// w = fp32(1 - |dot|) as an unsigned key in float order (-0 made +0 first; w is never NaN)
+__device__ __forceinline__ unsigned po_wkey(double dot) {
+  const unsigned b = __float_as_uint(__fadd_rn(__double2float_rn(__dsub_rn(1.0, fabs(dot))), 0.f));
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+// The anchor's distance key of vertex g (least wins) and its reference vector: the squared fp64
+// distance to the centroid (farthest first) or to view[s] (nearest first); NaN last.
+__device__ __forceinline__ unsigned long long po_akey(const OrientArgs& a, long long g, int s, double& rx,
+                                                      double& ry, double& rz) {
+  const float* p = a.data + g * a.stride;
+  if (a.anchor == SONET_NORMALS_AWAY_FROM_CENTROID) {
+    const double* c = a.cen + 3 * s;
+    rx = __dsub_rn(p[0], c[0]);
+    ry = __dsub_rn(p[1], c[1]);
+    rz = __dsub_rn(p[2], c[2]);
+  } else {
+    const float* v = a.view + 3 * s;
+    rx = __dsub_rn(v[0], p[0]);
+    ry = __dsub_rn(v[1], p[1]);
+    rz = __dsub_rn(v[2], p[2]);
+  }
+  const double d = __dadd_rn(__dadd_rn(__dmul_rn(rx, rx), __dmul_rn(ry, ry)), __dmul_rn(rz, rz));
+  const unsigned long long bits = static_cast<unsigned long long>(__double_as_longlong(d));   // d >= +0
+  if (d != d) return PO_NONE;
+  return a.anchor == SONET_NORMALS_AWAY_FROM_CENTROID ? 0x7ff0000000000000ull - bits : bits;
+}
+
+#define PO_ROWS(g, n)                                                                   \
+  for (long long g = static_cast<long long>(blockIdx.x) * PO_THREADS + threadIdx.x; g < (n); \
+       g += static_cast<long long>(gridDim.x) * PO_THREADS)
+
+// Each row's cloud (ragged_find) and vertex test; every root starts alone with parity 0.
+__global__ void __launch_bounds__(PO_THREADS) orient_init_kernel(OrientArgs a) {
+  if (blockIdx.x == 0 && threadIdx.x < PO_MAX_ROUNDS) a.merged[threadIdx.x] = 0;
+  PO_ROWS(g, a.T) {
+    long long lo, hi;
+    const int s = ragged_find(a.off, a.S, a.T, g, lo, hi);
+    bool vert = g >= lo && g < hi && g - lo < a.max_points;
+    if (vert) {
+      const float* p = a.data + g * a.stride;
+      const float* n = a.normals + g * a.nstride;
+      vert = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && isfinite(n[0]) && isfinite(n[1]) &&
+             isfinite(n[2]) && (n[0] != 0.f || n[1] != 0.f || n[2] != 0.f);
+    }
+    a.cid[g] = vert ? s : -1;
+    a.node[g] = static_cast<unsigned long long>(g) << 1;
+    a.bw[g] = ~0u;
+    a.be[g] = PO_NONE;
+    a.ak[g] = PO_NONE;
+    a.ai[g] = ~0u;
+  }
+}
+
+// PASS 0 offers the weight keys, PASS 1 the pairs of the entries at their root's least weight.
+template <int PASS>
+__global__ void __launch_bounds__(PO_THREADS) orient_offer_kernel(OrientArgs a, int round) {
+  if (!po_active(a.merged, round)) return;
+  PO_ROWS(e, a.T * a.K) {
+    const long long u = e / a.K;
+    const int s = a.cid[u];
+    if (s < 0) continue;
+    const int j = a.idx[e];
+    long long lo, hi;
+    ragged_range(a.off, s, a.T, lo, hi);
+    const long long ul = u - lo;
+    if (j < 0 || j >= hi - lo || j == ul || a.cid[lo + j] != s) continue;
+    const long long ru = static_cast<long long>(a.node[u] >> 1), rv = static_cast<long long>(a.node[lo + j] >> 1);
+    if (ru == rv) continue;
+    const unsigned key = po_wkey(po_dot(a.normals + u * a.nstride, a.normals + (lo + j) * a.nstride));
+    if (PASS == 0) {
+      atomicMin(a.bw + ru, key);
+      atomicMin(a.bw + rv, key);
+    } else {
+      const unsigned long long uj = static_cast<unsigned long long>(j), uu = static_cast<unsigned long long>(ul);
+      const unsigned long long pair = uu < uj ? (uu << 24) | uj : (uj << 24) | uu;
+      if (a.bw[ru] == key) atomicMin(a.be + ru, pair);
+      if (a.bw[rv] == key) atomicMin(a.be + rv, pair);
+    }
+  }
+}
+
+// Every root links to the root across its least edge, with its parity relative to that root.
+__global__ void __launch_bounds__(PO_THREADS) orient_hook_kernel(OrientArgs a, int round) {
+  if (!po_active(a.merged, round)) return;
+  PO_ROWS(g, a.T) {
+    const int s = a.cid[g];
+    if (s < 0 || static_cast<long long>(a.node[g] >> 1) != g) continue;
+    const unsigned long long e = a.be[g];
+    unsigned long long l = static_cast<unsigned long long>(g) << 1;
+    if (e != PO_NONE) {
+      long long lo, hi;
+      ragged_range(a.off, s, a.T, lo, hi);
+      const long long x = lo + static_cast<long long>(e >> 24), y = lo + static_cast<long long>(e & 0xffffffull);
+      const unsigned long long nx = a.node[x], ny = a.node[y];
+      const long long other = static_cast<long long>((nx >> 1) == static_cast<unsigned long long>(g) ? ny >> 1 : nx >> 1);
+      const unsigned long long flip = po_dot(a.normals + x * a.nstride, a.normals + y * a.nstride) < 0.0;
+      if (!(g < other && a.be[other] == e)) {   // a mutual pair keeps the lower row as root
+        l = (static_cast<unsigned long long>(other) << 1) | (((nx ^ ny) & 1ull) ^ flip);
+        a.merged[round] = 1;
+      }
+    }
+    a.link[g] = l;
+  }
+}
+
+// Every hooked root walks to its tree's root. Each step moves at least one link closer, and a tree
+// holds fewer than max_points roots, so max_points steps always reach it.
+__global__ void __launch_bounds__(PO_THREADS) orient_jump_kernel(OrientArgs a, int round) {
+  if (!po_active(a.merged, round + 1)) return;
+  PO_ROWS(g, a.T) {
+    if (a.cid[g] < 0 || static_cast<long long>(a.node[g] >> 1) != g) continue;
+    unsigned long long l = po_load(a.link + g);
+    for (int step = 0; step < a.max_points; ++step) {
+      const unsigned long long p = l >> 1;
+      if (p == static_cast<unsigned long long>(g)) break;
+      const unsigned long long lp = po_load(a.link + p);
+      if ((lp >> 1) == p) break;
+      l = (lp & ~1ull) | ((l ^ lp) & 1ull);
+      po_store(a.link + g, l);
+    }
+  }
+}
+
+// Every vertex moves onto its root's root; the per-root offers start over.
+__global__ void __launch_bounds__(PO_THREADS) orient_rebase_kernel(OrientArgs a, int round) {
+  if (!po_active(a.merged, round + 1)) return;
+  PO_ROWS(g, a.T) {
+    if (a.cid[g] < 0) continue;
+    const unsigned long long nd = a.node[g], l = a.link[nd >> 1];
+    a.node[g] = (l & ~1ull) | ((nd ^ l) & 1ull);
+    a.bw[g] = ~0u;
+    a.be[g] = PO_NONE;
+  }
+}
+
+// PASS 0: each component's least distance key; PASS 1: among its vertices at that key, the least
+// (local index << 1) | (anchor flip XOR parity relative to the root).
+template <int PASS>
+__global__ void __launch_bounds__(PO_THREADS) orient_anchor_kernel(OrientArgs a) {
+  PO_ROWS(g, a.T) {
+    const int s = a.cid[g];
+    if (s < 0) continue;
+    double rx, ry, rz;
+    const unsigned long long key = po_akey(a, g, s, rx, ry, rz), nd = a.node[g];
+    if (PASS == 0) {
+      atomicMin(a.ak + (nd >> 1), key);
+    } else if (a.ak[nd >> 1] == key) {
+      const float* n = a.normals + g * a.nstride;
+      const double dot = __dadd_rn(__dadd_rn(__dmul_rn(n[0], rx), __dmul_rn(n[1], ry)), __dmul_rn(n[2], rz));
+      long long lo, hi;
+      ragged_range(a.off, s, a.T, lo, hi);
+      atomicMin(a.ai + (nd >> 1), (static_cast<unsigned>(g - lo) << 1) | ((dot < 0.0) ^ static_cast<unsigned>(nd & 1ull)));
+    }
+  }
+}
+
+__global__ void __launch_bounds__(PO_THREADS) orient_write_kernel(OrientArgs a) {
+  PO_ROWS(g, a.T) {
+    if (a.cid[g] < 0) {
+      if (a.comp) a.comp[g] = -1;
+      continue;
+    }
+    const unsigned long long nd = a.node[g];
+    const unsigned w = a.ai[nd >> 1];
+    if ((w ^ static_cast<unsigned>(nd)) & 1u) {
+      float* n = a.normals + g * a.nstride;
+      n[0] = -n[0];
+      n[1] = -n[1];
+      n[2] = -n[2];
+    }
+    if (a.comp) a.comp[g] = static_cast<int32_t>(w >> 1);
+  }
+}
+#undef PO_ROWS
+
+static int po_rounds(int max_points) { return max_points <= 1 ? 0 : 32 - __builtin_clz(static_cast<unsigned>(max_points - 1)); }
+
+static size_t al256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
+
+// flags | centroids [S, 3] f64 | node, link, be, ak [T] u64 | cid, bw, ai [T] 32-bit
+static size_t po_scratch(long long T, int S) {
+  if (S == 0) return 0;
+  const size_t t = static_cast<size_t>(T);
+  return al256(sizeof(int) * PO_MAX_ROUNDS) + pn_scratch(S) + 4 * al256(8 * t) + 3 * al256(4 * t);
+}
+
+static unsigned po_blocks(long long n) {
+  const long long cap = 16LL * sm_count(), b = (n + PO_THREADS - 1) / PO_THREADS;
+  return static_cast<unsigned>(b < 1 ? 1 : (b > cap ? cap : b));
+}
+
 }  // namespace sonet
 
 extern "C" int sonet_point_knn_f32(const float* data, long long T, int stride, const int64_t* offsets, int S,
@@ -450,4 +696,93 @@ extern "C" int sonet_point_normals_f32(const float* data, long long T, int strid
   }
   point_normals_kernel<<<pk_grid(T, S, PN_THREADS), PN_THREADS, 0, st>>>(a);
   return check_launch("point_normals");
+}
+
+extern "C" long long sonet_point_normals_orient_scratch_bytes(long long T, int S) {
+  using namespace sonet;
+  SONET_REQUIRE(T >= 0 && S >= 0, "point_normals_orient_scratch_bytes: T=%lld and S=%d must be >= 0", T, S);
+  return static_cast<long long>(po_scratch(T, S));
+}
+
+extern "C" int sonet_point_normals_orient_f32(const float* data, long long T, int stride, const int64_t* offsets,
+                                              int S, int max_points, const int32_t* idx, int K, int anchor,
+                                              const float* view, void* scratch, long long scratch_bytes,
+                                              float* normals, int normal_stride, int32_t* component,
+                                              sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE(S >= 0, "point_normals_orient: S=%d must be >= 0", S);
+  SONET_REQUIRE(T >= 0, "point_normals_orient: T=%lld must be >= 0", T);
+  SONET_REQUIRE(stride >= 3, "point_normals_orient: stride=%d must be >= 3", stride);
+  SONET_REQUIRE(normal_stride >= 3, "point_normals_orient: normal_stride=%d must be >= 3", normal_stride);
+  SONET_REQUIRE(K >= 1 && K <= SONET_POINT_KNN_MAX_K, "point_normals_orient: K=%d outside [1, %d]", K,
+                SONET_POINT_KNN_MAX_K);
+  SONET_REQUIRE(max_points >= 0 && max_points < SONET_POINT_ORIENT_MAX_POINTS,
+                "point_normals_orient: max_points=%d outside [0, %d)", max_points, SONET_POINT_ORIENT_MAX_POINTS);
+  SONET_REQUIRE(anchor == SONET_NORMALS_AWAY_FROM_CENTROID || anchor == SONET_NORMALS_TOWARD_VIEWPOINT,
+                "point_normals_orient: anchor code %d is not SONET_NORMALS_AWAY_FROM_CENTROID (1) or "
+                "_TOWARD_VIEWPOINT (2)", anchor);
+  SONET_REQUIRE(offsets && normals, "point_normals_orient: offsets and normals must not be null");
+  SONET_REQUIRE((data && idx) || T == 0, "point_normals_orient: data and idx must not be null (T=%lld)", T);
+  SONET_REQUIRE(view || anchor != SONET_NORMALS_TOWARD_VIEWPOINT,
+                "point_normals_orient: view must not be null with SONET_NORMALS_TOWARD_VIEWPOINT");
+  const long long need = static_cast<long long>(po_scratch(T, S));
+  SONET_REQUIRE(need == 0 || (scratch && scratch_bytes >= need),
+                "point_normals_orient: needs %lld bytes of scratch, got %lld%s", need, scratch_bytes,
+                scratch ? "" : " (null)");
+  SONET_REQUIRE(need == 0 || (reinterpret_cast<uintptr_t>(scratch) & 255u) == 0,
+                "point_normals_orient: scratch must be 256-byte aligned");
+  if (S == 0) return SONET_OK;
+  cudaStream_t st = as_stream(stream);
+  char* p = static_cast<char*>(scratch);
+  const size_t t = static_cast<size_t>(T);
+  auto take = [&](size_t bytes) {
+    char* r = p;
+    p += al256(bytes);
+    return r;
+  };
+  OrientArgs a;
+  a.merged = reinterpret_cast<int*>(take(sizeof(int) * PO_MAX_ROUNDS));
+  double* cen = reinterpret_cast<double*>(take(sizeof(double) * 3 * static_cast<size_t>(S)));
+  a.node = reinterpret_cast<unsigned long long*>(take(8 * t));
+  a.link = reinterpret_cast<unsigned long long*>(take(8 * t));
+  a.be = reinterpret_cast<unsigned long long*>(take(8 * t));
+  a.ak = reinterpret_cast<unsigned long long*>(take(8 * t));
+  a.cid = reinterpret_cast<int32_t*>(take(4 * t));
+  a.bw = reinterpret_cast<unsigned int*>(take(4 * t));
+  a.ai = reinterpret_cast<unsigned int*>(take(4 * t));
+  a.data = data;
+  a.off = offsets;
+  a.idx = idx;
+  a.view = view;
+  a.cen = cen;
+  a.normals = normals;
+  a.comp = component;
+  a.T = T;
+  a.stride = stride;
+  a.nstride = normal_stride;
+  a.S = S;
+  a.K = K;
+  a.max_points = max_points;
+  a.anchor = anchor;
+  if (anchor == SONET_NORMALS_AWAY_FROM_CENTROID) {
+    point_centroid_kernel<<<S < 65535 ? S : 65535, PC_THREADS, 0, st>>>(data, T, stride, offsets, S, cen);
+    const int rc = check_launch("point_normals_orient (centroids)");
+    if (rc != SONET_OK) return rc;
+  }
+  const unsigned rows = po_blocks(T), entries = po_blocks(T * K);
+  orient_init_kernel<<<rows, PO_THREADS, 0, st>>>(a);
+  int rc = check_launch("point_normals_orient (init)");
+  for (int r = 0; r < po_rounds(max_points) && rc == SONET_OK; ++r) {
+    orient_offer_kernel<0><<<entries, PO_THREADS, 0, st>>>(a, r);
+    orient_offer_kernel<1><<<entries, PO_THREADS, 0, st>>>(a, r);
+    orient_hook_kernel<<<rows, PO_THREADS, 0, st>>>(a, r);
+    orient_jump_kernel<<<rows, PO_THREADS, 0, st>>>(a, r);
+    orient_rebase_kernel<<<rows, PO_THREADS, 0, st>>>(a, r);
+    rc = check_launch("point_normals_orient (round)");
+  }
+  if (rc != SONET_OK) return rc;
+  orient_anchor_kernel<0><<<rows, PO_THREADS, 0, st>>>(a);
+  orient_anchor_kernel<1><<<rows, PO_THREADS, 0, st>>>(a);
+  orient_write_kernel<<<rows, PO_THREADS, 0, st>>>(a);
+  return check_launch("point_normals_orient");
 }

@@ -330,6 +330,62 @@ def estimate_normals(data, offsets, idx, orient, view=None, out=None, want_curva
     return normals, curv
 
 
+POINT_ORIENT_MAX_POINTS = _C.CONSTANTS["SONET_POINT_ORIENT_MAX_POINTS"]
+POINT_ORIENT_MAX_ROUNDS = _C.CONSTANTS["SONET_POINT_ORIENT_MAX_ROUNDS"]
+
+
+def orient_rounds(max_points):
+    """The rounds sonet_point_normals_orient_f32 schedules: ceil(log2(max_points)), 0 below 2."""
+    return 0 if max_points <= 1 else int(max_points - 1).bit_length()
+
+
+def orient_normals(data, offsets, idx, normals, anchor, view=None, max_points=None,
+                   want_component=False, scratch=None):
+    """Consistent normal signs within each cloud, propagated along the minimum spanning tree of the
+    k-NN graph idx [T, K] i32 (point_knn's, cloud-local) and anchored per component by `anchor`
+    (NORMALS_AWAY_FROM_CENTROID or NORMALS_TOWARD_VIEWPOINT with view [S, 3] f32). normals: a [T, 3]
+    f32 CUDA view with unit column stride (e.g. data[:, 3:6]), negated in place where the tree says
+    so. max_points: the largest cloud, read from the offsets on the host when None. scratch: a uint8
+    CUDA tensor of at least sonet_point_normals_orient_scratch_bytes(T, S) bytes, or None for a new
+    one; its first POINT_ORIENT_MAX_ROUNDS int32 then say which rounds merged components.
+    -> (normals, component [T] i32 or None): the cloud-local index of each vertex's anchor, -1 off
+    the graph."""
+    T, stride = _rows_arg(data, "orient_normals")
+    _chk(offsets, "offsets", torch.int64)
+    _chk(idx, "idx", torch.int32)
+    _chk(view, "view", torch.float32, optional=True)
+    S = offsets.shape[0] - 1
+    if idx.dim() != 2 or idx.shape[0] != T:
+        raise RuntimeError("orient_normals: idx must be [%d, K], got %s" % (T, tuple(idx.shape)))
+    if view is not None and tuple(view.shape) != (S, 3):
+        raise RuntimeError("orient_normals: view must be [%d, 3], got %s" % (S, tuple(view.shape)))
+    if (not torch.is_tensor(normals) or not normals.is_cuda or normals.dtype != torch.float32
+            or normals.dim() != 2 or tuple(normals.shape) != (T, 3) or normals.stride(1) != 1
+            or (T > 1 and normals.stride(0) < 3)):
+        raise RuntimeError("orient_normals: normals must be a CUDA f32 [T, 3] view with unit column "
+                           "stride, got %s" % (tuple(normals.shape) if torch.is_tensor(normals)
+                                               else type(normals).__name__,))
+    if max_points is None:
+        off = offsets.cpu().clamp(0, T)
+        max_points = int((off[1:] - off[:-1]).clamp(min=0).max()) if S > 0 else 0
+    dev = data.device
+    with torch.cuda.device(dev):
+        comp = torch.empty((T,), dtype=torch.int32, device=dev) if want_component else None
+        nbytes = int(_C.lib().sonet_point_normals_orient_scratch_bytes(T, S))
+        _C.check(0 if nbytes >= 0 else nbytes, "sonet_point_normals_orient_scratch_bytes")
+        if scratch is None:
+            scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        elif not (scratch.is_cuda and scratch.dtype == torch.uint8 and scratch.numel() >= nbytes):
+            raise RuntimeError("orient_normals: scratch must be a CUDA uint8 tensor of >= %d bytes"
+                               % nbytes)
+        launches = 1 + 5 * orient_rounds(int(max_points)) + 3 + (anchor == NORMALS_AWAY_FROM_CENTROID)
+        _call("sonet_point_normals_orient_f32", _C.ptr(data), T, stride, _C.ptr(offsets), S,
+              int(max_points), _C.ptr(idx), idx.shape[1], int(anchor), _C.ptr(view), _C.ptr(scratch),
+              nbytes, _C.ptr(normals), max(normals.stride(0), 3), _C.ptr(comp), _stream(data),
+              kernels=(S > 0) * launches)
+    return normals, comp
+
+
 def som_decenter(x, sn, cluster_mean, min_idx_i32, k, want_centers=False):
     """-> (x_aug [B,3(+3),kN], centers [B,3,kN] or None)."""
     _chk(x, "x", torch.float32)

@@ -8,9 +8,12 @@ a cloud sampled by another tool, any [P, 3] array). Every SO-Net model reads a n
 2. Normals (estimate_normals): the unit normal of the plane fitted to each point's k neighbours, the
    eigenvector of the smallest eigenvalue of their covariance, in fp64. A PCA normal has no sign of
    its own: `orient` picks the rule (canonical, away from the cloud's centroid, or toward a
-   viewpoint per cloud). Centroid orientation is only right for roughly star-shaped objects; no
-   orientation is propagated over a neighbour graph.
-3. SOM nodes: the notebook's procedure (data/build_som/save_som.ipynb), n of each cloud's points
+   viewpoint per cloud). Centroid orientation is only right for roughly star-shaped objects.
+3. Orientation (orient_normals, or estimate_normals(orient="propagate")): signs propagated along
+   the minimum spanning tree of each cloud's k-NN graph (Hoppe et al. 1992), anchored once per
+   connected component, so that concave shapes (cups, chairs, the inner ring of a torus) get
+   consistent normals. Borůvka rounds on the device (csrc/point_normals.cu).
+4. SOM nodes: the notebook's procedure (data/build_som/save_som.ipynb), n of each cloud's points
    chosen without replacement, then BatchSOM(rows, cols).optimize, on ragged clouds.
 
 build_dataset chains them into an augmentation.DeviceDataset; save_npz writes the notebook's
@@ -27,6 +30,10 @@ from .som import BatchSOM
 
 _ORIENT = {None: ops.NORMALS_CANONICAL, "centroid": ops.NORMALS_AWAY_FROM_CENTROID,
            "viewpoint": ops.NORMALS_TOWARD_VIEWPOINT}
+# estimate_normals' tree rules: the canonical estimate, then orient_normals with this anchor
+_PROPAGATE = {"propagate": ops.NORMALS_AWAY_FROM_CENTROID,
+              "propagate-viewpoint": ops.NORMALS_TOWARD_VIEWPOINT}
+_ANCHOR = {"centroid": ops.NORMALS_AWAY_FROM_CENTROID, "viewpoint": ops.NORMALS_TOWARD_VIEWPOINT}
 
 
 def _check_k(k, what):
@@ -35,9 +42,9 @@ def _check_k(k, what):
     return int(k)
 
 
-def _check_input(data, offsets, what):
+def _check_input(data, offsets, what, min_points=3, need="a normal needs at least 3"):
     """The host copy of offsets, after checking data [T, >=3] f32 and offsets [S+1] i64 on one
-    CUDA device, the offsets within [0, T] and every cloud at least 3 points long."""
+    CUDA device, the offsets within [0, T] and every cloud at least min_points long."""
     if not (torch.is_tensor(data) and torch.is_tensor(offsets) and data.is_cuda and offsets.is_cuda):
         raise ValueError("%s: data and offsets must be CUDA tensors" % what)
     if data.dtype != torch.float32 or data.dim() != 2 or data.shape[1] < 3:
@@ -49,11 +56,30 @@ def _check_input(data, offsets, what):
     if off[0] < 0 or off[-1] > data.shape[0]:
         raise ValueError("%s: offsets must lie in [0, %d]" % (what, data.shape[0]))
     counts = np.diff(off)
-    if (counts < 3).any():
-        s = int(np.flatnonzero(counts < 3)[0])
-        raise ValueError("%s: cloud %d has %d points; a normal needs at least 3"
-                         % (what, s, int(counts[s])))
+    if (counts < min_points).any():
+        s = int(np.flatnonzero(counts < min_points)[0])
+        raise ValueError("%s: cloud %d has %d points; %s" % (what, s, int(counts[s]), need))
     return off
+
+
+def _viewpoint(viewpoint, S, device, what, orient):
+    """viewpoint as a [S, 3] f32 device tensor; ValueError when it is missing or misshapen."""
+    if viewpoint is None:
+        raise ValueError("%s: %s needs viewpoint [S, 3]" % (what, orient))
+    view = viewpoint if torch.is_tensor(viewpoint) else np.asarray(viewpoint, np.float32)
+    view = torch.as_tensor(view).to(device, torch.float32).contiguous()
+    if tuple(view.shape) != (S, 3):
+        raise ValueError("%s: viewpoint must be [%d, 3], got %s" % (what, S, tuple(view.shape)))
+    return view
+
+
+def _max_points(off, what):
+    """The largest cloud of the host offsets, which the orientation's round schedule needs."""
+    P = int(np.diff(off).max())
+    if P >= ops.POINT_ORIENT_MAX_POINTS:
+        raise ValueError("%s: a cloud of %d points; orientation supports at most %d"
+                         % (what, P, ops.POINT_ORIENT_MAX_POINTS - 1))
+    return P
 
 
 def knn(data, offsets, k):
@@ -70,31 +96,67 @@ def estimate_normals(data, offsets, k=16, orient="centroid", viewpoint=None, out
     """Unit surface normals [T, 3] f32 of every point of the ragged clouds data [T, >=3] f32 /
     offsets [S+1] i64 (CUDA tensors), from its k nearest neighbours within its cloud.
     orient: None (canonical: the component of largest magnitude is positive), "centroid" (pointing
-    away from the cloud's mean) or "viewpoint" (toward viewpoint [S, 3], one point per cloud, such as
-    the sensor's position). out: a [T, 3] f32 view to write into, such as data[:, 3:6]. With
+    away from the cloud's mean), "viewpoint" (toward viewpoint [S, 3], one point per cloud, such as
+    the sensor's position), or a sign propagated along the minimum spanning tree of the k-NN graph
+    (orient_normals on the canonical estimate, reusing its k-NN): "propagate" anchors each
+    component at its point farthest from the cloud's mean, "propagate-viewpoint" at its point
+    nearest viewpoint. out: a [T, 3] f32 view to write into, such as data[:, 3:6]. With
     want_curvature returns (normals, curvature [T]), the surface variation l0 / (l0 + l1 + l2). A
     degenerate neighbourhood (coincident or collinear points, non-finite coordinates) gives the zero
     vector and NaN curvature. Raises ValueError for k outside [3, 32], an unknown orient, a missing
     viewpoint, or a cloud with fewer than 3 points."""
     k = _check_k(k, "estimate_normals")
-    if not isinstance(orient, (str, type(None))) or orient not in _ORIENT:
-        raise ValueError("estimate_normals: orient=%r is not None, 'centroid' or 'viewpoint'"
-                         % (orient,))
+    if not isinstance(orient, (str, type(None))) or (orient not in _ORIENT and orient not in _PROPAGATE):
+        raise ValueError("estimate_normals: orient=%r is not None, 'centroid', 'viewpoint', "
+                         "'propagate' or 'propagate-viewpoint'" % (orient,))
     off = _check_input(data, offsets, "estimate_normals")
     view = None
-    if orient == "viewpoint":
-        if viewpoint is None:
-            raise ValueError("estimate_normals: orient='viewpoint' needs viewpoint [S, 3]")
-        view = viewpoint if torch.is_tensor(viewpoint) else np.asarray(viewpoint, np.float32)
-        view = torch.as_tensor(view).to(data.device, torch.float32).contiguous()
-        if tuple(view.shape) != (len(off) - 1, 3):
-            raise ValueError("estimate_normals: viewpoint must be [%d, 3], got %s"
-                             % (len(off) - 1, tuple(view.shape)))
+    if orient in ("viewpoint", "propagate-viewpoint"):
+        view = _viewpoint(viewpoint, len(off) - 1, data.device, "estimate_normals", "orient=%r" % orient)
     data, offsets = data.contiguous(), offsets.contiguous()
     idx, _ = ops.point_knn(data, offsets, k)
-    normals, curv = ops.estimate_normals(data, offsets, idx, _ORIENT[orient], view=view, out=out,
+    code = ops.NORMALS_CANONICAL if orient in _PROPAGATE else _ORIENT[orient]
+    normals, curv = ops.estimate_normals(data, offsets, idx, code, view=view, out=out,
                                          want_curvature=want_curvature)
+    if orient in _PROPAGATE:
+        ops.orient_normals(data, offsets, idx, normals, _PROPAGATE[orient], view=view,
+                           max_points=_max_points(off, "estimate_normals"))
     return (normals, curv) if want_curvature else normals
+
+
+def orient_normals(data, offsets, normals, k=16, anchor="centroid", viewpoint=None, idx=None,
+                   return_components=False):
+    """Orient the normals [T, 3] f32 (a CUDA view such as data[:, 3:6]; from a scanner, another
+    tool or estimate_normals) of the ragged clouds data [T, >=3] f32 / offsets [S+1] i64 in place,
+    consistently within each cloud: signs propagate along the minimum spanning tree of the k-NN
+    graph (weights 1 - |n_u . n_v|, Hoppe et al. 1992), and each connected component takes its
+    sign from one anchor point: anchor="centroid", its point farthest from the cloud's mean, made
+    to point away from it; anchor="viewpoint", its point nearest viewpoint [S, 3], made to point
+    toward it. idx: a [T, K] i32 cloud-local k-NN (knn's) to reuse, else knn(data, offsets, k).
+    Points with a non-finite coordinate or a zero or non-finite normal are left as they are.
+    A k-NN graph that bridges two close sheets (a thin wall) can carry a flip across them.
+    -> normals, or (normals, components [T] i32) with return_components: the cloud-local index
+    of each point's anchor, -1 for the points left out."""
+    if not isinstance(anchor, str) or anchor not in _ANCHOR:
+        raise ValueError("orient_normals: anchor=%r is not 'centroid' or 'viewpoint'" % (anchor,))
+    if idx is None:
+        k = _check_k(k, "orient_normals")
+    off = _check_input(data, offsets, "orient_normals", 1, "orienting needs at least 1")
+    S = len(off) - 1
+    view = None
+    if anchor == "viewpoint":
+        view = _viewpoint(viewpoint, S, data.device, "orient_normals", "anchor='viewpoint'")
+    data, offsets = data.contiguous(), offsets.contiguous()
+    if idx is None:
+        idx, _ = ops.point_knn(data, offsets, k)
+    elif not (torch.is_tensor(idx) and idx.is_cuda and idx.dtype == torch.int32 and idx.dim() == 2
+              and idx.shape[0] == data.shape[0] and 1 <= idx.shape[1] <= ops.POINT_KNN_MAX_K):
+        raise ValueError("orient_normals: idx must be a CUDA i32 [%d, K] tensor with K in [1, %d]"
+                         % (data.shape[0], ops.POINT_KNN_MAX_K))
+    normals, comp = ops.orient_normals(data, offsets, idx.contiguous(), normals, _ANCHOR[anchor],
+                                       view=view, max_points=_max_points(off, "orient_normals"),
+                                       want_component=return_components)
+    return (normals, comp) if return_components else normals
 
 
 def _to_device_rows(clouds, device):

@@ -4,8 +4,8 @@
 
 classifier (fused wgmma + pool at N=5000, graph replay), segmenter, auto-encoder (up-conv decoder,
 grouped / split-K GEMMs, Chamfer incl. the arg-min pass), BatchSOM training, augmentation,
-query_topk with the fused mask, standalone index_max, per-cloud k-NN and normal estimation, and one
-training step (BN / scatter / device pack kernels)."""
+query_topk with the fused mask, standalone index_max, per-cloud k-NN, normal estimation and
+orientation, and one training step (BN / scatter / device pack kernels)."""
 import os
 import sys
 
@@ -76,6 +76,8 @@ offs = torch.tensor([0, 100, 100, 1500], dtype=torch.int64, device=dev)
 nb, _ = ops.point_knn(pts, offs, 16)
 nrm, _ = ops.estimate_normals(pts, offs, nb, ops.NORMALS_AWAY_FROM_CENTROID, out=pts[:, 3:6])
 print("normals", int(nb.sum()), float(nrm.sum()))
+_, comp = ops.orient_normals(pts, offs, nb, pts[:, 3:6], ops.NORMALS_AWAY_FROM_CENTROID, want_component=True)
+print("orient", int(comp.sum()), float(pts[:, 3:6].sum()))
 m, a = build("classifier", 4, 256)
 m.set_input(*a)
 m.optimize()
