@@ -605,6 +605,24 @@ int sonet_kcopy_mean_f32(const float* in, int B, int C, int N, int k, float* out
 long long sonet_seg_loss_scratch_bytes(int B, int N);
 int sonet_seg_loss_f32(const float* score, const long long* target, int B, int C, int N,
                        int size_average, void* scratch, float* loss, sonet_stream_t stream);
+/* The same loss over whole shapes of any size (losses.seg_loss_ragged, INTEGRATION.md "Whole
+ * clouds: the segmenter"): score [T,C] f32 point-major, target [T] int64, cloud b is rows
+ * offsets[b] .. offsets[b+1] (offsets [B+1] int64 on the device, offsets_host the same values in
+ * host memory). loss: one float, the mean over every counted point of the batch (the rule of
+ * sonet_seg_loss_f32 with size_average=1: with equal sizes P it is that entry's bits on the scores
+ * laid out [B,C,P]); loss_array [B]: each cloud's own mean. Targets equal to -100 do not count; any
+ * other out-of-range target makes its cloud's mean and loss NaN, and no other cloud's; a cloud with
+ * no counted point has NaN in loss_array (0/0) and adds nothing to loss. Deterministic: fixed-order
+ * fp64 sums of 256-point tile partials. scratch: sonet_seg_loss_ragged_scratch_bytes(B, T) bytes of
+ * device memory; it also receives the clouds' tile-start prefix sums from the host (one pageable
+ * copy on the stream). Refused before any launch: B < 1, C < 1, T < 0, a null pointer,
+ * offsets_host not running from 0 to T without decreasing, a cloud of 2^31 - 256 points or more, 2^31
+ * partials or more. Device offsets that disagree with offsets_host are clamped into [0,T] (results
+ * unspecified, nothing out of range). No allocation, no host synchronisation. */
+long long sonet_seg_loss_ragged_scratch_bytes(int B, long long T);
+int sonet_seg_loss_ragged_f32(const float* score, const long long* target, const long long* offsets,
+                              const long long* offsets_host, int B, int C, long long T, void* scratch,
+                              float* loss, float* loss_array, sonet_stream_t stream);
 
 /* Part-segmentation IoU (models/losses.py:73-189 compute_iou_np_array / compute_iou, called by
  * part-seg/train.py:95). score [B,C,N] f32, seg [B,N] int64, label [B] int64; part table in CSR

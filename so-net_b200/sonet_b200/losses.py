@@ -4,7 +4,8 @@ ChamferLoss (losses.py:17-27, 192-296): the reference builds two Faiss IndexFlat
 round-trips through host numpy (losses.py:247-276). Here both nearest-neighbour searches of the
 whole batch, the sqrt(d^2 + 1e-8) terms and all means run on the device in four launches
 (csrc/chamfer.cu). No Faiss dependency. chamfer_ragged: the same numbers against whole
-ground-truth clouds of any size, for evaluation.
+ground-truth clouds of any size, for evaluation; seg_loss_ragged: CrossEntropyLossSeg's evaluation
+loss over whole shapes of any size (csrc/seg_loss.cu).
 
 compute_iou_np_array / compute_iou (losses.py:73-189), the part-segmentation metric of
 part-seg/train.py:95: one kernel for CUDA tensors, the same arithmetic in C++ for host tensors
@@ -120,6 +121,23 @@ def chamfer_ragged(predict_pc, points, offsets):
     r = ops.chamfer_ragged(predict_pc.detach().contiguous(), points.detach(), offsets)
     return ChamferRagged(r["loss"][2], r["loss"][0], r["loss"][1], r["fwd_arr"] + r["bwd_arr"],
                          r["fwd_arr"], r["bwd_arr"])
+
+
+def seg_loss_ragged(score, seg, offsets):
+    """CrossEntropyLossSeg's evaluation loss over whole shapes of any size: score [T,classes] (CUDA,
+    point-major, as segmenter.Model.segment_clouds and score_points return it), seg [T] int64 part
+    labels (-100: not counted), cloud b rows offsets[b] .. offsets[b+1]. Returns (loss,
+    loss_array): loss is the mean over every counted point of the batch, CrossEntropyLossSeg's rule
+    (with equal sizes, its bits on the [B,classes,N] scores); loss_array [B] is each shape's own
+    mean, so loss_array.mean() weighs every shape once whatever its size. An out-of-range label
+    other than -100 makes its shape's mean and loss NaN. Evaluation only: a score requiring a
+    gradient with grad mode on is refused."""
+    if torch.is_grad_enabled() and isinstance(score, torch.Tensor) and score.requires_grad:
+        raise RuntimeError("seg_loss_ragged is evaluation only: no gradient flows through it "
+                           "(call it under torch.no_grad() or on a detached score)")
+    if not isinstance(score, torch.Tensor) or not score.is_cuda:
+        raise RuntimeError("sonet_b200.seg_loss_ragged runs on CUDA tensors only (no CPU fallback)")
+    return ops.seg_loss_ragged(score.detach().contiguous(), seg.contiguous(), offsets.contiguous())
 
 
 def _seg_iou(score, seg, label, table=None, want_correct=False):

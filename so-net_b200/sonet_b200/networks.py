@@ -542,10 +542,13 @@ class Segmenter(nn.Module):
             out1 = self.layer1.instance_norm(out1)
         return self._tail(self.layer2(out1), k, N)
 
-    def _node_addend(self, n_pt, n_pp, node_first, node_knn, node_final, feature, label):
+    def _node_addend(self, n_pt, n_pp, node_first, node_knn, node_final, feature, label,
+                     zero_idx=None):
         """(addend, packed): layer 1's node- and cloud-level part [B,1024,M] (the node GEMM over
         cat(node_first, node_knn, node_final) plus the broadcast [B,1040] cloud GEMM) and the
-        packed split weights for _layer1_points."""
+        packed split weights for _layer1_points. zero_idx: the fp32 route's zero [B,M] int32
+        gather index, or None for the module's cached one (a caller that must not rebind the cache
+        a captured graph reads passes its own)."""
         B, M = node_first.shape[0], node_first.shape[2]
         packed = self._pack_layer1(
             n_pt, 16, n_pp, node_first.shape[1] + node_knn.shape[1] + node_final.shape[1])
@@ -565,7 +568,9 @@ class Segmenter(nn.Module):
             return addend, packed
         node_a = torch.cat((node_first, node_knn), dim=1).contiguous()
         addend = ops.pointwise_layer(node_a, w_node, None, None, False, x1=node_final.contiguous(),
-                                     addend=cloud_add, gidx=self._zero_idx(B, M, feature.device))
+                                     addend=cloud_add,
+                                    gidx=self._zero_idx(B, M, feature.device) if zero_idx is None
+                                    else zero_idx)
         return addend, packed
 
     def _layer1_points(self, pt, first_pn_out, addend, gidx, packed):

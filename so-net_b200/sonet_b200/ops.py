@@ -583,6 +583,41 @@ def seg_loss(score, target, size_average=True):
     return loss
 
 
+def seg_loss_ragged(score, target, offsets):
+    """seg_loss over whole shapes of any size: score [T,C] f32 point-major, target [T] int64,
+    offsets [B+1] int64 on score's device (cloud b is rows offsets[b] .. offsets[b+1]) -> (loss,
+    loss_array [B]): the mean NLL over every counted point of the batch (with equal sizes P,
+    seg_loss's bits on the scores laid out [B,C,P]) and each cloud's own mean (NaN for a cloud with
+    no counted point). Copies the offsets to the host (one synchronisation) and refuses bad offsets
+    before any launch."""
+    _chk(score, "score", torch.float32)
+    _chk(target, "target", torch.int64)
+    _chk(offsets, "offsets", torch.int64)
+    if score.dim() != 2 or score.shape[1] < 1 or tuple(target.shape) != (score.shape[0],):
+        raise RuntimeError("seg_loss_ragged: expected score [T,C] with C >= 1 and target [T], got "
+                           "%s and %s" % (tuple(score.shape), tuple(target.shape)))
+    if target.device != score.device or offsets.device != score.device:
+        raise RuntimeError("seg_loss_ragged: score, target and offsets must be on one device "
+                           "(got %s, %s, %s)" % (score.device, target.device, offsets.device))
+    T, C = score.shape
+    if offsets.dim() != 1 or offsets.numel() < 2:
+        raise RuntimeError("seg_loss_ragged: offsets must be [B+1] with B >= 1 (got %s)"
+                           % (tuple(offsets.shape),))
+    B = offsets.numel() - 1
+    off = ragged_offsets(offsets, T, B)
+    lib = _C.lib()
+    dev = score.device
+    with torch.cuda.device(dev):
+        scratch = torch.empty(int(lib.sonet_seg_loss_ragged_scratch_bytes(B, T)), dtype=torch.uint8,
+                              device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        loss_array = torch.empty((B,), dtype=torch.float32, device=dev)
+        _call("sonet_seg_loss_ragged_f32", _C.ptr(score), _C.ptr(target), _C.ptr(offsets),
+              off.ctypes.data, B, C, T, _C.ptr(scratch), _C.ptr(loss), _C.ptr(loss_array),
+              _stream(score), kernels=3)
+    return loss, loss_array
+
+
 # ShapeNetPart: category -> its part ids, in the reference's order (models/losses.py:74-91)
 SHAPENET_PART_TABLE = ((0, 1, 2, 3), (4, 5), (6, 7), (8, 9, 10, 11), (12, 13, 14, 15), (16, 17, 18),
                        (19, 20, 21), (22, 23), (24, 25, 26, 27), (28, 29), (30, 31, 32, 33, 34, 35),

@@ -7,8 +7,9 @@ test_model() and optimize(): _model_base.GraphedModel.
 """
 import torch
 
-from . import losses, networks, ops
+from . import augmentation, losses, networks, ops
 from ._model_base import ENCODER_SNAPSHOT, GraphedModel
+from .layers import tc_enabled
 
 
 class Model(GraphedModel):
@@ -156,7 +157,6 @@ class Model(GraphedModel):
                                % (self.input_pc.device, points.device))
         if chunk_rows is not None and chunk_rows < 1:
             raise RuntimeError("score_points: chunk_rows must be >= 1 (got %d)" % chunk_rows)
-        k = opt.k
         BN = B * self.input_pc.shape[2]      # the sampled forward's points: the layers' routes
         use_sn = opt.surface_normal == True  # noqa: E712
         with torch.no_grad():
@@ -165,17 +165,104 @@ class Model(GraphedModel):
             addend, packed = seg._node_addend(12 if use_sn else 9, 384, enc.first_pn_out_masked_max,
                                               enc.knn_feature_1, enc.final_pn_out, self.feature,
                                               self.input_label)
-            C, M = addend.shape[1], addend.shape[2]
-            addend_flat = addend.permute(1, 0, 2).reshape(1, C, B * M).contiguous()
             node = self.input_node.detach().to(torch.float32).contiguous()
-            score = torch.empty((T, opt.classes), dtype=torch.float32, device=points.device)
-            chunk = min(int(chunk_rows), T) if chunk_rows else self._default_chunk_rows(T)
-            q = self._ROW_QUANTUM
-            for r0 in range(0, T, max(chunk, 1)):
-                R = min(chunk, T - r0)
-                gidx, x_aug, pt = ops.seg_points_assign(points, offsets, node, enc.som_node, k,
-                                                        use_sn, r0, R, (R + q - 1) // q * q)
-                fpo = enc.first_pointnet(x_aug, route_rows=k * BN)
-                y = seg.forward_rows(pt, fpo, addend_flat, gidx, k, packed, BN)   # [1,classes,Rp]
-                score[r0:r0 + R].copy_(y[0, :, :R].t())
+            return self._point_head(points, offsets, node, enc.som_node, addend, packed, BN,
+                                    min(int(chunk_rows), T) if chunk_rows else None)
+
+    def segment_clouds(self, points, offsets, label, node, node_knn_I=None, seg=None,
+                       chunk_points=None):
+        """Part scores of EVERY point of whole shapes of any size, encoded from all of their points,
+        in eval mode: points [T,6] f32 (xyz | normal), offsets [B+1] int64 (cloud b is rows
+        offsets[b] .. offsets[b+1]), label [B] int64 category ids (the one-hot input), node [B,3,M]
+        the test-mode loader's SOM nodes (DeviceDataset.full_batch), node_knn_I [B,M,som_k] int64
+        or None to compute it with augmentation.som_knn, seg [T] int64 per-point part labels or
+        None. Returns a dict: score [T,classes] (row i: what score_segmenter [B,classes,N] holds
+        for a sampled point), feature [B,feature_num], and with seg the loss (the mean NLL over
+        every counted point, -100 not counted: CrossEntropyLossSeg's rule) and loss_array [B]
+        (each shape's own mean), else None for both.
+
+        Encoder.forward_ragged encodes every point of each cloud and returns the node-level
+        features; the per-point head of score_points then runs on them, with forward_ragged's
+        cluster means, and takes its routes from this batch's own T points (k*T columns for the
+        first PointResNet and layers 2-3, T for layers 4-5). With equal-size clouds, T = B*N and
+        every layer takes test_model()'s route: score and loss are its bits when test_model()
+        takes the group route for its cluster means, as forward_ragged does. chunk_points (default:
+        from the free device memory) bounds the encoder's runs of whole clouds and the head's row
+        chunks; neither changes a bit, and permuting the clouds permutes every output.
+
+        Reads no bound input and writes no attribute of the model: what test_model() left,
+        score_points on the bound batch and a captured eval graph stay as they were. Refused before
+        any launch: train mode, Encoder.check_ragged's cases (--normalization instance among
+        them), som_k < 2, a label or seg that is not [B] / [T] int64 on the model's device, and a
+        label outside the 16 categories."""
+        enc, head, opt = self.encoder, self.segmenter, self.opt
+        if enc.training or head.training:
+            raise RuntimeError("segment_clouds: the model is in train mode; call test_model() or "
+                               "eval() first")
+        enc.check_ragged(points, offsets, node, node_knn_I, chunk_points, what="segment_clouds")
+        if opt.som_k < 2:
+            raise RuntimeError("segment_clouds: needs the KNN module's node features (som_k >= 2)")
+        B, T, dev = node.shape[0], points.shape[0], points.device
+        for name, t, shape in (("label", label, (B,)), ("seg", seg, (T,))):
+            if t is None and name == "seg":
+                continue
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.int64 or tuple(t.shape) != shape:
+                raise RuntimeError("segment_clouds: %s must be an int64 tensor %s (got %s)" % (
+                    name, list(shape), (t.dtype, tuple(t.shape)) if isinstance(t, torch.Tensor)
+                    else type(t).__name__))
+            if t.device != dev:
+                raise RuntimeError("segment_clouds: %s must be on the model's device %s (got %s)"
+                                   % (name, dev, t.device))
+        lab = label.cpu()
+        if bool(((lab < 0) | (lab >= 16)).any()):
+            raise RuntimeError("segment_clouds: label holds a category outside [0, 16)")
+        use_sn = opt.surface_normal == True  # noqa: E712
+        with torch.no_grad():
+            if node_knn_I is None:
+                node_knn_I = augmentation.som_knn(node.detach().contiguous(), opt.som_k,
+                                                  node.shape[2])
+            feature, nodes = enc.forward_ragged(points, offsets, node, node_knn_I, chunk_points,
+                                                return_nodes=True)
+            M = node.shape[2]
+            # the fp32 route's zero gather index: its own, so that the cached one stays bound
+            zero_idx = None if tc_enabled() else torch.zeros((B, M), dtype=torch.int32, device=dev)
+            addend, packed = head._node_addend(12 if use_sn else 9, 384,
+                                               nodes["first_pn_out_masked_max"],
+                                               nodes["knn_feature_1"], nodes["final_pn_out"],
+                                               feature, label, zero_idx=zero_idx)
+            points = points.contiguous()
+            offsets = offsets.contiguous()
+            node = node.detach().contiguous()
+            chunk = min(int(chunk_points), T) if chunk_points else None
+            score = self._point_head(points, offsets, node, nodes["som_node"], addend, packed, T,
+                                     chunk)
+            loss = loss_array = None
+            if seg is not None:
+                loss, loss_array = losses.seg_loss_ragged(score, seg, offsets)
+        return dict(score=score, feature=feature, loss=loss, loss_array=loss_array)
+
+    def _point_head(self, points, offsets, node, cluster_mean, addend, packed, route_rows, chunk):
+        """The per-point head over rows of points [T,6] in chunks of `chunk` rows (None: from the
+        free device memory) -> score [T,classes]: each point assigned to its k nearest of its
+        cloud's loader nodes node [B,3,M], decentred by cluster_mean [B,3,M], then the first
+        PointResNet and Segmenter.forward_rows with the node/cloud addend [B,1024,M]. route_rows:
+        the point count whose routes the layers take (k*route_rows columns for the first
+        PointResNet and layers 2-3, route_rows for layers 4-5). Every layer computes each column
+        alone, so the chunking changes no bit."""
+        enc, seg, opt = self.encoder, self.segmenter, self.opt
+        k, T, B = opt.k, points.shape[0], node.shape[0]
+        use_sn = opt.surface_normal == True  # noqa: E712
+        C, M = addend.shape[1], addend.shape[2]
+        addend_flat = addend.permute(1, 0, 2).reshape(1, C, B * M).contiguous()
+        score = torch.empty((T, opt.classes), dtype=torch.float32, device=points.device)
+        if chunk is None:
+            chunk = self._default_chunk_rows(T)
+        q = self._ROW_QUANTUM
+        for r0 in range(0, T, max(chunk, 1)):
+            R = min(chunk, T - r0)
+            gidx, x_aug, pt = ops.seg_points_assign(points, offsets, node, cluster_mean, k, use_sn,
+                                                    r0, R, (R + q - 1) // q * q)
+            fpo = enc.first_pointnet(x_aug, route_rows=k * route_rows)
+            y = seg.forward_rows(pt, fpo, addend_flat, gidx, k, packed, route_rows)  # [1,classes,Rp]
+            score[r0:r0 + R].copy_(y[0, :, :R].t())
         return score

@@ -1,8 +1,9 @@
-"""Whole clouds of any size: classifier.Model.score_clouds (networks.Encoder.forward_ragged) and
-autoencoder.Model.reconstruct_clouds against the dense test_model() on the same clouds, and a batch
-of clouds of mixed sizes.
+"""Whole clouds of any size: classifier.Model.score_clouds (networks.Encoder.forward_ragged),
+autoencoder.Model.reconstruct_clouds and segmenter.Model.segment_clouds against the dense
+test_model() on the same clouds, and batches of clouds of mixed sizes.
 
-    python tools/ragged_bench.py [--reps 20] [--task all|classifier|autoencoder] [--out results.json]
+    python tools/ragged_bench.py [--reps 20] [--task all|classifier|autoencoder|segmenter]
+                                 [--out results.json]
 
   A  64 clouds x 10,000 points as one ragged batch, against dense test_model() at N = 10,000 and
      N = 5,000 on the same clouds (eager and with the eval CUDA graph).
@@ -14,6 +15,13 @@ of clouds of mixed sizes.
      decoder once over all features and the Chamfer terms against the whole clouds), the dense
      side at N = 10,000; AE_B splits the time into encoder, decoder and Chamfer (CUDA events
      around each stage) and gives the Chamfer's pair rate.
+
+  SEG_A  the segmenter on B = 32 shapes of 2,000 - 3,000 points (tools/seg_full_bench.py's shapes):
+     segment_clouds with its loss, against test_model() at N = 1,024 + score_points over every point
+     of the same shapes.
+  SEG_B  segment_clouds with its loss on 64 clouds x 10,000 points. Both split the time into the
+     ragged encoder, the per-point head (node/cloud addend and every point through the head) and
+     the ragged loss (CUDA events around each stage).
 
 Times are medians of --reps warm calls, each bracketed by CUDA events. Synthetic clouds and weights
 (synth.py), the default options of each task (k = 3, 8x8 SOM, som_k = 9; the auto-encoder's
@@ -171,7 +179,8 @@ def autoencoder_cases(res, reps):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--task", choices=("all", "classifier", "autoencoder"), default="all")
+    ap.add_argument("--task", choices=("all", "classifier", "autoencoder", "segmenter"),
+                    default="all")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -183,6 +192,8 @@ def main():
         autoencoder_cases(res, a.reps)
     if a.task in ("all", "classifier"):
         classifier_cases(res, a.reps)
+    if a.task in ("all", "segmenter"):
+        segmenter_cases(res, a.reps)
     print(json.dumps(res, indent=1))
     if a.out:
         with open(a.out, "w") as f:
@@ -227,6 +238,85 @@ def classifier_cases(res, reps):
     res["B_clouds_per_s"] = 1024 / (t[0] * 1e-3)
     res["B_points_per_s"] = float(sizes.sum()) / (t[0] * 1e-3)
     res["B_split_ms"] = stage_split(m, pts, off, node, knn)
+
+
+def seg_stage_split(m, pts, off, label, node, knn, seg, reps):
+    """Median device time of segment_clouds' three stages, each between CUDA events: the ragged
+    encoder, the per-point head (node/cloud addend + every point through the head) and the loss."""
+    from sonet_b200 import losses
+    enc, head, T = m.encoder, m.segmenter, pts.shape[0]
+    ts = {"encoder": [], "head": [], "loss": []}
+    for i in range(reps + 3):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        with torch.no_grad():
+            ev[0].record()
+            feat, nodes = enc.forward_ragged(pts, off, node, knn, return_nodes=True)
+            ev[1].record()
+            addend, packed = head._node_addend(12, 384, nodes["first_pn_out_masked_max"],
+                                               nodes["knn_feature_1"], nodes["final_pn_out"],
+                                               feat, label)
+            score = m._point_head(pts, off, node, nodes["som_node"], addend, packed, T, None)
+            ev[2].record()
+            losses.seg_loss_ragged(score, seg, off)
+            ev[3].record()
+        ev[3].synchronize()
+        if i >= 3:
+            for j, k in enumerate(ts):
+                ts[k].append(ev[j].elapsed_time(ev[j + 1]))
+    return {k: float(np.median(v)) for k, v in ts.items()}
+
+
+def segmenter_cases(res, reps):
+    import seg_full_bench
+    from sonet_b200 import segmenter
+    cpu_opt = synth.make_opt("segmenter")
+    states = (synth.synth_state_dict(networks.Encoder(cpu_opt), seed=1),
+              synth.synth_state_dict(networks.Segmenter(cpu_opt), seed=2))
+
+    def seg_model(B, N):
+        opt = synth.make_opt("segmenter", batch_size=B, input_pc_num=N, device=DEV)
+        m = segmenter.Model(opt)
+        m.encoder.load_state_dict(states[0])
+        m.segmenter.load_state_dict(states[1])
+        m.encoder.eval()
+        m.segmenter.eval()
+        return m
+
+    # ---- SEG_A: 32 shapes of 2,000 - 3,000 points, dense N = 1,024 + score_points ----
+    batch, h_pts, h_off, h_seg, sizes = seg_full_bench.make_case()
+    B, N = seg_full_bench.B, seg_full_bench.N
+    batch = [t.to(DEV) for t in batch]
+    pts, off = torch.from_numpy(h_pts).to(DEV), torch.from_numpy(h_off).to(DEV)
+    seg, label, node, knn = torch.from_numpy(h_seg).to(DEV), batch[2], batch[4], batch[5]
+    m = seg_model(B, N)
+    m.set_input(*batch)
+
+    def dense():
+        m.test_model()
+        m.score_points(pts, off)
+    res["SEG_A_points"] = int(sizes.sum())
+    res["SEG_A_dense_N%d_test_model_score_points_ms" % N] = median_ms(dense, reps)
+    res["SEG_A_ragged_ms"] = median_ms(
+        lambda: m.segment_clouds(pts, off, label, node, knn, seg=seg), reps)
+    res["SEG_A_split_ms"] = seg_stage_split(m, pts, off, label, node, knn, seg, reps)
+    del m
+    torch.cuda.empty_cache()
+
+    # ---- SEG_B: 64 clouds x 10,000 points ----
+    B, P, M = 64, 10000, 64
+    pts, off, node = clouds([P] * B, M, seed=0)
+    knn = augmentation.som_knn(node, 9, M)
+    rs = np.random.RandomState(3)
+    label = torch.from_numpy(rs.randint(0, 16, size=B).astype(np.int64)).to(DEV)
+    seg = torch.from_numpy(np.concatenate([rs.choice(ops.SHAPENET_PART_TABLE[l], size=P)
+                                           for l in label.tolist()])).to(DEV)
+    m = seg_model(1, 256)
+    t = median_ms(lambda: m.segment_clouds(pts, off, label, node, knn, seg=seg), reps)
+    res["SEG_B_ragged_64x10000_ms"] = t
+    res["SEG_B_points_per_s"] = B * P / (t[0] * 1e-3)
+    res["SEG_B_split_ms"] = seg_stage_split(m, pts, off, label, node, knn, seg, reps)
+    del m
+    torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":

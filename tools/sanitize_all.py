@@ -59,6 +59,9 @@ pts = torch.rand(1 + 1100 + 2500, 6, device=dev, generator=g)
 off = torch.tensor([0, 1, 1101, 3601], dtype=torch.int64, device=dev)
 r = ops.chamfer_ragged(torch.rand(3, 3, 300, device=dev, generator=g), pts, off, want_idx=True)
 print("chamfer_ragged idx", int(r["idx_fwd"].sum()), int(r["idx_bwd"].sum()))
+tgt = torch.randint(0, 50, (3601,), device=dev, generator=g)
+loss, arr = ops.seg_loss_ragged(torch.randn(3601, 50, device=dev, generator=g), tgt, off)
+print("seg_loss_ragged", float(loss), float(arr.sum()))
 x = torch.rand(2, 3, 1000, device=dev, generator=g) * 2 - 1
 s = som.BatchSOM(8, 8, 3, 0, 2)
 s.optimize(x)
