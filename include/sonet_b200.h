@@ -215,6 +215,39 @@ int sonet_bn_sync_backward_f32(const double* rec, const float* dy, const float* 
                                sonet_stream_t stream);
 int sonet_index_max_backward_f32(const float* grad_out, const int32_t* idx, int B, int C, int N, int K,
                                  float* grad_data, sonet_stream_t stream);
+/* Train-mode BatchNorm of a ragged batch: x [C, ld] is a [1,C,L] layer output whose cloud b owns the
+ * columns col_offsets[b] .. col_offsets[b+1] (device int64 [B+1], from 0 to L; k*offsets for the
+ * first PointResNet's stacked copies). The statistics cover all L columns, so a cloud weighs its size.
+ *   sonet_bn_cloud_partials_ragged_f32: record (b, c) of row c's columns of cloud b, into rec
+ *     [B,C,SONET_BN_REC_FWD | _BWD]: the dense record of that row at P = its length, with the same
+ *     pivot, walk and warp / CTA pattern (length 1: a thread; <= 1024: a warp; longer: a CTA).
+ *   sonet_bn_ragged_forward_f32 / _backward_f32: the B records folded in ascending cloud order, record
+ *     b standing for its own n_b = col_offsets[b+1] - col_offsets[b] values in the shift identity of
+ *     sonet_bn_sync_forward_f32, over n = L values; then y = act(BN(x)) / dx, dgamma, dbeta over
+ *     [1,C,L] (ld = L) with 1/n = 1/L. With B equal lengths P every output is the dense entries' bits.
+ * The device clamps offsets into [0, ld] (common.cuh); callers refuse empty ranges and offsets that do
+ * not run from 0 to L. Fail with SONET_ERR_BAD_ARG before any CUDA call for a null pointer, B or C
+ * outside [1, 65535], L (ld) outside [1, 2^31) or an unknown activation code.
+ *   sonet_index_max_ragged_backward_f32: the backward of sonet_index_max_ragged_f32's gather:
+ *     grad [C, ld] = 0, then grad[c, col_offsets[b] + idx[b,c,m]] += grad_out[b,c,m], m ascending, one
+ *     thread per (b, c) (index_max_backward's order), idx clamped into the cloud's columns. grad_out,
+ *     idx [B,C,M]; M in [1, 256]. */
+int sonet_bn_cloud_partials_ragged_f32(const float* x, const float* dy, const float* mean,
+                                       const float* invstd, const float* gamma, const float* beta,
+                                       int C, long long ld, const long long* col_offsets, int B,
+                                       int act, int backward, double* rec, sonet_stream_t stream);
+int sonet_bn_ragged_forward_f32(const double* rec, const long long* col_offsets, int B, const float* x,
+                                const float* gamma, const float* beta, int C, long long L, float eps,
+                                int act, float* y, float* mean, float* var, float* invstd,
+                                sonet_stream_t stream);
+int sonet_bn_ragged_backward_f32(const double* rec, const long long* col_offsets, int B,
+                                 const float* dy, const float* x, const float* mean,
+                                 const float* invstd, const float* gamma, const float* beta, int C,
+                                 long long L, int act, float* dx, float* dgamma, float* dbeta,
+                                 sonet_stream_t stream);
+int sonet_index_max_ragged_backward_f32(const float* grad_out, const int32_t* idx,
+                                        const long long* col_offsets, int B, int C, int M,
+                                        long long ld, float* grad, sonet_stream_t stream);
 /* Instance normalisation, nn.InstanceNorm1d/2d(C, affine=True) with track_running_stats=False
  * (models/layers.py:133, 179, 257): eval and train compute the same forward. For each
  * row r = b*C + c of z [B,C,P] (P = points, neighbour slots or pixels), the biased mean and
@@ -375,6 +408,18 @@ int sonet_augment_f32(const float* pc, const float* sn, const float* som, int B,
                       double clip_sn, double sigma_som, double clip_som, const double* noise_pc,
                       const double* noise_sn, const double* noise_som, unsigned long long seed,
                       float* pc_out, float* sn_out, float* som_out, sonet_stream_t stream);
+/* sonet_augment_ragged_f32: sonet_augment_f32's per-point arithmetic over whole clouds: points [T, ld]
+ * (ld >= 6) rows xyz | normal, cloud b the rows offsets[b] .. offsets[b+1] (device int64 [B+1],
+ * clamped into [0, T]), and som [B,3,M] (nullable with som_out). rot1, rot2, scale, shift as there,
+ * per cloud; the shift skips the normals. The jitter is always drawn in the kernel, keyed by (seed,
+ * cloud, array, cloud-local row): cloud b's row n gets the draws of point n of cloud b in
+ * sonet_augment_f32. Writes points_out [T, 6] and som_out. B in [1, 65535], T < 2^31. */
+int sonet_augment_ragged_f32(const float* points, long long T, int ld, const long long* offsets, int B,
+                             const float* som, int M, const double* rot1, const double* rot2,
+                             const double* scale, const double* shift, double sigma_pc,
+                             double clip_pc, double sigma_sn, double clip_sn, double sigma_som,
+                             double clip_som, unsigned long long seed, float* points_out,
+                             float* som_out, sonet_stream_t stream);
 
 /* ---- f-3: the loader's random choice of points, from a dataset in device memory ----------------
  * Replaces the head of the loaders' __getitem__ for a whole batch: np.random.choice(P, N,

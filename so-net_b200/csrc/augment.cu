@@ -17,6 +17,8 @@
 // stream, used by the parity tests) or from an in-kernel counter-based generator
 // (Philox4x32-10 + Box-Muller, keyed by seed / cloud / array / point) for production loaders,
 // where shipping 11 doubles per point from the host would cost more than the augmentation.
+#include <algorithm>
+
 #include "common.cuh"
 #include "philox.cuh"
 
@@ -69,7 +71,49 @@ __device__ __forceinline__ void rot_apply(const double* __restrict__ R, double (
   v[0] = o[0]; v[1] = o[1]; v[2] = o[2];
 }
 
-__global__ void __launch_bounds__(256) augment_kernel(AugParams p) {
+// rotations, jitter, scale and shift of one 3-vector v: element n of array `which` of cloud b
+__device__ __forceinline__ void augment_vec(const AugParams& p, const AugArray& a, const double (&sR)[2][9],
+                                            const double (&sS)[4], int b, int which, int n,
+                                            double (&v)[3]) {
+  if (p.rot1) rot_apply(sR[0], v);
+  if (p.rot2) rot_apply(sR[1], v);
+  if (a.sigma > 0.0) {
+    double g[3];
+    if (a.noise) {
+      const double* gp = a.noise + (static_cast<size_t>(b) * a.P + n) * 3;
+      g[0] = gp[0]; g[1] = gp[1]; g[2] = gp[2];
+    } else {
+      normal3(p.seed, static_cast<uint32_t>(b), static_cast<uint32_t>(which),
+              static_cast<uint32_t>(n), g);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const double j = fmin(fmax(__dmul_rn(a.sigma, g[c]), -a.clip), a.clip);
+      v[c] = __dadd_rn(j, v[c]);
+    }
+  }
+  if (p.scale) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = __dmul_rn(v[c], sS[3]);
+  }
+  if (p.shiftv && a.shift) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = __dadd_rn(v[c], sS[c]);
+  }
+}
+
+// Ragged clouds (sonet_augment_ragged_f32): arrays 0 and 1 are the columns 0-2 and 3-5 of the rows
+// offsets[b] .. offsets[b+1] of points [T, ld], written to rows of 6; row n of cloud b is its point n
+// (the Philox key's cloud-local index). The SOM nodes stay [B,3,M] planes.
+struct AugRows {
+  const long long* offsets;
+  long long T;
+  int ld;
+};
+
+// Rows: none, every array [B,3,P] planes; or one AugRows, the ragged points
+template <class... Rows>
+__global__ void __launch_bounds__(256) augment_kernel(AugParams p, Rows... rows) {
   const int b = blockIdx.y;
   const int which = blockIdx.z;
   const AugArray a = p.a[which];
@@ -85,37 +129,33 @@ __global__ void __launch_bounds__(256) augment_kernel(AugParams p) {
     sS[3] = p.scale ? p.scale[b] : 1.0;
   }
   __syncthreads();
+  if constexpr (sizeof...(Rows) == 1) {
+    if (which < 2) {
+      const AugRows r = (rows, ...);
+      long long lo, hi;
+      ragged_range(r.offsets, b, r.T, lo, hi);
+      const int P = static_cast<int>(hi - lo);
+      const float* in = a.in + lo * r.ld;
+      float* out = a.out + lo * 6;
+      for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < P; n += gridDim.x * blockDim.x) {
+        const float* q = in + static_cast<long long>(n) * r.ld;
+        double v[3] = {static_cast<double>(q[0]), static_cast<double>(q[1]), static_cast<double>(q[2])};
+        augment_vec(p, a, sR, sS, b, which, n, v);
+        float* o = out + static_cast<long long>(n) * 6;
+        o[0] = static_cast<float>(v[0]);
+        o[1] = static_cast<float>(v[1]);
+        o[2] = static_cast<float>(v[2]);
+      }
+      return;
+    }
+  }
   const int P = a.P;
   const float* in = a.in + static_cast<size_t>(b) * 3 * P;
   float* out = a.out + static_cast<size_t>(b) * 3 * P;
   for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < P; n += gridDim.x * blockDim.x) {
     double v[3] = {static_cast<double>(in[n]), static_cast<double>(in[P + n]),
                    static_cast<double>(in[2 * P + n])};
-    if (p.rot1) rot_apply(sR[0], v);
-    if (p.rot2) rot_apply(sR[1], v);
-    if (a.sigma > 0.0) {
-      double g[3];
-      if (a.noise) {
-        const double* gp = a.noise + (static_cast<size_t>(b) * P + n) * 3;
-        g[0] = gp[0]; g[1] = gp[1]; g[2] = gp[2];
-      } else {
-        normal3(p.seed, static_cast<uint32_t>(b), static_cast<uint32_t>(which),
-                static_cast<uint32_t>(n), g);
-      }
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const double j = fmin(fmax(__dmul_rn(a.sigma, g[c]), -a.clip), a.clip);
-        v[c] = __dadd_rn(j, v[c]);
-      }
-    }
-    if (p.scale) {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) v[c] = __dmul_rn(v[c], sS[3]);
-    }
-    if (p.shiftv && a.shift) {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) v[c] = __dadd_rn(v[c], sS[c]);
-    }
+    augment_vec(p, a, sR, sS, b, which, n, v);
     out[n] = static_cast<float>(v[0]);
     out[P + n] = static_cast<float>(v[1]);
     out[2 * P + n] = static_cast<float>(v[2]);
@@ -156,4 +196,37 @@ extern "C" int sonet_augment_f32(const float* pc, const float* sn, const float* 
   if (gx > 64) gx = 64;
   augment_kernel<<<dim3(gx, B, 3), 256, 0, as_stream(stream)>>>(p);
   return check_launch("augment");
+}
+
+extern "C" int sonet_augment_ragged_f32(const float* points, long long T, int ld, const long long* offsets,
+                                        int B, const float* som, int M, const double* rot1,
+                                        const double* rot2, const double* scale, const double* shift,
+                                        double sigma_pc, double clip_pc, double sigma_sn, double clip_sn,
+                                        double sigma_som, double clip_som, unsigned long long seed,
+                                        float* points_out, float* som_out, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE(B >= 1 && B <= 65535, "augment_ragged: B=%d outside [1, 65535]", B);
+  SONET_REQUIRE(T >= 0 && T < (1LL << 31) && M >= 0, "augment_ragged: bad dimension T=%lld M=%d", T, M);
+  SONET_REQUIRE(ld >= 6, "augment_ragged: row stride %d below the 6 columns (xyz | normal)", ld);
+  SONET_REQUIRE(offsets && (T == 0 || (points && points_out)), "augment_ragged: null pointer");
+  SONET_REQUIRE((som == nullptr) == (som_out == nullptr), "augment_ragged: som and som_out go together");
+  SONET_REQUIRE(points != points_out || T == 0 || ld == 6,
+                "augment_ragged: points_out may alias points only with ld = 6");
+  SONET_REQUIRE((sigma_pc <= 0 || clip_pc > 0) && (sigma_sn <= 0 || clip_sn > 0) &&
+                    (sigma_som <= 0 || clip_som > 0),
+                "augment_ragged: clip must be > 0 (data/augmentation.py:140)");
+  AugParams p;
+  p.a[0] = AugArray{T ? points : nullptr, points_out, nullptr, 0, sigma_pc, clip_pc, 1};
+  p.a[1] = AugArray{T ? points + 3 : nullptr, points_out + 3, nullptr, 0, sigma_sn, clip_sn, 0};
+  p.a[2] = AugArray{M ? som : nullptr, som_out, nullptr, M, sigma_som, clip_som, 1};
+  p.rot1 = rot1;
+  p.rot2 = rot2;
+  p.scale = scale;
+  p.shiftv = shift;
+  p.seed = seed;
+  const long long rows = std::max<long long>((T + B - 1) / B, M);
+  if (rows == 0) return SONET_OK;
+  const int gx = static_cast<int>(std::min<long long>((rows + 255) / 256, 64));
+  augment_kernel<<<dim3(gx, B, 3), 256, 0, as_stream(stream)>>>(p, AugRows{offsets, T, ld});
+  return check_launch("augment_ragged");
 }

@@ -29,6 +29,7 @@
 // All reductions are two-stage with fp64 partial sums in a fixed order: bit-reproducible.
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 
 #include "tc_common.cuh"
 
@@ -248,13 +249,48 @@ static void launch_instance_norm_red(int reduce, const float* z, const float* ga
                                                  save_invstd, st);
 }
 
-// grad_data[b,c,idx[b,c,k]] += grad_out[b,c,k], k ascending, one thread per (b,c) row
+// Where row r = b*C + c of a launch over x lies and how long it is, from the extent argument
+// `ext` of the kernel. Dense x [B,C,P]: ext = P, row r at r*P, P long. Ragged x [C, ld] (a [1,C,L]
+// layer output of a ragged batch): ext = RaggedCols, cloud b owns the columns cols[b] .. cols[b+1]
+// (clamped into [0, ld] like common.cuh's ragged_range), so row (b, c) starts at c*ld + cols[b]. The
+// ragged record launch runs all three record kernels over every row; each takes the rows of its own
+// length class, the dense launch's choice at P = the row's length.
+struct RaggedCols {
+  int C;
+  long long ld;
+  const long long* cols;
+};
+template <class Ext> constexpr bool kRaggedExt = !std::is_same<Ext, int>::value;
+__device__ __forceinline__ long long row_start(int P, long long r) { return r * P; }
+__device__ __forceinline__ int row_len(int P, long long) { return P; }
+__device__ __forceinline__ void row_range(const RaggedCols& e, long long r, long long& lo,
+                                          long long& hi) {
+  ragged_range(e.cols, static_cast<int>(r / e.C), e.ld, lo, hi);
+}
+__device__ __forceinline__ long long row_start(const RaggedCols& e, long long r) {
+  long long lo, hi;
+  row_range(e, r, lo, hi);
+  return (r % e.C) * e.ld + lo;
+}
+__device__ __forceinline__ int row_len(const RaggedCols& e, long long r) {
+  long long lo, hi;
+  row_range(e, r, lo, hi);
+  return static_cast<int>(hi - lo);
+}
+
+// grad_data[b,c,idx[b,c,k]] += grad_out[b,c,k], k ascending, one thread per (b,c) row, idx clamped
+// into the row. ext: N (grad_data [B,C,N]) or RaggedCols (grad [C, ld], row_start's layout)
+template <class Ext = int>
 __global__ void __launch_bounds__(128)
     index_max_backward_kernel(const float* __restrict__ grad_out, const int32_t* __restrict__ idx,
-                              long long rows, int N, int K, float* __restrict__ grad_data) {
+                              long long rows, Ext ext, int K, float* __restrict__ grad_data) {
   const long long r = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (r >= rows) return;
-  float* g = grad_data + r * N;
+  const int N = row_len(ext, r);
+  if constexpr (kRaggedExt<Ext>) {
+    if (N < 1) return;
+  }
+  float* g = grad_data + row_start(ext, r);
   const float* go = grad_out + r * K;
   const int32_t* ix = idx + r * K;
   for (int k = 0; k < K; ++k) {
@@ -440,12 +476,13 @@ struct BncRow {
   const float *xr, *gr;
   float mu, is, ga, be;
   double pivot;
+  template <class Ext>
   __device__ __forceinline__ BncRow(const float* x, const float* dy, const float* mean,
                                     const float* invstd, const float* gamma, const float* beta,
-                                    long long r, int C, int P) {
+                                    long long r, int C, Ext ext) {
     const int c = static_cast<int>(r % C);
-    xr = x + r * P;
-    gr = BWD ? dy + r * P : nullptr;
+    xr = x + row_start(ext, r);
+    gr = BWD ? dy + row_start(ext, r) : nullptr;
     mu = BWD ? mean[c] : 0.f;
     is = BWD ? invstd[c] : 1.f;
     ga = BWD && gamma ? gamma[c] : 1.f;
@@ -478,32 +515,50 @@ struct BncRow {
   }
 };
 
-// P == 1 (MyLinear's [B,C,1] view): a thread per row, consecutive threads on consecutive channels
-template <bool BWD, int ACT>
+// the point kernel's dense rows are one value long whatever its P argument says
+__device__ __forceinline__ int point_ext(int) { return 1; }
+__device__ __forceinline__ const RaggedCols& point_ext(const RaggedCols& e) { return e; }
+
+// P == 1 (MyLinear's [B,C,1] view): a thread per row, consecutive threads on consecutive channels.
+// A ragged row of no columns (refused by the callers) gets the record of nothing, all zeros.
+template <bool BWD, int ACT, class Ext = int>
 __global__ void __launch_bounds__(256)
     bn_cloud_point_kernel(const float* __restrict__ x, const float* __restrict__ dy,
                           const float* __restrict__ mean, const float* __restrict__ invstd,
                           const float* __restrict__ gamma, const float* __restrict__ beta, long long R,
-                          int C, double* __restrict__ rec) {
+                          int C, Ext ext, double* __restrict__ rec) {
   const long long r = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (r >= R) return;
-  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, 1);
+  if constexpr (kRaggedExt<Ext>) {
+    const int P = row_len(ext, r);
+    if (P > 1) return;
+    if (P == 0) {
+      for (int i = 0; i < (BWD ? SONET_BN_REC_BWD : SONET_BN_REC_FWD); ++i)
+        rec[r * (BWD ? SONET_BN_REC_BWD : SONET_BN_REC_FWD) + i] = 0.0;
+      return;
+    }
+  }
+  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, point_ext(ext));
   double a0 = 0.0, a1 = 0.0;
   row.add(0, a0, a1);
   row.store(rec, r, a0, a1);
 }
 
 // 1 < P <= BNC_WARP_P: warp w of the CTA owns row 8*blockIdx.x + w; lanes take p = lane, lane+32, ...
-template <bool BWD, int ACT>
+template <bool BWD, int ACT, class Ext = int>
 __global__ void __launch_bounds__(256)
     bn_cloud_warp_kernel(const float* __restrict__ x, const float* __restrict__ dy,
                          const float* __restrict__ mean, const float* __restrict__ invstd,
                          const float* __restrict__ gamma, const float* __restrict__ beta, long long R,
-                         int C, int P, double* __restrict__ rec) {
+                         int C, Ext ext, double* __restrict__ rec) {
   const long long r = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (r >= R) return;                                   // warp-uniform
-  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, P);
+  const int P = row_len(ext, r);
+  if constexpr (kRaggedExt<Ext>) {
+    if (P <= 1 || P > BNC_WARP_P) return;               // warp-uniform
+  }
+  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, ext);
   double a0 = 0.0, a1 = 0.0;
   for (int p = lane; p < P; p += 32) row.add(p, a0, a1);
   a0 = in_warp_sum(a0);
@@ -513,16 +568,20 @@ __global__ void __launch_bounds__(256)
 
 // P > BNC_WARP_P: CTA blockIdx.x owns row r; thread t takes p = t, t+256, ..., then the warp
 // butterfly and the 8 warp sums in ascending order
-template <bool BWD, int ACT>
+template <bool BWD, int ACT, class Ext = int>
 __global__ void __launch_bounds__(256)
     bn_cloud_cta_kernel(const float* __restrict__ x, const float* __restrict__ dy,
                         const float* __restrict__ mean, const float* __restrict__ invstd,
-                        const float* __restrict__ gamma, const float* __restrict__ beta, int C, int P,
+                        const float* __restrict__ gamma, const float* __restrict__ beta, int C, Ext ext,
                         double* __restrict__ rec) {
   static_assert(IN_THREADS == 256, "in_block_sum sums 8 warps");
   __shared__ double red[IN_THREADS / 32];
   const long long r = blockIdx.x;
-  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, P);
+  if constexpr (kRaggedExt<Ext>) {
+    if (row_len(ext, r) <= BNC_WARP_P) return;          // CTA-uniform, before any barrier
+  }
+  const BncRow<BWD, ACT> row(x, dy, mean, invstd, gamma, beta, r, C, ext);
+  const int P = row_len(ext, r);
   double a0 = 0.0, a1 = 0.0;
   for (int p = threadIdx.x; p < P; p += IN_THREADS) row.add(p, a0, a1);
   a0 = in_block_sum(a0, red);
@@ -536,7 +595,7 @@ static void launch_bn_cloud(const float* x, const float* dy, const float* mean, 
                             double* rec, cudaStream_t st) {
   if (P == 1)
     bn_cloud_point_kernel<BWD, ACT><<<static_cast<unsigned>((R + 255) / 256), 256, 0, st>>>(
-        x, dy, mean, invstd, gamma, beta, R, C, rec);
+        x, dy, mean, invstd, gamma, beta, R, C, P, rec);
   else if (P <= BNC_WARP_P)
     bn_cloud_warp_kernel<BWD, ACT><<<static_cast<unsigned>((R + 7) / 8), 256, 0, st>>>(
         x, dy, mean, invstd, gamma, beta, R, C, P, rec);
@@ -545,25 +604,60 @@ static void launch_bn_cloud(const float* x, const float* dy, const float* mean, 
         x, dy, mean, invstd, gamma, beta, C, P, rec);
 }
 
+// the ragged rows have every length: all three kernels run, each on the rows of its class
+template <bool BWD, int ACT>
+static void launch_bn_cloud_ragged(const float* x, const float* dy, const float* mean,
+                                   const float* invstd, const float* gamma, const float* beta, int B,
+                                   int C, long long ld, const long long* cols, double* rec,
+                                   cudaStream_t st) {
+  const long long R = static_cast<long long>(B) * C;
+  const RaggedCols ext{C, ld, cols};
+  bn_cloud_point_kernel<BWD, ACT><<<static_cast<unsigned>((R + 255) / 256), 256, 0, st>>>(
+      x, dy, mean, invstd, gamma, beta, R, C, ext, rec);
+  bn_cloud_warp_kernel<BWD, ACT><<<static_cast<unsigned>((R + 7) / 8), 256, 0, st>>>(
+      x, dy, mean, invstd, gamma, beta, R, C, ext, rec);
+  bn_cloud_cta_kernel<BWD, ACT><<<static_cast<unsigned>(R), IN_THREADS, 0, st>>>(
+      x, dy, mean, invstd, gamma, beta, C, ext, rec);
+}
+
+// How many values record b of a fold stands for, and n, their total. Dense: P each, Bg*P in all.
+// Ragged: cloud b's own column count cols[b+1] - cols[b] (clamped into [0, L]), L in all.
+struct DenseCounts {
+  int P;
+  __device__ __forceinline__ double count(int) const { return static_cast<double>(P); }
+  __device__ __forceinline__ double total(int Bg) const { return static_cast<double>(Bg) * P; }
+};
+struct RaggedCounts {
+  const long long* cols;
+  long long L;
+  __device__ __forceinline__ double count(int b) const {
+    long long lo, hi;
+    ragged_range(cols, b, L, lo, hi);
+    return static_cast<double>(hi - lo);
+  }
+  __device__ __forceinline__ double total(int) const { return static_cast<double>(L); }
+};
+
 // the forward records of Bg clouds, ascending, onto cloud 0's pivot p; then mean = p + E[x - p] and
-// the biased var = E[(x - p)^2] - E[x - p]^2 (F.batch_norm normalises with it). Shifting record b by
-// s = p_b - p (exact: both are fp32 values) is the identity
-// sum (x - p) = sum d_b + P s, sum (x - p)^2 = sum d_b^2 + 2 s sum d_b + P s^2.
-__global__ void bn_sync_stats_kernel(const double* __restrict__ rec, int Bg, int C, int P, float eps,
-                                     float* __restrict__ mean, float* __restrict__ var,
+// the biased var = E[(x - p)^2] - E[x - p]^2 (F.batch_norm normalises with it). Shifting record b of
+// n_b values by s = p_b - p (exact: both are fp32 values) is the identity
+// sum (x - p) = sum d_b + n_b s, sum (x - p)^2 = sum d_b^2 + 2 s sum d_b + n_b s^2.
+template <class Counts>
+__global__ void bn_sync_stats_kernel(const double* __restrict__ rec, int Bg, int C, Counts cnt,
+                                     float eps, float* __restrict__ mean, float* __restrict__ var,
                                      float* __restrict__ invstd) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const double p = rec[static_cast<size_t>(c) * SONET_BN_REC_FWD];
-  const double nb = static_cast<double>(P);
   double s1 = 0.0, s2 = 0.0;
   for (int b = 0; b < Bg; ++b) {
+    const double nb = cnt.count(b);
     const double* q = rec + (static_cast<size_t>(b) * C + c) * SONET_BN_REC_FWD;
     const double s = q[0] - p;
     s1 += q[1] + nb * s;
     s2 += q[2] + 2.0 * s * q[1] + nb * s * s;
   }
-  const double n = static_cast<double>(Bg) * P;
+  const double n = cnt.total(Bg);
   const double md = s1 / n;                                        // mean - pivot
   double v = s2 / n - md * md;
   if (v < 0.0) v = 0.0;
@@ -620,7 +714,8 @@ extern "C" int sonet_bn_sync_forward_f32(const double* rec, const float* x, cons
                 "bn_sync_forward: bad dims Bg=%d B=%d C=%d P=%d", Bg, B, C, P);
   SONET_REQUIRE(rec && x && y && mean && var && invstd, "bn_sync_forward: null pointer");
   cudaStream_t st = as_stream(stream);
-  bn_sync_stats_kernel<<<(C + 127) / 128, 128, 0, st>>>(rec, Bg, C, P, eps, mean, var, invstd);
+  bn_sync_stats_kernel<<<(C + 127) / 128, 128, 0, st>>>(rec, Bg, C, DenseCounts{P}, eps, mean, var,
+                                                     invstd);
   const dim3 grid((P + 1023) / 1024, C, B);
   if (act == SONET_ACT_ELU)
     bn_apply_kernel<true><<<grid, 256, 0, st>>>(x, mean, invstd, gamma, beta, C, P, 0, y);
@@ -650,6 +745,84 @@ extern "C" int sonet_bn_sync_backward_f32(const double* rec, const float* dy, co
     bn_bwd_apply_kernel<false><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
                                                      act, inv_n, dx);
   return check_launch("bn_sync_backward");
+}
+
+// ---- ragged batches: x [C, L], cloud b owning the columns cols[b] .. cols[b+1] ---------------------
+static int bn_ragged_dims(const char* what, int B, int C, long long L) {
+  using namespace sonet;
+  SONET_REQUIRE(B >= 1 && C >= 1 && B <= 65535 && C <= 65535, "%s: bad dims B=%d C=%d", what, B, C);
+  SONET_REQUIRE(L >= 1 && L < (1LL << 31), "%s: L=%lld columns outside [1, 2^31)", what, L);
+  return SONET_OK;
+}
+
+extern "C" int sonet_bn_cloud_partials_ragged_f32(const float* x, const float* dy, const float* mean,
+                                                  const float* invstd, const float* gamma,
+                                                  const float* beta, int C, long long ld,
+                                                  const long long* col_offsets, int B, int act,
+                                                  int backward, double* rec, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(act, "bn_cloud_partials_ragged");
+  if (int rc = bn_ragged_dims("bn_cloud_partials_ragged", B, C, ld)) return rc;
+  SONET_REQUIRE(x && col_offsets && rec && (!backward || (dy && mean && invstd)),
+                "bn_cloud_partials_ragged: null pointer");
+  cudaStream_t st = as_stream(stream);
+  if (!backward)
+    launch_bn_cloud_ragged<false, SONET_ACT_NONE>(x, nullptr, nullptr, nullptr, nullptr, nullptr, B, C,
+                                                  ld, col_offsets, rec, st);
+  else if (act == SONET_ACT_ELU)
+    launch_bn_cloud_ragged<true, SONET_ACT_ELU>(x, dy, mean, invstd, gamma, beta, B, C, ld, col_offsets,
+                                                rec, st);
+  else if (act == SONET_ACT_RELU)
+    launch_bn_cloud_ragged<true, SONET_ACT_RELU>(x, dy, mean, invstd, gamma, beta, B, C, ld, col_offsets,
+                                                 rec, st);
+  else
+    launch_bn_cloud_ragged<true, SONET_ACT_NONE>(x, dy, mean, invstd, gamma, beta, B, C, ld, col_offsets,
+                                                 rec, st);
+  return check_launch("bn_cloud_partials_ragged");
+}
+
+extern "C" int sonet_bn_ragged_forward_f32(const double* rec, const long long* col_offsets, int B,
+                                           const float* x, const float* gamma, const float* beta, int C,
+                                           long long L, float eps, int act, float* y, float* mean,
+                                           float* var, float* invstd, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(act, "bn_ragged_forward");
+  if (int rc = bn_ragged_dims("bn_ragged_forward", B, C, L)) return rc;
+  SONET_REQUIRE(rec && col_offsets && x && y && mean && var && invstd, "bn_ragged_forward: null pointer");
+  cudaStream_t st = as_stream(stream);
+  bn_sync_stats_kernel<<<(C + 127) / 128, 128, 0, st>>>(rec, B, C, RaggedCounts{col_offsets, L}, eps,
+                                                        mean, var, invstd);
+  const int P = static_cast<int>(L);
+  const dim3 grid((P + 1023) / 1024, C, 1);
+  if (act == SONET_ACT_ELU)
+    bn_apply_kernel<true><<<grid, 256, 0, st>>>(x, mean, invstd, gamma, beta, C, P, 0, y);
+  else
+    bn_apply_kernel<false><<<grid, 256, 0, st>>>(x, mean, invstd, gamma, beta, C, P, act, y);
+  return check_launch("bn_ragged_forward");
+}
+
+extern "C" int sonet_bn_ragged_backward_f32(const double* rec, const long long* col_offsets, int B,
+                                            const float* dy, const float* x, const float* mean,
+                                            const float* invstd, const float* gamma, const float* beta,
+                                            int C, long long L, int act, float* dx, float* dgamma,
+                                            float* dbeta, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE_ACT(act, "bn_ragged_backward");
+  if (int rc = bn_ragged_dims("bn_ragged_backward", B, C, L)) return rc;
+  SONET_REQUIRE(rec && col_offsets && dy && x && mean && invstd && dx && dgamma && dbeta,
+                "bn_ragged_backward: null pointer");
+  cudaStream_t st = as_stream(stream);
+  bn_sync_bwd_final_kernel<<<(C + 127) / 128, 128, 0, st>>>(rec, B, C, dgamma, dbeta);
+  const int P = static_cast<int>(L);
+  const dim3 grid((P + 1023) / 1024, C, 1);
+  const float inv_n = static_cast<float>(1.0 / static_cast<double>(L));
+  if (act == SONET_ACT_ELU)
+    bn_bwd_apply_kernel<true><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
+                                                    0, inv_n, dx);
+  else
+    bn_bwd_apply_kernel<false><<<grid, 256, 0, st>>>(dy, x, mean, invstd, gamma, beta, dgamma, dbeta, C, P,
+                                                     act, inv_n, dx);
+  return check_launch("bn_ragged_backward");
 }
 
 extern "C" int sonet_instance_norm_f32(const float* z, const float* gamma, const float* beta, int B,
@@ -697,6 +870,22 @@ extern "C" int sonet_index_max_backward_f32(const float* grad_out, const int32_t
   index_max_backward_kernel<<<static_cast<unsigned>((rows + 127) / 128), 128, 0, st>>>(
       grad_out, idx, rows, N, K, grad_data);
   return check_launch("index_max_backward");
+}
+
+extern "C" int sonet_index_max_ragged_backward_f32(const float* grad_out, const int32_t* idx,
+                                                   const long long* col_offsets, int B, int C, int M,
+                                                   long long ld, float* grad, sonet_stream_t stream) {
+  using namespace sonet;
+  SONET_REQUIRE(B >= 1 && C >= 1 && M >= 1 && M <= 256 && B <= 65535 && C <= 65535,
+                "index_max_ragged_backward: bad dims B=%d C=%d M=%d", B, C, M);
+  SONET_REQUIRE(ld >= 1 && ld < (1LL << 31), "index_max_ragged_backward: ld=%lld outside [1, 2^31)", ld);
+  SONET_REQUIRE(grad_out && idx && col_offsets && grad, "index_max_ragged_backward: null pointer");
+  cudaStream_t st = as_stream(stream);
+  const long long rows = static_cast<long long>(B) * C;
+  cudaMemsetAsync(grad, 0, sizeof(float) * static_cast<size_t>(C) * ld, st);
+  index_max_backward_kernel<<<static_cast<unsigned>((rows + 127) / 128), 128, 0, st>>>(
+      grad_out, idx, rows, RaggedCols{C, ld, col_offsets}, M, grad);
+  return check_launch("index_max_ragged_backward");
 }
 
 extern "C" long long sonet_pointwise_tc_blob_bytes(int Cout, int Cin);

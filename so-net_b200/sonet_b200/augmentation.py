@@ -145,6 +145,17 @@ def draw_batch_host(rng, counts, N, M, rule, train, **flags):
     return sel, params
 
 
+def _aug_flags(opt):
+    """draw_params' flags of the train loader that opt.dataset selects: the ShapeNet loader neither
+    rotates nor shifts (shapenet_loader.py:157-180)."""
+    flags = dict(rot_horizontal=bool(getattr(opt, "rot_horizontal", False)),
+                 rot_perturbation=bool(getattr(opt, "rot_perturbation", False)),
+                 translation_perturbation=bool(getattr(opt, "translation_perturbation", False)))
+    if getattr(opt, "dataset", None) == "shapenet":
+        flags = dict.fromkeys(flags, False)
+    return flags
+
+
 class DeviceDataset:
     """A whole dataset in device memory, drawn from batch by batch: the loaders' complete
     __getitem__ (random point choice, augmentation, SOM-node kNN) plus the collation, on the device.
@@ -233,15 +244,28 @@ class DeviceDataset:
         seg = None if self.seg is None else self.seg[rows].long()
         return self.data[rows], offsets, seg
 
-    def full_batch(self, index, opt):
+    def full_batch(self, index, opt, train=False, rng=None, seed=0):
         """(points [sum P_i, 6] f32, offsets [len(index)+1] int64, label [len(index)] int64,
         som_node [len(index),3,M] f32, som_knn_I [len(index),M,som_k] int64) of the clouds `index`:
-        every point of each (full_clouds), with the test-mode loader's SOM nodes and their kNN and
-        no augmentation — the input of classifier.Model.score_clouds and
-        networks.Encoder.forward_ragged."""
+        every point of each (full_clouds), with the loader's SOM nodes and their kNN — the input of
+        classifier.Model.score_clouds and networks.Encoder.forward_ragged.
+        train=False: no augmentation (the test-mode loader's). train=True: the train loader's
+        augmentation of whole clouds, the input of classifier.Model.optimize_clouds: the per-cloud
+        scalars from `rng` by draw_params, in the order and with the dataset's flags that
+        batch(train=True, host_noise=False) draws them, the jitter in the kernel keyed by `seed`
+        (cloud b's row n gets the draws of point n of cloud b in batch()), and the kNN of the
+        augmented nodes."""
         points, offsets, _ = self.full_clouds(index)
         cid = torch.from_numpy(np.asarray(index, dtype=np.int64).reshape(-1)).to(self.device)
         som = self.som_nodes.index_select(0, cid)
+        if train:
+            rng = rng if rng is not None else np.random
+            p = draw_params(rng, len(cid), 0, self.node_num, host_noise=False, **_aug_flags(opt))
+            d = self.device
+            points, som = ops.augment_ragged(
+                points.contiguous(), offsets, som, rot1=_dev(p["rot1"], d), rot2=_dev(p["rot2"], d),
+                scale=_dev(p["scale"], d), shift=_dev(p["shift"], d), jitter_pc=JITTER_PC,
+                jitter_sn=JITTER_PC, jitter_som=JITTER_SOM, seed=seed)
         return (points, offsets, self.labels.index_select(0, cid), som,
                 som_knn(som, opt.som_k, self.node_num))
 
@@ -281,12 +305,7 @@ class DeviceDataset:
             raise ValueError("Cannot take a larger sample than population when 'replace=False' "
                              "(cloud %d has %d points, N=%d)" % (ids[P < N][0], P[P < N][0], N))
         rng = rng if rng is not None else np.random
-        # the ShapeNet loader neither rotates nor shifts (shapenet_loader.py:157-180)
-        flags = dict(rot_horizontal=bool(getattr(opt, "rot_horizontal", False)),
-                     rot_perturbation=bool(getattr(opt, "rot_perturbation", False)),
-                     translation_perturbation=bool(getattr(opt, "translation_perturbation", False)))
-        if rule == ops.SAMPLE_FILL:
-            flags = dict.fromkeys(flags, False)
+        flags = _aug_flags(opt)
         params = None
         indices = None
         if host_noise:

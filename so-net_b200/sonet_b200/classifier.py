@@ -88,6 +88,47 @@ class Model(GraphedModel):
             feature = enc.forward_ragged(points, offsets, node, node_knn_I, chunk_points)
             return head.fc3(head.fc2(head.fc1(feature)))
 
+    def optimize_clouds(self, points, offsets, label, node, node_knn_I=None, epoch=None):
+        """One training step (optimize()'s: forward, zero_grad, CrossEntropyLoss, backward, both
+        Adam steps) on whole clouds of any size: points [T,6] f32, offsets [B+1] int64, label [B]
+        int64 in [0, classes), node [B,3,M] and node_knn_I [B,M,som_k] int64 or None to compute it
+        (DeviceDataset.full_batch(train=True) draws such batches). The encoder runs
+        Encoder.forward_ragged_train; the loss is the mean over the B clouds, so each cloud counts
+        once whatever its size. Returns dict(loss, score [B,classes]), both detached.
+
+        Shares optimize()'s optimizers, so interleaving the two is one training run. Always eager
+        (every batch has its own shapes), also after enable_train_graph(True) has made Adam
+        capturable; reads no bound input, rebinds no buffer of a captured graph and writes no model
+        attribute but the parameters, their gradients, the optimizer state and the BatchNorm running
+        statistics. Refused before any launch: Encoder.check_ragged(train=True)'s cases and a label
+        that is not [B] int64 on the model's device with values in [0, classes)."""
+        enc, opt = self.encoder, self.opt
+        enc.check_ragged(points, offsets, node, node_knn_I, what="optimize_clouds", train=True)
+        B = node.shape[0]
+        if not isinstance(label, torch.Tensor) or label.dtype != torch.int64 \
+                or tuple(label.shape) != (B,) or label.device != node.device:
+            raise RuntimeError("optimize_clouds: label must be a [%d] int64 tensor on %s (got %s)" % (
+                B, node.device, (label.dtype, tuple(label.shape), str(label.device))
+                if isinstance(label, torch.Tensor) else type(label).__name__))
+        lo, hi = (int(v) for v in torch.stack((label.min(), label.max())).cpu())
+        if lo < 0 or hi >= opt.classes:
+            raise RuntimeError("optimize_clouds: label values must lie in [0, %d) (got %d .. %d)"
+                               % (opt.classes, lo, hi))
+        if self._optim is None:
+            self._optim = self._make_optimizers()
+        enc.train()
+        self.classifier.train()
+        with torch.enable_grad():
+            feature = enc.forward_ragged_train(points, offsets, node, node_knn_I, epoch)
+            score = self.classifier(feature, epoch, store=False)
+            enc.zero_grad()
+            self.classifier.zero_grad()
+            loss = self.softmax_criteria(score, label)
+            loss.backward()
+        for o in self._optim:
+            o.step()
+        return dict(loss=loss.detach(), score=score.detach())
+
     def _make_optimizers(self):
         return (torch.optim.Adam(self.encoder.parameters(), lr=self.opt.lr,
                                  betas=(0.9, 0.999), weight_decay=0),

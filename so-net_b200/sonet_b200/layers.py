@@ -600,14 +600,15 @@ class EquivariantLayer(_PointwiseConvBase):
     def fast(self, *tensors):
         return _fast_ok(self, *tensors) and self._fast_eligible()
 
-    def forward(self, x, epoch=None, route_rows=None):
-        """route_rows: as forward_points (eval fast path only)."""
+    def forward(self, x, epoch=None, route_rows=None, cols=None):
+        """route_rows: as forward_points (eval fast path only). cols: the device column offsets of
+        a ragged batch's x [1,C,L] for the train kernels' BatchNorm (train_ops.norm_act_train)."""
         if self.fast(x) and x.dim() == 3:
             return self.forward_points(x.contiguous(), route_rows=route_rows)
         if self._train_kernels(x) and x.dim() == 3:
             return train_ops.conv_bn_act_train(
                 x, self._conv_weight2d(), self.conv.bias, self._train_norm(), self.activation,
-                epoch)
+                epoch, cols=cols)
         y = self.conv(x)
         if self.normalization == 'batch':
             y = self.norm(y, epoch)
@@ -846,9 +847,10 @@ class PointResNet(nn.Module):
             return blob.to(ws[0].device), fpar.to(ws[0].device)
         return self._tc.get(tuple(l._folded.version for l in self.layers), build)
 
-    def forward(self, x, epoch=None, x1=None, route_rows=None):
+    def forward(self, x, epoch=None, x1=None, route_rows=None, cols=None):
         """x [B,C,P]; x1: optional second tensor virtually concatenated to x (eval fast path);
-        route_rows: as EquivariantLayer.forward_points (the fused kernel has one route)."""
+        route_rows: as EquivariantLayer.forward_points (the fused kernel has one route); cols: as
+        EquivariantLayer.forward (train kernels)."""
         n = len(self.out_channels_list)
         first, last = self.layers[0], self.layers[n - 1]
         if first.fast(x) and x.dim() == 3 and all(l.fast(x) for l in self.layers) \
@@ -867,8 +869,8 @@ class PointResNet(nn.Module):
             return last.forward_points(layer0_out, x_tmp, route_rows=route_rows)
         if x1 is not None:
             x = torch.cat((x, x1), dim=1)
-        layer0_out = first(x, epoch)
+        layer0_out = first(x, epoch, cols=cols)
         x_tmp = layer0_out
         for l in range(1, n - 1):
-            x_tmp = self.layers[l](x_tmp, epoch)
+            x_tmp = self.layers[l](x_tmp, epoch, cols=cols)
         return last(torch.cat((layer0_out, x_tmp), dim=1), epoch)

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import ops, som, train_ops
+from . import augmentation, ops, som, train_ops
 from .layers import (EquivariantLayer, KNNModule, MyConv2d, MyLinear, PointNet, PointResNet,
                      UpConv, _Cache, _fast_ok, tc_enabled, tc_f16)
 
@@ -249,11 +249,23 @@ class Encoder(nn.Module):
     _RAGGED_MAX_POINTS = (1 << 24) - 1
 
     def check_ragged(self, points, offsets, node, node_knn_I=None, chunk_points=None,
-                     what="forward_ragged"):
+                     what="forward_ragged", train=False):
         """The refusals of forward_ragged (RuntimeError; ValueError for an empty cloud), raised
-        before any launch. Returns the offsets as a host numpy array."""
+        before any launch; with train, those of forward_ragged_train instead: the same but for the
+        train-mode refusal, plus k*T >= 2^31 stacked columns, train_ops.ENABLED off, an installed
+        DataParallelTraining and a random point dropout. Returns the offsets as a host numpy
+        array."""
         opt = self.opt
-        if self.training:
+        if train:
+            if not train_ops.ENABLED:
+                raise RuntimeError("%s: the train kernels are off (train_ops.ENABLED = False)" % what)
+            if train_ops.EXCHANGE is not None:
+                raise RuntimeError("%s: a DataParallelTraining is installed; ragged batches train in "
+                                   "one process" % what)
+            if opt.random_pc_dropout_lower_limit < 0.99:
+                raise RuntimeError("%s: random point dropout (random_pc_dropout_lower_limit=%s) is not "
+                                   "applied to whole clouds" % (what, opt.random_pc_dropout_lower_limit))
+        elif self.training:
             raise RuntimeError("%s: the encoder is in train mode; call eval() first" % what)
         if opt.normalization == 'instance':
             raise RuntimeError("%s: --normalization instance has no ragged per-cloud statistics"
@@ -297,7 +309,49 @@ class Encoder(nn.Module):
             raise RuntimeError("%s: cloud %d has %d points, more than %d"
                                % (what, int(counts.argmax()), int(counts.max()),
                                   self._RAGGED_MAX_POINTS))
+        if train and opt.k * points.shape[0] >= (1 << 31):
+            raise RuntimeError("%s: k*T = %d stacked columns, 2^31 or more"
+                               % (what, opt.k * points.shape[0]))
         return off
+
+    def forward_ragged_train(self, points, offsets, node, node_knn_I, epoch=None):
+        """The global feature [B,feature_num] of every cloud of a ragged batch from ALL of its points,
+        in train mode and differentiable w.r.t. the encoder's parameters (classifier.Model.
+        optimize_clouds). Inputs as forward_ragged; node_knn_I None: computed (augmentation.som_knn).
+
+        The ragged SOM assignment and the group route's cluster means (forward_ragged's, the whole
+        cloud's), the decentred copies x_aug [1,Cin,k*T] (detached, as in forward()), the first
+        PointResNet on the train kernels with cols = k*offsets, so that its BatchNorm statistics
+        cover every stacked copy of the batch (a cloud weighs its size), the per-cloud per-node max
+        (IndexMaxGatherRagged), then forward()'s train-mode node-level stage on [B,.,M]. No chunks:
+        BatchNorm needs the whole batch. Writes no encoder attribute; the BatchNorm running
+        statistics are updated as in a train step (with n = k*T in the first PointResNet).
+        Refused before any launch: eval mode and check_ragged(train=True)'s cases."""
+        if not self.training:
+            raise RuntimeError("forward_ragged_train: the encoder is in eval mode; call train() first")
+        self.check_ragged(points, offsets, node, node_knn_I, what="forward_ragged_train", train=True)
+        opt = self.opt
+        k, M = opt.k, node.shape[2]
+        use_sn = opt.surface_normal == True  # noqa: E712
+        points = points.detach().contiguous()
+        node = node.detach().contiguous()
+        with torch.no_grad():
+            if node_knn_I is None:
+                node_knn_I = augmentation.som_knn(node, opt.som_k, M)
+            idx, _, _ = ops.som_assign_ragged(points, offsets, node, k)
+            _, _, _, som_node = ops.som_group_decenter_ragged(points, offsets, idx, M, k, use_sn)
+            x_aug = ops.som_decenter_ragged(points, offsets, idx, som_node, k, use_sn)
+            cols = offsets * k
+        fpo = self.first_pointnet(x_aug, epoch, cols=cols)
+        masked_max = train_ops.IndexMaxGatherRagged.apply(fpo, idx, offsets, cols, M, k)
+        if opt.som_k >= 2:
+            center, knn_feature = self.knnlayer(som_node, masked_max, node_knn_I, opt.som_k,
+                                                opt.som_k_type, epoch)
+            final = self.final_pointnet.forward_pair(center, knn_feature, epoch)
+        else:
+            final = self.final_pointnet(som_node, epoch, x1=masked_max)
+        feature, _ = torch.max(final, dim=2, keepdim=False)
+        return feature
 
     def forward_ragged(self, points, offsets, node, node_knn_I, chunk_points=None,
                        return_nodes=False):
@@ -396,14 +450,17 @@ class Classifier(nn.Module):
         self.dropout1 = nn.Dropout(p=self.opt.dropout)
         self.dropout2 = nn.Dropout(p=self.opt.dropout)
 
-    def forward(self, feature, epoch=None):
+    def forward(self, feature, epoch=None, store=True):
+        """store=False: leave the fc2_out attribute alone (classifier.Model.optimize_clouds)."""
         fc1_out = self.fc1(feature, epoch)
         if self.opt.dropout > 0.1:
             fc1_out = self.dropout1(fc1_out)
-        self.fc2_out = self.fc2(fc1_out, epoch)
+        fc2_out = self.fc2(fc1_out, epoch)
         if self.opt.dropout > 0.1:
-            self.fc2_out = self.dropout2(self.fc2_out)
-        return self.fc3(self.fc2_out, epoch)
+            fc2_out = self.dropout2(fc2_out)
+        if store:
+            self.fc2_out = fc2_out
+        return self.fc3(fc2_out, epoch)
 
 
 class Segmenter(nn.Module):

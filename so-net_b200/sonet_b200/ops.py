@@ -860,6 +860,122 @@ def index_max_ragged(data, index, offsets, M, k):
     return out_idx, out_val
 
 
+
+def index_max_ragged_backward(grad_out, idx, col_offsets, L):
+    """The backward of index_max_ragged's gather: grad_out, idx [B,C,M] (index_max_ragged's out_idx),
+    col_offsets [B+1] int64 (cloud b's columns, k*offsets; checked by the caller) -> grad [C,L] f32,
+    zero but for grad[c, col_offsets[b] + idx[b,c,m]] += grad_out[b,c,m] in ascending m."""
+    _chk(grad_out, "grad_out", torch.float32)
+    _chk(idx, "idx", torch.int32)
+    _chk(col_offsets, "col_offsets", torch.int64)
+    if grad_out.dim() != 3 or tuple(idx.shape) != tuple(grad_out.shape) or col_offsets.dim() != 1 \
+            or col_offsets.numel() != grad_out.shape[0] + 1:
+        raise RuntimeError("index_max_ragged_backward: expected grad_out and idx [B,C,M], col_offsets "
+                           "[B+1], got %s, %s, %s" % (tuple(grad_out.shape), tuple(idx.shape),
+                                                      tuple(col_offsets.shape)))
+    B, C, M = grad_out.shape
+    dev = grad_out.device
+    with torch.cuda.device(dev):
+        grad = torch.empty((C, int(L)), dtype=torch.float32, device=dev)
+        _call("sonet_index_max_ragged_backward_f32", _C.ptr(grad_out), _C.ptr(idx), _C.ptr(col_offsets),
+              B, C, M, int(L), _C.ptr(grad), _stream(grad_out), kernels=2)
+    return grad
+
+
+def _bn_ragged_args(x, col_offsets, what):
+    _chk(x, "x", torch.float32)
+    _chk(col_offsets, "col_offsets", torch.int64)
+    if x.dim() == 3 and x.shape[0] == 1:
+        x = x[0]
+    if x.dim() != 2 or col_offsets.dim() != 1 or col_offsets.numel() < 2:
+        raise RuntimeError("%s: expected x [1,C,L] or [C,L] and col_offsets [B+1], got %s and %s"
+                           % (what, tuple(x.shape), tuple(col_offsets.shape)))
+    return x, col_offsets.numel() - 1
+
+
+def bn_cloud_partials_ragged(x, col_offsets, act=ACT_NONE, dy=None, mean=None, invstd=None,
+                             gamma=None, beta=None):
+    """The per-(cloud, channel) BatchNorm records of a ragged batch (csrc/train.cu): x [1,C,L] (or
+    [C,L]) with cloud b's columns col_offsets[b] .. col_offsets[b+1] (checked by the caller). Without
+    dy: the forward records [B,C,SONET_BN_REC_FWD]; with dy (and mean, invstd): the backward ones
+    [B,C,SONET_BN_REC_BWD] of act."""
+    x, B = _bn_ragged_args(x, col_offsets, "bn_cloud_partials_ragged")
+    bwd = dy is not None
+    if bwd:
+        dy = dy.reshape(x.shape)
+        for t, n in ((dy, "dy"), (mean, "mean"), (invstd, "invstd")):
+            _chk(t, n, torch.float32)
+    C, L = x.shape
+    dev = x.device
+    with torch.cuda.device(dev):
+        rec = torch.empty((B, C, _C.CONSTANTS["SONET_BN_REC_BWD" if bwd else "SONET_BN_REC_FWD"]),
+                          dtype=torch.float64, device=dev)
+        _call("sonet_bn_cloud_partials_ragged_f32", _C.ptr(x), _C.ptr(dy), _C.ptr(mean), _C.ptr(invstd),
+              _C.ptr(gamma), _C.ptr(beta), C, L, _C.ptr(col_offsets), B, act_code(act), int(bwd),
+              _C.ptr(rec), _stream(x), kernels=3)
+    return rec
+
+
+def bn_ragged_forward(rec, col_offsets, x, gamma, beta, eps, act):
+    """The forward records rec [B,C,3] folded with each cloud's own count, then act(BN(x)) over x
+    [1,C,L] -> (y [1,C,L], mean [C], var [C] (biased), invstd [C])."""
+    x2, B = _bn_ragged_args(x, col_offsets, "bn_ragged_forward")
+    _chk(rec, "rec", torch.float64)
+    C, L = x2.shape
+    dev = x2.device
+    with torch.cuda.device(dev):
+        y = torch.empty((1, C, L), dtype=torch.float32, device=dev)
+        mean, var, invstd = (torch.empty(C, dtype=torch.float32, device=dev) for _ in range(3))
+        _call("sonet_bn_ragged_forward_f32", _C.ptr(rec), _C.ptr(col_offsets), B, _C.ptr(x2),
+              _C.ptr(gamma), _C.ptr(beta), C, L, float(eps), act_code(act), _C.ptr(y), _C.ptr(mean),
+              _C.ptr(var), _C.ptr(invstd), _stream(x2), kernels=2)
+    return y, mean, var, invstd
+
+
+def bn_ragged_backward(rec, col_offsets, dy, x, mean, invstd, gamma, beta, act):
+    """The backward records rec [B,C,2] folded in ascending cloud order, then dx over x [1,C,L] ->
+    (dx [1,C,L], dgamma [C], dbeta [C])."""
+    x2, B = _bn_ragged_args(x, col_offsets, "bn_ragged_backward")
+    _chk(rec, "rec", torch.float64)
+    _chk(dy, "dy", torch.float32)
+    C, L = x2.shape
+    dev = x2.device
+    with torch.cuda.device(dev):
+        dx = torch.empty((1, C, L), dtype=torch.float32, device=dev)
+        dgamma = torch.empty(C, dtype=torch.float32, device=dev)
+        dbeta = torch.empty(C, dtype=torch.float32, device=dev)
+        _call("sonet_bn_ragged_backward_f32", _C.ptr(rec), _C.ptr(col_offsets), B, _C.ptr(dy),
+              _C.ptr(x2), _C.ptr(mean), _C.ptr(invstd), _C.ptr(gamma), _C.ptr(beta), C, L,
+              act_code(act), _C.ptr(dx), _C.ptr(dgamma), _C.ptr(dbeta), _stream(x2), kernels=2)
+    return dx, dgamma, dbeta
+
+
+def augment_ragged(points, offsets, som, rot1=None, rot2=None, scale=None, shift=None,
+                   jitter_pc=(0.0, 1.0), jitter_sn=(0.0, 1.0), jitter_som=(0.0, 1.0), seed=0):
+    """augment over whole clouds (csrc/augment.cu): points [T,6] f32 rows xyz | normal, offsets [B+1]
+    int64 (checked by the caller), som [B,3,M] f32 or None; rot1/rot2 [B,3,3], scale [B], shift
+    [B,3] float64 device tensors or None; the jitter drawn in the kernel from `seed`, cloud b's row
+    n as augment's point n of cloud b. -> (points' [T,6], som' or None)."""
+    T, B = _ragged_args(points, offsets, "augment_ragged")
+    _chk(som, "som", torch.float32, optional=True)
+    for t, n in ((rot1, "rot1"), (rot2, "rot2"), (scale, "scale"), (shift, "shift")):
+        _chk(t, n, torch.float64, optional=True)
+    M = 0 if som is None else som.shape[2]
+    if som is not None and (som.dim() != 3 or som.shape[0] != B or som.shape[1] != 3):
+        raise RuntimeError("augment_ragged: som must be [%d,3,M] (got %s)" % (B, tuple(som.shape)))
+    for t, shp, n in ((rot1, (B, 3, 3), "rot1"), (rot2, (B, 3, 3), "rot2"), (scale, (B,), "scale"),
+                      (shift, (B, 3), "shift")):
+        if t is not None and tuple(t.shape) != shp:
+            raise RuntimeError("augment_ragged: %s must have shape %s, got %s" % (n, shp, tuple(t.shape)))
+    with torch.cuda.device(points.device):
+        po = torch.empty_like(points)
+        mo = torch.empty_like(som) if som is not None else None
+        _call("sonet_augment_ragged_f32", _C.ptr(points), T, 6, _C.ptr(offsets), B, _C.ptr(som), M,
+              _C.ptr(rot1), _C.ptr(rot2), _C.ptr(scale), _C.ptr(shift), float(jitter_pc[0]),
+              float(jitter_pc[1]), float(jitter_sn[0]), float(jitter_sn[1]), float(jitter_som[0]),
+              float(jitter_som[1]), int(seed) & (2 ** 64 - 1), _C.ptr(po), _C.ptr(mo), _stream(points))
+    return po, mo
+
 RETRIEVAL_MAX_D = 1024
 RETRIEVAL_MAX_K = 4096
 RETRIEVAL_MAX_L = 4096

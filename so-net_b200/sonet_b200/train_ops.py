@@ -108,11 +108,24 @@ class BNActTrain(torch.autograd.Function):
     (sonet_bn_cloud_partials_f32, then sonet_bn_sync_forward_f32 / _backward_f32). The backward's
     dy is the gradient of this process's loss, a mean over its B clouds. The exchange works in
     units of the global-batch loss, whose gradient here is dy * B / Bg: dgamma and dbeta come out
-    as the global gradients, the same on every rank, and dx goes back to this rank's units."""
+    as the global gradients, the same on every rank, and dx goes back to this rank's units.
+
+    cols (device int64 [B+1]): x is a ragged batch's [1,C,L] layer output whose cloud b owns the
+    columns cols[b] .. cols[b+1]; the records are per (cloud, channel) over those columns and the
+    statistics cover all L columns (sonet_bn_cloud_partials_ragged_f32, sonet_bn_ragged_*_f32).
+    Single-process only."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, eps, act):
+    def forward(ctx, x, gamma, beta, eps, act, cols=None):
         x = x.contiguous()
+        ctx.cols = cols
+        if cols is not None:
+            ctx.act = ops.act_code(act)
+            rec = ops.bn_cloud_partials_ragged(x, cols)
+            y, mean, var, invstd = ops.bn_ragged_forward(rec, cols, x, gamma, beta, eps, ctx.act)
+            ctx.save_for_backward(x, mean, invstd, gamma, beta)
+            ctx.mark_non_differentiable(mean, var)
+            return y, mean, var
         B, C, P = x.shape
         dev = x.device
         ex = ctx.exchange = _exchange()
@@ -137,6 +150,11 @@ class BNActTrain(torch.autograd.Function):
     def backward(ctx, dy, _dm, _dv):
         x, mean, invstd, gamma, beta = ctx.saved_tensors
         dy = dy.contiguous()
+        if ctx.cols is not None:
+            rec = ops.bn_cloud_partials_ragged(x, ctx.cols, ctx.act, dy, mean, invstd, gamma, beta)
+            dx, dgamma, dbeta = ops.bn_ragged_backward(rec, ctx.cols, dy, x, mean, invstd, gamma, beta,
+                                                       ctx.act)
+            return dx, dgamma, dbeta, None, None, None
         B, C, P = x.shape
         dev = x.device
         share = B / ctx.exchange.global_rows(B)
@@ -150,7 +168,7 @@ class BNActTrain(torch.autograd.Function):
                          dbeta)
         if share != 1.0:
             dx.div_(share)
-        return dx, dgamma, dbeta, None, None
+        return dx, dgamma, dbeta, None, None, None
 
 
 class InstanceNormActTrain(torch.autograd.Function):
@@ -330,6 +348,27 @@ class ConvTC(torch.autograd.Function):
 WGRAD_TC = True
 
 
+class IndexMaxGatherRagged(torch.autograd.Function):
+    """The per-node max of a ragged batch's stacked copies, differentiable w.r.t. data: data
+    [1,C,k*T] (cloud b's columns cols[b] .. cols[b+1], cols = k*offsets), index [k*T] i32
+    cloud-local nodes -> [B,C,M] (index_max_ragged's values). Backward: a deterministic scatter of
+    each (cloud, channel)'s gradient in ascending node order (sonet_index_max_ragged_backward_f32)."""
+
+    @staticmethod
+    def forward(ctx, data, index, offsets, cols, M, k):
+        data = data.contiguous()
+        idx, val = ops.index_max_ragged(data.detach()[0], index, offsets, M, k)
+        ctx.save_for_backward(idx, cols)
+        ctx.L = data.shape[2]
+        return val
+
+    @staticmethod
+    def backward(ctx, g):
+        idx, cols = ctx.saved_tensors
+        gd = ops.index_max_ragged_backward(g.contiguous(), idx, cols, ctx.L)
+        return gd.unsqueeze(0), None, None, None, None, None
+
+
 class IndexMaxGather(torch.autograd.Function):
     """data [B,C,N], index [B,N] int32, K -> data.gather(2, idx * mask_row_max) [B,C,K]
     (models/networks.py:181-185), differentiable w.r.t. data."""
@@ -452,16 +491,22 @@ class LinearStrict(torch.autograd.Function):
         return dx, dW, db
 
 
-def norm_act_train(y0, norm, act, epoch=None, size=None):
+def norm_act_train(y0, norm, act, epoch=None, size=None, cols=None):
     """The norm / activation half of every train-mode layer on its pre-norm output y0 [B,C,P]:
     batch-stat BN (+ running-stat update with the reference's momentum schedule,
     models/layers.py:57-65; like F.batch_norm, num_batches_tracked is left alone) or instance norm
     (affine, no running statistics: nothing to update) or none -> act: the layer's activation
     (None, 'relu' or 'elu'; a bool means ReLU or none). size: the layer output's shape as the
-    reference sees it, for the messages of F.batch_norm's and F.instance_norm's ValueErrors."""
+    reference sees it, for the messages of F.batch_norm's and F.instance_norm's ValueErrors.
+    cols: the device column offsets of a ragged batch's y0 [1,C,L] (BNActTrain); the statistics
+    then cover n = L columns, in the running variance too. Refused with instance norm and with a
+    data-parallel exchange installed."""
     B, C, P = y0.shape
     size = y0.size() if size is None else torch.Size(size)
     instance = isinstance(norm, _InstanceNorm)
+    if cols is not None and (instance or EXCHANGE is not None):
+        raise RuntimeError("norm_act_train: a ragged batch (cols) has no %s" % (
+            "per-cloud instance statistics" if instance else "data-parallel BatchNorm exchange"))
     if instance and not (norm.affine and not norm.track_running_stats):
         raise RuntimeError("norm_act_train: instance norm needs affine=True and "
                            "track_running_stats=False")
@@ -476,12 +521,12 @@ def norm_act_train(y0, norm, act, epoch=None, size=None):
             return F.elu(y0)
         return torch.relu(y0) if code == ops.ACT_RELU else y0
     # with a BatchNorm exchange installed the statistics are those of the global batch
-    n = _exchange().global_rows(B) * P
+    n = P if cols is not None else _exchange().global_rows(B) * P
     if n == 1:         # F.batch_norm's check: a batch statistic of one value is undefined
         raise ValueError("Expected more than 1 value per channel when training, got input size "
                          "{}".format(size))
     norm.momentum = norm.momentum_at(epoch)
-    y, mean, var = BNActTrain.apply(y0, norm.weight, norm.bias, norm.eps, act)
+    y, mean, var = BNActTrain.apply(y0, norm.weight, norm.bias, norm.eps, act, cols)
     with torch.no_grad():
         m = norm.momentum
         norm.running_mean.mul_(1 - m).add_(mean, alpha=m)
@@ -489,16 +534,16 @@ def norm_act_train(y0, norm, act, epoch=None, size=None):
     return y
 
 
-def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None):
+def conv_bn_act_train(x3, weight2d, bias, norm, act, epoch=None, cols=None):
     """Train-mode EquivariantLayer / MyConv2d(1x1) body on [B,Cin,P]: conv (wgmma when dense
-    enough, else strict-fp32 cuDNN) -> norm_act_train."""
+    enough, else strict-fp32 cuDNN) -> norm_act_train (cols: a ragged batch's, as there)."""
     B, Cin, P = x3.shape
     Cout = weight2d.shape[0]
     if tc_eligible(Cin, Cout, B * P):
         y0 = ConvTC.apply(x3, weight2d, bias)
     else:
         y0 = ConvStrict.apply(x3, weight2d.unsqueeze(2), bias, [1], [0], [1], 1)
-    return norm_act_train(y0, norm, act, epoch)
+    return norm_act_train(y0, norm, act, epoch, cols=cols)
 
 
 # ---- the up-convolution (csrc/upconv.cu) -----------------------------------------------------------

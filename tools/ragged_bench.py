@@ -23,6 +23,14 @@ test_model() on the same clouds, and batches of clouds of mixed sizes.
      ragged encoder, the per-point head (node/cloud addend and every point through the head) and
      the ragged loss (CUDA events around each stage).
 
+  TRAIN_A  optimize_clouds on 32 clouds x 10,000 points (augmented by DeviceDataset.full_batch(train=
+     True)), against eager dense optimize() on the same clouds at N = 10,000 and N = 5,000.
+  TRAIN_B  optimize_clouds on 32 clouds with P uniform in [2,000, 10,000]. Both split one step into
+     augmentation, SOM (assignment, cluster means, decentring), the first PointResNet's forward +
+     backward (with the per-node max), the node-level stage's forward + backward (KNN module, final
+     PointNet, head and loss) and the optimizer (CUDA events; the backward split by a gradient hook
+     on the pooled features), and give the peak device memory of a step.
+
 Times are medians of --reps warm calls, each bracketed by CUDA events. Synthetic clouds and weights
 (synth.py), the default options of each task (k = 3, 8x8 SOM, som_k = 9; the auto-encoder's
 256 + 1024 output points); SONET_TC as set.
@@ -39,7 +47,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "so-net_b200")]
 
-from sonet_b200 import augmentation, autoencoder, classifier, networks, ops, synth  # noqa: E402
+from sonet_b200 import (augmentation, autoencoder, classifier, networks, ops, synth,  # noqa: E402
+                        train_ops)
 
 DEV = torch.device("cuda:0")
 
@@ -179,7 +188,7 @@ def autoencoder_cases(res, reps):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--task", choices=("all", "classifier", "autoencoder", "segmenter"),
+    ap.add_argument("--task", choices=("all", "classifier", "autoencoder", "segmenter", "train"),
                     default="all")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -194,6 +203,8 @@ def main():
         classifier_cases(res, a.reps)
     if a.task in ("all", "segmenter"):
         segmenter_cases(res, a.reps)
+    if a.task in ("all", "train"):
+        train_cases(res, a.reps)
     print(json.dumps(res, indent=1))
     if a.out:
         with open(a.out, "w") as f:
@@ -317,6 +328,119 @@ def segmenter_cases(res, reps):
     res["SEG_B_split_ms"] = seg_stage_split(m, pts, off, label, node, knn, seg, reps)
     del m
     torch.cuda.empty_cache()
+
+
+
+# ---- training on whole clouds -----------------------------------------------------------------------
+def train_model(B, N, states):
+    opt = synth.make_opt("classifier", batch_size=B, input_pc_num=N, device=DEV, rot_horizontal=True,
+                         rot_perturbation=True, translation_perturbation=True)
+    m = classifier.Model(opt)
+    m.encoder.load_state_dict(states[0])
+    m.classifier.load_state_dict(states[1])
+    return m
+
+
+def train_stage_split(m, ds, idx, reps):
+    """Median device time of one optimize_clouds step's stages, each between CUDA events: the step
+    written out as optimize_clouds runs it, the backward split by a hook on the pooled features'
+    gradient (the node-level stage's backward ends there, the first PointResNet's begins)."""
+    enc, opt = m.encoder, m.opt
+    k, M = opt.k, ds.node_num
+    names = ("augment", "som", "first_pointresnet_fwd_bwd", "node_level_fwd_bwd", "optimizer")
+    ts = {n: [] for n in names}
+    rng = np.random.RandomState(0)
+    for i in range(reps + 3):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(8)]
+        ev[0].record()
+        pts, off, label, node, knn = ds.full_batch(idx, opt, train=True, rng=rng, seed=i)
+        ev[1].record()
+        m.encoder.train()
+        m.classifier.train()
+        with torch.no_grad():
+            a, _, _ = ops.som_assign_ragged(pts, off, node, k)
+            _, _, _, cm = ops.som_group_decenter_ragged(pts, off, a, M, k, True)
+            x_aug = ops.som_decenter_ragged(pts, off, a, cm, k, True)
+            cols = off * k
+        ev[2].record()
+        with torch.enable_grad():
+            fpo = enc.first_pointnet(x_aug, 0, cols=cols)
+            mm = train_ops.IndexMaxGatherRagged.apply(fpo, a, off, cols, M, k)
+            mm.register_hook(lambda g: ev[5].record())
+            ev[3].record()
+            c, f = enc.knnlayer(cm, mm, knn, opt.som_k, opt.som_k_type, 0)
+            feature = enc.final_pointnet.forward_pair(c, f, 0).max(dim=2)[0]
+            loss = m.softmax_criteria(m.classifier(feature, 0, store=False), label)
+            enc.zero_grad()
+            m.classifier.zero_grad()
+            ev[4].record()
+            loss.backward()
+        ev[6].record()
+        for o in m._optim:
+            o.step()
+        ev[7].record()
+        ev[7].synchronize()
+        if i >= 3:
+            e = lambda a, b: ev[a].elapsed_time(ev[b])  # noqa: E731
+            ts["augment"].append(e(0, 1))
+            ts["som"].append(e(1, 2))
+            ts["first_pointresnet_fwd_bwd"].append(e(2, 3) + e(5, 6))
+            ts["node_level_fwd_bwd"].append(e(3, 4) + e(4, 5))
+            ts["optimizer"].append(e(6, 7))
+    return {n: float(np.median(v)) for n, v in ts.items()}
+
+
+def train_cases(res, reps):
+    cpu_opt = synth.make_opt("classifier")
+    states = (synth.synth_state_dict(networks.Encoder(cpu_opt), seed=1),
+              synth.synth_state_dict(networks.Classifier(cpu_opt), seed=2))
+    M = 64
+    rs = np.random.RandomState(5)
+    for case, sizes in (("TRAIN_A_32x10000", [10000] * 32),
+                        ("TRAIN_B_mixed_32", list(rs.randint(2000, 10001, size=32)))):
+        B = len(sizes)
+        pts, off, node = clouds(sizes, M, seed=2)
+        ds = augmentation.DeviceDataset.from_device(
+            pts, off, torch.from_numpy(rs.randint(0, 40, size=B)).to(DEV), node)
+        idx = np.arange(B)
+        m = train_model(B, 256, states)
+        rng = np.random.RandomState(1)
+        batch = ds.full_batch(idx, m.opt, train=True, rng=rng, seed=0)
+        res[case + "_points"] = int(sum(sizes))
+        res[case + "_step_ms"] = median_ms(lambda: m.optimize_clouds(*batch, epoch=0), reps)
+        res[case + "_augment_ms"] = median_ms(
+            lambda: ds.full_batch(idx, m.opt, train=True, rng=rng, seed=1), reps)
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats(DEV)
+        base = torch.cuda.memory_allocated(DEV)
+        m.optimize_clouds(*batch, epoch=0)
+        torch.cuda.synchronize()
+        res[case + "_peak_step_bytes"] = int(torch.cuda.max_memory_allocated(DEV) - base)
+        res[case + "_split_ms"] = train_stage_split(m, ds, idx, reps)
+        del m
+        torch.cuda.empty_cache()
+        if case.startswith("TRAIN_A"):
+            P = sizes[0]
+            for N in (10000, 5000):
+                md = train_model(B, N, states)
+                pc = pts.view(B, P, 6)[:, :N, :3].permute(0, 2, 1).contiguous()
+                sn = pts.view(B, P, 6)[:, :N, 3:].permute(0, 2, 1).contiguous()
+                knn = augmentation.som_knn(node, 9, M)
+                label = ds.labels
+
+                def dense():
+                    md.set_input(pc, sn, label, node, knn)
+                    md.optimize(epoch=0)
+                res["TRAIN_A_dense_optimize_N%d_ms" % N] = median_ms(dense, reps)
+                torch.cuda.synchronize()
+                torch.cuda.reset_peak_memory_stats(DEV)
+                base = torch.cuda.memory_allocated(DEV)
+                dense()
+                torch.cuda.synchronize()
+                res["TRAIN_A_dense_optimize_N%d_peak_step_bytes" % N] = int(
+                    torch.cuda.max_memory_allocated(DEV) - base)
+                del md
+                torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":
